@@ -27,7 +27,7 @@ struct DecoderLayout {
   int64_t final_ln_w, final_ln_b, heads, rope_cos, rope_sin, c_heads;
   // cluster step kernel (step2.cu): a second copy of the six per-layer matrices, cut into one contiguous slice per
   // (phase, cluster, rank): the n-tiles the cluster owns x the K range the rank reduces.  cl_NC == 0: shape not covered.
-  int cl_C, cl_NC;          // CTAs per cluster (8), clusters (= heads)
+  int cl_C, cl_NC;          // CTAs per cluster (2), clusters (4 per head)
   int64_t rm[7];            // per layer (bf16 only): ROW-MAJOR copies of wqkv, wo, wqc, wkvc, woc, fc1, fc2 for the wgmma prefill
                             // GEMM (gemm_tc.cu: TMA-tiled K-major operands); same order as rm_src()
   int64_t cp[6];            // per layer: offset of phase p's slices (A qkv | B o | C q_cross | D o_cross | E fc1 | F fc2)
@@ -35,10 +35,10 @@ struct DecoderLayout {
   int64_t total;
 };
 
-// Shapes the cluster step kernel covers: bf16, MHA for self- and cross-attention, two clusters of 4 CTAs per head (at most 18 heads;
+// Shapes the cluster step kernel covers: bf16, MHA for self- and cross-attention, four clusters of 2 CTAs per head (at most 18 heads;
 // whether the device holds the grid co-resident is asked at session set-up, step2.cu cluster_step_available: a 132-SM H100 holds
-// 30 clusters of 4, i.e. up to 15 heads), K halves that are whole k32 tiles, H / (2 heads) = 32 out-proj features per cluster, at most 4 fc1 n-tiles per rank, and
-// the shared-memory plan of step2.cu (sized for H <= 1024, F <= 4096).
+// 66 clusters of 2, i.e. up to 16 heads), K a whole number of 8-tile groups (step.cu's 8-way K split), H / (4 heads) = 16 out-proj features per cluster, at
+// most 4 fc1 n-tiles per rank, and the shared-memory plan of step2.cu (sized for H <= 1024, F <= 4096).
 static inline bool cluster_shape_ok(const ptts_decoder_config& c) {
   const int H = c.hidden_size, nh = c.num_heads, F = c.ffn_dim;
   return c.dtype == PTTS_BF16 && c.num_kv_heads == nh && c.num_cross_kv_heads == nh && nh * 8 <= 144 && H == nh * PTTS_HEAD_DIM &&
@@ -83,11 +83,11 @@ static inline DecoderLayout make_layout(const ptts_decoder_config& c) {
   l.cl_C = l.cl_NC = 0;
   for (int i = 0; i < 6; i++) l.cp[i] = l.cp_slice[i] = 0;
   if (cluster_shape_ok(c)) {
-    l.cl_C = 4; l.cl_NC = 2 * l.nh;
-    const int64_t ks = l.H / 4 / 32, ksf = l.F / 4 / 32;                 // k32 tiles per rank: K = H phases, K = F phase
-    // n-tiles per slice: a head's q|k|v (192 features), a cluster's 32 out-proj features, a head's q_cross, ..., F / 32 fc1 features
-    const int64_t nt[6] = {24, 4, 8, 4, l.F / (2 * l.nh) / 8, 4};
-    const int64_t owners[6] = {l.nh, 2 * l.nh, l.nh, 2 * l.nh, 2 * l.nh, 2 * l.nh};   // head phases: one slice set per head
+    l.cl_C = 2; l.cl_NC = 4 * l.nh;
+    const int64_t ks = l.H / 2 / 32, ksf = l.F / 2 / 32;                 // k32 tiles per rank: K = H phases, K = F phase
+    // n-tiles per slice: a head's q|k|v (192 features), a cluster's 16 out-proj features, a head's q_cross, ..., F / (4 nh) fc1 features
+    const int64_t nt[6] = {24, 2, 8, 2, l.F / (4 * l.nh) / 8, 2};
+    const int64_t owners[6] = {l.nh, 4 * l.nh, l.nh, 4 * l.nh, 4 * l.nh, 4 * l.nh};   // head phases: one slice set per head
     for (int i = 0; i < 6; i++) {
       l.cp_slice[i] = nt[i] * (i == 5 ? ksf : ks) * 512;
       l.cp[i] = take(l.cp_slice[i] * owners[i] * l.cl_C) - base;
@@ -145,7 +145,7 @@ struct WorkspaceLayout {
   int64_t ctrl, progress, gen, raw_ids, cur_ids, eos_seen, unfinished, first_unf, prompt_mask, enc_mask;
   int64_t x, qkv, attn, qc, hbuf, hidden, logits, scores, cross_tmp, cross_kv, self_kv;
   int64_t img_x, img_attn, img_h;  // fused step kernel: activations as tile images [chunk][32][H + 8] (step.cu stage_tile)
-  int64_t cl_x, cl_attn, cl_h;     // cluster step kernel: K-sliced images [4][32][K/4 + 8] (step2.cu)
+  int64_t cl_x, cl_attn, cl_h;     // cluster step kernel: K-sliced images [2][32][H/2 + 8], fc2's in quarters [4][32][F/4 + 8] (step2.cu)
   int64_t row_stats;               // [max(B*(P+1), B*S)][2] f32: LayerNorm row statistics of the wgmma prefill GEMMs
   int64_t cross_layer_stride, self_layer_stride;  // bytes
   int64_t raw_ld;                                  // raw_ids leading dimension (elements)
@@ -181,8 +181,8 @@ static inline WorkspaceLayout make_workspace(const ptts_decoder_config& c, int B
   w.img_attn = take((int64_t)32 * (l.H + 8) * 2);
   w.img_h = take((int64_t)((l.F + l.H - 1) / l.H) * 32 * (l.H + 8) * 2);
   w.row_stats = take((int64_t)(w.Mmax > rows_enc ? w.Mmax : rows_enc) * 2 * 4);
-  w.cl_x = take((int64_t)4 * 32 * (l.H / 4 + 8) * 2);
-  w.cl_attn = take((int64_t)4 * 32 * (l.H / 4 + 8) * 2);
+  w.cl_x = take((int64_t)2 * 32 * (l.H / 2 + 8) * 2);
+  w.cl_attn = take((int64_t)2 * 32 * (l.H / 2 + 8) * 2);
   w.cl_h = take((int64_t)4 * 32 * (l.F / 4 + 8) * 2);
   w.logits = take((int64_t)w.BK * l.V * 4);
   w.scores = take((int64_t)w.BK * l.V * 4);

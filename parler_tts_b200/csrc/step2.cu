@@ -6,29 +6,32 @@
 // dependent phases of a layer: each phase pays a device-wide barrier, the pull of the 66 KB tile, LayerNorm statistics over it
 // and an 8-warp split-K reduction through shared memory.  This kernel cuts the dependent chain and the per-CTA fixed work:
 //
-//   * grid = 2 clusters of 4 CTAs per head (cudaLaunchAttributeClusterDimension; the whole grid must be co-resident, which
-//     cluster_step_available asks the occupancy API -- a 132-SM H100 holds 30 clusters of 4, so Mini's 32 run step.cu there).
-//     Every GEMM is split 8 ways along K: rank r of a cluster stages K-slice
-//     r (K/4 columns: 8-17 KB of activations instead of 66 KB) and its two warp groups reduce one half of it each ("virtual
-//     ranks" v = 2 r + half).  Every warp owns whole n-tiles (no split-K through shared memory inside a CTA); the eight partial
-//     sums meet through DISTRIBUTED SHARED MEMORY: one cp.async.bulk (shared::cta -> shared::cluster, mbarrier complete_tx) per peer.
-//   * out-proj / cross out-proj / fc1 / fc2: cluster c owns N/32 output features, rank d finalises a quarter of them
+//   * grid = 4 clusters of 2 CTAs per head (cudaLaunchAttributeClusterDimension; the whole grid must be co-resident, which
+//     cluster_step_available asks the occupancy API -- a 132-SM H100 holds 66 clusters of 2, one per TPC, and Mini needs 64).
+//     Every GEMM is split 8 ways along K as step.cu splits it over its 8 warps (k32 tile kt -> residue class kt mod 8): rank r
+//     of a cluster stages the k-tiles of classes 4r .. 4r+3 (half of K: 8-33 KB of activations instead of 66 KB) and warp w
+//     reduces class 4 r + (w >> 1) for destination (w & 1).  Every warp owns whole n-tiles (no split-K through shared memory
+//     inside a CTA); the eight partial sums meet through DISTRIBUTED SHARED MEMORY: one cp.async.bulk (shared::cta ->
+//     shared::cluster, mbarrier complete_tx) per peer, and every destination adds them in class order 0..7.
+//   * out-proj / cross out-proj / fc1 / fc2: cluster c owns N/(4 nh) output features, rank d finalises half of them
 //     (feature-partitioned exchange).  The residual-stream slice a CTA owns (32 rows x 8 features) never leaves its shared memory.
-//   * QKV and q_cross: clusters 2h and 2h+1 own HEAD h for batch rows 0-15 / 16-31; the exchange is ROW-partitioned (rank d
-//     receives rows 4d..4d+3 of q|k|v), so RoPE, the KV-cache append and the attention of those 4 (row, head) items run inside
-//     the same phase: QKV -> self-attention and q_cross -> cross-attention need no device-wide barrier between them.
-//     6 barriers per layer instead of 8.
+//   * QKV and q_cross: clusters 4h .. 4h+3 own HEAD h for batch rows 8j .. 8j+7 (one m16 tile with 8 live rows); the exchange is
+//     ROW-partitioned (rank d receives rows 8j+4d .. 8j+4d+3 of q|k|v), so RoPE, the KV-cache append and the attention of those 4
+//     (row, head) items run inside the same phase: QKV -> self-attention and q_cross -> cross-attention need no device-wide barrier
+//     between them.  6 barriers per layer instead of 8.  A warp carries 12 QKV n-tiles (4 q_cross) in two passes of 6 (2): the
+//     head's 192 KB QKV slice of a rank streams through the 2 x 64 KB weight ring as four jobs.
 //   * weights: one contiguous slice per (phase, cluster, rank) (layout.h cpack, built once by ptts_decoder_finalize), streamed by
 //     ONE bulk copy per job into a 2 x 64 KB ring two jobs ahead, with an L2 evict-first policy like the K/V rows (1.2 GB per token
 //     must not evict the kernel's own instructions and the small reused tensors).  HBM -> L2 prefetches a layer ahead exist behind
 //     PTTS_DBG=1/2 (experiments, off by default).
-//   * fc2 (one n-tile per destination, K slice F/4): every warp takes all four n-tiles over an eighth of the K slice, the partial
-//     tiles are added inside the CTA and one block per destination crosses the cluster (A fragments read once per CTA).
+//   * fc2 (one n-tile per destination, half of F = 128 KB of activations): staged in two quarters of F, one after the other; a
+//     warp's accumulators carry its residue class from the first quarter into the second.
+//   * attention: the sweep step.cu's attention phase runs (attention_decode_item_warp, two warps per item, 32-key chunks).
 //   * the activation slice of the next phase is requested by the barrier's polling thread the moment the barrier opens; the
 //     per-phase cluster barrier that guards buffer reuse arrives .relaxed (its default .release is a gpu-scope MEMBAR per warp).
 //   * one launch runs up to StepParams.n_steps tokens: cur_len, the unfinished count and the stop decision advance on the device.
-// Reduction orders are fixed (k-tiles ascending inside a warp, virtual ranks 0..7 across the cluster): bit-reproducible run to
-// run.  They differ from step.cu / gemm.cu, so the two paths agree to bf16 accumulation-order noise, not bitwise.
+// Reduction orders are fixed and are step.cu's (k-tiles ascending in one accumulator per warp, warp partials 0..7 added from zero;
+// the same LayerNorm statistics, attention and lm-head split): the two step kernels produce the same bits, run to run.
 #include "attn_core.cuh"
 #include "common.cuh"
 #include "kernels.h"
@@ -42,23 +45,35 @@
 namespace ptts {
 namespace cl {
 
-constexpr int C = 4;            // CTAs per cluster
-constexpr int V = 8;            // virtual ranks = warps per CTA: warp w reduces K-half (w >> 2) for destination rank (w & 3)
+constexpr int C = 2;            // CTAs per cluster
+constexpr int V = 8;            // K residue classes = warps per CTA: warp w reduces class 4 rank + (w >> 1) for destination (w & 1)
 constexpr int THREADS = 256;
-constexpr int ROWS = 32;        // batch rows (two m16 tiles; the head phases work on one half = one m16 tile)
-constexpr int ATT_CH = 16;      // keys per K/V ring stage of an attention warp
+constexpr int ROWS = 32;        // batch rows (two m16 tiles; the head phases work on 8 rows = one m16 tile with rows 8-15 repeated)
+constexpr int HROWS = 8;        // batch rows of a head-phase cluster
+constexpr int ATT_SMEM = attn_decode_smem_per_warp<bf16>();   // one attention warp's scratch: two 32-key K/V stages + 192 floats
 constexpr int PROF_STRIDE = 16;  // clock64 stamps per phase row of the optional profile buffer (tools/profile_step2.py)
-constexpr int QMAX = 6;         // n-tiles per warp (QKV: 24 n-tiles of a head over 4 destination groups)
+constexpr int QMAX = 6;         // n-tiles per warp and pass (QKV: 24 n-tiles of a head = 2 passes x 2 warp groups x 6)
 constexpr int OFF_STATS = 256, OFF_PART = 512, OFF_RES = 2560, OFF_CVEC = 3584;
 constexpr int HDR = 5632;       // mbarriers | row stats | stat partials | residual slice | folded-LN vectors c1[256] c2[256]
 constexpr int WB_BYTES = 65536; // one weight ring buffer
 constexpr int R_OFF = HDR + 2 * WB_BYTES;
-// R region: [activation slice | 8 send blocks | 8 receive slots], split per phase; attention scratch and the lm-head tile alias it.
-// Sized for Mini (H = 1024, F = 4096): fc1 = 16.5 KB slice + 2 x 8 blocks of (256 B stats + 32 x 34 floats).
+// R region: [send blocks | receive slots] over the activation slice, split per phase; attention scratch and the lm-head tile alias it.
+// The send blocks are written once the phase's MMAs have retired, so they start at 0 over the dead activation slice; the receive
+// slots, which peers fill while this CTA may still run its MMAs, start behind both.  Largest plans (H = 1024, F = 4096):
+//   fc1   : 32.5 KB slice, 8 send blocks of (256 B stats + 32 x 34 floats) = 36 KB, receive slots [36 KB, 72 KB)
+//   fc2   : 64.5 KB quarter slice, 8 send blocks of (256 B + 32 x 8 floats), receive slots [64.5 KB, 74.5 KB)
+//   QKV   : 8.1 KB slice, 16 send blocks of (32 B stats + 4 x 96 floats) = 24.5 KB, receive slots [24.5 KB, 49 KB), the first pass's
+//           tiles at R_PASS0 until the exchange, q|k|v at QKV_OFF; the attention scratch of warps 0-4 below QKV_OFF
+//   lm heads: the whole x image (65 KB)
 constexpr int R_BYTES = 92160;
+constexpr int R_PASS0 = 65536;            // [8 warps][6 n-tiles][32 lanes] float4: the head phases' first-pass tiles
 constexpr int QKV_OFF = R_BYTES - 2048;   // [4 rows][192] bf16 q|k|v (or [4][64] q_cross) of this rank's attention items
 constexpr int SMEM_BYTES = R_OFF + R_BYTES;
 static_assert(SMEM_BYTES + 1024 <= 227 * 1024, "cluster step kernel shared memory");
+static_assert(ROWS * (1024 / 2 + 8) * 2 <= V * (256 + ROWS * 34 * 4) && 2 * V * (256 + ROWS * 34 * 4) <= R_BYTES, "fc1 plan");
+static_assert(2 * V * C * (32 + 4 * 96 * 4) <= R_PASS0 && R_PASS0 + V * QMAX * 32 * 16 <= QKV_OFF, "QKV plan");
+static_assert(5 * ATT_SMEM <= QKV_OFF && 3 * ATT_SMEM <= WB_BYTES && 16384 + 4 * 128 * 4 <= WB_BYTES, "attention plan");
+static_assert(ROWS * (4096 / 4 + 8) * 2 + V * (256 + ROWS * 8 * 4) <= R_BYTES, "fc2 plan");
 
 // ---- PTX helpers ---------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t s32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -151,84 +166,73 @@ __device__ __forceinline__ unsigned grid_sync(unsigned* ctr, unsigned target, in
   return target;
 }
 
-// One warp's MMA loop: QN n-tiles x MT m-tiles over k-tiles [kt_lo, kt_hi) of the staged slice.  SETS independent accumulator
-// sets (k-tile parity x k16 half) break the dependent HMMA chain of the narrow phases (q = 1: out-proj, fc2 -- 32 dependent
-// MMAs at 16 k-tiles otherwise); they are summed in a fixed order at the end.  STATS: the warp also accumulates the LayerNorm
-// row sums of its k-tiles from the A fragments it has loaded anyway (the four destination groups of a K half repeat this work:
-// 6 extra MMAs per k-tile and m-tile buy an exchange without any CTA-wide synchronisation).
-template <int QN, int MT, int SETS, bool STATS>
-__device__ __forceinline__ void mma_slice(float (&out)[2][6][4], RowStatFrag& rst, const bf16* xs, int apitch, const uint4* wb, int KT, int kt_lo,
-                                          int kt_hi, int dgrp, int lrow, int lcol) {
-  float acc[SETS][MT][QN][4];
+// K-slice layout of the activation images and of the packed weights: rank r holds the k32 tiles kt with (kt & 7) >> 2 == r, in
+// ascending order.  Warp e4 of rank r then reduces the k-tiles kt = 4 r + e4 (mod 8): the tiles, in the order, that warp 4 r + e4
+// of step.cu's 8-warp K split reduces, and every destination adds the eight partial sums in that warp order -- so both step
+// kernels compute the same bits (step.cu serves the shapes and devices this kernel does not cover).
+__host__ __device__ __forceinline__ int kslice(int kt) { return (kt & 7) >> 2; }
+__host__ __device__ __forceinline__ int klocal(int kt) { return ((kt >> 3) << 2) | (kt & 3); }
+__host__ __device__ __forceinline__ int kglobal(int rank, int lk) { return ((lk >> 2) << 3) | (rank << 2) | (lk & 3); }
+
+// One warp's MMA loop: QN n-tiles x MT m-tiles over the local k-tiles kt0, kt0 + 4, ... < kt_end of the staged slice, one
+// accumulator per output (the dependent chain of step.cu, whose sums it must reproduce).  ACC: continue from `out` (fc2's second
+// quarter of F).  STATS: the warp also accumulates the LayerNorm row sums of its k-tiles from the A fragments it has loaded anyway
+// (the two destination groups of a residue class repeat this work: 6 extra MMAs per k-tile and m-tile buy an exchange without any
+// CTA-wide synchronisation).
+template <int QN, int MT, bool STATS, bool ACC = false>
+__device__ __forceinline__ void mma_slice(float (&out)[2][6][4], RowStatFrag& rst, const bf16* xs, int apitch, const uint4* wb, int KT, int kt0,
+                                          int kt_end, int lrow, int lcol) {
+  float acc[MT][QN][4];
 #pragma unroll
-  for (int s = 0; s < SETS; s++)
+  for (int a = 0; a < MT; a++)
 #pragma unroll
-    for (int a = 0; a < MT; a++)
+    for (int j = 0; j < QN; j++)
 #pragma unroll
-      for (int j = 0; j < QN; j++)
-#pragma unroll
-        for (int e = 0; e < 4; e++) acc[s][a][j][e] = 0.f;
-  // one k-tile into accumulator set S0 (and S0 + 1 for its second k16 half when SETS >= 2)
-  auto k_tile = [&](int kt, auto s0_tag) {
-    constexpr int S0 = decltype(s0_tag)::value;
+      for (int e = 0; e < 4; e++) acc[a][j][e] = ACC ? out[a][j][e] : 0.f;
+  for (int kt = kt0; kt < kt_end; kt += 4) {
     uint32_t a[MT][2][4];
 #pragma unroll
     for (int mt = 0; mt < MT; mt++)
 #pragma unroll
       for (int j = 0; j < 2; j++) ldsm4(a[mt][j], xs + (size_t)(mt * 16 + lrow) * apitch + kt * 32 + j * 16 + lcol);
-    if (STATS) {   // every k-tile of this warp's K half: the (dest, K half) block then carries complete statistics for its K range
+    if (STATS) {   // every k-tile of this warp's residue class: its blocks then carry complete statistics for it
 #pragma unroll
       for (int mt = 0; mt < MT; mt++) { row_stat_mma(rst, mt, a[mt][0]); row_stat_mma(rst, mt, a[mt][1]); }
     }
-    constexpr int SB = (SETS >= 2) ? 1 : 0;
 #pragma unroll
     for (int j = 0; j < QN; j++) {
       const uint4 w = wb[((size_t)j * KT + kt) * 32];
 #pragma unroll
       for (int mt = 0; mt < MT; mt++) {
-        mma_bf16_16816(acc[S0][mt][j], a[mt][0], w.x, w.y);
-        mma_bf16_16816(acc[S0 + SB][mt][j], a[mt][1], w.z, w.w);
+        mma_bf16_16816(acc[mt][j], a[mt][0], w.x, w.y);
+        mma_bf16_16816(acc[mt][j], a[mt][1], w.z, w.w);
       }
     }
-  };
-  // SETS == 4 takes k-tiles in pairs (the set index must be a compile-time constant).  A half of an odd number of k-tiles
-  // (H = 768: 3 per half) ends with one unpaired tile; it must not run a pair past kt_hi, which would read the next half's
-  // activations and weights (or past the staged slice) and add them in.
-  int kt = kt_lo;
-  if (SETS == 4) {
-    for (; kt + 2 <= kt_hi; kt += 2) { k_tile(kt, std::integral_constant<int, 0>{}); k_tile(kt + 1, std::integral_constant<int, 2>{}); }
-    if (kt < kt_hi) k_tile(kt, std::integral_constant<int, 0>{});
-  } else {
-    for (; kt < kt_hi; kt++) k_tile(kt, std::integral_constant<int, 0>{});
   }
 #pragma unroll
   for (int mt = 0; mt < MT; mt++)
 #pragma unroll
     for (int j = 0; j < QN; j++)
 #pragma unroll
-      for (int e = 0; e < 4; e++) {
-        float v = acc[0][mt][j][e];
-#pragma unroll
-        for (int s2 = 1; s2 < SETS; s2++) v += acc[s2][mt][j][e];
-        out[mt][j][e] = v;
-      }
+      for (int e = 0; e < 4; e++) out[mt][j][e] = acc[mt][j][e];
 }
 
 // phase kinds of a layer
 enum { PH_QKV = 0, PH_O = 1, PH_QC = 2, PH_OC = 3, PH_FC1 = 4, PH_FC2 = 5 };
-constexpr int JOBS_PER_LAYER = 7;   // weight jobs: QKV (two halves of 12 n-tiles), O, QC, OC, FC1, FC2
+constexpr int JOBS_PER_LAYER = 9;   // weight jobs: QKV (four quarters of 6 n-tiles), O, QC, OC, FC1, FC2
+constexpr int QKV_JOBS = 4;
 
-// source of weight job j for this CTA (7 per layer, then this CTA's lm-head tasks)
+// source of weight job j for this CTA (9 per layer, then this CTA's lm-head tasks)
 __device__ __forceinline__ bool weight_job(const StepParams& p, int j, int cta, int rank, const char*& src, uint32_t& bytes) {
   const int nl = JOBS_PER_LAYER * p.L;
   if (j < nl) {
     const int l = j / JOBS_PER_LAYER, jl = j - JOBS_PER_LAYER * l;
-    const int ph = jl < 2 ? 0 : jl - 1;
-    // the head phases' slices are shared by the two row-half clusters of a head: indexed (head, rank)
+    const int ph = jl < QKV_JOBS ? 0 : jl - (QKV_JOBS - 1);
+    // the head phases' slices are shared by the four row-block clusters of a head: indexed (head, rank)
     const int64_t idx = (ph == PH_QKV || ph == PH_QC) ? (int64_t)(cta >> 3) * C + rank : (int64_t)cta;
     const int64_t sz = p.cp_slice[ph];
-    bytes = (uint32_t)(ph == PH_QKV ? sz / 2 : sz);
-    src = p.blob + p.layer0 + p.layer_stride * l + p.cp[ph] + idx * sz + (jl == 1 ? sz / 2 : 0);
+    bytes = (uint32_t)(ph == PH_QKV ? sz / QKV_JOBS : sz);
+    src = p.blob + p.layer0 + p.layer_stride * l + p.cp[ph] + idx * sz + (ph == PH_QKV ? jl * (sz / QKV_JOBS) : 0);
     return true;
   }
   const int task = cta + (int)gridDim.x * (j - nl);
@@ -251,18 +255,18 @@ __global__ void __launch_bounds__(THREADS, 1) decode_step_cluster_kernel(const _
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int H = p.H, F = p.F, B = p.B;
   const int rank = (int)cluster_rank();
-  const int cta = (int)blockIdx.x;         // = cluster * 4 + rank
-  const int cluster = cta >> 2;
-  const int head = cluster >> 1, half = cluster & 1;   // head phases: this cluster's head and its batch-row half (rows 16 half ..)
-  const int Ks = H / C, KsF = F / C;       // K-slice widths of a CTA
+  const int cta = (int)blockIdx.x;         // = cluster * 2 + rank
+  const int cluster = cta >> 1;
+  const int head = cluster >> 2, rblk = cluster & 3;   // head phases: this cluster's head and its batch-row block (rows 8 rblk ..)
+  const int Ks = H / C, KsF = F / 4;       // K-slice widths: a CTA's half of H, a quarter of F (fc2 stages its half in two)
   const int pitch = Ks + 8, pitchF = KsF + 8;
   const int qe = F / p.nh / 64;            // fc1 n-tiles per destination rank (Mini: 4)
-  const int dgrp = warp & 3, kh = warp >> 2;  // this warp: destination group, K half of the CTA's slice
+  const int dgrp = warp & 1, e4 = warp >> 1;  // this warp: destination rank (head phases: n-tile group), K class 4 rank + e4
 
   uint64_t* abar = reinterpret_cast<uint64_t*>(smem);        // activation slice
   uint64_t* wbar = abar + 1;                                  // [2] weight ring
   uint64_t* xbar = abar + 3;                                  // cluster exchange
-  uint64_t* attbars = reinterpret_cast<uint64_t*>(smem + 128);  // [8 warps][2] K/V rings
+  uint64_t* attbars = reinterpret_cast<uint64_t*>(smem + 128);  // [8 warps][2] K/V ring stages of the attention
   float* stats = reinterpret_cast<float*>(smem + OFF_STATS);   // [32][2] mean, rstd
   float* part = reinterpret_cast<float*>(smem + OFF_PART);     // [8][32][2]
   float* res_s = reinterpret_cast<float*>(smem + OFF_RES);     // [32][8] residual stream slice owned by this CTA
@@ -309,7 +313,7 @@ __global__ void __launch_bounds__(THREADS, 1) decode_step_cluster_kernel(const _
   };
   auto prefetch_kv_part = [&](int l, bool cross, int w) {  // warp w: item w >> 1, K (even w) or V (odd w)
     const int T = cross ? p.S : p.Tmax, n = cross ? p.S : pos;
-    const int b = 16 * half + 4 * rank + (w >> 1);
+    const int b = HROWS * rblk + 4 * rank + (w >> 1);
     if (!pf_kv || n <= 0 || b >= B) return;
     const char* kc = cross ? p.cross_kv + p.cross_layer_stride * l : p.self_kv + p.self_layer_stride * l;
     const char* k = kc + ((size_t)b * p.nh + head) * T * HD * 2 + ((w & 1) ? (size_t)B * p.nh * T * HD * 2 : 0);
@@ -332,13 +336,18 @@ __global__ void __launch_bounds__(THREADS, 1) decode_step_cluster_kernel(const _
     prefetch_kv_part(0, false, warp); prefetch_kv_part(0, true, warp);
   }
 
-  // global activation images, K-sliced for their consumer: [4 slices][32 rows][slice width + 8] bf16
-  bf16* const x_img = p.cl_x;       // slices of H/4 columns (consumers: QKV, q_cross, fc1, lm heads)
-  bf16* const a_img = p.cl_attn;    // slices of H/4 columns = 4 heads (consumers: out_proj, cross out_proj)
-  bf16* const h_img = p.cl_h;       // slices of F/4 columns (consumer: fc2)
+  // global activation images, K-sliced for their consumer: [slices][32 rows][slice width + 8] bf16
+  bf16* const x_img = p.cl_x;       // 2 slices of H/2 columns (consumers: QKV, q_cross, fc1, lm heads)
+  bf16* const a_img = p.cl_attn;    // 2 slices of H/2 columns = 8 heads (consumers: out_proj, cross out_proj)
+  bf16* const h_img = p.cl_h;       // 4 slices of F/4 columns (consumer: fc2, two per rank)
   const int x_slice_elems = ROWS * pitch, h_slice_elems = ROWS * pitchF;
-  // where this CTA's 8 residual / out-proj features live in the x image: feature n = cta * 8 + f
-  const int xo_slice = (cta * 8) / Ks, xo_col = (cta * 8) % Ks;
+  // h feature n -> (quarter 2 kslice + local k-tile / (F / 128), column) of the fc2 image (row 0)
+  auto h_offset = [&](int n) {
+    const int lk = klocal(n >> 5), kq = KsF >> 5;
+    return (size_t)(2 * kslice(n >> 5) + lk / kq) * h_slice_elems + (lk % kq) * 32 + (n & 31);
+  };
+  // where this CTA's 8 residual / out-proj features live in the x image: feature n = cta * 8 + f (one k32 tile, kslice)
+  const int xo_slice = kslice(cta >> 2), xo_col = klocal(cta >> 2) * 32 + (cta & 3) * 8;
 
   // ---- embeddings: this CTA's 32 x 8 slice of sum_k embed_k[id] (+ position) -> residual slice + x image -----------------
   {
@@ -347,13 +356,17 @@ __global__ void __launch_bounds__(THREADS, 1) decode_step_cluster_kernel(const _
     const int row = tid >> 3, f = tid & 7, n = cta * 8 + f;
     float v = 0.f;
     if (row < B) {
-      float ev[16];
+      // codebooks in groups of 8: the loads of a group are in flight together, and the group's values are all that is live
+#pragma unroll 1
+      for (int k0 = 0; k0 < p.K; k0 += 8) {
+        float ev[8];
 #pragma unroll
-      for (int k = 0; k < 16; k++)
-        if (k < p.K) ev[k] = __bfloat162float(tables[((size_t)k * (p.V + 1) + p.sa.cur_ids[row * p.K + k]) * H + n]);
+        for (int k = 0; k < 8; k++)
+          if (k0 + k < p.K) ev[k] = __bfloat162float(tables[((size_t)(k0 + k) * (p.V + 1) + p.sa.cur_ids[row * p.K + k0 + k]) * H + n]);
 #pragma unroll
-      for (int k = 0; k < 16; k++)
-        if (k < p.K) v = (k == 0) ? ev[k] : DT<bf16>::rnd(v + ev[k]);
+        for (int k = 0; k < 8; k++)
+          if (k0 + k < p.K) v = (k0 + k == 0) ? ev[k] : DT<bf16>::rnd(v + ev[k]);
+      }
       if (postab != nullptr) v = DT<bf16>::rnd(v + __bfloat162float(postab[(size_t)pos * H + n]));
     }
     res_s[row * 8 + f] = v;
@@ -365,12 +378,13 @@ __global__ void __launch_bounds__(THREADS, 1) decode_step_cluster_kernel(const _
     mbar_expect_tx(abar, bytes);
     bulk_g2s(Rg, img_slice, bytes, abar);
   };
-  // activation slice of phase kind `sub`: rows of this cluster's half for the head phases, all 32 rows otherwise
+  // activation slice of phase kind `sub`: rows of this cluster's row block for the head phases, all 32 rows otherwise; fc2: the
+  // first of this rank's two quarters of F (the second is requested when the first one's MMAs have retired)
   auto slice_of = [&](int sub, const bf16*& img, uint32_t& bytes) {
-    if (sub == PH_QKV || sub == PH_QC) { img = x_img + (size_t)rank * x_slice_elems + (size_t)(16 * half) * pitch; bytes = (uint32_t)(16 * pitch * 2); }
+    if (sub == PH_QKV || sub == PH_QC) { img = x_img + (size_t)rank * x_slice_elems + (size_t)(HROWS * rblk) * pitch; bytes = (uint32_t)(HROWS * pitch * 2); }
     else if (sub == PH_O || sub == PH_OC) { img = a_img + (size_t)rank * x_slice_elems; bytes = (uint32_t)(x_slice_elems * 2); }
     else if (sub == PH_FC1) { img = x_img + (size_t)rank * x_slice_elems; bytes = (uint32_t)(x_slice_elems * 2); }
-    else { img = h_img + (size_t)rank * h_slice_elems; bytes = (uint32_t)(h_slice_elems * 2); }
+    else { img = h_img + (size_t)(2 * rank) * h_slice_elems; bytes = (uint32_t)(h_slice_elems * 2); }
   };
   {
     const bf16* nimg; uint32_t nbytes;
@@ -383,15 +397,10 @@ __global__ void __launch_bounds__(THREADS, 1) decode_step_cluster_kernel(const _
   const int g = lane >> 2, t4 = lane & 3;
   const int n_phases = 6 * p.L;
 
-  // per-warp constants of the attention items (row 16 half + 4 rank + (warp >> 1), this cluster's head): element offsets of the item's
-  // K rows inside a layer's self / cross cache, the V planes' distance, and where its output goes in the attn image
-  const int att_row = 16 * half + 4 * rank + (warp >> 1);
-  const size_t self_item = ((size_t)att_row * p.nh + head) * p.Tmax * HD, self_vofs = (size_t)B * p.nh * p.Tmax * HD;
-  const size_t cross_item = ((size_t)att_row * p.nh + head) * p.S * HD, cross_vofs = (size_t)B * p.nh * p.S * HD;
-  // head h's 64 output features sit in K-slice (h HD) / Ks at column (h HD) % Ks (Ks = H / 4 is a multiple of HD: a head never
-  // straddles two slices; Mini has 4 heads per slice, H = 768 three)
-  const int att_slice = head * HD / Ks, att_col = head * HD % Ks;
-  bf16* const att_out = a_img + (size_t)att_slice * x_slice_elems + (size_t)att_row * pitch + att_col;
+  // this warp's attention item: row 8 rblk + 4 rank + (warp >> 1), this cluster's head, whose 64 output features are k-tiles
+  // 2 head, 2 head + 1 (adjacent in one K-slice of the attn image)
+  const int att_row = HROWS * rblk + 4 * rank + (warp >> 1);
+  const int att_slice = kslice(2 * head), att_col = klocal(2 * head) * 32;
 
 #pragma unroll 1
   for (int ph = 0; ph < n_phases; ph++) {
@@ -401,22 +410,19 @@ __global__ void __launch_bounds__(THREADS, 1) decode_step_cluster_kernel(const _
     const char* lb = blob + p.layer0 + p.layer_stride * l;
     const bool rowpart = (sub == PH_QKV || sub == PH_QC);
     const bool has_ln = (sub == PH_QKV || sub == PH_QC || sub == PH_FC1);
-    const int q = (sub == PH_QKV) ? 6 : (sub == PH_QC ? 2 : (sub == PH_FC1 ? qe : 1));   // n-tiles per warp
-    const int Nc = 4 * q * 8;                                        // features of this cluster in this phase
-    const int KT = (sub == PH_FC2 ? KsF : Ks) >> 5;                  // k32 tiles of this CTA's slice; a warp reduces half of them
+    // n-tiles per warp: head phases per pass (two passes: QKV 2 x 6 of the head's 24, q_cross 2 x 2 of its 8), otherwise per destination
+    const int q = (sub == PH_QKV) ? 6 : (sub == PH_QC ? 2 : (sub == PH_FC1 ? qe : 1));
+    const int Nc = 4 * q * 8;                                        // head phases: features of the head
+    const int KT = (sub == PH_FC2 ? KsF : Ks) >> 5;                  // k32 tiles of a staged slice (fc2: of one quarter of F)
     const int apitch = (sub == PH_FC2) ? pitchF : pitch;
-    const int act_bytes = (rowpart ? 16 : ROWS) * apitch * 2;
-    // exchange geometry: block (destination rank d, K half) at index 2 d + kh
+    const int act_bytes = (rowpart ? HROWS : ROWS) * apitch * 2;
+    // exchange geometry.  feature-partitioned: one block per warp, landing in slot (K class) at its destination;
+    // row-partitioned: one block per (warp, destination) with the warp's columns of both passes, slot 8 rank + warp
     const int RS = (q == 1) ? 8 : 8 * q + 2;                         // floats per row of a feature-partitioned block
-    const int blk = rowpart ? 32 + 4 * 8 * q * 4 : 256 + ROWS * RS * 4;   // one exchanged block: [statistics][rows][columns]
-    const int wsend = rowpart ? C * blk : blk;                       // bytes a warp stages (one block per destination rank)
-    const int j0 = JOBS_PER_LAYER * l + (sub == 0 ? 0 : sub + 1);    // first weight job of this phase
-    const int njobs = sub == 0 ? 2 : 1;
-    // fc2 (K slice of F/4, one n-tile per destination): with the (destination, K half) warp mapping four warps read the same A
-    // fragments -- 512 B of shared memory per HMMA, 262 KB per phase, and the shared-memory port (128 B/clk), not the tensor pipe,
-    // would set the phase time.  Instead every warp takes ALL four n-tiles over an eighth of the K slice (A read once per CTA); the eight
-    // partial tiles are added inside the CTA (shared memory, fixed order) and ONE block per destination crosses the cluster.
-    const bool fc2_wide = (sub == PH_FC2) && q == 1 && (KT & 7) == 0 && !(p.dbg & 512);
+    const int blk = rowpart ? 32 + 4 * 16 * q * 4 : 256 + ROWS * RS * 4;   // one exchanged block: [statistics][rows][columns]
+    const int wsend = rowpart ? C * blk : blk;                       // bytes a warp stages
+    const int j0 = JOBS_PER_LAYER * l + (sub == 0 ? 0 : sub + QKV_JOBS - 1);   // first weight job of this phase
+    const int njobs = sub == 0 ? QKV_JOBS : 1;
 
     // folded-LayerNorm vectors of this phase's features: requested now, parked in shared memory after the MMA loop (a global
     // load followed at once by its shared-memory store would park the warp for an L2 round trip in front of the MMAs)
@@ -437,34 +443,73 @@ __global__ void __launch_bounds__(THREADS, 1) decode_step_cluster_kernel(const _
       }
     }
 
-    // ---- MMA: this warp's q n-tiles (destination group dgrp) over its half of the CTA's K slice ----
-    for (int i = 0; i < njobs; i++) {
-      mbar_wait(&wbar[(j0 + i) & 1], (par_w >> ((j0 + i) & 1)) & 1u, 1);
-      par_w ^= 1u << ((j0 + i) & 1);
-    }
+    // ---- MMA: this warp's n-tiles over its K residue class of the CTA's slice ----
+    auto wait_job = [&](int j) {
+      mbar_wait(&wbar[j & 1], (par_w >> (j & 1)) & 1u, 1);
+      par_w ^= 1u << (j & 1);
+    };
+    auto ring = [&](int j) { return reinterpret_cast<const uint4*>(smem + HDR + (j & 1) * WB_BYTES) + lane; };
+    wait_job(j0);
+    if (sub == PH_QKV) wait_job(j0 + 1);
     mbar_wait(abar, par_a, 0);
     par_a ^= 1u;
     prof_mark(prof, 1);
     float acc[2][QMAX][4];
+    float4* const pass0 = reinterpret_cast<float4*>(Rg + R_PASS0) + (size_t)warp * QMAX * 32 + lane;   // head phases: [warp][n-tile][lane]
     RowStatFrag rst;
     row_stat_zero(rst);
     {
       const bf16* xs = reinterpret_cast<const bf16*>(Rg);
-      // QKV: destination groups 0,1 read the first weight job (n-tiles 0..11), groups 2,3 the second (12..23)
-      const int wjob = (sub == PH_QKV) ? j0 + (dgrp >> 1) : j0;
-      const int nt0 = (sub == PH_QKV) ? (dgrp & 1) * q : dgrp * q;   // first n-tile of this warp inside that job's slice
-      const uint4* wb = reinterpret_cast<const uint4*>(smem + HDR + (wjob & 1) * WB_BYTES) + (size_t)nt0 * KT * 32 + lane;
-      const int kt_lo = kh * (KT >> 1), kt_hi = kt_lo + (KT >> 1);
-      if (sub == PH_QKV) mma_slice<6, 1, 1, true>(acc, rst, xs, apitch, wb, KT, kt_lo, kt_hi, dgrp, lrow, lcol);
-      else if (sub == PH_QC) mma_slice<2, 1, 4, true>(acc, rst, xs, apitch, wb, KT, kt_lo, kt_hi, dgrp, lrow, lcol);
-      else if (sub == PH_FC1) {
-        if (q == 4) mma_slice<4, 2, 1, true>(acc, rst, xs, apitch, wb, KT, kt_lo, kt_hi, dgrp, lrow, lcol);
-        else if (q == 2) mma_slice<2, 2, 2, true>(acc, rst, xs, apitch, wb, KT, kt_lo, kt_hi, dgrp, lrow, lcol);
-        else mma_slice<1, 2, 4, true>(acc, rst, xs, apitch, wb, KT, kt_lo, kt_hi, dgrp, lrow, lcol);
-      } else if (fc2_wide) {
-        const uint4* wall = reinterpret_cast<const uint4*>(smem + HDR + (j0 & 1) * WB_BYTES) + lane;   // all four n-tiles
-        mma_slice<4, 2, 1, false>(acc, rst, xs, apitch, wall, KT, warp * (KT >> 3), (warp + 1) * (KT >> 3), 0, lrow, lcol);
-      } else mma_slice<1, 2, 4, false>(acc, rst, xs, apitch, wb, KT, kt_lo, kt_hi, dgrp, lrow, lcol);
+      if (rowpart) {
+        // 8 live rows: the ldmatrix rows 8-15 repeat rows 0-7 (what they produce is never read).  Pass P: warp group dgrp takes
+        // unit u = 2 P + dgrp of the head's n-tiles (QKV: weight job j0 + u; q_cross: n-tiles 2 u, 2 u + 1 of job j0).  Pass 0's
+        // tiles wait in shared memory (the attention scratch, idle until the exchange), pass 1's in acc[0].
+        auto head_pass = [&](auto pass_tag) {
+          constexpr int P = decltype(pass_tag)::value;
+          const int u = 2 * P + dgrp;
+          float t[2][QMAX][4];
+          if (sub == PH_QKV) mma_slice<6, 1, P == 0>(t, rst, xs, apitch, ring(j0 + u), KT, e4, KT, lrow & 7, lcol);
+          else mma_slice<2, 1, P == 0>(t, rst, xs, apitch, ring(j0) + (size_t)(2 * u) * KT * 32, KT, e4, KT, lrow & 7, lcol);
+#pragma unroll
+          for (int j = 0; j < QMAX; j++)
+            if (j < q) {
+              if (P == 0) pass0[j * 32] = make_float4(t[0][j][0], t[0][j][1], t[0][j][2], t[0][j][3]);
+              else {
+#pragma unroll
+                for (int e = 0; e < 4; e++) acc[0][j][e] = t[0][j][e];
+              }
+            }
+        };
+        head_pass(std::integral_constant<int, 0>{});
+        if (sub == PH_QKV) {   // quarters 2 and 3 of the head's QKV slice take the ring buffers of quarters 0 and 1
+          __syncthreads();
+          if (tid == 0) { issue_weight_job(j0 + 2); issue_weight_job(j0 + 3); }
+          wait_job(j0 + 2);
+          wait_job(j0 + 3);
+        }
+        head_pass(std::integral_constant<int, 1>{});
+      } else if (sub == PH_FC2) {
+        // quarter 2 rank + qq of F holds local k-tiles [qq KT, (qq + 1) KT) of the weight slice (2 KT per n-tile); the warp's
+        // residue class continues from the first quarter into the second in the same accumulators
+        auto quarter = [&](auto qq_tag) {
+          constexpr int QQ = decltype(qq_tag)::value;
+          const uint4* wq = ring(j0) + (size_t)dgrp * 2 * KT * 32 + (size_t)QQ * KT * 32;
+          mma_slice<1, 2, false, QQ == 1>(acc, rst, xs, apitch, wq, 2 * KT, (e4 - QQ * KT) & 3, KT, lrow, lcol);
+        };
+        quarter(std::integral_constant<int, 0>{});
+        __syncthreads();   // the first quarter is dead: the second one replaces it
+        if (tid == 0) request_slice(h_img + (size_t)(2 * rank + 1) * h_slice_elems, (uint32_t)(h_slice_elems * 2));
+        mbar_wait(abar, par_a, 0);
+        par_a ^= 1u;
+        quarter(std::integral_constant<int, 1>{});
+      } else {
+        const uint4* wb = ring(j0) + (size_t)(dgrp * q) * KT * 32;   // this destination's n-tiles
+        if (sub == PH_FC1) {
+          if (q == 4) mma_slice<4, 2, true>(acc, rst, xs, apitch, wb, KT, e4, KT, lrow, lcol);
+          else if (q == 2) mma_slice<2, 2, true>(acc, rst, xs, apitch, wb, KT, e4, KT, lrow, lcol);
+          else mma_slice<1, 2, true>(acc, rst, xs, apitch, wb, KT, e4, KT, lrow, lcol);
+        } else mma_slice<1, 2, false>(acc, rst, xs, apitch, wb, KT, e4, KT, lrow, lcol);
+      }
     }
     prof_mark(prof, 2);
     if (has_ln && tid < (rowpart ? Nc : 8 * q)) { cvec[tid] = cv1; cvec[256 + tid] = cv2; }   // read in the epilogue, several barriers later
@@ -486,44 +531,16 @@ __global__ void __launch_bounds__(THREADS, 1) decode_step_cluster_kernel(const _
 
     // ---- exchange: each warp stages its partial block in shared memory and ships it with ONE cp.async.bulk per destination
     // (shared::cta -> shared::cluster, complete_tx on the destination's mbarrier); no CTA-wide synchronisation on the way ----
-    //   feature-partitioned: warp (dgrp, kh) -> rank dgrp, slot 2 rank + kh: [stats 32 x 2][32 rows][RS]
-    //   row-partitioned    : warp w -> every rank d, slot 8 rank + w:        [stats 4 x 2][4 rows][8 q]  (rows 4d..4d+3, the warp's columns)
-    const int nslots = rowpart ? V * C : (fc2_wide ? C : V);
-    unsigned char* send = Rg + ((act_bytes + 127) & ~127);
-    unsigned char* recv = send + ((V * wsend + 127) & ~127);
+    //   feature-partitioned: warp (e4, dgrp) -> rank dgrp, slot 4 rank + e4: [stats 32 x 2][32 rows][RS]
+    //   row-partitioned    : warp w -> every rank d, slot 8 rank + w:        [stats 4 x 2][4 rows][16 q]  (rows 4d..4d+3, the warp's columns)
+    // The send blocks start at the head of R (over the dead activation slice), the receive slots behind both the send blocks and the
+    // activation slice.
+    const int nslots = rowpart ? V * C : V;
+    unsigned char* send = Rg;
+    const int send_end = V * wsend;
+    unsigned char* recv = Rg + (((send_end > act_bytes ? send_end : act_bytes) + 127) & ~127);
     if (tid == 0) mbar_expect_tx(xbar, (uint32_t)(nslots * blk));
-    if (fc2_wide) {
-      // stage the warp's four partial tiles in the (dead) activation slice: [warp][destination][32 rows][8] fp32
-      float* stg = reinterpret_cast<float*>(Rg) + (size_t)warp * (C * ROWS * 8);
-#pragma unroll
-      for (int mt = 0; mt < 2; mt++)
-#pragma unroll
-        for (int j = 0; j < 4; j++) {
-          float* base = stg + (size_t)j * (ROWS * 8) + (mt * 16 + g) * 8 + 2 * t4;
-          *reinterpret_cast<float2*>(base) = make_float2(acc[mt][j][0], acc[mt][j][1]);
-          *reinterpret_cast<float2*>(base + 64) = make_float2(acc[mt][j][2], acc[mt][j][3]);
-        }
-      __syncthreads();
-      prof_mark(prof, 14);
-      // warp w adds the eight tiles of destination w >> 1, rows 16 (w & 1) .. + 15 (lane: row l & 15, features 4 (l >> 4) .. + 3)
-      {
-        const int d = warp >> 1, row = 16 * (warp & 1) + (lane & 15), f0 = 4 * (lane >> 4);
-        const float* src = reinterpret_cast<const float*>(Rg) + (size_t)d * (ROWS * 8) + row * 8 + f0;
-        float4 v = *reinterpret_cast<const float4*>(src);
-#pragma unroll
-        for (int sw = 1; sw < 8; sw++) {
-          const float4 x = *reinterpret_cast<const float4*>(src + (size_t)sw * (C * ROWS * 8));
-          v.x += x.x; v.y += x.y; v.z += x.z; v.w += x.w;
-        }
-        unsigned char* blk_d = send + (size_t)d * blk;
-        *reinterpret_cast<float4*>(reinterpret_cast<float*>(blk_d + 256) + row * RS + f0) = v;
-        asm volatile("bar.sync %0, 64;" ::"r"((warp >> 1) + 1) : "memory");   // the two warps of this destination
-        if ((warp & 1) == 0 && lane == 0) {
-          fence_proxy_async_smem();
-          bulk_s2peer(mapa(s32(recv + (size_t)rank * blk), (uint32_t)d), blk_d, (uint32_t)blk, mapa(s32(xbar), (uint32_t)d));
-        }
-      }
-    } else {
+    {
       unsigned char* mine = send + (size_t)warp * wsend;
       const bool merged = rowpart && !(p.dbg & 1024);
       if (!rowpart) {
@@ -538,7 +555,7 @@ __global__ void __launch_bounds__(THREADS, 1) decode_step_cluster_kernel(const _
               *reinterpret_cast<float2*>(base + 8 * RS) = make_float2(acc[mt][j][2], acc[mt][j][3]);
             }
           }
-        if (has_ln) {   // (S1, S2) of rows g / g+8 of each m-tile over this warp's K half (lane layout: ln_stats.cuh)
+        if (has_ln) {   // (S1, S2) of rows g / g+8 of each m-tile over this warp's K class (lane layout: ln_stats.cuh)
           float* st = reinterpret_cast<float*>(mine);
 #pragma unroll
           for (int mt = 0; mt < 2; mt++) {
@@ -551,29 +568,28 @@ __global__ void __launch_bounds__(THREADS, 1) decode_step_cluster_kernel(const _
           }
         }
       } else {
-        const int qc = 8 * q;   // this warp's columns
+        const int qc = 16 * q;   // this warp's columns: pass 0, then pass 1
+        // live row g (fragment elements 0, 1) -> destination rank g >> 2, row g & 3 of its block.  [destination][warp] order, so
+        // that ONE copy per destination ships all eight warps' blocks (every bulk copy costs issue time through the uniform datapath,
+        // on every warp's critical path; PTTS_DBG=1024 keeps the per-warp copies, [warp][destination] order)
+        unsigned char* blk_d = merged ? send + ((size_t)(g >> 2) * V + warp) * blk : mine + (size_t)(g >> 2) * blk;
+        float* bp = reinterpret_cast<float*>(blk_d + 32) + (g & 3) * qc + 2 * t4;
 #pragma unroll
-        for (int hh = 0; hh < 2; hh++) {
-          const int row = g + 8 * hh;
-          // block of destination rank d = row >> 2: [destination][warp] order, so that ONE copy per destination ships all eight warps'
-          // blocks (every bulk copy costs issue time through the uniform datapath, on every warp's critical path;
-          // PTTS_DBG=1024 keeps the per-warp copies, [warp][destination] order)
-          unsigned char* blk_d = merged ? send + ((size_t)(row >> 2) * V + warp) * blk : mine + (size_t)(row >> 2) * blk;
-          float* bp = reinterpret_cast<float*>(blk_d + 32) + (row & 3) * qc + 2 * t4;
+        for (int P = 0; P < 2; P++)
 #pragma unroll
           for (int j = 0; j < QMAX; j++)
-            if (j < q) *reinterpret_cast<float2*>(bp + j * 8) = make_float2(acc[0][j][2 * hh], acc[0][j][2 * hh + 1]);
-          float* st = reinterpret_cast<float*>(blk_d) + (row & 3) * 2;
-          if (t4 == 0) st[0] = hh ? rst.s1[0][2] : rst.s1[0][0];
-          if (t4 == (g >> 1)) st[1] = hh ? ((g & 1) ? rst.sq[0][1][3] : rst.sq[0][1][2]) : ((g & 1) ? rst.sq[0][0][1] : rst.sq[0][0][0]);
-        }
+            if (j < q) *reinterpret_cast<float2*>(bp + P * 8 * q + j * 8) = P == 0 ? make_float2(pass0[j * 32].x, pass0[j * 32].y)
+                                                                                   : make_float2(acc[0][j][0], acc[0][j][1]);
+        float* st = reinterpret_cast<float*>(blk_d) + (g & 3) * 2;
+        if (t4 == 0) st[0] = rst.s1[0][0];
+        if (t4 == (g >> 1)) st[1] = (g & 1) ? rst.sq[0][0][1] : rst.sq[0][0][0];
       }
       __syncwarp();
       prof_mark(prof, 14);
       if (!rowpart) {
         if (lane == 0) {
           fence_proxy_async_smem();
-          bulk_s2peer(mapa(s32(recv + (size_t)(2 * rank + kh) * blk), (uint32_t)dgrp), mine, (uint32_t)blk, mapa(s32(xbar), (uint32_t)dgrp));
+          bulk_s2peer(mapa(s32(recv + (size_t)(4 * rank + e4) * blk), (uint32_t)dgrp), mine, (uint32_t)blk, mapa(s32(xbar), (uint32_t)dgrp));
         }
       } else if (merged) {
         __syncthreads();   // all eight warps' blocks are staged
@@ -586,57 +602,10 @@ __global__ void __launch_bounds__(THREADS, 1) decode_step_cluster_kernel(const _
         bulk_s2peer(mapa(s32(recv + (size_t)(8 * rank + warp) * blk), (uint32_t)lane), mine + (size_t)lane * blk, (uint32_t)blk, mapa(s32(xbar), (uint32_t)lane));
       }
     }
-    // Requests that are not on the critical path go out now, while the partial sums travel: the weight ring's refill (two jobs
-    // ahead; q_cross holds fc1's weights back until its attention is done, the K/V rings live in that buffer meanwhile) and, for
-    // the head phases, the first K/V stage of this warp's attention item.  The rings live in the weight ring's idle space (the
-    // phase's own weights are dead, the next jobs fill only the heads of the buffers), so they alias nothing the exchange uses.
-    if (warp == 1 && lane == 0 && sub != PH_QC) for (int i = 0; i < njobs; i++) issue_weight_job(j0 + i + 2);
-    TcItem item{};
-    int att_b = B;
-    unsigned char* att_ring = nullptr; unsigned char* att_ring1 = nullptr; float* att_f = nullptr; float* att_xch = nullptr;
-    if (rowpart) {
-      // row b = 16 half + 4 rank + (warp >> 1), this cluster's head: q at qkv_s[warp >> 1][0..63] (k at +64, v at +128 in the self phase)
-      const bf16* qrow = reinterpret_cast<const bf16*>(Rg + QKV_OFF) + (size_t)(warp >> 1) * Nc;
-      att_b = att_row;
-      item.q = qrow;
-      item.pos = pos; item.rope = p.rope; item.scale = p.scale;
-      item.rope_cos = reinterpret_cast<const bf16*>(blob + p.rope_cos); item.rope_sin = reinterpret_cast<const bf16*>(blob + p.rope_sin);
-      // attn image: row b, head h -> slice h / 4, column (h % 4) * 64
-      item.out = att_out;
-      unsigned char* wb0 = smem + HDR;   // the two weight ring buffers
-      if (sub == PH_QKV) {
-        item.knew = qrow + HD; item.vnew = qrow + 2 * HD;
-        bf16* kc = reinterpret_cast<bf16*>(p.self_kv + p.self_layer_stride * l) + self_item;
-        item.kc = kc; item.vc = kc + self_vofs;
-        item.km = p.prompt_mask ? p.prompt_mask + (size_t)att_b * p.P : nullptr; item.mask_len = p.P;
-        item.cross = 0; item.n_cached = pos;
-        // out-proj's 16 KB go to the head of buffer (j0+2)&1, q_cross's 32 KB to the head of the other one.  Stage 0 of every warp
-        // (requested now) sits in those buffers' tails; stage 1 (requested when the attention starts) in what the exchange has
-        // released by then: the receive slots [34 KB, 58 KB) and the activation slice [0, 8 KB) of R, the gap behind the query
-        // scratch [71 KB, 87 KB), and the rest of the q_cross buffer's tail.
-        unsigned char* bB = wb0 + ((j0 + 2) & 1) * WB_BYTES; unsigned char* bC = wb0 + ((j0 + 3) & 1) * WB_BYTES;
-        att_ring = warp < 6 ? bB + 16384 + warp * ATT_TC_STAGE_BYTES : bC + 32768 + (warp - 6) * ATT_TC_STAGE_BYTES;
-        att_ring1 = warp < 3 ? Rg + 34048 + warp * ATT_TC_STAGE_BYTES : (warp < 5 ? Rg + 72704 + (warp - 3) * ATT_TC_STAGE_BYTES
-                  : (warp == 5 ? Rg : bC + 49152 + (warp - 6) * ATT_TC_STAGE_BYTES));
-        att_xch = reinterpret_cast<float*>(Rg + 59648) + (warp >> 1) * 128;
-      } else {
-        item.knew = nullptr; item.vnew = nullptr;
-        bf16* ck = reinterpret_cast<bf16*>(p.cross_kv + p.cross_layer_stride * l) + cross_item;
-        item.kc = ck; item.vc = ck + cross_vofs;
-        item.km = p.enc_mask ? p.enc_mask + (size_t)att_b * p.S : nullptr; item.mask_len = p.S;
-        item.cross = 1; item.n_cached = p.S;
-        // this phase's own (dead) weight buffer holds stage 0 of every warp; cross out-proj's 16 KB sit at the head of the other one.
-        // Stage 1 (descriptions longer than 64 positions): R behind the exchange buffers, the gap behind the query scratch, and
-        // the cross out-proj buffer's tail.
-        unsigned char* bD = wb0 + ((j0 + 1) & 1) * WB_BYTES;
-        att_ring = wb0 + (j0 & 1) * WB_BYTES + warp * ATT_TC_STAGE_BYTES;
-        att_ring1 = warp < 4 ? Rg + 28672 + warp * ATT_TC_STAGE_BYTES : (warp < 6 ? Rg + 72704 + (warp - 4) * ATT_TC_STAGE_BYTES
-                  : bD + 16384 + (warp - 6) * ATT_TC_STAGE_BYTES);
-        att_xch = reinterpret_cast<float*>(bD + 32768) + (warp >> 1) * 128;
-      }
-      att_f = reinterpret_cast<float*>(Rg + 65536) + warp * 192;   // query / new key / new value: a corner of R the exchange never uses
-      if (att_b < B && !(p.dbg & 16)) attention_tc_issue_first(item, att_ring, attbars + 2 * warp, lane, warp & 1, 2, !(p.dbg & 256));
-    }
+    // The weight ring's refill goes out now, while the partial sums travel (two jobs ahead; the head phases hold the next head
+    // phase's or fc1's weights back until their attention is done: the attention uses that buffer meanwhile).
+    if (warp == 1 && lane == 0 && !rowpart) issue_weight_job(j0 + 2);
+    if (warp == 1 && lane == 0 && sub == PH_QKV) issue_weight_job(j0 + QKV_JOBS);   // out-proj
     prof_mark(prof, 15);
     mbar_wait(xbar, par_x, 2);
     par_x ^= 1u;
@@ -664,26 +633,19 @@ __global__ void __launch_bounds__(THREADS, 1) decode_step_cluster_kernel(const _
         }
 #pragma unroll
         for (int e = 0; e < 4; e++) v[e] = apply_act(DT<bf16>::rnd(ln_rstd * (v[e] - ln_mean * cvec[f + e]) + cvec[256 + f + e]), p.act);
-        const int n = cta * 32 + f;
         uint2 pk;
         pk.x = att_pack(v[0], v[1]); pk.y = att_pack(v[2], v[3]);
-        *reinterpret_cast<uint2*>(h_img + (size_t)(n / KsF) * h_slice_elems + row * pitchF + (n % KsF)) = pk;
+        *reinterpret_cast<uint2*>(h_img + h_offset(cta * 32 + f) + row * pitchF) = pk;
       } else if (row < B) {
         for (int i = 0; i < q; i++) {
           const int f = f0 + 8 * i;
           float v = 0.f;
-          if (fc2_wide) {
 #pragma unroll
-            for (int sv = 0; sv < C; sv++) v += reinterpret_cast<const float*>(recv + (size_t)sv * blk + 256)[row * RS + f];
-          } else {
-#pragma unroll
-            for (int sv = 0; sv < V; sv++) v += reinterpret_cast<const float*>(recv + (size_t)sv * blk + 256)[row * RS + f];
-          }
+          for (int sv = 0; sv < V; sv++) v += reinterpret_cast<const float*>(recv + (size_t)sv * blk + 256)[row * RS + f];
           if (sub == PH_FC1) {
             v = ln_rstd * (v - ln_mean * cvec[f]) + cvec[256 + f];
             v = apply_act(DT<bf16>::rnd(v), p.act);
-            const int n = cta * 8 * q + f;   // h feature -> slice n / KsF of the fc2 image
-            h_img[(size_t)(n / KsF) * h_slice_elems + row * pitchF + (n % KsF)] = __float2bfloat16_rn(v);
+            h_img[h_offset(cta * 8 * q + f) + row * pitchF] = __float2bfloat16_rn(v);
           } else {  // out-proj / cross out-proj / fc2: residual add on the slice this CTA owns
             v = DT<bf16>::rnd(res_s[row * 8 + f] + DT<bf16>::rnd(v));
             res_s[row * 8 + f] = v;
@@ -693,84 +655,86 @@ __global__ void __launch_bounds__(THREADS, 1) decode_step_cluster_kernel(const _
       }
     } else {
       bf16* qkv_s = reinterpret_cast<bf16*>(Rg + QKV_OFF);  // [4][Nc]
-      auto gather = [&](auto qc_tag) {   // (the column count per warp is a constant of the phase: no run-time divisions)
-        constexpr int QC = decltype(qc_tag)::value, NC = 4 * QC;
+      auto gather = [&](auto jw_tag) {   // (the column counts are constants of the phase: no run-time divisions)
+        constexpr int JW = decltype(jw_tag)::value, NC = 4 * JW, QCW = 2 * JW;   // columns of a unit, of the head, of a warp
         for (int idx = tid; idx < 4 * NC; idx += THREADS) {
           const int r4 = idx / NC, col = idx - r4 * NC;
-          const int dg = col / QC, cw = col - dg * QC;           // the warps with dgrp == dg hold this column
-          // row 16 half + 4 rank + r4: statistics from the dgrp == 0 warp of every (source rank, K half), added by every thread itself
-          // (broadcast loads: a warp's 32 elements share the row) instead of a 4-thread pass + CTA barrier
+          const int u = col / JW, cw = (u >> 1) * JW + (col - u * JW);   // unit u = 2 pass + warp group: the warps with dgrp == u & 1
+          // row 8 rblk + 4 rank + r4: statistics from the dgrp == 0 warp of every K class, added by every thread itself (broadcast
+          // loads: a warp's 32 elements share the row) instead of a 4-thread pass + CTA barrier
           float S1 = 0.f, S2 = 0.f;
 #pragma unroll
-          for (int sr = 0; sr < C; sr++)
-#pragma unroll
-            for (int k2 = 0; k2 < 2; k2++) {
-              const float2 x = *reinterpret_cast<const float2*>(recv + (size_t)(8 * sr + 4 * k2) * blk + r4 * 8);
-              S1 += x.x; S2 += x.y;
-            }
+          for (int e = 0; e < V; e++) {
+            const float2 x = *reinterpret_cast<const float2*>(recv + (size_t)(8 * (e >> 2) + 2 * (e & 3)) * blk + r4 * 8);
+            S1 += x.x; S2 += x.y;
+          }
           const float ln_mean = S1 / (float)H;
           const float ln_rstd = rsqrtf(fmaxf(S2 / (float)H - ln_mean * ln_mean, 0.f) + p.eps);
           float v = 0.f;
 #pragma unroll
-          for (int sv = 0; sv < V; sv++)   // (source rank, K half) in order: warp index = 4 (sv & 1) + dg of rank sv >> 1
-            v += reinterpret_cast<const float*>(recv + (size_t)(8 * (sv >> 1) + 4 * (sv & 1) + dg) * blk + 32)[r4 * QC + cw];
+          for (int e = 0; e < V; e++)   // K classes in order: warp 2 (e & 3) + (u & 1) of rank e >> 2
+            v += reinterpret_cast<const float*>(recv + (size_t)(8 * (e >> 2) + 2 * (e & 3) + (u & 1)) * blk + 32)[r4 * QCW + cw];
           v = ln_rstd * (v - ln_mean * cvec[col]) + cvec[256 + col];
           qkv_s[idx] = __float2bfloat16_rn(v);
         }
       };
       if (sub == PH_QKV) gather(std::integral_constant<int, 48>{}); else gather(std::integral_constant<int, 16>{});
-      static_assert(HD == 64, "q = 6 (q|k|v of a head over 4 warps) and q = 2 n-tiles per warp");
+      static_assert(HD == 64, "QKV: 2 x 2 units of 6 n-tiles (q|k|v of a head), q_cross: 2 x 2 units of 2 n-tiles");
     }
     prof_mark(prof, 4);
     __syncthreads();   // this CTA's receive slots are consumed (and q|k|v complete): peers may send the next phase's partials
     cluster_arrive_reuse((p.dbg & 64) != 0);
-    if (rowpart && (p.dbg & 16)) {
-      // the SIMT attention's scratch aliases the send blocks: the peers must have RECEIVED them (each is past its exchange wait) first
+    if (rowpart) {
+      // the attention's scratch aliases the send blocks: the peers must have RECEIVED them (each is past its exchange wait) first
       cluster_wait();
       cluster_arrive();  // re-arm for the next phase's "exchange buffers free" wait
     }
 
-    // ---- attention of this rank's 4 (row, head) items: two warps per item (first two K/V stages were requested after the MMA) ----
+    // ---- attention of this rank's 4 (row, head) items: two warps per item, the sweep and the call step.cu's attention phase
+    // makes (same key chunks, same split over the two warps, same merge), so the two step kernels agree bit for bit ----
     if (rowpart) {
-      if (att_b < B) {
-        if (p.dbg & 16) {  // A/B: the SIMT sweep (its ring layout: K/V stages then 192 floats, inside the R region)
-          AttnArgs att{};
-          att.ctrl = nullptr; att.B = B; att.nh = p.nh; att.nkv = p.nh; att.q_len = 1;
-          att.past_from_ctrl = 0; att.past_len = pos; att.prefix = p.P;
-          att.rope = p.rope; att.rope_cos = blob + p.rope_cos; att.rope_sin = blob + p.rope_sin; att.scale = p.scale;
-          const bf16* qkv_s = reinterpret_cast<const bf16*>(Rg + QKV_OFF);
-          const int row_base = 16 * half + 4 * rank;
-          const bf16* qbase = qkv_s - (size_t)row_base * Nc - (size_t)head * HD;
-          att.q = qbase; att.ldq = Nc; att.q_col0 = 0;
-          att.ldo = pitch;
-          att.out = a_img + (size_t)att_slice * x_slice_elems + att_col - (size_t)head * HD;
-          if (sub == PH_QKV) {
-            att.knew = qbase; att.vnew = qbase; att.ldkv = Nc; att.k_col0 = HD; att.v_col0 = 2 * HD;
-            char* kc = p.self_kv + p.self_layer_stride * l;
-            att.kcache = kc; att.vcache = kc + (size_t)B * p.nh * p.Tmax * HD * 2;
-            att.kv_b_stride = (int64_t)p.nh * p.Tmax * HD; att.kv_h_stride = (int64_t)p.Tmax * HD; att.kv_t_stride = HD;
-            att.key_mask = p.prompt_mask; att.mask_len = p.P; att.mask_ld = p.P;
-            att.cross = 0; att.kv_len = 0; att.kv_capacity = p.Tmax;
-          } else {
-            att.knew = nullptr; att.vnew = nullptr;
-            char* ck = p.cross_kv + p.cross_layer_stride * l;
-            att.kcache = ck; att.vcache = ck + (size_t)B * p.nh * p.S * HD * 2;
-            att.kv_b_stride = (int64_t)p.nh * p.S * HD; att.kv_h_stride = (int64_t)p.S * HD; att.kv_t_stride = HD;
-            att.key_mask = p.enc_mask; att.mask_len = p.S; att.mask_ld = p.S;
-            att.cross = 1; att.kv_len = p.S; att.kv_capacity = p.S;
-          }
-          unsigned char* region = Rg + (size_t)warp * attn_decode_smem_per_warp<bf16, ATT_CH>();
-          float* xr = reinterpret_cast<float*>(Rg + 73728) + (warp >> 1) * 128;
-          attention_decode_item_warp<bf16, ATT_CH>(att, att_b, head, pos, region, attbars + 2 * warp, lane, att_parity, warp & 1, 2, xr, (warp >> 1) + 1);
+      if (att_row < B) {
+        AttnArgs att{};
+        att.ctrl = nullptr; att.B = B; att.nh = p.nh; att.nkv = p.nh; att.q_len = 1;
+        att.past_from_ctrl = 0; att.past_len = pos; att.prefix = p.P;
+        att.rope = p.rope; att.rope_cos = blob + p.rope_cos; att.rope_sin = blob + p.rope_sin; att.scale = p.scale;
+        const bf16* qkv_s = reinterpret_cast<const bf16*>(Rg + QKV_OFF);
+        const int row_base = HROWS * rblk + 4 * rank;
+        const bf16* qbase = qkv_s - (size_t)row_base * Nc - (size_t)head * HD;
+        att.q = qbase; att.ldq = Nc; att.q_col0 = 0;
+        att.ldo = pitch;
+        att.out = a_img + (size_t)att_slice * x_slice_elems + att_col - (size_t)head * HD;
+        if (sub == PH_QKV) {
+          att.knew = qbase; att.vnew = qbase; att.ldkv = Nc; att.k_col0 = HD; att.v_col0 = 2 * HD;
+          char* kc = p.self_kv + p.self_layer_stride * l;
+          att.kcache = kc; att.vcache = kc + (size_t)B * p.nh * p.Tmax * HD * 2;
+          att.kv_b_stride = (int64_t)p.nh * p.Tmax * HD; att.kv_h_stride = (int64_t)p.Tmax * HD; att.kv_t_stride = HD;
+          att.key_mask = p.prompt_mask; att.mask_len = p.P; att.mask_ld = p.P;
+          att.cross = 0; att.kv_len = 0; att.kv_capacity = p.Tmax;
         } else {
-          attention_decode_item_warp_tc(item, att_ring, att_ring1, att_f, attbars + 2 * warp, lane, att_parity, warp & 1, 2, att_xch,
-                                        (warp >> 1) + 1, warp == 0 ? prof : nullptr, true, !(p.dbg & 256));
+          att.knew = nullptr; att.vnew = nullptr;
+          char* ck = p.cross_kv + p.cross_layer_stride * l;
+          att.kcache = ck; att.vcache = ck + (size_t)B * p.nh * p.S * HD * 2;
+          att.kv_b_stride = (int64_t)p.nh * p.S * HD; att.kv_h_stride = (int64_t)p.S * HD; att.kv_t_stride = HD;
+          att.key_mask = p.enc_mask; att.mask_len = p.S; att.mask_ld = p.S;
+          att.cross = 1; att.kv_len = p.S; att.kv_capacity = p.S;
         }
+        // per-warp scratch (K/V ring stages, then 192 floats): warps 0-4 in R below the q|k|v rows, warps 5-7 in the weight buffer
+        // whose job is held back; the pair merge in the other buffer's tail, behind out-proj's / cross out-proj's 16 KB
+        unsigned char* wb0 = smem + HDR;
+        unsigned char* held = wb0 + ((sub == PH_QKV ? j0 + 1 : j0) & 1) * WB_BYTES;
+        unsigned char* other = wb0 + ((sub == PH_QKV ? j0 : j0 + 1) & 1) * WB_BYTES;
+        unsigned char* region = warp < 5 ? Rg + (size_t)warp * ATT_SMEM : held + (size_t)(warp - 5) * ATT_SMEM;
+        float* xr = reinterpret_cast<float*>(other + 16384) + (warp >> 1) * 128;
+        attention_decode_item_warp<bf16>(att, att_row, head, pos, region, attbars + 2 * warp, lane, att_parity, warp & 1, 2, xr, (warp >> 1) + 1);
       }
       prof_mark(prof, 5);
-      if (sub == PH_QC) {   // fc1's weights were held back: the K/V rings used their buffer
-        __syncthreads();
-        if (tid == 32) issue_weight_job(j0 + 2);
+      // q_cross's (QKV phase) or fc1's (q_cross phase) weights were held back: the attention used their buffer (its floats are
+      // written with generic stores: the fence orders them before the bulk copy's writes)
+      __syncthreads();
+      if (tid == 32) {
+        fence_proxy_async_smem();
+        issue_weight_job(sub == PH_QKV ? j0 + QKV_JOBS + 1 : j0 + 2);
       }
     }
     prof_mark(prof, 6);
@@ -790,7 +754,8 @@ __global__ void __launch_bounds__(THREADS, 1) decode_step_cluster_kernel(const _
   }
   cluster_wait();  // balance the last phase's arrive
 
-  // ---- final LayerNorm + K lm heads: N-split over all CTAs (4 n-tiles per task, full K), no exchange ----
+  // ---- final LayerNorm + K lm heads: N-split over all CTAs (4 n-tiles per task, full K), no exchange; warp w reduces the
+  // k-tiles kt = w (mod 8) and the eight partial tiles are added in warp order, as step.cu's lm-head phase does ----
   prof = prof0 ? prof0 + (size_t)(n_phases + 1) * PROF_STRIDE : nullptr;
   prof_mark(prof, 0);
   {
@@ -802,13 +767,14 @@ __global__ void __launch_bounds__(THREADS, 1) decode_step_cluster_kernel(const _
     }
     mbar_wait(abar, par_a, 3);
     par_a ^= 1u;
-    const bf16* xs = reinterpret_cast<const bf16*>(Rg);   // [4 slices][32][pitch]
-    const int KTH = H >> 5, KTS = Ks >> 5;                 // k32 tiles of the full row / of one slice
+    const bf16* xs = reinterpret_cast<const bf16*>(Rg);   // [2 slices][32][pitch]
+    const int KTH = H >> 5;                                // k32 tiles of the full row
+    auto ktile = [&](int kt) { return xs + (size_t)kslice(kt) * x_slice_elems + klocal(kt) * 32; };
     {  // row statistics over the full rows: k-tile kt by warp kt % 8
       RowStatFrag rst;
       row_stat_zero(rst);
       for (int kt = warp; kt < KTH; kt += 8) {
-        const bf16* sl = xs + (size_t)(kt / KTS) * x_slice_elems + (kt % KTS) * 32;
+        const bf16* sl = ktile(kt);
 #pragma unroll
         for (int mt = 0; mt < 2; mt++)
 #pragma unroll
@@ -824,58 +790,67 @@ __global__ void __launch_bounds__(THREADS, 1) decode_step_cluster_kernel(const _
       __syncthreads();
     }
     prof_mark(prof, 1);
-    float* red = reinterpret_cast<float*>(Rg + (size_t)C * x_slice_elems * 2);  // [4 n-tiles][32][8] partials of the upper K half
-    const int jn = warp >> 1, khh = warp & 1;   // this warp: n-tile jn of the task, K half khh
+    constexpr int HRS = 40;   // row stride (floats) of the partial tiles [8 warps][32 rows][HRS]: conflict-free epilogue reads
     int job = JOBS_PER_LAYER * p.L;
     for (int task = cta; task < ntasks; task += (int)gridDim.x, job++) {
       mbar_wait(&wbar[job & 1], (par_w >> (job & 1)) & 1u, 4);
       par_w ^= 1u << (job & 1);
-      float acc[2][4];
+      float acc[2][4][4];
 #pragma unroll
       for (int a = 0; a < 2; a++)
 #pragma unroll
-        for (int e = 0; e < 4; e++) acc[a][e] = 0.f;
-      const uint4* wb = reinterpret_cast<const uint4*>(smem + HDR + (job & 1) * WB_BYTES) + (size_t)jn * KTH * 32 + lane;
-      for (int kt = khh * (KTH / 2); kt < (khh + 1) * (KTH / 2); kt++) {
-        const bf16* sl = xs + (size_t)(kt / KTS) * x_slice_elems + (kt % KTS) * 32;
-        const uint4 w = wb[(size_t)kt * 32];
+        for (int j = 0; j < 4; j++)
 #pragma unroll
-        for (int mt = 0; mt < 2; mt++) {
-          uint32_t a0[4], a1[4];
-          ldsm4(a0, sl + (size_t)(mt * 16 + lrow) * pitch + lcol);
-          ldsm4(a1, sl + (size_t)(mt * 16 + lrow) * pitch + 16 + lcol);
-          mma_bf16_16816(acc[mt], a0, w.x, w.y);
-          mma_bf16_16816(acc[mt], a1, w.z, w.w);
-        }
-      }
-      if (khh == 1) {
-#pragma unroll
-        for (int mt = 0; mt < 2; mt++) {
-          float* base = red + ((size_t)jn * 32 + mt * 16 + g) * 8 + 2 * t4;
-          *reinterpret_cast<float2*>(base) = make_float2(acc[mt][0], acc[mt][1]);
-          *reinterpret_cast<float2*>(base + 64) = make_float2(acc[mt][2], acc[mt][3]);
-        }
-      }
-      __syncthreads();  // weight buffer dead, upper-half partials visible
-      if (tid == 32) issue_weight_job(job + 2);
-      if (khh == 0) {
-        const int n0 = task * 32 + jn * 8 + 2 * t4;
-        const float2 c1v = *reinterpret_cast<const float2*>(c1 + n0), c2v = *reinterpret_cast<const float2*>(c2 + n0);
+          for (int e = 0; e < 4; e++) acc[a][j][e] = 0.f;
+      unsigned char* wbuf = smem + HDR + (job & 1) * WB_BYTES;
+      const uint4* wb = reinterpret_cast<const uint4*>(wbuf) + lane;
+      for (int kt = warp; kt < KTH; kt += 8) {
+        const bf16* sl = ktile(kt);
+        uint32_t a[2][2][4];
 #pragma unroll
         for (int mt = 0; mt < 2; mt++)
 #pragma unroll
-          for (int hh = 0; hh < 2; hh++) {
-            const int row = mt * 16 + g + 8 * hh;
-            if (row < B) {
-              const float2 up = *reinterpret_cast<const float2*>(red + ((size_t)jn * 32 + row) * 8 + 2 * t4);
-              const float mean = stats[2 * row], rstd = stats[2 * row + 1];
-              const float v0 = DT<bf16>::rnd(rstd * (acc[mt][2 * hh] + up.x - mean * c1v.x) + c2v.x);
-              const float v1 = DT<bf16>::rnd(rstd * (acc[mt][2 * hh + 1] + up.y - mean * c1v.y) + c2v.y);
-              *reinterpret_cast<float2*>(p.logits + (size_t)row * p.K * p.V + n0) = make_float2(v0, v1);
-            }
+          for (int j = 0; j < 2; j++) ldsm4(a[mt][j], sl + (size_t)(mt * 16 + lrow) * pitch + j * 16 + lcol);
+#pragma unroll
+        for (int j = 0; j < 4; j++) {
+          const uint4 w = wb[((size_t)j * KTH + kt) * 32];
+#pragma unroll
+          for (int mt = 0; mt < 2; mt++) {
+            mma_bf16_16816(acc[mt][j], a[mt][0], w.x, w.y);
+            mma_bf16_16816(acc[mt][j], a[mt][1], w.z, w.w);
           }
+        }
       }
-      __syncthreads();  // `red` is reused by the next task
+      __syncthreads();  // the weight buffer is dead: it takes the partial tiles
+      float* red = reinterpret_cast<float*>(wbuf);
+#pragma unroll
+      for (int mt = 0; mt < 2; mt++)
+#pragma unroll
+        for (int j = 0; j < 4; j++) {
+          float* base = red + ((size_t)warp * 32 + mt * 16 + g) * HRS + j * 8 + 2 * t4;
+          *reinterpret_cast<float2*>(base) = make_float2(acc[mt][j][0], acc[mt][j][1]);
+          *reinterpret_cast<float2*>(base + 8 * HRS) = make_float2(acc[mt][j][2], acc[mt][j][3]);
+        }
+      __syncthreads();
+      {
+        const int er = tid >> 3, ec = tid & 7;
+        if (er < B) {
+          const float mean = stats[2 * er], rstd = stats[2 * er + 1];
+#pragma unroll
+          for (int j = 0; j < 4; j++) {
+            const int cidx = j * 8 + ec, n = task * 32 + cidx;
+            float v = 0.f;
+#pragma unroll
+            for (int w = 0; w < 8; w++) v += red[((size_t)w * 32 + er) * HRS + cidx];
+            p.logits[(size_t)er * p.K * p.V + n] = DT<bf16>::rnd(rstd * (v - mean * c1[n]) + c2[n]);
+          }
+        }
+      }
+      __syncthreads();  // the partial tiles are consumed: the buffer takes job + 2 (the fence orders their generic writes first)
+      if (tid == 32) {
+        fence_proxy_async_smem();
+        issue_weight_job(job + 2);
+      }
     }
   }
   prof_mark(prof, 6);
@@ -922,18 +897,18 @@ __global__ void __launch_bounds__(THREADS, 1) decode_step_cluster_kernel(const _
 
 // ---- weight repack: fragment-order matrices -> one contiguous slice per (phase, cluster or head, rank) -------------------
 // Both layouts are made of the same 512-byte (n8 x k32) tiles, so the repack is a tile gather.
-//   head phases (QKV, q_cross): slice (head, rank) = the head's n-tiles x k-tiles [rank kts, (rank + 1) kts)
-//   the others: slice cta = cluster * 4 + rank = the cluster's ntc n-tiles x the rank's k-tiles
+//   head phases (QKV, q_cross): slice (head, rank) = the head's n-tiles x the rank's k-tiles kglobal(rank, 0 .. kts - 1)
+//   the others: slice cta = cluster * 2 + rank = the cluster's ntc n-tiles x the rank's k-tiles
 __global__ void cluster_pack_kernel(const uint4* __restrict__ src, uint4* __restrict__ dst, int ph, int nh, int ntc, int kts, int KT_src) {
   const int64_t tile = blockIdx.x;   // dst tile index = (slice * ntc + j) * kts + ktl
   const int ktl = (int)(tile % kts);
   const int j = (int)((tile / kts) % ntc);
   const int slice = (int)(tile / ((int64_t)kts * ntc));
-  const int rank = slice & 3, owner = slice >> 2;   // owner = head (head phases) or cluster
+  const int rank = slice & 1, owner = slice >> 1;   // owner = head (head phases) or cluster
   int n_tile;
   if (ph == PH_QKV) n_tile = (j >> 3) * (nh * 8) + owner * 8 + (j & 7);   // q | k | v rows of head `owner` in the fused matrix
   else n_tile = owner * ntc + j;
-  const int kt = rank * kts + ktl;
+  const int kt = kglobal(rank, ktl);
   dst[tile * 32 + threadIdx.x] = src[((int64_t)n_tile * KT_src + kt) * 32 + threadIdx.x];
 }
 
@@ -942,13 +917,13 @@ __global__ void cluster_pack_kernel(const uint4* __restrict__ src, uint4* __rest
 // ---- host side ----------------------------------------------------------------------------------
 int cluster_pack_layer(const char* layer_src, char* layer_dst, const int64_t* mat_off, const int64_t* cp_off, int nh, int H, int F, cudaStream_t st) {
   // mat_off: byte offsets (inside the layer) of wqkv, wo, wqc, woc, fc1, fc2; cp_off: of the six packed regions
-  const int ks = H / 4 / 32, ksf = F / 4 / 32;
-  const int ntc[6] = {24, 4, 8, 4, F / (2 * nh) / 8, 4};
-  const int owners[6] = {nh, 2 * nh, nh, 2 * nh, 2 * nh, 2 * nh};
+  const int ks = H / cl::C / 32, ksf = F / cl::C / 32;
+  const int ntc[6] = {24, 2, 8, 2, F / (4 * nh) / 8, 2};
+  const int owners[6] = {nh, 4 * nh, nh, 4 * nh, 4 * nh, 4 * nh};
   for (int ph = 0; ph < 6; ph++) {
     const int kts = (ph == 5) ? ksf : ks;
     const int KT_src = (ph == 5) ? F / 32 : H / 32;
-    const int64_t tiles = (int64_t)owners[ph] * 4 * ntc[ph] * kts;
+    const int64_t tiles = (int64_t)owners[ph] * cl::C * ntc[ph] * kts;
     cl::cluster_pack_kernel<<<(unsigned)tiles, 32, 0, st>>>(reinterpret_cast<const uint4*>(layer_src + mat_off[ph]),
                                                             reinterpret_cast<uint4*>(layer_dst + cp_off[ph]), ph, nh, ntc[ph], kts, KT_src);
   }
@@ -964,7 +939,7 @@ static const void* cluster_kernel_fn(const StepParams& p) {
 
 static void cluster_launch_config(const StepParams& p, cudaLaunchConfig_t& cfg, cudaLaunchAttribute* at, cudaStream_t st) {
   cfg = cudaLaunchConfig_t{};
-  cfg.gridDim = dim3((unsigned)(2 * p.nh * cl::C));   // 2 clusters per head
+  cfg.gridDim = dim3((unsigned)(4 * p.nh * cl::C));   // 4 clusters per head
   cfg.blockDim = dim3(cl::THREADS);
   cfg.dynamicSmemBytes = cl::SMEM_BYTES;
   cfg.stream = st;
@@ -979,13 +954,13 @@ static void cluster_launch_config(const StepParams& p, cudaLaunchConfig_t& cfg, 
   cfg.numAttrs = coop ? 2 : 1;
 }
 
-// true when the 32 x 4 cluster grid can be co-resident on this device
+// true when the grid of 4 nh clusters of 2 can be co-resident on this device (Mini: 64 of the 66 a 132-SM H100 holds)
 bool cluster_step_available(const StepParams& p) {
   const void* fn = cluster_kernel_fn(p);
   static bool told = false;
   auto why = [&](const char* what, cudaError_t e, int n) {
     if (!told) fprintf(stderr, "ptts_b200: cluster step kernel not used (%s: %s, %d co-resident clusters of %d, need %d); the one-CTA-per-SM step kernel runs instead\n",
-                       what, cudaGetErrorString(e), n, cl::C, 2 * p.nh);
+                       what, cudaGetErrorString(e), n, cl::C, 4 * p.nh);
     told = true;
     cudaGetLastError();
     return false;
@@ -998,7 +973,7 @@ bool cluster_step_available(const StepParams& p) {
   int n = 0;
   e = cudaOccupancyMaxActiveClusters(&n, fn, &cfg);
   if (e != cudaSuccess) return why("cluster occupancy query", e, n);
-  if (n < 2 * p.nh) return why("too few co-resident clusters", cudaSuccess, n);
+  if (n < 4 * p.nh) return why("too few co-resident clusters", cudaSuccess, n);
   return true;
 }
 

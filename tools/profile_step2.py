@@ -67,9 +67,9 @@ if arrive.max() > 0:   # barrier arrival skew of the middle layer (globaltimer, 
     for sub in range(6):
         a = (arrive[sub] - arrive[sub].min()) / 1e3
         order = np.argsort(a)
-        by_rank = [a[r::4].mean() for r in range(4)]
+        by_rank = [a[r::2].mean() for r in range(2)]
         print(f"arrival skew {names[sub]:20s}: CTA0 {a[0]:.2f}  median {np.median(a):.2f}  p90 {np.percentile(a, 90):.2f}  max {a.max():.2f} us (CTA {order[-1]}, {order[-2]}, {order[-3]}); "
-              f"mean by cluster rank {' '.join(f'{x:.2f}' for x in by_rank)}; clusters 0-15 {a[:64].mean():.2f} / 16-31 {a[64:].mean():.2f}")
+              f"mean by cluster rank {' '.join(f'{x:.2f}' for x in by_rank)}; heads 0-7 {a[:64].mean():.2f} / 8-15 {a[64:].mean():.2f}")
 r0, rh, rt = t[0], t[nph + 1], t[nph + 2]
 print(f"prologue {us(r0[0] - rt[3]):.2f} | embed {us(r0[6] - r0[0]):.2f} + barrier {us(r0[7] - r0[6]):.2f} | lm heads {us(rh[6] - rh[0]):.2f} "
       f"(tile + stats {us(rh[1] - rh[0]):.2f}) | barrier {us(rt[0] - rh[6]):.2f} | sampling {us(rt[1] - rt[0]):.2f} | last barrier {us(rt[2] - rt[1]):.2f} "
