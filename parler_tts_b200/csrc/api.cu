@@ -310,7 +310,6 @@ static bool setup_fused(ptts_session* s) {
   if (p.sample_items > 9) return fused_declined(s, "vocab_size > 2304");
   p.do_sample_phase = 1;
   p.prof = s->prof;
-  { const char* d = getenv("PTTS_DBG"); p.dbg = d ? atoi(d) : 0; }
   // cluster variant (step2.cu) when the shape and the device allow it; PTTS_STEP=legacy keeps step.cu (A/B runs, cross-checks)
   for (int i = 0; i < 6; i++) { p.cp[i] = L.cp[i]; p.cp_slice[i] = L.cp_slice[i]; }
   p.cl_x = (bf16*)(ws + W.cl_x); p.cl_attn = (bf16*)(ws + W.cl_attn); p.cl_h = (bf16*)(ws + W.cl_h);

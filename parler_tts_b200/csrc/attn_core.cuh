@@ -3,6 +3,7 @@
 #pragma once
 #include "common.cuh"
 #include "kernels.h"
+#include "ptx.cuh"
 
 namespace ptts {
 
@@ -196,8 +197,6 @@ namespace ptts {
 // is taken from shared memory (it is also written to the cache for later steps), so no global read-after-write.
 // No block-level barrier anywhere: used by attention_decode_kernel (8 items per CTA) and by the fused step
 // kernel -- both run exactly this code, hence bit-identical results.
-__device__ __forceinline__ uint32_t att_smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
 template <typename T> struct AttChunk { static constexpr int CH = 32; };
 template <> struct AttChunk<float> { static constexpr int CH = 16; };
 
@@ -235,22 +234,23 @@ __device__ __forceinline__ void attention_decode_item_warp(const AttnArgs& p, in
     const int st = i & 1;
     const int t0 = (part + nparts * i) * CH;
     const int n = (n_cached - t0 < CH) ? (n_cached - t0) : CH;
-    const uint32_t bar = att_smem_u32(&bars[st]);
-    if (lane == 0) asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"((uint32_t)(2 * n * HD * sizeof(T))) : "memory");
+    const uint32_t bar = smem_u32(&bars[st]);
+    if (lane == 0) mbar_expect_tx(bar, (uint32_t)(2 * n * HD * sizeof(T)));
     __syncwarp();
     if (lane < 2) {  // one bulk copy for the K rows, one for the V rows (rows of an item are contiguous)
       const T* src = (lane == 0 ? kc : vc) + (size_t)t0 * HD;
       T* dst = (lane == 0 ? kst : vst) + st * STAGE_ELEMS;
+      // (written out rather than through bulk_g2s: the wrapper call reorders ptxas's schedule of attention_decode_kernel)
       asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                   ::"r"(att_smem_u32(dst)), "l"(src), "r"((uint32_t)(n * HD * sizeof(T))), "r"(bar) : "memory");
+                   ::"r"(smem_u32(dst)), "l"(src), "r"((uint32_t)(n * HD * sizeof(T))), "r"(bar) : "memory");
     }
   };
   auto wait_stage = [&](int st) {
-    const uint32_t bar = att_smem_u32(&bars[st]);
+    const uint32_t bar = smem_u32(&bars[st]);
     const uint32_t par = (parity >> st) & 1u;
     uint32_t ok, spins = 0;
     do {
-      asm volatile("{\n.reg .pred p;\nmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\nselp.u32 %0, 1, 0, p;\n}" : "=r"(ok) : "r"(bar), "r"(par) : "memory");
+      ok = mbar_try_wait(bar, par);
       if (!ok && ++spins > (1u << 16)) { if (lane == 0) printf("ptts: attention KV mbarrier timeout (cta %d b %d kvh %d stage %d cross %d n_cached %d chunks %d par %u)\n", (int)blockIdx.x, b, kvh, st, p.cross, n_cached, n_chunks, parity); __trap(); }
     } while (!ok);
     parity ^= (1u << st);
@@ -258,7 +258,7 @@ __device__ __forceinline__ void attention_decode_item_warp(const AttnArgs& p, in
 
   // all lanes are past their shared-memory reads of the previous item: the ring may be refilled
   __syncwarp();
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+  fence_proxy_async_smem();
   if (n_chunks > 0) issue(0);
   if (n_chunks > 1) issue(1);
 
@@ -370,7 +370,7 @@ __device__ __forceinline__ void attention_decode_item_warp(const AttnArgs& p, in
 
     if (rr > 0) {  // GQA: further query heads re-stream the same cache rows
       __syncwarp();
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+      fence_proxy_async_smem();
       if (n_chunks > 0) issue(0);
       if (n_chunks > 1) issue(1);
     }
@@ -383,7 +383,7 @@ __device__ __forceinline__ void attention_decode_item_warp(const AttnArgs& p, in
       process(kst + st * STAGE_ELEMS, vst + st * STAGE_ELEMS, __ballot_sync(0xffffffffu, mk != 0), n);
       if (c + 2 < n_chunks) {
         __syncwarp();
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+        fence_proxy_async_smem();
         issue(c + 2);
       }
     }
@@ -457,16 +457,6 @@ __device__ __forceinline__ void attention_decode_item_warp(const AttnArgs& p, in
 // The K/V rows are stored swizzled (kv_swz, common.cuh), so the contiguous bulk copy of a stage is a conflict-free ldmatrix tile.
 // Only lanes 0..3 (fragment row 0) carry softmax state; fp32 scores / running max / sum, probabilities rounded to bf16 before
 // P V like the SIMT path and torch's flash kernels.
-__device__ __forceinline__ void att_ldsm4(uint32_t (&r)[4], uint32_t addr) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];" : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr));
-}
-__device__ __forceinline__ void att_ldsm4_t(uint32_t (&r)[4], uint32_t addr) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];" : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr));
-}
-__device__ __forceinline__ void att_mma(float (&d)[4], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0, uint32_t b1) {
-  asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]) : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
-}
 __device__ __forceinline__ uint32_t att_pack(float lo, float hi) {
   const __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);
   return *reinterpret_cast<const uint32_t*>(&v);
@@ -478,17 +468,10 @@ __device__ __forceinline__ float att_ex2(float x) {   // 2^x, 2 ulp; ex2(-inf) =
   return y;
 }
 
-// one K or V stage: global -> shared memory; `stream`: evict-first in L2 (the rows are read once per token; step2.cu bulk_g2s_stream)
+// one K or V stage: global -> shared memory; `stream`: evict-first in L2 (the rows are read once per token)
 __device__ __forceinline__ void att_bulk_kv(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar, bool stream) {
-  if (stream) {
-    uint64_t pol;
-    asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;"
-                 ::"r"(dst), "l"(src), "r"(bytes), "r"(bar), "l"(pol) : "memory");
-  } else {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                 ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
-  }
+  if (stream) bulk_g2s_evict_first(dst, src, bytes, bar);
+  else bulk_g2s(dst, src, bytes, bar);
 }
 
 constexpr int ATT_TC_CH = 32;   // keys per ring stage: one softmax / rescale chain per 32 keys (the chain, not the MMAs, bounds a stage)
@@ -529,13 +512,13 @@ __device__ __forceinline__ void attention_tc_issue_first(const TcItem& p, unsign
   const bf16* vc = p.vc;
   // (no proxy fence: the stage was last written by the async proxy and read with generic loads; see step2.cu issue_weight_job)
   __syncwarp();
-  const uint32_t bar = att_smem_u32(&bars[0]);
-  if (lane == 0) asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"((uint32_t)(2 * n * HD * 2)) : "memory");
+  const uint32_t bar = smem_u32(&bars[0]);
+  if (lane == 0) mbar_expect_tx(bar, (uint32_t)(2 * n * HD * 2));
   __syncwarp();
   if (lane < 2) {
     const bf16* src = (lane == 0 ? kc : vc) + (size_t)t0 * HD;
     bf16* dst = reinterpret_cast<bf16*>(ring0) + (lane == 0 ? 0 : CH * HD);
-    att_bulk_kv(att_smem_u32(dst), src, (uint32_t)(n * HD * 2), bar, stream);
+    att_bulk_kv(smem_u32(dst), src, (uint32_t)(n * HD * 2), bar, stream);
   }
 }
 
@@ -564,21 +547,21 @@ __device__ __forceinline__ void attention_decode_item_warp_tc(const TcItem& p, u
     const int st = i & 1;
     const int t0 = (part + nparts * i) * CH;
     const int n = (n_cached - t0 < CH) ? (n_cached - t0) : CH;
-    const uint32_t bar = att_smem_u32(&bars[st]);
-    if (lane == 0) asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"((uint32_t)(2 * n * HD * 2)) : "memory");
+    const uint32_t bar = smem_u32(&bars[st]);
+    if (lane == 0) mbar_expect_tx(bar, (uint32_t)(2 * n * HD * 2));
     __syncwarp();
     if (lane < 2) {
       const bf16* src = (lane == 0 ? kc : vc) + (size_t)t0 * HD;
       bf16* dst = reinterpret_cast<bf16*>(st ? ring1 : ring0) + (lane == 0 ? 0 : CH * HD);
-      att_bulk_kv(att_smem_u32(dst), src, (uint32_t)(n * HD * 2), bar, stream);
+      att_bulk_kv(smem_u32(dst), src, (uint32_t)(n * HD * 2), bar, stream);
     }
   };
   auto wait_stage = [&](int st) {
-    const uint32_t bar = att_smem_u32(&bars[st]);
+    const uint32_t bar = smem_u32(&bars[st]);
     const uint32_t par = (parity >> st) & 1u;
     uint32_t ok, spins = 0;
     do {
-      asm volatile("{\n.reg .pred p;\nmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\nselp.u32 %0, 1, 0, p;\n}" : "=r"(ok) : "r"(bar), "r"(par) : "memory");
+      ok = mbar_try_wait(bar, par);
       if (!ok && ++spins > (1u << 16)) { if (lane == 0) printf("ptts: tc attention KV mbarrier timeout (cta %d warp %d stage %d cross %d n_cached %d)\n", (int)blockIdx.x, (int)(threadIdx.x >> 5), st, p.cross, n_cached); __trap(); }
     } while (!ok);
     parity ^= (1u << st);
@@ -659,7 +642,7 @@ __device__ __forceinline__ void attention_decode_item_warp_tc(const TcItem& p, u
     uint32_t vword = __ballot_sync(0xffffffffu, mk != 0);
     if (n < CH) vword &= (1u << n) - 1u;
     bf16* stage = reinterpret_cast<bf16*>(st ? ring1 : ring0);
-    const uint32_t kbase = att_smem_u32(stage), vbase = att_smem_u32(stage + CH * HD);
+    const uint32_t kbase = smem_u32(stage), vbase = smem_u32(stage + CH * HD);
     if (n < CH) {  // last, partial stage: the copy filled n rows; whatever the rest of the V stage holds must not meet the MMA
       // (probability 0 x a stale NaN bit pattern is NaN); stale K rows only produce scores that are replaced by -inf below
       for (int i = lane; i < (CH - n) * 8; i += 32)
@@ -675,9 +658,9 @@ __device__ __forceinline__ void attention_decode_item_warp_tc(const TcItem& p, u
 #pragma unroll
       for (int half = 0; half < 2; half++) {   // chunks 4 half .. 4 half + 3 of the key rows = k-steps 2 half, 2 half + 1
         uint32_t kb[4];
-        att_ldsm4(kb, kbase + (uint32_t)((8 * nt + r8) * 128 + (((4 * half + mi) ^ r8) << 4)));
-        att_mma(s[nt], qa0[2 * half], 0u, qa2[2 * half], 0u, kb[0], kb[1]);
-        att_mma(s[nt], qa0[2 * half + 1], 0u, qa2[2 * half + 1], 0u, kb[2], kb[3]);
+        ldmatrix_x4(kb, kbase + (uint32_t)((8 * nt + r8) * 128 + (((4 * half + mi) ^ r8) << 4)));
+        mma_bf16_16816(s[nt], qa0[2 * half], 0u, qa2[2 * half], 0u, kb[0], kb[1]);
+        mma_bf16_16816(s[nt], qa0[2 * half + 1], 0u, qa2[2 * half + 1], 0u, kb[2], kb[3]);
       }
     }
     // rows g < 4 all hold s[nt][0], s[nt][1] = keys 8 nt + 2 t, 8 nt + 2 t + 1; lane (g, t) keeps n-tile g
@@ -706,9 +689,9 @@ __device__ __forceinline__ void attention_decode_item_warp_tc(const TcItem& p, u
           uint32_t vb[4];
           // matrices: (n-tile 2jp, keys 0-7), (2jp, keys 8-15), (2jp+1, keys 0-7), (2jp+1, keys 8-15) of this k-step; rows = keys, transposed on load
           const int key = 16 * kp + (mi & 1) * 8 + r8, chunk = 2 * jp + (mi >> 1);
-          att_ldsm4_t(vb, vbase + (uint32_t)(key * 128 + ((chunk ^ r8) << 4)));
-          att_mma(o[2 * jp], pa0, 0u, pa2, 0u, vb[0], vb[1]);
-          att_mma(o[2 * jp + 1], pa0, 0u, pa2, 0u, vb[2], vb[3]);
+          ldmatrix_x4_trans(vb, vbase + (uint32_t)(key * 128 + ((chunk ^ r8) << 4)));
+          mma_bf16_16816(o[2 * jp], pa0, 0u, pa2, 0u, vb[0], vb[1]);
+          mma_bf16_16816(o[2 * jp + 1], pa0, 0u, pa2, 0u, vb[2], vb[3]);
         }
       }
     }
@@ -790,8 +773,8 @@ __device__ __forceinline__ void attention_decode_item_warp_tc(const TcItem& p, u
 // per-warp mbarrier setup (once per kernel); bars = this warp's two mbarriers
 __device__ __forceinline__ void attention_decode_init_warp(uint64_t* bars, int lane) {
   if (lane == 0) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(att_smem_u32(&bars[0])));
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(att_smem_u32(&bars[1])));
+    mbar_init<1>(&bars[0]);
+    mbar_init<1>(&bars[1]);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncwarp();

@@ -19,20 +19,11 @@
 #include "common.cuh"
 #include "kernels.h"
 #include "ln_stats.cuh"
+#include "ptx.cuh"
 
 namespace ptts {
 
 // ---- bf16 tensor-core path ----------------------------------------------------------------------
-__device__ __forceinline__ void ldmatrix_x4(uint32_t (&r)[4], const void* smem_ptr) {
-  uint32_t a = (uint32_t)__cvta_generic_to_shared(smem_ptr);
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(a));
-}
-__device__ __forceinline__ void mma_bf16(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-  asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
 __device__ __forceinline__ uint4 ldg_stream(const uint4* p) {
   uint4 r;
   asm volatile("ld.global.nc.L1::no_allocate.v4.u32 {%0,%1,%2,%3}, [%4];"
@@ -124,8 +115,8 @@ __global__ void __launch_bounds__(GEMM_THREADS) linear_bf16_kernel(LinearArgs p)
             const uint4 w = wr[s][j];
 #pragma unroll
             for (int mt = 0; mt < 2; mt++) {
-              mma_bf16(acc[mt][j], a[mt][0], w.x, w.y);
-              mma_bf16(acc[mt][j], a[mt][1], w.z, w.w);
+              mma_bf16_16816(acc[mt][j], a[mt][0], w.x, w.y);
+              mma_bf16_16816(acc[mt][j], a[mt][1], w.z, w.w);
             }
           }
           if (i + PF < per_chunk) load_w(wr[s], c, i + PF);

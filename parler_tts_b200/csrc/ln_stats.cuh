@@ -19,14 +19,9 @@
 // over warps and the same fixed reduction order: the two paths stay bit-identical.
 #pragma once
 #include "common.cuh"
+#include "ptx.cuh"
 
 namespace ptts {
-
-__device__ __forceinline__ void mma_bf16_16816(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-  asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
 
 // accumulators of one warp for a 32-row tile (two m16 tiles)
 struct RowStatFrag {
@@ -59,8 +54,7 @@ __device__ __forceinline__ void row_stat_pass(RowStatFrag& st, const bf16* xs, i
 #pragma unroll
       for (int j = 0; j < 2; j++) {
         uint32_t a[4];
-        const uint32_t addr = (uint32_t)__cvta_generic_to_shared(xs + (size_t)(mt * 16 + lrow) * pitch + kt * 32 + j * 16 + lcol);
-        asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];" : "=r"(a[0]), "=r"(a[1]), "=r"(a[2]), "=r"(a[3]) : "r"(addr));
+        ldmatrix_x4(a, xs + (size_t)(mt * 16 + lrow) * pitch + kt * 32 + j * 16 + lcol);
         row_stat_mma(st, mt, a);
       }
   }

@@ -22,7 +22,9 @@
 #include "kernels.h"
 #include "ln_stats.cuh"
 #include "sample_core.cuh"
+#include "ptx.cuh"
 #include "step.h"
+#include "step_common.cuh"
 
 namespace ptts {
 
@@ -30,96 +32,13 @@ constexpr int ST_THREADS = 256;
 constexpr int ST_WARPS = 8;
 constexpr int ST_HEADER = 512 + 8 * 32 * 2 * 4 + 256;  // mbarriers [0,256) | row stats [256,512) | stat partials [512,2560) | c1,c2 of the task [2560,2816)
 
-// ---- PTX helpers --------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   uint32_t ok;
   uint32_t spins = 0;
   do {
-    asm volatile("{\n.reg .pred p;\nmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\nselp.u32 %0, 1, 0, p;\n}"
-                 : "=r"(ok) : "r"(smem_u32(bar)), "r"(parity) : "memory");
+    ok = mbar_try_wait(bar, parity);
     if (!ok && ++spins > (1u << 22)) { printf("ptts: tile mbarrier timeout (cta %d)\n", (int)blockIdx.x); __trap(); }
   } while (!ok);
-}
-__device__ __forceinline__ void bulk_g2s(void* dst_smem, const void* src, uint32_t bytes, uint64_t* bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-               ::"r"(smem_u32(dst_smem)), "l"(src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
-}
-// orders this thread's prior generic-proxy accesses (shared AND the acquired global data) before later async-proxy (TMA) accesses
-__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async;" ::: "memory"); }
-__device__ __forceinline__ void l2_prefetch(const void* p, uint32_t bytes) {
-  const char* c = reinterpret_cast<const char*>(p);
-  while (bytes > 0) {
-    const uint32_t n = bytes > 32768u ? 32768u : bytes;
-    asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(c), "r"(n) : "memory");
-    c += n;
-    bytes -= n;
-  }
-}
-__device__ __forceinline__ unsigned ld_relaxed(const unsigned* p) {
-  unsigned v;
-  asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-  return v;
-}
-__device__ __forceinline__ void red_release_add(unsigned* p, unsigned v) {
-  asm volatile("red.release.gpu.global.add.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
-}
-__device__ __forceinline__ void fence_acq_rel_gpu() { asm volatile("fence.acq_rel.gpu;" ::: "memory"); }
-__device__ __forceinline__ void ldmatrix_x4s(uint32_t (&r)[4], const void* smem_ptr) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(smem_u32(smem_ptr)));
-}
-__device__ __forceinline__ void mma_bf16s(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-  asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-__device__ __forceinline__ uint4 ldg_stream_s(const uint4* p) {
-  uint4 r;
-  asm volatile("ld.global.nc.L1::no_allocate.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "l"(p));
-  return r;
-}
-
-// ---- device-wide barrier ------------------------------------------------------------------------
-// Arrive = red.release (cumulative over the CTA's writes ordered by the preceding bar.sync); the spin is a
-// RELAXED load (an acquire load would invalidate L1 on every poll); one acquire fence after the exit.
-// `side` runs on thread 32 between the two CTA barriers, i.e. while thread 0 polls: work that needs the whole CTA to be
-// past its shared-memory accesses but not the other CTAs (the next phase's weight copy) costs nothing there.
-struct NoSideJob { __device__ __forceinline__ void operator()() const {} };
-template <typename Side = NoSideJob>
-__device__ __forceinline__ unsigned grid_sync(unsigned* ctr, unsigned target, int* progress = nullptr, int ph = 0, Side side = Side()) {
-  target += gridDim.x;
-  // this thread's global writes (generic proxy) -> later TMA reads by other CTAs (async proxy): the proxy fence sits on the
-  // writer side of the release/acquire chain, where it overlaps the store drain instead of delaying the next tile copy
-  asm volatile("fence.proxy.async.global;" ::: "memory");
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    if (progress) progress[blockIdx.x] = ph;
-    red_release_add(ctr, 1u);
-    unsigned spins = 0;
-    while (ld_relaxed(ctr) < target) {
-      if (++spins > (1u << 24)) {
-        printf("ptts: grid barrier timeout (cta %d target %u seen %u ph %d)\n", (int)blockIdx.x, target, ld_relaxed(ctr), ph);
-        if (progress) for (int i = 0; i < (int)gridDim.x; i++) if (((volatile int*)progress)[i] != ph) printf("ptts:   cta %d is at phase %d\n", i, ((volatile int*)progress)[i]);
-        __trap();
-      }
-    }
-    fence_acq_rel_gpu();
-  } else if (threadIdx.x == 32) {
-    side();
-  }
-  __syncthreads();
-  return target;
-}
-
-__device__ __forceinline__ void prof_mark(long long* prof, int slot) {
-  if (prof != nullptr && threadIdx.x == 0) prof[slot] = clock64();
 }
 
 // ---- shared-memory context ----------------------------------------------------------------------
@@ -135,7 +54,6 @@ struct Smem {
   long long* prof;  // CTA 0 / thread 0 timestamps of the current phase (nullptr = off)
   int pitch;
   int nbuf;
-  int dbg;
 };
 
 __device__ __forceinline__ bf16* tile_of(const Smem& sm, int buf) { return sm.tile0 + (size_t)buf * 32 * sm.pitch; }
@@ -147,7 +65,7 @@ __device__ __forceinline__ bf16* tile_of(const Smem& sm, int buf) { return sm.ti
 __device__ __forceinline__ void stage_tile(Smem& sm, int buf, const bf16* img, int M, bool mark) {
   __syncthreads();  // every generic-proxy access to the buffer (ldmatrix, reduction scratch) is done
   if (threadIdx.x == 0) {
-    if (!(sm.dbg & 8)) asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // tile buffer: generic accesses (above barrier) before the async write
+    fence_proxy_async_smem();  // tile buffer: generic accesses (above barrier) before the async write
     const uint32_t bytes = (uint32_t)(M * sm.pitch * 2);
     mbar_expect_tx(&sm.bars[buf], bytes);
     bulk_g2s(tile_of(sm, buf), img, bytes, &sm.bars[buf]);
@@ -213,8 +131,7 @@ __device__ __forceinline__ void prefetch_kv(const StepParams& p, int l, int pos)
 }
 
 __device__ __forceinline__ void issue_prefetch(const StepParams& p, const PrefetchJob& j) {
-  if (p.dbg & 1) return;
-  if (j.kv_layer >= 0 && !(p.dbg & 2)) prefetch_kv(p, j.kv_layer, j.pos);
+  if (j.kv_layer >= 0) prefetch_kv(p, j.kv_layer, j.pos);
   if (threadIdx.x == ST_THREADS - 32) {
     if (j.w != nullptr) prefetch_slice(j.w, j.N, j.K, j.nt);
     if (j.v != nullptr) l2_prefetch(j.v, j.v_bytes);
@@ -252,7 +169,7 @@ __device__ __forceinline__ void issue_weights_thread(const StepParams& p, Smem& 
   gemm_matrix(p, ph, W, N, K, nt);
   if (task >= N / (8 * nt)) return;
   const uint32_t bytes = (uint32_t)nt * (uint32_t)K * 16u;
-  if (!(p.dbg & 4)) asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+  fence_proxy_async_smem();
   mbar_expect_tx(&sm.bars[WBAR], bytes);
   bulk_g2s(const_cast<uint4*>(sm.wbuf), W + (size_t)task * bytes, bytes, &sm.bars[WBAR]);
 }
@@ -330,14 +247,14 @@ __device__ __forceinline__ void gemm_tasks(const StepParams& p, Smem& sm, const 
 #pragma unroll
         for (int mt = 0; mt < 2; mt++)
 #pragma unroll
-          for (int j = 0; j < 2; j++) ldmatrix_x4s(a[mt][j], xs + (size_t)(mt * 16 + lrow) * sm.pitch + kt * 32 + j * 16 + lcol);
+          for (int j = 0; j < 2; j++) ldmatrix_x4(a[mt][j], xs + (size_t)(mt * 16 + lrow) * sm.pitch + kt * 32 + j * 16 + lcol);
 #pragma unroll
         for (int j = 0; j < NT_MAX; j++) {
           if (j < nt) {
 #pragma unroll
             for (int mt = 0; mt < 2; mt++) {
-              mma_bf16s(acc[mt][j], a[mt][0], w[j].x, w[j].y);
-              mma_bf16s(acc[mt][j], a[mt][1], w[j].z, w[j].w);
+              mma_bf16_16816(acc[mt][j], a[mt][0], w[j].x, w[j].y);
+              mma_bf16_16816(acc[mt][j], a[mt][1], w[j].z, w[j].w);
             }
           }
         }
@@ -412,12 +329,6 @@ __device__ __forceinline__ void attn_phase(const StepParams& p, Smem& sm, const 
     attention_decode_item_warp<bf16>(a, it / nkv, it % nkv, pos, region, bars, lane, att_parity, part, 2, xch, pair + 1);
 }
 
-// one CTA per (utterance, codebook) row (sample_core.cuh): 288 rows over one CTA per SM at Mini / batch 32
-template <int ITEMS>
-__device__ __noinline__ void sample_phase(const SampleArgs& sa, const ptts_gen_params& gp, int BK, int cur_len) {
-  sample_all_rows_cta<ITEMS>(sa, gp, (int)blockIdx.x, (int)gridDim.x, BK, cur_len);
-}
-
 template <int ITEMS>
 __global__ void __launch_bounds__(ST_THREADS, 1) decode_step_kernel(const __grid_constant__ StepParams p) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
@@ -439,14 +350,13 @@ __global__ void __launch_bounds__(ST_THREADS, 1) decode_step_kernel(const __grid
   sm.wbuf = reinterpret_cast<const uint4*>(smem_raw + ST_HEADER + p.wbuf_offset);
   sm.pitch = H + 8;
   sm.nbuf = p.nbuf;
-  sm.dbg = p.dbg;
   sm.tile0 = reinterpret_cast<bf16*>(sm.scratch);
   sm.parity = 0;
   sm.prof = nullptr;
   if (tid == 0) {
-    mbar_init(&sm.bars[0], 1);
-    mbar_init(&sm.bars[1], 1);
-    mbar_init(&sm.bars[WBAR], 1);
+    mbar_init<1>(&sm.bars[0]);
+    mbar_init<1>(&sm.bars[1]);
+    mbar_init<1>(&sm.bars[WBAR]);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   attention_decode_init_warp(sm.bars + 2 + 2 * warp, lane);  // per-warp K/V ring barriers: header bytes [16, 144)
@@ -477,26 +387,15 @@ __global__ void __launch_bounds__(ST_THREADS, 1) decode_step_kernel(const __grid
     prefetch_slice(lb + p.fc2, H, p.F, p.nt_h);
   }
   {
-    const bf16* tables = reinterpret_cast<const bf16*>(blob + p.embed);
-    const bf16* postab = p.rope ? nullptr : reinterpret_cast<const bf16*>(blob + p.pos);
     const int cpr = (H + ST_THREADS - 1) / ST_THREADS;  // column chunks per row: (row, chunk) items spread over all CTAs
     for (int it = blockIdx.x; it < p.B * cpr; it += gridDim.x) {
       const int b = it / cpr, c = (it - b * cpr) * ST_THREADS + tid;
       if (c >= H) continue;
-      float ev[16];
-#pragma unroll
-      for (int k = 0; k < 16; k++)  // all K gathers in flight, then the left-to-right rounded sum
-        if (k < p.K) ev[k] = __bfloat162float(tables[((size_t)k * (p.V + 1) + p.sa.cur_ids[b * p.K + k]) * H + c]);
-      float v = 0.f;
-#pragma unroll
-      for (int k = 0; k < 16; k++)
-        if (k < p.K) v = (k == 0) ? ev[k] : DT<bf16>::rnd(v + ev[k]);
-      if (postab != nullptr) v = DT<bf16>::rnd(v + __bfloat162float(postab[(size_t)pos * H + c]));
-      p.x[(size_t)b * sm.pitch + c] = __float2bfloat16_rn(v);
+      p.x[(size_t)b * sm.pitch + c] = __float2bfloat16_rn(embed_value(p, b, c, pos));
     }
   }
   prof_mark(sm.prof, 6);
-  bar_target = grid_sync(bar_ctr, bar_target);
+  bar_target = grid_sync(bar_ctr, bar_target, 0, true);
   prof_mark(sm.prof, 7);
 
   // One loop over all 8L+1 dependent phases (single call site per phase type keeps code size and registers sane).
@@ -507,25 +406,13 @@ __global__ void __launch_bounds__(ST_THREADS, 1) decode_step_kernel(const __grid
     prof_mark(sm.prof, 0);
     const char* lb = blob + p.layer0 + p.layer_stride * (l < p.L ? l : p.L - 1);
     if (sub == 1 || sub == 4) {
-      AttnArgs a{};
-      a.ldo = sm.pitch; a.out = p.attn; a.ctrl = nullptr; a.B = p.B; a.nh = p.nh; a.q_len = 1;
-      a.past_from_ctrl = 0; a.past_len = pos; a.prefix = p.P;
-      a.rope = p.rope; a.rope_cos = blob + p.rope_cos; a.rope_sin = blob + p.rope_sin; a.scale = p.scale;
+      AttnArgs a = decode_attn_args(p, l, pos, sub == 4);
+      a.ldo = sm.pitch; a.out = p.attn;
       if (sub == 1) {  // self-attention over the cache (+ append of the new K/V row)
-        a.q = p.qkv; a.ldq = p.qkv_rows; a.q_col0 = 0;
+        a.q = p.qkv; a.ldq = p.qkv_rows;
         a.knew = p.qkv; a.vnew = p.qkv; a.ldkv = p.qkv_rows; a.k_col0 = p.nh * HD; a.v_col0 = (p.nh + p.nkv) * HD;
-        char* kc = p.self_kv + p.self_layer_stride * l;
-        a.kcache = kc; a.vcache = kc + (size_t)p.B * p.nkv * p.Tmax * HD * 2;
-        a.kv_b_stride = (int64_t)p.nkv * p.Tmax * HD; a.kv_h_stride = (int64_t)p.Tmax * HD; a.kv_t_stride = HD;
-        a.key_mask = p.prompt_mask; a.mask_len = p.P; a.mask_ld = p.P;
-        a.nkv = p.nkv; a.cross = 0; a.kv_len = 0; a.kv_capacity = p.Tmax;
       } else {         // cross-attention over the cached encoder K/V
-        a.q = p.qc; a.ldq = H; a.q_col0 = 0; a.knew = nullptr; a.vnew = nullptr;
-        char* ck = p.cross_kv + p.cross_layer_stride * l;
-        a.kcache = ck; a.vcache = ck + (size_t)p.B * p.nckv * p.S * HD * 2;
-        a.kv_b_stride = (int64_t)p.nckv * p.S * HD; a.kv_h_stride = (int64_t)p.S * HD; a.kv_t_stride = HD;
-        a.key_mask = p.enc_mask; a.mask_len = p.S; a.mask_ld = p.S;
-        a.nkv = p.nckv; a.cross = 1; a.kv_len = p.S; a.kv_capacity = p.S;
+        a.q = p.qc; a.ldq = H;
       }
       attn_phase(p, sm, a, a.nkv, pos, att_parity, ph);
     } else {
@@ -597,11 +484,11 @@ __global__ void __launch_bounds__(ST_THREADS, 1) decode_step_kernel(const __grid
       // while thread 0 polls the barrier, thread 32 requests this CTA's weight slice of the next phase when that is a GEMM
       // (every reader of the weight buffer -- and of the attention scratch it may alias -- is past the CTA barrier by then)
       const int wph = is_attn_phase(p, ph + 1) ? -1 : ph + 1;
-      bar_target = grid_sync(bar_ctr, bar_target, p.progress, ph + 1, [&]() { if (wph >= 0) issue_weights_thread(p, sm, wph, blockIdx.x); });
+      bar_target = grid_sync(bar_ctr, bar_target, ph + 1, true, p.progress, NoHook(), [&]() { if (wph >= 0) issue_weights_thread(p, sm, wph, blockIdx.x); });
     }
     prof_mark(sm.prof, 7);
   }
-  bar_target = grid_sync(bar_ctr, bar_target);
+  bar_target = grid_sync(bar_ctr, bar_target, 0, true);
   sm.prof = prof0 ? prof0 + (size_t)(8 * p.L + 2) * 8 : nullptr;  // tail row: barrier / sampling / barrier
   prof_mark(sm.prof, 0);
   if (p.do_sample_phase) {
@@ -609,7 +496,7 @@ __global__ void __launch_bounds__(ST_THREADS, 1) decode_step_kernel(const __grid
     const int BK = p.B * p.K;
     sample_phase<ITEMS>(p.sa, gp, BK, cur_len);
     prof_mark(sm.prof, 1);
-    bar_target = grid_sync(bar_ctr, bar_target);
+    bar_target = grid_sync(bar_ctr, bar_target, 0, true);
     prof_mark(sm.prof, 2);
   }
   if (blockIdx.x == 0 && tid == 0) {

@@ -33,14 +33,10 @@ struct StepParams {
   int sample_items;        // ceil(V / 256): logits per thread of the one-CTA-per-row sampler
   int* progress;           // debug: last phase each CTA arrived at (printed on a barrier timeout)
   int n_steps;             // cluster kernel: tokens one launch may run (stops early when every row is finished); 0 / 1 = one
-  int dbg;                 // PTTS_DBG measurement switches (bit mask, all off by default; INTEGRATION.md lists them).  step.cu: 1 no weight
-                           // L2 prefetch, 2 no K/V prefetch, 4 / 8 omit a proxy fence.  step2.cu: 1 / 2 weight / K/V L2 prefetches ON,
-                           // 32 acquire fence at the layer barriers, 64 release-form cluster arrive, 128 cold sampling pass first,
-                           // 256 default L2 policy for the streamed weights, 1024 one exchange copy per warp in the head phases
   long long* prof;         // optional [(8L+3)][8] clock64 timestamps written by CTA 0 (debug / profiles)
   // ---- cluster step kernel (step2.cu) ----
   int64_t cp[6], cp_slice[6];   // per-layer offsets / slice bytes of the (phase, cluster, rank) weight slices (layout.h)
-  bf16 *cl_x, *cl_attn, *cl_h;  // K-sliced activation images [4][32][K/4 + 8]
+  bf16 *cl_x, *cl_attn, *cl_h;  // K-sliced activation images [slices][32][slice width + 8]: x, attn 2 slices of H/2; h 4 of F/4
 };
 
 int step_smem_bytes(const StepParams& p);

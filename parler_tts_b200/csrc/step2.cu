@@ -22,8 +22,8 @@
 //     head's 192 KB QKV slice of a rank streams through the 2 x 64 KB weight ring as four jobs.
 //   * weights: one contiguous slice per (phase, cluster, rank) (layout.h cpack, built once by ptts_decoder_finalize), streamed by
 //     ONE bulk copy per job into a 2 x 64 KB ring two jobs ahead, with an L2 evict-first policy like the K/V rows (1.2 GB per token
-//     must not evict the kernel's own instructions and the small reused tensors).  HBM -> L2 prefetches a layer ahead exist behind
-//     PTTS_DBG=1/2 (experiments, off by default).
+//     must not evict the kernel's own instructions and the small reused tensors).  No HBM -> L2 prefetch: the ring already runs two
+//     jobs ahead of its consumer, and every cp.async.bulk.prefetch.L2 costs issue time inside a phase.
 //   * fc2 (one n-tile per destination, half of F = 128 KB of activations): staged in two quarters of F, one after the other; a
 //     warp's accumulators carry its residue class from the first quarter into the second.
 //   * attention: the sweep step.cu's attention phase runs (attention_decode_item_warp, two warps per item, 32-key chunks).
@@ -37,10 +37,10 @@
 #include "kernels.h"
 #include "ln_stats.cuh"
 #include "sample_core.cuh"
+#include "ptx.cuh"
 #include "step.h"
+#include "step_common.cuh"
 #include <type_traits>
-
-#include <cstdlib>
 
 namespace ptts {
 namespace cl {
@@ -75,40 +75,18 @@ static_assert(2 * V * C * (32 + 4 * 96 * 4) <= R_PASS0 && R_PASS0 + V * QMAX * 3
 static_assert(5 * ATT_SMEM <= QKV_OFF && 3 * ATT_SMEM <= WB_BYTES && 16384 + 4 * 128 * 4 <= WB_BYTES, "attention plan");
 static_assert(ROWS * (4096 / 4 + 8) * 2 + V * (256 + ROWS * 8 * 4) <= R_BYTES, "fc2 plan");
 
-// ---- PTX helpers ---------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t s32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) { asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(s32(bar)), "r"(count)); }
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(s32(bar)), "r"(bytes) : "memory");
-}
+// ---- PTX helpers used by this kernel only (ptx.cuh has the shared ones) ------------------------------
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity, int what) {
   uint32_t ok, spins = 0;
   do {
-    asm volatile("{\n.reg .pred p;\nmbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%1], %2;\nselp.u32 %0, 1, 0, p;\n}"
-                 : "=r"(ok) : "r"(s32(bar)), "r"(parity) : "memory");
+    ok = mbar_try_wait_cluster(bar, parity);
     if (!ok && ++spins > (1u << 22)) { printf("ptts: cluster step mbarrier timeout (cta %d, barrier kind %d)\n", (int)blockIdx.x, what); __trap(); }
   } while (!ok);
-}
-__device__ __forceinline__ void bulk_g2s(void* dst_smem, const void* src, uint32_t bytes, uint64_t* bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-               ::"r"(s32(dst_smem)), "l"(src), "r"(bytes), "r"(s32(bar)) : "memory");
-}
-// Streamed-once data (the weights, the K/V rows: ~1.2 GB per token, ten times the L2) is requested with an evict-first policy so that
-// it does not push out what IS reused between and inside launches: this kernel's instructions (the once-per-token phases ran at
-// ~10 cycles per instruction on cold fetches), the folded-LayerNorm vectors, the activation images, the logits.
-__device__ __forceinline__ uint64_t l2_evict_first_policy() {
-  uint64_t pol;
-  asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
-  return pol;
-}
-__device__ __forceinline__ void bulk_g2s_stream(void* dst_smem, const void* src, uint32_t bytes, uint64_t* bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;"
-               ::"r"(s32(dst_smem)), "l"(src), "r"(bytes), "r"(s32(bar)), "l"(l2_evict_first_policy()) : "memory");
 }
 // this CTA's shared memory -> a peer's shared memory (DSMEM), completion counted on the PEER's mbarrier
 __device__ __forceinline__ void bulk_s2peer(uint32_t dst_cluster_addr, const void* src_smem, uint32_t bytes, uint32_t bar_cluster_addr) {
   asm volatile("cp.async.bulk.shared::cluster.shared::cta.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-               ::"r"(dst_cluster_addr), "r"(s32(src_smem)), "r"(bytes), "r"(bar_cluster_addr) : "memory");
+               ::"r"(dst_cluster_addr), "r"(smem_u32(src_smem)), "r"(bytes), "r"(bar_cluster_addr) : "memory");
 }
 __device__ __forceinline__ uint32_t mapa(uint32_t addr, uint32_t rank) { uint32_t r; asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(rank)); return r; }
 __device__ __forceinline__ uint32_t cluster_rank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
@@ -117,54 +95,8 @@ __device__ __forceinline__ void cluster_wait() { asm volatile("barrier.cluster.w
 // The per-phase cluster barrier only guards buffer REUSE (a peer may overwrite my receive slots / I may overwrite a send block once
 // everyone has consumed the previous phase's); the data itself is ordered by the exchange mbarrier.  A write-after-read needs no
 // release: the default .release arrive is a gpu-scope MEMBAR per warp (it waits for the epilogue's global stores to be acknowledged,
-// a second time before the layer barrier does).  PTTS_DBG=64 restores the release form for A/B runs.
-__device__ __forceinline__ void cluster_arrive_reuse(bool release) {
-  if (release) asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  else asm volatile("barrier.cluster.arrive.relaxed.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void l2_prefetch(const void* p, uint32_t bytes, bool on = true) {
-  if (!on) return;
-  const char* c = reinterpret_cast<const char*>(p);
-  while (bytes > 0) {
-    const uint32_t n = bytes > 32768u ? 32768u : bytes;
-    asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(c), "r"(n) : "memory");
-    c += n;
-    bytes -= n;
-  }
-}
-__device__ __forceinline__ unsigned ld_relaxed(const unsigned* p) { unsigned v; asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory"); return v; }
-__device__ __forceinline__ void red_release_add(unsigned* p, unsigned v) { asm volatile("red.release.gpu.global.add.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory"); }
-__device__ __forceinline__ void ldsm4(uint32_t (&r)[4], const void* smem_ptr) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];" : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(s32(smem_ptr)));
-}
-__device__ __forceinline__ void prof_mark(long long* prof, int slot) { if (prof != nullptr && threadIdx.x == 0) prof[slot] = clock64(); }
-
-// ---- device-wide barrier (same protocol as step.cu) -----------------------------------------------
-// `post` runs on thread 0 the moment the barrier opens (before the CTA is released): the next phase's activation copy.
-// `side` runs on thread 32 while thread 0 polls.
-template <typename Post, typename Side>
-__device__ __forceinline__ unsigned grid_sync(unsigned* ctr, unsigned target, int ph, Post post, Side side, bool acq_fence = true) {
-  target += gridDim.x;
-  asm volatile("fence.proxy.async.global;" ::: "memory");  // this thread's global writes -> other CTAs' TMA reads (writer side)
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    red_release_add(ctr, 1u);
-    unsigned spins = 0;
-    while (ld_relaxed(ctr) < target) {
-      if (++spins > (1u << 24)) { printf("ptts: cluster step grid barrier timeout (cta %d target %u seen %u phase %d)\n", (int)blockIdx.x, target, ld_relaxed(ctr), ph); __trap(); }
-    }
-    // Everything this kernel reads that another CTA wrote during the same launch goes through L2 (TMA bulk copies of the images
-    // and the K/V rows, __ldcg of the logits / EOS columns), so the L1 invalidation of an acquire fence protects nothing here and
-    // costs time at every barrier: the per-layer barriers skip it, PTTS_DBG=32 puts it back.
-    if (acq_fence) asm volatile("fence.acq_rel.gpu;" ::: "memory");
-    post();
-  } else if (threadIdx.x == 32) {
-    side();
-  }
-  __syncthreads();
-  return target;
-}
+// a second time before the layer barrier does).
+__device__ __forceinline__ void cluster_arrive_reuse() { asm volatile("barrier.cluster.arrive.relaxed.aligned;" ::: "memory"); }
 
 // K-slice layout of the activation images and of the packed weights: rank r holds the k32 tiles kt with (kt & 7) >> 2 == r, in
 // ascending order.  Warp e4 of rank r then reduces the k-tiles kt = 4 r + e4 (mod 8): the tiles, in the order, that warp 4 r + e4
@@ -194,7 +126,7 @@ __device__ __forceinline__ void mma_slice(float (&out)[2][6][4], RowStatFrag& rs
 #pragma unroll
     for (int mt = 0; mt < MT; mt++)
 #pragma unroll
-      for (int j = 0; j < 2; j++) ldsm4(a[mt][j], xs + (size_t)(mt * 16 + lrow) * apitch + kt * 32 + j * 16 + lcol);
+      for (int j = 0; j < 2; j++) ldmatrix_x4(a[mt][j], xs + (size_t)(mt * 16 + lrow) * apitch + kt * 32 + j * 16 + lcol);
     if (STATS) {   // every k-tile of this warp's residue class: its blocks then carry complete statistics for it
 #pragma unroll
       for (int mt = 0; mt < MT; mt++) { row_stat_mma(rst, mt, a[mt][0]); row_stat_mma(rst, mt, a[mt][1]); }
@@ -275,16 +207,11 @@ __global__ void __launch_bounds__(THREADS, 1) decode_step_cluster_kernel(const _
   uint32_t par_a = 0, par_w = 0, par_x = 0, att_parity = 0;
 
   if (tid == 0) {
-    mbar_init(abar, 1); mbar_init(&wbar[0], 1); mbar_init(&wbar[1], 1); mbar_init(xbar, 1);
+    mbar_init<1>(abar); mbar_init<1>(&wbar[0]); mbar_init<1>(&wbar[1]); mbar_init<1>(xbar);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   attention_decode_init_warp(attbars + 2 * warp, lane);
   cluster_arrive(); cluster_wait();   // every peer's mbarriers exist before any remote complete_tx
-  // HBM -> L2 prefetches a layer ahead are off by default (the shared-memory ring already runs two jobs ahead of its consumer,
-  // and every cp.async.bulk.prefetch.L2 costs issue time inside a phase); PTTS_DBG=1 switches them on
-  const bool pf_on = (p.dbg & 1) != 0;   // PTTS_DBG=1: weight / folded-LN L2 prefetches on
-  const bool pf_kv = (p.dbg & 2) != 0;   // PTTS_DBG=2: next layer's K/V rows -> L2 during the out-proj phases
-  const bool acq = (p.dbg & 32) != 0;   // PTTS_DBG=32: put the acquire fence back (grid_sync explains why it is not needed)
   unsigned* const bar_ctr = p.bar + (gen & 1u);
   unsigned bar_target = 0u;
   if (cta == 0 && tid == 0) p.bar[(gen + 1u) & 1u] = 0u;  // the counter the NEXT launch will use
@@ -303,21 +230,7 @@ __global__ void __launch_bounds__(THREADS, 1) decode_step_cluster_kernel(const _
     // in flight (a stall wherever one sits behind a 64 KB weight copy).  The one generic-written corner (the attention
     // merge scratch of the q_cross phase) is covered by the fence thread 0 executes at every device-wide barrier (request_slice).
     mbar_expect_tx(&wbar[j & 1], bytes);
-    if (p.dbg & 256) bulk_g2s(smem + HDR + (j & 1) * WB_BYTES, src, bytes, &wbar[j & 1]);   // (A/B: default L2 policy)
-    else bulk_g2s_stream(smem + HDR + (j & 1) * WB_BYTES, src, bytes, &wbar[j & 1]);
-  };
-  // the same requests cut into one piece per warp (issued by lane 0 of every warp: a prefetch is ~100 cycles of issue time)
-  auto prefetch_weight_job_part = [&](int j, int w) {
-    const char* src; uint32_t bytes;
-    if (pf_on && weight_job(p, j, cta, rank, src, bytes)) { const uint32_t pc = (bytes / V) & ~15u; l2_prefetch(src + (size_t)w * pc, w == V - 1 ? bytes - (V - 1) * pc : pc); }
-  };
-  auto prefetch_kv_part = [&](int l, bool cross, int w) {  // warp w: item w >> 1, K (even w) or V (odd w)
-    const int T = cross ? p.S : p.Tmax, n = cross ? p.S : pos;
-    const int b = HROWS * rblk + 4 * rank + (w >> 1);
-    if (!pf_kv || n <= 0 || b >= B) return;
-    const char* kc = cross ? p.cross_kv + p.cross_layer_stride * l : p.self_kv + p.self_layer_stride * l;
-    const char* k = kc + ((size_t)b * p.nh + head) * T * HD * 2 + ((w & 1) ? (size_t)B * p.nh * T * HD * 2 : 0);
-    l2_prefetch(k, (uint32_t)(n * HD * 2));
+    bulk_g2s_evict_first(smem + HDR + (j & 1) * WB_BYTES, src, bytes, &wbar[j & 1]);
   };
   // ---- one launch runs up to p.n_steps tokens (ptts_decode_steps): the gap between dependent cooperative launches, the launch
   // skew in front of the first barrier and the cold instruction fetches of the once-per-token phases are paid once per launch.
@@ -329,12 +242,8 @@ __global__ void __launch_bounds__(THREADS, 1) decode_step_cluster_kernel(const _
   for (int it = 0; it < n_steps; it++) {
   pos = p.P + cur_len - 1;
   prof = prof0;
-  cluster_arrive_reuse(false);        // pre-arm: pairs with the first phase's "exchange buffers free" wait
+  cluster_arrive_reuse();             // pre-arm: pairs with the first phase's "exchange buffers free" wait
   if (tid == 0) { issue_weight_job(0); issue_weight_job(1); }
-  if (lane == 0) {
-    for (int j = 2; j < JOBS_PER_LAYER; j++) prefetch_weight_job_part(j, warp);
-    prefetch_kv_part(0, false, warp); prefetch_kv_part(0, true, warp);
-  }
 
   // global activation images, K-sliced for their consumer: [slices][32 rows][slice width + 8] bf16
   bf16* const x_img = p.cl_x;       // 2 slices of H/2 columns (consumers: QKV, q_cross, fc1, lm heads)
@@ -351,24 +260,8 @@ __global__ void __launch_bounds__(THREADS, 1) decode_step_cluster_kernel(const _
 
   // ---- embeddings: this CTA's 32 x 8 slice of sum_k embed_k[id] (+ position) -> residual slice + x image -----------------
   {
-    const bf16* tables = reinterpret_cast<const bf16*>(blob + p.embed);
-    const bf16* postab = p.rope ? nullptr : reinterpret_cast<const bf16*>(blob + p.pos);
     const int row = tid >> 3, f = tid & 7, n = cta * 8 + f;
-    float v = 0.f;
-    if (row < B) {
-      // codebooks in groups of 8: the loads of a group are in flight together, and the group's values are all that is live
-#pragma unroll 1
-      for (int k0 = 0; k0 < p.K; k0 += 8) {
-        float ev[8];
-#pragma unroll
-        for (int k = 0; k < 8; k++)
-          if (k0 + k < p.K) ev[k] = __bfloat162float(tables[((size_t)(k0 + k) * (p.V + 1) + p.sa.cur_ids[row * p.K + k0 + k]) * H + n]);
-#pragma unroll
-        for (int k = 0; k < 8; k++)
-          if (k0 + k < p.K) v = (k0 + k == 0) ? ev[k] : DT<bf16>::rnd(v + ev[k]);
-      }
-      if (postab != nullptr) v = DT<bf16>::rnd(v + __bfloat162float(postab[(size_t)pos * H + n]));
-    }
+    const float v = row < B ? embed_value(p, row, n, pos) : 0.f;
     res_s[row * 8 + f] = v;
     x_img[(size_t)xo_slice * x_slice_elems + row * pitch + xo_col + f] = __float2bfloat16_rn(v);
   }
@@ -389,7 +282,7 @@ __global__ void __launch_bounds__(THREADS, 1) decode_step_cluster_kernel(const _
   {
     const bf16* nimg; uint32_t nbytes;
     slice_of(PH_QKV, nimg, nbytes);
-    bar_target = grid_sync(bar_ctr, bar_target, -1, [&]() { request_slice(nimg, nbytes); }, []() {}, acq);
+    bar_target = grid_sync(bar_ctr, bar_target, -1, false, nullptr, [&]() { request_slice(nimg, nbytes); });
   }
   prof_mark(prof, 7);
 
@@ -422,7 +315,6 @@ __global__ void __launch_bounds__(THREADS, 1) decode_step_cluster_kernel(const _
     const int blk = rowpart ? 32 + 4 * 16 * q * 4 : 256 + ROWS * RS * 4;   // one exchanged block: [statistics][rows][columns]
     const int wsend = rowpart ? C * blk : blk;                       // bytes a warp stages
     const int j0 = JOBS_PER_LAYER * l + (sub == 0 ? 0 : sub + QKV_JOBS - 1);   // first weight job of this phase
-    const int njobs = sub == 0 ? QKV_JOBS : 1;
 
     // folded-LayerNorm vectors of this phase's features: requested now, parked in shared memory after the MMA loop (a global
     // load followed at once by its shared-memory store would park the warp for an L2 round trip in front of the MMAs)
@@ -514,17 +406,6 @@ __global__ void __launch_bounds__(THREADS, 1) decode_step_cluster_kernel(const _
     prof_mark(prof, 2);
     if (has_ln && tid < (rowpart ? Nc : 8 * q)) { cvec[tid] = cv1; cvec[256 + tid] = cv2; }   // read in the epilogue, several barriers later
     __syncthreads();  // activation slice and weight buffer(s) are dead
-    if (lane == 0 && (pf_on || pf_kv)) {  // asynchronous requests, one or two per warp so that no single thread holds the CTA back
-      for (int i = 0; i < njobs; i++) prefetch_weight_job_part(j0 + i + JOBS_PER_LAYER, warp);  // same job, next layer (or lm heads) -> L2
-      if (sub == PH_QKV && warp == 2 && l + 1 < p.L) {   // next layer's folded-LN vectors: every CTA pulls a 1/grid share into L2
-        const int64_t c_bytes = p.c_fc1 + (int64_t)2 * F * 4 - p.c_qkv;
-        const uint32_t share = (uint32_t)(((c_bytes / (int)gridDim.x) + 15) & ~15);
-        const int64_t o = (int64_t)cta * share;
-        if (pf_on && o < c_bytes) l2_prefetch(lb + p.layer_stride + p.c_qkv + o, (uint32_t)(c_bytes - o < share ? c_bytes - o : share));
-      }
-      if (sub == PH_O && l + 1 < p.L) prefetch_kv_part(l + 1, false, warp);
-      if (sub == PH_OC && l + 1 < p.L) prefetch_kv_part(l + 1, true, warp);
-    }
     prof_mark(prof, 12);
     cluster_wait();  // every peer is past its previous epilogue: my send blocks have been read, its receive slots are free
     prof_mark(prof, 13);
@@ -542,7 +423,6 @@ __global__ void __launch_bounds__(THREADS, 1) decode_step_cluster_kernel(const _
     if (tid == 0) mbar_expect_tx(xbar, (uint32_t)(nslots * blk));
     {
       unsigned char* mine = send + (size_t)warp * wsend;
-      const bool merged = rowpart && !(p.dbg & 1024);
       if (!rowpart) {
         float* bp = reinterpret_cast<float*>(mine + 256);
 #pragma unroll
@@ -571,8 +451,8 @@ __global__ void __launch_bounds__(THREADS, 1) decode_step_cluster_kernel(const _
         const int qc = 16 * q;   // this warp's columns: pass 0, then pass 1
         // live row g (fragment elements 0, 1) -> destination rank g >> 2, row g & 3 of its block.  [destination][warp] order, so
         // that ONE copy per destination ships all eight warps' blocks (every bulk copy costs issue time through the uniform datapath,
-        // on every warp's critical path; PTTS_DBG=1024 keeps the per-warp copies, [warp][destination] order)
-        unsigned char* blk_d = merged ? send + ((size_t)(g >> 2) * V + warp) * blk : mine + (size_t)(g >> 2) * blk;
+        // on every warp's critical path)
+        unsigned char* blk_d = send + ((size_t)(g >> 2) * V + warp) * blk;
         float* bp = reinterpret_cast<float*>(blk_d + 32) + (g & 3) * qc + 2 * t4;
 #pragma unroll
         for (int P = 0; P < 2; P++)
@@ -589,17 +469,14 @@ __global__ void __launch_bounds__(THREADS, 1) decode_step_cluster_kernel(const _
       if (!rowpart) {
         if (lane == 0) {
           fence_proxy_async_smem();
-          bulk_s2peer(mapa(s32(recv + (size_t)(4 * rank + e4) * blk), (uint32_t)dgrp), mine, (uint32_t)blk, mapa(s32(xbar), (uint32_t)dgrp));
+          bulk_s2peer(mapa(smem_u32(recv + (size_t)(4 * rank + e4) * blk), (uint32_t)dgrp), mine, (uint32_t)blk, mapa(smem_u32(xbar), (uint32_t)dgrp));
         }
-      } else if (merged) {
+      } else {
         __syncthreads();   // all eight warps' blocks are staged
         if (warp < C && lane == 0) {   // warp d ships [d][0..7] to rank d: it lands as slots 8 rank .. 8 rank + 7 there
           fence_proxy_async_smem();
-          bulk_s2peer(mapa(s32(recv + (size_t)(8 * rank) * blk), (uint32_t)warp), send + (size_t)warp * V * blk, (uint32_t)(V * blk), mapa(s32(xbar), (uint32_t)warp));
+          bulk_s2peer(mapa(smem_u32(recv + (size_t)(8 * rank) * blk), (uint32_t)warp), send + (size_t)warp * V * blk, (uint32_t)(V * blk), mapa(smem_u32(xbar), (uint32_t)warp));
         }
-      } else if (lane < C) {
-        fence_proxy_async_smem();
-        bulk_s2peer(mapa(s32(recv + (size_t)(8 * rank + warp) * blk), (uint32_t)lane), mine + (size_t)lane * blk, (uint32_t)blk, mapa(s32(xbar), (uint32_t)lane));
       }
     }
     // The weight ring's refill goes out now, while the partial sums travel (two jobs ahead; the head phases hold the next head
@@ -683,7 +560,7 @@ __global__ void __launch_bounds__(THREADS, 1) decode_step_cluster_kernel(const _
     }
     prof_mark(prof, 4);
     __syncthreads();   // this CTA's receive slots are consumed (and q|k|v complete): peers may send the next phase's partials
-    cluster_arrive_reuse((p.dbg & 64) != 0);
+    cluster_arrive_reuse();
     if (rowpart) {
       // the attention's scratch aliases the send blocks: the peers must have RECEIVED them (each is past its exchange wait) first
       cluster_wait();
@@ -694,31 +571,14 @@ __global__ void __launch_bounds__(THREADS, 1) decode_step_cluster_kernel(const _
     // makes (same key chunks, same split over the two warps, same merge), so the two step kernels agree bit for bit ----
     if (rowpart) {
       if (att_row < B) {
-        AttnArgs att{};
-        att.ctrl = nullptr; att.B = B; att.nh = p.nh; att.nkv = p.nh; att.q_len = 1;
-        att.past_from_ctrl = 0; att.past_len = pos; att.prefix = p.P;
-        att.rope = p.rope; att.rope_cos = blob + p.rope_cos; att.rope_sin = blob + p.rope_sin; att.scale = p.scale;
+        AttnArgs att = decode_attn_args(p, l, pos, sub == PH_QC);
         const bf16* qkv_s = reinterpret_cast<const bf16*>(Rg + QKV_OFF);
         const int row_base = HROWS * rblk + 4 * rank;
         const bf16* qbase = qkv_s - (size_t)row_base * Nc - (size_t)head * HD;
-        att.q = qbase; att.ldq = Nc; att.q_col0 = 0;
+        att.q = qbase; att.ldq = Nc;
         att.ldo = pitch;
         att.out = a_img + (size_t)att_slice * x_slice_elems + att_col - (size_t)head * HD;
-        if (sub == PH_QKV) {
-          att.knew = qbase; att.vnew = qbase; att.ldkv = Nc; att.k_col0 = HD; att.v_col0 = 2 * HD;
-          char* kc = p.self_kv + p.self_layer_stride * l;
-          att.kcache = kc; att.vcache = kc + (size_t)B * p.nh * p.Tmax * HD * 2;
-          att.kv_b_stride = (int64_t)p.nh * p.Tmax * HD; att.kv_h_stride = (int64_t)p.Tmax * HD; att.kv_t_stride = HD;
-          att.key_mask = p.prompt_mask; att.mask_len = p.P; att.mask_ld = p.P;
-          att.cross = 0; att.kv_len = 0; att.kv_capacity = p.Tmax;
-        } else {
-          att.knew = nullptr; att.vnew = nullptr;
-          char* ck = p.cross_kv + p.cross_layer_stride * l;
-          att.kcache = ck; att.vcache = ck + (size_t)B * p.nh * p.S * HD * 2;
-          att.kv_b_stride = (int64_t)p.nh * p.S * HD; att.kv_h_stride = (int64_t)p.S * HD; att.kv_t_stride = HD;
-          att.key_mask = p.enc_mask; att.mask_len = p.S; att.mask_ld = p.S;
-          att.cross = 1; att.kv_len = p.S; att.kv_capacity = p.S;
-        }
+        if (sub == PH_QKV) { att.knew = qbase; att.vnew = qbase; att.ldkv = Nc; att.k_col0 = HD; att.v_col0 = 2 * HD; }
         // per-warp scratch (K/V ring stages, then 192 floats): warps 0-4 in R below the q|k|v rows, warps 5-7 in the weight buffer
         // whose job is held back; the pair merge in the other buffer's tail, behind out-proj's / cross out-proj's 16 KB
         unsigned char* wb0 = smem + HDR;
@@ -749,7 +609,10 @@ __global__ void __launch_bounds__(THREADS, 1) decode_step_cluster_kernel(const _
     const bf16* nimg; uint32_t nbytes;
     if (last) { nimg = x_img; nbytes = (uint32_t)(C * x_slice_elems * 2); }   // lm heads: the whole x image
     else slice_of((sub + 1) % 6, nimg, nbytes);
-    bar_target = grid_sync(bar_ctr, bar_target, ph, [&]() { request_slice(nimg, nbytes); }, []() {}, acq);
+    // Everything this kernel reads that another CTA wrote during the same launch goes through L2 (TMA bulk copies of the images
+    // and the K/V rows, __ldcg of the logits / EOS columns), so the L1 invalidation of an acquire fence protects nothing here and
+    // would cost time at every barrier: the per-layer barriers (and the first one) go without it.
+    bar_target = grid_sync(bar_ctr, bar_target, ph, false, nullptr, [&]() { request_slice(nimg, nbytes); });
     prof_mark(prof, 7);
   }
   cluster_wait();  // balance the last phase's arrive
@@ -762,9 +625,6 @@ __global__ void __launch_bounds__(THREADS, 1) decode_step_cluster_kernel(const _
     const int ntasks = p.K * p.V / 32;
     const float* c1 = reinterpret_cast<const float*>(blob + p.c_heads);
     const float* c2 = c1 + p.K * p.V;
-    if (lane == 0) {  // layer 0 of the NEXT token -> L2 (the cache outlives the kernel): its first phases start warm
-      for (int j = 0; j < JOBS_PER_LAYER; j++) prefetch_weight_job_part(j, warp);
-    }
     mbar_wait(abar, par_a, 3);
     par_a ^= 1u;
     const bf16* xs = reinterpret_cast<const bf16*>(Rg);   // [2 slices][32][pitch]
@@ -780,7 +640,7 @@ __global__ void __launch_bounds__(THREADS, 1) decode_step_cluster_kernel(const _
 #pragma unroll
           for (int j = 0; j < 2; j++) {
             uint32_t a[4];
-            ldsm4(a, sl + (size_t)(mt * 16 + lrow) * pitch + j * 16 + lcol);
+            ldmatrix_x4(a, sl + (size_t)(mt * 16 + lrow) * pitch + j * 16 + lcol);
             row_stat_mma(rst, mt, a);
           }
       }
@@ -810,7 +670,7 @@ __global__ void __launch_bounds__(THREADS, 1) decode_step_cluster_kernel(const _
 #pragma unroll
         for (int mt = 0; mt < 2; mt++)
 #pragma unroll
-          for (int j = 0; j < 2; j++) ldsm4(a[mt][j], sl + (size_t)(mt * 16 + lrow) * pitch + j * 16 + lcol);
+          for (int j = 0; j < 2; j++) ldmatrix_x4(a[mt][j], sl + (size_t)(mt * 16 + lrow) * pitch + j * 16 + lcol);
 #pragma unroll
         for (int j = 0; j < 4; j++) {
           const uint4 w = wb[((size_t)j * KTH + kt) * 32];
@@ -854,24 +714,21 @@ __global__ void __launch_bounds__(THREADS, 1) decode_step_cluster_kernel(const _
     }
   }
   prof_mark(prof, 6);
-  bar_target = grid_sync(bar_ctr, bar_target, n_phases, []() {}, []() {});
+  bar_target = grid_sync(bar_ctr, bar_target, n_phases, true);
   prof = prof0 ? prof0 + (size_t)(n_phases + 2) * PROF_STRIDE : nullptr;  // tail row: sampling / barrier
   prof_mark(prof, 0);
   if (p.do_sample_phase) {
     const ptts_gen_params gp = *p.sa.gen;
     const int BK = B * p.K;
-    // PTTS_DBG=128 (measurement only): a first, cold pass (instruction fetch) before the stamped one; the pass is idempotent
-    for (int pass = (p.dbg & 128) ? 0 : 1; pass < 2; pass++) {
-      sample_all_rows_cta<ITEMS>(p.sa, gp, cta, (int)gridDim.x, BK, cur_len);
-      prof_mark(prof, pass == 0 ? 4 : 1);
-    }
+    sample_phase<ITEMS>(p.sa, gp, BK, cur_len);
+    prof_mark(prof, 1);
     // every CTA learns whether any row is still unfinished: thread 0 reads the counter the moment the barrier opens (after its
     // acquire fence); the counter is reset only when the launch ends, so a step's count is the growth since the previous step
-    bar_target = grid_sync(bar_ctr, bar_target, n_phases + 1, [&]() {
+    bar_target = grid_sync(bar_ctr, bar_target, n_phases + 1, true, nullptr, [&]() {
       const int tot = *reinterpret_cast<volatile int*>(&ctrl->n_unfinished);
       s_next_active = (tot - unfinished_prev > 0) ? 1 : 0;
       unfinished_prev = tot;
-    }, []() {});
+    });
     prof_mark(prof, 2);
   }
   bool go_on = false;
@@ -948,10 +805,7 @@ static void cluster_launch_config(const StepParams& p, cudaLaunchConfig_t& cfg, 
   at[1].id = cudaLaunchAttributeCooperative;   // every CTA spins on the others: co-residency must be guaranteed
   at[1].val.cooperative = 1;
   cfg.attrs = at;
-  // PTTS_STEP_COOP=0: cluster attribute only (Nsight Compute cannot launch a cooperative cluster grid; the 128 CTAs of an
-  // otherwise idle GPU are co-resident anyway -- profiling runs only)
-  static const bool coop = [] { const char* v = getenv("PTTS_STEP_COOP"); return !(v && v[0] == '0'); }();
-  cfg.numAttrs = coop ? 2 : 1;
+  cfg.numAttrs = 2;
 }
 
 // true when the grid of 4 nh clusters of 2 can be co-resident on this device (Mini: 64 of the 66 a 132-SM H100 holds)

@@ -12,6 +12,7 @@
 #include <cuda.h>
 
 #include "common.cuh"
+#include "ptx.cuh"
 
 namespace ptts {
 namespace wg {
@@ -28,28 +29,23 @@ template <int N> constexpr int STAGE_BYTES = (A_BYTES + N * K_STAGE * 2 + 1023) 
 // dynamic shared memory of a CTA: alignment slack, the stage ring, then 128 B of mbarriers, then `extra` bytes for the caller
 template <int N> constexpr size_t smem_bytes(int extra) { return 1024 + (size_t)STAGES * STAGE_BYTES<N> + 128 + extra; }
 
-__device__ __forceinline__ uint32_t smem_addr(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint64_t* b, uint32_t n) { asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_addr(b)), "r"(n)); }
-__device__ __forceinline__ void mbar_expect(uint64_t* b, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_addr(b)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t* b) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_addr(b)) : "memory"); }
+__device__ __forceinline__ void mbar_arrive(uint64_t* b) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(b)) : "memory"); }
 // A wait that never completes traps (the launch fails) instead of hanging the GPU.  No printf here: a function call inside
 // the consumer's K loop would make ptxas serialise the wgmma pipeline.
 __device__ __forceinline__ void mbar_wait(uint64_t* b, uint32_t parity) {
   uint32_t ok, spins = 0;
   do {
-    asm volatile("{\n.reg .pred p;\nmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\nselp.u32 %0, 1, 0, p;\n}" : "=r"(ok) : "r"(smem_addr(b)), "r"(parity) : "memory");
+    ok = mbar_try_wait(b, parity);
     if (!ok && ++spins > (1u << 24)) __trap();
   } while (!ok);
 }
 __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, int c0, int c1, uint64_t* bar) {
   asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
-               ::"r"(smem_addr(dst)), "l"(map), "r"(c0), "r"(c1), "r"(smem_addr(bar)) : "memory");
+               ::"r"(smem_u32(dst)), "l"(map), "r"(c0), "r"(c1), "r"(smem_u32(bar)) : "memory");
 }
 __device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* map, int c0, int c1, int c2, uint64_t* bar) {
   asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4}], [%5];"
-               ::"r"(smem_addr(dst)), "l"(map), "r"(c0), "r"(c1), "r"(c2), "r"(smem_addr(bar)) : "memory");
+               ::"r"(smem_u32(dst)), "l"(map), "r"(c0), "r"(c1), "r"(c2), "r"(smem_u32(bar)) : "memory");
 }
 
 // wgmma shared-memory matrix descriptor, K-major, 128-byte swizzle: 8-row groups 1024 B apart (stride byte offset); the
@@ -109,12 +105,12 @@ struct Pipe {
 template <int N>
 __device__ __forceinline__ Pipe pipe_setup(unsigned char* smem_raw) {
   Pipe p;
-  p.stages = smem_raw + ((1024u - (smem_addr(smem_raw) & 1023u)) & 1023u);
+  p.stages = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   p.full = reinterpret_cast<uint64_t*>(p.stages + STAGES * STAGE_BYTES<N>);
   p.empty = p.full + STAGES;
   p.extra = reinterpret_cast<unsigned char*>(p.full) + 128;
   if (threadIdx.x == 0) {
-    for (int s = 0; s < STAGES; s++) { mbar_init(&p.full[s], 1); mbar_init(&p.empty[s], CONSUMER_WARPS); }
+    for (int s = 0; s < STAGES; s++) { mbar_init<1>(&p.full[s]); mbar_init<CONSUMER_WARPS>(&p.empty[s]); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   return p;
@@ -131,7 +127,7 @@ __device__ __forceinline__ void mainloop(const Pipe& p, int n_iter, Load load, f
         const int s = it % STAGES, use = it / STAGES;
         if (use > 0) mbar_wait(&p.empty[s], (use - 1) & 1);
         unsigned char* a_dst = p.stages + (size_t)s * STAGE_BYTES<N>;
-        mbar_expect(&p.full[s], (uint32_t)(A_BYTES + N * K_STAGE * 2));
+        mbar_expect_tx(&p.full[s], (uint32_t)(A_BYTES + N * K_STAGE * 2));
         load(it, a_dst, a_dst + A_BYTES, &p.full[s]);
       }
     }
@@ -141,7 +137,7 @@ __device__ __forceinline__ void mainloop(const Pipe& p, int n_iter, Load load, f
   for (int it = 0; it < n_iter; it++) {
     const int s = it % STAGES;
     mbar_wait(&p.full[s], (it / STAGES) & 1);
-    const uint32_t a_addr = smem_addr(p.stages + (size_t)s * STAGE_BYTES<N>);
+    const uint32_t a_addr = smem_u32(p.stages + (size_t)s * STAGE_BYTES<N>);
     const uint64_t da = desc_sw128(a_addr + a_row0), db = desc_sw128(a_addr + A_BYTES);
     asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
 #pragma unroll

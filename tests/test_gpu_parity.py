@@ -493,9 +493,9 @@ def test_fused_step_mini_shape_batch32(monkeypatch):
     assert np.array_equal(a_log, b_log)
 
 
-# Mini (16 heads: 32 clusters of 4 CTAs) and a 12-head shape (H 768, F 3072: 24 clusters).  At H = 768 each K half of a rank's
+# Mini (16 heads: 64 clusters of 2 CTAs) and a 12-head shape (H 768, F 3072: 48 clusters).  At H = 768 each K half of a rank's
 # slice is an ODD number of k-tiles (3) and a K slice holds three heads, not four: the cases mma_slice's paired k-tile loop and the
-# attention output placement must handle.  A 132-SM H100 holds 30 clusters of 4 co-resident: the 12-head shape only.
+# attention output placement must handle.  A 132-SM H100 holds 66 clusters of 2 co-resident: both shapes.
 CLUSTER_SHAPES = {"mini": {}, "h768": dict(hidden_size=768, num_attention_heads=12, ffn_dim=3072)}
 _cluster_fit = {}
 
