@@ -183,6 +183,22 @@ int ptts_logits_processor(const int64_t* input_ids, int32_t BK, int32_t seq_len,
 int ptts_op_linear(const ptts_decoder_config* cfg, const void* blob, int32_t tensor_id, int32_t index,
                    const void* x, int32_t M, int32_t use_ln, int32_t epilogue /*0 store,1 act,2 +res,3 f32*/,
                    const void* residual, void* y, void* stream);
+/* Self- or cross-attention of q_len new positions per batch row (ParlerTTSSdpaAttention after the projections, :858-914), with
+ * the kernels the decoder launches.  Test hook for the attention sweeps.
+ *   dtype PTTS_BF16 / PTTS_F32; nh query heads, nkv K/V heads (nh % nkv == 0); head_dim 64; scale 1/8.
+ *   self  (cross == 0): qkv [B*q_len, (nh + 2 nkv)*64] = q | k | v of the new positions, at cache positions past_len .. past_len +
+ *                       q_len - 1; the new K (rotary applied) and V rows are appended to the caches; causal over the cache.
+ *   cross (cross != 0): qkv = q [B*q_len, nh*64]; keys are the kv_len cached rows; past_len only sets the rotary position.
+ *   kcache, vcache [B][nkv][capacity][64], rows stored swizzled (element d of row t at (((d/8) ^ t) % 8)*8 + d%8).
+ *   rope != 0: rope_cos / rope_sin [max_pos][64] in dtype, applied to q (and to the appended K rows).
+ *   key_mask [B][mask_len] int32 or NULL: key t < mask_len with key_mask[b][t] == 0 is excluded.
+ *   prefill_sweep (q_len > 1): 0 = the decoder's choice (the tensor-core sweep for bf16 with nh == nkv unless
+ *                  PTTS_PREFILL_ATTN_TC=0), 1 = always the scalar sweep (attention_item).
+ *   out [B*q_len, nh*64] in dtype. */
+int ptts_op_attention(int32_t dtype, int32_t B, int32_t nh, int32_t nkv, int32_t q_len, int32_t past_len, int32_t cross,
+                      int32_t kv_len, int32_t capacity, int32_t rope, const void* rope_cos, const void* rope_sin, const void* qkv,
+                      void* kcache, void* vcache, const int32_t* key_mask, int32_t mask_len, int32_t prefill_sweep, void* out,
+                      void* stream);
 
 /* ---- DAC decode ------------------------------------------------------------------------------ */
 typedef struct ptts_dac_config {

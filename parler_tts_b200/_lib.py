@@ -70,6 +70,8 @@ _SIGS = {
     "ptts_delay_apply": (C.c_int, [_VP, _I32, _I32, _I64, _VP, _I64, _VP, _VP]),
     "ptts_logits_processor": (C.c_int, [_VP, _I32, _I32, _I64, _VP, _I32, _I64, _I32, _VP, _VP]),
     "ptts_op_linear": (C.c_int, [C.POINTER(DecoderConfigC), _VP, _I32, _I32, _VP, _I32, _I32, _I32, _VP, _VP, _VP]),
+    "ptts_op_attention": (C.c_int, [_I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _VP, _VP, _VP, _VP, _VP, _VP,
+                                    _I32, _I32, _VP, _VP]),
     "ptts_dac_blob_bytes": (C.c_int, [C.POINTER(DacConfigC), C.POINTER(_I64)]),
     "ptts_dac_num_tensors": (C.c_int, [C.POINTER(DacConfigC), C.POINTER(_I32)]),
     "ptts_dac_pack": (C.c_int, [C.POINTER(DacConfigC), _VP, _I32, _VP, _I32, _I64, _VP]),

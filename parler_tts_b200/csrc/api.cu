@@ -409,7 +409,7 @@ static int run_forward(ptts_session* s, cudaStream_t st, bool prefill, const voi
     at.rope = c.rope; at.rope_cos = blob + L.rope_cos; at.rope_sin = blob + L.rope_sin;
     at.kv_capacity = prefill ? q_len : W.Tmax;
     at.scale = 0.125f;  // head_dim ** -0.5, applied inside SDPA (quirk Q1)
-    if (int e = launch_attention(at, c.dtype, st, pdl)) return e;
+    if (int e = launch_attention(at, c.dtype, st, pdl, prefill_attn_tc_default())) return e;
     s->launches++;
     if (int e = lin(ws + W.attn, H, lb + L.wo, H, H, nullptr, nullptr, EPI_RESIDUAL, x, x, H, M)) return e;
     if (int e = lin(x, H, lb + L.wqc, H, H, (const float*)(blob + lb + L.ln2_w), (const float*)(blob + lb + L.ln2_b),
@@ -422,7 +422,7 @@ static int run_forward(ptts_session* s, cudaStream_t st, bool prefill, const voi
     ct.kv_b_stride = (int64_t)L.nckv * S * D; ct.kv_h_stride = (int64_t)S * D; ct.kv_t_stride = D;
     ct.key_mask = s->has_enc_mask ? (const int*)(ws + W.enc_mask) : nullptr; ct.mask_len = S; ct.mask_ld = S;
     ct.nkv = L.nckv; ct.cross = 1; ct.kv_len = S; ct.kv_capacity = S;
-    if (int e = launch_attention(ct, c.dtype, st, pdl)) return e;
+    if (int e = launch_attention(ct, c.dtype, st, pdl, prefill_attn_tc_default())) return e;
     s->launches++;
     if (int e = lin(ws + W.attn, H, lb + L.woc, H, H, nullptr, nullptr, EPI_RESIDUAL, x, x, H, M)) return e;
     if (int e = lin(x, H, lb + L.fc1, L.F, H, (const float*)(blob + lb + L.ln3_w), (const float*)(blob + lb + L.ln3_b),
@@ -609,6 +609,38 @@ int ptts_op_linear(const ptts_decoder_config* cfg, const void* blob, int32_t ten
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sm, cudaDevAttrMultiProcessorCount, dev);
   return launch_linear(a, cfg->dtype, (cudaStream_t)stream, false, sm);
+}
+
+int ptts_op_attention(int32_t dtype, int32_t B, int32_t nh, int32_t nkv, int32_t q_len, int32_t past_len, int32_t cross,
+                      int32_t kv_len, int32_t capacity, int32_t rope, const void* rope_cos, const void* rope_sin, const void* qkv,
+                      void* kcache, void* vcache, const int32_t* key_mask, int32_t mask_len, int32_t prefill_sweep, void* out,
+                      void* stream) {
+  PTTS_REQUIRE(qkv && kcache && vcache && out, "null argument");
+  PTTS_REQUIRE(dtype == PTTS_BF16 || dtype == PTTS_F32, "op_attention: dtype must be bf16 or f32");
+  PTTS_REQUIRE(B > 0 && nh > 0 && nkv > 0 && nh % nkv == 0 && q_len > 0 && past_len >= 0, "op_attention: bad shape");
+  PTTS_REQUIRE(cross ? (kv_len > 0 && kv_len <= capacity) : (past_len + q_len <= capacity),
+               "op_attention: %d keys do not fit a cache of %d positions", cross ? kv_len : past_len + q_len, capacity);
+  PTTS_REQUIRE(!rope || (rope_cos && rope_sin), "op_attention: rope needs both tables");
+  PTTS_REQUIRE(mask_len >= 0 && (key_mask || mask_len == 0), "op_attention: bad key mask");
+  PTTS_REQUIRE(prefill_sweep == 0 || prefill_sweep == 1, "op_attention: prefill_sweep is 0 (product choice) or 1 (attention_item)");
+  const int D = PTTS_HEAD_DIM;
+  AttnArgs a{};
+  if (cross) {  // q [B*q_len, nh*64]
+    a.q = qkv; a.ldq = (int64_t)nh * D;
+  } else {      // fused projections [B*q_len, (nh + 2 nkv)*64]: q | k | v, as run_forward's qkv matrix
+    a.q = a.knew = a.vnew = qkv;
+    a.ldq = a.ldkv = (int64_t)(nh + 2 * nkv) * D; a.k_col0 = nh * D; a.v_col0 = (nh + nkv) * D;
+  }
+  a.kcache = kcache; a.vcache = vcache;
+  a.kv_b_stride = (int64_t)nkv * capacity * D; a.kv_h_stride = (int64_t)capacity * D; a.kv_t_stride = D;
+  a.out = out; a.ldo = (int64_t)nh * D;
+  a.key_mask = key_mask; a.mask_len = mask_len; a.mask_ld = mask_len;
+  a.B = B; a.nh = nh; a.nkv = nkv; a.q_len = q_len;
+  a.past_len = past_len; a.cross = cross ? 1 : 0; a.kv_len = cross ? kv_len : 0;
+  a.rope = rope; a.rope_cos = rope_cos; a.rope_sin = rope_sin;
+  a.kv_capacity = cross ? kv_len : past_len + q_len;   // keys per query at most (attention_item's score buffer)
+  a.scale = 0.125f;
+  return launch_attention(a, dtype, (cudaStream_t)stream, false, prefill_sweep == 0 && prefill_attn_tc_default());
 }
 
 // ---- DAC ----------------------------------------------------------------------------------------

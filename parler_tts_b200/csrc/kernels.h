@@ -45,7 +45,10 @@ struct AttnArgs {
   int kv_capacity;      // upper bound on keys per query (sizes the score buffer)
   float scale;
 };
-int launch_attention(const AttnArgs& a, int dtype, cudaStream_t st, bool pdl);
+// prefill_tc: bf16 MHA prefill (q_len > 1) runs on the tensor-core sweep (attention_prefill_tc_kernel) rather than attention_item
+int launch_attention(const AttnArgs& a, int dtype, cudaStream_t st, bool pdl, bool prefill_tc);
+// the product's choice of prefill sweep: on unless PTTS_PREFILL_ATTN_TC=0 (read once per process)
+bool prefill_attn_tc_default();
 
 // ---- embedding (embed.cu) -----------------------------------------------------------------------
 struct EmbedArgs {
