@@ -374,10 +374,12 @@ __global__ void __launch_bounds__(THREADS, 1) decode_step_cluster_kernel(const _
         };
         head_pass(std::integral_constant<int, 0>{});
         if (sub == PH_QKV) {   // quarters 2 and 3 of the head's QKV slice take the ring buffers of quarters 0 and 1
+          prof_mark(prof, 8);
           __syncthreads();
           if (tid == 0) { issue_weight_job(j0 + 2); issue_weight_job(j0 + 3); }
           wait_job(j0 + 2);
           wait_job(j0 + 3);
+          prof_mark(prof, 9);
         }
         head_pass(std::integral_constant<int, 1>{});
       } else if (sub == PH_FC2) {
@@ -389,10 +391,12 @@ __global__ void __launch_bounds__(THREADS, 1) decode_step_cluster_kernel(const _
           mma_slice<1, 2, false, QQ == 1>(acc, rst, xs, apitch, wq, 2 * KT, (e4 - QQ * KT) & 3, KT, lrow, lcol);
         };
         quarter(std::integral_constant<int, 0>{});
+        prof_mark(prof, 8);
         __syncthreads();   // the first quarter is dead: the second one replaces it
         if (tid == 0) request_slice(h_img + (size_t)(2 * rank + 1) * h_slice_elems, (uint32_t)(h_slice_elems * 2));
         mbar_wait(abar, par_a, 0);
         par_a ^= 1u;
+        prof_mark(prof, 9);
         quarter(std::integral_constant<int, 1>{});
       } else {
         const uint4* wb = ring(j0) + (size_t)(dgrp * q) * KT * 32;   // this destination's n-tiles
@@ -479,9 +483,10 @@ __global__ void __launch_bounds__(THREADS, 1) decode_step_cluster_kernel(const _
         }
       }
     }
-    // The weight ring's refill goes out now, while the partial sums travel (two jobs ahead; the head phases hold the next head
-    // phase's or fc1's weights back until their attention is done: the attention uses that buffer meanwhile).
-    if (warp == 1 && lane == 0 && !rowpart) issue_weight_job(j0 + 2);
+    // The weight ring's refill goes out now, while the partial sums travel (two jobs ahead).  The head phases hold the next head
+    // phase's or fc1's weights back until their attention is done (the attention uses that buffer meanwhile), and cross out-proj
+    // holds fc2's back: those three go out when the barrier opens (below).
+    if (warp == 1 && lane == 0 && !rowpart && sub != PH_OC) issue_weight_job(j0 + 2);
     if (warp == 1 && lane == 0 && sub == PH_QKV) issue_weight_job(j0 + QKV_JOBS);   // out-proj
     prof_mark(prof, 15);
     mbar_wait(xbar, par_x, 2);
@@ -589,13 +594,6 @@ __global__ void __launch_bounds__(THREADS, 1) decode_step_cluster_kernel(const _
         attention_decode_item_warp<bf16>(att, att_row, head, pos, region, attbars + 2 * warp, lane, att_parity, warp & 1, 2, xr, (warp >> 1) + 1);
       }
       prof_mark(prof, 5);
-      // q_cross's (QKV phase) or fc1's (q_cross phase) weights were held back: the attention used their buffer (its floats are
-      // written with generic stores: the fence orders them before the bulk copy's writes)
-      __syncthreads();
-      if (tid == 32) {
-        fence_proxy_async_smem();
-        issue_weight_job(sub == PH_QKV ? j0 + QKV_JOBS + 1 : j0 + 2);
-      }
     }
     prof_mark(prof, 6);
     if (p.prof != nullptr && l == p.L / 2 && tid == 0) {   // profiling runs: when does EACH CTA reach the barrier of the middle layer's phases
@@ -612,7 +610,15 @@ __global__ void __launch_bounds__(THREADS, 1) decode_step_cluster_kernel(const _
     // Everything this kernel reads that another CTA wrote during the same launch goes through L2 (TMA bulk copies of the images
     // and the K/V rows, __ldcg of the logits / EOS columns), so the L1 invalidation of an acquire fence protects nothing here and
     // would cost time at every barrier: the per-layer barriers (and the first one) go without it.
-    bar_target = grid_sync(bar_ctr, bar_target, ph, false, nullptr, [&]() { request_slice(nimg, nbytes); });
+    // A 64 KB weight copy issued shortly before the barrier (q_cross's after the self-attention, fc1's after the cross-attention,
+    // fc2's during the cross out-proj exchange) is still in flight when the barrier opens; with it there, these barriers took
+    // 2-2.5 us longer on an H100.  Those jobs are requested right after the next phase's activation slice instead
+    // (request_slice's proxy fence also orders the attention's generic writes into the held buffer before the copy).
+    const int held_job = sub == PH_QKV ? j0 + QKV_JOBS + 1 : (sub == PH_QC || sub == PH_OC) ? j0 + 2 : -1;
+    bar_target = grid_sync(bar_ctr, bar_target, ph, false, nullptr, [&]() {
+      request_slice(nimg, nbytes);
+      if (held_job >= 0) issue_weight_job(held_job);
+    });
     prof_mark(prof, 7);
   }
   cluster_wait();  // balance the last phase's arrive
