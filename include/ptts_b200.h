@@ -72,7 +72,8 @@ typedef struct ptts_gen_params {
   int32_t row_base;        /* global index of this session's first row (= first utterance * num_codebooks): with a batch
                             * sharded over GPUs every shard passes its own offset, so the draws of an utterance do not
                             * depend on the number of shards (SURVEY 8e) */
-  int32_t reserved_;
+  int32_t input_len;       /* n0: columns of the BOS-led decoder input the generation continues from (0 means 1, the BOS
+                            * column alone).  MinNewTokens skips these columns.  ptts_generate_begin_ids sets it. */
 } ptts_gen_params;
 
 /* Tensor ids for ptts_decoder_pack(). `index` = layer (per-layer tensors) or codebook (EMBED/LM_HEAD). */
@@ -115,11 +116,20 @@ int ptts_decoder_finalize(const ptts_decoder_config* cfg, void* blob, void* stre
 int ptts_workspace_bytes(const ptts_decoder_config* cfg, int32_t B, int32_t P, int32_t S,
                          int32_t max_cache_len, int64_t* out_bytes);
 
+/* Same, for a session that may continue from up to max_input_len decoder input columns (ptts_generate_begin_ids): the prefill
+ * activations are sized for B * (P + max_input_len) rows.  max_input_len = 1 gives exactly ptts_workspace_bytes. */
+int ptts_workspace_bytes2(const ptts_decoder_config* cfg, int32_t B, int32_t P, int32_t S, int32_t max_cache_len,
+                          int32_t max_input_len, int64_t* out_bytes);
+
 typedef struct ptts_session ptts_session; /* host-side object: pointers into blob/workspace + CUDA graphs */
 
 int ptts_session_create(const ptts_decoder_config* cfg, const void* blob, void* workspace,
                         int64_t workspace_bytes, int32_t B, int32_t P, int32_t S, int32_t max_cache_len,
                         ptts_session** out);
+/* Same, with the max_input_len of ptts_workspace_bytes2 (= ptts_session_create when 1). */
+int ptts_session_create2(const ptts_decoder_config* cfg, const void* blob, void* workspace,
+                         int64_t workspace_bytes, int32_t B, int32_t P, int32_t S, int32_t max_cache_len,
+                         int32_t max_input_len, ptts_session** out);
 int ptts_session_destroy(ptts_session* s);
 
 /* Start a generate() call: reset per-call state (ids history = BOS column, processor state,
@@ -128,8 +138,18 @@ int ptts_session_destroy(ptts_session* s);
  * ParlerTTSLogitsProcessor constructor (logits_processors.py:23-42). */
 int ptts_generate_begin(ptts_session* s, const ptts_gen_params* gen, void* stream);
 
-/* Step 0 (prefill): prompt prefix + BOS through the decoder, cross-attention K/V projected once,
- * self-attention cache filled at positions [0, P].  Leaves f32 logits [B*K, V] in the workspace.
+/* Start a generate() call that continues from audio codes (decoder_input_ids, modeling_parler_tts.py:2988-3024, :3523).
+ *   input_ids [B*K, n0] int64 device, BOS-led (the caller prepends the BOS column, :3012-3024), ids in [0, vocab_size];
+ *             NULL with n0 == 1 is the BOS column (= ptts_generate_begin).  1 <= n0 <= max_input_len, n0 < gen->max_length.
+ * On the device, without a host sync: the delayed input (the first n0 columns of build_delay_pattern_mask(input_ids, bos, pad,
+ * max_length), :214-276) becomes the history, the K-1 pattern cells past it are kept for the next-input override (:2909),
+ * cur_len = n0, and the processor state sees the EOS ids inside the prefix.  ptts_prefill then runs the prompt prefix and the n0
+ * columns in one pass (:3033-3044); gen->input_len is set to n0. */
+int ptts_generate_begin_ids(ptts_session* s, const ptts_gen_params* gen, const int64_t* input_ids, int32_t n0, void* stream);
+
+/* Step 0 (prefill): prompt prefix + the n0 delayed input columns (the BOS column unless the call began with
+ * ptts_generate_begin_ids) through the decoder, cross-attention K/V projected once,
+ * self-attention cache filled at positions [0, P + n0).  Leaves f32 logits [B*K, V] in the workspace.
  * Replaces ParlerTTSForCausalLM.forward at step 0 (:1865-1974, :1392-1655, :872-889).
  *   prompt_hidden [B, P, H] model dtype (may be NULL when P == 0)   (:3099-3134 output)
  *   prompt_mask   [B, P] int64 or NULL                              (prompt_attention_mask)

@@ -30,7 +30,7 @@ class GenParamsC(C.Structure):
     _fields_ = [("max_length", C.c_int32), ("min_new_tokens", C.c_int32), ("do_sample", C.c_int32),
                 ("top_k", C.c_int32), ("top_p", C.c_float), ("temperature", C.c_float), ("seed", C.c_uint64),
                 ("suppress_special", C.c_int32), ("codebook_size", C.c_int32),
-                ("row_base", C.c_int32), ("reserved_", C.c_int32)]
+                ("row_base", C.c_int32), ("input_len", C.c_int32)]
 
 
 class DacConfigC(C.Structure):
@@ -53,8 +53,11 @@ _SIGS = {
     "ptts_decoder_finalize": (C.c_int, [C.POINTER(DecoderConfigC), _VP, _VP]),
     "ptts_workspace_bytes": (C.c_int, [C.POINTER(DecoderConfigC), _I32, _I32, _I32, _I32, C.POINTER(_I64)]),
     "ptts_session_create": (C.c_int, [C.POINTER(DecoderConfigC), _VP, _VP, _I64, _I32, _I32, _I32, _I32, C.POINTER(_VP)]),
+    "ptts_workspace_bytes2": (C.c_int, [C.POINTER(DecoderConfigC), _I32, _I32, _I32, _I32, _I32, C.POINTER(_I64)]),
+    "ptts_session_create2": (C.c_int, [C.POINTER(DecoderConfigC), _VP, _VP, _I64, _I32, _I32, _I32, _I32, _I32, C.POINTER(_VP)]),
     "ptts_session_destroy": (C.c_int, [_VP]),
     "ptts_generate_begin": (C.c_int, [_VP, C.POINTER(GenParamsC), _VP]),
+    "ptts_generate_begin_ids": (C.c_int, [_VP, C.POINTER(GenParamsC), _VP, _I32, _VP]),
     "ptts_prefill": (C.c_int, [_VP, _VP, _VP, _VP, _VP, _VP]),
     "ptts_decode_forward": (C.c_int, [_VP, _VP]),
     "ptts_sample": (C.c_int, [_VP, _VP, _VP]),

@@ -42,6 +42,7 @@ struct ptts_session {
   bool pdl, use_graph;
   bool has_prompt_mask, has_enc_mask, begun, prefilled;
   ptts_gen_params gen;
+  int n0;            // decoder input columns of the current generate() call (1: the BOS column; > 1: continuing from codes)
   cudaStream_t cap_stream;
   cudaGraphExec_t exec;
   bool graph_ready;
@@ -156,27 +157,34 @@ int ptts_decoder_finalize(const ptts_decoder_config* cfg, void* blob, void* stre
   return PTTS_OK;
 }
 
-int ptts_workspace_bytes(const ptts_decoder_config* cfg, int32_t B, int32_t P, int32_t S, int32_t max_cache_len, int64_t* out_bytes) {
+int ptts_workspace_bytes2(const ptts_decoder_config* cfg, int32_t B, int32_t P, int32_t S, int32_t max_cache_len, int32_t max_input_len,
+                          int64_t* out_bytes) {
   PTTS_REQUIRE(cfg && out_bytes, "null argument");
   if (int e = validate_config(*cfg)) return e;
   PTTS_REQUIRE(B > 0 && P >= 0 && S > 0 && max_cache_len > P, "workspace: need B>0, P>=0, S>0, max_cache_len>P (got %d %d %d %d)", B, P, S, max_cache_len);
-  PTTS_REQUIRE(max_cache_len <= cfg->max_positions || cfg->rope == 0 || true, "unreachable");
-  *out_bytes = make_workspace(*cfg, B, P, S, max_cache_len).total;
+  PTTS_REQUIRE(max_input_len >= 1 && max_input_len < max_cache_len - P + 1, "workspace: max_input_len %d must be in [1, max_cache_len - P]", max_input_len);
+  *out_bytes = make_workspace(*cfg, B, P, S, max_cache_len, max_input_len).total;
   return PTTS_OK;
 }
 
+int ptts_workspace_bytes(const ptts_decoder_config* cfg, int32_t B, int32_t P, int32_t S, int32_t max_cache_len, int64_t* out_bytes) {
+  return ptts_workspace_bytes2(cfg, B, P, S, max_cache_len, 1, out_bytes);
+}
+
 // ---- session ------------------------------------------------------------------------------------
-int ptts_session_create(const ptts_decoder_config* cfg, const void* blob, void* workspace, int64_t workspace_bytes,
-                        int32_t B, int32_t P, int32_t S, int32_t max_cache_len, ptts_session** out) {
+int ptts_session_create2(const ptts_decoder_config* cfg, const void* blob, void* workspace, int64_t workspace_bytes,
+                         int32_t B, int32_t P, int32_t S, int32_t max_cache_len, int32_t max_input_len, ptts_session** out) {
   PTTS_REQUIRE(cfg && blob && workspace && out, "null argument");
   if (int e = validate_config(*cfg)) return e;
   PTTS_REQUIRE(B > 0 && P >= 0 && S > 0 && max_cache_len > P, "session: bad shape B=%d P=%d S=%d Tmax=%d", B, P, S, max_cache_len);
   PTTS_REQUIRE(max_cache_len <= cfg->max_positions, "session: cache length %d exceeds max_position_embeddings %d", max_cache_len, cfg->max_positions);
+  PTTS_REQUIRE(max_input_len >= 1 && max_input_len < max_cache_len - P + 1, "session: max_input_len %d must be in [1, max_cache_len - P]", max_input_len);
   ptts_session* s = new (std::nothrow) ptts_session();
   PTTS_REQUIRE(s, "out of host memory");
   s->cfg = *cfg;
   s->L = make_layout(*cfg);
-  s->W = make_workspace(*cfg, B, P, S, max_cache_len);
+  s->W = make_workspace(*cfg, B, P, S, max_cache_len, max_input_len);
+  s->n0 = 1;
   if (workspace_bytes < s->W.total) {
     int64_t need = s->W.total;
     delete s;
@@ -203,6 +211,11 @@ int ptts_session_create(const ptts_decoder_config* cfg, const void* blob, void* 
   return PTTS_OK;
 }
 
+int ptts_session_create(const ptts_decoder_config* cfg, const void* blob, void* workspace, int64_t workspace_bytes,
+                        int32_t B, int32_t P, int32_t S, int32_t max_cache_len, ptts_session** out) {
+  return ptts_session_create2(cfg, blob, workspace, workspace_bytes, B, P, S, max_cache_len, 1, out);
+}
+
 int ptts_session_destroy(ptts_session* s) {
   if (!s) return PTTS_OK;
   if (s->exec) cudaGraphExecDestroy(s->exec);
@@ -224,6 +237,7 @@ static SampleArgs sample_args(ptts_session* s) {
   a.first_unf = (int*)(s->ws + W.first_unf);
   a.ctrl = (Ctrl*)(s->ws + W.ctrl);
   a.gen = (const ptts_gen_params*)(s->ws + W.gen);
+  a.prefix_cells = W.prefix_cells >= 0 ? (int64_t*)(s->ws + W.prefix_cells) : nullptr;
   a.B = W.B; a.K = s->cfg.num_codebooks; a.V = s->cfg.vocab_size;
   a.bos = s->cfg.bos_token_id; a.pad = s->cfg.pad_token_id; a.eos = s->cfg.eos_token_id;
   return a;
@@ -318,29 +332,38 @@ static bool setup_fused(ptts_session* s) {
   return true;
 }
 
-int ptts_generate_begin(ptts_session* s, const ptts_gen_params* gen, void* stream) {
+int ptts_generate_begin_ids(ptts_session* s, const ptts_gen_params* gen, const int64_t* input_ids, int32_t n0, void* stream) {
   PTTS_REQUIRE(s && gen, "null argument");
+  PTTS_REQUIRE(n0 >= 1 && n0 <= s->W.max_input, "generate: %d decoder input columns, the session takes 1 .. %d", n0, s->W.max_input);
+  PTTS_REQUIRE(input_ids != nullptr || n0 == 1, "generate: input_ids is required for %d input columns", n0);
   PTTS_REQUIRE(gen->max_length >= 2, "generate: max_length must be >= 2, got %d", gen->max_length);
   PTTS_REQUIRE(gen->max_length <= s->W.raw_ld, "generate: max_length %d exceeds the session's capacity %lld", gen->max_length, (long long)s->W.raw_ld);
   PTTS_REQUIRE(!gen->do_sample || gen->temperature > 0.f, "`temperature` has to be a strictly positive float, got %f", gen->temperature);
   PTTS_REQUIRE(gen->top_k >= 0, "`top_k` has to be a non-negative integer");
   PTTS_REQUIRE(s->cfg.eos_token_id >= 0 && s->cfg.eos_token_id < s->cfg.vocab_size, "eos_token_id out of vocabulary");
+  PTTS_REQUIRE(n0 < gen->max_length, "generate: %d input columns leave nothing to generate within max_length %d", n0, gen->max_length);
   cudaStream_t st = (cudaStream_t)stream;
   s->gen = *gen;
+  s->gen.input_len = n0;
+  s->n0 = n0;
   PTTS_CHECK_CUDA(cudaMemcpyAsync(s->ws + s->W.gen, &s->gen, sizeof(ptts_gen_params), cudaMemcpyHostToDevice, st));
-  if (int e = launch_generate_begin(sample_args(s), st)) return e;
+  if (int e = launch_generate_begin(sample_args(s), input_ids, n0, gen->max_length, st)) return e;
   s->begun = true;
   s->prefilled = false;
   return PTTS_OK;
 }
 
-// one decoder pass over q_len new positions per batch row (q_len = P+1 at prefill, 1 at decode)
+int ptts_generate_begin(ptts_session* s, const ptts_gen_params* gen, void* stream) {
+  return ptts_generate_begin_ids(s, gen, nullptr, 1, stream);
+}
+
+// one decoder pass over q_len new positions per batch row (q_len = P+n0 at prefill, 1 at decode)
 static int run_forward(ptts_session* s, cudaStream_t st, bool prefill, const void* prompt_hidden, const void* enc_hidden) {
   const ptts_decoder_config& c = s->cfg;
   const DecoderLayout& L = s->L;
   const WorkspaceLayout& W = s->W;
   const int B = W.B, P = W.P, S = W.S, H = L.H, D = PTTS_HEAD_DIM;
-  const int q_len = prefill ? P + 1 : 1;
+  const int q_len = prefill ? P + s->n0 : 1;
   const int M = B * q_len;
   const bool pdl = s->pdl && !prefill;  // the one-off prefill stays on plain stream order
   const Ctrl* ctrl = prefill ? nullptr : (const Ctrl*)(s->ws + W.ctrl);
@@ -353,9 +376,10 @@ static int run_forward(ptts_session* s, cudaStream_t st, bool prefill, const voi
   ea.pos = c.rope ? nullptr : blob + L.pos;
   ea.prefix = prefill ? prompt_hidden : nullptr;
   ea.ids = (const int*)(ws + W.cur_ids);
+  ea.hist = prefill ? (const int64_t*)(ws + W.raw_ids) : nullptr; ea.hist_ld = W.raw_ld;  // prefill: the n0 input columns
   ea.x = ws + W.x;
   ea.ctrl = ctrl;
-  ea.B = B; ea.K = L.K; ea.V1 = L.V + 1; ea.H = H; ea.P = prefill ? P : 0;
+  ea.B = B; ea.K = L.K; ea.V1 = L.V + 1; ea.H = H; ea.P = prefill ? P : 0; ea.n_cols = prefill ? s->n0 : 1;
   ea.pos_from_ctrl = prefill ? 0 : 1; ea.pos0 = 0; ea.prefix_len = P;
   if (int e = launch_embed(ea, c.dtype, st, pdl)) return e;
   s->launches++;
@@ -372,7 +396,7 @@ static int run_forward(ptts_session* s, cudaStream_t st, bool prefill, const voi
     a.epi = epi; a.act = c.activation; a.ctrl = ctrl;
     s->launches++;
     if (prefill && s->prefill_tc && woff >= L.layer0 && woff < L.layer0 + L.layer_stride * L.L && linear_tc_supported(a)) {
-      // the same matrix, row-major (layout.h rm[]): M = B*(P+1) or B*S rows are tensor-core work (wgmma, gemm_tc.cu)
+      // the same matrix, row-major (layout.h rm[]): M = B*(P+n0) or B*S rows are tensor-core work (wgmma, gemm_tc.cu)
       const int64_t in_layer = (woff - L.layer0) % L.layer_stride, lbase = woff - in_layer;
       const int64_t frag[7] = {L.wqkv, L.wo, L.wqc, L.wkvc, L.woc, L.fc1, L.fc2};
       for (int m = 0; m < 7; m++)

@@ -55,10 +55,12 @@ struct EmbedArgs {
   const void* tables;  // [K][V+1][H]
   const void* pos;     // [max_pos][H] or nullptr (rope)
   const void* prefix;  // [B][P][H] prompt hidden states or nullptr
-  const int* ids;      // [B*K] current (delay-masked) input ids
-  void* x;             // [B*(P+1) or B][H]
+  const int* ids;      // [B*K] current (delay-masked) input ids (decode)
+  const int64_t* hist; int64_t hist_ld;  // prefill: [B*K][hist_ld] history whose first n_cols columns are the (delayed) input
+  void* x;             // [B*(P+n_cols) or B][H]
   const Ctrl* ctrl;
   int B, K, V1, H, P;  // P = prefix rows per batch in THIS call (0 at decode)
+  int n_cols;          // code columns per batch row after the prefix (1 at decode)
   int pos_from_ctrl, pos0, prefix_len;  // decode: position = prefix_len + cur_len - 1
 };
 int launch_embed(const EmbedArgs& a, int dtype, cudaStream_t st, bool pdl);
@@ -70,11 +72,13 @@ struct SampleArgs {
   int* cur_ids; int* eos_seen; int* unfinished; int* first_unf;  // first_unf [2][B]
   Ctrl* ctrl;
   const ptts_gen_params* gen;  // device copy
+  int64_t* prefix_cells;       // [B*K][K-1] pattern cells past a multi-column input (nullptr: the session takes the BOS column only)
   int B, K, V;
   int bos, pad, eos;
 };
 int launch_sample(const SampleArgs& a, const int64_t* forced, cudaStream_t st, bool pdl);
-int launch_generate_begin(const SampleArgs& a, cudaStream_t st);
+// ids == nullptr: the BOS column (n0 = 1); otherwise the BOS-led [B*K][n0] input the generation continues from
+int launch_generate_begin(const SampleArgs& a, const int64_t* ids, int n0, int max_length, cudaStream_t st);
 int launch_delay_build(const int64_t* ids, int BK, int seq, int K, int64_t bos, int64_t pad, int L, int64_t* mask, cudaStream_t st);
 int launch_delay_apply(const int64_t* ids, int BK, int seq, int64_t ld_ids, const int64_t* mask, int64_t ld_mask, int64_t* out, cudaStream_t st);
 int launch_logits_processor(const int64_t* ids, int BK, int seq, int64_t ld_ids, float* scores, int V, int64_t eos, int K, int64_t* first_unf, cudaStream_t st);

@@ -142,21 +142,25 @@ static inline bool matrix_slot(const DecoderLayout& l, int tensor_id, int index,
 // ---- workspace ----------------------------------------------------------------------------------
 struct WorkspaceLayout {
   int B, P, S, Tmax, Mmax, BK;
+  int max_input;                   // largest decoder input (BOS column + code prefix) a generate() call may continue from
   int64_t ctrl, progress, gen, raw_ids, cur_ids, eos_seen, unfinished, first_unf, prompt_mask, enc_mask;
+  int64_t prefix_cells;            // [BK][K-1] int64: delay-pattern cells just past the input (max_input > 1 only; -1 = none)
   int64_t x, qkv, attn, qc, hbuf, hidden, logits, scores, cross_tmp, cross_kv, self_kv;
   int64_t img_x, img_attn, img_h;  // fused step kernel: activations as tile images [chunk][32][H + 8] (step.cu stage_tile)
   int64_t cl_x, cl_attn, cl_h;     // cluster step kernel: K-sliced images [2][32][H/2 + 8], fc2's in quarters [4][32][F/4 + 8] (step2.cu)
-  int64_t row_stats;               // [max(B*(P+1), B*S)][2] f32: LayerNorm row statistics of the wgmma prefill GEMMs
+  int64_t row_stats;               // [max(B*(P+max_input), B*S)][2] f32: LayerNorm row statistics of the wgmma prefill GEMMs
   int64_t cross_layer_stride, self_layer_stride;  // bytes
   int64_t raw_ld;                                  // raw_ids leading dimension (elements)
   int64_t total;
 };
 
-static inline WorkspaceLayout make_workspace(const ptts_decoder_config& c, int B, int P, int S, int Tmax) {
+// max_input = 1: the BOS column only; the layout is then the same as before continuation existed (prefix_cells takes no bytes).
+static inline WorkspaceLayout make_workspace(const ptts_decoder_config& c, int B, int P, int S, int Tmax, int max_input = 1) {
   DecoderLayout l = make_layout(c);
   WorkspaceLayout w{};
   w.B = B; w.P = P; w.S = S; w.Tmax = Tmax; w.BK = B * c.num_codebooks;
-  w.Mmax = B * (P + 1);
+  w.max_input = max_input;
+  w.Mmax = B * (P + max_input);
   int64_t o = 0;
   auto take = [&](int64_t bytes) { int64_t r = o; o = align_up(o + bytes, 256); return r; };
   w.ctrl = take(sizeof(Ctrl));
@@ -170,6 +174,8 @@ static inline WorkspaceLayout make_workspace(const ptts_decoder_config& c, int B
   w.first_unf = take((int64_t)2 * B * 4);
   w.prompt_mask = take((int64_t)B * (P > 0 ? P : 1) * 4);
   w.enc_mask = take((int64_t)B * S * 4);
+  w.prefix_cells = -1;
+  if (max_input > 1 && c.num_codebooks > 1) w.prefix_cells = take((int64_t)w.BK * (c.num_codebooks - 1) * 8);
   int64_t rows_enc = (int64_t)B * S;
   w.x = take((int64_t)w.Mmax * l.H * l.es);
   w.qkv = take((int64_t)w.Mmax * l.qkv_rows * l.es);

@@ -62,25 +62,54 @@ int launch_sample(const SampleArgs& a, const int64_t* forced, cudaStream_t st, b
   return PTTS_OK;
 }
 
-__global__ void generate_begin_kernel(SampleArgs p) {
+// build_delay_pattern_mask (modeling_parler_tts.py:214-276), cell c of row `row` (codebook k) for the BOS-led ids [B*K][seq]: the
+// id shifted by k, BOS over the lower triangle, PAD over the upper one (:261); -1 = free (predicted).  No pattern below 2K-1 columns.
+__device__ __forceinline__ int64_t delay_pattern_cell(const int64_t* ids, int row, int seq, int k, int K, int64_t bos, int64_t pad, int L, int c) {
+  if (L < 2 * K - 1) return -1;
+  const bool bos_pat = c <= k;
+  const bool eos_pat = (c - k) >= (L - K + 1);
+  const int64_t shifted = (c >= k && c < seq + k) ? ids[(size_t)row * seq + (c - k)] : -1;
+  return ((!bos_pat && !eos_pat) ? shifted : 0) + (bos_pat ? bos : 0) + (eos_pat ? pad : 0);
+}
+
+// ids == nullptr: the BOS column.  Otherwise the history starts with the delayed input: the first n0 columns of the pattern (:3523;
+// where the pattern is free -- max_length < 2K-1 -- the ids themselves), the K-1 cells after it are kept for the sampler's next-input
+// override, and eos_seen records the first EOS inside the input (ParlerTTSLogitsProcessor counts the whole history, :46).
+__global__ void generate_begin_kernel(SampleArgs p, const int64_t* __restrict__ ids, int n0, int L) {
   const int BK = p.B * p.K;
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i == 0) {
-    p.ctrl->cur_len = 1; p.ctrl->active = 1; p.ctrl->n_unfinished = 0; p.ctrl->done_blocks = 0; p.ctrl->steps_run = 0;
+    p.ctrl->cur_len = n0; p.ctrl->active = 1; p.ctrl->n_unfinished = 0; p.ctrl->done_blocks = 0; p.ctrl->steps_run = 0;
     p.ctrl->launch_gen = 0;
     for (int j = 0; j < 32; j++) p.ctrl->bar[j] = 0;
   }
   if (i < BK) {
-    p.raw_ids[(size_t)i * p.raw_ld] = p.bos;
-    p.cur_ids[i] = p.bos;
-    p.eos_seen[i] = 0;
+    if (ids == nullptr) {
+      p.raw_ids[(size_t)i * p.raw_ld] = p.bos;
+      p.cur_ids[i] = p.bos;
+      p.eos_seen[i] = 0;
+    } else {
+      const int k = i % p.K;
+      int64_t v = 0;
+      int es = 0;
+      for (int c = 0; c < n0; c++) {
+        const int64_t m = delay_pattern_cell(ids, i, n0, k, p.K, p.bos, p.pad, L, c);
+        v = (m == -1) ? ids[(size_t)i * n0 + c] : m;
+        p.raw_ids[(size_t)i * p.raw_ld + c] = v;
+        if (v == p.eos && es == 0) es = c + 1;
+      }
+      p.cur_ids[i] = (int)v;
+      p.eos_seen[i] = es;
+      if (p.prefix_cells != nullptr)
+        for (int c = 0; c < p.K - 1; c++) p.prefix_cells[(size_t)i * (p.K - 1) + c] = delay_pattern_cell(ids, i, n0, k, p.K, p.bos, p.pad, L, n0 + c);
+    }
     p.unfinished[i] = 1;
   }
   if (i < p.B) { p.first_unf[i] = i * p.K; p.first_unf[p.B + i] = i * p.K; }
 }
-int launch_generate_begin(const SampleArgs& a, cudaStream_t st) {
+int launch_generate_begin(const SampleArgs& a, const int64_t* ids, int n0, int max_length, cudaStream_t st) {
   const int n = a.B * a.K;
-  generate_begin_kernel<<<(n + 127) / 128, 128, 0, st>>>(a);
+  generate_begin_kernel<<<(n + 127) / 128, 128, 0, st>>>(a, ids, ids == nullptr ? 1 : n0, max_length);
   PTTS_LAUNCH_CHECK();
   return PTTS_OK;
 }
@@ -90,16 +119,7 @@ int launch_generate_begin(const SampleArgs& a, cudaStream_t st) {
 __global__ void delay_build_kernel(const int64_t* ids, int BK, int seq, int K, int64_t bos, int64_t pad, int L, int64_t* mask) {
   const int row = blockIdx.x;
   const int k = row % K;
-  for (int c = threadIdx.x; c < L; c += blockDim.x) {
-    int64_t out = -1;
-    if (L >= 2 * K - 1) {
-      const bool bos_pat = c <= k;
-      const bool eos_pat = (c - k) >= (L - K + 1);
-      const int64_t shifted = (c >= k && c < seq + k) ? ids[(size_t)row * seq + (c - k)] : -1;
-      out = ((!bos_pat && !eos_pat) ? shifted : 0) + (bos_pat ? bos : 0) + (eos_pat ? pad : 0);
-    }
-    mask[(size_t)row * L + c] = out;
-  }
+  for (int c = threadIdx.x; c < L; c += blockDim.x) mask[(size_t)row * L + c] = delay_pattern_cell(ids, row, seq, k, K, bos, pad, L, c);
 }
 int launch_delay_build(const int64_t* ids, int BK, int seq, int K, int64_t bos, int64_t pad, int L, int64_t* mask, cudaStream_t st) {
   delay_build_kernel<<<BK, 128, 0, st>>>(ids, BK, seq, K, bos, pad, L, mask);

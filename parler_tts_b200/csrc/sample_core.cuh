@@ -126,8 +126,8 @@ __device__ __forceinline__ void sample_rows_cta(const SampleArgs& p, const ptts_
   for (int r = 0; r < R; r++) {
     const int b = row[r] / p.K, k = row[r] - b * p.K;
     bool mask_eos = false;
-    // MinNewTokensLength: prompt_length_to_skip = 1 (the BOS column)
-    if (cur_len - 1 < g.min_new_tokens) mask_eos = true;
+    // MinNewTokensLength: prompt_length_to_skip = the decoder input's columns (the BOS column, or n0 when continuing)
+    if (cur_len - (g.input_len > 1 ? g.input_len : 1) < g.min_new_tokens) mask_eos = true;
     // ParlerTTSLogitsProcessor (stateful; state double-buffered on the column parity)
     if (valid[r]) {
       const int par = cur_len & 1;
@@ -357,6 +357,8 @@ __device__ __forceinline__ void sample_rows_cta(const SampleArgs& p, const ptts_
       const bool is_bos = cur_len <= k;
       const bool is_pad = (cur_len - k) >= (g.max_length - p.K + 1);
       if (is_bos || is_pad) nxt = (is_bos ? p.bos : 0) + (is_pad ? p.pad : 0);
+      // continuing from n0 input columns: codebook k's prefix ids reach up to column n0-1+k, past the delayed input (:246-248)
+      else if (g.input_len > 1 && cur_len - g.input_len < k) nxt = (int)p.prefix_cells[(size_t)my_row * (p.K - 1) + (cur_len - g.input_len)];
     }
     p.cur_ids[my_row] = nxt;
     if (still_unfinished) atomicAdd(&p.ctrl->n_unfinished, 1);

@@ -24,10 +24,20 @@ def shard_row_base(n: int, rank: int, world: int, num_codebooks: int) -> int:
 
 
 def shard_batch(tensors: dict, rank: int, world: int) -> dict:
-    """Slice every [B, ...] tensor of a generate() kwarg dict to this rank's utterances."""
-    B = next(v.shape[0] for v in tensors.values() if isinstance(v, torch.Tensor))
+    """Slice every [B, ...] tensor of a generate() kwarg dict to this rank's utterances.  `decoder_input_ids` ([B * K, N] audio
+    codes) is split by its K-row groups, one group per utterance."""
+    B = next(v.shape[0] for k, v in tensors.items() if isinstance(v, torch.Tensor) and k != "decoder_input_ids")
     lo, hi = shard_range(B, rank, world)
-    return {k: (v[lo:hi] if isinstance(v, torch.Tensor) and v.shape[0] == B else v) for k, v in tensors.items()}
+    out = {}
+    for k, v in tensors.items():
+        if k == "decoder_input_ids" and isinstance(v, torch.Tensor):
+            if v.shape[0] % B != 0:
+                raise ValueError(f"decoder_input_ids has {v.shape[0]} rows, not a multiple of the batch size {B}")
+            K = v.shape[0] // B
+            out[k] = v[lo * K:hi * K]
+        else:
+            out[k] = v[lo:hi] if isinstance(v, torch.Tensor) and v.shape[0] == B else v
+    return out
 
 
 def broadcast_blob(blob: torch.Tensor, src: int = 0, group=None) -> torch.Tensor:

@@ -55,6 +55,39 @@ def apply_delay_pattern_mask(input_ids: torch.LongTensor, decoder_pad_token_mask
     return out.reshape(input_ids.shape)
 
 
+def prepare_decoder_input_ids(decoder_input_ids, batch_size: int, num_codebooks: int, vocab_size: int, decoder_start_token_id: int,
+                              device) -> torch.Tensor:
+    """generate()'s `decoder_input_ids` (audio codes to continue from) -> the BOS-led decoder input [B * K, n0] int64 on `device`.
+
+    Anything `reshape(-1, K, N)` accepts is taken: [B * K, N], [B, K, N] or [1, B, K, N] (generate(return_codes=True)'s audio_codes
+    with its frame dimension).  A BOS column is prepended unless every row already starts with it (:3012-3024).  Ids must lie in
+    [0, vocab_size] (the embedding tables have vocab_size + 1 rows, :1353)."""
+    B, K, V = int(batch_size), int(num_codebooks), int(vocab_size)
+    ids = torch.as_tensor(decoder_input_ids)
+    if ids.is_floating_point() or ids.is_complex() or ids.dtype == torch.bool:
+        raise ValueError(f"decoder_input_ids must hold integer audio codes, got {ids.dtype}")
+    N = ids.shape[-1] if ids.dim() >= 1 else 0
+    if N < 1 or ids.numel() != B * K * N:
+        raise ValueError(f"decoder_input_ids must have batch_size * num_codebooks = {B * K} rows of codes, got shape {tuple(ids.shape)}")
+    ids = ids.reshape(B * K, N).to(device=device, dtype=torch.int64)
+    lo, hi = int(ids.min()), int(ids.max())
+    if lo < 0 or hi > V:
+        raise ValueError(f"decoder_input_ids must lie in [0, vocab_size = {V}], got values in [{lo}, {hi}]")
+    if bool((ids[:, 0] != decoder_start_token_id).all()):
+        ids = torch.cat([torch.full((B * K, 1), int(decoder_start_token_id), dtype=torch.int64, device=ids.device), ids], dim=1)
+    return ids.contiguous()
+
+
+def check_continuation_length(n0: int, prompt_len: int, max_length: int, max_position_embeddings: int):
+    """A continuation from n0 input columns must leave a new column within max_length, and the prompt prefix plus max_length
+    positions must fit the position table."""
+    if n0 >= max_length:
+        raise ValueError(f"decoder_input_ids has {n0} columns (BOS included): max_length {max_length} leaves no new token; "
+                         "raise max_length or pass max_new_tokens")
+    if prompt_len + max_length > max_position_embeddings:
+        raise ValueError(f"{prompt_len} prompt positions + max_length {max_length} exceed max_position_embeddings {max_position_embeddings}")
+
+
 class ParlerTTSLogitsProcessor:
     """Stateful EOS gating across codebooks; HF LogitsProcessor protocol (__call__(input_ids, scores))."""
 
@@ -184,13 +217,14 @@ class DecoderEngine:
             return sd[f"{prefix}lm_heads.weight"][k * V:(k + 1) * V]
         raise ValueError(f"missing weight {prefix}lm_heads.{k}.weight")
 
-    def session(self, B: int, P: int, S: int, max_cache_len: int) -> "GenSession":
+    def session(self, B: int, P: int, S: int, max_cache_len: int, max_input_len: int = 1) -> "GenSession":
+        """max_input_len: the most decoder input columns (BOS column + code prefix) a generate() call on it may continue from."""
         key = (B, P, S)
         s = self._sessions.get(key)
-        if s is None or s.max_cache_len < max_cache_len:
+        if s is None or s.max_cache_len < max_cache_len or s.max_input_len < max_input_len:
             if s is not None:
                 s.close()
-            s = GenSession(self, B, P, S, max_cache_len)
+            s = GenSession(self, B, P, S, max_cache_len, max_input_len)
             self._sessions = {key: s}  # keep one live session (the reference keeps one `_cache`, :3254-3309)
         return s
 
@@ -198,19 +232,22 @@ class DecoderEngine:
 class GenSession:
     """Device-resident generation state for (B, P, S): KV caches, token history, processor state."""
 
-    def __init__(self, eng: DecoderEngine, B: int, P: int, S: int, max_cache_len: int):
+    def __init__(self, eng: DecoderEngine, B: int, P: int, S: int, max_cache_len: int, max_input_len: int = 1):
         self.eng, self.B, self.P, self.S, self.max_cache_len = eng, B, P, S, max_cache_len
+        self.max_input_len = int(max_input_len)
         lib = _lib.lib()
         n = C.c_int64()
-        _lib.check(lib.ptts_workspace_bytes(C.byref(eng.c), B, P, S, max_cache_len, C.byref(n)))
+        _lib.check(lib.ptts_workspace_bytes2(C.byref(eng.c), B, P, S, max_cache_len, self.max_input_len, C.byref(n)))
         self.ws = torch.zeros(n.value, dtype=torch.uint8, device=eng.device)
         h = C.c_void_p()
-        _lib.check(lib.ptts_session_create(C.byref(eng.c), _lib.ptr(eng.blob), _lib.ptr(self.ws), n.value, B, P, S,
-                                           max_cache_len, C.byref(h)))
+        _lib.check(lib.ptts_session_create2(C.byref(eng.c), _lib.ptr(eng.blob), _lib.ptr(self.ws), n.value, B, P, S,
+                                            max_cache_len, self.max_input_len, C.byref(h)))
         self.h = h
         self.K, self.V = eng.cfg.num_codebooks, eng.cfg.vocab_size
         self._keep: list[Any] = []
         self._forced = None
+        self._input_ids = None
+        self.n0 = 1
 
     def close(self):
         if self.h is not None:
@@ -265,13 +302,23 @@ class GenSession:
         return n.value
 
     def begin(self, max_length: int, do_sample=False, temperature=1.0, top_k=0, top_p=1.0, min_new_tokens=0, seed=0,
-              suppress_special=False, codebook_size=1024, row_base=0):
+              suppress_special=False, codebook_size=1024, row_base=0, input_ids: Optional[torch.Tensor] = None):
+        """input_ids: None (the BOS column) or the BOS-led decoder input [B*K, n0] the generation continues from; the history
+        then starts with its delayed form and the first sampled column is n0 (ptts_generate_begin_ids)."""
         g = _lib.GenParamsC()
         g.max_length, g.min_new_tokens, g.do_sample = int(max_length), int(min_new_tokens or 0), int(bool(do_sample))
         g.top_k, g.top_p, g.temperature = int(top_k or 0), float(1.0 if top_p is None else top_p), float(temperature or 1.0)
         g.seed, g.suppress_special, g.codebook_size = int(seed) & (2 ** 64 - 1), int(bool(suppress_special)), int(codebook_size)
         g.row_base = int(row_base)  # global row of this shard's first (utterance, codebook) stream: Philox substream key
-        _lib.check(_lib.lib().ptts_generate_begin(self.h, C.byref(g), _lib.stream_ptr()))
+        if input_ids is None:
+            self._input_ids, self.n0 = None, 1
+            _lib.check(_lib.lib().ptts_generate_begin(self.h, C.byref(g), _lib.stream_ptr()))
+        else:
+            ids = input_ids.to(device=self.eng.device, dtype=torch.int64).contiguous()
+            if ids.dim() != 2 or ids.shape[0] != self.B * self.K:
+                raise ValueError(f"input_ids must be [{self.B * self.K}, n0], got {tuple(ids.shape)}")
+            self._input_ids, self.n0 = ids, int(ids.shape[1])   # kept alive until the asynchronous begin kernel has read it
+            _lib.check(_lib.lib().ptts_generate_begin_ids(self.h, C.byref(g), _lib.ptr(ids), self.n0, _lib.stream_ptr()))
         self.max_length = int(max_length)
 
     def prefill(self, prompt_hidden, prompt_mask, enc_hidden, enc_mask):
@@ -565,7 +612,7 @@ class ParlerTTSForConditionalGeneration:
         return s_out.clone()
 
     # -- generate with user-supplied processors / stopping criteria --------------------------------
-    def _host_driven_loop(self, sess: "GenSession", gc, max_length, user_processors, user_criteria, streamer, seed):
+    def _host_driven_loop(self, sess: "GenSession", gc, max_length, user_processors, user_criteria, streamer, seed, stream_col):
         """One host iteration per token, like GenerationMixin._sample: the decoder step still runs on the fused kernel
         (ptts_decode_forward), the built-in processors run as their device operators (MinNewTokens as a mask,
         ParlerTTSLogitsProcessor = ptts_logits_processor), then the caller's `logits_processor` list, the HF warpers and the draw
@@ -576,11 +623,11 @@ class ParlerTTSForConditionalGeneration:
         parler = ParlerTTSLogitsProcessor(d.eos_token_id, K, sess.B, self.device)
         gen = torch.Generator(device=self.device).manual_seed(int(seed))
         unfinished = torch.ones(BK, dtype=torch.long, device=self.device)
-        cur = 1
+        cur = sess.n0   # the first new column follows the decoder input (the BOS column, or BOS + code prefix)
         while True:
             ids = sess.raw_ids[:, :cur]
             scores = sess.logits.clone()
-            if (gc.min_new_tokens or 0) > 0 and cur - 1 < gc.min_new_tokens:
+            if (gc.min_new_tokens or 0) > 0 and cur - sess.n0 < gc.min_new_tokens:
                 scores[:, d.eos_token_id] = -float("inf")
             scores = parler(ids, scores)
             for proc in user_processors:
@@ -601,9 +648,9 @@ class ParlerTTSForConditionalGeneration:
                 nxt = scores.argmax(-1)
             nxt = nxt * unfinished + d.pad_token_id * (1 - unfinished)
             sess.sample(forced=nxt)           # append (+ delay-pattern override of the next input), device-side stopping state
-            cur += 1
             if streamer is not None:
-                streamer.put(nxt.cpu())
+                streamer.put(stream_col(cur, nxt).cpu())
+            cur += 1
             unfinished = unfinished & ~((nxt == d.eos_token_id) | (cur >= max_length)).long()
             stop = unfinished.max().item() == 0
             for crit in user_criteria:
@@ -624,37 +671,47 @@ class ParlerTTSForConditionalGeneration:
         return 32
 
     def _run_token_loop(self, enc_hidden, attention_mask, prompt_hidden, prompt_mask, *, gc, max_length, seed, suppress_special, row_base,
-                        streamer=None, custom=None):
-        """begin + prefill + the token loop of one session; returns the raw token matrix [B * K, generated length]."""
+                        streamer=None, custom=None, input_ids=None):
+        """begin + prefill + the token loop of one session; returns the raw token matrix [B * K, generated length].
+        input_ids: None, or the BOS-led decoder input [B * K, n0] this shard continues from."""
         d = self.config.decoder
         K = d.num_codebooks
         B, S, _ = enc_hidden.shape
         P = 0 if prompt_hidden is None else prompt_hidden.shape[1]
-        sess = self.decoder.engine.session(B, P, S, P + max_length)
+        n0 = 1 if input_ids is None else int(input_ids.shape[1])
+        sess = self.decoder.engine.session(B, P, S, P + max_length, max_input_len=n0)
         sess.begin(max_length, do_sample=gc.do_sample, temperature=gc.temperature, top_k=gc.top_k if gc.do_sample else 0,
                    top_p=gc.top_p, min_new_tokens=gc.min_new_tokens or 0, seed=seed, suppress_special=suppress_special,
-                   codebook_size=self.config.audio_encoder.codebook_size, row_base=row_base)
+                   codebook_size=self.config.audio_encoder.codebook_size, row_base=row_base, input_ids=input_ids)
+        stream_col = lambda col, v: v
         if streamer is not None:
-            delayed = torch.full((B * K, 1), d.bos_token_id, dtype=torch.int64)
-            streamer.put(delayed)
+            if input_ids is None:
+                streamer.put(torch.full((B * K, 1), d.bos_token_id, dtype=torch.int64))
+            else:
+                streamer.put(sess.raw_ids[:, :n0].cpu())   # the whole delayed input first (:3534)
+                # Codebook k's prefix ids reach K-1 columns past the delayed input; generate()'s result takes them there
+                # (the pattern mask, :3586), so the streamed columns carry them too.
+                _, pm = build_delay_pattern_mask(input_ids, d.bos_token_id, d.pad_token_id, max_length, K)
+                cells = pm[:, n0:n0 + K - 1]
+                stream_col = lambda col, v: (torch.where(cells[:, col - n0] == -1, v, cells[:, col - n0]) if col - n0 < cells.shape[1] else v)
         sess.prefill(prompt_hidden, prompt_mask, enc_hidden, attention_mask)
         if custom is not None:
-            self._host_driven_loop(sess, gc, max_length, custom[0], custom[1], streamer, seed)
+            self._host_driven_loop(sess, gc, max_length, custom[0], custom[1], streamer, seed, stream_col)
         elif streamer is not None:
             sess.sample()
-            steps_left = max_length - 2
+            steps_left = max_length - n0 - 1
             # the streamer contract is one host-visible token column per step (_sample -> streamer.put(next.cpu()))
-            col = 1
-            streamer.put(sess.raw_ids[:, col].cpu())
+            col = n0
+            streamer.put(stream_col(col, sess.raw_ids[:, col]).cpu())
             while steps_left > 0 and int(sess.state[1].item()) == 1:
                 sess.decode_steps(1)
                 col += 1
                 steps_left -= 1
-                streamer.put(sess.raw_ids[:, col].cpu())
+                streamer.put(stream_col(col, sess.raw_ids[:, col]).cpu())
             streamer.end()
         else:
             sess.sample()
-            steps_left = max_length - 2
+            steps_left = max_length - n0 - 1
             # no per-step host sync: enqueue graph replays in chunks and poll the device `active` flag between chunks
             chunk = 64
             while steps_left > 0:
@@ -697,8 +754,9 @@ class ParlerTTSForConditionalGeneration:
             raise ValueError("Got incompatible mode for generation, should be one of greedy or sampling. "
                              "Ensure that beam search is de-activated by setting `num_beams=1` and `num_beam_groups=1`.")
         custom_loop = bool(logits_processor) or bool(stopping_criteria)   # merged with the built-in ones like :3540-3552
-        if mk.get("decoder_input_ids") is not None or mk.get("input_values") is not None:
-            raise ValueError("audio-prompt continuation (decoder_input_ids / input_values) is outside this path")
+        if mk.get("input_values") is not None:
+            raise ValueError("`input_values` (an audio prompt to encode) is not supported on this path: encode the prompt to audio "
+                             "codes and pass them as `decoder_input_ids`")
         input_ids = mk.get("input_ids", inputs)
         attention_mask = mk.get("attention_mask")
         enc = mk.get("encoder_outputs")
@@ -718,15 +776,23 @@ class ParlerTTSForConditionalGeneration:
         prompt_mask = mk.get("prompt_attention_mask") if prompt_hidden is not None else None
         P = 0 if prompt_hidden is None else prompt_hidden.shape[1]
 
-        # generated length (:3458-3469): max_new_tokens wins over max_length; input_ids_length == 1
+        d = self.config.decoder
+        K = d.num_codebooks
+        dec_ids = None
+        if mk.get("decoder_input_ids") is not None:   # -> the BOS-led [B * K, n0] on the device (:3012-3024)
+            start = gc.decoder_start_token_id if gc.decoder_start_token_id is not None else d.bos_token_id
+            dec_ids = prepare_decoder_input_ids(mk["decoder_input_ids"], B, K, d.vocab_size, start, self.device)
+        n0 = 1 if dec_ids is None else dec_ids.shape[1]
+
+        # generated length (:3458-3469): max_new_tokens wins over max_length (both count the n0 input columns)
         if gc.max_new_tokens is not None:
-            max_length = int(gc.max_new_tokens) + 1
+            max_length = int(gc.max_new_tokens) + n0
         else:
             max_length = int(user_max_length if user_max_length is not None else gc.max_length)
         if max_length < 2:
             raise ValueError(f"max_length must allow at least one new token, got {max_length}")
-        d = self.config.decoder
-        K = d.num_codebooks
+        if dec_ids is not None:
+            check_continuation_length(n0, P, max_length, d.max_position_embeddings)
         run = dict(gc=gc, max_length=max_length, seed=seed, suppress_special=suppress_special)
         limit = self._fused_batch_limit()
         if limit is not None and B > limit and not custom_loop and streamer is None:
@@ -738,17 +804,21 @@ class ParlerTTSForConditionalGeneration:
                 sl = slice(b0, min(B, b0 + limit))
                 parts.append(self._run_token_loop(enc_hidden[sl], None if attention_mask is None else attention_mask[sl],
                                                   None if prompt_hidden is None else prompt_hidden[sl],
-                                                  None if prompt_mask is None else prompt_mask[sl], row_base=row_base + b0 * K, **run))
+                                                  None if prompt_mask is None else prompt_mask[sl], row_base=row_base + b0 * K,
+                                                  input_ids=None if dec_ids is None else dec_ids[sl.start * K:sl.stop * K], **run))
             n = max(t.shape[1] for t in parts)
             output_ids = torch.cat([torch.nn.functional.pad(t, (0, n - t.shape[1]), value=d.pad_token_id) for t in parts], dim=0)
         else:
             output_ids = self._run_token_loop(enc_hidden, attention_mask, prompt_hidden, prompt_mask, row_base=row_base, streamer=streamer,
-                                              custom=(logits_processor or [], stopping_criteria or []) if custom_loop else None, **run)
+                                              custom=(logits_processor or [], stopping_criteria or []) if custom_loop else None,
+                                              input_ids=dec_ids, **run)
 
-        # apply the stashed delay mask, then keep only the free cells (:3586-3597)
-        _, full_mask = build_delay_pattern_mask(output_ids[:, :1], d.bos_token_id, d.pad_token_id, max_length, K)
+        # apply the stashed delay mask, then keep only the free cells (:3586-3597); both masks come from the whole decoder input,
+        # so a continuation's codes begin with its prefix frames
+        mask_src = output_ids[:, :1] if dec_ids is None else dec_ids
+        _, full_mask = build_delay_pattern_mask(mask_src, d.bos_token_id, d.pad_token_id, max_length, K)
         output_ids = apply_delay_pattern_mask(output_ids, full_mask)
-        _, mask = build_delay_pattern_mask(output_ids[:, :1], d.bos_token_id, d.pad_token_id, output_ids.shape[1], K)
+        _, mask = build_delay_pattern_mask(mask_src, d.bos_token_id, d.pad_token_id, output_ids.shape[1], K)
         keep = (mask != d.bos_token_id) & (mask != d.pad_token_id)
         codes = output_ids[keep].reshape(B, K, -1)
         audio_codes = codes[None, ...]  # frame dim (:3600)

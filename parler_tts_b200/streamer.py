@@ -1,6 +1,7 @@
 """ParlerTTSStreamer: the reference's streaming contract (parler_tts/streamer.py:11-146) over the CUDA codec path.
 
-Contract kept (what `generate(streamer=...)` and consumer threads rely on): `put(value)` receives the initial [B*K, 1] ids and
+Contract kept (what `generate(streamer=...)` and consumer threads rely on): `put(value)` receives the initial [B*K, n0] ids (the
+BOS column, or the delayed input of a continuation from `decoder_input_ids`) and
 then one [B*K] token column per decode step (CPU tensors, as `_sample` hands them over), `end()` closes the stream, and the
 object is an iterator over numpy audio chunks fed through a queue (a `timeout` guards both sides).
 
@@ -168,7 +169,9 @@ class ParlerTTSStreamer:
         if not self.incremental and value.shape[0] // self.decoder.num_codebooks > 1:
             raise ValueError("ParlerTTSStreamer only supports batch size 1")   # (reference :110-112; incremental=True lifts it)
         self._frames.add(value)
-        if self._frames.n % self.play_steps == 0:
+        if self.incremental and value.dim() == 2 and value.shape[1] > 1:
+            self._flush_incremental(False)   # a continuation's first put holds the whole delayed input: its frames go out first
+        elif self._frames.n % self.play_steps == 0:
             (self._flush_incremental if self.incremental else self._flush_reference)(False)
 
     def end(self):
