@@ -11,8 +11,9 @@
 //     Every GEMM is split 8 ways along K as step.cu splits it over its 8 warps (k32 tile kt -> residue class kt mod 8): rank r
 //     of a cluster stages the k-tiles of classes 4r .. 4r+3 (half of K: 8-33 KB of activations instead of 66 KB) and warp w
 //     reduces class 4 r + (w >> 1) for destination (w & 1).  Every warp owns whole n-tiles (no split-K through shared memory
-//     inside a CTA); the eight partial sums meet through DISTRIBUTED SHARED MEMORY: one cp.async.bulk (shared::cta ->
-//     shared::cluster, mbarrier complete_tx) per peer, and every destination adds them in class order 0..7.
+//     inside a CTA); the eight partial sums meet through DISTRIBUTED SHARED MEMORY: every lane stores its accumulators straight
+//     from registers into the peer's receive slots (st.async, bytes completing on the peer's mbarrier; plain stores into its own
+//     CTA's slots), and every destination adds them in class order 0..7.
 //   * out-proj / cross out-proj / fc1 / fc2: cluster c owns N/(4 nh) output features, rank d finalises half of them
 //     (feature-partitioned exchange).  The residual-stream slice a CTA owns (32 rows x 8 features) never leaves its shared memory.
 //   * QKV and q_cross: clusters 4h .. 4h+3 own HEAD h for batch rows 8j .. 8j+7 (one m16 tile with 8 live rows); the exchange is
@@ -57,21 +58,19 @@ constexpr int OFF_STATS = 256, OFF_PART = 512, OFF_RES = 2560, OFF_CVEC = 3584;
 constexpr int HDR = 5632;       // mbarriers | row stats | stat partials | residual slice | folded-LN vectors c1[256] c2[256]
 constexpr int WB_BYTES = 65536; // one weight ring buffer
 constexpr int R_OFF = HDR + 2 * WB_BYTES;
-// R region: [send blocks | receive slots] over the activation slice, split per phase; attention scratch and the lm-head tile alias it.
-// The send blocks are written once the phase's MMAs have retired, so they start at 0 over the dead activation slice; the receive
-// slots, which peers fill while this CTA may still run its MMAs, start behind both.  Largest plans (H = 1024, F = 4096):
-//   fc1   : 32.5 KB slice, 8 send blocks of (256 B stats + 32 x 34 floats) = 36 KB, receive slots [36 KB, 72 KB)
-//   fc2   : 64.5 KB quarter slice, 8 send blocks of (256 B + 32 x 8 floats), receive slots [64.5 KB, 74.5 KB)
-//   QKV   : 8.1 KB slice, 16 send blocks of (32 B stats + 4 x 96 floats) = 24.5 KB, receive slots [24.5 KB, 49 KB), the first pass's
-//           tiles at R_PASS0 until the exchange, q|k|v at QKV_OFF; the attention scratch of warps 0-4 below QKV_OFF
+// R region: [activation slice | receive slots], split per phase; attention scratch and the lm-head tile alias it.  The receive
+// slots, which peers fill while this CTA may still run its MMAs, start right behind the slice.  Largest plans (H = 1024, F = 4096):
+//   fc1   : 32.5 KB slice, receive slots 8 x (256 B stats + 32 x 34 floats) = 36 KB: [32.5 KB, 68.5 KB)
+//   fc2   : 64.5 KB quarter slice, receive slots 8 x (256 B + 32 x 8 floats): [64.5 KB, 74.5 KB)
+//   QKV   : 8.1 KB slice, receive slots 16 x (32 B stats + 4 x 96 floats) = 24.5 KB: [8.1 KB, 32.6 KB), q|k|v at QKV_OFF; the
+//           attention scratch of warps 0-4 below QKV_OFF
 //   lm heads: the whole x image (65 KB)
 constexpr int R_BYTES = 92160;
-constexpr int R_PASS0 = 65536;            // [8 warps][6 n-tiles][32 lanes] float4: the head phases' first-pass tiles
 constexpr int QKV_OFF = R_BYTES - 2048;   // [4 rows][192] bf16 q|k|v (or [4][64] q_cross) of this rank's attention items
 constexpr int SMEM_BYTES = R_OFF + R_BYTES;
 static_assert(SMEM_BYTES + 1024 <= 227 * 1024, "cluster step kernel shared memory");
-static_assert(ROWS * (1024 / 2 + 8) * 2 <= V * (256 + ROWS * 34 * 4) && 2 * V * (256 + ROWS * 34 * 4) <= R_BYTES, "fc1 plan");
-static_assert(2 * V * C * (32 + 4 * 96 * 4) <= R_PASS0 && R_PASS0 + V * QMAX * 32 * 16 <= QKV_OFF, "QKV plan");
+static_assert(ROWS * (1024 / 2 + 8) * 2 + V * (256 + ROWS * 34 * 4) <= R_BYTES, "fc1 plan");
+static_assert(HROWS * (1024 / 2 + 8) * 2 + V * C * (32 + 4 * 96 * 4) <= QKV_OFF, "QKV plan");
 static_assert(5 * ATT_SMEM <= QKV_OFF && 3 * ATT_SMEM <= WB_BYTES && 16384 + 4 * 128 * 4 <= WB_BYTES, "attention plan");
 static_assert(ROWS * (4096 / 4 + 8) * 2 + V * (256 + ROWS * 8 * 4) <= R_BYTES, "fc2 plan");
 
@@ -83,17 +82,25 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity, int wh
     if (!ok && ++spins > (1u << 22)) { printf("ptts: cluster step mbarrier timeout (cta %d, barrier kind %d)\n", (int)blockIdx.x, what); __trap(); }
   } while (!ok);
 }
-// this CTA's shared memory -> a peer's shared memory (DSMEM), completion counted on the PEER's mbarrier
-__device__ __forceinline__ void bulk_s2peer(uint32_t dst_cluster_addr, const void* src_smem, uint32_t bytes, uint32_t bar_cluster_addr) {
-  asm volatile("cp.async.bulk.shared::cluster.shared::cta.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-               ::"r"(dst_cluster_addr), "r"(smem_u32(src_smem)), "r"(bytes), "r"(bar_cluster_addr) : "memory");
+// registers -> a peer's shared memory (DSMEM): a remote store whose bytes complete on the peer's mbarrier, with no release and no
+// acknowledgement round trip.  Both addresses are the peer's (mapa); the PTX ISA leaves st.async to the executing CTA undefined.
+// It is a weak store of the memory model, so the receive slots count as written through the generic proxy: every TMA write over
+// them later (the next activation slice, the attention's K/V stages) follows a fence.proxy.async on its issuing thread, after that
+// thread's exchange wait (request_slice at each device-wide barrier; the attention before its first K/V stage).
+__device__ __forceinline__ void st_async(uint32_t dst_cluster_addr, float v, uint32_t bar_cluster_addr) {
+  asm volatile("st.async.shared::cluster.mbarrier::complete_tx::bytes.b32 [%0], %1, [%2];"
+               ::"r"(dst_cluster_addr), "r"(__float_as_uint(v)), "r"(bar_cluster_addr) : "memory");
+}
+__device__ __forceinline__ void st_async(uint32_t dst_cluster_addr, float2 v, uint32_t bar_cluster_addr) {
+  asm volatile("st.async.shared::cluster.mbarrier::complete_tx::bytes.v2.f32 [%0], {%1, %2}, [%3];"
+               ::"r"(dst_cluster_addr), "f"(v.x), "f"(v.y), "r"(bar_cluster_addr) : "memory");
 }
 __device__ __forceinline__ uint32_t mapa(uint32_t addr, uint32_t rank) { uint32_t r; asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(rank)); return r; }
 __device__ __forceinline__ uint32_t cluster_rank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
 __device__ __forceinline__ void cluster_arrive() { asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory"); }
 __device__ __forceinline__ void cluster_wait() { asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory"); }
-// The per-phase cluster barrier only guards buffer REUSE (a peer may overwrite my receive slots / I may overwrite a send block once
-// everyone has consumed the previous phase's); the data itself is ordered by the exchange mbarrier.  A write-after-read needs no
+// The per-phase cluster barrier only guards buffer REUSE (a peer may overwrite my receive slots once I have consumed the previous
+// phase's); the data itself is ordered by the exchange mbarrier.  A write-after-read needs no
 // release: the default .release arrive is a gpu-scope MEMBAR per warp (it waits for the epilogue's global stores to be acknowledged,
 // a second time before the layer barrier does).
 __device__ __forceinline__ void cluster_arrive_reuse() { asm volatile("barrier.cluster.arrive.relaxed.aligned;" ::: "memory"); }
@@ -186,7 +193,7 @@ __global__ void __launch_bounds__(THREADS, 1) decode_step_cluster_kernel(const _
   int pos = p.P + cur_len - 1;  // cache position of the token being fed
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int H = p.H, F = p.F, B = p.B;
-  const int rank = (int)cluster_rank();
+  const int rank = (int)cluster_rank(), peer = rank ^ 1;
   const int cta = (int)blockIdx.x;         // = cluster * 2 + rank
   const int cluster = cta >> 1;
   const int head = cluster >> 2, rblk = cluster & 3;   // head phases: this cluster's head and its batch-row block (rows 8 rblk ..)
@@ -204,6 +211,7 @@ __global__ void __launch_bounds__(THREADS, 1) decode_step_cluster_kernel(const _
   float* res_s = reinterpret_cast<float*>(smem + OFF_RES);     // [32][8] residual stream slice owned by this CTA
   float* cvec = reinterpret_cast<float*>(smem + OFF_CVEC);     // c1[256] | c2[256] of the current phase's features
   unsigned char* Rg = smem + R_OFF;
+  const uint32_t peer_xbar = mapa(smem_u32(xbar), (uint32_t)peer);
   uint32_t par_a = 0, par_w = 0, par_x = 0, att_parity = 0;
 
   if (tid == 0) {
@@ -309,12 +317,25 @@ __global__ void __launch_bounds__(THREADS, 1) decode_step_cluster_kernel(const _
     const int KT = (sub == PH_FC2 ? KsF : Ks) >> 5;                  // k32 tiles of a staged slice (fc2: of one quarter of F)
     const int apitch = (sub == PH_FC2) ? pitchF : pitch;
     const int act_bytes = (rowpart ? HROWS : ROWS) * apitch * 2;
-    // exchange geometry.  feature-partitioned: one block per warp, landing in slot (K class) at its destination;
-    // row-partitioned: one block per (warp, destination) with the warp's columns of both passes, slot 8 rank + warp
+    // exchange geometry (receive slots right behind the activation slice).  feature-partitioned: one block per warp, landing in
+    // slot (K class) at its destination; row-partitioned: one block per (warp, destination) with the warp's columns of both
+    // passes, slot 8 rank + warp
     const int RS = (q == 1) ? 8 : 8 * q + 2;                         // floats per row of a feature-partitioned block
     const int blk = rowpart ? 32 + 4 * 16 * q * 4 : 256 + ROWS * RS * 4;   // one exchanged block: [statistics][rows][columns]
-    const int wsend = rowpart ? C * blk : blk;                       // bytes a warp stages
+    unsigned char* const recv = Rg + ((act_bytes + 127) & ~127);
+    const uint32_t peer_recv = mapa(smem_u32(recv), (uint32_t)peer);
+    // bytes the PEER stores into this CTA's slots (its own slots take plain stores); row padding and unread statistics are not sent:
+    //   feature-partitioned: V / C slots x (32 rows x 8 q columns, + 32 rows x (S1, S2) with a LayerNorm) x 4 B
+    //   row-partitioned    : V slots x 4 rows x 16 q columns + the V / 2 dgrp == 0 warps' 4 rows x (S1, S2), x 4 B
+    const uint32_t xbytes = 4u * (rowpart ? V * 4 * 16 * q + V / 2 * 4 * 2 : V / C * (ROWS * 8 * q + (has_ln ? ROWS * 2 : 0)));
+    // one value (pair) of this CTA's partial sums -> byte `off` of destination d's receive slots: st.async into the peer, a plain
+    // store into this CTA's own slots (published to the epilogue by the CTA barrier in front of the exchange wait)
+    auto put = [&](int d, uint32_t off, auto v) {
+      if (d == rank) *reinterpret_cast<decltype(v)*>(recv + off) = v;
+      else st_async(peer_recv + off, v, peer_xbar);
+    };
     const int j0 = JOBS_PER_LAYER * l + (sub == 0 ? 0 : sub + QKV_JOBS - 1);   // first weight job of this phase
+    if (tid == 0) mbar_expect_tx(xbar, xbytes);
 
     // folded-LayerNorm vectors of this phase's features: requested now, parked in shared memory after the MMA loop (a global
     // load followed at once by its shared-memory store would park the warp for an L2 round trip in front of the MMAs)
@@ -347,30 +368,35 @@ __global__ void __launch_bounds__(THREADS, 1) decode_step_cluster_kernel(const _
     par_a ^= 1u;
     prof_mark(prof, 1);
     float acc[2][QMAX][4];
-    float4* const pass0 = reinterpret_cast<float4*>(Rg + R_PASS0) + (size_t)warp * QMAX * 32 + lane;   // head phases: [warp][n-tile][lane]
     RowStatFrag rst;
     row_stat_zero(rst);
     {
       const bf16* xs = reinterpret_cast<const bf16*>(Rg);
       if (rowpart) {
         // 8 live rows: the ldmatrix rows 8-15 repeat rows 0-7 (what they produce is never read).  Pass P: warp group dgrp takes
-        // unit u = 2 P + dgrp of the head's n-tiles (QKV: weight job j0 + u; q_cross: n-tiles 2 u, 2 u + 1 of job j0).  Pass 0's
-        // tiles wait in shared memory (the attention scratch, idle until the exchange), pass 1's in acc[0].
+        // unit u = 2 P + dgrp of the head's n-tiles (QKV: weight job j0 + u; q_cross: n-tiles 2 u, 2 u + 1 of job j0).  Each pass's
+        // tiles go to their destinations as soon as its MMAs retire, pass 0's with the LayerNorm statistics (complete after it):
+        // live row g (fragment elements 0, 1) -> rank g >> 2, row g & 3 of slot 8 rank + warp: [stats 4 x 2][4 rows][16 q]
         auto head_pass = [&](auto pass_tag) {
           constexpr int P = decltype(pass_tag)::value;
           const int u = 2 * P + dgrp;
           float t[2][QMAX][4];
           if (sub == PH_QKV) mma_slice<6, 1, P == 0>(t, rst, xs, apitch, ring(j0 + u), KT, e4, KT, lrow & 7, lcol);
           else mma_slice<2, 1, P == 0>(t, rst, xs, apitch, ring(j0) + (size_t)(2 * u) * KT * 32, KT, e4, KT, lrow & 7, lcol);
+          const int d = g >> 2;
+          const uint32_t slot = (uint32_t)((8 * rank + warp) * blk);
+          if (P == 0) {
+            // the peer is past its previous epilogue (it arrived before the device-wide barrier opened): its slots are free
+            cluster_wait();
+            if (dgrp == 0) {   // the epilogue reads each K class's statistics from its dgrp == 0 warp
+              const uint32_t so = slot + 8 * (g & 3);
+              if (t4 == 0) put(d, so, rst.s1[0][0]);
+              if (t4 == (g >> 1)) put(d, so + 4, (g & 1) ? rst.sq[0][0][1] : rst.sq[0][0][0]);
+            }
+          }
 #pragma unroll
           for (int j = 0; j < QMAX; j++)
-            if (j < q) {
-              if (P == 0) pass0[j * 32] = make_float4(t[0][j][0], t[0][j][1], t[0][j][2], t[0][j][3]);
-              else {
-#pragma unroll
-                for (int e = 0; e < 4; e++) acc[0][j][e] = t[0][j][e];
-              }
-            }
+            if (j < q) put(d, slot + 32 + 4 * ((g & 3) * 16 * q + P * 8 * q + j * 8 + 2 * t4), make_float2(t[0][j][0], t[0][j][1]));
         };
         head_pass(std::integral_constant<int, 0>{});
         if (sub == PH_QKV) {   // quarters 2 and 3 of the head's QKV slice take the ring buffers of quarters 0 and 1
@@ -408,81 +434,41 @@ __global__ void __launch_bounds__(THREADS, 1) decode_step_cluster_kernel(const _
       }
     }
     prof_mark(prof, 2);
-    if (has_ln && tid < (rowpart ? Nc : 8 * q)) { cvec[tid] = cv1; cvec[256 + tid] = cv2; }   // read in the epilogue, several barriers later
-    __syncthreads();  // activation slice and weight buffer(s) are dead
-    prof_mark(prof, 12);
-    cluster_wait();  // every peer is past its previous epilogue: my send blocks have been read, its receive slots are free
-    prof_mark(prof, 13);
-
-    // ---- exchange: each warp stages its partial block in shared memory and ships it with ONE cp.async.bulk per destination
-    // (shared::cta -> shared::cluster, complete_tx on the destination's mbarrier); no CTA-wide synchronisation on the way ----
+    // ---- exchange: every warp stores its partial block straight into its destination's receive slot, with no CTA-wide
+    // synchronisation on the way (the head phases did so inside their passes).  Profile stamps: 12 -> 13 cluster wait, 13 -> 14
+    // the stores, 14 -> 15 CTA barrier + weight refill, 15 -> 3 the wait for the peer's bytes ----
     //   feature-partitioned: warp (e4, dgrp) -> rank dgrp, slot 4 rank + e4: [stats 32 x 2][32 rows][RS]
     //   row-partitioned    : warp w -> every rank d, slot 8 rank + w:        [stats 4 x 2][4 rows][16 q]  (rows 4d..4d+3, the warp's columns)
-    // The send blocks start at the head of R (over the dead activation slice), the receive slots behind both the send blocks and the
-    // activation slice.
-    const int nslots = rowpart ? V * C : V;
-    unsigned char* send = Rg;
-    const int send_end = V * wsend;
-    unsigned char* recv = Rg + (((send_end > act_bytes ? send_end : act_bytes) + 127) & ~127);
-    if (tid == 0) mbar_expect_tx(xbar, (uint32_t)(nslots * blk));
-    {
-      unsigned char* mine = send + (size_t)warp * wsend;
-      if (!rowpart) {
-        float* bp = reinterpret_cast<float*>(mine + 256);
+    prof_mark(prof, 12);
+    if (!rowpart) cluster_wait();  // the peer is past its previous epilogue: its receive slots are free
+    prof_mark(prof, 13);
+    if (!rowpart) {
+      const uint32_t slot = (uint32_t)((4 * rank + e4) * blk);
 #pragma unroll
-        for (int mt = 0; mt < 2; mt++)
+      for (int mt = 0; mt < 2; mt++)
 #pragma unroll
-          for (int j = 0; j < QMAX; j++) {
-            if (j < q) {
-              float* base = bp + (size_t)(mt * 16 + g) * RS + j * 8 + 2 * t4;
-              *reinterpret_cast<float2*>(base) = make_float2(acc[mt][j][0], acc[mt][j][1]);
-              *reinterpret_cast<float2*>(base + 8 * RS) = make_float2(acc[mt][j][2], acc[mt][j][3]);
-            }
-          }
-        if (has_ln) {   // (S1, S2) of rows g / g+8 of each m-tile over this warp's K class (lane layout: ln_stats.cuh)
-          float* st = reinterpret_cast<float*>(mine);
-#pragma unroll
-          for (int mt = 0; mt < 2; mt++) {
-            const int r0 = mt * 16 + g;
-            if (t4 == 0) { st[2 * r0] = rst.s1[mt][0]; st[2 * (r0 + 8)] = rst.s1[mt][2]; }
-            if (t4 == (g >> 1)) {
-              st[2 * r0 + 1] = (g & 1) ? rst.sq[mt][0][1] : rst.sq[mt][0][0];
-              st[2 * (r0 + 8) + 1] = (g & 1) ? rst.sq[mt][1][3] : rst.sq[mt][1][2];
-            }
+        for (int j = 0; j < QMAX; j++) {
+          if (j < q) {
+            const uint32_t o = slot + 256 + 4 * ((mt * 16 + g) * RS + j * 8 + 2 * t4);
+            put(dgrp, o, make_float2(acc[mt][j][0], acc[mt][j][1]));
+            put(dgrp, o + 4 * 8 * RS, make_float2(acc[mt][j][2], acc[mt][j][3]));
           }
         }
-      } else {
-        const int qc = 16 * q;   // this warp's columns: pass 0, then pass 1
-        // live row g (fragment elements 0, 1) -> destination rank g >> 2, row g & 3 of its block.  [destination][warp] order, so
-        // that ONE copy per destination ships all eight warps' blocks (every bulk copy costs issue time through the uniform datapath,
-        // on every warp's critical path)
-        unsigned char* blk_d = send + ((size_t)(g >> 2) * V + warp) * blk;
-        float* bp = reinterpret_cast<float*>(blk_d + 32) + (g & 3) * qc + 2 * t4;
+      if (has_ln) {   // (S1, S2) of rows g / g+8 of each m-tile over this warp's K class (lane layout: ln_stats.cuh)
 #pragma unroll
-        for (int P = 0; P < 2; P++)
-#pragma unroll
-          for (int j = 0; j < QMAX; j++)
-            if (j < q) *reinterpret_cast<float2*>(bp + P * 8 * q + j * 8) = P == 0 ? make_float2(pass0[j * 32].x, pass0[j * 32].y)
-                                                                                   : make_float2(acc[0][j][0], acc[0][j][1]);
-        float* st = reinterpret_cast<float*>(blk_d) + (g & 3) * 2;
-        if (t4 == 0) st[0] = rst.s1[0][0];
-        if (t4 == (g >> 1)) st[1] = (g & 1) ? rst.sq[0][0][1] : rst.sq[0][0][0];
-      }
-      __syncwarp();
-      prof_mark(prof, 14);
-      if (!rowpart) {
-        if (lane == 0) {
-          fence_proxy_async_smem();
-          bulk_s2peer(mapa(smem_u32(recv + (size_t)(4 * rank + e4) * blk), (uint32_t)dgrp), mine, (uint32_t)blk, mapa(smem_u32(xbar), (uint32_t)dgrp));
-        }
-      } else {
-        __syncthreads();   // all eight warps' blocks are staged
-        if (warp < C && lane == 0) {   // warp d ships [d][0..7] to rank d: it lands as slots 8 rank .. 8 rank + 7 there
-          fence_proxy_async_smem();
-          bulk_s2peer(mapa(smem_u32(recv + (size_t)(8 * rank) * blk), (uint32_t)warp), send + (size_t)warp * V * blk, (uint32_t)(V * blk), mapa(smem_u32(xbar), (uint32_t)warp));
+        for (int mt = 0; mt < 2; mt++) {
+          const uint32_t s0 = slot + 8 * (mt * 16 + g), s8 = s0 + 8 * 8;
+          if (t4 == 0) { put(dgrp, s0, rst.s1[mt][0]); put(dgrp, s8, rst.s1[mt][2]); }
+          if (t4 == (g >> 1)) {
+            put(dgrp, s0 + 4, (g & 1) ? rst.sq[mt][0][1] : rst.sq[mt][0][0]);
+            put(dgrp, s8 + 4, (g & 1) ? rst.sq[mt][1][3] : rst.sq[mt][1][2]);
+          }
         }
       }
     }
+    prof_mark(prof, 14);
+    if (has_ln && tid < (rowpart ? Nc : 8 * q)) { cvec[tid] = cv1; cvec[256 + tid] = cv2; }   // read in the epilogue, several barriers later
+    __syncthreads();  // activation slice and weight buffer(s) are dead; this CTA's stores into its own receive slots are visible
     // The weight ring's refill goes out now, while the partial sums travel (two jobs ahead).  The head phases hold the next head
     // phase's or fc1's weights back until their attention is done (the attention uses that buffer meanwhile), and cross out-proj
     // holds fc2's back: those three go out when the barrier opens (below).
@@ -566,11 +552,6 @@ __global__ void __launch_bounds__(THREADS, 1) decode_step_cluster_kernel(const _
     prof_mark(prof, 4);
     __syncthreads();   // this CTA's receive slots are consumed (and q|k|v complete): peers may send the next phase's partials
     cluster_arrive_reuse();
-    if (rowpart) {
-      // the attention's scratch aliases the send blocks: the peers must have RECEIVED them (each is past its exchange wait) first
-      cluster_wait();
-      cluster_arrive();  // re-arm for the next phase's "exchange buffers free" wait
-    }
 
     // ---- attention of this rank's 4 (row, head) items: two warps per item, the sweep and the call step.cu's attention phase
     // makes (same key chunks, same split over the two warps, same merge), so the two step kernels agree bit for bit ----
