@@ -199,10 +199,17 @@ int ptts_delay_apply(const int64_t* input_ids, int32_t BK, int32_t seq_len, int6
 int ptts_logits_processor(const int64_t* input_ids, int32_t BK, int32_t seq_len, int64_t ld_ids,
                           float* scores, int32_t V, int64_t eos, int32_t num_codebooks,
                           int64_t* first_unfinished, void* stream);
-/* y[M,N] = epi(LN?(x[M,K]) @ W^T): W taken from a packed blob slot. Test hook for the GEMM kernels. */
+/* y[M,N] = epi(LN?(x[M,K]) @ W^T): W taken from a packed blob slot (the whole fused matrix it belongs to).  Test hook for the
+ * GEMM kernels.  path 0: the decode GEMM (launch_linear, every dtype); path 1: the wgmma prefill GEMM (launch_linear_tc) over
+ * the matrix's row-major copy, with the same eligibility rule and the same blob lookup as the prefill -- PTTS_EINVAL when it
+ * does not apply (f32, M < 128, the f32 epilogue, or a matrix without a row-major copy such as the lm heads).
+ * row_stats: float[2*M] scratch for path 1 with use_ln (may be NULL otherwise).  residual may equal y (in place). */
+int ptts_op_linear2(const ptts_decoder_config* cfg, const void* blob, int32_t tensor_id, int32_t index,
+                    const void* x, int32_t M, int32_t use_ln, int32_t epilogue /*0 store,1 act,2 +res,3 f32*/,
+                    const void* residual, void* y, int32_t path, float* row_stats, void* stream);
+/* ptts_op_linear2 with path 0 (the decode GEMM): the original signature, kept for existing callers. */
 int ptts_op_linear(const ptts_decoder_config* cfg, const void* blob, int32_t tensor_id, int32_t index,
-                   const void* x, int32_t M, int32_t use_ln, int32_t epilogue /*0 store,1 act,2 +res,3 f32*/,
-                   const void* residual, void* y, void* stream);
+                   const void* x, int32_t M, int32_t use_ln, int32_t epilogue, const void* residual, void* y, void* stream);
 /* Self- or cross-attention of q_len new positions per batch row (ParlerTTSSdpaAttention after the projections, :858-914), with
  * the kernels the decoder launches.  Test hook for the attention sweeps.
  *   dtype PTTS_BF16 / PTTS_F32; nh query heads, nkv K/V heads (nh % nkv == 0); head_dim 64; scale 1/8.

@@ -357,6 +357,17 @@ int ptts_generate_begin(ptts_session* s, const ptts_gen_params* gen, void* strea
   return ptts_generate_begin_ids(s, gen, nullptr, 1, stream);
 }
 
+// Blob offset of the row-major copy (layout.h rm[]) of the layer matrix stored at blob offset woff, which the wgmma GEMM
+// (gemm_tc.cu) reads; -1 when there is none (f32 model dtype, or not a layer matrix: the lm heads).
+static int64_t rowmajor_offset(const DecoderLayout& L, int64_t woff) {
+  if (L.es != 2 || woff < L.layer0 || woff >= L.layer0 + L.layer_stride * L.L) return -1;
+  const int64_t in_layer = (woff - L.layer0) % L.layer_stride, lbase = woff - in_layer;
+  const int64_t frag[7] = {L.wqkv, L.wo, L.wqc, L.wkvc, L.woc, L.fc1, L.fc2};
+  for (int m = 0; m < 7; m++)
+    if (in_layer == frag[m]) return lbase + L.rm[m];
+  return -1;
+}
+
 // one decoder pass over q_len new positions per batch row (q_len = P+n0 at prefill, 1 at decode)
 static int run_forward(ptts_session* s, cudaStream_t st, bool prefill, const void* prompt_hidden, const void* enc_hidden) {
   const ptts_decoder_config& c = s->cfg;
@@ -395,15 +406,11 @@ static int run_forward(ptts_session* s, cudaStream_t st, bool prefill, const voi
     a.M = Mrows; a.N = N; a.K = K; a.Kc = (K > H && K % H == 0) ? H : K;
     a.epi = epi; a.act = c.activation; a.ctrl = ctrl;
     s->launches++;
-    if (prefill && s->prefill_tc && woff >= L.layer0 && woff < L.layer0 + L.layer_stride * L.L && linear_tc_supported(a)) {
-      // the same matrix, row-major (layout.h rm[]): M = B*(P+n0) or B*S rows are tensor-core work (wgmma, gemm_tc.cu)
-      const int64_t in_layer = (woff - L.layer0) % L.layer_stride, lbase = woff - in_layer;
-      const int64_t frag[7] = {L.wqkv, L.wo, L.wqc, L.wkvc, L.woc, L.fc1, L.fc2};
-      for (int m = 0; m < 7; m++)
-        if (in_layer == frag[m]) {
-          if (a.c1 != nullptr) s->launches++;  // row statistics kernel
-          return launch_linear_tc(a, blob + lbase + L.rm[m], (float*)(ws + W.row_stats), st);
-        }
+    // the same matrix, row-major: M = B*(P+n0) or B*S rows are tensor-core work (wgmma, gemm_tc.cu)
+    const int64_t rm = (prefill && s->prefill_tc) ? rowmajor_offset(L, woff) : -1;
+    if (rm >= 0 && linear_tc_supported(a)) {
+      if (a.c1 != nullptr) s->launches++;  // row statistics kernel
+      return launch_linear_tc(a, blob + rm, (float*)(ws + W.row_stats), st);
     }
     return launch_linear(a, c.dtype, st, pdl, s->sm_count);
   };
@@ -590,9 +597,11 @@ int ptts_logits_processor(const int64_t* input_ids, int32_t BK, int32_t seq_len,
   return launch_logits_processor(input_ids, BK, seq_len, ld_ids, scores, V, eos, num_codebooks, first_unfinished, (cudaStream_t)stream);
 }
 
-int ptts_op_linear(const ptts_decoder_config* cfg, const void* blob, int32_t tensor_id, int32_t index, const void* x, int32_t M,
-                   int32_t use_ln, int32_t epilogue, const void* residual, void* y, void* stream) {
+int ptts_op_linear2(const ptts_decoder_config* cfg, const void* blob, int32_t tensor_id, int32_t index, const void* x, int32_t M,
+                    int32_t use_ln, int32_t epilogue, const void* residual, void* y, int32_t path, float* row_stats, void* stream) {
   PTTS_REQUIRE(cfg && blob && x && y, "null argument");
+  PTTS_REQUIRE(path == 0 || path == 1, "op_linear: path is 0 (decode GEMM) or 1 (wgmma prefill GEMM), got %d", path);
+  PTTS_REQUIRE(M > 0, "op_linear: M must be positive, got %d", M);
   if (int e = validate_config(*cfg)) return e;
   const DecoderLayout L = make_layout(*cfg);
   MatSlot ms;
@@ -629,10 +638,23 @@ int ptts_op_linear(const ptts_decoder_config* cfg, const void* blob, int32_t ten
   a.epi = epilogue; a.act = cfg->activation; a.ctrl = nullptr;
   PTTS_REQUIRE(epilogue >= 0 && epilogue <= 3, "op_linear: bad epilogue");
   PTTS_REQUIRE(epilogue != EPI_RESIDUAL || residual, "op_linear: residual required");
+  if (path == 1) {  // the prefill's rule: bf16, linear_tc_supported, a row-major copy
+    PTTS_REQUIRE(cfg->dtype == PTTS_BF16 && linear_tc_supported(a), "op_linear: the wgmma GEMM does not take this problem (dtype %d, M %d, N %d, K %d, epilogue %d)",
+                 cfg->dtype, M, ms.N, ms.K, epilogue);
+    const int64_t rm = rowmajor_offset(L, ms.off);
+    PTTS_REQUIRE(rm >= 0, "op_linear: tensor %d has no row-major copy for the wgmma GEMM", tensor_id);
+    PTTS_REQUIRE(a.c1 == nullptr || row_stats, "op_linear: row_stats scratch required with LayerNorm");
+    return launch_linear_tc(a, (const char*)blob + rm, row_stats, (cudaStream_t)stream);
+  }
   int sm = 132, dev = 0;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sm, cudaDevAttrMultiProcessorCount, dev);
   return launch_linear(a, cfg->dtype, (cudaStream_t)stream, false, sm);
+}
+
+int ptts_op_linear(const ptts_decoder_config* cfg, const void* blob, int32_t tensor_id, int32_t index, const void* x, int32_t M,
+                   int32_t use_ln, int32_t epilogue, const void* residual, void* y, void* stream) {
+  return ptts_op_linear2(cfg, blob, tensor_id, index, x, M, use_ln, epilogue, residual, y, 0, nullptr, stream);
 }
 
 int ptts_op_attention(int32_t dtype, int32_t B, int32_t nh, int32_t nkv, int32_t q_len, int32_t past_len, int32_t cross,

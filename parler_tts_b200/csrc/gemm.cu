@@ -279,7 +279,7 @@ int launch_linear(const LinearArgs& a_in, int dtype, cudaStream_t st, bool pdl, 
   }
   PTTS_REQUIRE(a.Kc <= 2048 && a.K % a.Kc == 0 && a.Kc % 32 == 0, "linear: bad K tile %d for K=%d", a.Kc, a.K);
   // n-tiles per CTA: the largest tile that still gives ~one CTA per SM (132 on an H100) for this matrix; fewer,
-  // fatter CTAs mean fewer copies of the 32-row activation tile pulled through the L2->SM crossbar.
+  // fatter CTAs mean fewer copies of the 32-row activation tile pulled through the L2->SM crossbar.  (Restated by ntile_pick in tests/test_linear_reference.py, which asserts the decode shapes reach every variant: keep the two in step.)
   const int ntiles = a.N / 8;
   const int cand[6] = {8, 6, 4, 3, 2, 1};
   const int want = ntiles < (sm_count * 85) / 100 ? ntiles : (sm_count * 85) / 100;

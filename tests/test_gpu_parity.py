@@ -59,56 +59,6 @@ def test_logits_processor_rejects_bad_eos():
         ParlerTTSLogitsProcessor(-1, 4, 2, DEV)
 
 
-# ---- linear kernels ------------------------------------------------------------------------------
-@pytest.mark.parametrize("dtype", [torch.float32, torch.bfloat16])
-@pytest.mark.parametrize("M", [1, 7, 32, 45])
-def test_linear_kernel(dtype, M):
-    """LN-fused and plain GEMM vs torch on the CPU in the same dtype (fp32 accumulate, one rounding)."""
-    import ctypes as C
-    from parler_tts_b200 import _lib
-    from parler_tts_b200.modeling import DecoderEngine
-    cfg = tiny_cfg(hidden_size=256, num_attention_heads=4, ffn_dim=1024)
-    w = make_decoder_weights(cfg, seed=5, std=0.05)
-    eng = DecoderEngine(product_decoder_config(cfg), DEV, dtype).load_state_dict(w)
-    g = torch.Generator().manual_seed(M)
-    x = torch.randn(M, cfg.hidden_size, generator=g).to(dtype)
-    h = torch.randn(M, cfg.ffn_dim, generator=g).to(dtype)
-    res = torch.randn(M, cfg.hidden_size, generator=g).to(dtype)
-    p = "decoder.model.decoder.layers.1."
-    wd = {k: v.to(dtype) for k, v in w.items()}
-    F = torch.nn.functional
-
-    def run(tid, idx, xin, use_ln, epi, residual, N):
-        y = torch.empty(M, N, dtype=(torch.float32 if epi == 3 else dtype), device=DEV)
-        xd = xin.to(DEV).contiguous()
-        rd = None if residual is None else residual.to(DEV).contiguous()
-        _lib.check(_lib.lib().ptts_op_linear(C.byref(eng.c), _lib.ptr(eng.blob), tid, idx, _lib.ptr(xd), M, use_ln, epi,
-                                             _lib.ptr(rd), _lib.ptr(y), _lib.stream_ptr()))
-        torch.cuda.synchronize()
-        return y.float().cpu()
-
-    tol = 2e-5 if dtype == torch.float32 else 2e-2
-    # fused q|k|v with LayerNorm in front
-    ln = F.layer_norm(x, (cfg.hidden_size,), wd[p + "self_attn_layer_norm.weight"], wd[p + "self_attn_layer_norm.bias"], 1e-5)
-    ref = torch.cat([F.linear(ln, wd[p + f"self_attn.{n}_proj.weight"]) for n in ("q", "k", "v")], dim=1).float()
-    got = run(_lib.T_SELF_Q, 1, x, 1, 0, None, ref.shape[1])
-    assert (got - ref).abs().max() < tol * max(1.0, ref.abs().max()), (got - ref).abs().max()
-    # fc1 + GELU
-    ln3 = F.layer_norm(x, (cfg.hidden_size,), wd[p + "final_layer_norm.weight"], wd[p + "final_layer_norm.bias"], 1e-5)
-    ref = F.gelu(F.linear(ln3, wd[p + "fc1.weight"])).float()
-    got = run(_lib.T_FC1, 1, x, 1, 1, None, cfg.ffn_dim)
-    assert (got - ref).abs().max() < tol * max(1.0, ref.abs().max())
-    # fc2 (K = 4H, chunked activation tile) + residual
-    ref = (res + F.linear(h, wd[p + "fc2.weight"])).float()
-    got = run(_lib.T_FC2, 1, h, 0, 2, res, cfg.hidden_size)
-    assert (got - ref).abs().max() < tol * max(1.0, ref.abs().max())
-    # lm heads -> f32 logits
-    lnf = F.layer_norm(x, (cfg.hidden_size,), wd["decoder.model.decoder.layer_norm.weight"], wd["decoder.model.decoder.layer_norm.bias"], 1e-5)
-    ref = torch.cat([F.linear(lnf, wd[f"decoder.lm_heads.{k}.weight"]) for k in range(cfg.num_codebooks)], dim=1).float()
-    got = run(_lib.T_LM_HEAD, 0, x, 1, 3, None, ref.shape[1])
-    assert (got - ref).abs().max() < tol * max(1.0, ref.abs().max())
-
-
 # ---- decoder: teacher-forced logits and greedy tokens ------------------------------------------------
 def _variant(name):
     if name == "abs":
