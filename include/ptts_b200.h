@@ -219,8 +219,8 @@ int ptts_op_linear(const ptts_decoder_config* cfg, const void* blob, int32_t ten
  *   kcache, vcache [B][nkv][capacity][64], rows stored swizzled (element d of row t at (((d/8) ^ t) % 8)*8 + d%8).
  *   rope != 0: rope_cos / rope_sin [max_pos][64] in dtype, applied to q (and to the appended K rows).
  *   key_mask [B][mask_len] int32 or NULL: key t < mask_len with key_mask[b][t] == 0 is excluded.
- *   prefill_sweep (q_len > 1): 0 = the decoder's choice (the tensor-core sweep for bf16 with nh == nkv unless
- *                  PTTS_PREFILL_ATTN_TC=0), 1 = always the scalar sweep (attention_item).
+ *   prefill_sweep (q_len > 1): 0 = the decoder's choice (the tensor-core sweep for bf16 with nh == nkv),
+ *                  1 = always the scalar sweep (attention_item).
  *   out [B*q_len, nh*64] in dtype. */
 int ptts_op_attention(int32_t dtype, int32_t B, int32_t nh, int32_t nkv, int32_t q_len, int32_t past_len, int32_t cross,
                       int32_t kv_len, int32_t capacity, int32_t rope, const void* rope_cos, const void* rope_sin, const void* qkv,

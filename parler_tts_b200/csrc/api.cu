@@ -32,6 +32,13 @@ static bool env_flag(const char* name, bool dflt) {
 
 using namespace ptts;
 
+// How a session runs its decode steps; ptts_session_fused reports the value.
+enum DecodePath {
+  DECODE_MULTI_KERNEL = 0,  // 8L+3 kernels per token, replayed from a CUDA graph
+  DECODE_STEP = 1,          // one persistent kernel per token (step.cu)
+  DECODE_CLUSTER = 2,       // the cluster variant of that kernel (step2.cu: 6 device-wide phases per layer)
+};
+
 struct ptts_session {
   ptts_decoder_config cfg;
   DecoderLayout L;
@@ -39,7 +46,6 @@ struct ptts_session {
   const char* blob;
   char* ws;
   int sm_count;
-  bool pdl, use_graph;
   bool has_prompt_mask, has_enc_mask, begun, prefilled;
   ptts_gen_params gen;
   int n0;            // decoder input columns of the current generate() call (1: the BOS column; > 1: continuing from codes)
@@ -48,12 +54,8 @@ struct ptts_session {
   bool graph_ready;
   int64_t launches;  // kernels launched through this session (bench.py reports it)
   long long* prof;
-  bool fused;        // decode steps run as the single persistent kernel (step.cu) instead of 8L+3 kernels
-  bool cluster;      // ... and that kernel is the cluster variant (step2.cu: 6 device-wide phases per layer)
-  StepParams sp;
-  // prefill linear layers as wgmma GEMMs (gemm_tc.cu) over the row-major weight copies ptts_decoder_finalize leaves in the
-  // blob (layout.h rm[]); PTTS_PREFILL_TC=0 keeps the mma.sync kernel (A/B runs)
-  bool prefill_tc;
+  DecodePath path;
+  StepParams sp;     // the step kernels' parameters (DECODE_STEP, DECODE_CLUSTER)
 };
 
 extern "C" {
@@ -148,11 +150,8 @@ int ptts_decoder_finalize(const ptts_decoder_config* cfg, void* blob, void* stre
     }
   }
   if (L.cl_NC > 0) {  // second copy of the layer matrices, sliced per (phase, cluster, rank) for the cluster step kernel (step2.cu)
-    const int64_t mat_off[6] = {L.wqkv, L.wo, L.wqc, L.woc, L.fc1, L.fc2};
-    for (int i = 0; i < L.L; i++) {
-      char* lb = b + L.layer0 + L.layer_stride * i;
-      if (int e = cluster_pack_layer(lb, lb, mat_off, L.cp, L.nh, L.H, L.F, st)) return e;
-    }
+    for (int i = 0; i < L.L; i++)
+      if (int e = cluster_pack_layer(L, b + L.layer0 + L.layer_stride * i, st)) return e;
   }
   return PTTS_OK;
 }
@@ -196,17 +195,13 @@ int ptts_session_create2(const ptts_decoder_config* cfg, const void* blob, void*
   cudaGetDevice(&dev);
   s->sm_count = 132;
   cudaDeviceGetAttribute(&s->sm_count, cudaDevAttrMultiProcessorCount, dev);
-  s->pdl = env_flag("PTTS_PDL", true);
-  s->use_graph = env_flag("PTTS_GRAPH", true);
   s->graph_ready = false;
   s->exec = nullptr;
   s->cap_stream = nullptr;
   s->begun = s->prefilled = false;
-  s->fused = false;
-  s->cluster = false;
+  s->path = DECODE_MULTI_KERNEL;
   s->prof = nullptr;
   s->launches = 0;
-  s->prefill_tc = (cfg->dtype == PTTS_BF16) && env_flag("PTTS_PREFILL_TC", true);
   *out = s;
   return PTTS_OK;
 }
@@ -244,45 +239,33 @@ static SampleArgs sample_args(ptts_session* s) {
 }
 
 
-// Fused-step schedule: largest n-tile count that keeps ~one task per CTA.
-static int pick_nt(int ntiles, int grid) {
-  const int cand[4] = {4, 3, 2, 1};  // the variants instantiated in step.cu::run_gemm
-  for (int i = 0; i < 4; i++)
-    if (ntiles % cand[i] == 0 && ntiles / cand[i] >= (grid * 8) / 10) return cand[i];
-  for (int i = 0; i < 4; i++)
-    if (ntiles % cand[i] == 0 && ntiles / cand[i] >= grid / 2) return cand[i];
-  return 1;
-}
-
-// The fused kernel covers bf16, B <= 32, K <= 16: anything else runs the 8L+3-kernel path -- a 2x slower step.  Say so once per
-// process instead of degrading silently, and count it (ptts_session_fused reports which path a session uses).
-static bool fused_declined(ptts_session* s, const char* why) {
+// The step kernels cover bf16, B <= 32, K <= 16: anything else runs the 8L+3-kernel path -- a 2x slower step.  Say so once per
+// process instead of degrading silently (ptts_session_fused reports which path a session uses).
+static DecodePath step_declined(ptts_session* s, const char* why) {
   static bool warned = false;
   if (!warned) {
     fprintf(stderr, "ptts_b200: fused decode step not used for this session (B=%d, H=%d, K=%d: %s); decode steps run the multi-kernel path\n",
             s->W.B, s->L.H, s->L.K, why);
     warned = true;
   }
-  return false;
+  return DECODE_MULTI_KERNEL;
 }
 
-static bool setup_fused(ptts_session* s) {
+// The fastest decode path the session's shape and the device allow; fills s->sp for the step kernels.  PTTS_FUSED=0 keeps the
+// multi-kernel path and PTTS_STEP=legacy keeps step.cu where step2.cu applies: each is the bit-exact reference of the next.
+static DecodePath choose_decode_path(ptts_session* s) {
   const ptts_decoder_config& c = s->cfg;
   const DecoderLayout& L = s->L;
   const WorkspaceLayout& W = s->W;
-  if (c.dtype != PTTS_BF16 || !env_flag("PTTS_FUSED", true)) return false;
-  if (W.B > 32 || L.K > 16 || L.H % 64 != 0 || L.F % L.H != 0) return fused_declined(s, "batch > 32 rows, > 16 codebooks or an unsupported width");
+  if (c.dtype != PTTS_BF16 || !env_flag("PTTS_FUSED", true)) return DECODE_MULTI_KERNEL;
+  if (W.B > 32 || L.K > 16 || L.H % 64 != 0 || L.F % L.H != 0) return step_declined(s, "batch > 32 rows, > 16 codebooks or an unsupported width");
   StepParams& p = s->sp;
   memset(&p, 0, sizeof(p));
   p.B = W.B; p.H = L.H; p.F = L.F; p.V = L.V; p.K = L.K; p.L = L.L; p.nh = L.nh; p.nkv = L.nkv; p.nckv = L.nckv;
   p.S = W.S; p.P = W.P; p.Tmax = W.Tmax; p.rope = c.rope; p.act = c.activation; p.qkv_rows = L.qkv_rows; p.ckv_rows = L.ckv_rows;
   p.eps = c.layer_norm_eps; p.scale = 0.125f;
   p.blob = s->blob;
-  p.embed = L.embed; p.pos = L.pos; p.layer0 = L.layer0; p.layer_stride = L.layer_stride;
-  p.ln1_w = L.ln1_w; p.ln1_b = L.ln1_b; p.wqkv = L.wqkv; p.wo = L.wo; p.ln2_w = L.ln2_w; p.ln2_b = L.ln2_b; p.wqc = L.wqc; p.woc = L.woc;
-  p.ln3_w = L.ln3_w; p.ln3_b = L.ln3_b; p.fc1 = L.fc1; p.fc2 = L.fc2;
-  p.c_qkv = L.c_qkv; p.c_qc = L.c_qc; p.c_fc1 = L.c_fc1; p.c_heads = L.c_heads;
-  p.final_ln_w = L.final_ln_w; p.final_ln_b = L.final_ln_b; p.heads = L.heads; p.rope_cos = L.rope_cos; p.rope_sin = L.rope_sin;
+  p.lay = L;
   char* ws = s->ws;
   p.x = (bf16*)(ws + W.img_x); p.qkv = (bf16*)(ws + W.qkv); p.attn = (bf16*)(ws + W.img_attn); p.qc = (bf16*)(ws + W.qc); p.hbuf = (bf16*)(ws + W.img_h);
   p.logits = (float*)(ws + W.logits);
@@ -293,43 +276,13 @@ static bool setup_fused(ptts_session* s) {
   p.sa = sample_args(s);
   p.bar = ((Ctrl*)(ws + W.ctrl))->bar;
   p.progress = (int*)(ws + W.progress);
-  const int G = s->sm_count;
-  p.nt_qkv = pick_nt(L.qkv_rows / 8, G);
-  p.nt_h = pick_nt(L.H / 8, G);
-  p.nt_fc1 = pick_nt(L.F / 8, G);
-  p.nt_heads = pick_nt(L.K * L.V / 8, G);
-  int ntmax = p.nt_qkv;
-  if (p.nt_h > ntmax) ntmax = p.nt_h;
-  if (p.nt_fc1 > ntmax) ntmax = p.nt_fc1;
-  if (p.nt_heads > ntmax) ntmax = p.nt_heads;
-  const int64_t tile = (int64_t)32 * (L.H + 8) * 2;
-  const int64_t red = (int64_t)8 * 32 * (8 * ntmax + 8) * 4;  // K-reduction scratch [8 warps][32][RS], step.cu
-  // weight buffer: the largest per-task slice (nt n-tiles x K, 16 bytes per (n-tile, k-pair) fragment row)
-  int64_t wbytes = (int64_t)p.nt_qkv * L.H * 16;
-  if ((int64_t)p.nt_h * L.F * 16 > wbytes) wbytes = (int64_t)p.nt_h * L.F * 16;
-  if ((int64_t)p.nt_fc1 * L.H * 16 > wbytes) wbytes = (int64_t)p.nt_fc1 * L.H * 16;
-  if ((int64_t)p.nt_heads * L.H * 16 > wbytes) wbytes = (int64_t)p.nt_heads * L.H * 16;
-  p.attn_floats_per_warp = 0;
-  const int64_t att = (int64_t)8 * (2 * 2 * 32 * 64 * 2 + 3 * 64 * 4) + 4 * 128 * 4;  // 8 x attn_decode_smem_per_warp<bf16>() + pair exchange
-  const int64_t budget = 215 * 1024 - 2816;  // step.cu ST_HEADER
-  p.nbuf = (2 * tile + wbytes <= budget) ? 2 : 1;
-  if (p.nbuf * tile < red) return fused_declined(s, "the K-reduction scratch does not fit the activation tile");
-  p.wbuf_offset = align_up(p.nbuf * tile, 128);
-  int64_t region = p.wbuf_offset + wbytes;
-  if (att > region) region = att;
-  region = align_up(region, 16);
-  if (region > budget) return fused_declined(s, "tile + weight slice exceed the shared memory of an SM");
-  p.tile_region_bytes = region;
-  p.sample_items = (L.V + 255) / 256;
-  if (p.sample_items > 9) return fused_declined(s, "vocab_size > 2304");
+  if (const char* why = plan_decode_step(p, s->sm_count)) return step_declined(s, why);
   p.do_sample_phase = 1;
   p.prof = s->prof;
-  // cluster variant (step2.cu) when the shape and the device allow it; PTTS_STEP=legacy keeps step.cu (A/B runs, cross-checks)
-  for (int i = 0; i < 6; i++) { p.cp[i] = L.cp[i]; p.cp_slice[i] = L.cp_slice[i]; }
   p.cl_x = (bf16*)(ws + W.cl_x); p.cl_attn = (bf16*)(ws + W.cl_attn); p.cl_h = (bf16*)(ws + W.cl_h);
   const char* mode = getenv("PTTS_STEP");
-  s->cluster = L.cl_NC > 0 && !(mode && strcmp(mode, "legacy") == 0) && cluster_step_available(p);
-  return true;
+  if (L.cl_NC > 0 && !(mode && strcmp(mode, "legacy") == 0) && cluster_step_available(p)) return DECODE_CLUSTER;
+  return DECODE_STEP;
 }
 
 int ptts_generate_begin_ids(ptts_session* s, const ptts_gen_params* gen, const int64_t* input_ids, int32_t n0, void* stream) {
@@ -376,7 +329,7 @@ static int run_forward(ptts_session* s, cudaStream_t st, bool prefill, const voi
   const int B = W.B, P = W.P, S = W.S, H = L.H, D = PTTS_HEAD_DIM;
   const int q_len = prefill ? P + s->n0 : 1;
   const int M = B * q_len;
-  const bool pdl = s->pdl && !prefill;  // the one-off prefill stays on plain stream order
+  const bool pdl = !prefill;  // the one-off prefill stays on plain stream order
   const Ctrl* ctrl = prefill ? nullptr : (const Ctrl*)(s->ws + W.ctrl);
   const int es = L.es;
   char* ws = s->ws;
@@ -407,7 +360,7 @@ static int run_forward(ptts_session* s, cudaStream_t st, bool prefill, const voi
     a.epi = epi; a.act = c.activation; a.ctrl = ctrl;
     s->launches++;
     // the same matrix, row-major: M = B*(P+n0) or B*S rows are tensor-core work (wgmma, gemm_tc.cu)
-    const int64_t rm = (prefill && s->prefill_tc) ? rowmajor_offset(L, woff) : -1;
+    const int64_t rm = prefill ? rowmajor_offset(L, woff) : -1;
     if (rm >= 0 && linear_tc_supported(a)) {
       if (a.c1 != nullptr) s->launches++;  // row statistics kernel
       return launch_linear_tc(a, blob + rm, (float*)(ws + W.row_stats), st);
@@ -440,7 +393,7 @@ static int run_forward(ptts_session* s, cudaStream_t st, bool prefill, const voi
     at.rope = c.rope; at.rope_cos = blob + L.rope_cos; at.rope_sin = blob + L.rope_sin;
     at.kv_capacity = prefill ? q_len : W.Tmax;
     at.scale = 0.125f;  // head_dim ** -0.5, applied inside SDPA (quirk Q1)
-    if (int e = launch_attention(at, c.dtype, st, pdl, prefill_attn_tc_default())) return e;
+    if (int e = launch_attention(at, c.dtype, st, pdl, true)) return e;
     s->launches++;
     if (int e = lin(ws + W.attn, H, lb + L.wo, H, H, nullptr, nullptr, EPI_RESIDUAL, x, x, H, M)) return e;
     if (int e = lin(x, H, lb + L.wqc, H, H, (const float*)(blob + lb + L.ln2_w), (const float*)(blob + lb + L.ln2_b),
@@ -453,7 +406,7 @@ static int run_forward(ptts_session* s, cudaStream_t st, bool prefill, const voi
     ct.kv_b_stride = (int64_t)L.nckv * S * D; ct.kv_h_stride = (int64_t)S * D; ct.kv_t_stride = D;
     ct.key_mask = s->has_enc_mask ? (const int*)(ws + W.enc_mask) : nullptr; ct.mask_len = S; ct.mask_ld = S;
     ct.nkv = L.nckv; ct.cross = 1; ct.kv_len = S; ct.kv_capacity = S;
-    if (int e = launch_attention(ct, c.dtype, st, pdl, prefill_attn_tc_default())) return e;
+    if (int e = launch_attention(ct, c.dtype, st, pdl, true)) return e;
     s->launches++;
     if (int e = lin(ws + W.attn, H, lb + L.woc, H, H, nullptr, nullptr, EPI_RESIDUAL, x, x, H, M)) return e;
     if (int e = lin(x, H, lb + L.fc1, L.F, H, (const float*)(blob + lb + L.ln3_w), (const float*)(blob + lb + L.ln3_b),
@@ -478,7 +431,7 @@ int ptts_prefill(ptts_session* s, const void* prompt_hidden, const int64_t* prom
   if (s->has_enc_mask) { if (int e = launch_mask_convert(enc_mask, s->W.B * s->W.S, (int*)(s->ws + s->W.enc_mask), st)) return e; }
   if (int e = run_forward(s, st, true, prompt_hidden, enc_hidden)) return e;
   s->prefilled = true;
-  s->fused = setup_fused(s);
+  s->path = choose_decode_path(s);
   // mask presence is baked into the captured graph: re-capture if it changed
   if (s->exec) { cudaGraphExecDestroy(s->exec); s->exec = nullptr; s->graph_ready = false; }
   return PTTS_OK;
@@ -487,14 +440,15 @@ int ptts_prefill(ptts_session* s, const void* prompt_hidden, const int64_t* prom
 int ptts_decode_forward(ptts_session* s, void* stream) {
   PTTS_REQUIRE(s, "null argument");
   if (!s->prefilled) return fail(PTTS_ESTATE, "ptts_decode_forward called before ptts_prefill");
-  if (s->fused) {
-    StepParams p = s->sp;
-    p.do_sample_phase = 0;
-    s->launches++;
-    if (s->cluster) return launch_decode_step_cluster(p, (cudaStream_t)stream);
-    return launch_decode_step(p, s->sm_count, (cudaStream_t)stream);
+  cudaStream_t st = (cudaStream_t)stream;
+  StepParams p = s->sp;
+  p.do_sample_phase = 0;
+  switch (s->path) {
+    case DECODE_CLUSTER: s->launches++; return launch_decode_step_cluster(p, st);
+    case DECODE_STEP: s->launches++; return launch_decode_step(p, s->sm_count, st);
+    case DECODE_MULTI_KERNEL: break;
   }
-  return run_forward(s, (cudaStream_t)stream, false, nullptr, nullptr);
+  return run_forward(s, st, false, nullptr, nullptr);
 }
 
 int ptts_sample(ptts_session* s, const int64_t* forced_tokens, void* stream) {
@@ -508,40 +462,34 @@ int ptts_decode_steps(ptts_session* s, int32_t n_steps, void* stream) {
   PTTS_REQUIRE(s && n_steps >= 0, "bad argument");
   if (!s->prefilled) return fail(PTTS_ESTATE, "ptts_decode_steps called before ptts_prefill");
   cudaStream_t st = (cudaStream_t)stream;
-  if (s->fused && s->cluster) {  // the cluster kernel loops over tokens itself: up to PTTS_STEPS_PER_LAUNCH (default 64) per launch
-    const char* env = getenv("PTTS_STEPS_PER_LAUNCH");   // (read per call: tests compare 1 against the default)
-    const int per_launch = env ? (atoi(env) < 1 ? 1 : atoi(env)) : 64;
-    for (int done = 0; done < n_steps;) {
-      const int m = (n_steps - done < per_launch) ? n_steps - done : per_launch;
-      s->sp.n_steps = m;
-      const int e = launch_decode_step_cluster(s->sp, st);
-      s->sp.n_steps = 1;
-      if (e) return e;
-      done += m;
-      s->launches += 1;
+  switch (s->path) {
+    case DECODE_CLUSTER: {  // the kernel loops over tokens itself: up to PTTS_STEPS_PER_LAUNCH (default 64) per launch
+      const char* env = getenv("PTTS_STEPS_PER_LAUNCH");   // (read per call: tests compare 1 against the default)
+      const int per_launch = env ? (atoi(env) < 1 ? 1 : atoi(env)) : 64;
+      for (int done = 0; done < n_steps;) {
+        const int m = (n_steps - done < per_launch) ? n_steps - done : per_launch;
+        s->sp.n_steps = m;
+        const int e = launch_decode_step_cluster(s->sp, st);
+        s->sp.n_steps = 1;
+        if (e) return e;
+        done += m;
+        s->launches += 1;
+      }
+      return PTTS_OK;
     }
-    return PTTS_OK;
-  }
-  if (s->fused) {  // one persistent kernel per token: nothing to gain from a graph
-    for (int i = 0; i < n_steps; i++)
-      if (int e = launch_decode_step(s->sp, s->sm_count, st)) return e;
-    s->launches += n_steps;
-    return PTTS_OK;
-  }
-  if (!s->use_graph) {
-    for (int i = 0; i < n_steps; i++) {
-      if (int e = run_forward(s, st, false, nullptr, nullptr)) return e;
-      s->launches++;
-      if (int e = launch_sample(sample_args(s), nullptr, st, s->pdl)) return e;
-    }
-    return PTTS_OK;
+    case DECODE_STEP:  // one persistent kernel per token: nothing to gain from a graph
+      for (int i = 0; i < n_steps; i++)
+        if (int e = launch_decode_step(s->sp, s->sm_count, st)) return e;
+      s->launches += n_steps;
+      return PTTS_OK;
+    case DECODE_MULTI_KERNEL: break;
   }
   if (!s->graph_ready) {
     if (!s->cap_stream) PTTS_CHECK_CUDA(cudaStreamCreateWithFlags(&s->cap_stream, cudaStreamNonBlocking));
     const int64_t before = s->launches;
     PTTS_CHECK_CUDA(cudaStreamBeginCapture(s->cap_stream, cudaStreamCaptureModeThreadLocal));
     int e = run_forward(s, s->cap_stream, false, nullptr, nullptr);
-    if (!e) { s->launches++; e = launch_sample(sample_args(s), nullptr, s->cap_stream, s->pdl); }
+    if (!e) { s->launches++; e = launch_sample(sample_args(s), nullptr, s->cap_stream, true); }
     cudaGraph_t graph = nullptr;
     cudaError_t ce = cudaStreamEndCapture(s->cap_stream, &graph);
     s->launches = before;
@@ -575,7 +523,7 @@ int ptts_session_set_profile(ptts_session* s, void* buf) {
   s->sp.prof = s->prof;
   return PTTS_OK;
 }
-int ptts_session_fused(ptts_session* s, int32_t* out) { PTTS_REQUIRE(s && out, "null"); *out = s->fused ? (s->cluster ? 2 : 1) : 0; return PTTS_OK; }
+int ptts_session_fused(ptts_session* s, int32_t* out) { PTTS_REQUIRE(s && out, "null"); *out = s->path; return PTTS_OK; }
 int ptts_session_launches(ptts_session* s, int64_t* out) { PTTS_REQUIRE(s && out, "null"); *out = s->launches; return PTTS_OK; }
 
 // ---- stand-alone operators ----------------------------------------------------------------------
@@ -686,7 +634,7 @@ int ptts_op_attention(int32_t dtype, int32_t B, int32_t nh, int32_t nkv, int32_t
   a.rope = rope; a.rope_cos = rope_cos; a.rope_sin = rope_sin;
   a.kv_capacity = cross ? kv_len : past_len + q_len;   // keys per query at most (attention_item's score buffer)
   a.scale = 0.125f;
-  return launch_attention(a, dtype, (cudaStream_t)stream, false, prefill_sweep == 0 && prefill_attn_tc_default());
+  return launch_attention(a, dtype, (cudaStream_t)stream, false, prefill_sweep == 0);
 }
 
 // ---- DAC ----------------------------------------------------------------------------------------
@@ -790,7 +738,7 @@ int ptts_dac_decode(const ptts_dac_config* cfg, const void* blob, void* workspac
       }
     }
     const int cl = C >> cfg->n_blocks;
-    if (final_conv_supported(cl) && env_flag("PTTS_DAC_FINAL_FAST", true))   // one thread per output sample (dac.cu)
+    if (final_conv_supported(cl))   // one thread per output sample (dac.cu)
       return launch_final_conv_tanh(act, tpp(ti + 1), tpp(ti + 2), audio_out, cl, Tlen, B, st);
     ConvArgs f{};  // final conv (Cout = 1) + tanh on the already snake'd tensor: generic kernel
     f.x = act; f.w = tpp(ti + 1); f.bias = tpp(ti + 2); f.alpha = nullptr; f.res = nullptr; f.out = audio_out;

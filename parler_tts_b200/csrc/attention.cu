@@ -10,8 +10,6 @@
 // once) -- SURVEY 8(d)'s kv_tok term.  One CTA per (kv head, batch row); 8 lanes cover one 128 B key
 // row with 16 B loads (fully coalesced), 16 keys in flight per CTA iteration, fp32 softmax,
 // probabilities rounded to the model dtype before P.V exactly like the flash kernels torch calls.
-#include <cstdlib>
-
 #include "common.cuh"
 #include "kernels.h"
 #include "attn_core.cuh"
@@ -110,11 +108,6 @@ __global__ void __launch_bounds__(PRE_TC_WARPS * 32) attention_prefill_tc_kernel
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // the zero-filled tail of a partial V stage (generic writes) before the next item's refill
     __syncwarp();
   }
-}
-
-bool prefill_attn_tc_default() {
-  static const bool pre_tc = []() { const char* e = getenv("PTTS_PREFILL_ATTN_TC"); return !(e && e[0] == '0'); }();
-  return pre_tc;
 }
 
 int launch_attention(const AttnArgs& a, int dtype, cudaStream_t st, bool pdl, bool prefill_tc) {

@@ -1,5 +1,5 @@
-// gemm_tc.cu -- the prefill linear layers as Hopper wgmma GEMMs (default for the bf16 model dtype; PTTS_PREFILL_TC=0 switches back
-// to the mma.sync kernel of gemm.cu for A/B runs; tests/test_gpu_parity.py::test_prefill_tc_matches_default_prefill compares them).
+// gemm_tc.cu -- the prefill linear layers as Hopper wgmma GEMMs (bf16 model dtype; what linear_tc_supported rejects, and fp32, run
+// the mma.sync kernel of gemm.cu; tests/test_linear_reference.py checks both against float64 at every tile edge).
 //
 // Why: at prefill the decoder's linear layers see M = B*(P+1) (prompt) or B*S (encoder K/V projection) rows, ~1000-2000 for
 // the bench workload: 6.6 GFLOP per matrix, tensor-bound.  The decode GEMM (gemm.cu: 32-row tiles, mma.sync, weights re-read

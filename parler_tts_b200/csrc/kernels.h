@@ -18,7 +18,7 @@ struct LinearArgs {
   const Ctrl* ctrl;            // device control block: kernels no-op once generation has finished
 };
 int launch_linear(const LinearArgs& a, int dtype, cudaStream_t st, bool pdl, int sm_count);
-// wgmma prefill GEMM (gemm_tc.cu; the bf16 default, PTTS_PREFILL_TC=0 turns it off)
+// wgmma prefill GEMM (gemm_tc.cu): the bf16 prefill's linear layers wherever linear_tc_supported holds
 bool linear_tc_supported(const LinearArgs& a);
 int launch_linear_tc(const LinearArgs& a, const void* w_rowmajor, float* stats_scratch, cudaStream_t st);
 int unpack_fragments(const void* frag, void* dst_rowmajor, int64_t N, int K, cudaStream_t st);
@@ -47,8 +47,6 @@ struct AttnArgs {
 };
 // prefill_tc: bf16 MHA prefill (q_len > 1) runs on the tensor-core sweep (attention_prefill_tc_kernel) rather than attention_item
 int launch_attention(const AttnArgs& a, int dtype, cudaStream_t st, bool pdl, bool prefill_tc);
-// the product's choice of prefill sweep: on unless PTTS_PREFILL_ATTN_TC=0 (read once per process)
-bool prefill_attn_tc_default();
 
 // ---- embedding (embed.cu) -----------------------------------------------------------------------
 struct EmbedArgs {

@@ -48,6 +48,22 @@ static inline bool cluster_shape_ok(const ptts_decoder_config& c) {
 
 static inline int dtype_size(int dt) { return dt == PTTS_BF16 ? 2 : 4; }
 
+// Cluster step kernel (step2.cu): how phase ph of a layer (A qkv | B o | C q_cross | D o_cross | E fc1 | F fc2) cuts its matrix
+// into slices.  A slice is nt n-tiles (a head's q|k|v = 192 features, a cluster's 16 out-proj features, a head's q_cross, ...,
+// F / (4 nh) fc1 features) x the kt k32 tiles of one rank; the head phases keep one slice set per head, the others one per cluster.
+struct ClusterPhase {
+  int64_t mat;     // offset of the fragment-order matrix inside the layer
+  int nt, owners;  // n-tiles per slice; slice owners (heads or clusters), each with cl_C slices
+  int kt, kt_src;  // k32 tiles per rank; of the whole matrix
+};
+static inline ClusterPhase cluster_phase(const DecoderLayout& l, int ph) {
+  const int64_t mat[6] = {l.wqkv, l.wo, l.wqc, l.woc, l.fc1, l.fc2};
+  const int nt[6] = {24, 2, 8, 2, l.F / (4 * l.nh) / 8, 2};
+  const int owners[6] = {l.nh, 4 * l.nh, l.nh, 4 * l.nh, 4 * l.nh, 4 * l.nh};
+  const int K = (ph == 5) ? l.F : l.H;
+  return {mat[ph], nt[ph], owners[ph], K / l.cl_C / 32, K / 32};
+}
+
 static inline DecoderLayout make_layout(const ptts_decoder_config& c) {
   DecoderLayout l{};
   l.es = dtype_size(c.dtype);
@@ -84,13 +100,10 @@ static inline DecoderLayout make_layout(const ptts_decoder_config& c) {
   for (int i = 0; i < 6; i++) l.cp[i] = l.cp_slice[i] = 0;
   if (cluster_shape_ok(c)) {
     l.cl_C = 2; l.cl_NC = 4 * l.nh;
-    const int64_t ks = l.H / 2 / 32, ksf = l.F / 2 / 32;                 // k32 tiles per rank: K = H phases, K = F phase
-    // n-tiles per slice: a head's q|k|v (192 features), a cluster's 16 out-proj features, a head's q_cross, ..., F / (4 nh) fc1 features
-    const int64_t nt[6] = {24, 2, 8, 2, l.F / (4 * l.nh) / 8, 2};
-    const int64_t owners[6] = {l.nh, 4 * l.nh, l.nh, 4 * l.nh, 4 * l.nh, 4 * l.nh};   // head phases: one slice set per head
     for (int i = 0; i < 6; i++) {
-      l.cp_slice[i] = nt[i] * (i == 5 ? ksf : ks) * 512;
-      l.cp[i] = take(l.cp_slice[i] * owners[i] * l.cl_C) - base;
+      const ClusterPhase cp = cluster_phase(l, i);
+      l.cp_slice[i] = (int64_t)cp.nt * cp.kt * 512;
+      l.cp[i] = take(l.cp_slice[i] * cp.owners * l.cl_C) - base;
     }
   }
   l.layer_stride = o - base;

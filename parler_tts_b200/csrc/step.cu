@@ -17,6 +17,8 @@
 //   * weights stream from L2 in mma B-fragment order straight into registers (gemm.cu's layout);
 //   * attention processes two (row, kv head) items per CTA concurrently (128 threads each, named barriers).
 // All reductions keep a fixed order: results are bit-reproducible and identical to the multi-kernel path.
+#include <algorithm>
+
 #include "attn_core.cuh"
 #include "common.cuh"
 #include "kernels.h"
@@ -31,6 +33,7 @@ namespace ptts {
 constexpr int ST_THREADS = 256;
 constexpr int ST_WARPS = 8;
 constexpr int ST_HEADER = 512 + 8 * 32 * 2 * 4 + 256;  // mbarriers [0,256) | row stats [256,512) | stat partials [512,2560) | c1,c2 of the task [2560,2816)
+constexpr int ST_SMEM_LIMIT = 215 * 1024;  // dynamic shared memory of a launch at most: header + tile region (+ 256 B static: the sampler scratch)
 
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   uint32_t ok;
@@ -150,16 +153,16 @@ struct WeightJob { const char* src; uint32_t bytes; };
 // matrix of GEMM phase `ph` (not an attention phase): packed weights, N, K and n-tiles per task
 __device__ __forceinline__ void gemm_matrix(const StepParams& p, int ph, const char*& W, int& N, int& K, int& nt) {
   const int l = ph >> 3, sub = (ph >= 8 * p.L) ? 8 : (ph & 7);
-  const char* lb = p.blob + p.layer0 + p.layer_stride * (l < p.L ? l : p.L - 1);
+  const char* lb = p.blob + p.lay.layer0 + p.lay.layer_stride * (l < p.L ? l : p.L - 1);
   const int H = p.H;
   switch (sub) {
-    case 0: W = lb + p.wqkv; N = p.qkv_rows; K = H; nt = p.nt_qkv; break;
-    case 2: W = lb + p.wo; N = H; K = H; nt = p.nt_h; break;
-    case 3: W = lb + p.wqc; N = H; K = H; nt = p.nt_h; break;
-    case 5: W = lb + p.woc; N = H; K = H; nt = p.nt_h; break;
-    case 6: W = lb + p.fc1; N = p.F; K = H; nt = p.nt_fc1; break;
-    case 7: W = lb + p.fc2; N = H; K = p.F; nt = p.nt_h; break;
-    default: W = p.blob + p.heads; N = p.K * p.V; K = H; nt = p.nt_heads; break;
+    case 0: W = lb + p.lay.wqkv; N = p.qkv_rows; K = H; nt = p.nt_qkv; break;
+    case 2: W = lb + p.lay.wo; N = H; K = H; nt = p.nt_h; break;
+    case 3: W = lb + p.lay.wqc; N = H; K = H; nt = p.nt_h; break;
+    case 5: W = lb + p.lay.woc; N = H; K = H; nt = p.nt_h; break;
+    case 6: W = lb + p.lay.fc1; N = p.F; K = H; nt = p.nt_fc1; break;
+    case 7: W = lb + p.lay.fc2; N = H; K = p.F; nt = p.nt_h; break;
+    default: W = p.blob + p.lay.heads; N = p.K * p.V; K = H; nt = p.nt_heads; break;
   }
 }
 
@@ -377,14 +380,14 @@ __global__ void __launch_bounds__(ST_THREADS, 1) decode_step_kernel(const __grid
   prof_mark(sm.prof, 0);
   // ---- phase 0: embeddings + L2 prefetch of layer 0 ----
   if (tid == 0) {
-    const char* lb = blob + p.layer0;
-    prefetch_slice(lb + p.wqkv, p.qkv_rows, H, p.nt_qkv);
-    l2_prefetch(lb + p.c_qkv, (uint32_t)p.qkv_rows * 8); l2_prefetch(lb + p.c_qc, (uint32_t)H * 8); l2_prefetch(lb + p.c_fc1, (uint32_t)p.F * 8);
-    prefetch_slice(lb + p.wo, H, H, p.nt_h);
-    prefetch_slice(lb + p.wqc, H, H, p.nt_h);
-    prefetch_slice(lb + p.woc, H, H, p.nt_h);
-    prefetch_slice(lb + p.fc1, p.F, H, p.nt_fc1);
-    prefetch_slice(lb + p.fc2, H, p.F, p.nt_h);
+    const char* lb = blob + p.lay.layer0;
+    prefetch_slice(lb + p.lay.wqkv, p.qkv_rows, H, p.nt_qkv);
+    l2_prefetch(lb + p.lay.c_qkv, (uint32_t)p.qkv_rows * 8); l2_prefetch(lb + p.lay.c_qc, (uint32_t)H * 8); l2_prefetch(lb + p.lay.c_fc1, (uint32_t)p.F * 8);
+    prefetch_slice(lb + p.lay.wo, H, H, p.nt_h);
+    prefetch_slice(lb + p.lay.wqc, H, H, p.nt_h);
+    prefetch_slice(lb + p.lay.woc, H, H, p.nt_h);
+    prefetch_slice(lb + p.lay.fc1, p.F, H, p.nt_fc1);
+    prefetch_slice(lb + p.lay.fc2, H, p.F, p.nt_h);
   }
   {
     const int cpr = (H + ST_THREADS - 1) / ST_THREADS;  // column chunks per row: (row, chunk) items spread over all CTAs
@@ -404,7 +407,7 @@ __global__ void __launch_bounds__(ST_THREADS, 1) decode_step_kernel(const __grid
     const int l = ph >> 3, sub = (ph == 8 * p.L) ? 8 : (ph & 7);
     sm.prof = prof0 ? prof0 + (size_t)(ph + 1) * 8 : nullptr;
     prof_mark(sm.prof, 0);
-    const char* lb = blob + p.layer0 + p.layer_stride * (l < p.L ? l : p.L - 1);
+    const char* lb = blob + p.lay.layer0 + p.lay.layer_stride * (l < p.L ? l : p.L - 1);
     if (sub == 1 || sub == 4) {
       AttnArgs a = decode_attn_args(p, l, pos, sub == 4);
       a.ldo = sm.pitch; a.out = p.attn;
@@ -420,7 +423,7 @@ __global__ void __launch_bounds__(ST_THREADS, 1) decode_step_kernel(const __grid
       // SAME phase of the next layer will use into L2 (PrefetchJob), so the HBM stream is spread over the layer;
       // folded-LayerNorm vectors ride along, and the qkv phase prefetches this layer's K/V rows.
       const bool last = (l + 1 >= p.L);
-      const char* nb = lb + p.layer_stride;
+      const char* nb = lb + p.lay.layer_stride;
       const int64_t img = (int64_t)32 * sm.pitch;  // elements per tile image
       const int ld = sm.pitch;
       GemmDesc g{};
@@ -434,45 +437,45 @@ __global__ void __launch_bounds__(ST_THREADS, 1) decode_step_kernel(const __grid
       };
       switch (sub) {
         case 0:  // qkv = LN1(x) Wqkv^T
-          g.X = p.x; g.W = reinterpret_cast<const uint4*>(lb + p.wqkv); g.N = p.qkv_rows; g.K = H;
-          g.c1 = reinterpret_cast<const float*>(lb + p.c_qkv); g.c2 = g.c1 + p.qkv_rows;
+          g.X = p.x; g.W = reinterpret_cast<const uint4*>(lb + p.lay.wqkv); g.N = p.qkv_rows; g.K = H;
+          g.c1 = reinterpret_cast<const float*>(lb + p.lay.c_qkv); g.c2 = g.c1 + p.qkv_rows;
           g.epi = EPI_STORE; g.R = nullptr; g.Y = p.qkv; g.ldy = p.qkv_rows;
           nt = p.nt_qkv;
-          set_pf(p.wqkv, p.qkv_rows, H, p.nt_qkv, p.c_qkv, p.qkv_rows);
-          if (last) { g.pf.w = blob + p.heads; g.pf.N = p.K * p.V; g.pf.K = H; g.pf.nt = p.nt_heads; g.pf.v = blob + p.c_heads; g.pf.v_bytes = (uint32_t)(p.K * p.V) * 8; }
+          set_pf(p.lay.wqkv, p.qkv_rows, H, p.nt_qkv, p.lay.c_qkv, p.qkv_rows);
+          if (last) { g.pf.w = blob + p.lay.heads; g.pf.N = p.K * p.V; g.pf.K = H; g.pf.nt = p.nt_heads; g.pf.v = blob + p.lay.c_heads; g.pf.v_bytes = (uint32_t)(p.K * p.V) * 8; }
           g.pf.kv_layer = l;
           break;
         case 2:  // x += attn Wo^T
-          g.X = p.attn; g.W = reinterpret_cast<const uint4*>(lb + p.wo); g.N = H; g.K = H; g.c1 = nullptr; g.c2 = nullptr;
+          g.X = p.attn; g.W = reinterpret_cast<const uint4*>(lb + p.lay.wo); g.N = H; g.K = H; g.c1 = nullptr; g.c2 = nullptr;
           g.epi = EPI_RESIDUAL; g.R = p.x; g.Y = p.x; g.ldy = ld;
-          set_pf(p.wo, H, H, p.nt_h, 0, 0);
+          set_pf(p.lay.wo, H, H, p.nt_h, 0, 0);
           break;
         case 3:  // q_cross = LN2(x) Wq^T
-          g.X = p.x; g.W = reinterpret_cast<const uint4*>(lb + p.wqc); g.N = H; g.K = H;
-          g.c1 = reinterpret_cast<const float*>(lb + p.c_qc); g.c2 = g.c1 + H;
+          g.X = p.x; g.W = reinterpret_cast<const uint4*>(lb + p.lay.wqc); g.N = H; g.K = H;
+          g.c1 = reinterpret_cast<const float*>(lb + p.lay.c_qc); g.c2 = g.c1 + H;
           g.epi = EPI_STORE; g.R = nullptr; g.Y = p.qc; g.ldy = H;
-          set_pf(p.wqc, H, H, p.nt_h, p.c_qc, H);
+          set_pf(p.lay.wqc, H, H, p.nt_h, p.lay.c_qc, H);
           break;
         case 5:  // x += attn Wo_cross^T
-          g.X = p.attn; g.W = reinterpret_cast<const uint4*>(lb + p.woc); g.N = H; g.K = H; g.c1 = nullptr; g.c2 = nullptr;
+          g.X = p.attn; g.W = reinterpret_cast<const uint4*>(lb + p.lay.woc); g.N = H; g.K = H; g.c1 = nullptr; g.c2 = nullptr;
           g.epi = EPI_RESIDUAL; g.R = p.x; g.Y = p.x; g.ldy = ld;
-          set_pf(p.woc, H, H, p.nt_h, 0, 0);
+          set_pf(p.lay.woc, H, H, p.nt_h, 0, 0);
           break;
         case 6:  // h = act(LN3(x) W1^T), written as F/H tile images
-          g.X = p.x; g.W = reinterpret_cast<const uint4*>(lb + p.fc1); g.N = p.F; g.K = H;
-          g.c1 = reinterpret_cast<const float*>(lb + p.c_fc1); g.c2 = g.c1 + p.F;
+          g.X = p.x; g.W = reinterpret_cast<const uint4*>(lb + p.lay.fc1); g.N = p.F; g.K = H;
+          g.c1 = reinterpret_cast<const float*>(lb + p.lay.c_fc1); g.c2 = g.c1 + p.F;
           g.epi = EPI_ACT; g.R = nullptr; g.Y = p.hbuf; g.ldy = ld; g.y_chunk = H; g.y_chunk_stride = img;
           nt = p.nt_fc1;
-          set_pf(p.fc1, p.F, H, p.nt_fc1, p.c_fc1, p.F);
+          set_pf(p.lay.fc1, p.F, H, p.nt_fc1, p.lay.c_fc1, p.F);
           break;
         case 7:  // x += h W2^T
-          g.X = p.hbuf; g.W = reinterpret_cast<const uint4*>(lb + p.fc2); g.N = H; g.K = p.F; g.c1 = nullptr; g.c2 = nullptr;
+          g.X = p.hbuf; g.W = reinterpret_cast<const uint4*>(lb + p.lay.fc2); g.N = H; g.K = p.F; g.c1 = nullptr; g.c2 = nullptr;
           g.epi = EPI_RESIDUAL; g.R = p.x; g.Y = p.x; g.ldy = ld;
-          set_pf(p.fc2, H, p.F, p.nt_h, 0, 0);
+          set_pf(p.lay.fc2, H, p.F, p.nt_h, 0, 0);
           break;
         default:  // final LayerNorm + K lm heads -> f32 logits [B, K*V]
-          g.X = p.x; g.W = reinterpret_cast<const uint4*>(blob + p.heads); g.N = p.K * p.V; g.K = H;
-          g.c1 = reinterpret_cast<const float*>(blob + p.c_heads); g.c2 = g.c1 + p.K * p.V;
+          g.X = p.x; g.W = reinterpret_cast<const uint4*>(blob + p.lay.heads); g.N = p.K * p.V; g.K = H;
+          g.c1 = reinterpret_cast<const float*>(blob + p.lay.c_heads); g.c2 = g.c1 + p.K * p.V;
           g.epi = EPI_F32; g.R = nullptr; g.Y = p.logits; g.ldy = (int64_t)p.K * p.V;
           nt = p.nt_heads;
           break;
@@ -512,12 +515,41 @@ __global__ void __launch_bounds__(ST_THREADS, 1) decode_step_kernel(const __grid
 }
 
 // ---- host side ----------------------------------------------------------------------------------
-int step_smem_bytes(const StepParams& p) {
-  return (int)(ST_HEADER + p.tile_region_bytes);
+// Largest n-tile count among run_gemm's instantiations that keeps ~one task per CTA.
+static int pick_nt(int ntiles, int grid) {
+  const int cand[4] = {4, 3, 2, 1};
+  for (int i = 0; i < 4; i++)
+    if (ntiles % cand[i] == 0 && ntiles / cand[i] >= (grid * 8) / 10) return cand[i];
+  for (int i = 0; i < 4; i++)
+    if (ntiles % cand[i] == 0 && ntiles / cand[i] >= grid / 2) return cand[i];
+  return 1;
+}
+
+const char* plan_decode_step(StepParams& p, int grid) {
+  p.nt_qkv = pick_nt(p.qkv_rows / 8, grid);
+  p.nt_h = pick_nt(p.H / 8, grid);
+  p.nt_fc1 = pick_nt(p.F / 8, grid);
+  p.nt_heads = pick_nt(p.K * p.V / 8, grid);
+  const int ntmax = std::max({p.nt_qkv, p.nt_h, p.nt_fc1, p.nt_heads});
+  const int64_t tile = (int64_t)32 * (p.H + 8) * 2;                  // one activation tile buffer (stage_tile)
+  const int64_t red = (int64_t)ST_WARPS * 32 * (8 * ntmax + 8) * 4;  // K-reduction scratch [8 warps][32][RS] (gemm_tasks)
+  // weight buffer: the largest per-task slice (nt n-tiles x K, 16 bytes per (n-tile, k-pair) fragment row)
+  const int64_t wbytes = 16 * std::max({(int64_t)p.nt_qkv * p.H, (int64_t)p.nt_h * p.F, (int64_t)p.nt_fc1 * p.H, (int64_t)p.nt_heads * p.H});
+  const int64_t att = (int64_t)ST_WARPS * attn_decode_smem_per_warp<bf16>() + (ST_WARPS / 2) * 128 * 4;  // attn_phase: per-warp scratch + pair exchange
+  const int64_t budget = ST_SMEM_LIMIT - ST_HEADER;
+  p.nbuf = (2 * tile + wbytes <= budget) ? 2 : 1;
+  if (p.nbuf * tile < red) return "the K-reduction scratch does not fit the activation tile";
+  p.wbuf_offset = align_up(p.nbuf * tile, 128);
+  const int64_t region = align_up(std::max(p.wbuf_offset + wbytes, att), 16);
+  if (region > budget) return "tile + weight slice exceed the shared memory of an SM";
+  p.tile_region_bytes = region;
+  p.sample_items = (p.V + 255) / 256;
+  if (p.sample_items > 9) return "vocab_size > 2304";  // decode_step_kernel's largest sampler instantiation
+  return nullptr;
 }
 
 int launch_decode_step(const StepParams& p, int grid, cudaStream_t st) {
-  const int smem = step_smem_bytes(p);
+  const int smem = (int)(ST_HEADER + p.tile_region_bytes);
   void* args[] = {(void*)&p};
   const void* fn;
   if (p.sample_items <= 1) fn = (const void*)decode_step_kernel<1>;
@@ -526,7 +558,7 @@ int launch_decode_step(const StepParams& p, int grid, cudaStream_t st) {
   static int attr_done[3] = {0, 0, 0};
   const int fi = p.sample_items <= 1 ? 0 : (p.sample_items <= 5 ? 1 : 2);
   if (!attr_done[fi]) {
-    PTTS_CHECK_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024));  // (+ 256 B of static shared memory: the sampler scratch)
+    PTTS_CHECK_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, ST_SMEM_LIMIT));
     attr_done[fi] = 1;
   }
   PTTS_CHECK_CUDA(cudaLaunchCooperativeKernel(fn, dim3(grid), dim3(ST_THREADS), args, (size_t)smem, st));

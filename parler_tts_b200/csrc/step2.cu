@@ -21,7 +21,7 @@
 //     (row, head) items run inside the same phase: QKV -> self-attention and q_cross -> cross-attention need no device-wide barrier
 //     between them.  6 barriers per layer instead of 8.  A warp carries 12 QKV n-tiles (4 q_cross) in two passes of 6 (2): the
 //     head's 192 KB QKV slice of a rank streams through the 2 x 64 KB weight ring as four jobs.
-//   * weights: one contiguous slice per (phase, cluster, rank) (layout.h cpack, built once by ptts_decoder_finalize), streamed by
+//   * weights: one contiguous slice per (phase, cluster, rank) (layout.h cluster_phase, built once by ptts_decoder_finalize), streamed by
 //     ONE bulk copy per job into a 2 x 64 KB ring two jobs ahead, with an L2 evict-first policy like the K/V rows (1.2 GB per token
 //     must not evict the kernel's own instructions and the small reused tensors).  No HBM -> L2 prefetch: the ring already runs two
 //     jobs ahead of its consumer, and every cp.async.bulk.prefetch.L2 costs issue time inside a phase.
@@ -169,16 +169,16 @@ __device__ __forceinline__ bool weight_job(const StepParams& p, int j, int cta, 
     const int ph = jl < QKV_JOBS ? 0 : jl - (QKV_JOBS - 1);
     // the head phases' slices are shared by the four row-block clusters of a head: indexed (head, rank)
     const int64_t idx = (ph == PH_QKV || ph == PH_QC) ? (int64_t)(cta >> 3) * C + rank : (int64_t)cta;
-    const int64_t sz = p.cp_slice[ph];
+    const int64_t sz = p.lay.cp_slice[ph];
     bytes = (uint32_t)(ph == PH_QKV ? sz / QKV_JOBS : sz);
-    src = p.blob + p.layer0 + p.layer_stride * l + p.cp[ph] + idx * sz + (ph == PH_QKV ? jl * (sz / QKV_JOBS) : 0);
+    src = p.blob + p.lay.layer0 + p.lay.layer_stride * l + p.lay.cp[ph] + idx * sz + (ph == PH_QKV ? jl * (sz / QKV_JOBS) : 0);
     return true;
   }
   const int task = cta + (int)gridDim.x * (j - nl);
   const int ntasks = p.K * p.V / 32;
   if (task >= ntasks) return false;
   bytes = (uint32_t)(4 * p.H * 16);  // 4 n-tiles x K (fragment order: 16 B per (n-tile, k-pair) lane row)
-  src = p.blob + p.heads + (int64_t)task * bytes;
+  src = p.blob + p.lay.heads + (int64_t)task * bytes;
   return true;
 }
 
@@ -308,7 +308,7 @@ __global__ void __launch_bounds__(THREADS, 1) decode_step_cluster_kernel(const _
     const int l = ph / 6, sub = ph - 6 * l;
     prof = prof0 ? prof0 + (size_t)(ph + 1) * PROF_STRIDE : nullptr;
     prof_mark(prof, 0);
-    const char* lb = blob + p.layer0 + p.layer_stride * l;
+    const char* lb = blob + p.lay.layer0 + p.lay.layer_stride * l;
     const bool rowpart = (sub == PH_QKV || sub == PH_QC);
     const bool has_ln = (sub == PH_QKV || sub == PH_QC || sub == PH_FC1);
     // n-tiles per warp: head phases per pass (two passes: QKV 2 x 6 of the head's 24, q_cross 2 x 2 of its 8), otherwise per destination
@@ -342,9 +342,9 @@ __global__ void __launch_bounds__(THREADS, 1) decode_step_cluster_kernel(const _
     float cv1 = 0.f, cv2 = 0.f;
     if (has_ln) {
       const float* c1; int ntot;
-      if (sub == PH_QKV) { c1 = reinterpret_cast<const float*>(lb + p.c_qkv); ntot = p.qkv_rows; }
-      else if (sub == PH_QC) { c1 = reinterpret_cast<const float*>(lb + p.c_qc); ntot = H; }
-      else { c1 = reinterpret_cast<const float*>(lb + p.c_fc1); ntot = F; }
+      if (sub == PH_QKV) { c1 = reinterpret_cast<const float*>(lb + p.lay.c_qkv); ntot = p.qkv_rows; }
+      else if (sub == PH_QC) { c1 = reinterpret_cast<const float*>(lb + p.lay.c_qc); ntot = H; }
+      else { c1 = reinterpret_cast<const float*>(lb + p.lay.c_fc1); ntot = F; }
       const int nown = rowpart ? Nc : 8 * q;
       if (tid < nown) {
         int n;
@@ -610,7 +610,7 @@ __global__ void __launch_bounds__(THREADS, 1) decode_step_cluster_kernel(const _
   prof_mark(prof, 0);
   {
     const int ntasks = p.K * p.V / 32;
-    const float* c1 = reinterpret_cast<const float*>(blob + p.c_heads);
+    const float* c1 = reinterpret_cast<const float*>(blob + p.lay.c_heads);
     const float* c2 = c1 + p.K * p.V;
     mbar_wait(abar, par_a, 3);
     par_a ^= 1u;
@@ -759,17 +759,12 @@ __global__ void cluster_pack_kernel(const uint4* __restrict__ src, uint4* __rest
 }  // namespace cl
 
 // ---- host side ----------------------------------------------------------------------------------
-int cluster_pack_layer(const char* layer_src, char* layer_dst, const int64_t* mat_off, const int64_t* cp_off, int nh, int H, int F, cudaStream_t st) {
-  // mat_off: byte offsets (inside the layer) of wqkv, wo, wqc, woc, fc1, fc2; cp_off: of the six packed regions
-  const int ks = H / cl::C / 32, ksf = F / cl::C / 32;
-  const int ntc[6] = {24, 2, 8, 2, F / (4 * nh) / 8, 2};
-  const int owners[6] = {nh, 4 * nh, nh, 4 * nh, 4 * nh, 4 * nh};
+int cluster_pack_layer(const DecoderLayout& L, char* layer, cudaStream_t st) {
   for (int ph = 0; ph < 6; ph++) {
-    const int kts = (ph == 5) ? ksf : ks;
-    const int KT_src = (ph == 5) ? F / 32 : H / 32;
-    const int64_t tiles = (int64_t)owners[ph] * cl::C * ntc[ph] * kts;
-    cl::cluster_pack_kernel<<<(unsigned)tiles, 32, 0, st>>>(reinterpret_cast<const uint4*>(layer_src + mat_off[ph]),
-                                                            reinterpret_cast<uint4*>(layer_dst + cp_off[ph]), ph, nh, ntc[ph], kts, KT_src);
+    const ClusterPhase cp = cluster_phase(L, ph);
+    const int64_t tiles = (int64_t)cp.owners * cl::C * cp.nt * cp.kt;
+    cl::cluster_pack_kernel<<<(unsigned)tiles, 32, 0, st>>>(reinterpret_cast<const uint4*>(layer + cp.mat),
+                                                            reinterpret_cast<uint4*>(layer + L.cp[ph]), ph, L.nh, cp.nt, cp.kt, cp.kt_src);
   }
   PTTS_LAUNCH_CHECK();
   return PTTS_OK;

@@ -12,7 +12,7 @@ namespace ptts {
 // row's current ids added left to right with a bf16 rounding after each add, then the position embedding (models without
 // rope).  Codebooks go in groups of 8: the loads of a group are in flight together, and the group's values are all that is live.
 __device__ __forceinline__ float embed_value(const StepParams& p, int row, int col, int pos) {
-  const bf16* tables = reinterpret_cast<const bf16*>(p.blob + p.embed);
+  const bf16* tables = reinterpret_cast<const bf16*>(p.blob + p.lay.embed);
   float v = 0.f;
 #pragma unroll 1
   for (int k0 = 0; k0 < p.K; k0 += 8) {
@@ -24,7 +24,7 @@ __device__ __forceinline__ float embed_value(const StepParams& p, int row, int c
     for (int k = 0; k < 8; k++)
       if (k0 + k < p.K) v = (k0 + k == 0) ? ev[k] : DT<bf16>::rnd(v + ev[k]);
   }
-  if (!p.rope) v = DT<bf16>::rnd(v + __bfloat162float(reinterpret_cast<const bf16*>(p.blob + p.pos)[(size_t)pos * p.H + col]));
+  if (!p.rope) v = DT<bf16>::rnd(v + __bfloat162float(reinterpret_cast<const bf16*>(p.blob + p.lay.pos)[(size_t)pos * p.H + col]));
   return v;
 }
 
@@ -35,7 +35,7 @@ __device__ __forceinline__ AttnArgs decode_attn_args(const StepParams& p, int l,
   AttnArgs a{};
   a.ctrl = nullptr; a.B = p.B; a.nh = p.nh; a.q_len = 1;
   a.past_from_ctrl = 0; a.past_len = pos; a.prefix = p.P;
-  a.rope = p.rope; a.rope_cos = p.blob + p.rope_cos; a.rope_sin = p.blob + p.rope_sin; a.scale = p.scale;
+  a.rope = p.rope; a.rope_cos = p.blob + p.lay.rope_cos; a.rope_sin = p.blob + p.lay.rope_sin; a.scale = p.scale;
   if (!cross) {
     char* kc = p.self_kv + p.self_layer_stride * l;
     a.kcache = kc; a.vcache = kc + (size_t)p.B * p.nkv * p.Tmax * HD * 2;

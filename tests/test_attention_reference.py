@@ -19,7 +19,6 @@ from __future__ import annotations
 import ctypes as C
 import dataclasses
 import math
-import os
 
 import numpy as np
 import pytest
@@ -580,8 +579,6 @@ def test_decode_sweep_against_fp64(kind, n, dt, record_property):
 @pytest.mark.parametrize("kind,n,dt,sweep", PREFILL_IDS,
                          ids=[f"{k}-n{n}-{d}-{'tc' if s == 0 else 'item'}" for k, n, d, s in PREFILL_IDS])
 def test_prefill_sweep_against_fp64(kind, n, dt, sweep, record_property):
-    if sweep == 0 and os.environ.get("PTTS_PREFILL_ATTN_TC", "1").startswith("0"):
-        pytest.skip("PTTS_PREFILL_ATTN_TC=0: the decoder's prefill sweep is attention_item")
     check_against_reference(_prefill_case(kind, n, dt, sweep), record_property)
 
 
