@@ -206,16 +206,59 @@ __host__ __device__ constexpr int attn_decode_smem_per_warp() {
   return 2 * 2 * CH * HD * (int)sizeof(T) + (3 * HD) * (int)sizeof(float);
 }
 
+// chunks of `n_cached` cached keys that fall to warp `part` of `nparts` (chunk c of the item belongs to warp c % nparts)
+__host__ __device__ __forceinline__ int attn_decode_warp_chunks(int n_cached, int CH, int part, int nparts) {
+  const int n_chunks_all = (n_cached + CH - 1) / CH;
+  return (n_chunks_all > part) ? (n_chunks_all - part + nparts - 1) / nparts : 0;
+}
+
+// TMA: this warp's i-th chunk of the item's cached rows -> one ring stage ([CH][64] K | [CH][64] V), bytes completing on `bar`
+template <typename T, int CH>
+__device__ __forceinline__ void attn_decode_issue_chunk(const T* kc, const T* vc, int n_cached, int i, int part, int nparts, T* stage, uint64_t* bar_p, int lane) {
+  const int t0 = (part + nparts * i) * CH;
+  const int n = (n_cached - t0 < CH) ? (n_cached - t0) : CH;
+  const uint32_t bar = smem_u32(bar_p);
+  if (lane == 0) mbar_expect_tx(bar, (uint32_t)(2 * n * HD * sizeof(T)));
+  __syncwarp();
+  if (lane < 2) {  // one bulk copy for the K rows, one for the V rows (rows of an item are contiguous)
+    const T* src = (lane == 0 ? kc : vc) + (size_t)t0 * HD;
+    T* dst = stage + (lane == 0 ? 0 : CH * HD);
+    // (written out rather than through bulk_g2s: the wrapper call reorders ptxas's schedule of attention_decode_kernel)
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                 ::"r"(smem_u32(dst)), "l"(src), "r"((uint32_t)(n * HD * sizeof(T))), "r"(bar) : "memory");
+  }
+}
+
+// The REQUEST of an item's first chunk, apart from its sweep: a caller that knows the item before it has the query (the cluster
+// step kernel at the top of a head phase) sends the warp's first K/V chunk into `stage0` here and passes pre_issued = true to
+// attention_decode_sweep, which then waits for it without having asked.  Same copies onto the same mbarrier (bars[0]) as the
+// sweep's own request; a warp without cached keys requests nothing and its parity does not move.  No proxy fence: the caller
+// gives a stage that, since the last fence.proxy.async ordered before this call, has only been written by bulk copies.
+// Self-attention reads rows < pos only, which earlier tokens stored (the row of `pos` never comes from the cache in its own step).
 template <typename T, int CH = AttChunk<T>::CH>
-__device__ __forceinline__ void attention_decode_item_warp(const AttnArgs& p, int b, int kvh, int pos, unsigned char* sm_warp, uint64_t* bars,
-                                                           int lane, uint32_t& parity, int part = 0, int nparts = 1, float* xch = nullptr,
-                                                           int pair_bar = 0) {
+__device__ __forceinline__ void attention_decode_request(const AttnArgs& p, int b, int kvh, int pos, unsigned char* stage0, uint64_t* bars, int lane,
+                                                         int part, int nparts) {
+  const T* kc = reinterpret_cast<const T*>(p.kcache) + (size_t)b * p.kv_b_stride + (size_t)kvh * p.kv_h_stride;
+  const T* vc = reinterpret_cast<const T*>(p.vcache) + (size_t)b * p.kv_b_stride + (size_t)kvh * p.kv_h_stride;
+  const int n_cached = p.cross ? p.kv_len : pos;
+  if (attn_decode_warp_chunks(n_cached, CH, part, nparts) > 0)
+    attn_decode_issue_chunk<T, CH>(kc, vc, n_cached, 0, part, nparts, reinterpret_cast<T*>(stage0), &bars[0], lane);
+}
+
+// stage0: ring stage 0 ([CH][64] K | [CH][64] V); rest: ring stage 1 (same layout), then 192 floats (query, this step's key and
+// value).  The two may lie anywhere in shared memory (16-byte aligned).  pre_issued: attention_decode_request has been called
+// for this item.  prof: optional profile row; slot 11 takes lane 0's clock64 when the item's first stage has landed.
+template <typename T, int CH = AttChunk<T>::CH>
+__device__ __forceinline__ void attention_decode_sweep(const AttnArgs& p, int b, int kvh, int pos, unsigned char* stage0, unsigned char* rest, uint64_t* bars,
+                                                       int lane, uint32_t& parity, int part = 0, int nparts = 1, float* xch = nullptr,
+                                                       int pair_bar = 0, bool pre_issued = false, long long* prof = nullptr) {
   // part / nparts: the item's cached keys are split between `nparts` warps (chunk c belongs to warp c % nparts);
   // partial (max, sum, accumulator) triples are merged through `xch` with a 64-thread named barrier `pair_bar`.
   constexpr int STAGE_ELEMS = CH * HD;  // per K (or V) stage
-  T* kst = reinterpret_cast<T*>(sm_warp);                   // [2][CH][64]
-  T* vst = kst + 2 * STAGE_ELEMS;                            // [2][CH][64]
-  float* qs = reinterpret_cast<float*>(vst + 2 * STAGE_ELEMS);  // [64] query
+  T* const st0 = reinterpret_cast<T*>(stage0);               // [CH][64] K | [CH][64] V
+  // stage 1 = st0 + st_step (an offset, not a second pointer: on one contiguous scratch it is a constant)
+  const int st_step = (int)(reinterpret_cast<T*>(rest) - st0);
+  float* qs = reinterpret_cast<float*>(rest + 2 * STAGE_ELEMS * sizeof(T));  // [64] query
   float* kn = qs + HD;                                       // [64] this step's key   (self only)
   float* vn = kn + HD;                                       // [64] this step's value (self only)
   // bars[2]: this warp's mbarriers, initialised ONCE per kernel in memory that is never aliased (re-initialising
@@ -227,23 +270,10 @@ __device__ __forceinline__ void attention_decode_item_warp(const AttnArgs& p, in
   T* vc = reinterpret_cast<T*>(p.vcache) + (size_t)b * p.kv_b_stride + (size_t)kvh * p.kv_h_stride;
   const int lo = lane, hi = lane + HD / 2;
   const int n_cached = p.cross ? p.kv_len : pos;  // keys that come from the cache
-  const int n_chunks_all = (n_cached + CH - 1) / CH;
-  const int n_chunks = (n_chunks_all > part) ? (n_chunks_all - part + nparts - 1) / nparts : 0;  // chunks of THIS warp
+  const int n_chunks = attn_decode_warp_chunks(n_cached, CH, part, nparts);  // chunks of THIS warp
 
-  auto issue = [&](int i) {  // TMA: this warp's i-th chunk -> stage i&1
-    const int st = i & 1;
-    const int t0 = (part + nparts * i) * CH;
-    const int n = (n_cached - t0 < CH) ? (n_cached - t0) : CH;
-    const uint32_t bar = smem_u32(&bars[st]);
-    if (lane == 0) mbar_expect_tx(bar, (uint32_t)(2 * n * HD * sizeof(T)));
-    __syncwarp();
-    if (lane < 2) {  // one bulk copy for the K rows, one for the V rows (rows of an item are contiguous)
-      const T* src = (lane == 0 ? kc : vc) + (size_t)t0 * HD;
-      T* dst = (lane == 0 ? kst : vst) + st * STAGE_ELEMS;
-      // (written out rather than through bulk_g2s: the wrapper call reorders ptxas's schedule of attention_decode_kernel)
-      asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                   ::"r"(smem_u32(dst)), "l"(src), "r"((uint32_t)(n * HD * sizeof(T))), "r"(bar) : "memory");
-    }
+  auto issue = [&](int i) {  // this warp's i-th chunk -> stage i&1
+    attn_decode_issue_chunk<T, CH>(kc, vc, n_cached, i, part, nparts, st0 + (i & 1) * st_step, &bars[i & 1], lane);
   };
   auto wait_stage = [&](int st) {
     const uint32_t bar = smem_u32(&bars[st]);
@@ -258,9 +288,14 @@ __device__ __forceinline__ void attention_decode_item_warp(const AttnArgs& p, in
 
   // all lanes are past their shared-memory reads of the previous item: the ring may be refilled
   __syncwarp();
-  fence_proxy_async_smem();
-  if (n_chunks > 0) issue(0);
-  if (n_chunks > 1) issue(1);
+  if (!pre_issued) {
+    fence_proxy_async_smem();
+    if (n_chunks > 0) issue(0);
+    if (n_chunks > 1) issue(1);
+  } else if (n_chunks > 1) {  // stage 0 is in flight or has landed; a warp with one chunk has nothing to ask for (and no fence to wait in)
+    fence_proxy_async_smem();
+    issue(1);
+  }
 
   // the first query head's elements are requested before the K/V append below (its stores would otherwise order the loads
   // behind a second L2 round trip)
@@ -380,7 +415,9 @@ __device__ __forceinline__ void attention_decode_item_warp(const AttnArgs& p, in
       const int n = (n_cached - t0 < CH) ? (n_cached - t0) : CH;
       const int mk = mask_bits(t0);
       wait_stage(st);
-      process(kst + st * STAGE_ELEMS, vst + st * STAGE_ELEMS, __ballot_sync(0xffffffffu, mk != 0), n);
+      if (prof != nullptr && c == 0 && rr == 0 && lane == 0) prof[11] = clock64();
+      const T* stg = st0 + st * st_step;
+      process(stg, stg + STAGE_ELEMS, __ballot_sync(0xffffffffu, mk != 0), n);
       if (c + 2 < n_chunks) {
         __syncwarp();
         fence_proxy_async_smem();
@@ -445,6 +482,14 @@ __device__ __forceinline__ void attention_decode_item_warp(const AttnArgs& p, in
       store8(reinterpret_cast<T*>(p.out) + (size_t)b * p.ldo + h * HD + d0, o);
     }
   }
+}
+
+// Request and sweep back to back on one contiguous scratch of attn_decode_smem_per_warp<T>() bytes: stage 0 | stage 1 | 192 floats.
+template <typename T, int CH = AttChunk<T>::CH>
+__device__ __forceinline__ void attention_decode_item_warp(const AttnArgs& p, int b, int kvh, int pos, unsigned char* sm_warp, uint64_t* bars,
+                                                           int lane, uint32_t& parity, int part = 0, int nparts = 1, float* xch = nullptr,
+                                                           int pair_bar = 0) {
+  attention_decode_sweep<T, CH>(p, b, kvh, pos, sm_warp, sm_warp + 2 * CH * HD * sizeof(T), bars, lane, parity, part, nparts, xch, pair_bar);
 }
 
 // ---- decode attention on the tensor cores (bf16, MHA: one query head per K/V head) -----------------------------------------

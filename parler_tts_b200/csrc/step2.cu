@@ -27,7 +27,9 @@
 //     jobs ahead of its consumer, and every cp.async.bulk.prefetch.L2 costs issue time inside a phase.
 //   * fc2 (one n-tile per destination, half of F = 128 KB of activations): staged in two quarters of F, one after the other; a
 //     warp's accumulators carry its residue class from the first quarter into the second.
-//   * attention: the sweep step.cu's attention phase runs (attention_decode_item_warp, two warps per item, 32-key chunks).
+//   * attention: the sweep step.cu's attention phase runs (attention_decode_sweep, two warps per item, 32-key chunks).  Every
+//     warp's first K/V chunk is requested at the TOP of the head phase into a stage nothing else touches during the phase, so the
+//     HBM round trip runs under the weights wait, the MMAs, the exchange and the epilogue instead of after them.
 //   * the activation slice of the next phase is requested by the barrier's polling thread the moment the barrier opens; the
 //     per-phase cluster barrier that guards buffer reuse arrives .relaxed (its default .release is a gpu-scope MEMBAR per warp).
 //   * one launch runs up to StepParams.n_steps tokens: cur_len, the unfinished count and the stop decision advance on the device.
@@ -63,7 +65,11 @@ constexpr int R_OFF = HDR + 2 * WB_BYTES;
 //   fc1   : 32.5 KB slice, receive slots 8 x (256 B stats + 32 x 34 floats) = 36 KB: [32.5 KB, 68.5 KB)
 //   fc2   : 64.5 KB quarter slice, receive slots 8 x (256 B + 32 x 8 floats): [64.5 KB, 74.5 KB)
 //   QKV   : 8.1 KB slice, receive slots 16 x (32 B stats + 4 x 96 floats) = 24.5 KB: [8.1 KB, 32.6 KB), q|k|v at QKV_OFF; the
-//           attention scratch of warps 0-4 below QKV_OFF
+//           first K/V stage of attention warps 0-5 in [34 KB, 82 KB), idle for the whole phase (warps 6, 7: the last 8 KB of the
+//           two weight buffers, which no job of the phase reaches)
+//   q_cross: 8.1 KB slice, receive slots 16 x (32 B + 4 x 32 floats) = 8.5 KB: [8.1 KB, 16.6 KB), q at QKV_OFF; the first K/V
+//           stage of all eight attention warps in [24 KB, 88 KB)
+//   both head phases: the second K/V stage + 192 floats of attention warps 0, 1 from R's start (over the dead slice and slots)
 //   lm heads: the whole x image (65 KB)
 constexpr int R_BYTES = 92160;
 constexpr int QKV_OFF = R_BYTES - 2048;   // [4 rows][192] bf16 q|k|v (or [4][64] q_cross) of this rank's attention items
@@ -71,7 +77,19 @@ constexpr int SMEM_BYTES = R_OFF + R_BYTES;
 static_assert(SMEM_BYTES + 1024 <= 227 * 1024, "cluster step kernel shared memory");
 static_assert(ROWS * (1024 / 2 + 8) * 2 + V * (256 + ROWS * 34 * 4) <= R_BYTES, "fc1 plan");
 static_assert(HROWS * (1024 / 2 + 8) * 2 + V * C * (32 + 4 * 96 * 4) <= QKV_OFF, "QKV plan");
-static_assert(5 * ATT_SMEM <= QKV_OFF && 3 * ATT_SMEM <= WB_BYTES && 16384 + 4 * 128 * 4 <= WB_BYTES, "attention plan");
+// Attention plan of the head phases.  A warp's first K/V stage is requested at the top of the phase and read at its end, so it
+// lies where neither the slice, the receive slots, q|k|v, a weight job of the phase (QKV: four of 48 KB and out-proj's 16 KB;
+// q_cross fills one buffer, so its stages are all in R) nor the pair-merge scratch reaches.  The rest of a warp's scratch (second
+// stage + 192 floats) is first touched when the attention starts: warps 0, 1 at R's start, warps 2-7 in the held weight buffer.
+constexpr int ATT_STAGE = 2 * 32 * HD * 2;         // one K/V stage: 32 keys x (K row + V row)
+constexpr int ATT_REST = ATT_SMEM - ATT_STAGE;     // second stage + 192 floats
+constexpr int ATT_S0_QKV = 34 * 1024;              // R offset of warp 0's first stage, QKV phase (warps 0-5)
+constexpr int ATT_S0_QC = QKV_OFF - V * ATT_STAGE; // R offset of warp 0's first stage, q_cross phase (warps 0-7)
+constexpr int ATT_S0_WB = WB_BYTES - ATT_STAGE;    // weight-buffer offset of the first stage of warps 6 (buffer 0) and 7 (buffer 1), QKV phase
+static_assert(HROWS * (1024 / 2 + 8) * 2 + V * C * (32 + 4 * 96 * 4) <= ATT_S0_QKV && ATT_S0_QKV + 6 * ATT_STAGE <= QKV_OFF, "attention plan: QKV stages in R");
+static_assert(HROWS * (1024 / 2 + 8) * 2 + V * C * (32 + 4 * 32 * 4) <= ATT_S0_QC, "attention plan: q_cross stages in R");
+static_assert(2 * ATT_REST <= ATT_S0_QC && 2 * ATT_REST <= ATT_S0_QKV && 6 * ATT_REST <= ATT_S0_WB, "attention plan: second stages");
+static_assert(6 * 8 * (1024 / 2) * 2 <= ATT_S0_WB && 16384 + 4 * 128 * 4 <= ATT_S0_WB, "attention plan: QKV weight jobs, out-proj job + pair merge");
 static_assert(ROWS * (4096 / 4 + 8) * 2 + V * (256 + ROWS * 8 * 4) <= R_BYTES, "fc2 plan");
 
 // ---- PTX helpers used by this kernel only (ptx.cuh has the shared ones) ------------------------------
@@ -337,6 +355,20 @@ __global__ void __launch_bounds__(THREADS, 1) decode_step_cluster_kernel(const _
     const int j0 = JOBS_PER_LAYER * l + (sub == 0 ? 0 : sub + QKV_JOBS - 1);   // first weight job of this phase
     if (tid == 0) mbar_expect_tx(xbar, xbytes);
 
+    // Head phases: this warp's first K/V chunk is requested NOW, so that it lands while the projection runs (the attention at the
+    // end of the phase otherwise starts with every warp of the grid waiting for a cold HBM read).  What it reads does not depend
+    // on this token: cross-attention rows were written by the prefill; self-attention reads rows < pos, each stored by an earlier
+    // token and followed there by fence.proxy.async.global + a device-wide barrier (grid_sync) -- with several tokens per launch
+    // too, 6 L barriers lie between a token's append and the next token's request -- and row `pos` comes from shared memory.
+    // No fence.proxy.async: thread 0's fence when the last barrier opened (request_slice) is ordered before this by the
+    // barrier's closing __syncthreads, and only bulk copies write the stage from then to the end of the attention.
+    auto att_stage0 = [&]() -> unsigned char* {   // (computed at each use: nothing more is carried across the MMA loop)
+      if (sub == PH_QC) return Rg + ATT_S0_QC + warp * ATT_STAGE;
+      return warp < 6 ? Rg + ATT_S0_QKV + warp * ATT_STAGE : smem + HDR + (warp - 6) * WB_BYTES + ATT_S0_WB;
+    };
+    if (rowpart && att_row < B)
+      attention_decode_request<bf16>(decode_attn_args(p, l, pos, sub == PH_QC), att_row, head, pos, att_stage0(), attbars + 2 * warp, lane, warp & 1, 2);
+
     // folded-LayerNorm vectors of this phase's features: requested now, parked in shared memory after the MMA loop (a global
     // load followed at once by its shared-memory store would park the warp for an L2 round trip in front of the MMAs)
     float cv1 = 0.f, cv2 = 0.f;
@@ -565,14 +597,17 @@ __global__ void __launch_bounds__(THREADS, 1) decode_step_cluster_kernel(const _
         att.ldo = pitch;
         att.out = a_img + (size_t)att_slice * x_slice_elems + att_col - (size_t)head * HD;
         if (sub == PH_QKV) { att.knew = qbase; att.vnew = qbase; att.ldkv = Nc; att.k_col0 = HD; att.v_col0 = 2 * HD; }
-        // per-warp scratch (K/V ring stages, then 192 floats): warps 0-4 in R below the q|k|v rows, warps 5-7 in the weight buffer
-        // whose job is held back; the pair merge in the other buffer's tail, behind out-proj's / cross out-proj's 16 KB
+        // the first K/V stage is where the top of the phase asked for it; the rest of a warp's scratch (second stage, then 192
+        // floats): warps 0, 1 at R's start, warps 2-7 in the weight buffer whose job is held back; the pair merge in the other
+        // buffer behind out-proj's / cross out-proj's 16 KB
         unsigned char* wb0 = smem + HDR;
         unsigned char* held = wb0 + ((sub == PH_QKV ? j0 + 1 : j0) & 1) * WB_BYTES;
         unsigned char* other = wb0 + ((sub == PH_QKV ? j0 : j0 + 1) & 1) * WB_BYTES;
-        unsigned char* region = warp < 5 ? Rg + (size_t)warp * ATT_SMEM : held + (size_t)(warp - 5) * ATT_SMEM;
+        unsigned char* rest = warp < 2 ? Rg + (size_t)warp * ATT_REST : held + (size_t)(warp - 2) * ATT_REST;
         float* xr = reinterpret_cast<float*>(other + 16384) + (warp >> 1) * 128;
-        attention_decode_item_warp<bf16>(att, att_row, head, pos, region, attbars + 2 * warp, lane, att_parity, warp & 1, 2, xr, (warp >> 1) + 1);
+        prof_mark(prof, 10);
+        attention_decode_sweep<bf16>(att, att_row, head, pos, att_stage0(), rest, attbars + 2 * warp, lane, att_parity, warp & 1, 2, xr, (warp >> 1) + 1,
+                                     true, tid == 0 ? prof : nullptr);
       }
       prof_mark(prof, 5);
     }

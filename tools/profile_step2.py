@@ -4,6 +4,7 @@ Each value profiles one step at its own cached length (T = bench.P_LEN + steps +
 tools_out/step2_phases.json."""
 import json
 import os
+import subprocess
 import sys
 
 import numpy as np
@@ -48,7 +49,7 @@ def profile(steps_before):
     T = bench.P_LEN + steps_before + 2
     print(f"\nstep (event) {e0.elapsed_time(e1) * 1e3:.1f} us ; T = {T} cached keys")
     print("per phase (us, mean over 24 layers, CTA 0): wait = phase start -> slice + weights landed | mma | exch = partials sent and received |"
-          " epi | attn | barrier = done -> released")
+          " epi | attn (head phases: kv_wait = attention entered -> thread 0's first K/V stage landed) | barrier = done -> released")
     out = {}
     tot_l = 0.0
     for sub in range(6):
@@ -59,13 +60,16 @@ def profile(steps_before):
         work = us(rows[:, 6] - rows[:, 0])
         # inside the MMA span: QKV's wait for its second-pass weights, fc2's wait for its second quarter of F (stamps 8 -> 9)
         inner = us(rows[:, 9] - rows[:, 8]) if sub in (0, 5) else np.zeros(NL)
+        kv_wait = us(rows[:, 11] - rows[:, 10]) if sub in (0, 2) else np.zeros(NL)   # stamps 10 -> 11
         out[names[sub]] = dict(work=work.mean(), barrier=barr.mean(), wait=wait.mean(), mma=mma.mean(), exch=exch.mean(), epi=epi.mean(),
-                               attn=attn.mean(), inner_wait=inner.mean())
+                               attn=attn.mean(), kv_wait=kv_wait.mean(), inner_wait=inner.mean())
         tot_l += work.mean() + barr.mean()
         extra = (f"  [exch: pre {us(rows[:, 12] - rows[:, 2]).mean():.2f} clwait {us(rows[:, 13] - rows[:, 12]).mean():.2f} stage {us(rows[:, 14] - rows[:, 13]).mean():.2f}"
                  f" issue {us(rows[:, 15] - rows[:, 14]).mean():.2f} wait {us(rows[:, 3] - rows[:, 15]).mean():.2f}]")
         if sub in (0, 5):
             extra += f"  [mma: inner wait {inner.mean():.2f}]"
+        if sub in (0, 2):
+            extra += f"  [attn: kv_wait {kv_wait.mean():.2f}]"
         print(f"{names[sub]:20s} work {work.mean():6.2f}  barrier {barr.mean():5.2f} | wait {wait.mean():5.2f}  mma {mma.mean():5.2f}  exch {exch.mean():5.2f}"
               f"  epi {epi.mean():5.2f}  attn {attn.mean():5.2f}{extra}")
     print(f"per layer {tot_l:.1f} us -> {tot_l * NL:.0f} us for {NL} layers")
@@ -87,6 +91,15 @@ def profile(steps_before):
     return dict(T=T, steps_before=steps_before, step_us=e0.elapsed_time(e1) * 1e3, per_layer_us=tot_l, phases_us=out, tail_us=tail)
 
 
+def card():   # what the numbers were measured on (read-only query)
+    try:
+        q = "name,power.limit,clocks.sm,clocks.max.sm,clocks_event_reasons.active"
+        return subprocess.run(["nvidia-smi", "-i", "0", f"--query-gpu={q}", "--format=csv,noheader"], capture_output=True, text=True, timeout=30).stdout.strip()
+    except Exception as ex:
+        return f"nvidia-smi unavailable ({ex!r})"
+
+
 res = [profile(n) for n in befores]
+print(f"\ncard (name, power limit, SM clock, max SM clock, active clock event reasons): {card()}")
 os.makedirs("tools_out", exist_ok=True)
-json.dump({"lib": os.environ.get("PTTS_LIB", "(product)"), "runs": res}, open("tools_out/step2_phases.json", "w"), indent=1)
+json.dump({"lib": os.environ.get("PTTS_LIB", "(product)"), "card": card(), "runs": res}, open("tools_out/step2_phases.json", "w"), indent=1)
