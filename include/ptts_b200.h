@@ -235,6 +235,10 @@ typedef struct ptts_dac_config {
   int32_t n_blocks;            /* 4 */
   int32_t strides[8];          /* 8,8,4,2 */
   int32_t dtype;               /* storage dtype of activations/weights: PTTS_BF16 or PTTS_F32 */
+  /* encoder (descript-audio-codec Encoder / transformers DacEncoder, modeling_dac.py:442-472); encoder_dim = 0: decode only */
+  int32_t encoder_dim;         /* 64: channels after the input conv, doubled by every block */
+  int32_t n_enc_blocks;        /* 4 */
+  int32_t encoder_rates[8];    /* 2,4,8,8: even, <= 32, product = the decoder hop */
 } ptts_dac_config;
 
 int ptts_dac_blob_bytes(const ptts_dac_config* cfg, int64_t* out_bytes);
@@ -248,6 +252,26 @@ int ptts_dac_workspace_bytes(const ptts_dac_config* cfg, int32_t B, int32_t T, i
  * audio [B, 1, hop*T] in cfg->dtype.  = quantizer.from_codes (:138) + model.decode (:139). */
 int ptts_dac_decode(const ptts_dac_config* cfg, const void* blob, void* workspace, int64_t workspace_bytes,
                     const int64_t* codes, int32_t B, int32_t T, void* audio_out, void* stream);
+
+/* ---- DAC encode ------------------------------------------------------------------------------ */
+/* The encoder weights (encoder convs and snake alphas, quantizer in_proj, unit-normalised codebooks) live in a second blob
+ * with its own tensor table; the decode blob above is unchanged.  All of these fail with PTTS_EINVAL when
+ * cfg->encoder_dim == 0, a stride is odd or > 32, or the encoder hop differs from the decoder hop. */
+int ptts_dac_encoder_blob_bytes(const ptts_dac_config* cfg, int64_t* out_bytes);
+int ptts_dac_encoder_num_tensors(const ptts_dac_config* cfg, int32_t* out);
+/* Pack one weight-norm-folded tensor; parler_tts_b200/dac_wrapper.py::_dac_encoder_tensor_list gives the (id -> key)
+ * table.  Load-time only (the reference builds these modules in descript's DAC(), dac_wrapper/modeling_dac.py:24-31). */
+int ptts_dac_encoder_pack(const ptts_dac_config* cfg, void* enc_blob, int32_t name_id, const void* src,
+                          int32_t src_dtype, int64_t numel, void* stream);
+int ptts_dac_encode_workspace_bytes(const ptts_dac_config* cfg, int32_t B, int32_t samples, int64_t* out_bytes);
+/* DACModel.encode (dac_wrapper/modeling_dac.py:33-104): model.preprocess's right zero-pad to the hop (:64) + model.encode
+ * (:95) = encoder + residual vector quantizer over the first n_q codebooks.
+ *   audio [B][samples] in cfg->dtype (channel 0 of input_values);  codes_out [B][n_q][ceil(samples / hop)] int64;
+ *   latents_out: NULL, or the encoder output [B][T][latent_dim] in cfg->dtype (a test hook).
+ * Needs the decode blob too: the quantizer's raw codebooks and out_proj live there. */
+int ptts_dac_encode(const ptts_dac_config* cfg, const void* dec_blob, const void* enc_blob, void* workspace,
+                    int64_t workspace_bytes, const void* audio, int32_t B, int32_t samples, int32_t n_q, int64_t* codes_out,
+                    void* latents_out, void* stream);
 
 #ifdef __cplusplus
 }

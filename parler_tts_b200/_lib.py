@@ -36,7 +36,8 @@ class GenParamsC(C.Structure):
 class DacConfigC(C.Structure):
     _fields_ = [("n_codebooks", C.c_int32), ("codebook_size", C.c_int32), ("codebook_dim", C.c_int32),
                 ("latent_dim", C.c_int32), ("decoder_dim", C.c_int32), ("n_blocks", C.c_int32),
-                ("strides", C.c_int32 * 8), ("dtype", C.c_int32)]
+                ("strides", C.c_int32 * 8), ("dtype", C.c_int32),
+                ("encoder_dim", C.c_int32), ("n_enc_blocks", C.c_int32), ("encoder_rates", C.c_int32 * 8)]
 
 
 # tensor ids (include/ptts_b200.h)
@@ -81,6 +82,11 @@ _SIGS = {
     "ptts_dac_pack": (C.c_int, [C.POINTER(DacConfigC), _VP, _I32, _VP, _I32, _I64, _VP]),
     "ptts_dac_workspace_bytes": (C.c_int, [C.POINTER(DacConfigC), _I32, _I32, C.POINTER(_I64)]),
     "ptts_dac_decode": (C.c_int, [C.POINTER(DacConfigC), _VP, _VP, _I64, _VP, _I32, _I32, _VP, _VP]),
+    "ptts_dac_encoder_blob_bytes": (C.c_int, [C.POINTER(DacConfigC), C.POINTER(_I64)]),
+    "ptts_dac_encoder_num_tensors": (C.c_int, [C.POINTER(DacConfigC), C.POINTER(_I32)]),
+    "ptts_dac_encoder_pack": (C.c_int, [C.POINTER(DacConfigC), _VP, _I32, _VP, _I32, _I64, _VP]),
+    "ptts_dac_encode_workspace_bytes": (C.c_int, [C.POINTER(DacConfigC), _I32, _I32, C.POINTER(_I64)]),
+    "ptts_dac_encode": (C.c_int, [C.POINTER(DacConfigC), _VP, _VP, _VP, _I64, _VP, _I32, _I32, _I32, _VP, _VP, _VP]),
 }
 EXPORTED_SYMBOLS = tuple(_SIGS)
 

@@ -1,5 +1,5 @@
 // api.cu -- the C ABI (include/ptts_b200.h): argument validation, weight packing, the generation
-// session (prefill / decode step / sample / CUDA-graph replay) and DAC decode orchestration.
+// session (prefill / decode step / sample / CUDA-graph replay) and DAC decode / encode orchestration.
 #include <cstdarg>
 #include <cstdlib>
 #include <cstring>
@@ -786,6 +786,153 @@ int ptts_dac_decode(const ptts_dac_config* cfg, const void* blob, void* workspac
   }
   const int cl = C >> cfg->n_blocks;
   return conv(cur, ti + 1, ti + 2, tp(ti), nullptr, audio_out, cl, 1, Tlen, 7, 1, 1);
+}
+
+// ---- DAC encode -----------------------------------------------------------------------------------
+int ptts_dac_encoder_blob_bytes(const ptts_dac_config* cfg, int64_t* out_bytes) {
+  PTTS_REQUIRE(cfg && out_bytes, "null argument");
+  if (int e = validate_dac_encoder(*cfg)) return e;
+  *out_bytes = make_dac_enc_layout(*cfg).total;
+  return PTTS_OK;
+}
+int ptts_dac_encoder_num_tensors(const ptts_dac_config* cfg, int32_t* out) {
+  PTTS_REQUIRE(cfg && out, "null argument");
+  if (int e = validate_dac_encoder(*cfg)) return e;
+  *out = (int32_t)make_dac_enc_layout(*cfg).t.size();
+  return PTTS_OK;
+}
+int ptts_dac_encoder_pack(const ptts_dac_config* cfg, void* enc_blob, int32_t name_id, const void* src, int32_t src_dtype, int64_t numel,
+                          void* stream) {
+  PTTS_REQUIRE(cfg && enc_blob && src, "null argument");
+  if (int e = validate_dac_encoder(*cfg)) return e;
+  PTTS_REQUIRE(src_dtype == PTTS_BF16 || src_dtype == PTTS_F32, "dac encoder pack: src dtype must be bf16 or f32");
+  const DacEncLayout L = make_dac_enc_layout(*cfg);
+  PTTS_REQUIRE(name_id >= 0 && name_id < (int)L.t.size(), "dac encoder pack: tensor id %d out of range", name_id);
+  const DacEncTensor& t = L.t[name_id];
+  PTTS_REQUIRE(numel == t.numel, "dac encoder pack: tensor %d expects %lld elements, got %lld", name_id, (long long)t.numel, (long long)numel);
+  cudaStream_t st = (cudaStream_t)stream;
+  char* base = (char*)enc_blob;
+  switch (t.kind) {
+    case EK_PLAIN:
+      if (int e = pack_plain(src, src_dtype, numel, base + t.off, cfg->dtype, st)) return e;
+      for (int i = 0; t.off_t >= 0 && i < t.tile; i++)
+        if (int e = pack_plain(src, src_dtype, numel, base + t.off_t + (int64_t)i * numel * L.es, cfg->dtype, st)) return e;
+      return PTTS_OK;
+    case EK_CODEBOOK:
+      return pack_normalized_codebook(src, src_dtype, (float*)(base + t.off), t.d0, t.d1, cfg->dtype == PTTS_BF16, st);
+    case EK_CONV:
+      if (t.off_k >= 0)
+        if (int e = pack_conv_kmajor(src, src_dtype, base + t.off_k, t.d0, t.d1, t.k, 0, st)) return e;
+      return pack_conv(src, src_dtype, base + t.off, cfg->dtype, t.d0, t.d1, t.k, 0, st);
+    default:   // EK_SCONV
+      if (t.off_k >= 0)
+        if (int e = pack_strided_conv(src, src_dtype, base + t.off_k, PTTS_BF16, t.d0, t.d1, t.k / 2, 1, st)) return e;
+      return pack_strided_conv(src, src_dtype, base + t.off, cfg->dtype, t.d0, t.d1, t.k / 2, 0, st);
+  }
+}
+int ptts_dac_encode_workspace_bytes(const ptts_dac_config* cfg, int32_t B, int32_t samples, int64_t* out_bytes) {
+  PTTS_REQUIRE(cfg && out_bytes && B > 0 && samples > 0, "bad argument");
+  if (int e = validate_dac_encoder(*cfg)) return e;
+  const int64_t T = (samples + dac_hop(*cfg) - 1) / dac_hop(*cfg), es = dtype_size(cfg->dtype);
+  *out_bytes = 3 * align_up(dac_enc_max_act_per_frame(*cfg) * B * T * es, 1024) + align_up((int64_t)cfg->latent_dim * B * T * es, 1024);
+  return PTTS_OK;
+}
+
+int ptts_dac_encode(const ptts_dac_config* cfg, const void* dec_blob, const void* enc_blob, void* workspace, int64_t workspace_bytes,
+                    const void* audio, int32_t B, int32_t samples, int32_t n_q, int64_t* codes_out, void* latents_out, void* stream) {
+  PTTS_REQUIRE(cfg && dec_blob && enc_blob && workspace && audio && codes_out, "null argument");
+  if (int e = validate_dac_encoder(*cfg)) return e;
+  PTTS_REQUIRE(B > 0 && samples > 0, "dac encode: empty input B=%d samples=%d", B, samples);
+  PTTS_REQUIRE(n_q >= 1 && n_q <= cfg->n_codebooks, "dac encode: n_q %d outside 1..%d", n_q, cfg->n_codebooks);
+  const DacEncLayout L = make_dac_enc_layout(*cfg);
+  const DacLayout DL = make_dac_layout(*cfg);
+  const int es = L.es, hop = dac_hop(*cfg), T = (samples + hop - 1) / hop, Tp = T * hop, Z = cfg->latent_dim;
+  const int64_t half = align_up(dac_enc_max_act_per_frame(*cfg) * B * T * es, 1024);
+  PTTS_REQUIRE(workspace_bytes >= 3 * half + align_up((int64_t)Z * B * T * es, 1024), "dac encode: workspace too small");
+  cudaStream_t st = (cudaStream_t)stream;
+  const char* bl = (const char*)enc_blob;
+  char* bufX = (char*)workspace;   // residual stream of the current block
+  char* act = bufX + half;         // activation the next conv reads
+  char* oth = act + half;
+  void* z = latents_out ? latents_out : (void*)(oth + half);
+  auto tp = [&](int i) { return bl + L.t[i].off; };
+  const int nb = cfg->n_enc_blocks, C0 = cfg->encoder_dim, cf = C0 << nb;
+  const int dil[3] = {1, 3, 9};
+  int ti = 2;   // tensor cursor (make_dac_enc_layout order): past the input conv
+  int Tlen = Tp;
+  // ---- tensor-core path: bf16, every conv after the input conv as a wgmma implicit GEMM (strided ones over the s*C view) ----
+  bool use_tc = cfg->dtype == PTTS_BF16 && env_flag("PTTS_DAC_TC", true) && C0 % 2 == 0 && conv_tc_supported(cf, Z);
+  for (int bi = 0; bi < nb && use_tc; bi++)
+    use_tc = conv_tc_supported(C0 << bi, C0 << bi) && conv_tc_supported(cfg->encoder_rates[bi] * (C0 << bi), 2 * (C0 << bi));
+  if (use_tc) {
+    auto tpk = [&](int i) { return bl + L.t[i].off_k; };
+    auto convk = [&](const void* x, int w_i, int b_i, const void* res, void* out_raw, void* out_act, const void* alpha_next, int Cin, int Cout,
+                     int Tl, int ks, int dl) {
+      ConvArgs a{};
+      a.x = x; a.bias = tp(b_i); a.res = res;
+      a.Cin = Cin; a.Cout = Cout; a.Tin = Tl; a.Tout = Tl; a.q_count = Tl;
+      a.n_taps = ks; a.off_base = -((ks - 1) / 2) * dl; a.off_step = dl; a.wt_base = 0; a.wt_step = 1;
+      a.n_phase = 1; a.wt_phase_step = 0; a.o_mul = 1; a.o_add = 0; a.o_phase_step = 0;
+      return launch_conv_tc(a, tpk(w_i), ks, alpha_next, out_raw, out_act, B, st);
+    };
+    // input conv: raw -> X, snake_{block0.res_unit1.snake1}(x) -> act
+    if (int e = launch_enc_input_conv(audio, tp(0), tp(1), tp(ti), bufX, act, C0, samples, Tp, B, st)) return e;
+    for (int bi = 0; bi < nb; bi++) {
+      const int C = C0 << bi, s = cfg->encoder_rates[bi];
+      for (int r = 0; r < 3; r++) {
+        // y = conv7(snake1(x)) -> only snake2(y) is stored; x += conv1(snake2(y)), plus snake_next(x): the next unit's snake1 or
+        // the block's snake1 (ti + 6 either way)
+        if (int e = convk(act, ti + 1, ti + 2, nullptr, nullptr, oth, tp(ti + 3), C, C, Tlen, 7, dil[r])) return e;
+        if (int e = convk(oth, ti + 4, ti + 5, bufX, bufX, act, tp(ti + 6), C, C, Tlen, 1, 1)) return e;
+        ti += 6;
+      }
+      // strided conv over super-rows of s time steps: 3 taps at rows q-1, q, q+1 of the [B][T/s][s*C] view; TMA zero fill of
+      // rows -1 and T/s is the conv padding.  Raw -> X (the next block's residual stream; not needed after the last block),
+      // snake of the next layer (next block's res_unit1.snake1 or the encoder's snake1, both at ti + 3) -> the other buffer
+      ConvArgs a{};
+      a.x = act; a.bias = tp(ti + 2); a.res = nullptr;
+      a.Cin = s * C; a.Cout = 2 * C; a.Tin = Tlen / s; a.Tout = Tlen / s; a.q_count = Tlen / s;
+      a.n_taps = 3; a.off_base = -1; a.off_step = 1; a.wt_base = 0; a.wt_step = 1;
+      a.n_phase = 1; a.wt_phase_step = 0; a.o_mul = 1; a.o_add = 0; a.o_phase_step = 0;
+      if (int e = launch_conv_tc(a, tpk(ti + 1), 3, tp(ti + 3), bi + 1 < nb ? bufX : nullptr, oth, B, st)) return e;
+      std::swap(act, oth);
+      Tlen /= s;
+      ti += 3;
+    }
+    if (int e = convk(act, ti + 1, ti + 2, nullptr, z, nullptr, nullptr, cf, Z, Tlen, 3, 1)) return e;
+  } else {
+    // ---- generic path (f32, or widths the wgmma kernel does not take): snake applied on the fly to each conv's input ----
+    auto conv = [&](const void* x, const void* w, const void* bias, const void* alpha, const void* res, void* out, int Cin, int Cout,
+                    int Tin, int Tout, int ks, int dl, int off_base) {
+      ConvArgs a{};
+      a.x = x; a.w = w; a.bias = bias; a.alpha = alpha; a.res = res; a.out = out;
+      a.Cin = Cin; a.Cout = Cout; a.Tin = Tin; a.Tout = Tout; a.q_count = Tout;
+      a.n_taps = ks; a.off_base = off_base; a.off_step = dl; a.wt_base = 0; a.wt_step = 1;
+      a.n_phase = 1; a.wt_phase_step = 0; a.o_mul = 1; a.o_add = 0; a.o_phase_step = 0; a.tanh_out = 0;
+      return launch_conv(a, cfg->dtype, B, st);
+    };
+    char* cur = bufX;
+    // input conv: rows past `samples` read zeros (the pad to the hop)
+    if (int e = conv(audio, tp(0), tp(1), nullptr, nullptr, cur, 1, C0, samples, Tp, 7, 1, -3)) return e;
+    for (int bi = 0; bi < nb; bi++) {
+      const int C = C0 << bi, s = cfg->encoder_rates[bi];
+      for (int r = 0; r < 3; r++) {
+        if (int e = conv(cur, tp(ti + 1), tp(ti + 2), tp(ti), nullptr, oth, C, C, Tlen, Tlen, 7, dil[r], -3 * dil[r])) return e;
+        if (int e = conv(oth, tp(ti + 4), tp(ti + 5), tp(ti + 3), cur, cur, C, C, Tlen, Tlen, 1, 1, 0)) return e;
+        ti += 6;
+      }
+      // strided conv over the super-row view; the block's snake1 alpha is tiled s times to match its s*C input channels
+      if (int e = conv(cur, tp(ti + 1), tp(ti + 2), bl + L.t[ti].off_t, nullptr, oth, s * C, 2 * C, Tlen / s, Tlen / s, 3, 1, -1)) return e;
+      std::swap(cur, oth);
+      Tlen /= s;
+      ti += 3;
+    }
+    if (int e = conv(cur, tp(ti + 1), tp(ti + 2), tp(ti), nullptr, z, cf, Z, Tlen, Tlen, 3, 1, -1)) return e;
+  }
+  const char* dbl = (const char*)dec_blob;
+  QuantizeArgs q{z, bl + L.in_w, bl + L.in_b, (const float*)(bl + L.cb_norm), dbl + DL.codebooks, dbl + DL.proj_w, dbl + DL.proj_b,
+                 codes_out, n_q, cfg->codebook_dim, Z, T, cfg->codebook_size};
+  return launch_quantize(q, cfg->dtype, B, st);
 }
 
 }  // extern "C"

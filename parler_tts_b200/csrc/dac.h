@@ -1,4 +1,4 @@
-// dac.h -- DAC decode: kernel argument structs, blob layout and tensor table.
+// dac.h -- DAC decode and encode: kernel argument structs, blob layouts and tensor tables.
 #pragma once
 #include <vector>
 #include "common.cuh"
@@ -105,6 +105,116 @@ static inline int dac_hop(const ptts_dac_config& c) {
   int h = 1;
   for (int i = 0; i < c.n_blocks; i++) h *= c.strides[i];
   return h;
+}
+
+// ---- DAC encode (dac_enc.cu) ----------------------------------------------------------------------
+// A strided Conv1d(C -> 2C, k = 2s, stride s, pad s/2) over [B][T][C] is an ordinary 3-tap conv over the [B][T/s][s*C] view
+// ("super-rows" q-1, q, q+1; tap j, in-row offset r carries weight tap r + j*s - s/2 when that lies in [0, 2s), else 0).
+// kmajor != 0: [3][Cout][s*C] bf16 (wgmma path); else [3][s*C][Cout] in dst_dtype (generic conv_kernel).
+int pack_strided_conv(const void* src, int src_dtype, void* dst, int dst_dtype, int Cout, int C, int s, int kmajor, cudaStream_t st);
+// codebook [n][D] (rounded to bf16 first when round_bf16) -> rows / max(||row||, 1e-12) in fp32 (F.normalize)
+int pack_normalized_codebook(const void* src, int src_dtype, float* dst, int n, int D, int round_bf16, cudaStream_t st);
+// Conv1d(1 -> C, k = 7, pad 3) over the waveform [B][samples] (zero beyond `samples`, T rows out, bf16): raw [B][T][C] and
+// snake_{alpha_next}(raw) for the next layer -- the wgmma kernel needs Cin >= 64.
+int launch_enc_input_conv(const void* audio, const void* w, const void* bias, const void* alpha_next, void* out_raw, void* out_act,
+                          int C, int samples, int T, int B, cudaStream_t st);
+struct QuantizeArgs {
+  const void* z;          // [B][T][Z] encoder output
+  const void* in_w;       // [K][D][Z]
+  const void* in_b;       // [K][D]
+  const float* cb_norm;   // [K][cs][D] fp32, unit rows
+  const void* codebooks;  // [K][cs][D] raw (decode blob)
+  const void* out_w;      // [K][Z][D] (decode blob)
+  const void* out_b;      // [K][Z]   (decode blob)
+  int64_t* codes;         // [B][n_q][T]
+  int n_q, D, Z, T, codebook_size;
+};
+bool quantize_supported(int Z, int D);
+int launch_quantize(const QuantizeArgs& a, int dtype, int B, cudaStream_t st);
+
+// Encoder tensor table (ptts_dac_encoder_pack ids): dac_wrapper.py::_dac_encoder_tensor_list gives the state-dict keys.
+enum { EK_PLAIN = 0, EK_CONV = 1, EK_SCONV = 2, EK_CODEBOOK = 3 };
+struct DacEncTensor {
+  int kind;
+  int d0, d1, k;   // conv: co, ci, k; plain / codebook: numel or rows, 1 / D, 1
+  int tile;        // plain: > 1 also stores the vector tiled `tile` times at off_t (snake before a strided conv, generic path)
+  int64_t off, numel;
+  int64_t off_k;   // conv weights, bf16 config: [tap][Cout][Cin] k-major copy (strided: the super-row form) for wgmma; -1: none
+  int64_t off_t;
+};
+struct DacEncLayout {
+  std::vector<DacEncTensor> t;
+  int64_t in_w, in_b, cb_norm;   // quantizer arrays, contiguous over codebooks
+  int64_t total;
+  int es;
+};
+
+static inline int validate_dac_encoder(const ptts_dac_config& c) {
+  if (int e = validate_dac(c)) return e;
+  PTTS_REQUIRE(c.encoder_dim > 0, "dac config has no encoder (encoder_dim = 0: decode only)");
+  PTTS_REQUIRE(c.n_enc_blocks >= 1 && c.n_enc_blocks <= 8, "dac encoder block count %d out of range", c.n_enc_blocks);
+  int hop = 1;
+  for (int i = 0; i < c.n_enc_blocks; i++) {
+    PTTS_REQUIRE(c.encoder_rates[i] >= 2 && c.encoder_rates[i] % 2 == 0 && c.encoder_rates[i] <= 32,
+                 "dac encoder stride %d must be even and <= 32", c.encoder_rates[i]);
+    hop *= c.encoder_rates[i];
+  }
+  PTTS_REQUIRE(hop == dac_hop(c), "dac encoder hop %d differs from the decoder hop %d", hop, dac_hop(c));
+  PTTS_REQUIRE(((int64_t)c.encoder_dim << c.n_enc_blocks) <= 65536, "dac encoder_dim too large");
+  return PTTS_OK;
+}
+
+static inline DacEncLayout make_dac_enc_layout(const ptts_dac_config& c) {
+  DacEncLayout L;
+  L.es = dtype_size(c.dtype);
+  const int K = c.n_codebooks, D = c.codebook_dim, Z = c.latent_dim, cs = c.codebook_size;
+  L.in_w = 0;
+  L.in_b = align_up((int64_t)K * D * Z * L.es, 256);
+  L.cb_norm = L.in_b + align_up((int64_t)K * D * L.es, 256);
+  int64_t o = L.cb_norm + align_up((int64_t)K * cs * D * 4, 256);
+  const bool tc = c.dtype == PTTS_BF16;
+  auto add = [&](int kind, int d0, int d1, int k, int tile) {
+    DacEncTensor t{kind, d0, d1, k, tile, o, (int64_t)d0 * d1 * k, -1, -1};
+    // a strided conv's generic copy is the [3][s*C][Cout] super-row form: 1.5x the source weight
+    const int64_t stored = kind == EK_SCONV ? (int64_t)3 * d0 * d1 * (k / 2) : t.numel;
+    o = align_up(o + stored * L.es, 256);
+    if (tc && (kind == EK_SCONV || (kind == EK_CONV && d1 > 1))) { t.off_k = o; o = align_up(o + stored * 2, 1024); }
+    if (tile > 1) { t.off_t = o; o = align_up(o + t.numel * tile * L.es, 256); }
+    L.t.push_back(t);
+  };
+  add(EK_CONV, c.encoder_dim, 1, 7, 1); add(EK_PLAIN, c.encoder_dim, 1, 1, 1);
+  for (int bi = 0; bi < c.n_enc_blocks; bi++) {
+    const int C = c.encoder_dim << bi, s = c.encoder_rates[bi];
+    for (int r = 0; r < 3; r++) {
+      add(EK_PLAIN, C, 1, 1, 1);
+      add(EK_CONV, C, C, 7, 1); add(EK_PLAIN, C, 1, 1, 1);
+      add(EK_PLAIN, C, 1, 1, 1);
+      add(EK_CONV, C, C, 1, 1); add(EK_PLAIN, C, 1, 1, 1);
+    }
+    add(EK_PLAIN, C, 1, 1, s);
+    add(EK_SCONV, 2 * C, C, 2 * s, 1); add(EK_PLAIN, 2 * C, 1, 1, 1);
+  }
+  const int cf = c.encoder_dim << c.n_enc_blocks;
+  add(EK_PLAIN, cf, 1, 1, 1);
+  add(EK_CONV, Z, cf, 3, 1); add(EK_PLAIN, Z, 1, 1, 1);
+  for (int k = 0; k < K; k++) {
+    L.t.push_back({EK_PLAIN, D * Z, 1, 1, 1, L.in_w + (int64_t)k * D * Z * L.es, (int64_t)D * Z, -1, -1});
+    L.t.push_back({EK_PLAIN, D, 1, 1, 1, L.in_b + (int64_t)k * D * L.es, (int64_t)D, -1, -1});
+    L.t.push_back({EK_CODEBOOK, cs, D, 1, 1, L.cb_norm + (int64_t)k * cs * D * 4, (int64_t)cs * D, -1, -1});
+  }
+  L.total = o;
+  return L;
+}
+
+// elements per (batch, code frame) of the largest encoder activation
+static inline int64_t dac_enc_max_act_per_frame(const ptts_dac_config& c) {
+  int64_t per = dac_hop(c), m = (int64_t)c.latent_dim;
+  for (int bi = 0; bi <= c.n_enc_blocks; bi++) {
+    const int64_t e = per * ((int64_t)c.encoder_dim << bi);
+    if (e > m) m = e;
+    if (bi < c.n_enc_blocks) per /= c.encoder_rates[bi];
+  }
+  return m;
 }
 // elements per (batch, code frame) of the largest activation
 static inline int64_t dac_max_act_per_frame(const ptts_dac_config& c) {

@@ -1,0 +1,226 @@
+// dac_enc.cu -- DAC codec encode: waveform -> latent -> codebook ids.
+//
+// Replaces DACModel.encode (parler_tts/dac_wrapper/modeling_dac.py:33-104), i.e. descript-audio-codec's model.preprocess
+// (:64, right zero-pad to the hop) and model.encode (:95).  Arithmetic restated from transformers' DacModel
+// (models/dac/modeling_dac.py:442-472 encoder, :210-231 block, :173-207 residual unit, :281-343 residual vector quantizer,
+// :102-170 vector quantize).  The encoder's residual units and its final k3 conv run on the decode path's conv kernels
+// (conv_tc_kernel in dac_tc.cu, conv_kernel in dac.cu); this file adds what those cannot do:
+//   * the input conv (Cin = 1; the wgmma kernel needs Cin >= 64),
+//   * the weight packs of the strided convs, which run as 3-tap convs over the [B][T/s][s*C] view (dac.h),
+//   * the residual vector quantizer.
+#include <math.h>
+
+#include "common.cuh"
+#include "dac.h"
+
+namespace ptts {
+
+// ---- strided conv weight: [Cout][C][2s] -> the super-row form (dac.h) ----------------------------------------------------
+template <typename S, typename D>
+__global__ void pack_strided_conv_kernel(const S* __restrict__ src, D* __restrict__ dst, int Cout, int C, int s, int kmajor) {
+  const int64_t sc = (int64_t)s * C;
+  const int64_t n = 3 * sc * Cout;
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  int64_t cip; int co, j;
+  if (kmajor) { cip = i % sc; co = (int)((i / sc) % Cout); j = (int)(i / (sc * Cout)); }
+  else { co = (int)(i % Cout); cip = (i / Cout) % sc; j = (int)(i / (sc * Cout)); }
+  const int r = (int)(cip / C), ci = (int)(cip - (int64_t)r * C);
+  const int k = r + j * s - s / 2;
+  float v = 0.f;
+  if (k >= 0 && k < 2 * s) {
+    const S w = src[((int64_t)co * C + ci) * (2 * s) + k];
+    if constexpr (sizeof(S) == 2) v = __bfloat162float(w); else v = w;
+  }
+  if constexpr (sizeof(D) == 2) dst[i] = __float2bfloat16_rn(v); else dst[i] = v;
+}
+int pack_strided_conv(const void* src, int src_dtype, void* dst, int dst_dtype, int Cout, int C, int s, int kmajor, cudaStream_t st) {
+  const int64_t n = (int64_t)3 * s * C * Cout;
+  const int blocks = (int)((n + 255) / 256);
+  if (src_dtype == PTTS_BF16 && dst_dtype == PTTS_BF16) pack_strided_conv_kernel<bf16, bf16><<<blocks, 256, 0, st>>>((const bf16*)src, (bf16*)dst, Cout, C, s, kmajor);
+  else if (src_dtype == PTTS_BF16) pack_strided_conv_kernel<bf16, float><<<blocks, 256, 0, st>>>((const bf16*)src, (float*)dst, Cout, C, s, kmajor);
+  else if (dst_dtype == PTTS_BF16) pack_strided_conv_kernel<float, bf16><<<blocks, 256, 0, st>>>((const float*)src, (bf16*)dst, Cout, C, s, kmajor);
+  else pack_strided_conv_kernel<float, float><<<blocks, 256, 0, st>>>((const float*)src, (float*)dst, Cout, C, s, kmajor);
+  PTTS_LAUNCH_CHECK();
+  return PTTS_OK;
+}
+
+// ---- codebook rows -> unit rows in fp32 (F.normalize in decode_latents, :160-161) ----------------------------------------
+template <typename S>
+__global__ void pack_normalized_codebook_kernel(const S* __restrict__ src, float* __restrict__ dst, int n, int D, int round_bf16) {
+  const int row = blockIdx.x * blockDim.x + threadIdx.x;
+  if (row >= n) return;
+  auto f = [&](int d) {   // the codebook as the model holds it (bf16 model: rounded to bf16), then normalised in fp32
+    const S v = src[(int64_t)row * D + d];
+    float x;
+    if constexpr (sizeof(S) == 2) x = __bfloat162float(v); else x = (float)v;
+    return round_bf16 ? __bfloat162float(__float2bfloat16_rn(x)) : x;
+  };
+  float ss = 0.f;
+  for (int d = 0; d < D; d++) ss = fmaf(f(d), f(d), ss);
+  const float inv = 1.0f / fmaxf(sqrtf(ss), 1e-12f);
+  for (int d = 0; d < D; d++) dst[(int64_t)row * D + d] = f(d) * inv;
+}
+int pack_normalized_codebook(const void* src, int src_dtype, float* dst, int n, int D, int round_bf16, cudaStream_t st) {
+  const int blocks = (n + 255) / 256;
+  if (src_dtype == PTTS_BF16) pack_normalized_codebook_kernel<bf16><<<blocks, 256, 0, st>>>((const bf16*)src, dst, n, D, round_bf16);
+  else pack_normalized_codebook_kernel<float><<<blocks, 256, 0, st>>>((const float*)src, dst, n, D, round_bf16);
+  PTTS_LAUNCH_CHECK();
+  return PTTS_OK;
+}
+
+// ---- input conv: Conv1d(1 -> C, k = 7, pad 3) on the bf16 waveform --------------------------------------------------------
+// One block covers IC_ROWS output rows x all C channels; its waveform window and the [7][C] weights sit in shared memory.  Each
+// thread writes channel pairs, with the same bf16x2 epilogue as conv_tc_kernel: raw = bf16(acc + bias) (taps summed in order
+// 0..6 in fp32), act = raw + inv * sin(alpha * raw)^2 for the next layer.
+constexpr int IC_ROWS = 64;
+__global__ void __launch_bounds__(256) enc_input_conv_kernel(const bf16* __restrict__ audio, const bf16* __restrict__ w, const bf16* __restrict__ bias,
+                                                             const bf16* __restrict__ alpha_next, bf16* __restrict__ out_raw, bf16* __restrict__ out_act,
+                                                             int C, int samples, int T) {
+  extern __shared__ float icm[];
+  float* xs = icm;                    // [IC_ROWS + 6] waveform window
+  float* ws = xs + IC_ROWS + 8;       // [7][C]
+  __nv_bfloat162* chan = reinterpret_cast<__nv_bfloat162*>(ws + 7 * C);   // [3][C/2]: bias | alpha | 1/(alpha + 1e-9)
+  const int b = blockIdx.y, t0 = blockIdx.x * IC_ROWS, tid = threadIdx.x, half = C / 2;
+  for (int e = tid; e < IC_ROWS + 6; e += blockDim.x) {
+    const int t = t0 - 3 + e;
+    xs[e] = (t >= 0 && t < samples) ? __bfloat162float(audio[(size_t)b * samples + t]) : 0.f;   // conv padding + the pad to the hop
+  }
+  for (int e = tid; e < 7 * C; e += blockDim.x) ws[e] = __bfloat162float(w[e]);
+  for (int c = tid; c < half; c += blockDim.x) {
+    const __nv_bfloat162 a = reinterpret_cast<const __nv_bfloat162*>(alpha_next)[c];
+    const float2 af = __bfloat1622float2(a);
+    chan[c] = reinterpret_cast<const __nv_bfloat162*>(bias)[c];
+    chan[half + c] = a;
+    chan[2 * half + c] = __floats2bfloat162_rn(1.0f / __bfloat162float(__float2bfloat16_rn(af.x + 1e-9f)),
+                                               1.0f / __bfloat162float(__float2bfloat16_rn(af.y + 1e-9f)));
+  }
+  __syncthreads();
+  for (int e = tid; e < IC_ROWS * half; e += blockDim.x) {
+    const int r = e / half, cp = e - r * half, t = t0 + r;
+    if (t >= T) break;
+    float a0 = 0.f, a1 = 0.f;
+#pragma unroll
+    for (int j = 0; j < 7; j++) {
+      const float x = xs[r + j];
+      a0 = fmaf(x, ws[j * C + 2 * cp], a0);
+      a1 = fmaf(x, ws[j * C + 2 * cp + 1], a1);
+    }
+    const float2 bb = __bfloat1622float2(chan[cp]);
+    const __nv_bfloat162 r2 = __floats2bfloat162_rn(a0 + bb.x, a1 + bb.y);
+    const size_t o = ((size_t)b * T + t) * C + 2 * cp;
+    *reinterpret_cast<__nv_bfloat162*>(out_raw + o) = r2;
+    const __nv_bfloat162 ax = __hmul2(chan[half + cp], r2);
+    const float2 axf = __bfloat1622float2(ax);
+    const __nv_bfloat162 sn = __floats2bfloat162_rn(__sinf(axf.x), __sinf(axf.y));
+    *reinterpret_cast<__nv_bfloat162*>(out_act + o) = __hadd2(r2, __hmul2(chan[2 * half + cp], __hmul2(sn, sn)));
+  }
+}
+int launch_enc_input_conv(const void* audio, const void* w, const void* bias, const void* alpha_next, void* out_raw, void* out_act,
+                          int C, int samples, int T, int B, cudaStream_t st) {
+  PTTS_REQUIRE(C % 2 == 0 && C <= 4096, "dac encode: input conv width %d unsupported", C);
+  const size_t smem = (size_t)(IC_ROWS + 8 + 7 * C) * 4 + (size_t)3 * C * 2;
+  static bool attr = false;
+  if (!attr) { PTTS_CHECK_CUDA(cudaFuncSetAttribute(enc_input_conv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024)); attr = true; }
+  enc_input_conv_kernel<<<dim3((T + IC_ROWS - 1) / IC_ROWS, B), 256, smem, st>>>((const bf16*)audio, (const bf16*)w, (const bf16*)bias,
+                                                                                (const bf16*)alpha_next, (bf16*)out_raw, (bf16*)out_act, C, samples, T);
+  PTTS_LAUNCH_CHECK();
+  return PTTS_OK;
+}
+
+// ---- residual vector quantizer (DacResidualVectorQuantizer.forward, :320-338) --------------------------------------------
+// One warp per code frame, all n_q codebooks in turn; lane l owns latent channels l, l + 32, ... of the residual (shared
+// memory), so in_proj and the residual update need no exchange beyond the D warp sums of in_proj.  Per codebook:
+//   z_e = in_proj(residual)                                  bf16(acc + bias) like torch's 1x1 conv
+//   code = argmax_c <z_e / |z_e|, c_hat>                     fp32, c_hat normalised at pack time; ties -> lowest index
+//   (with unit rows, -(|e|^2 - 2 e.c) + |c|^2 = 2 e.c: the reference's distance ranks the codes by this cosine)
+//   st = z_e + (z_q - z_e)                                   the straight-through expression, each op rounded (:149)
+//   residual -= out_proj(st)                                 bf16(acc + bias), then the rounded difference (:331)
+constexpr int QZ_WARPS = 8;
+template <typename T, int D>
+__global__ void __launch_bounds__(QZ_WARPS * 32) quantize_kernel(QuantizeArgs p, int n_frames) {
+  extern __shared__ float qres[];   // [QZ_WARPS][Z]
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int f = blockIdx.x * QZ_WARPS + warp;
+  if (f >= n_frames) return;
+  const int Z = p.Z, cs = p.codebook_size;
+  float* r = qres + (size_t)warp * Z;
+  const T* z = reinterpret_cast<const T*>(p.z) + (size_t)f * Z;
+  for (int c = lane; c < Z; c += 32) r[c] = DT<T>::to_f(z[c]);
+  const int b = f / p.T, t = f - b * p.T;
+  for (int k = 0; k < p.n_q; k++) {
+    const T* W = reinterpret_cast<const T*>(p.in_w) + (size_t)k * D * Z;
+    float e[D];
+#pragma unroll
+    for (int d = 0; d < D; d++) e[d] = 0.f;
+    for (int c = lane; c < Z; c += 32) {
+      const float rc = r[c];
+#pragma unroll
+      for (int d = 0; d < D; d++) e[d] = fmaf(DT<T>::to_f(W[(size_t)d * Z + c]), rc, e[d]);
+    }
+    float n2 = 0.f;
+#pragma unroll
+    for (int d = 0; d < D; d++) {
+      e[d] = DT<T>::rnd(warp_sum(e[d]) + DT<T>::to_f(reinterpret_cast<const T*>(p.in_b)[k * D + d]));
+      n2 = fmaf(e[d], e[d], n2);
+    }
+    const float inv = 1.0f / fmaxf(sqrtf(n2), 1e-12f);
+    float en[D];
+#pragma unroll
+    for (int d = 0; d < D; d++) en[d] = e[d] * inv;
+    const float* cb = p.cb_norm + (size_t)k * cs * D;
+    float best = -INFINITY;
+    int bi = cs;
+    for (int j = lane; j < cs; j += 32) {
+      const float4* row = reinterpret_cast<const float4*>(cb + (size_t)j * D);
+      float s = 0.f;
+#pragma unroll
+      for (int q = 0; q < D / 4; q++) {
+        const float4 v = row[q];
+        s = fmaf(en[4 * q], v.x, s); s = fmaf(en[4 * q + 1], v.y, s);
+        s = fmaf(en[4 * q + 2], v.z, s); s = fmaf(en[4 * q + 3], v.w, s);
+      }
+      if (s > best) { best = s; bi = j; }   // j rises: the first of equal values stays
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      const float ov = __shfl_xor_sync(0xffffffffu, best, o);
+      const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+      if (ov > best || (ov == best && oi < bi)) { best = ov; bi = oi; }
+    }
+    if (bi >= cs) bi = 0;   // every similarity NaN (a NaN latent): the reference's max() would not pick a valid row either
+    if (lane == 0) p.codes[((size_t)b * p.n_q + k) * p.T + t] = bi;
+    const T* zq = reinterpret_cast<const T*>(p.codebooks) + ((size_t)k * cs + bi) * D;
+    float st[D];
+#pragma unroll
+    for (int d = 0; d < D; d++) st[d] = DT<T>::rnd(e[d] + DT<T>::rnd(DT<T>::to_f(zq[d]) - e[d]));
+    const T* Wo = reinterpret_cast<const T*>(p.out_w) + (size_t)k * Z * D;
+    const T* bo = reinterpret_cast<const T*>(p.out_b) + (size_t)k * Z;
+    for (int c = lane; c < Z; c += 32) {
+      float q = 0.f;
+#pragma unroll
+      for (int d = 0; d < D; d++) q = fmaf(DT<T>::to_f(Wo[(size_t)c * D + d]), st[d], q);
+      q = DT<T>::rnd(q + DT<T>::to_f(bo[c]));
+      r[c] = DT<T>::rnd(r[c] - q);
+    }
+  }
+}
+
+bool quantize_supported(int Z, int D) { return (D == 4 || D == 8 || D == 16) && Z >= 1 && Z <= 1536; }
+template <typename T>
+static int launch_quantize_t(const QuantizeArgs& a, int B, cudaStream_t st) {
+  const int n = B * a.T;
+  const size_t smem = (size_t)QZ_WARPS * a.Z * 4;
+  dim3 grid((n + QZ_WARPS - 1) / QZ_WARPS);
+  if (a.D == 4) quantize_kernel<T, 4><<<grid, QZ_WARPS * 32, smem, st>>>(a, n);
+  else if (a.D == 8) quantize_kernel<T, 8><<<grid, QZ_WARPS * 32, smem, st>>>(a, n);
+  else quantize_kernel<T, 16><<<grid, QZ_WARPS * 32, smem, st>>>(a, n);
+  PTTS_LAUNCH_CHECK();
+  return PTTS_OK;
+}
+int launch_quantize(const QuantizeArgs& a, int dtype, int B, cudaStream_t st) {
+  PTTS_REQUIRE(quantize_supported(a.Z, a.D), "dac encode: quantizer shape latent %d / codebook_dim %d unsupported", a.Z, a.D);
+  return dtype == PTTS_BF16 ? launch_quantize_t<bf16>(a, B, st) : launch_quantize_t<float>(a, B, st);
+}
+
+}  // namespace ptts

@@ -1,11 +1,12 @@
-"""DACModel: the reference's codec wrapper surface, backed by the sm_90a DAC decode kernels.
+"""DACModel: the reference's codec wrapper surface, backed by the sm_90a DAC kernels.
 
-Mirrors parler_tts/dac_wrapper/modeling_dac.py:14-164 for the decode path:
+Mirrors parler_tts/dac_wrapper/modeling_dac.py:14-164:
+  DACModel.encode(input_values, padding_mask=None, bandwidth=None, return_dict=None, n_quantizers=None, sample_rate=None) (:33-104)
   DACModel.decode(audio_codes, audio_scales, padding_mask=None, return_dict=None)   (:106-142)
-`encode` (voice-prompt path) is out of this path's scope (SURVEY.md 8f rank 4) and raises.
-Weights: either folded tensors under transformers-DacModel style keys (decoder.conv1.weight, ...) or
-descript-audio-codec checkpoint keys with weight-norm parameters (weight_g / weight_v, or
-parametrizations.weight.original0/1), folded here as w = g * v / ||v|| (reference :148-157).
+Weights: either folded tensors under transformers-DacModel style keys (decoder.conv1.weight, encoder.block.0.res_unit1..., ...)
+or descript-audio-codec checkpoint keys with weight-norm parameters (weight_g / weight_v, or
+parametrizations.weight.original0/1), folded here as w = g * v / ||v|| (reference :148-157).  The encoder's weights go to a
+blob of their own; a state dict without them (decode only) stays valid, and encode then raises.
 """
 from __future__ import annotations
 import ctypes as C
@@ -26,6 +27,16 @@ class DACDecoderOutput:
 
     def __getitem__(self, i):
         return (self.audio_values,)[i]
+
+
+@dataclass
+class DACEncoderOutput:
+    """Stands in for transformers' EncodecEncoderOutput (audio_codes [1, B, K, T], audio_scales [None])."""
+    audio_codes: torch.Tensor = None
+    audio_scales: list = None
+
+    def __getitem__(self, i):
+        return (self.audio_codes, self.audio_scales)[i]
 
 
 def _dac_tensor_list(cfg: DACConfig) -> list[str]:
@@ -101,6 +112,72 @@ def _from_descript_keys(sd: dict[str, torch.Tensor], n_blocks: int) -> dict[str,
     return out
 
 
+def _dac_encoder_tensor_list(cfg: DACConfig) -> list[str]:
+    """(id -> key) table of the encoder blob, in the order csrc/dac.h::make_dac_enc_layout enumerates tensors."""
+    names = ["encoder.conv1.weight", "encoder.conv1.bias"]
+    for bi in range(len(cfg.encoder_rates)):
+        p = f"encoder.block.{bi}."
+        for r in (1, 2, 3):
+            u = p + f"res_unit{r}."
+            names += [u + "snake1.alpha", u + "conv1.weight", u + "conv1.bias", u + "snake2.alpha", u + "conv2.weight", u + "conv2.bias"]
+        names += [p + "snake1.alpha", p + "conv1.weight", p + "conv1.bias"]
+    names += ["encoder.snake1.alpha", "encoder.conv2.weight", "encoder.conv2.bias"]
+    for i in range(cfg.num_codebooks):
+        q = f"quantizer.quantizers.{i}."
+        names += [q + "in_proj.weight", q + "in_proj.bias", q + "codebook.weight"]
+    return names
+
+
+# descript's Encoder is one Sequential (encoder.block.N.weight, encoder.block.N.block.M...); transformers' DacEncoder names its
+# modules (encoder.block.N.res_unitM..., encoder.conv1...)
+_DESCRIPT_ENCODER_KEY = re.compile(r"encoder\.block\.\d+\.(block\.|weight$|bias$|alpha$)")
+
+
+def _from_descript_encoder_keys(sd: dict[str, torch.Tensor], n_blocks: int) -> dict[str, torch.Tensor]:
+    """descript-audio-codec encoder paths -> the transformers-DacModel style keys used internally.
+
+    descript layout: encoder.block = [WNConv1d(k7), EncoderBlock x n, Snake1d, WNConv1d(k3)]; EncoderBlock.block =
+    [ResidualUnit x 3, Snake1d, WNConv1d(k=2s, stride s)]; ResidualUnit.block = [Snake1d, WNConv1d(k7), Snake1d, WNConv1d(k1)]."""
+    out = {}
+    for k, v in sd.items():
+        m = re.match(r"encoder\.block\.(\d+)\.(.*)$", k)
+        if not m:
+            continue
+        i, rest = int(m.group(1)), m.group(2)
+        if i == 0:
+            out["encoder.conv1." + rest] = v
+        elif 1 <= i <= n_blocks:
+            mm = re.match(r"block\.(\d+)\.(.*)$", rest)
+            if not mm:
+                continue
+            j, r2 = int(mm.group(1)), mm.group(2)
+            p = f"encoder.block.{i - 1}."
+            if j < 3:
+                m3 = re.match(r"block\.(\d+)\.(.*)$", r2)
+                u, r3 = int(m3.group(1)), m3.group(2)
+                name = {0: "snake1.", 1: "conv1.", 2: "snake2.", 3: "conv2."}[u]
+                out[p + f"res_unit{j + 1}." + name + r3] = v
+            elif j == 3:
+                out[p + "snake1." + r2] = v
+            elif j == 4:
+                out[p + "conv1." + r2] = v
+        elif i == n_blocks + 1:
+            out["encoder.snake1." + rest] = v
+        elif i == n_blocks + 2:
+            out["encoder.conv2." + rest] = v
+    return out
+
+
+def _encoder_state_dict(sd: dict[str, torch.Tensor], n_blocks: int) -> dict[str, torch.Tensor]:
+    """The encoder and quantizer keys of a folded state dict, in transformers-DacModel style whichever layout it came in."""
+    if any(_DESCRIPT_ENCODER_KEY.match(k) for k in sd):
+        out = _from_descript_encoder_keys(sd, n_blocks)
+    else:
+        out = {k: v for k, v in sd.items() if k.startswith("encoder.")}
+    out.update({k: v for k, v in sd.items() if k.startswith("quantizer.")})
+    return out
+
+
 class DACModel:
     config_class = DACConfig
     main_input_name = "input_values"
@@ -127,11 +204,32 @@ class DACModel:
         self.blob = torch.zeros(nbytes.value, dtype=torch.uint8, device=self.device)
         self.loaded = False
         self._ws = None
+        # the encoder blob, likewise from construction on; None when the config has no usable encoder (encoder_dim = 0, or
+        # rates the kernels do not take, such as a hop that differs from the decoder's): decode still works, encode raises
+        self.encoder_blob = None
+        self.encoder_loaded = False
+        self._encoder_error = "the config has no encoder (encoder_dim = 0)"
+        self._enc_ws = None
+        rates = list(getattr(config, "encoder_rates", None) or [])
+        if getattr(config, "encoder_dim", 0) and len(rates) > 8:
+            self._encoder_error = f"{len(rates)} encoder blocks (at most 8)"
+        elif getattr(config, "encoder_dim", 0):
+            self._c.encoder_dim = int(config.encoder_dim)
+            self._c.n_enc_blocks = len(rates)
+            for i, s in enumerate(rates):
+                self._c.encoder_rates[i] = int(s)
+            try:
+                _lib.check(_lib.lib().ptts_dac_encoder_blob_bytes(C.byref(self._c), C.byref(nbytes)))
+                self.encoder_blob = torch.zeros(nbytes.value, dtype=torch.uint8, device=self.device)
+                self._encoder_error = None
+            except ValueError as e:
+                self._encoder_error = str(e)
 
     # -- weights -----------------------------------------------------------------------------------
     def load_state_dict(self, sd: dict[str, torch.Tensor], strict: bool = True):
         sd = {(k[len("model."):] if k.startswith("model.") else k): v for k, v in sd.items()}
         sd = _fold_weight_norm(sd)
+        enc_sd = _encoder_state_dict(sd, len(getattr(self.config, "encoder_rates", None) or []))
         if any(k.startswith("decoder.model.") for k in sd):
             sd = _from_descript_keys(sd, len(self.config.decoder_rates))
         names = _dac_tensor_list(self.config)
@@ -154,7 +252,34 @@ class DACModel:
                                          t.numel(), _lib.stream_ptr()))
         torch.cuda.current_stream().synchronize()  # staging tensors above go out of scope
         self.loaded = True
+        self._load_encoder(enc_sd, strict)
         return self
+
+    def _load_encoder(self, sd: dict[str, torch.Tensor], strict: bool):
+        """Pack the encoder keys of `sd` (from _encoder_state_dict) into the encoder blob; none present: decode only."""
+        self.encoder_loaded = False
+        if self.encoder_blob is None or not any(k.startswith("encoder.") for k in sd):
+            return
+        names = _dac_encoder_tensor_list(self.config)
+        missing = [n for n in names if n not in sd]
+        if missing and strict:
+            raise ValueError(f"DACModel.load_state_dict: missing encoder keys {missing[:5]}{'...' if len(missing) > 5 else ''}")
+        lib = _lib.lib()
+        n = C.c_int32()
+        _lib.check(lib.ptts_dac_encoder_num_tensors(C.byref(self._c), C.byref(n)))
+        assert n.value == len(names), (n.value, len(names))
+        self.encoder_blob.zero_()
+        for i, name in enumerate(names):
+            if name not in sd:
+                continue
+            t = sd[name].to(device=self.device)
+            if t.dtype not in (torch.float32, torch.bfloat16):
+                t = t.float()
+            t = t.contiguous()
+            _lib.check(lib.ptts_dac_encoder_pack(C.byref(self._c), _lib.ptr(self.encoder_blob), i, _lib.ptr(t), _lib.dtype_code(t.dtype),
+                                                 t.numel(), _lib.stream_ptr()))
+        torch.cuda.current_stream().synchronize()
+        self.encoder_loaded = True
 
     def to(self, *args, **kwargs):
         return self
@@ -163,8 +288,57 @@ class DACModel:
         return self
 
     # -- reference surface -------------------------------------------------------------------------
-    def encode(self, *args, **kwargs):
-        raise NotImplementedError("DACModel.encode (voice-prompt path) is outside the generate() hot path")
+    @torch.no_grad()
+    def encode(self, input_values, padding_mask=None, bandwidth=None, return_dict=None, n_quantizers=None, sample_rate=None):
+        """input_values [B, 1, samples] -> DACEncoderOutput(audio_codes [1, B, n_q, ceil(samples / hop)] int64, audio_scales [None]).
+
+        One chunk, right zero-padded to the hop like model.preprocess (:64); n_q = n_quantizers or every codebook.
+        `padding_mask` and `bandwidth` are unused, as in the reference.  Float32 or model-dtype audio; it is rounded to the
+        model dtype before the first conv."""
+        if not isinstance(input_values, torch.Tensor) or input_values.dim() != 3:
+            raise ValueError(f"input_values must be [batch, channels, samples], got {getattr(input_values, 'shape', type(input_values))}")
+        B, channels, n = input_values.shape
+        if channels < 1 or channels > 2:
+            raise ValueError(f"Number of audio channels must be 1 or 2, but got {channels}")
+        if channels == 2:
+            raise ValueError("the DAC encoder takes mono audio [B, 1, samples] (its first conv has one input channel), got 2 channels")
+        if sample_rate is not None and int(sample_rate) != self.config.sampling_rate:
+            raise ValueError(f"sample_rate {sample_rate} differs from the codec's {self.config.sampling_rate}")
+        if B == 0 or n == 0:
+            raise ValueError(f"input_values is empty: shape {tuple(input_values.shape)}")
+        if not input_values.is_floating_point():
+            raise ValueError(f"input_values must be a floating-point waveform, got {input_values.dtype}")
+        K = self.config.num_codebooks
+        n_q = K if n_quantizers is None else int(n_quantizers)
+        if not 1 <= n_q <= K:
+            raise ValueError(f"n_quantizers must lie in 1..{K}, got {n_quantizers}")
+        codes, _ = self._encode(input_values[:, 0, :], n_q)
+        codes = codes[None]
+        if return_dict is False:
+            return (codes, [None])
+        return DACEncoderOutput(codes, [None])
+
+    def _encode(self, audio: torch.Tensor, n_q: int, return_latents: bool = False):
+        """audio [B, samples] -> (codes [B, n_q, T] int64, encoder output [B, T, latent_dim] in the model dtype or None)."""
+        if self.encoder_blob is None:
+            raise ValueError(f"DACModel.encode is not available for this config: {self._encoder_error}")
+        if not (self.encoder_loaded and self.loaded):
+            raise RuntimeError("DACModel has no encoder weights loaded (a decode-only state dict): encode needs the encoder.* and "
+                               "quantizer.quantizers.N.{in_proj,codebook,out_proj} weights")
+        audio = audio.to(device=self.device, dtype=self.dtype).contiguous()
+        B, n = audio.shape
+        T = -(-n // self.hop_length)
+        lib = _lib.lib()
+        need = C.c_int64()
+        _lib.check(lib.ptts_dac_encode_workspace_bytes(C.byref(self._c), B, n, C.byref(need)))
+        if self._enc_ws is None or self._enc_ws.numel() < need.value:
+            self._enc_ws = torch.empty(need.value, dtype=torch.uint8, device=self.device)
+        codes = torch.empty(B, n_q, T, dtype=torch.int64, device=self.device)
+        latents = torch.empty(B, T, self.config.latent_dim, dtype=self.dtype, device=self.device) if return_latents else None
+        _lib.check(lib.ptts_dac_encode(C.byref(self._c), _lib.ptr(self.blob), _lib.ptr(self.encoder_blob), _lib.ptr(self._enc_ws),
+                                       self._enc_ws.numel(), _lib.ptr(audio), B, n, n_q, _lib.ptr(codes), _lib.ptr(latents),
+                                       _lib.stream_ptr()))
+        return codes, latents
 
     @torch.no_grad()
     def decode(self, audio_codes, audio_scales=None, padding_mask=None, return_dict=None):

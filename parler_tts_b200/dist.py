@@ -49,11 +49,15 @@ def broadcast_blob(blob: torch.Tensor, src: int = 0, group=None) -> torch.Tensor
 
 def model_weight_tensors(model) -> list[torch.Tensor]:
     """Every device tensor that holds weights, in a fixed order that depends on the CONFIG only (never on what a rank has
-    loaded): the packed decoder blob, the packed DAC blob, the prompt embedding table and, when the text encoder's width
-    differs from the decoder's, enc_to_dec_proj (modeling_parler_tts.py:2388-2392).  All exist from construction on."""
+    loaded): the packed decoder blob, the packed DAC blob, the prompt embedding table, when the text encoder's width
+    differs from the decoder's, enc_to_dec_proj (modeling_parler_tts.py:2388-2392), and the DAC encoder blob when the codec
+    config has an encoder.  All exist from construction on."""
     ts = [model.decoder.engine.blob, model.audio_encoder.blob, model.embed_prompts_weight]
     if model.enc_to_dec_proj is not None:
         ts += list(model.enc_to_dec_proj)
+    enc_blob = getattr(model.audio_encoder, "encoder_blob", None)
+    if enc_blob is not None:
+        ts.append(enc_blob)
     return ts
 
 
@@ -63,11 +67,14 @@ def broadcast_model_weights(model, src: int = 0, group=None):
     ts = model_weight_tensors(model)
     for t in ts:
         broadcast_blob(t, src, group)
-    flags = torch.tensor([int(model.audio_encoder.loaded), int(model._side_loaded)], dtype=torch.int32, device=ts[0].device)
+    flags = torch.tensor([int(model.audio_encoder.loaded), int(model._side_loaded), int(getattr(model.audio_encoder, "encoder_loaded", False))],
+                         dtype=torch.int32, device=ts[0].device)
     broadcast_blob(flags, src, group)
     loaded = flags.cpu().tolist()
     model.audio_encoder.loaded = bool(loaded[0])
     model._side_loaded = bool(loaded[1])
+    if hasattr(model.audio_encoder, "encoder_loaded"):
+        model.audio_encoder.encoder_loaded = bool(loaded[2])
     return model
 
 

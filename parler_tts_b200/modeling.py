@@ -754,9 +754,6 @@ class ParlerTTSForConditionalGeneration:
             raise ValueError("Got incompatible mode for generation, should be one of greedy or sampling. "
                              "Ensure that beam search is de-activated by setting `num_beams=1` and `num_beam_groups=1`.")
         custom_loop = bool(logits_processor) or bool(stopping_criteria)   # merged with the built-in ones like :3540-3552
-        if mk.get("input_values") is not None:
-            raise ValueError("`input_values` (an audio prompt to encode) is not supported on this path: encode the prompt to audio "
-                             "codes and pass them as `decoder_input_ids`")
         input_ids = mk.get("input_ids", inputs)
         attention_mask = mk.get("attention_mask")
         enc = mk.get("encoder_outputs")
@@ -779,6 +776,16 @@ class ParlerTTSForConditionalGeneration:
         d = self.config.decoder
         K = d.num_codebooks
         dec_ids = None
+        if mk.get("decoder_input_ids") is None and mk.get("input_values") is not None:
+            # audio prompt (:3442-3446, :3136-3194): encoded once, with every codebook; its codes continue like decoder_input_ids.
+            # padding_mask does not reach the encoder, as in the reference.
+            wav = mk["input_values"]
+            if wav.dim() != 3 or wav.shape[0] != B:
+                raise ValueError(f"input_values must be [batch_size = {B}, 1, samples], got {tuple(wav.shape)}")
+            if self.config.audio_encoder.num_codebooks != K:
+                raise ValueError(f"the codec has {self.config.audio_encoder.num_codebooks} codebooks, the decoder {K}: "
+                                 "its codes cannot continue this decoder")
+            mk["decoder_input_ids"] = self.audio_encoder.encode(wav).audio_codes
         if mk.get("decoder_input_ids") is not None:   # -> the BOS-led [B * K, n0] on the device (:3012-3024)
             start = gc.decoder_start_token_id if gc.decoder_start_token_id is not None else d.bos_token_id
             dec_ids = prepare_decoder_input_ids(mk["decoder_input_ids"], B, K, d.vocab_size, start, self.device)
