@@ -158,6 +158,31 @@ int ptts_generate_begin_ids(ptts_session* s, const ptts_gen_params* gen, const i
 int ptts_prefill(ptts_session* s, const void* prompt_hidden, const int64_t* prompt_mask,
                  const void* enc_hidden, const int64_t* enc_mask, void* stream);
 
+/* ---- teacher-forced scoring ---------------------------------------------------------------- */
+/* The fused scoring kernel reads the K lm heads row-major ([K*V][H] bf16, LayerNorm folded as in the blob).  The blob keeps them
+ * in mma fragment order only, so the copy lives in a separate caller-owned buffer of ptts_lm_heads_rowmajor_bytes bytes, filled
+ * by ptts_lm_heads_rowmajor_pack after ptts_decoder_finalize.  bf16 models only (PTTS_EINVAL otherwise). */
+int ptts_lm_heads_rowmajor_bytes(const ptts_decoder_config* cfg, int64_t* out_bytes);
+int ptts_lm_heads_rowmajor_pack(const ptts_decoder_config* cfg, const void* blob, void* heads_rm, void* stream);
+
+/* The teacher-forced forward with labels (ParlerTTSForConditionalGeneration.forward, :2695-2880; loss :1922-1974) on a session
+ * created with max_input_len >= T: the prompt prefix and the T decoder input columns go through the decoder in one prefill pass,
+ * then the K lm heads run over the T label positions of every utterance.
+ *   prompt_hidden, prompt_mask, enc_hidden, enc_mask   as for ptts_prefill
+ *   dec_ids   [B*K, T] int64 in [0, vocab_size]: the decoder input AS GIVEN (already delayed / shifted; no delay is applied)
+ *   labels    [B, T, K] int64 in {-100} u [0, vocab_size), or NULL (logits only).  As in the reference, a BOS label counts as
+ *             -100, and a cell (b, t, k) counts iff labels != -100 and dec_ids[b*K + k][t] != eos.
+ *   heads_rm  the row-major heads (ptts_lm_heads_rowmajor_pack): required by the fused bf16 path, unused otherwise
+ *   out_token_nll      [B, T, K] f32: logsumexp(logits) - logits[label] per counted cell, 0 elsewhere (needs labels)
+ *   out_logits         NULL, or [B*K, T, V] f32: the logits (the unfused route: the decoder's heads GEMM one frame at a time)
+ *   out_codebook_sums  NULL, or [K][2] f32: per codebook the sum of out_token_nll over counted cells and their count
+ * bf16 without out_logits runs the fused heads + cross-entropy kernel (the logits never reach memory); f32 models and calls that
+ * want the logits take the unfused route.  The session's caches and history are overwritten: a generation on it starts again
+ * with ptts_generate_begin*. */
+int ptts_score(ptts_session* s, const void* prompt_hidden, const int64_t* prompt_mask, const void* enc_hidden,
+               const int64_t* enc_mask, const int64_t* dec_ids, const int64_t* labels, int32_t T, const void* heads_rm,
+               float* out_token_nll, float* out_logits, float* out_codebook_sums, void* stream);
+
 /* One cached decode step for the ids currently staged in the workspace (the delay-masked last
  * column).  Leaves f32 logits [B*K, V] in the workspace.  Replaces prepare_inputs_for_generation
  * (:2882-2986) + ParlerTTSForCausalLM.forward with q_len == 1. */

@@ -60,6 +60,9 @@ _SIGS = {
     "ptts_generate_begin": (C.c_int, [_VP, C.POINTER(GenParamsC), _VP]),
     "ptts_generate_begin_ids": (C.c_int, [_VP, C.POINTER(GenParamsC), _VP, _I32, _VP]),
     "ptts_prefill": (C.c_int, [_VP, _VP, _VP, _VP, _VP, _VP]),
+    "ptts_lm_heads_rowmajor_bytes": (C.c_int, [C.POINTER(DecoderConfigC), C.POINTER(_I64)]),
+    "ptts_lm_heads_rowmajor_pack": (C.c_int, [C.POINTER(DecoderConfigC), _VP, _VP, _VP]),
+    "ptts_score": (C.c_int, [_VP, _VP, _VP, _VP, _VP, _VP, _VP, _I32, _VP, _VP, _VP, _VP, _VP]),
     "ptts_decode_forward": (C.c_int, [_VP, _VP]),
     "ptts_sample": (C.c_int, [_VP, _VP, _VP]),
     "ptts_decode_steps": (C.c_int, [_VP, _I32, _VP]),

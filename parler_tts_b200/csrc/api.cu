@@ -321,8 +321,10 @@ static int64_t rowmajor_offset(const DecoderLayout& L, int64_t woff) {
   return -1;
 }
 
-// one decoder pass over q_len new positions per batch row (q_len = P+n0 at prefill, 1 at decode)
-static int run_forward(ptts_session* s, cudaStream_t st, bool prefill, const void* prompt_hidden, const void* enc_hidden) {
+// one decoder pass over q_len new positions per batch row (q_len = P+n0 at prefill, 1 at decode); heads == false stops after
+// the last layer and leaves the residual stream x [B][q_len][H] for the caller (ptts_score)
+static int run_forward(ptts_session* s, cudaStream_t st, bool prefill, const void* prompt_hidden, const void* enc_hidden,
+                       bool heads = true) {
   const ptts_decoder_config& c = s->cfg;
   const DecoderLayout& L = s->L;
   const WorkspaceLayout& W = s->W;
@@ -413,6 +415,7 @@ static int run_forward(ptts_session* s, cudaStream_t st, bool prefill, const voi
                     EPI_ACT, nullptr, ws + W.hbuf, L.F, M, lb + L.c_fc1)) return e;
     if (int e = lin(ws + W.hbuf, L.F, lb + L.fc2, H, L.F, nullptr, nullptr, EPI_RESIDUAL, x, x, H, M)) return e;
   }
+  if (!heads) return PTTS_OK;
   // final LayerNorm + K lm heads on the last position of every batch row -> f32 logits [B, K*V] == [B*K, V]
   const char* xlast = ws + W.x + (int64_t)(q_len - 1) * H * es;
   return lin(xlast, (int64_t)q_len * H, L.heads, L.K * L.V, H, (const float*)(blob + L.final_ln_w), (const float*)(blob + L.final_ln_b),
@@ -434,6 +437,78 @@ int ptts_prefill(ptts_session* s, const void* prompt_hidden, const int64_t* prom
   s->path = choose_decode_path(s);
   // mask presence is baked into the captured graph: re-capture if it changed
   if (s->exec) { cudaGraphExecDestroy(s->exec); s->exec = nullptr; s->graph_ready = false; }
+  return PTTS_OK;
+}
+
+// ---- teacher-forced scoring --------------------------------------------------------------------
+int ptts_lm_heads_rowmajor_bytes(const ptts_decoder_config* cfg, int64_t* out_bytes) {
+  PTTS_REQUIRE(cfg && out_bytes, "null argument");
+  if (int e = validate_config(*cfg)) return e;
+  PTTS_REQUIRE(cfg->dtype == PTTS_BF16, "lm heads row-major copy: only bf16 models score on the fused kernel");
+  *out_bytes = (int64_t)cfg->num_codebooks * cfg->vocab_size * cfg->hidden_size * 2;
+  return PTTS_OK;
+}
+
+int ptts_lm_heads_rowmajor_pack(const ptts_decoder_config* cfg, const void* blob, void* heads_rm, void* stream) {
+  PTTS_REQUIRE(cfg && blob && heads_rm, "null argument");
+  if (int e = validate_config(*cfg)) return e;
+  PTTS_REQUIRE(cfg->dtype == PTTS_BF16, "lm heads row-major copy: only bf16 models score on the fused kernel");
+  const DecoderLayout L = make_layout(*cfg);
+  return unpack_fragments((const char*)blob + L.heads, heads_rm, (int64_t)L.K * L.V, L.H, (cudaStream_t)stream);
+}
+
+int ptts_score(ptts_session* s, const void* prompt_hidden, const int64_t* prompt_mask, const void* enc_hidden, const int64_t* enc_mask,
+               const int64_t* dec_ids, const int64_t* labels, int32_t T, const void* heads_rm, float* out_token_nll, float* out_logits,
+               float* out_codebook_sums, void* stream) {
+  PTTS_REQUIRE(s && enc_hidden && dec_ids, "null argument");
+  const ptts_decoder_config& c = s->cfg;
+  const DecoderLayout& L = s->L;
+  const WorkspaceLayout& W = s->W;
+  PTTS_REQUIRE(T >= 1 && T <= W.max_input, "score: %d decoder input columns, the session takes 1 .. %d", T, W.max_input);
+  PTTS_REQUIRE(W.P == 0 || prompt_hidden, "score: prompt_hidden is required when P > 0");
+  PTTS_REQUIRE(labels ? (out_token_nll != nullptr) : (out_logits != nullptr && out_codebook_sums == nullptr),
+               "score: labels need out_token_nll; without labels only out_logits can be filled");
+  const bool fused = (c.dtype == PTTS_BF16 && out_logits == nullptr);
+  PTTS_REQUIRE(!fused || heads_rm, "score: the fused bf16 path needs the row-major heads (ptts_lm_heads_rowmajor_pack)");
+  PTTS_REQUIRE(!fused || score_fused_supported(L.H, L.V), "score: hidden_size %d / vocab_size %d are outside the fused kernel", L.H, L.V);
+  cudaStream_t st = (cudaStream_t)stream;
+  // the decoder input goes into the history as given: it is already delayed (no ptts_generate_begin_ids)
+  PTTS_CHECK_CUDA(cudaMemcpy2DAsync(s->ws + W.raw_ids, W.raw_ld * 8, dec_ids, (size_t)T * 8, (size_t)T * 8, W.BK, cudaMemcpyDeviceToDevice, st));
+  s->has_prompt_mask = (prompt_mask != nullptr && W.P > 0);
+  s->has_enc_mask = (enc_mask != nullptr);
+  if (s->has_prompt_mask) { if (int e = launch_mask_convert(prompt_mask, W.B * W.P, (int*)(s->ws + W.prompt_mask), st)) return e; }
+  if (s->has_enc_mask) { if (int e = launch_mask_convert(enc_mask, W.B * W.S, (int*)(s->ws + W.enc_mask), st)) return e; }
+  s->n0 = T;
+  s->begun = s->prefilled = false;  // the caches now hold this call's positions: a generation has to begin again
+  if (int e = run_forward(s, st, true, prompt_hidden, enc_hidden, false)) return e;
+
+  ScoreArgs a{};
+  a.labels = labels; a.dec_ids = dec_ids; a.token_nll = out_token_nll;
+  a.M = W.B * T; a.B = W.B; a.T = T; a.K = L.K; a.V = L.V; a.H = L.H;
+  a.bos = c.bos_token_id; a.eos = c.eos_token_id;
+  const int q_len = W.P + T;
+  if (fused) {
+    a.c1 = (const float*)(s->blob + L.c_heads); a.c2 = a.c1 + (int64_t)L.K * L.V;
+    s->launches += 2;
+    if (int e = launch_score_fused(a, s->ws + W.x, W.P, c.layer_norm_eps, s->ws + W.qc, (float*)(s->ws + W.row_stats), heads_rm, st)) return e;
+  } else {  // the decoder's heads GEMM over the B rows of one frame at a time, into the workspace logits [B*K][V]
+    for (int t = 0; t < T; t++) {
+      LinearArgs h{};
+      h.X = s->ws + W.x + (int64_t)(W.P + t) * L.H * L.es; h.ldx = (int64_t)q_len * L.H;
+      h.W = s->blob + L.heads; h.Y = s->ws + W.logits; h.ldy = (int64_t)L.K * L.V; h.ldr = h.ldy;
+      h.ln_w = (const float*)(s->blob + L.final_ln_w); h.ln_b = (const float*)(s->blob + L.final_ln_b); h.eps = c.layer_norm_eps;
+      if (c.dtype == PTTS_BF16) { h.c1 = (const float*)(s->blob + L.c_heads); h.c2 = h.c1 + (int64_t)L.K * L.V; }
+      h.M = W.B; h.N = L.K * L.V; h.K = L.H; h.Kc = L.H;
+      h.epi = EPI_F32; h.act = c.activation;
+      if (int e = launch_linear(h, c.dtype, st, false, s->sm_count)) return e;
+      if (int e = launch_score_rows(a, (const float*)(s->ws + W.logits), t, out_logits, st)) return e;
+      s->launches += 2;
+    }
+  }
+  if (out_codebook_sums != nullptr) {
+    s->launches++;
+    if (int e = launch_score_reduce(a, out_codebook_sums, st)) return e;
+  }
   return PTTS_OK;
 }
 

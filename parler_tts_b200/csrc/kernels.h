@@ -84,4 +84,23 @@ int launch_mask_convert(const int64_t* src, int n, int* dst, cudaStream_t st);  
 int launch_cross_kv_relayout(const void* src, void* dst, int B, int S, int nckv, int dtype, cudaStream_t st);
 int launch_gather_rows(const void* src, int64_t ld_src, int64_t row0, int64_t row_step, void* dst, int rows, int cols, int dtype, cudaStream_t st);
 
+// ---- teacher-forced scoring (score.cu) ----------------------------------------------------------
+struct ScoreArgs {
+  const int64_t* labels;   // [B][T][K] int64, -100 = ignored (nullptr: logits only, no NLL)
+  const int64_t* dec_ids;  // [B*K][T] int64: the decoder input (a cell whose input id is eos is not counted)
+  float* token_nll;        // [B][T][K] f32: logsumexp - logit[label], 0 where the cell is not counted
+  const float* c1; const float* c2;  // fused kernel: the heads' folded-LayerNorm vectors [K*V]
+  int M, B, T, K, V, H;    // M = B*T label rows
+  int bos, eos;
+};
+bool score_fused_supported(int H, int V);
+// bf16: x = the decoder output [B][P+T][H]; gathers the label rows into xs_scratch [M][H] (+ LayerNorm stats), then the fused
+// heads + cross-entropy kernel over heads_rm (row-major folded heads [K*V][H])
+int launch_score_fused(const ScoreArgs& a, const void* x, int P, float eps, void* xs_scratch, float* stats_scratch,
+                       const void* heads_rm, cudaStream_t st);
+// unfused, frame t: the heads GEMM's f32 logits [B*K][V] -> token_nll (labels != nullptr) and logits_out [B*K][T][V] (if set)
+int launch_score_rows(const ScoreArgs& a, const float* logits, int t, float* logits_out, cudaStream_t st);
+// out [K][2] f32: per codebook, the sum of token_nll over counted cells and their count
+int launch_score_reduce(const ScoreArgs& a, float* out, cudaStream_t st);
+
 }  // namespace ptts

@@ -88,6 +88,79 @@ def check_continuation_length(n0: int, prompt_len: int, max_length: int, max_pos
         raise ValueError(f"{prompt_len} prompt positions + max_length {max_length} exceed max_position_embeddings {max_position_embeddings}")
 
 
+def shift_tokens_right(input_ids: torch.Tensor, pad_token_id: int, decoder_start_token_id: int):
+    """The reference's shift_tokens_right (:308-323): one position to the right along dim 1, decoder_start_token_id first, -100
+    replaced by pad_token_id.  Host-side integer work: labels [B, T, K] -> the decoder input [B, T, K]."""
+    if decoder_start_token_id is None:
+        raise ValueError("Make sure to set the decoder_start_token_id attribute of the model's configuration.")
+    if pad_token_id is None:
+        raise ValueError("Make sure to set the pad_token_id attribute of the model's configuration.")
+    shifted = input_ids.new_zeros(input_ids.shape)
+    shifted[:, 1:] = input_ids[:, :-1].clone()
+    shifted[:, 0] = decoder_start_token_id
+    shifted.masked_fill_(shifted == -100, pad_token_id)
+    return shifted
+
+
+def scoring_label_mask(labels: torch.Tensor, decoder_input_ids: torch.Tensor, bos_token_id: int, eos_token_id: int):
+    """The reference's loss mask (:1935-1946): BOS labels become -100, and a cell (b, t, k) counts iff its label is not -100 and its
+    decoder input id is not eos.  labels [B, T, K], decoder_input_ids [B * K, T] -> (labels, mask [B, T, K] bool).  ptts_score
+    applies the same rule on the device; this mirror is what the tests hold against the reference."""
+    B, T, K = labels.shape
+    labels = labels.masked_fill(labels == bos_token_id, -100)
+    dec = decoder_input_ids.reshape(B, K, T).transpose(1, 2)
+    return labels, (dec != eos_token_id) & (labels != -100)
+
+
+def check_scoring_inputs(labels, decoder_input_ids, decoder_attention_mask, *, batch_size: int, num_codebooks: int, vocab_size: int,
+                         pad_token_id: int, decoder_start_token_id: int, prompt_len: int, max_position_embeddings: int):
+    """forward()'s decoder side -> (labels [B, T, K] int64 or None, decoder input [B * K, T] int64), on the inputs' device.
+
+    Without decoder_input_ids the input is shift_tokens_right(labels).transpose(1, 2) (:2820-2823).  Raises ValueError for labels
+    outside {-100} u [0, vocab_size), decoder ids outside [0, vocab_size], shapes that do not match the batch / codebooks / each
+    other, a decoder_attention_mask that is not right padding, and prompt_len + T above max_position_embeddings."""
+    B, K, V = int(batch_size), int(num_codebooks), int(vocab_size)
+
+    def integer(t, name):
+        t = torch.as_tensor(t)
+        if t.is_floating_point() or t.is_complex() or t.dtype == torch.bool:
+            raise ValueError(f"{name} must hold integer ids, got {t.dtype}")
+        return t.to(torch.int64)
+
+    if labels is None and decoder_input_ids is None:
+        raise ValueError("forward() needs `labels` or `decoder_input_ids`")
+    if labels is not None:
+        labels = integer(labels, "labels")
+        if labels.dim() != 3 or labels.shape[0] != B or labels.shape[2] != K or labels.shape[1] < 1:
+            raise ValueError(f"labels must be [batch_size = {B}, sequence_length, num_codebooks = {K}], got {tuple(labels.shape)}")
+        if not bool(((labels == -100) | ((labels >= 0) & (labels < V))).all()):
+            raise ValueError(f"labels must be -100 or lie in [0, vocab_size = {V})")
+    if decoder_input_ids is None:
+        dec = shift_tokens_right(labels, pad_token_id, decoder_start_token_id).transpose(1, 2)
+    else:
+        dec = integer(decoder_input_ids, "decoder_input_ids")
+        if dec.dim() not in (2, 3) or dec.shape[-1] < 1 or dec.numel() != B * K * dec.shape[-1] or dec.shape[0] not in (B, B * K):
+            raise ValueError(f"decoder_input_ids must be [batch_size * num_codebooks = {B * K}, T] or [{B}, {K}, T], got {tuple(dec.shape)}")
+        if labels is not None and dec.shape[-1] != labels.shape[1]:
+            raise ValueError(f"decoder_input_ids has {dec.shape[-1]} positions, labels {labels.shape[1]}")
+        lo, hi = int(dec.min()), int(dec.max())
+        if lo < 0 or hi > V:
+            raise ValueError(f"decoder_input_ids must lie in [0, vocab_size = {V}], got values in [{lo}, {hi}]")
+    dec = dec.reshape(B * K, -1).contiguous()
+    T = dec.shape[1]
+    if decoder_attention_mask is not None:
+        m = torch.as_tensor(decoder_attention_mask)
+        if tuple(m.shape) != (B, T):
+            raise ValueError(f"decoder_attention_mask must be [{B}, {T}], got {tuple(m.shape)}")
+        m = m.to(torch.int64)
+        # right padding only: under the causal mask it changes no position the loss keeps, so it is accepted and not needed
+        if not bool(((m == 0) | (m == 1)).all()) or not bool((m[:, 1:] <= m[:, :-1]).all()):
+            raise ValueError("decoder_attention_mask must be right padding (ones, then zeros)")
+    if prompt_len + T > max_position_embeddings:
+        raise ValueError(f"{prompt_len} prompt positions + {T} decoder positions exceed max_position_embeddings {max_position_embeddings}")
+    return labels, dec
+
+
 class ParlerTTSLogitsProcessor:
     """Stateful EOS gating across codebooks; HF LogitsProcessor protocol (__call__(input_ids, scores))."""
 
@@ -167,6 +240,20 @@ class DecoderEngine:
         _lib.check(_lib.lib().ptts_decoder_blob_bytes(C.byref(self.c), C.byref(n)))
         self.blob = torch.zeros(n.value, dtype=torch.uint8, device=self.device)
         self._sessions: dict[tuple, "GenSession"] = {}
+        self._heads_rm: Optional[torch.Tensor] = None
+
+    def heads_rowmajor(self) -> Optional[torch.Tensor]:
+        """The folded lm heads row-major [K * V, H] for the fused scoring kernel (bf16; None for fp32, which scores unfused).
+        A separate buffer (20 MB at Mini), made on the first scoring call."""
+        if self.dtype != torch.bfloat16:
+            return None
+        if self._heads_rm is None:
+            n = C.c_int64()
+            _lib.check(_lib.lib().ptts_lm_heads_rowmajor_bytes(C.byref(self.c), C.byref(n)))
+            buf = torch.empty(n.value, dtype=torch.uint8, device=self.device)
+            _lib.check(_lib.lib().ptts_lm_heads_rowmajor_pack(C.byref(self.c), _lib.ptr(self.blob), _lib.ptr(buf), _lib.stream_ptr()))
+            self._heads_rm = buf
+        return self._heads_rm
 
     def _pack(self, tid: int, index: int, t: torch.Tensor):
         t = t.to(device=self.device)
@@ -206,6 +293,7 @@ class DecoderEngine:
         self._pack(L.T_FINAL_LN_W, 0, need(p + "layer_norm.weight"))
         self._pack(L.T_FINAL_LN_B, 0, need(p + "layer_norm.bias"))
         _lib.check(_lib.lib().ptts_decoder_finalize(C.byref(self.c), _lib.ptr(self.blob), _lib.stream_ptr()))
+        self._heads_rm = None   # repacked from the new weights at the next scoring call
         torch.cuda.current_stream().synchronize()
         return self
 
@@ -339,6 +427,28 @@ class GenSession:
         _lib.check(_lib.lib().ptts_prefill(self.h, _lib.ptr(prompt_hidden) if self.P > 0 else None, _lib.ptr(pm),
                                            _lib.ptr(enc_hidden), _lib.ptr(em), _lib.stream_ptr()))
 
+    def score(self, prompt_hidden, prompt_mask, enc_hidden, enc_mask, dec_ids, labels, token_nll, logits=None, sums=None):
+        """ptts_score: dec_ids [B * K, T] (as given), labels [B, T, K] or None -> token_nll [B, T, K], logits [B * K, T, V] and
+        sums [K, 2] (per-codebook NLL sum and count) where given.  The session's caches are overwritten."""
+        dt, dev = self.eng.dtype, self.eng.device
+        H = self.eng.cfg.hidden_size
+        enc_hidden = enc_hidden.to(device=dev, dtype=dt).contiguous()
+        if tuple(enc_hidden.shape) != (self.B, self.S, H):
+            raise ValueError(f"encoder states must be [{self.B}, {self.S}, {H}], got {tuple(enc_hidden.shape)}")
+        if self.P > 0:
+            prompt_hidden = prompt_hidden.to(device=dev, dtype=dt).contiguous()
+            if tuple(prompt_hidden.shape) != (self.B, self.P, H):
+                raise ValueError(f"prompt states must be [{self.B}, {self.P}, {H}], got {tuple(prompt_hidden.shape)}")
+        pm = None if prompt_mask is None or self.P == 0 else prompt_mask.to(device=dev, dtype=torch.int64).contiguous()
+        em = None if enc_mask is None else enc_mask.to(device=dev, dtype=torch.int64).contiguous()
+        dec_ids = dec_ids.to(device=dev, dtype=torch.int64).contiguous()
+        labels = None if labels is None else labels.to(device=dev, dtype=torch.int64).contiguous()
+        heads = self.eng.heads_rowmajor() if (labels is not None and logits is None) else None
+        self._keep = [prompt_hidden, enc_hidden, pm, em, dec_ids, labels]
+        _lib.check(_lib.lib().ptts_score(self.h, _lib.ptr(prompt_hidden) if self.P > 0 else None, _lib.ptr(pm), _lib.ptr(enc_hidden),
+                                         _lib.ptr(em), _lib.ptr(dec_ids), _lib.ptr(labels), int(dec_ids.shape[1]), _lib.ptr(heads),
+                                         _lib.ptr(token_nll), _lib.ptr(logits), _lib.ptr(sums), _lib.stream_ptr()))
+
     def decode_forward(self):
         _lib.check(_lib.lib().ptts_decode_forward(self.h, _lib.stream_ptr()))
 
@@ -363,6 +473,12 @@ class GenerateOutput(dict):
 
     def __setattr__(self, k, v):
         self[k] = v
+
+
+class ParlerTTSSeq2SeqLMOutput(GenerateOutput):
+    """ParlerTTSForConditionalGeneration.forward's result: loss, per_codebook_losses (K scalars), token_losses [B, T, K] (the NLL
+    of each counted label, 0 elsewhere), logits [B * K, T, V] (None when labels are given without return_logits=True) and
+    encoder_last_hidden_state."""
 
 
 class ParlerTTSCache:
@@ -722,6 +838,94 @@ class ParlerTTSForConditionalGeneration:
                     break
         cur_len = int(sess.state[0].item())
         return sess.raw_ids[:, :cur_len].clone()
+
+    # -- teacher-forced forward (scoring) ------------------------------------------------------------
+    _SCORE_SHARD = 32   # utterances per ptts_score call: the workspace is sized for one shard
+
+    @torch.no_grad()
+    def forward(self, input_ids=None, attention_mask=None, input_values=None, padding_mask=None, decoder_input_ids=None,
+                decoder_attention_mask=None, encoder_outputs=None, prompt_input_ids=None, prompt_attention_mask=None,
+                prompt_hidden_states=None, labels=None, loss_reduction: str = "mean", return_logits: bool = False, **kwargs):
+        """The reference's model call (:2695-2880) for inference-time scoring: the decoder over the prompt prefix and the T decoder
+        input columns in one prefill pass, the K lm heads over the T positions, and the loss of :1922-1974.
+
+        labels [B, T, K] (training format: delayed, -100 where ignored) give decoder_input_ids = shift_tokens_right(labels)
+        .transpose(1, 2) unless decoder_input_ids are passed ([B * K, T] or [B, K, T], used as given).  loss_reduction is "mean"
+        or "sum"; config.decoder.codebook_weights weight the codebooks as in the reference.  Returns a ParlerTTSSeq2SeqLMOutput
+        with loss, per_codebook_losses and token_losses [B, T, K] (the NLL of each counted label, 0 elsewhere: what a reranker
+        sums per utterance).  One deviation: with labels, `logits` [B * K, T, V] is filled only if return_logits=True (otherwise
+        None), because the fused kernel exists so that tensor (0.5-3 GB) is never built; without labels it is always filled.
+        decoder_attention_mask must be right padding, which changes nothing the loss keeps under the causal mask.  Training
+        (backward) is out of scope."""
+        if kwargs:
+            raise ValueError(f"forward() got arguments this path does not take: {sorted(kwargs)}")
+        if loss_reduction not in ("mean", "sum"):
+            raise ValueError(f"loss_reduction must be 'mean' or 'sum', got {loss_reduction!r}")
+        if labels is None and decoder_input_ids is None:
+            if input_values is not None:
+                raise ValueError("forward(input_values=...) without labels or decoder_input_ids: encode the audio with "
+                                 "audio_encoder.encode(...) and pass its codes as decoder_input_ids")
+            raise ValueError("forward() needs `labels` or `decoder_input_ids`")
+        if encoder_outputs is not None:
+            enc = encoder_outputs
+            enc_hidden = enc[0] if isinstance(enc, (tuple, list)) else getattr(enc, "last_hidden_state", enc)
+        else:
+            if input_ids is None:
+                raise ValueError("forward() needs `input_ids` (description) or `encoder_outputs`")
+            enc_hidden = self._encode_text(input_ids, attention_mask)
+        enc_hidden = enc_hidden.to(self.device, self.dtype)
+        if enc_hidden.dim() != 3 or enc_hidden.shape[2] != self.config.decoder.hidden_size:
+            raise ValueError(f"encoder states must be [batch, length, {self.config.decoder.hidden_size}], got {tuple(enc_hidden.shape)}")
+        B, S, _ = enc_hidden.shape
+        if attention_mask is not None and tuple(attention_mask.shape) != (B, S):
+            raise ValueError(f"attention_mask must be [{B}, {S}], got {tuple(attention_mask.shape)}")
+        prompt_hidden = prompt_hidden_states
+        if prompt_hidden is None and prompt_input_ids is not None:
+            if not self._side_loaded:
+                raise ValueError("no embed_prompts weights loaded")
+            prompt_hidden = torch.nn.functional.embedding(prompt_input_ids.to(self.device), self.embed_prompts_weight)
+        P = 0 if prompt_hidden is None else prompt_hidden.shape[1]
+        prompt_mask = prompt_attention_mask if prompt_hidden is not None else None
+        if prompt_hidden is not None and (prompt_hidden.dim() != 3 or prompt_hidden.shape[0] != B):
+            raise ValueError(f"prompt states must be [{B}, P, H], got {tuple(prompt_hidden.shape)}")
+        if prompt_mask is not None and tuple(prompt_mask.shape) != (B, P):
+            raise ValueError(f"prompt_attention_mask must be [{B}, {P}], got {tuple(prompt_mask.shape)}")
+        d = self.config.decoder
+        K, V = d.num_codebooks, d.vocab_size
+        labels, dec = check_scoring_inputs(labels, decoder_input_ids, decoder_attention_mask, batch_size=B, num_codebooks=K,
+                                           vocab_size=V, pad_token_id=self.config.pad_token_id,   # the top-level ids, as :2821
+                                           decoder_start_token_id=self.config.decoder_start_token_id, prompt_len=P,
+                                           max_position_embeddings=d.max_position_embeddings)
+        T = dec.shape[1]
+        dev = self.device
+        want_logits = labels is None or bool(return_logits)
+        token_nll = None if labels is None else torch.empty(B, T, K, dtype=torch.float32, device=dev)
+        logits = torch.empty(B * K, T, V, dtype=torch.float32, device=dev) if want_logits else None
+        n_shards = (B + self._SCORE_SHARD - 1) // self._SCORE_SHARD
+        sums = None if labels is None else torch.empty(n_shards, K, 2, dtype=torch.float32, device=dev)
+        cut = lambda t, sl: None if t is None else t[sl]
+        for i, b0 in enumerate(range(0, B, self._SCORE_SHARD)):
+            sl = slice(b0, min(B, b0 + self._SCORE_SHARD))
+            sess = self.decoder.engine.session(sl.stop - sl.start, P, S, P + T, max_input_len=T)
+            sess.score(cut(prompt_hidden, sl), cut(prompt_mask, sl), enc_hidden[sl], cut(attention_mask, sl),
+                       dec[sl.start * K:sl.stop * K], cut(labels, sl), cut(token_nll, sl),
+                       None if logits is None else logits[sl.start * K:sl.stop * K], None if sums is None else sums[i])
+        loss = per_codebook = None
+        if labels is not None:
+            # per codebook: sum (and count) over the shards, then the reference's reduction; a mean over no cell is NaN as in torch
+            tot = sums.double().sum(0)
+            per = tot[:, 0] / tot[:, 1] if loss_reduction == "mean" else tot[:, 0]
+            w = d.codebook_weights
+            if w is not None:
+                wt = torch.tensor([float(x) for x in w], dtype=torch.float64, device=dev)
+                loss = ((per * wt).sum() / wt.sum()).float()
+            else:
+                loss = (per.sum() / K).float()
+            per_codebook = [per[k].float() for k in range(K)]
+        return ParlerTTSSeq2SeqLMOutput(loss=loss, logits=logits, per_codebook_losses=per_codebook, token_losses=token_nll,
+                                        encoder_last_hidden_state=enc_hidden)
+
+    __call__ = forward
 
     # -- generate ----------------------------------------------------------------------------------
     @torch.no_grad()
