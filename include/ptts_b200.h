@@ -76,6 +76,17 @@ typedef struct ptts_gen_params {
                             * column alone).  MinNewTokens skips these columns.  ptts_generate_begin_ids sets it. */
 } ptts_gen_params;
 
+/* The further processors of transformers' _get_logits_processor, in its order: NoRepeatNGram before the EOS masks' processors,
+ * then, when sampling, MinP, Typical, Epsilon and Eta after top-p.  All zero except typical_p = 1 is off. */
+typedef struct ptts_sampling_ext {
+  int32_t no_repeat_ngram_size; /* 0 = off; greedy and sampling: bans the next id of every earlier n-gram that repeats the
+                                 * row's last n-1 ids */
+  float min_p;                  /* [0, 1]: remove p < min_p * p_max (sampling only; 0 = off) */
+  float typical_p;              /* (0, 1]: locally typical mass (sampling only; 1 = off) */
+  float epsilon_cutoff;         /* [0, 1): remove p < epsilon (sampling only; 0 = off) */
+  float eta_cutoff;             /* [0, 1): remove p < min(eta, sqrt(eta) exp(-entropy)) (sampling only; 0 = off) */
+} ptts_sampling_ext;
+
 /* Tensor ids for ptts_decoder_pack(). `index` = layer (per-layer tensors) or codebook (EMBED/LM_HEAD). */
 enum {
   PTTS_T_EMBED_TOKENS = 0, /* [vocab+1, H]  decoder.model.decoder.embed_tokens.N.weight (:1354) */
@@ -198,6 +209,13 @@ int ptts_sample(ptts_session* s, const int64_t* forced_tokens, void* stream);
 /* n_steps x (ptts_decode_forward + ptts_sample), replayed from a CUDA graph, no host sync.
  * Steps after every row finished are device-side no-ops. */
 int ptts_decode_steps(ptts_session* s, int32_t n_steps, void* stream);
+
+/* The processors of ptts_sampling_ext for the generation begun last (ptts_generate_begin* resets them to off; NULL = off).
+ * Out-of-range values give PTTS_EINVAL.  While any is active (no_repeat_ngram_size > 0, or a warper with do_sample),
+ * ptts_sample runs a sampler that applies them, and ptts_decode_steps runs every token as the decoder step without its
+ * sampling phase followed by that sampler: one launch pair per token instead of the step kernel's many tokens per launch.
+ * A row left with no candidate gets token 0 (the reference's torch.multinomial raises there). */
+int ptts_generate_set_sampling_ext(ptts_session* s, const ptts_sampling_ext* ext);
 
 /* Device pointers into the workspace (valid for the session lifetime). */
 int ptts_session_logits(ptts_session* s, float** out);          /* [B*K, V] f32, last step's raw logits */

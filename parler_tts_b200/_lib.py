@@ -33,6 +33,11 @@ class GenParamsC(C.Structure):
                 ("row_base", C.c_int32), ("input_len", C.c_int32)]
 
 
+class SamplingExtC(C.Structure):
+    _fields_ = [("no_repeat_ngram_size", C.c_int32), ("min_p", C.c_float), ("typical_p", C.c_float),
+                ("epsilon_cutoff", C.c_float), ("eta_cutoff", C.c_float)]
+
+
 class DacConfigC(C.Structure):
     _fields_ = [("n_codebooks", C.c_int32), ("codebook_size", C.c_int32), ("codebook_dim", C.c_int32),
                 ("latent_dim", C.c_int32), ("decoder_dim", C.c_int32), ("n_blocks", C.c_int32),
@@ -59,6 +64,7 @@ _SIGS = {
     "ptts_session_destroy": (C.c_int, [_VP]),
     "ptts_generate_begin": (C.c_int, [_VP, C.POINTER(GenParamsC), _VP]),
     "ptts_generate_begin_ids": (C.c_int, [_VP, C.POINTER(GenParamsC), _VP, _I32, _VP]),
+    "ptts_generate_set_sampling_ext": (C.c_int, [_VP, C.POINTER(SamplingExtC)]),
     "ptts_prefill": (C.c_int, [_VP, _VP, _VP, _VP, _VP, _VP]),
     "ptts_lm_heads_rowmajor_bytes": (C.c_int, [C.POINTER(DecoderConfigC), C.POINTER(_I64)]),
     "ptts_lm_heads_rowmajor_pack": (C.c_int, [C.POINTER(DecoderConfigC), _VP, _VP, _VP]),

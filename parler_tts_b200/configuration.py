@@ -100,7 +100,7 @@ class GenerationConfig(_Record):
                  decoder_start_token_id=None, return_dict_in_generate=False, num_beams=1, num_beam_groups=1,
                  num_return_sequences=1, repetition_penalty=1.0, no_repeat_ngram_size=0, length_penalty=1.0, typical_p=1.0,
                  epsilon_cutoff=0.0, eta_cutoff=0.0, min_length=0, penalty_alpha=None, bad_words_ids=None, force_words_ids=None,
-                 guidance_scale=None, **kwargs):
+                 guidance_scale=None, min_p=None, **kwargs):
         self.max_length = max_length
         self.max_new_tokens = max_new_tokens
         self.min_new_tokens = min_new_tokens
@@ -114,11 +114,14 @@ class GenerationConfig(_Record):
         self.decoder_start_token_id = decoder_start_token_id
         self.return_dict_in_generate = return_dict_in_generate
         self.num_beams = num_beams
+        # further processors the device loop runs (modeling.resolve_sampling_ext): n-gram bans and min_length with greedy and
+        # sampling, the min_p / typical_p / epsilon_cutoff / eta_cutoff warpers with sampling
+        self.no_repeat_ngram_size, self.min_length, self.min_p = no_repeat_ngram_size, min_length, min_p
+        self.typical_p, self.epsilon_cutoff, self.eta_cutoff = typical_p, epsilon_cutoff, eta_cutoff
         # knobs the device loop does not implement: kept so that generate() can REJECT a non-neutral value instead of
         # silently ignoring it (modeling.py::_NEUTRAL_GENERATION_KNOBS)
         self.num_beam_groups, self.num_return_sequences = num_beam_groups, num_return_sequences
-        self.repetition_penalty, self.no_repeat_ngram_size, self.length_penalty = repetition_penalty, no_repeat_ngram_size, length_penalty
-        self.typical_p, self.epsilon_cutoff, self.eta_cutoff, self.min_length = typical_p, epsilon_cutoff, eta_cutoff, min_length
+        self.repetition_penalty, self.length_penalty = repetition_penalty, length_penalty
         self.penalty_alpha, self.bad_words_ids, self.force_words_ids, self.guidance_scale = penalty_alpha, bad_words_ids, force_words_ids, guidance_scale
 
     def update(self, **kwargs) -> dict[str, Any]:

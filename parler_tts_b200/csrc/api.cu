@@ -56,7 +56,16 @@ struct ptts_session {
   long long* prof;
   DecodePath path;
   StepParams sp;     // the step kernels' parameters (DECODE_STEP, DECODE_CLUSTER)
+  ptts_sampling_ext ext;  // ptts_generate_set_sampling_ext; off after every ptts_generate_begin*
 };
+
+static const ptts_sampling_ext kExtOff = {0, 0.f, 1.f, 0.f, 0.f};
+// the sampler with the ptts_sampling_ext stages, or nullptr while none of them changes the result
+static const ptts_sampling_ext* active_ext(const ptts_session* s) {
+  const ptts_sampling_ext& x = s->ext;
+  const bool warp = s->gen.do_sample && (x.min_p > 0.f || x.typical_p < 1.f || x.epsilon_cutoff > 0.f || x.eta_cutoff > 0.f);
+  return (x.no_repeat_ngram_size > 0 || warp) ? &s->ext : nullptr;
+}
 
 extern "C" {
 
@@ -184,6 +193,7 @@ int ptts_session_create2(const ptts_decoder_config* cfg, const void* blob, void*
   s->L = make_layout(*cfg);
   s->W = make_workspace(*cfg, B, P, S, max_cache_len, max_input_len);
   s->n0 = 1;
+  s->ext = kExtOff;
   if (workspace_bytes < s->W.total) {
     int64_t need = s->W.total;
     delete s;
@@ -299,6 +309,7 @@ int ptts_generate_begin_ids(ptts_session* s, const ptts_gen_params* gen, const i
   s->gen = *gen;
   s->gen.input_len = n0;
   s->n0 = n0;
+  s->ext = kExtOff;
   PTTS_CHECK_CUDA(cudaMemcpyAsync(s->ws + s->W.gen, &s->gen, sizeof(ptts_gen_params), cudaMemcpyHostToDevice, st));
   if (int e = launch_generate_begin(sample_args(s), input_ids, n0, gen->max_length, st)) return e;
   s->begun = true;
@@ -308,6 +319,21 @@ int ptts_generate_begin_ids(ptts_session* s, const ptts_gen_params* gen, const i
 
 int ptts_generate_begin(ptts_session* s, const ptts_gen_params* gen, void* stream) {
   return ptts_generate_begin_ids(s, gen, nullptr, 1, stream);
+}
+
+int ptts_generate_set_sampling_ext(ptts_session* s, const ptts_sampling_ext* ext) {
+  PTTS_REQUIRE(s, "null argument");
+  if (!s->begun) return fail(PTTS_ESTATE, "ptts_generate_set_sampling_ext called before ptts_generate_begin");
+  const ptts_sampling_ext x = ext ? *ext : kExtOff;
+  PTTS_REQUIRE(x.no_repeat_ngram_size >= 0, "`no_repeat_ngram_size` has to be a non-negative integer, got %d", x.no_repeat_ngram_size);
+  PTTS_REQUIRE(x.min_p >= 0.f && x.min_p <= 1.f, "`min_p` has to be a float in the [0, 1] interval, got %f", x.min_p);
+  PTTS_REQUIRE(x.typical_p > 0.f && x.typical_p <= 1.f, "`typical_p` has to be a float in (0, 1] (1 = off), got %f", x.typical_p);
+  PTTS_REQUIRE(x.epsilon_cutoff >= 0.f && x.epsilon_cutoff < 1.f, "`epsilon_cutoff` has to be a float in [0, 1) (0 = off), got %f", x.epsilon_cutoff);
+  PTTS_REQUIRE(x.eta_cutoff >= 0.f && x.eta_cutoff < 1.f, "`eta_cutoff` has to be a float in [0, 1) (0 = off), got %f", x.eta_cutoff);
+  s->ext = x;
+  // the knobs are a by-value argument of the captured graph's sampler node: capture again
+  if (s->exec) { cudaGraphExecDestroy(s->exec); s->exec = nullptr; s->graph_ready = false; }
+  return PTTS_OK;
 }
 
 // Blob offset of the row-major copy (layout.h rm[]) of the layer matrix stored at blob offset woff, which the wgmma GEMM
@@ -530,13 +556,26 @@ int ptts_sample(ptts_session* s, const int64_t* forced_tokens, void* stream) {
   PTTS_REQUIRE(s, "null argument");
   if (!s->prefilled) return fail(PTTS_ESTATE, "ptts_sample called before ptts_prefill");
   s->launches++;
-  return launch_sample(sample_args(s), forced_tokens, (cudaStream_t)stream, false);
+  return launch_sample(sample_args(s), forced_tokens, (cudaStream_t)stream, false, active_ext(s));
 }
 
 int ptts_decode_steps(ptts_session* s, int32_t n_steps, void* stream) {
   PTTS_REQUIRE(s && n_steps >= 0, "bad argument");
   if (!s->prefilled) return fail(PTTS_ESTATE, "ptts_decode_steps called before ptts_prefill");
   cudaStream_t st = (cudaStream_t)stream;
+  const ptts_sampling_ext* ext = active_ext(s);
+  if (ext != nullptr && s->path != DECODE_MULTI_KERNEL) {
+    // the step kernel stops at the logits and the EXT sampler follows, token by token; both return at once after the last token
+    StepParams p = s->sp;
+    p.do_sample_phase = 0;
+    for (int i = 0; i < n_steps; i++) {
+      const int e = s->path == DECODE_CLUSTER ? launch_decode_step_cluster(p, st) : launch_decode_step(p, s->sm_count, st);
+      if (e) return e;
+      if (int e2 = launch_sample(sample_args(s), nullptr, st, false, ext)) return e2;
+    }
+    s->launches += 2 * (int64_t)n_steps;
+    return PTTS_OK;
+  }
   switch (s->path) {
     case DECODE_CLUSTER: {  // the kernel loops over tokens itself: up to PTTS_STEPS_PER_LAUNCH (default 64) per launch
       const char* env = getenv("PTTS_STEPS_PER_LAUNCH");   // (read per call: tests compare 1 against the default)
@@ -564,7 +603,7 @@ int ptts_decode_steps(ptts_session* s, int32_t n_steps, void* stream) {
     const int64_t before = s->launches;
     PTTS_CHECK_CUDA(cudaStreamBeginCapture(s->cap_stream, cudaStreamCaptureModeThreadLocal));
     int e = run_forward(s, s->cap_stream, false, nullptr, nullptr);
-    if (!e) { s->launches++; e = launch_sample(sample_args(s), nullptr, s->cap_stream, true); }
+    if (!e) { s->launches++; e = launch_sample(sample_args(s), nullptr, s->cap_stream, true, ext); }
     cudaGraph_t graph = nullptr;
     cudaError_t ce = cudaStreamEndCapture(s->cap_stream, &graph);
     s->launches = before;

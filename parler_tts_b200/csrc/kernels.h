@@ -74,7 +74,8 @@ struct SampleArgs {
   int B, K, V;
   int bos, pad, eos;
 };
-int launch_sample(const SampleArgs& a, const int64_t* forced, cudaStream_t st, bool pdl);
+// ext != nullptr: the sampler with the ptts_sampling_ext stages (the caller passes it only while one is active)
+int launch_sample(const SampleArgs& a, const int64_t* forced, cudaStream_t st, bool pdl, const ptts_sampling_ext* ext = nullptr);
 // ids == nullptr: the BOS column (n0 = 1); otherwise the BOS-led [B*K][n0] input the generation continues from
 int launch_generate_begin(const SampleArgs& a, const int64_t* ids, int n0, int max_length, cudaStream_t st);
 int launch_delay_build(const int64_t* ids, int BK, int seq, int K, int64_t bos, int64_t pad, int L, int64_t* mask, cudaStream_t st);

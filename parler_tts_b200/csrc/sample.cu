@@ -16,15 +16,15 @@
 
 namespace ptts {
 
-template <int ITEMS>
-__global__ void __launch_bounds__(SMP_THREADS) sample_kernel(SampleArgs p, const int64_t* __restrict__ forced) {
+template <int ITEMS, bool EXT>
+__device__ __forceinline__ void sample_kernel_body(const SampleArgs& p, const int64_t* __restrict__ forced, const ptts_sampling_ext& x) {
   pdl_launch_dependents();
   pdl_wait();
   if (p.ctrl->active == 0) return;
   const int row = blockIdx.x;           // one CTA per (utterance, codebook) row
   const int cur_len = p.ctrl->cur_len;  // the new token becomes column `cur_len`
   const ptts_gen_params g = *p.gen;
-  sample_row_cta<ITEMS>(p, g, forced, row, cur_len);
+  sample_rows_cta<ITEMS, 1, EXT>(p, g, forced, row, 0, row + 1, cur_len, x);
   // last block advances the control block
   __threadfence();
   __syncthreads();
@@ -43,7 +43,18 @@ __global__ void __launch_bounds__(SMP_THREADS) sample_kernel(SampleArgs p, const
   }
 }
 
-int launch_sample(const SampleArgs& a, const int64_t* forced, cudaStream_t st, bool pdl) {
+template <int ITEMS>
+__global__ void __launch_bounds__(SMP_THREADS) sample_kernel(SampleArgs p, const int64_t* __restrict__ forced) {
+  sample_kernel_body<ITEMS, false>(p, forced, ptts_sampling_ext{});
+}
+
+// the ptts_sampling_ext stages (sample_core.cuh, EXT = true); the knobs come by value, so a captured graph holds them
+template <int ITEMS, bool EXT>
+__global__ void __launch_bounds__(SMP_THREADS) sample_kernel(SampleArgs p, const int64_t* __restrict__ forced, ptts_sampling_ext x) {
+  sample_kernel_body<ITEMS, EXT>(p, forced, x);
+}
+
+int launch_sample(const SampleArgs& a, const int64_t* forced, cudaStream_t st, bool pdl, const ptts_sampling_ext* ext) {
   const int BK = a.B * a.K;
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = dim3(BK);
@@ -56,6 +67,12 @@ int launch_sample(const SampleArgs& a, const int64_t* forced, cudaStream_t st, b
   cfg.numAttrs = pdl ? 1 : 0;
   const int items = (a.V + SMP_THREADS - 1) / SMP_THREADS;
   PTTS_REQUIRE(items <= 9, "sample: vocab_size %d > 2304 not supported", a.V);
+  if (ext != nullptr) {
+    if (items <= 1) PTTS_CHECK_CUDA(cudaLaunchKernelEx(&cfg, sample_kernel<1, true>, a, forced, *ext));
+    else if (items <= 5) PTTS_CHECK_CUDA(cudaLaunchKernelEx(&cfg, sample_kernel<5, true>, a, forced, *ext));
+    else PTTS_CHECK_CUDA(cudaLaunchKernelEx(&cfg, sample_kernel<9, true>, a, forced, *ext));
+    return PTTS_OK;
+  }
   if (items <= 1) PTTS_CHECK_CUDA(cudaLaunchKernelEx(&cfg, sample_kernel<1>, a, forced));
   else if (items <= 5) PTTS_CHECK_CUDA(cudaLaunchKernelEx(&cfg, sample_kernel<5>, a, forced));
   else PTTS_CHECK_CUDA(cudaLaunchKernelEx(&cfg, sample_kernel<9>, a, forced));

@@ -46,10 +46,19 @@ __device__ __forceinline__ SmpScratch& smp_scratch() {
   __shared__ SmpScratch sc;
   return sc;
 }
+// EXT: the no_repeat_ngram bans of each row, one bit per id of the largest vocabulary a CTA takes (9 slots of 256)
+constexpr int SMP_BAN_WORDS = 9 * SMP_THREADS / 32;
+__device__ __forceinline__ uint32_t (&smp_bans())[SMP_MAX_ROWS][SMP_BAN_WORDS] {
+  __shared__ uint32_t ban[SMP_MAX_ROWS][SMP_BAN_WORDS];
+  return ban;
+}
 
-template <int ITEMS, int R>
+// EXT = true adds the ptts_sampling_ext stages (sample_kernel's second set of instantiations): the n-gram bans join the EOS masks,
+// and MinP, Typical, Epsilon and Eta run after top-p on the same arrays, each a fixed-order CTA reduction or a bitwise threshold
+// search, so draws stay bit-reproducible.  With every stage off it computes what EXT = false computes.
+template <int ITEMS, int R, bool EXT = false>
 __device__ __forceinline__ void sample_rows_cta(const SampleArgs& p, const ptts_gen_params& g, const int64_t* __restrict__ forced,
-                                                int row0, int stride, int n_rows, int cur_len) {
+                                                int row0, int stride, int n_rows, int cur_len, ptts_sampling_ext x = {}) {
   static_assert(R >= 1 && R <= SMP_MAX_ROWS, "rows per pass");
   SmpScratch& sc = smp_scratch();   // one static buffer for every instantiation inlined into a kernel
   float (&s_f)[2][SMP_MAX_ROWS][SMP_WARPS] = sc.f;
@@ -122,6 +131,32 @@ __device__ __forceinline__ void sample_rows_cta(const SampleArgs& p, const ptts_
   // the tail's inputs (thread r finishes row r): requested now, consumed after the draw
   int t_unf = 0, t_es = 0;
   if (tid < R && row0 + tid * stride < n_rows) { t_unf = p.unfinished[row0 + tid * stride]; t_es = p.eos_seen[row0 + tid * stride]; }
+  // NoRepeatNGram over the row's history, columns [0, cur_len): every i in [0, cur_len - n] whose ids[i, i + n - 1) equal the last
+  // n - 1 ids bans ids[i + n - 1].  Nothing is banned while cur_len + 1 < n.
+  const int ngram = EXT ? x.no_repeat_ngram_size : 0;
+  const bool bans = EXT && ngram > 0 && cur_len + 1 >= ngram;
+  if constexpr (EXT) {
+    if (bans) {
+      uint32_t (&ban)[SMP_MAX_ROWS][SMP_BAN_WORDS] = smp_bans();
+#pragma unroll
+      for (int r = 0; r < R; r++)
+        for (int w = tid; w < SMP_BAN_WORDS; w += SMP_THREADS) ban[r][w] = 0u;
+      __syncthreads();
+#pragma unroll
+      for (int r = 0; r < R; r++) {
+        if (!valid[r]) continue;
+        const int64_t* h = p.raw_ids + (size_t)row[r] * p.raw_ld;
+        const int64_t* tail = h + cur_len - ngram + 1;
+        for (int i = tid; i <= cur_len - ngram; i += SMP_THREADS) {
+          bool match = true;
+          for (int q = 0; q < ngram - 1 && match; q++) match = h[i + q] == tail[q];
+          const int64_t t = h[i + ngram - 1];
+          if (match && t >= 0 && t < p.V) atomicOr(&ban[r][t >> 5], 1u << (t & 31));
+        }
+      }
+      __syncthreads();
+    }
+  }
 #pragma unroll
   for (int r = 0; r < R; r++) {
     const int b = row[r] / p.K, k = row[r] - b * p.K;
@@ -145,6 +180,8 @@ __device__ __forceinline__ void sample_rows_cta(const SampleArgs& p, const ptts_
       const int i = tid + SMP_THREADS * j;
       if (mask_eos && i == p.eos) v[r][j] = -INFINITY;
       if (g.suppress_special && i >= g.codebook_size) v[r][j] = -INFINITY;
+      if constexpr (EXT)
+        if (bans && ((smp_bans()[r][i >> 5] >> (i & 31)) & 1u)) v[r][j] = -INFINITY;
     }
   }
   int tok[R];
@@ -236,6 +273,77 @@ __device__ __forceinline__ void sample_rows_cta(const SampleArgs& p, const ptts_
       }
       cta_sum_f(s);
     }
+    if constexpr (EXT) {
+      // The warpers after top-p (transformers' order: MinP, Typical, Epsilon, Eta).  Each sees the softmax of the scores the
+      // previous one left: p_j = e_j / s with e_j = exp(v_j - m).  The max is never removed, so m stays the max.
+      auto drop_where = [&](auto&& remove) {
+#pragma unroll
+        for (int r = 0; r < R; r++) {
+          const float inv = 1.0f / s[r];
+          s[r] = 0.f;
+#pragma unroll
+          for (int j = 0; j < ITEMS; j++) {
+            if (remove(r, j, inv)) { v[r][j] = -INFINITY; e[r][j] = 0.f; }
+            s[r] += e[r][j];
+          }
+        }
+        cta_sum_f(s);
+      };
+      // entropy -sum p log p of the current scores, with log p = v - m - log s (log_softmax); removed ids add nothing
+      auto entropy = [&](float (&ent)[R], float (&lse)[R]) {
+#pragma unroll
+        for (int r = 0; r < R; r++) {
+          lse[r] = m[r] + logf(s[r]);
+          ent[r] = 0.f;
+#pragma unroll
+          for (int j = 0; j < ITEMS; j++)
+            if (v[r][j] > -INFINITY) { const float lp = v[r][j] - lse[r]; ent[r] += lp * expf(lp); }
+        }
+        cta_sum_f(ent);
+#pragma unroll
+        for (int r = 0; r < R; r++) ent[r] = -ent[r];
+      };
+      if (x.min_p > 0.f)  // p < min_p * p_max; p_max = 1 / s
+        drop_where([&](int r, int j, float inv) { return e[r][j] * inv < x.min_p * inv; });
+      if (x.typical_p < 1.0f) {
+        // shifted_j = |-log p_j - H|.  Sorted ascending, the first position whose cumulative p reaches the mass gives the
+        // threshold T; ids with shifted > T go.  T is found as the key after the largest key th with mass(shifted <= th) < typical_p.
+        float ent[R], lse[R];
+        entropy(ent, lse);
+        uint32_t key[R][ITEMS], th[R];
+#pragma unroll
+        for (int r = 0; r < R; r++) {
+          th[r] = 0;
+#pragma unroll
+          for (int j = 0; j < ITEMS; j++) key[r][j] = fkey(v[r][j] > -INFINITY ? fabsf(lse[r] - v[r][j] - ent[r]) : INFINITY);
+        }
+        for (int bit = 31; bit >= 0; bit--) {
+          float c[R];
+#pragma unroll
+          for (int r = 0; r < R; r++) {
+            const uint32_t cand = th[r] | (1u << bit);
+            c[r] = 0.f;
+#pragma unroll
+            for (int j = 0; j < ITEMS; j++) c[r] += (key[r][j] <= cand) ? e[r][j] : 0.f;
+          }
+          cta_sum_f(c);
+#pragma unroll
+          for (int r = 0; r < R; r++)
+            if (c[r] < x.typical_p * s[r]) th[r] |= (1u << bit);
+        }
+        // th = 0xffffffff: the mass is never reached (rounding), the threshold is the largest shifted value and nothing goes
+        drop_where([&](int r, int j, float) { return th[r] != 0xffffffffu && key[r][j] > th[r] + 1u; });
+      }
+      if (x.epsilon_cutoff > 0.f)
+        drop_where([&](int r, int j, float inv) { return e[r][j] * inv < x.epsilon_cutoff && v[r][j] < m[r]; });
+      if (x.eta_cutoff > 0.f) {
+        float ent[R], lse[R];
+        entropy(ent, lse);
+        drop_where([&](int r, int j, float inv) {
+          return e[r][j] * inv < fminf(x.eta_cutoff, sqrtf(x.eta_cutoff) * expf(-ent[r])) && v[r][j] < m[r];
+        });
+      }
+    }
     // inverse-CDF draw in index order: CTA-wide inclusive scan per slot j (elements 256 j .. 256 j + 255)
     float target[R], carry[R];
     int found[R], last_nz[R];
@@ -291,6 +399,11 @@ __device__ __forceinline__ void sample_rows_cta(const SampleArgs& p, const ptts_
     }
 #pragma unroll
     for (int r = 0; r < R; r++) tok[r] = found[r] >= 0 ? found[r] : last_nz[r];
+    if constexpr (EXT) {  // every id removed (the bans can do that): token 0, as greedy's argmax gives
+#pragma unroll
+      for (int r = 0; r < R; r++)
+        if (tok[r] < 0) tok[r] = 0;
+    }
   } else {
     // argmax, smallest index on ties
 #pragma unroll

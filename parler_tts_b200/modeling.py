@@ -161,6 +161,92 @@ def check_scoring_inputs(labels, decoder_input_ids, decoder_attention_mask, *, b
     return labels, dec
 
 
+def resolve_sampling_ext(gc, n0: int):
+    """The further processors of transformers' `_get_logits_processor` from a GenerationConfig -> (ext, min_new_tokens).
+
+    ext is None, or the dict of ptts_sampling_ext values (off: 0 / 0 / 1 / 0 / 0) when one of them changes the result.  The
+    rules are the library's: `no_repeat_ngram_size` > 0 must be an int (<= 0 is off); `min_length` > 0 must be an int and is
+    folded into min_new_tokens = max(0, min_length - n0), which a given `min_new_tokens` overrides (`_prepare_generated_length`);
+    the warpers exist only with do_sample: `min_p` outside [0, 1] and `typical_p` <= 0 raise, `typical_p` >= 1 is off, and
+    `epsilon_cutoff` / `eta_cutoff` outside (0, 1) are off without an error."""
+    mnt = gc.min_new_tokens
+    if mnt is None:
+        ml = getattr(gc, "min_length", 0)
+        if ml is not None and ml > 0:
+            if not isinstance(ml, int):
+                raise ValueError(f"`min_length` has to be a non-negative integer, but is {ml}")
+            mnt = max(0, ml - int(n0))
+    n = getattr(gc, "no_repeat_ngram_size", 0)
+    if n is None or n <= 0:
+        n = 0
+    elif not isinstance(n, int):
+        raise ValueError(f"`ngram_size` has to be a strictly positive integer, but is {n}")
+    ext = dict(no_repeat_ngram_size=int(n), min_p=0.0, typical_p=1.0, epsilon_cutoff=0.0, eta_cutoff=0.0)
+    if gc.do_sample:
+        mp = getattr(gc, "min_p", None)
+        if mp is not None:
+            if not (0 <= mp <= 1.0):
+                raise ValueError(f"`min_p` has to be a float in the [0, 1] interval, but is {mp}")
+            ext["min_p"] = float(mp)
+        tp = getattr(gc, "typical_p", 1.0)
+        if tp is not None and tp < 1.0:
+            if not float(tp) > 0:
+                raise ValueError(f"`typical_p` has to be a float > 0 and < 1, but is {tp}")
+            ext["typical_p"] = float(tp)
+        for k in ("epsilon_cutoff", "eta_cutoff"):
+            v = getattr(gc, k, 0.0)
+            if v is not None and 0.0 < v < 1.0:
+                ext[k] = float(v)
+    active = ext["no_repeat_ngram_size"] > 0 or ext["min_p"] > 0 or ext["typical_p"] < 1 or ext["epsilon_cutoff"] > 0 or ext["eta_cutoff"] > 0
+    return (ext if active else None), int(mnt or 0)
+
+
+def no_repeat_ngram_mask(ids: torch.Tensor, scores: torch.Tensor, n: int) -> torch.Tensor:
+    """NoRepeatNGramLogitsProcessor as torch ops: ids [R, cur_len] -> scores with the ids banned by repeated n-grams at -inf."""
+    cur = ids.shape[1]
+    if n <= 0 or cur < n:   # no complete n-gram yet
+        return scores
+    win = ids.unfold(1, n, 1)                                           # [R, cur - n + 1, n]
+    match = (win[:, :, :n - 1] == ids[:, cur - n + 1:].unsqueeze(1)).all(-1)
+    nxt = win[:, :, n - 1]
+    ok = match & (nxt >= 0) & (nxt < scores.shape[1])
+    hits = torch.zeros(scores.shape, dtype=torch.int32, device=scores.device)
+    hits.scatter_add_(1, nxt.clamp(0, scores.shape[1] - 1), ok.to(torch.int32))
+    return scores.masked_fill(hits > 0, -float("inf"))
+
+
+def sampling_ext_warpers(scores: torch.Tensor, ext: dict) -> torch.Tensor:
+    """transformers' MinP, Typical, Epsilon and Eta warpers as torch ops, in that order (min_tokens_to_keep = 1)."""
+    ninf = -float("inf")
+    if ext["min_p"] > 0:
+        probs = scores.softmax(-1)
+        rm = probs < ext["min_p"] * probs.amax(-1, keepdim=True)
+        rm.scatter_(-1, probs.argmax(-1, keepdim=True), False)
+        scores = scores.masked_fill(rm, ninf)
+    if ext["typical_p"] < 1:
+        nl = torch.log_softmax(scores, -1)
+        ent = -(nl * nl.exp()).nansum(-1, keepdim=True)
+        shifted = (-nl - ent).abs()
+        ss, si = torch.sort(shifted, descending=False)
+        cum = scores.gather(-1, si).softmax(-1).cumsum(-1)
+        last = (cum < ext["typical_p"]).sum(1).clamp(max=ss.shape[-1] - 1)
+        rm = ss > ss.gather(1, last.view(-1, 1))
+        rm[..., :1] = False
+        scores = scores.masked_fill(rm.scatter(1, si, rm), ninf)
+    for k in ("epsilon_cutoff", "eta_cutoff"):
+        eps = ext[k]
+        if eps <= 0:
+            continue
+        probs = scores.softmax(-1)
+        if k == "eta_cutoff":
+            e = torch.tensor(eps, device=scores.device)
+            ent = torch.distributions.Categorical(logits=scores).entropy()
+            eps = torch.min(e, torch.sqrt(e) * torch.exp(-ent))[..., None]
+        rm = (probs < eps) & (scores < scores.amax(-1, keepdim=True))
+        scores = scores.masked_fill(rm, ninf)
+    return scores
+
+
 class ParlerTTSLogitsProcessor:
     """Stateful EOS gating across codebooks; HF LogitsProcessor protocol (__call__(input_ids, scores))."""
 
@@ -390,9 +476,11 @@ class GenSession:
         return n.value
 
     def begin(self, max_length: int, do_sample=False, temperature=1.0, top_k=0, top_p=1.0, min_new_tokens=0, seed=0,
-              suppress_special=False, codebook_size=1024, row_base=0, input_ids: Optional[torch.Tensor] = None):
+              suppress_special=False, codebook_size=1024, row_base=0, input_ids: Optional[torch.Tensor] = None,
+              ext: Optional[dict] = None):
         """input_ids: None (the BOS column) or the BOS-led decoder input [B*K, n0] the generation continues from; the history
-        then starts with its delayed form and the first sampled column is n0 (ptts_generate_begin_ids)."""
+        then starts with its delayed form and the first sampled column is n0 (ptts_generate_begin_ids).
+        ext: None, or the ptts_sampling_ext values (resolve_sampling_ext) for this generation."""
         g = _lib.GenParamsC()
         g.max_length, g.min_new_tokens, g.do_sample = int(max_length), int(min_new_tokens or 0), int(bool(do_sample))
         g.top_k, g.top_p, g.temperature = int(top_k or 0), float(1.0 if top_p is None else top_p), float(temperature or 1.0)
@@ -407,6 +495,8 @@ class GenSession:
                 raise ValueError(f"input_ids must be [{self.B * self.K}, n0], got {tuple(ids.shape)}")
             self._input_ids, self.n0 = ids, int(ids.shape[1])   # kept alive until the asynchronous begin kernel has read it
             _lib.check(_lib.lib().ptts_generate_begin_ids(self.h, C.byref(g), _lib.ptr(ids), self.n0, _lib.stream_ptr()))
+        if ext is not None:
+            _lib.check(_lib.lib().ptts_generate_set_sampling_ext(self.h, C.byref(_lib.SamplingExtC(**ext))))
         self.max_length = int(max_length)
 
     def prefill(self, prompt_hidden, prompt_mask, enc_hidden, enc_mask):
@@ -576,8 +666,7 @@ class ParlerTTSForConditionalGeneration:
                                "encoder_outputs", "input_values", "decoder_input_ids", "padding_mask", "use_cache",
                                "cache_implementation", "output_attentions", "output_hidden_states", "output_scores"})
     # GenerationConfig fields the device loop does not implement, with the value that means "off"
-    _NEUTRAL_GENERATION_KNOBS = {"num_return_sequences": 1, "num_beam_groups": 1, "repetition_penalty": 1.0, "no_repeat_ngram_size": 0,
-                                 "length_penalty": 1.0, "typical_p": 1.0, "epsilon_cutoff": 0.0, "eta_cutoff": 0.0, "min_length": 0,
+    _NEUTRAL_GENERATION_KNOBS = {"num_return_sequences": 1, "num_beam_groups": 1, "repetition_penalty": 1.0, "length_penalty": 1.0,
                                  "penalty_alpha": None, "bad_words_ids": None, "force_words_ids": None, "guidance_scale": None}
 
     def __init__(self, config: ParlerTTSConfig, device="cuda", dtype=torch.bfloat16, text_encoder=None):
@@ -728,12 +817,15 @@ class ParlerTTSForConditionalGeneration:
         return s_out.clone()
 
     # -- generate with user-supplied processors / stopping criteria --------------------------------
-    def _host_driven_loop(self, sess: "GenSession", gc, max_length, user_processors, user_criteria, streamer, seed, stream_col):
+    def _host_driven_loop(self, sess: "GenSession", gc, max_length, user_processors, user_criteria, streamer, seed, stream_col, ext,
+                          min_new_tokens):
         """One host iteration per token, like GenerationMixin._sample: the decoder step still runs on the fused kernel
         (ptts_decode_forward), the built-in processors run as their device operators (MinNewTokens as a mask,
         ParlerTTSLogitsProcessor = ptts_logits_processor), then the caller's `logits_processor` list, the HF warpers and the draw
         as torch ops on the device scores, and the token is appended with ptts_sample(forced).  Used only when the caller passes
-        processors or criteria the device loop does not know (the reference merges such lists at :3540-3552)."""
+        processors or criteria the device loop does not know (the reference merges such lists at :3540-3552).  `ext`
+        (resolve_sampling_ext) adds the n-gram bans before the EOS masks and the MinP / Typical / Epsilon / Eta warpers after
+        top-p, in transformers' order."""
         d = self.config.decoder
         K, BK = d.num_codebooks, sess.B * d.num_codebooks
         parler = ParlerTTSLogitsProcessor(d.eos_token_id, K, sess.B, self.device)
@@ -743,7 +835,9 @@ class ParlerTTSForConditionalGeneration:
         while True:
             ids = sess.raw_ids[:, :cur]
             scores = sess.logits.clone()
-            if (gc.min_new_tokens or 0) > 0 and cur - sess.n0 < gc.min_new_tokens:
+            if ext is not None:
+                scores = no_repeat_ngram_mask(ids, scores, ext["no_repeat_ngram_size"])
+            if min_new_tokens > 0 and cur - sess.n0 < min_new_tokens:
                 scores[:, d.eos_token_id] = -float("inf")
             scores = parler(ids, scores)
             for proc in user_processors:
@@ -759,6 +853,8 @@ class ParlerTTSForConditionalGeneration:
                     rem = ss.softmax(-1).cumsum(-1) <= (1 - gc.top_p)
                     rem[..., -1:] = False
                     scores = scores.masked_fill(rem.scatter(1, si, rem), -float("inf"))
+                if ext is not None:
+                    scores = sampling_ext_warpers(scores, ext)
                 nxt = torch.multinomial(scores.softmax(-1), 1, generator=gen).squeeze(1)
             else:
                 nxt = scores.argmax(-1)
@@ -787,7 +883,7 @@ class ParlerTTSForConditionalGeneration:
         return 32
 
     def _run_token_loop(self, enc_hidden, attention_mask, prompt_hidden, prompt_mask, *, gc, max_length, seed, suppress_special, row_base,
-                        streamer=None, custom=None, input_ids=None):
+                        ext, min_new_tokens, streamer=None, custom=None, input_ids=None):
         """begin + prefill + the token loop of one session; returns the raw token matrix [B * K, generated length].
         input_ids: None, or the BOS-led decoder input [B * K, n0] this shard continues from."""
         d = self.config.decoder
@@ -797,8 +893,9 @@ class ParlerTTSForConditionalGeneration:
         n0 = 1 if input_ids is None else int(input_ids.shape[1])
         sess = self.decoder.engine.session(B, P, S, P + max_length, max_input_len=n0)
         sess.begin(max_length, do_sample=gc.do_sample, temperature=gc.temperature, top_k=gc.top_k if gc.do_sample else 0,
-                   top_p=gc.top_p, min_new_tokens=gc.min_new_tokens or 0, seed=seed, suppress_special=suppress_special,
-                   codebook_size=self.config.audio_encoder.codebook_size, row_base=row_base, input_ids=input_ids)
+                   top_p=gc.top_p, min_new_tokens=min_new_tokens, seed=seed, suppress_special=suppress_special,
+                   codebook_size=self.config.audio_encoder.codebook_size, row_base=row_base, input_ids=input_ids,
+                   ext=None if custom is not None else ext)   # the host-driven loop applies them as torch ops
         stream_col = lambda col, v: v
         if streamer is not None:
             if input_ids is None:
@@ -812,7 +909,7 @@ class ParlerTTSForConditionalGeneration:
                 stream_col = lambda col, v: (torch.where(cells[:, col - n0] == -1, v, cells[:, col - n0]) if col - n0 < cells.shape[1] else v)
         sess.prefill(prompt_hidden, prompt_mask, enc_hidden, attention_mask)
         if custom is not None:
-            self._host_driven_loop(sess, gc, max_length, custom[0], custom[1], streamer, seed, stream_col)
+            self._host_driven_loop(sess, gc, max_length, custom[0], custom[1], streamer, seed, stream_col, ext, min_new_tokens)
         elif streamer is not None:
             sess.sample()
             steps_left = max_length - n0 - 1
@@ -952,8 +1049,9 @@ class ParlerTTSForConditionalGeneration:
             mk.pop(k, None)   # accepted for call compatibility: the device loop always uses its static cache
         unsupported = {k: getattr(gc, k) for k, neutral in self._NEUTRAL_GENERATION_KNOBS.items() if getattr(gc, k, neutral) != neutral}
         if unsupported:
-            raise ValueError(f"generation options {unsupported} are not supported by the device loop "
-                             "(greedy / temperature / top-k / top-p sampling with min_new_tokens only)")
+            raise ValueError(f"generation options {unsupported} are not supported by the device loop (greedy / sampling with "
+                             "temperature, top_k, top_p, min_p, typical_p, epsilon_cutoff, eta_cutoff, no_repeat_ngram_size, "
+                             "min_length and min_new_tokens only)")
         if gc.num_beams != 1:
             raise ValueError("Got incompatible mode for generation, should be one of greedy or sampling. "
                              "Ensure that beam search is de-activated by setting `num_beams=1` and `num_beam_groups=1`.")
@@ -1004,7 +1102,8 @@ class ParlerTTSForConditionalGeneration:
             raise ValueError(f"max_length must allow at least one new token, got {max_length}")
         if dec_ids is not None:
             check_continuation_length(n0, P, max_length, d.max_position_embeddings)
-        run = dict(gc=gc, max_length=max_length, seed=seed, suppress_special=suppress_special)
+        ext, min_new_tokens = resolve_sampling_ext(gc, n0)
+        run = dict(gc=gc, max_length=max_length, seed=seed, suppress_special=suppress_special, ext=ext, min_new_tokens=min_new_tokens)
         limit = self._fused_batch_limit()
         if limit is not None and B > limit and not custom_loop and streamer is None:
             # The fused decode-step kernels hold one 32-row tile: a larger batch runs as consecutive shards of <= 32 utterances through
