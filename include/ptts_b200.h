@@ -217,6 +217,18 @@ int ptts_decode_steps(ptts_session* s, int32_t n_steps, void* stream);
  * A row left with no candidate gets token 0 (the reference's torch.multinomial raises there). */
 int ptts_generate_set_sampling_ext(ptts_session* s, const ptts_sampling_ext* ext);
 
+/* generate()'s output_logits / output_scores for the generation begun last: the sampler records, for every step (step =
+ * cur_len - n0, the column it draws minus the decoder input's columns) inside [first_step, first_step + n_steps), the raw f32
+ * logits row it reads and the processed scores row the token is drawn from (after every processor and warper; removed ids are
+ * -inf).  Buffers are caller-owned device memory; slot s of row r is at ptr + (s - first_step) * step_stride + r * V floats, so a
+ * shard passes a pointer to its first row inside a whole-batch buffer.  Either pointer may be NULL; both NULL = off, which
+ * ptts_generate_begin* restores.  PTTS_EINVAL for first_step < 0, n_steps < 0 or step_stride < B*K*V.  May be called between
+ * ptts_decode_steps calls to move the window.  While set, ptts_sample and every token of ptts_decode_steps run the EXT sampler
+ * (the split path of ptts_generate_set_sampling_ext; the step kernels' own sampling phase is not used), and the multi-kernel
+ * path's graph is captured again when the window moves.  Steps after the generation stopped write nothing. */
+int ptts_generate_set_outputs(ptts_session* s, float* logits, float* scores, int32_t first_step, int32_t n_steps,
+                              int64_t step_stride);
+
 /* Device pointers into the workspace (valid for the session lifetime). */
 int ptts_session_logits(ptts_session* s, float** out);          /* [B*K, V] f32, last step's raw logits */
 int ptts_session_scores(ptts_session* s, float** out);          /* [B*K, V] f32, processed scores      */

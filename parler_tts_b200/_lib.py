@@ -65,6 +65,7 @@ _SIGS = {
     "ptts_generate_begin": (C.c_int, [_VP, C.POINTER(GenParamsC), _VP]),
     "ptts_generate_begin_ids": (C.c_int, [_VP, C.POINTER(GenParamsC), _VP, _I32, _VP]),
     "ptts_generate_set_sampling_ext": (C.c_int, [_VP, C.POINTER(SamplingExtC)]),
+    "ptts_generate_set_outputs": (C.c_int, [_VP, _VP, _VP, _I32, _I32, _I64]),
     "ptts_prefill": (C.c_int, [_VP, _VP, _VP, _VP, _VP, _VP]),
     "ptts_lm_heads_rowmajor_bytes": (C.c_int, [C.POINTER(DecoderConfigC), C.POINTER(_I64)]),
     "ptts_lm_heads_rowmajor_pack": (C.c_int, [C.POINTER(DecoderConfigC), _VP, _VP, _VP]),

@@ -57,6 +57,7 @@ struct ptts_session {
   DecodePath path;
   StepParams sp;     // the step kernels' parameters (DECODE_STEP, DECODE_CLUSTER)
   ptts_sampling_ext ext;  // ptts_generate_set_sampling_ext; off after every ptts_generate_begin*
+  SampleOut out;          // ptts_generate_set_outputs; off (both pointers null) after every ptts_generate_begin*
 };
 
 static const ptts_sampling_ext kExtOff = {0, 0.f, 1.f, 0.f, 0.f};
@@ -65,6 +66,16 @@ static const ptts_sampling_ext* active_ext(const ptts_session* s) {
   const ptts_sampling_ext& x = s->ext;
   const bool warp = s->gen.do_sample && (x.min_p > 0.f || x.typical_p < 1.f || x.epsilon_cutoff > 0.f || x.eta_cutoff > 0.f);
   return (x.no_repeat_ngram_size > 0 || warp) ? &s->ext : nullptr;
+}
+// the per-step outputs, or nullptr while none is set
+static const SampleOut* active_out(const ptts_session* s) {
+  return (s->out.logits != nullptr || s->out.scores != nullptr) ? &s->out : nullptr;
+}
+// the knobs of the EXT sampler, or nullptr for the plain one: the outputs are recorded by the EXT sampler, with every stage off
+// when none is active (it then computes what the plain sampler computes)
+static const ptts_sampling_ext* sampler_ext(const ptts_session* s) {
+  const ptts_sampling_ext* x = active_ext(s);
+  return (x == nullptr && active_out(s) != nullptr) ? &kExtOff : x;
 }
 
 extern "C" {
@@ -194,6 +205,7 @@ int ptts_session_create2(const ptts_decoder_config* cfg, const void* blob, void*
   s->W = make_workspace(*cfg, B, P, S, max_cache_len, max_input_len);
   s->n0 = 1;
   s->ext = kExtOff;
+  s->out = SampleOut{};
   if (workspace_bytes < s->W.total) {
     int64_t need = s->W.total;
     delete s;
@@ -310,6 +322,7 @@ int ptts_generate_begin_ids(ptts_session* s, const ptts_gen_params* gen, const i
   s->gen.input_len = n0;
   s->n0 = n0;
   s->ext = kExtOff;
+  s->out = SampleOut{};
   PTTS_CHECK_CUDA(cudaMemcpyAsync(s->ws + s->W.gen, &s->gen, sizeof(ptts_gen_params), cudaMemcpyHostToDevice, st));
   if (int e = launch_generate_begin(sample_args(s), input_ids, n0, gen->max_length, st)) return e;
   s->begun = true;
@@ -333,6 +346,24 @@ int ptts_generate_set_sampling_ext(ptts_session* s, const ptts_sampling_ext* ext
   s->ext = x;
   // the knobs are a by-value argument of the captured graph's sampler node: capture again
   if (s->exec) { cudaGraphExecDestroy(s->exec); s->exec = nullptr; s->graph_ready = false; }
+  return PTTS_OK;
+}
+
+int ptts_generate_set_outputs(ptts_session* s, float* logits, float* scores, int32_t first_step, int32_t n_steps, int64_t step_stride) {
+  PTTS_REQUIRE(s, "null argument");
+  if (!s->begun) return fail(PTTS_ESTATE, "ptts_generate_set_outputs called before ptts_generate_begin");
+  PTTS_REQUIRE(first_step >= 0 && n_steps >= 0, "outputs: the window needs first_step >= 0 and n_steps >= 0, got %d and %d", first_step, n_steps);
+  SampleOut o{};
+  if (logits != nullptr || scores != nullptr) {
+    const int64_t rows = (int64_t)s->W.B * s->cfg.num_codebooks * s->cfg.vocab_size;
+    PTTS_REQUIRE(step_stride >= rows, "outputs: step_stride %lld is below the session's B*K*V = %lld floats", (long long)step_stride, (long long)rows);
+    o = SampleOut{logits, scores, first_step, n_steps, step_stride};
+  }
+  const bool same = o.logits == s->out.logits && o.scores == s->out.scores && o.first_step == s->out.first_step &&
+                    o.n_steps == s->out.n_steps && o.step_stride == s->out.step_stride;
+  s->out = o;
+  // the window is a by-value argument of the captured graph's sampler node: capture again when it moved
+  if (!same && s->exec) { cudaGraphExecDestroy(s->exec); s->exec = nullptr; s->graph_ready = false; }
   return PTTS_OK;
 }
 
@@ -556,22 +587,24 @@ int ptts_sample(ptts_session* s, const int64_t* forced_tokens, void* stream) {
   PTTS_REQUIRE(s, "null argument");
   if (!s->prefilled) return fail(PTTS_ESTATE, "ptts_sample called before ptts_prefill");
   s->launches++;
-  return launch_sample(sample_args(s), forced_tokens, (cudaStream_t)stream, false, active_ext(s));
+  return launch_sample(sample_args(s), forced_tokens, (cudaStream_t)stream, false, sampler_ext(s), active_out(s));
 }
 
 int ptts_decode_steps(ptts_session* s, int32_t n_steps, void* stream) {
   PTTS_REQUIRE(s && n_steps >= 0, "bad argument");
   if (!s->prefilled) return fail(PTTS_ESTATE, "ptts_decode_steps called before ptts_prefill");
   cudaStream_t st = (cudaStream_t)stream;
-  const ptts_sampling_ext* ext = active_ext(s);
+  const ptts_sampling_ext* ext = sampler_ext(s);
+  const SampleOut* out = active_out(s);
   if (ext != nullptr && s->path != DECODE_MULTI_KERNEL) {
-    // the step kernel stops at the logits and the EXT sampler follows, token by token; both return at once after the last token
+    // an EXT stage is active or the outputs are set: the step kernel stops at the logits and the EXT sampler follows, token by
+    // token; both return at once after the last token
     StepParams p = s->sp;
     p.do_sample_phase = 0;
     for (int i = 0; i < n_steps; i++) {
       const int e = s->path == DECODE_CLUSTER ? launch_decode_step_cluster(p, st) : launch_decode_step(p, s->sm_count, st);
       if (e) return e;
-      if (int e2 = launch_sample(sample_args(s), nullptr, st, false, ext)) return e2;
+      if (int e2 = launch_sample(sample_args(s), nullptr, st, false, ext, out)) return e2;
     }
     s->launches += 2 * (int64_t)n_steps;
     return PTTS_OK;
@@ -603,7 +636,7 @@ int ptts_decode_steps(ptts_session* s, int32_t n_steps, void* stream) {
     const int64_t before = s->launches;
     PTTS_CHECK_CUDA(cudaStreamBeginCapture(s->cap_stream, cudaStreamCaptureModeThreadLocal));
     int e = run_forward(s, s->cap_stream, false, nullptr, nullptr);
-    if (!e) { s->launches++; e = launch_sample(sample_args(s), nullptr, s->cap_stream, true, ext); }
+    if (!e) { s->launches++; e = launch_sample(sample_args(s), nullptr, s->cap_stream, true, ext, out); }
     cudaGraph_t graph = nullptr;
     cudaError_t ce = cudaStreamEndCapture(s->cap_stream, &graph);
     s->launches = before;

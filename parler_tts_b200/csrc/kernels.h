@@ -74,8 +74,16 @@ struct SampleArgs {
   int B, K, V;
   int bos, pad, eos;
 };
-// ext != nullptr: the sampler with the ptts_sampling_ext stages (the caller passes it only while one is active)
-int launch_sample(const SampleArgs& a, const int64_t* forced, cudaStream_t st, bool pdl, const ptts_sampling_ext* ext = nullptr);
+// generate()'s per-step outputs (ptts_generate_set_outputs): slot s of row r lives at ptr + (s - first_step) * step_stride + r * V
+struct SampleOut {
+  float* logits; float* scores;  // either may be nullptr
+  int first_step, n_steps;       // the window of steps (step = cur_len - input_len) that are recorded
+  int64_t step_stride;           // floats between consecutive slots
+};
+// ext != nullptr: the sampler with the ptts_sampling_ext stages (the caller passes it while one is active, or all off while out is
+// set); out != nullptr (needs ext): that sampler also records the raw logits and the processed scores of the steps in its window
+int launch_sample(const SampleArgs& a, const int64_t* forced, cudaStream_t st, bool pdl, const ptts_sampling_ext* ext = nullptr,
+                  const SampleOut* out = nullptr);
 // ids == nullptr: the BOS column (n0 = 1); otherwise the BOS-led [B*K][n0] input the generation continues from
 int launch_generate_begin(const SampleArgs& a, const int64_t* ids, int n0, int max_length, cudaStream_t st);
 int launch_delay_build(const int64_t* ids, int BK, int seq, int K, int64_t bos, int64_t pad, int L, int64_t* mask, cudaStream_t st);

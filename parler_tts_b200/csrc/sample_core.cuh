@@ -55,10 +55,13 @@ __device__ __forceinline__ uint32_t (&smp_bans())[SMP_MAX_ROWS][SMP_BAN_WORDS] {
 
 // EXT = true adds the ptts_sampling_ext stages (sample_kernel's second set of instantiations): the n-gram bans join the EOS masks,
 // and MinP, Typical, Epsilon and Eta run after top-p on the same arrays, each a fixed-order CTA reduction or a bitwise threshold
-// search, so draws stay bit-reproducible.  With every stage off it computes what EXT = false computes.
+// search, so draws stay bit-reproducible.  With every stage off it computes what EXT = false computes.  EXT = true also records
+// generate()'s per-step outputs when the step (cur_len - input_len) lies in o's window: the raw row as loaded, and the final
+// processed row where p.scores gets it.
 template <int ITEMS, int R, bool EXT = false>
 __device__ __forceinline__ void sample_rows_cta(const SampleArgs& p, const ptts_gen_params& g, const int64_t* __restrict__ forced,
-                                                int row0, int stride, int n_rows, int cur_len, ptts_sampling_ext x = {}) {
+                                                int row0, int stride, int n_rows, int cur_len, ptts_sampling_ext x = {},
+                                                SampleOut o = {}) {
   static_assert(R >= 1 && R <= SMP_MAX_ROWS, "rows per pass");
   SmpScratch& sc = smp_scratch();   // one static buffer for every instantiation inlined into a kernel
   float (&s_f)[2][SMP_MAX_ROWS][SMP_WARPS] = sc.f;
@@ -126,6 +129,24 @@ __device__ __forceinline__ void sample_rows_cta(const SampleArgs& p, const ptts_
     for (int j = 0; j < ITEMS; j++) {
       const int i = tid + SMP_THREADS * j;
       v[r][j] = (valid[r] && i < p.V) ? __ldcg(p.logits + (size_t)row[r] * p.V + i) : -INFINITY;  // written by other CTAs of this launch: L2, not L1
+    }
+  }
+  // this step's slot of row r in an output buffer of o (nullptr: not recorded); recomputed where used, nothing stays live
+  auto out_row = [&](float* base, int r) -> float* {
+    const int step = cur_len - (g.input_len > 1 ? g.input_len : 1);
+    if (base == nullptr || !valid[r] || step < o.first_step || step - o.first_step >= o.n_steps) return nullptr;
+    return base + (int64_t)(step - o.first_step) * o.step_stride + (int64_t)row[r] * p.V;
+  };
+  if constexpr (EXT) {  // the raw rows, before any processor (streaming stores: the host reads them after the loop)
+#pragma unroll
+    for (int r = 0; r < R; r++) {
+      if (float* dst = out_row(o.logits, r)) {
+#pragma unroll
+        for (int j = 0; j < ITEMS; j++) {
+          const int i = tid + SMP_THREADS * j;
+          if (i < p.V) __stcs(dst + i, v[r][j]);
+        }
+      }
     }
   }
   // the tail's inputs (thread r finishes row r): requested now, consumed after the draw
@@ -445,6 +466,15 @@ __device__ __forceinline__ void sample_rows_cta(const SampleArgs& p, const ptts_
     for (int j = 0; j < ITEMS; j++) {
       const int i = tid + SMP_THREADS * j;
       if (i < p.V) p.scores[(size_t)row[r] * p.V + i] = v[r][j];
+    }
+    if constexpr (EXT) {
+      if (float* dst = out_row(o.scores, r)) {
+#pragma unroll
+        for (int j = 0; j < ITEMS; j++) {
+          const int i = tid + SMP_THREADS * j;
+          if (i < p.V) __stcs(dst + i, v[r][j]);
+        }
+      }
     }
   }
   // thread r finishes row r (the rows are independent: each owns its entries of every array below)

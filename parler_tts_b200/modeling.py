@@ -420,6 +420,7 @@ class GenSession:
         self.K, self.V = eng.cfg.num_codebooks, eng.cfg.vocab_size
         self._keep: list[Any] = []
         self._forced = None
+        self._outputs = None
         self._input_ids = None
         self.n0 = 1
 
@@ -497,6 +498,7 @@ class GenSession:
             _lib.check(_lib.lib().ptts_generate_begin_ids(self.h, C.byref(g), _lib.ptr(ids), self.n0, _lib.stream_ptr()))
         if ext is not None:
             _lib.check(_lib.lib().ptts_generate_set_sampling_ext(self.h, C.byref(_lib.SamplingExtC(**ext))))
+        self._outputs = None   # the begin calls switch the per-step outputs off
         self.max_length = int(max_length)
 
     def prefill(self, prompt_hidden, prompt_mask, enc_hidden, enc_mask):
@@ -549,6 +551,71 @@ class GenSession:
 
     def decode_steps(self, n: int):
         _lib.check(_lib.lib().ptts_decode_steps(self.h, int(n), _lib.stream_ptr()))
+
+    def set_outputs(self, logits: Optional[torch.Tensor], scores: Optional[torch.Tensor], first_step: int = 0, n_steps: int = 0,
+                    step_stride: int = 0):
+        """ptts_generate_set_outputs: the sampler records the raw logits and the processed scores of steps [first_step, first_step
+        + n_steps) from the first element of `logits` / `scores` (fp32 CUDA tensors or views; None = not recorded), slot s of row r
+        at (s - first_step) * step_stride + r * V floats.  Both None switches it off; generate_begin does too."""
+        def addr(t):
+            if t is None:
+                return None
+            if not t.is_cuda or t.dtype != torch.float32:
+                raise ValueError("the output buffers must be float32 CUDA tensors")
+            return C.c_void_p(t.data_ptr())
+        self._outputs = (logits, scores)   # the buffers stay alive while the sampler may write them
+        _lib.check(_lib.lib().ptts_generate_set_outputs(self.h, addr(logits), addr(scores), int(first_step), int(n_steps),
+                                                        int(step_stride)))
+
+
+def output_window(step: int, chunk: int) -> tuple[int, int]:
+    """The chunk of generate()'s per-step outputs that holds `step`: (index, first step)."""
+    return step // chunk, (step // chunk) * chunk
+
+
+def steps_in_window(step: int, steps_left: int, chunk: int) -> int:
+    """Decode steps to enqueue from `step` on: up to steps_left, without crossing a chunk boundary, so one ptts_decode_steps call
+    writes inside one output window."""
+    return min(chunk - step % chunk, steps_left)
+
+
+class StepOutputs:
+    """generate()'s `scores` / `logits`: one fp32 [rows, V] block per generated column, kept in chunks of CHUNK steps (the device
+    loop's chunk).  A chunk is allocated NaN-filled when a loop first reaches it, so nothing is sized by max_length up front.  The
+    shards of one batch share the chunks and write their own rows; a shard that ended leaves its rows NaN."""
+    CHUNK = 64
+
+    def __init__(self, rows: int, vocab_size: int, device, scores: bool, logits: bool):
+        self.rows, self.V, self.device = int(rows), int(vocab_size), device
+        self.chunks = {k: [] for k, on in (("scores", scores), ("logits", logits)) if on}
+
+    def chunk(self, c: int) -> dict:
+        for lst in self.chunks.values():
+            while len(lst) <= c:
+                lst.append(torch.full((self.CHUNK, self.rows, self.V), float("nan"), dtype=torch.float32, device=self.device))
+        return {k: lst[c] for k, lst in self.chunks.items()}
+
+    def set_window(self, sess: "GenSession", step: int, row0: int):
+        """Points the session's sampler at the chunk holding `step`, at this shard's first row row0."""
+        c, first = output_window(step, self.CHUNK)
+        ch = self.chunk(c)
+        at = lambda k: ch[k][0, row0] if k in ch else None
+        sess.set_outputs(at("logits"), at("scores"), first, self.CHUNK, self.rows * self.V)
+
+    def put(self, step: int, row0: int, logits: torch.Tensor, scores: torch.Tensor):
+        """Stores one step's rows from torch (the host-driven loop)."""
+        c, first = output_window(step, self.CHUNK)
+        ch = self.chunk(c)
+        for k, t in (("logits", logits), ("scores", scores)):
+            if k in ch:
+                ch[k][step - first, row0:row0 + t.shape[0]].copy_(t)
+
+    def result(self, n_steps: int) -> dict:
+        """{"scores": tuple of n_steps [rows, V] views, "logits": ...} for the outputs asked for."""
+        C_ = self.CHUNK
+        if n_steps > 0:
+            self.chunk((n_steps - 1) // C_)
+        return {k: tuple(lst[t // C_][t % C_] for t in range(n_steps)) for k, lst in self.chunks.items()}
 
 
 # ---- model classes -------------------------------------------------------------------------------
@@ -664,7 +731,7 @@ class ParlerTTSForConditionalGeneration:
     # model kwargs generate() understands (reference: _validate_model_kwargs over forward()'s signature)
     _MODEL_KWARGS = frozenset({"input_ids", "attention_mask", "prompt_input_ids", "prompt_attention_mask", "prompt_hidden_states",
                                "encoder_outputs", "input_values", "decoder_input_ids", "padding_mask", "use_cache",
-                               "cache_implementation", "output_attentions", "output_hidden_states", "output_scores"})
+                               "cache_implementation", "output_attentions", "output_hidden_states"})
     # GenerationConfig fields the device loop does not implement, with the value that means "off"
     _NEUTRAL_GENERATION_KNOBS = {"num_return_sequences": 1, "num_beam_groups": 1, "repetition_penalty": 1.0, "length_penalty": 1.0,
                                  "penalty_alpha": None, "bad_words_ids": None, "force_words_ids": None, "guidance_scale": None}
@@ -818,14 +885,14 @@ class ParlerTTSForConditionalGeneration:
 
     # -- generate with user-supplied processors / stopping criteria --------------------------------
     def _host_driven_loop(self, sess: "GenSession", gc, max_length, user_processors, user_criteria, streamer, seed, stream_col, ext,
-                          min_new_tokens):
+                          min_new_tokens, outputs=None, out_row=0):
         """One host iteration per token, like GenerationMixin._sample: the decoder step still runs on the fused kernel
         (ptts_decode_forward), the built-in processors run as their device operators (MinNewTokens as a mask,
         ParlerTTSLogitsProcessor = ptts_logits_processor), then the caller's `logits_processor` list, the HF warpers and the draw
         as torch ops on the device scores, and the token is appended with ptts_sample(forced).  Used only when the caller passes
         processors or criteria the device loop does not know (the reference merges such lists at :3540-3552).  `ext`
         (resolve_sampling_ext) adds the n-gram bans before the EOS masks and the MinP / Typical / Epsilon / Eta warpers after
-        top-p, in transformers' order."""
+        top-p, in transformers' order.  `outputs` (StepOutputs) records each step's raw logits and final scores before the draw."""
         d = self.config.decoder
         K, BK = d.num_codebooks, sess.B * d.num_codebooks
         parler = ParlerTTSLogitsProcessor(d.eos_token_id, K, sess.B, self.device)
@@ -855,6 +922,9 @@ class ParlerTTSForConditionalGeneration:
                     scores = scores.masked_fill(rem.scatter(1, si, rem), -float("inf"))
                 if ext is not None:
                     scores = sampling_ext_warpers(scores, ext)
+            if outputs is not None:
+                outputs.put(cur - sess.n0, out_row, sess.logits, scores)
+            if gc.do_sample:
                 nxt = torch.multinomial(scores.softmax(-1), 1, generator=gen).squeeze(1)
             else:
                 nxt = scores.argmax(-1)
@@ -883,9 +953,11 @@ class ParlerTTSForConditionalGeneration:
         return 32
 
     def _run_token_loop(self, enc_hidden, attention_mask, prompt_hidden, prompt_mask, *, gc, max_length, seed, suppress_special, row_base,
-                        ext, min_new_tokens, streamer=None, custom=None, input_ids=None):
+                        ext, min_new_tokens, streamer=None, custom=None, input_ids=None, outputs=None, out_row=0):
         """begin + prefill + the token loop of one session; returns the raw token matrix [B * K, generated length].
-        input_ids: None, or the BOS-led decoder input [B * K, n0] this shard continues from."""
+        input_ids: None, or the BOS-led decoder input [B * K, n0] this shard continues from.
+        outputs: None, or the StepOutputs this session's rows (from row out_row of the batch) are recorded into.  The device
+        loop then sets the sampler's window before every call and keeps each call inside one chunk."""
         d = self.config.decoder
         K = d.num_codebooks
         B, S, _ = enc_hidden.shape
@@ -908,32 +980,42 @@ class ParlerTTSForConditionalGeneration:
                 cells = pm[:, n0:n0 + K - 1]
                 stream_col = lambda col, v: (torch.where(cells[:, col - n0] == -1, v, cells[:, col - n0]) if col - n0 < cells.shape[1] else v)
         sess.prefill(prompt_hidden, prompt_mask, enc_hidden, attention_mask)
+        window = (lambda step: outputs.set_window(sess, step, out_row)) if outputs is not None else (lambda step: None)
         if custom is not None:
-            self._host_driven_loop(sess, gc, max_length, custom[0], custom[1], streamer, seed, stream_col, ext, min_new_tokens)
+            self._host_driven_loop(sess, gc, max_length, custom[0], custom[1], streamer, seed, stream_col, ext, min_new_tokens,
+                                   outputs, out_row)
         elif streamer is not None:
+            window(0)
             sess.sample()
             steps_left = max_length - n0 - 1
             # the streamer contract is one host-visible token column per step (_sample -> streamer.put(next.cpu()))
             col = n0
             streamer.put(stream_col(col, sess.raw_ids[:, col]).cpu())
             while steps_left > 0 and int(sess.state[1].item()) == 1:
+                window(col + 1 - n0)
                 sess.decode_steps(1)
                 col += 1
                 steps_left -= 1
                 streamer.put(stream_col(col, sess.raw_ids[:, col]).cpu())
             streamer.end()
         else:
+            window(0)
             sess.sample()
             steps_left = max_length - n0 - 1
             # no per-step host sync: enqueue graph replays in chunks and poll the device `active` flag between chunks
             chunk = 64
+            step = 1
             while steps_left > 0:
-                n = min(chunk, steps_left)
+                n = min(chunk, steps_left) if outputs is None else steps_in_window(step, steps_left, StepOutputs.CHUNK)
+                window(step)
                 sess.decode_steps(n)
                 steps_left -= n
+                step += n
                 if steps_left > 0 and int(sess.state[1].item()) == 0:
                     break
         cur_len = int(sess.state[0].item())
+        if outputs is not None:
+            sess.set_outputs(None, None)   # the session keeps no reference to the chunks
         return sess.raw_ids[:, :cur_len].clone()
 
     # -- teacher-forced forward (scoring) ------------------------------------------------------------
@@ -1031,6 +1113,12 @@ class ParlerTTSForConditionalGeneration:
         """Same call contract as the reference generate() (:3322-3653) for greedy / sampling modes.
 
         Extra kwargs: `seed` (Philox key for sampling, default 0), `return_codes` (also return audio codes).
+
+        With return_dict_in_generate=True, output_scores / output_logits add `scores` / `logits` as in transformers' _sample: a
+        tuple with one fp32 [B * K, V] entry per generated column (column n0 + t was drawn from entry t), the processed scores the
+        token was drawn from (-inf where removed) and the raw logits.  Rows that finished keep being recorded while the session
+        runs.  Deviation: a batch above 32 utterances runs as shards of 32, and a shard that ended holds NaN in both up to the
+        longest shard's end.  output_attentions / output_hidden_states are accepted and ignored.
         """
         import copy
         gc = copy.deepcopy(generation_config if generation_config is not None else self.generation_config)
@@ -1045,7 +1133,7 @@ class ParlerTTSForConditionalGeneration:
         if unknown:
             raise ValueError(f"The following `model_kwargs` are not used by the model: {unknown} (note: typos in the generate "
                              "arguments will also show up in this list)")
-        for k in ("use_cache", "cache_implementation", "output_attentions", "output_hidden_states", "output_scores"):
+        for k in ("use_cache", "cache_implementation", "output_attentions", "output_hidden_states"):
             mk.pop(k, None)   # accepted for call compatibility: the device loop always uses its static cache
         unsupported = {k: getattr(gc, k) for k, neutral in self._NEUTRAL_GENERATION_KNOBS.items() if getattr(gc, k, neutral) != neutral}
         if unsupported:
@@ -1104,6 +1192,10 @@ class ParlerTTSForConditionalGeneration:
             check_continuation_length(n0, P, max_length, d.max_position_embeddings)
         ext, min_new_tokens = resolve_sampling_ext(gc, n0)
         run = dict(gc=gc, max_length=max_length, seed=seed, suppress_special=suppress_special, ext=ext, min_new_tokens=min_new_tokens)
+        # output_scores / output_logits exist only in the dict return, as in transformers; without it nothing is recorded
+        want_scores = bool(gc.return_dict_in_generate and gc.output_scores)
+        want_logits = bool(gc.return_dict_in_generate and gc.output_logits)
+        outputs = StepOutputs(B * K, d.vocab_size, self.device, want_scores, want_logits) if (want_scores or want_logits) else None
         limit = self._fused_batch_limit()
         if limit is not None and B > limit and not custom_loop and streamer is None:
             # The fused decode-step kernels hold one 32-row tile: a larger batch runs as consecutive shards of <= 32 utterances through
@@ -1115,13 +1207,14 @@ class ParlerTTSForConditionalGeneration:
                 parts.append(self._run_token_loop(enc_hidden[sl], None if attention_mask is None else attention_mask[sl],
                                                   None if prompt_hidden is None else prompt_hidden[sl],
                                                   None if prompt_mask is None else prompt_mask[sl], row_base=row_base + b0 * K,
-                                                  input_ids=None if dec_ids is None else dec_ids[sl.start * K:sl.stop * K], **run))
+                                                  input_ids=None if dec_ids is None else dec_ids[sl.start * K:sl.stop * K],
+                                                  outputs=outputs, out_row=b0 * K, **run))
             n = max(t.shape[1] for t in parts)
             output_ids = torch.cat([torch.nn.functional.pad(t, (0, n - t.shape[1]), value=d.pad_token_id) for t in parts], dim=0)
         else:
             output_ids = self._run_token_loop(enc_hidden, attention_mask, prompt_hidden, prompt_mask, row_base=row_base, streamer=streamer,
                                               custom=(logits_processor or [], stopping_criteria or []) if custom_loop else None,
-                                              input_ids=dec_ids, **run)
+                                              input_ids=dec_ids, outputs=outputs, **run)
 
         # apply the stashed delay mask, then keep only the free cells (:3586-3597); both masks come from the whole decoder input,
         # so a continuation's codes begin with its prefix frames
@@ -1157,6 +1250,9 @@ class ParlerTTSForConditionalGeneration:
             output_values = torch.nn.utils.rnn.pad_sequence(outs, batch_first=True, padding_value=0)
         if gc.return_dict_in_generate or return_codes:
             out = GenerateOutput(sequences=output_values, audios_length=lengths, audio_codes=codes, raw_ids=output_ids)
+            if outputs is not None:   # one entry per generated column: column n0 + t was drawn from entry t
+                rec = outputs.result(output_ids.shape[1] - n0)
+                out.update(scores=rec.get("scores"), logits=rec.get("logits"))
             if gc.return_dict_in_generate:
                 return out
             return output_values, out
