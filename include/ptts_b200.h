@@ -229,6 +229,26 @@ int ptts_generate_set_sampling_ext(ptts_session* s, const ptts_sampling_ext* ext
 int ptts_generate_set_outputs(ptts_session* s, float* logits, float* scores, int32_t first_step, int32_t n_steps,
                               int64_t step_stride);
 
+/* output_attentions / output_hidden_states: the decoder passes write, for every step inside [first_step, first_step + n_steps)
+ * (step 0 = the prefill of ptts_prefill or ptts_score, with q = P + n0 rows; step t >= 1 = the decode step whose token is column
+ * n0 + t, q = 1), into caller-owned device buffers in the model dtype.  Slot s (= step - first_step) starts at ptr + s * *_step
+ * elements and holds, for q rows per batch row:
+ *   self_attn  [B][L][nh][q][self_ld]   the self-attention weights of T_kv = P + n0 + step keys (the prefill: P + n0) in the
+ *                                       first T_kv elements of each row; self_ld >= the longest T_kv of the window
+ *   cross_attn [B][L][nh][q][S]         the cross-attention weights
+ *   hidden     [B][L + 1][q][H]         the residual stream after the embedding and after layers 0 .. L-2, then the final
+ *                                       LayerNorm of the last layer's output
+ * Batch rows are outermost, so a shard passes pointers to its first row inside whole-batch buffers (the step strides then span
+ * the whole batch).
+ * The weights follow the reference's eager attention (dtype scores, fp32 softmax, finfo.min mask), from the q and K the session's
+ * own attention reads; the tokens do not depend on them.  Any pointer may be NULL; all NULL = off, which ptts_generate_begin*
+ * restores.  While a window is set, ptts_decode_steps and ptts_decode_forward run the multi-kernel path (the step kernels hold
+ * no per-layer state to write out), whose graph is captured again whenever the window moves; ptts_session_fused still reports the
+ * path the session uses without one.  PTTS_EINVAL for a negative window, self_ld below the window's longest row or strides below
+ * one slot. */
+int ptts_generate_set_probes(ptts_session* s, void* self_attn, void* cross_attn, void* hidden, int32_t first_step, int32_t n_steps,
+                             int64_t self_ld, int64_t self_step, int64_t cross_step, int64_t hidden_step);
+
 /* Device pointers into the workspace (valid for the session lifetime). */
 int ptts_session_logits(ptts_session* s, float** out);          /* [B*K, V] f32, last step's raw logits */
 int ptts_session_scores(ptts_session* s, float** out);          /* [B*K, V] f32, processed scores      */
@@ -281,6 +301,14 @@ int ptts_op_attention(int32_t dtype, int32_t B, int32_t nh, int32_t nkv, int32_t
                       int32_t kv_len, int32_t capacity, int32_t rope, const void* rope_cos, const void* rope_sin, const void* qkv,
                       void* kcache, void* vcache, const int32_t* key_mask, int32_t mask_len, int32_t prefill_sweep, void* out,
                       void* stream);
+
+/* Attention weights of one layer by the eager definition of ptts_generate_set_probes, with the kernel the decoder launches for
+ * it.  Test hook.  q: [B*q_len, ldq] with head h at columns h*64 (before RoPE and scaling); kcache [B][nkv][capacity][64]
+ * swizzled as for ptts_op_attention; self (cross == 0): query row j sits at position past_len + j and sees keys 0 .. past_len + j
+ * of kv_len = past_len + q_len; cross: all kv_len keys.  key_mask as for ptts_op_attention.  out [B][nh][q_len][kv_len]. */
+int ptts_op_attention_probs(int32_t dtype, int32_t B, int32_t nh, int32_t nkv, int32_t q_len, int32_t past_len, int32_t cross,
+                            int32_t kv_len, int32_t capacity, int32_t rope, const void* rope_cos, const void* rope_sin, const void* q,
+                            int64_t ldq, const void* kcache, const int32_t* key_mask, int32_t mask_len, void* out, void* stream);
 
 /* ---- DAC decode ------------------------------------------------------------------------------ */
 typedef struct ptts_dac_config {

@@ -66,6 +66,7 @@ _SIGS = {
     "ptts_generate_begin_ids": (C.c_int, [_VP, C.POINTER(GenParamsC), _VP, _I32, _VP]),
     "ptts_generate_set_sampling_ext": (C.c_int, [_VP, C.POINTER(SamplingExtC)]),
     "ptts_generate_set_outputs": (C.c_int, [_VP, _VP, _VP, _I32, _I32, _I64]),
+    "ptts_generate_set_probes": (C.c_int, [_VP, _VP, _VP, _VP, _I32, _I32, _I64, _I64, _I64, _I64]),
     "ptts_prefill": (C.c_int, [_VP, _VP, _VP, _VP, _VP, _VP]),
     "ptts_lm_heads_rowmajor_bytes": (C.c_int, [C.POINTER(DecoderConfigC), C.POINTER(_I64)]),
     "ptts_lm_heads_rowmajor_pack": (C.c_int, [C.POINTER(DecoderConfigC), _VP, _VP, _VP]),
@@ -87,6 +88,8 @@ _SIGS = {
     "ptts_op_linear2": (C.c_int, [C.POINTER(DecoderConfigC), _VP, _I32, _I32, _VP, _I32, _I32, _I32, _VP, _VP, _I32, _VP, _VP]),
     "ptts_op_attention": (C.c_int, [_I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _VP, _VP, _VP, _VP, _VP, _VP,
                                     _I32, _I32, _VP, _VP]),
+    "ptts_op_attention_probs": (C.c_int, [_I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _VP, _VP, _VP, _I64, _VP,
+                                          _VP, _I32, _VP, _VP]),
     "ptts_dac_blob_bytes": (C.c_int, [C.POINTER(DacConfigC), C.POINTER(_I64)]),
     "ptts_dac_num_tensors": (C.c_int, [C.POINTER(DacConfigC), C.POINTER(_I32)]),
     "ptts_dac_pack": (C.c_int, [C.POINTER(DacConfigC), _VP, _I32, _VP, _I32, _I64, _VP]),

@@ -100,7 +100,8 @@ class GenerationConfig(_Record):
                  decoder_start_token_id=None, return_dict_in_generate=False, num_beams=1, num_beam_groups=1,
                  num_return_sequences=1, repetition_penalty=1.0, no_repeat_ngram_size=0, length_penalty=1.0, typical_p=1.0,
                  epsilon_cutoff=0.0, eta_cutoff=0.0, min_length=0, penalty_alpha=None, bad_words_ids=None, force_words_ids=None,
-                 guidance_scale=None, min_p=None, output_scores=False, output_logits=False, **kwargs):
+                 guidance_scale=None, min_p=None, output_scores=False, output_logits=False,
+                 output_attentions=False, output_hidden_states=False, **kwargs):
         self.max_length = max_length
         self.max_new_tokens = max_new_tokens
         self.min_new_tokens = min_new_tokens
@@ -115,6 +116,8 @@ class GenerationConfig(_Record):
         self.return_dict_in_generate = return_dict_in_generate
         # per generated column, the processed scores each token was drawn from / the raw fp32 logits (with return_dict_in_generate)
         self.output_scores, self.output_logits = output_scores, output_logits
+        # per generated column, the decoder's self- / cross-attention weights and hidden states (with return_dict_in_generate)
+        self.output_attentions, self.output_hidden_states = output_attentions, output_hidden_states
         self.num_beams = num_beams
         # further processors the device loop runs (modeling.resolve_sampling_ext): n-gram bans and min_length with greedy and
         # sampling, the min_p / typical_p / epsilon_cutoff / eta_cutoff warpers with sampling

@@ -39,6 +39,13 @@ enum DecodePath {
   DECODE_CLUSTER = 2,       // the cluster variant of that kernel (step2.cu: 6 device-wide phases per layer)
 };
 
+// ptts_generate_set_probes: slot s of each output at ptr + s * *_step elements (model dtype)
+struct ProbeWindow {
+  void* self_attn; void* cross_attn; void* hidden;
+  int first_step, n_steps;
+  int64_t self_ld, self_step, cross_step, hidden_step;
+};
+
 struct ptts_session {
   ptts_decoder_config cfg;
   DecoderLayout L;
@@ -58,6 +65,8 @@ struct ptts_session {
   StepParams sp;     // the step kernels' parameters (DECODE_STEP, DECODE_CLUSTER)
   ptts_sampling_ext ext;  // ptts_generate_set_sampling_ext; off after every ptts_generate_begin*
   SampleOut out;          // ptts_generate_set_outputs; off (both pointers null) after every ptts_generate_begin*
+  ProbeWindow probe;      // ptts_generate_set_probes; off (all pointers null) after every ptts_generate_begin*
+  int64_t graph_launches; // kernels of one replay of the captured decode graph
 };
 
 static const ptts_sampling_ext kExtOff = {0, 0.f, 1.f, 0.f, 0.f};
@@ -71,6 +80,14 @@ static const ptts_sampling_ext* active_ext(const ptts_session* s) {
 static const SampleOut* active_out(const ptts_session* s) {
   return (s->out.logits != nullptr || s->out.scores != nullptr) ? &s->out : nullptr;
 }
+// the attention / hidden-state window, or nullptr while none is set
+static const ProbeWindow* active_probe(const ptts_session* s) {
+  const ProbeWindow& w = s->probe;
+  return (w.self_attn != nullptr || w.cross_attn != nullptr || w.hidden != nullptr) ? &w : nullptr;
+}
+// the path decode steps take now: a probe window needs the per-layer kernels of the multi-kernel path
+static DecodePath decode_path(const ptts_session* s) { return active_probe(s) != nullptr ? DECODE_MULTI_KERNEL : s->path; }
+
 // the knobs of the EXT sampler, or nullptr for the plain one: the outputs are recorded by the EXT sampler, with every stage off
 // when none is active (it then computes what the plain sampler computes)
 static const ptts_sampling_ext* sampler_ext(const ptts_session* s) {
@@ -206,6 +223,8 @@ int ptts_session_create2(const ptts_decoder_config* cfg, const void* blob, void*
   s->n0 = 1;
   s->ext = kExtOff;
   s->out = SampleOut{};
+  s->probe = ProbeWindow{};
+  s->graph_launches = 0;
   if (workspace_bytes < s->W.total) {
     int64_t need = s->W.total;
     delete s;
@@ -323,6 +342,8 @@ int ptts_generate_begin_ids(ptts_session* s, const ptts_gen_params* gen, const i
   s->n0 = n0;
   s->ext = kExtOff;
   s->out = SampleOut{};
+  if (active_probe(s) && s->exec) { cudaGraphExecDestroy(s->exec); s->exec = nullptr; s->graph_ready = false; }
+  s->probe = ProbeWindow{};
   PTTS_CHECK_CUDA(cudaMemcpyAsync(s->ws + s->W.gen, &s->gen, sizeof(ptts_gen_params), cudaMemcpyHostToDevice, st));
   if (int e = launch_generate_begin(sample_args(s), input_ids, n0, gen->max_length, st)) return e;
   s->begun = true;
@@ -367,6 +388,34 @@ int ptts_generate_set_outputs(ptts_session* s, float* logits, float* scores, int
   return PTTS_OK;
 }
 
+int ptts_generate_set_probes(ptts_session* s, void* self_attn, void* cross_attn, void* hidden, int32_t first_step, int32_t n_steps,
+                             int64_t self_ld, int64_t self_step, int64_t cross_step, int64_t hidden_step) {
+  PTTS_REQUIRE(s, "null argument");
+  PTTS_REQUIRE(first_step >= 0 && n_steps >= 0, "probes: the window needs first_step >= 0 and n_steps >= 0, got %d and %d", first_step, n_steps);
+  ProbeWindow w{};
+  if (self_attn != nullptr || cross_attn != nullptr || hidden != nullptr) {
+    const WorkspaceLayout& W = s->W;
+    const DecoderLayout& L = s->L;
+    // (the prefill slot's row count P + n0 is only known when ptts_prefill / ptts_score runs: run_forward checks self_ld there)
+    PTTS_REQUIRE(first_step > 0 || n_steps <= 1, "probes: the prefill slot (step 0) takes a window of its own (n_steps 1)");
+    const int64_t longest = W.P + s->n0 + first_step + (int64_t)n_steps - 1;
+    PTTS_REQUIRE(self_attn == nullptr || first_step == 0 || self_ld >= longest, "probes: self_ld %lld is below the window's %lld keys",
+                 (long long)self_ld, (long long)longest);
+    PTTS_REQUIRE(self_attn == nullptr || n_steps <= 1 || self_step >= (int64_t)L.L * W.B * L.nh * self_ld, "probes: self_step is below one slot");
+    PTTS_REQUIRE(cross_attn == nullptr || n_steps <= 1 || cross_step >= (int64_t)L.L * W.B * L.nh * W.S, "probes: cross_step is below one slot");
+    PTTS_REQUIRE(hidden == nullptr || n_steps <= 1 || hidden_step >= (int64_t)(L.L + 1) * W.B * L.H, "probes: hidden_step is below one slot");
+    w = ProbeWindow{self_attn, cross_attn, hidden, first_step, n_steps, self_ld, self_step, cross_step, hidden_step};
+  }
+  const ProbeWindow& o = s->probe;
+  const bool same = w.self_attn == o.self_attn && w.cross_attn == o.cross_attn && w.hidden == o.hidden && w.first_step == o.first_step &&
+                    w.n_steps == o.n_steps && w.self_ld == o.self_ld && w.self_step == o.self_step && w.cross_step == o.cross_step &&
+                    w.hidden_step == o.hidden_step;
+  s->probe = w;
+  // the window is a by-value argument of the captured graph's probe nodes (and it switches the path): capture again when it moved
+  if (!same && s->exec) { cudaGraphExecDestroy(s->exec); s->exec = nullptr; s->graph_ready = false; }
+  return PTTS_OK;
+}
+
 // Blob offset of the row-major copy (layout.h rm[]) of the layer matrix stored at blob offset woff, which the wgmma GEMM
 // (gemm_tc.cu) reads; -1 when there is none (f32 model dtype, or not a layer matrix: the lm heads).
 static int64_t rowmajor_offset(const DecoderLayout& L, int64_t woff) {
@@ -406,6 +455,45 @@ static int run_forward(ptts_session* s, cudaStream_t st, bool prefill, const voi
   ea.pos_from_ctrl = prefill ? 0 : 1; ea.pos0 = 0; ea.prefix_len = P;
   if (int e = launch_embed(ea, c.dtype, st, pdl)) return e;
   s->launches++;
+
+  // output_attentions / output_hidden_states (ptts_generate_set_probes): the prefill writes slot 0 when its window holds step 0,
+  // a decode step finds its slot on the device (the graph is replayed for every step)
+  const ProbeWindow* pw = active_probe(s);
+  if (pw != nullptr && prefill && pw->first_step != 0) pw = nullptr;
+  if (pw != nullptr && prefill && pw->self_attn != nullptr && pw->self_ld < q_len)
+    return fail(PTTS_EINVAL, "probes: self_ld %lld is below the prefill's %d keys", (long long)pw->self_ld, q_len);
+  const int64_t esz = es;
+  auto probe_rows = [&](int entry, bool final_ln) -> int {
+    if (pw == nullptr || pw->hidden == nullptr) return PTTS_OK;
+    ProbeRowsArgs r{};
+    r.x = ws + W.x; r.rows = M; r.H = H;
+    if (final_ln) { r.ln_w = (const float*)(blob + L.final_ln_w); r.ln_b = (const float*)(blob + L.final_ln_b); }
+    r.eps = c.layer_norm_eps;
+    r.q_len = q_len; r.out_b = (int64_t)(L.L + 1) * q_len * H;   // [B][L+1][q][H]
+    r.out = (char*)pw->hidden + (int64_t)entry * q_len * H * esz;
+    r.ctrl = ctrl; r.n0 = s->n0; r.first_step = pw->first_step; r.n_steps = pw->n_steps; r.step_bytes = pw->hidden_step * esz;
+    s->launches++;
+    return launch_probe_rows(r, c.dtype, st);
+  };
+  auto probe_attn = [&](const AttnArgs& at, int layer) -> int {
+    void* base = at.cross ? pw->cross_attn : pw->self_attn;
+    if (base == nullptr) return PTTS_OK;
+    AttnProbeArgs p{};
+    p.q = at.q; p.ldq = at.ldq; p.q_col0 = at.q_col0;
+    p.kcache = at.kcache; p.kv_b_stride = at.kv_b_stride; p.kv_h_stride = at.kv_h_stride;
+    p.key_mask = at.key_mask; p.mask_len = at.mask_len; p.mask_ld = at.mask_ld;
+    p.B = B; p.nh = L.nh; p.nkv = at.nkv; p.q_len = q_len; p.cross = at.cross;
+    const int64_t ld = at.cross ? S : pw->self_ld;
+    p.kv_len = at.cross ? S : q_len; p.pos0 = 0; p.kv_cap = at.cross ? S : (prefill ? q_len : W.Tmax);
+    p.rope = at.rope; p.rope_cos = at.rope_cos; p.rope_sin = at.rope_sin; p.scale = at.scale;
+    p.out_q = ld; p.out_h = (int64_t)q_len * ld; p.out_b = (int64_t)L.L * L.nh * p.out_h;   // [B][L][nh][q][ld]
+    p.out = (char*)base + (int64_t)layer * L.nh * p.out_h * esz;
+    p.ctrl = ctrl; p.n0 = s->n0; p.prefix = P; p.first_step = pw->first_step; p.n_steps = pw->n_steps;
+    p.step_bytes = (at.cross ? pw->cross_step : pw->self_step) * esz;
+    s->launches++;
+    return launch_attention_probs(p, c.dtype, st);
+  };
+  if (int e = probe_rows(0, false)) return e;
 
   auto lin = [&](const void* X, int64_t ldx, int64_t woff, int N, int K, const float* lw, const float* lb, int epi,
                  const void* R, void* Y, int64_t ldy, int Mrows, int64_t coff = -1) -> int {
@@ -454,6 +542,7 @@ static int run_forward(ptts_session* s, cudaStream_t st, bool prefill, const voi
     at.scale = 0.125f;  // head_dim ** -0.5, applied inside SDPA (quirk Q1)
     if (int e = launch_attention(at, c.dtype, st, pdl, true)) return e;
     s->launches++;
+    if (pw != nullptr) { if (int e = probe_attn(at, i)) return e; }
     if (int e = lin(ws + W.attn, H, lb + L.wo, H, H, nullptr, nullptr, EPI_RESIDUAL, x, x, H, M)) return e;
     if (int e = lin(x, H, lb + L.wqc, H, H, (const float*)(blob + lb + L.ln2_w), (const float*)(blob + lb + L.ln2_b),
                     EPI_STORE, nullptr, ws + W.qc, H, M, lb + L.c_qc)) return e;
@@ -467,10 +556,12 @@ static int run_forward(ptts_session* s, cudaStream_t st, bool prefill, const voi
     ct.nkv = L.nckv; ct.cross = 1; ct.kv_len = S; ct.kv_capacity = S;
     if (int e = launch_attention(ct, c.dtype, st, pdl, true)) return e;
     s->launches++;
+    if (pw != nullptr) { if (int e = probe_attn(ct, i)) return e; }
     if (int e = lin(ws + W.attn, H, lb + L.woc, H, H, nullptr, nullptr, EPI_RESIDUAL, x, x, H, M)) return e;
     if (int e = lin(x, H, lb + L.fc1, L.F, H, (const float*)(blob + lb + L.ln3_w), (const float*)(blob + lb + L.ln3_b),
                     EPI_ACT, nullptr, ws + W.hbuf, L.F, M, lb + L.c_fc1)) return e;
     if (int e = lin(ws + W.hbuf, L.F, lb + L.fc2, H, L.F, nullptr, nullptr, EPI_RESIDUAL, x, x, H, M)) return e;
+    if (int e = probe_rows(i + 1, i == L.L - 1)) return e;   // entry L: the final LayerNorm of the last layer's output
   }
   if (!heads) return PTTS_OK;
   // final LayerNorm + K lm heads on the last position of every batch row -> f32 logits [B, K*V] == [B*K, V]
@@ -575,7 +666,7 @@ int ptts_decode_forward(ptts_session* s, void* stream) {
   cudaStream_t st = (cudaStream_t)stream;
   StepParams p = s->sp;
   p.do_sample_phase = 0;
-  switch (s->path) {
+  switch (decode_path(s)) {
     case DECODE_CLUSTER: s->launches++; return launch_decode_step_cluster(p, st);
     case DECODE_STEP: s->launches++; return launch_decode_step(p, s->sm_count, st);
     case DECODE_MULTI_KERNEL: break;
@@ -596,20 +687,21 @@ int ptts_decode_steps(ptts_session* s, int32_t n_steps, void* stream) {
   cudaStream_t st = (cudaStream_t)stream;
   const ptts_sampling_ext* ext = sampler_ext(s);
   const SampleOut* out = active_out(s);
-  if (ext != nullptr && s->path != DECODE_MULTI_KERNEL) {
+  const DecodePath path = decode_path(s);
+  if (ext != nullptr && path != DECODE_MULTI_KERNEL) {
     // an EXT stage is active or the outputs are set: the step kernel stops at the logits and the EXT sampler follows, token by
     // token; both return at once after the last token
     StepParams p = s->sp;
     p.do_sample_phase = 0;
     for (int i = 0; i < n_steps; i++) {
-      const int e = s->path == DECODE_CLUSTER ? launch_decode_step_cluster(p, st) : launch_decode_step(p, s->sm_count, st);
+      const int e = path == DECODE_CLUSTER ? launch_decode_step_cluster(p, st) : launch_decode_step(p, s->sm_count, st);
       if (e) return e;
       if (int e2 = launch_sample(sample_args(s), nullptr, st, false, ext, out)) return e2;
     }
     s->launches += 2 * (int64_t)n_steps;
     return PTTS_OK;
   }
-  switch (s->path) {
+  switch (path) {
     case DECODE_CLUSTER: {  // the kernel loops over tokens itself: up to PTTS_STEPS_PER_LAUNCH (default 64) per launch
       const char* env = getenv("PTTS_STEPS_PER_LAUNCH");   // (read per call: tests compare 1 against the default)
       const int per_launch = env ? (atoi(env) < 1 ? 1 : atoi(env)) : 64;
@@ -639,6 +731,7 @@ int ptts_decode_steps(ptts_session* s, int32_t n_steps, void* stream) {
     if (!e) { s->launches++; e = launch_sample(sample_args(s), nullptr, s->cap_stream, true, ext, out); }
     cudaGraph_t graph = nullptr;
     cudaError_t ce = cudaStreamEndCapture(s->cap_stream, &graph);
+    s->graph_launches = s->launches - before;   // embed + 8 kernels per layer + heads + sample (+ the probe kernels)
     s->launches = before;
     if (e) { if (graph) cudaGraphDestroy(graph); return e; }
     if (ce != cudaSuccess) return fail(PTTS_ECUDA, "graph capture failed: %s", cudaGetErrorString(ce));
@@ -647,9 +740,8 @@ int ptts_decode_steps(ptts_session* s, int32_t n_steps, void* stream) {
     if (ce != cudaSuccess) return fail(PTTS_ECUDA, "graph instantiate failed: %s", cudaGetErrorString(ce));
     s->graph_ready = true;
   }
-  const int per_step = 2 + 8 * s->L.L + 1;  // embed + 8 kernels/layer + heads + sample
   for (int i = 0; i < n_steps; i++) PTTS_CHECK_CUDA(cudaGraphLaunch(s->exec, st));
-  s->launches += (int64_t)per_step * n_steps;
+  s->launches += s->graph_launches * n_steps;
   return PTTS_OK;
 }
 
@@ -782,6 +874,28 @@ int ptts_op_attention(int32_t dtype, int32_t B, int32_t nh, int32_t nkv, int32_t
   a.kv_capacity = cross ? kv_len : past_len + q_len;   // keys per query at most (attention_item's score buffer)
   a.scale = 0.125f;
   return launch_attention(a, dtype, (cudaStream_t)stream, false, prefill_sweep == 0);
+}
+
+int ptts_op_attention_probs(int32_t dtype, int32_t B, int32_t nh, int32_t nkv, int32_t q_len, int32_t past_len, int32_t cross,
+                            int32_t kv_len, int32_t capacity, int32_t rope, const void* rope_cos, const void* rope_sin, const void* q,
+                            int64_t ldq, const void* kcache, const int32_t* key_mask, int32_t mask_len, void* out, void* stream) {
+  PTTS_REQUIRE(q && kcache && out, "null argument");
+  PTTS_REQUIRE(dtype == PTTS_BF16 || dtype == PTTS_F32, "op_attention_probs: dtype must be bf16 or f32");
+  PTTS_REQUIRE(B > 0 && nh > 0 && nkv > 0 && nh % nkv == 0 && q_len > 0 && past_len >= 0 && ldq >= (int64_t)nh * PTTS_HEAD_DIM,
+               "op_attention_probs: bad shape");
+  PTTS_REQUIRE(kv_len > 0 && kv_len <= capacity && (cross || kv_len == past_len + q_len),
+               "op_attention_probs: %d keys (self: past_len + q_len) in a cache of %d positions", kv_len, capacity);
+  PTTS_REQUIRE(!rope || (rope_cos && rope_sin), "op_attention_probs: rope needs both tables");
+  PTTS_REQUIRE(mask_len >= 0 && (key_mask || mask_len == 0), "op_attention_probs: bad key mask");
+  AttnProbeArgs a{};
+  a.q = q; a.ldq = ldq; a.q_col0 = 0;
+  a.kcache = kcache; a.kv_b_stride = (int64_t)nkv * capacity * PTTS_HEAD_DIM; a.kv_h_stride = (int64_t)capacity * PTTS_HEAD_DIM;
+  a.key_mask = key_mask; a.mask_len = mask_len; a.mask_ld = mask_len;
+  a.B = B; a.nh = nh; a.nkv = nkv; a.q_len = q_len; a.cross = cross ? 1 : 0;
+  a.kv_len = kv_len; a.pos0 = past_len; a.kv_cap = kv_len;
+  a.rope = rope; a.rope_cos = rope_cos; a.rope_sin = rope_sin; a.scale = 0.125f;
+  a.out = out; a.out_q = kv_len; a.out_h = (int64_t)q_len * kv_len; a.out_b = (int64_t)nh * a.out_h;
+  return launch_attention_probs(a, dtype, (cudaStream_t)stream);
 }
 
 // ---- DAC ----------------------------------------------------------------------------------------

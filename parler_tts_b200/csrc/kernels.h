@@ -48,6 +48,32 @@ struct AttnArgs {
 // prefill_tc: bf16 MHA prefill (q_len > 1) runs on the tensor-core sweep (attention_prefill_tc_kernel) rather than attention_item
 int launch_attention(const AttnArgs& a, int dtype, cudaStream_t st, bool pdl, bool prefill_tc);
 
+// ---- output_attentions / output_hidden_states (probe.cu) ----------------------------------------
+// Decode window (both structs): ctrl != nullptr -> the step is ctrl->cur_len - n0, written to out + (step - first_step) * step_bytes
+// when it lies in [first_step, first_step + n_steps), nothing otherwise or once ctrl->active is 0.  ctrl == nullptr: out as given.
+struct AttnProbeArgs {
+  const void* q; int64_t ldq; int q_col0;          // row b*q_len + j, head h at columns q_col0 + h*64 (before RoPE and scaling)
+  const void* kcache; int64_t kv_b_stride, kv_h_stride;  // K rows [..][64], swizzled (kv_swz)
+  const int* key_mask; int mask_len, mask_ld;      // keys t < mask_len with key_mask[b*mask_ld+t] == 0 are masked
+  int B, nh, nkv, q_len;
+  int cross;                                       // 1: kv_len keys, no causal mask
+  int kv_len, pos0;                                // ctrl == nullptr: keys per row, position of query row 0 (self: keys <= pos)
+  int kv_cap;                                      // upper bound on keys per row (sizes shared memory)
+  int rope; const void* rope_cos; const void* rope_sin;
+  float scale;
+  void* out; int64_t out_b, out_h, out_q;          // element strides of [B][nh][q_len][keys]; keys contiguous
+  const Ctrl* ctrl; int n0, prefix, first_step, n_steps; int64_t step_bytes;  // decode: position = prefix + cur_len - 1
+};
+int launch_attention_probs(const AttnProbeArgs& a, int dtype, cudaStream_t st);
+struct ProbeRowsArgs {
+  const void* x; int rows, H;                      // [rows][H]
+  const float* ln_w; const float* ln_b; float eps; // nullptr: copy; else the LayerNorm of each row
+  int q_len; int64_t out_b;                        // row r = b*q_len + j goes to out + b*out_b + j*H
+  void* out;
+  const Ctrl* ctrl; int n0, first_step, n_steps; int64_t step_bytes;
+};
+int launch_probe_rows(const ProbeRowsArgs& a, int dtype, cudaStream_t st);
+
 // ---- embedding (embed.cu) -----------------------------------------------------------------------
 struct EmbedArgs {
   const void* tables;  // [K][V+1][H]

@@ -421,6 +421,7 @@ class GenSession:
         self._keep: list[Any] = []
         self._forced = None
         self._outputs = None
+        self._probes = None   # the buffers of the last ptts_generate_set_probes window (None: never set)
         self._input_ids = None
         self.n0 = 1
 
@@ -568,6 +569,24 @@ class GenSession:
                                                         int(step_stride)))
 
 
+    def set_probes(self, self_attn: Optional[torch.Tensor] = None, cross_attn: Optional[torch.Tensor] = None,
+                   hidden: Optional[torch.Tensor] = None, first_step: int = 0, n_steps: int = 0, self_ld: int = 0):
+        """ptts_generate_set_probes: the decoder passes write the attention weights and hidden states of steps [first_step,
+        first_step + n_steps) (step 0: the prefill / score pass) into the given model-dtype CUDA tensors, each of which starts at
+        this session's first batch row of slot first_step and steps by its stride(0) per slot.  All None switches it off."""
+        def addr(t):
+            if t is None:
+                return None
+            if not t.is_cuda or t.dtype != self.eng.dtype:
+                raise ValueError(f"the probe buffers must be {self.eng.dtype} CUDA tensors")
+            return C.c_void_p(t.data_ptr())
+        step = lambda t: 0 if t is None or t.dim() == 0 else int(t.stride(0))
+        bufs = (self_attn, cross_attn, hidden)
+        self._probes = None if all(t is None for t in bufs) else bufs   # the buffers stay alive while the kernels may write them
+        _lib.check(_lib.lib().ptts_generate_set_probes(self.h, addr(self_attn), addr(cross_attn), addr(hidden), int(first_step),
+                                                       int(n_steps), int(self_ld), step(self_attn), step(cross_attn), step(hidden)))
+
+
 def output_window(step: int, chunk: int) -> tuple[int, int]:
     """The chunk of generate()'s per-step outputs that holds `step`: (index, first step)."""
     return step // chunk, (step // chunk) * chunk
@@ -616,6 +635,98 @@ class StepOutputs:
         if n_steps > 0:
             self.chunk((n_steps - 1) // C_)
         return {k: tuple(lst[t // C_][t % C_] for t in range(n_steps)) for k, lst in self.chunks.items()}
+
+
+class StepProbes:
+    """generate()'s output_attentions / output_hidden_states, written by the decoder passes in the model dtype.
+
+    Entry 0 (the prefill, q = P + n0 rows) has buffers of its own; the decode steps t >= 1 (q = 1) live in the chunks of
+    StepOutputs.CHUNK steps that the device loop already cuts its calls at.  Chunk c holds, per step, self-attention rows
+    [B, L, heads, T_hi(c)] with T_hi(c) = P + n0 + the chunk's last step (the longest row in it), cross-attention rows
+    [B, L, heads, S] and hidden rows [B, L + 1, H]; it is allocated NaN-filled when a loop first reaches it, and the entries are
+    views narrowed to their own T_kv = P + n0 + t.  Batch rows are outermost, so shards write their own rows; a shard that ended
+    leaves its rows NaN.  Memory is what the entries hold: the self-attention alone is L * B * heads * sum(T_kv) * 2 bytes in
+    bf16 (10 s of Parler-TTS-Mini audio, ~860 steps: ~0.3 GB per utterance, ~10 GB at B = 32), the order of the reference's."""
+    CHUNK = StepOutputs.CHUNK
+
+    def __init__(self, n_layers: int, batch: int, heads: int, S: int, H: int, P: int, n0: int, dtype, device, attentions: bool,
+                 hidden: bool, chunk: int = CHUNK):
+        """chunk: steps per chunk (generate(): StepOutputs.CHUNK; 1 for one step of the step operator, which then holds that
+        step's rows only, each exactly its T_kv long)."""
+        self.CHUNK = int(chunk)
+        self.L, self.B, self.nh, self.S, self.H, self.P, self.n0 = n_layers, batch, heads, S, H, P, n0
+        self.dtype, self.device, self.attn, self.hid = dtype, device, bool(attentions), bool(hidden)
+        self.entry0 = None
+        self.chunks: dict[int, dict] = {}
+
+    def _full(self, *shape):
+        return torch.full(shape, float("nan"), dtype=self.dtype, device=self.device)
+
+    def t_hi(self, c: int) -> int:
+        return self.P + self.n0 + (c + 1) * self.CHUNK - 1
+
+    def _entry0(self) -> dict:
+        if self.entry0 is None:
+            q, L, B = self.P + self.n0, self.L, self.B
+            self.entry0 = {}
+            if self.attn:
+                self.entry0["self"] = self._full(1, B, L, self.nh, q, q)
+                self.entry0["cross"] = self._full(1, B, L, self.nh, q, self.S)
+            if self.hid:
+                self.entry0["hidden"] = self._full(1, B, L + 1, q, self.H)
+        return self.entry0
+
+    def chunk(self, c: int) -> dict:
+        if c not in self.chunks:
+            L, B, n = self.L, self.B, self.CHUNK
+            ch = {}
+            if self.attn:
+                ch["self"] = self._full(n, B, L, self.nh, self.t_hi(c))
+                ch["cross"] = self._full(n, B, L, self.nh, self.S)
+            if self.hid:
+                ch["hidden"] = self._full(n, B, L + 1, self.H)
+            self.chunks[c] = ch
+        return self.chunks[c]
+
+    def set_prefill(self, sess: "GenSession", b0: int):
+        """Points the session's prefill at entry 0, from batch row b0 on."""
+        e = self._entry0()
+        at = lambda k: e[k][:, b0] if k in e else None
+        sess.set_probes(at("self"), at("cross"), at("hidden"), 0, 1, self.P + self.n0)
+
+    def set_window(self, sess: "GenSession", step: int, b0: int):
+        """Points the session's decode steps at the chunk holding `step` (>= 1), from batch row b0 on."""
+        c, first = output_window(step, self.CHUNK)
+        f = max(first, 1)   # (slot 0 of chunk 0 stays unused: step 0 is entry 0)
+        ch = self.chunk(c)
+        at = lambda k: ch[k][f - first:, b0] if k in ch else None
+        sess.set_probes(at("self"), at("cross"), at("hidden"), f, first + self.CHUNK - f, self.t_hi(c))
+
+    def entry(self, t: int) -> dict:
+        """Entry t: decoder_attentions / cross_attentions (tuples of L [B, heads, q, T_kv] / [B, heads, q, S]) and
+        decoder_hidden_states (a tuple of L + 1 [B, q, H]), for the outputs asked for (views; NaN where nothing was written)."""
+        L, out = self.L, {}
+        if t == 0:
+            e = self._entry0()
+            sa, ca, hs = (e.get(k) for k in ("self", "cross", "hidden"))
+            if self.attn:
+                out["decoder_attentions"] = tuple(sa[0, :, l] for l in range(L))
+                out["cross_attentions"] = tuple(ca[0, :, l] for l in range(L))
+            if self.hid:
+                out["decoder_hidden_states"] = tuple(hs[0, :, i] for i in range(L + 1))
+            return out
+        ch, i = self.chunk(t // self.CHUNK), t % self.CHUNK
+        if self.attn:
+            out["decoder_attentions"] = tuple(ch["self"][i, :, l, :, None, :self.P + self.n0 + t] for l in range(L))
+            out["cross_attentions"] = tuple(ch["cross"][i, :, l, :, None, :] for l in range(L))
+        if self.hid:
+            out["decoder_hidden_states"] = tuple(ch["hidden"][i, :, j, None, :] for j in range(L + 1))
+        return out
+
+    def result(self, n_steps: int) -> dict:
+        """The entries 0 .. n_steps - 1 as transformers' tuples (one entry per generated column)."""
+        entries = [self.entry(t) for t in range(n_steps)]
+        return {k: tuple(e[k] for e in entries) for k in (entries[0] if entries else {})}
 
 
 # ---- model classes -------------------------------------------------------------------------------
@@ -674,7 +785,8 @@ class ParlerTTSForCausalLM:
     @torch.no_grad()
     def forward(self, input_ids: torch.LongTensor = None, attention_mask=None, encoder_hidden_states=None,
                 encoder_attention_mask=None, prompt_hidden_states=None, prompt_attention_mask=None, past_key_values=None,
-                use_cache: bool = True, cache_position=None, return_dict: bool = True, max_cache_len: Optional[int] = None, **kwargs):
+                use_cache: bool = True, cache_position=None, return_dict: bool = True, max_cache_len: Optional[int] = None,
+                output_attentions: bool = False, output_hidden_states: bool = False, **kwargs):
         """The step operator an HF-style loop calls (reference :1865-1974): input_ids [B*K, 1] (delay mask already applied, as
         prepare_inputs_for_generation does at :2909) -> logits [B*K, 1, V], over a KV cache kept in `past_key_values`.
 
@@ -685,7 +797,11 @@ class ParlerTTSForCausalLM:
         * later calls: the ids are appended (ptts_sample with forced tokens) and one cached step runs on the fused kernel
           (ptts_decode_forward).
         Inputs longer than one column, `inputs_embeds`, `labels` and `use_cache=False` belong to training / the no-cache path and
-        are outside this operator (ValueError)."""
+        are outside this operator (ValueError).
+        output_attentions / output_hidden_states add this call's `attentions` / `cross_attentions` (L x [B, heads, q, T_kv] /
+        [B, heads, q, S]) and `hidden_states` (L+1 x [B, q, H]), q = P + 1 at the first call and 1 after it (the weights by the
+        reference's eager definition, see ParlerTTSForConditionalGeneration.generate); the step then runs the multi-kernel
+        path, with the same logits."""
         if kwargs.get("inputs_embeds") is not None or kwargs.get("labels") is not None or not use_cache:
             raise ValueError("ParlerTTSForCausalLM.forward on this path is the cached decode-step operator: input_ids [B*K, 1], use_cache=True")
         if input_ids is None or input_ids.dim() != 2 or input_ids.shape[1] != 1 or input_ids.shape[0] % self.num_codebooks != 0:
@@ -702,19 +818,47 @@ class ParlerTTSForCausalLM:
             sess.begin(cap - P, do_sample=False)
             if not bool((ids == self.config.bos_token_id).all()):
                 raise ValueError("the first call must feed the decoder start (BOS) column")
-            sess.prefill(prompt_hidden_states, prompt_attention_mask if P > 0 else None, encoder_hidden_states, encoder_attention_mask)
+            probes = self._probes(B, P, S, output_attentions, output_hidden_states)
+            try:
+                if probes is not None:
+                    probes.set_prefill(sess, 0)
+                sess.prefill(prompt_hidden_states, prompt_attention_mask if P > 0 else None, encoder_hidden_states, encoder_attention_mask)
+            finally:
+                if probes is not None:
+                    sess.set_probes()   # the window never outlives the call, whatever happens in it
             past_key_values = ParlerTTSCache(sess)
         else:
             if not isinstance(past_key_values, ParlerTTSCache) or past_key_values.session.B != B:
                 raise ValueError("past_key_values must be the ParlerTTSCache returned by the first call (same batch)")
             sess = past_key_values.session
             sess.sample(forced=ids)
-            sess.decode_forward()
+            step = past_key_values.steps + 1
+            probes = self._probes(B, sess.P, sess.S, output_attentions, output_hidden_states)
+            try:
+                if probes is not None:
+                    probes.set_window(sess, step, 0)
+                sess.decode_forward()
+            finally:
+                if probes is not None:
+                    sess.set_probes()
             past_key_values.steps += 1
         logits = sess.logits.clone().unsqueeze(1)   # [B*K, 1, V] fp32
         if not return_dict:
             return (logits, past_key_values)
-        return GenerateOutput(logits=logits, past_key_values=past_key_values)
+        out = GenerateOutput(logits=logits, past_key_values=past_key_values)
+        if probes is not None:
+            names = dict(decoder_attentions="attentions", cross_attentions="cross_attentions", decoder_hidden_states="hidden_states")
+            out.update({names[k]: v for k, v in probes.entry(past_key_values.steps).items()})
+        return out
+
+    def _probes(self, B, P, S, attentions, hidden):
+        """A StepProbes for one call of the step operator, or None when nothing is asked: chunks of one step, so a decode
+        step's entry is exactly its own rows (its self-attention T_kv long) and keeps nothing else alive."""
+        if not (attentions or hidden):
+            return None
+        c = self.config
+        return StepProbes(c.num_hidden_layers, B, c.num_attention_heads, S, c.hidden_size, P, 1, self.dtype, self.device,
+                          attentions, hidden, chunk=1)
 
     __call__ = forward
 
@@ -823,19 +967,21 @@ class ParlerTTSForConditionalGeneration:
         return self
 
     # -- side inputs (not replaced; PyTorch) -------------------------------------------------------
-    def _encode_text_eager(self, input_ids, attention_mask):
+    def _encode_text_eager(self, input_ids, attention_mask, flags: Optional[dict] = None):
+        """flags: None, or output_attentions / output_hidden_states for the encoder: then (states, the encoder's output)."""
         enc_mask = attention_mask
         if attention_mask is not None and attention_mask.dim() == 2:
             # the 4-D additive form HF derives from a 2-D padding mask (0 keep / finfo.min drop), built here with device ops only:
             # the library's own conversion creates CPU scalars on the way, which a CUDA-graph capture cannot contain
             edt = next(self.text_encoder.parameters()).dtype
             enc_mask = (1 - attention_mask)[:, None, None, :].to(edt) * torch.finfo(edt).min
-        h = self.text_encoder(input_ids=input_ids, attention_mask=enc_mask, return_dict=True).last_hidden_state
+        eo = self.text_encoder(input_ids=input_ids, attention_mask=enc_mask, return_dict=True, **(flags or {}))
+        h = eo.last_hidden_state
         if self.enc_to_dec_proj is not None:
             h = torch.nn.functional.linear(h, *self.enc_to_dec_proj)        # :2388-2392 / :3087-3090
         if attention_mask is not None:
             h = h * attention_mask[..., None]                               # :3092-3093
-        return h.to(self.dtype)
+        return h.to(self.dtype) if flags is None else (h.to(self.dtype), eo)
 
     def _encode_text(self, input_ids, attention_mask):
         """Description ids -> encoder_hidden_states (reference :3048-3097): T5 encoder + enc_to_dec_proj + mask multiply.
@@ -885,14 +1031,15 @@ class ParlerTTSForConditionalGeneration:
 
     # -- generate with user-supplied processors / stopping criteria --------------------------------
     def _host_driven_loop(self, sess: "GenSession", gc, max_length, user_processors, user_criteria, streamer, seed, stream_col, ext,
-                          min_new_tokens, outputs=None, out_row=0):
+                          min_new_tokens, outputs=None, out_row=0, probe_window=None):
         """One host iteration per token, like GenerationMixin._sample: the decoder step still runs on the fused kernel
         (ptts_decode_forward), the built-in processors run as their device operators (MinNewTokens as a mask,
         ParlerTTSLogitsProcessor = ptts_logits_processor), then the caller's `logits_processor` list, the HF warpers and the draw
         as torch ops on the device scores, and the token is appended with ptts_sample(forced).  Used only when the caller passes
         processors or criteria the device loop does not know (the reference merges such lists at :3540-3552).  `ext`
         (resolve_sampling_ext) adds the n-gram bans before the EOS masks and the MinP / Typical / Epsilon / Eta warpers after
-        top-p, in transformers' order.  `outputs` (StepOutputs) records each step's raw logits and final scores before the draw."""
+        top-p, in transformers' order.  `outputs` (StepOutputs) records each step's raw logits and final scores before the draw;
+        `probe_window(step)` (StepProbes) points the decoder's attention / hidden-state outputs at the next step's slot."""
         d = self.config.decoder
         K, BK = d.num_codebooks, sess.B * d.num_codebooks
         parler = ParlerTTSLogitsProcessor(d.eos_token_id, K, sess.B, self.device)
@@ -942,6 +1089,8 @@ class ParlerTTSForConditionalGeneration:
                 stop = stop or unfinished.max().item() == 0
             if stop:
                 break
+            if probe_window is not None:
+                probe_window(cur - sess.n0)
             sess.decode_forward()
         if streamer is not None:
             streamer.end()
@@ -953,11 +1102,13 @@ class ParlerTTSForConditionalGeneration:
         return 32
 
     def _run_token_loop(self, enc_hidden, attention_mask, prompt_hidden, prompt_mask, *, gc, max_length, seed, suppress_special, row_base,
-                        ext, min_new_tokens, streamer=None, custom=None, input_ids=None, outputs=None, out_row=0):
+                        ext, min_new_tokens, streamer=None, custom=None, input_ids=None, outputs=None, out_row=0, probes=None):
         """begin + prefill + the token loop of one session; returns the raw token matrix [B * K, generated length].
         input_ids: None, or the BOS-led decoder input [B * K, n0] this shard continues from.
         outputs: None, or the StepOutputs this session's rows (from row out_row of the batch) are recorded into.  The device
-        loop then sets the sampler's window before every call and keeps each call inside one chunk."""
+        loop then sets the sampler's window before every call and keeps each call inside one chunk.
+        probes: None, or the StepProbes this session's attention weights / hidden states (from utterance out_row // K) go to;
+        its windows follow the same chunks, and the decode steps then run the multi-kernel path (ptts_generate_set_probes)."""
         d = self.config.decoder
         K = d.num_codebooks
         B, S, _ = enc_hidden.shape
@@ -979,40 +1130,52 @@ class ParlerTTSForConditionalGeneration:
                 _, pm = build_delay_pattern_mask(input_ids, d.bos_token_id, d.pad_token_id, max_length, K)
                 cells = pm[:, n0:n0 + K - 1]
                 stream_col = lambda col, v: (torch.where(cells[:, col - n0] == -1, v, cells[:, col - n0]) if col - n0 < cells.shape[1] else v)
-        sess.prefill(prompt_hidden, prompt_mask, enc_hidden, attention_mask)
-        window = (lambda step: outputs.set_window(sess, step, out_row)) if outputs is not None else (lambda step: None)
-        if custom is not None:
-            self._host_driven_loop(sess, gc, max_length, custom[0], custom[1], streamer, seed, stream_col, ext, min_new_tokens,
-                                   outputs, out_row)
-        elif streamer is not None:
-            window(0)
-            sess.sample()
-            steps_left = max_length - n0 - 1
-            # the streamer contract is one host-visible token column per step (_sample -> streamer.put(next.cpu()))
-            col = n0
-            streamer.put(stream_col(col, sess.raw_ids[:, col]).cpu())
-            while steps_left > 0 and int(sess.state[1].item()) == 1:
-                window(col + 1 - n0)
-                sess.decode_steps(1)
-                col += 1
-                steps_left -= 1
+        try:
+            if probes is not None:
+                probes.set_prefill(sess, out_row // K)
+            sess.prefill(prompt_hidden, prompt_mask, enc_hidden, attention_mask)
+            probe_window = (lambda step: probes.set_window(sess, step, out_row // K)) if probes is not None else None
+
+            def window(step):
+                if outputs is not None:
+                    outputs.set_window(sess, step, out_row)
+                if probe_window is not None and step > 0:
+                    probe_window(step)
+            if custom is not None:
+                self._host_driven_loop(sess, gc, max_length, custom[0], custom[1], streamer, seed, stream_col, ext, min_new_tokens,
+                                       outputs, out_row, probe_window)
+            elif streamer is not None:
+                window(0)
+                sess.sample()
+                steps_left = max_length - n0 - 1
+                # the streamer contract is one host-visible token column per step (_sample -> streamer.put(next.cpu()))
+                col = n0
                 streamer.put(stream_col(col, sess.raw_ids[:, col]).cpu())
-            streamer.end()
-        else:
-            window(0)
-            sess.sample()
-            steps_left = max_length - n0 - 1
-            # no per-step host sync: enqueue graph replays in chunks and poll the device `active` flag between chunks
-            chunk = 64
-            step = 1
-            while steps_left > 0:
-                n = min(chunk, steps_left) if outputs is None else steps_in_window(step, steps_left, StepOutputs.CHUNK)
-                window(step)
-                sess.decode_steps(n)
-                steps_left -= n
-                step += n
-                if steps_left > 0 and int(sess.state[1].item()) == 0:
-                    break
+                while steps_left > 0 and int(sess.state[1].item()) == 1:
+                    window(col + 1 - n0)
+                    sess.decode_steps(1)
+                    col += 1
+                    steps_left -= 1
+                    streamer.put(stream_col(col, sess.raw_ids[:, col]).cpu())
+                streamer.end()
+            else:
+                window(0)
+                sess.sample()
+                steps_left = max_length - n0 - 1
+                # no per-step host sync: enqueue graph replays in chunks and poll the device `active` flag between chunks
+                chunk = 64
+                step = 1
+                while steps_left > 0:
+                    n = min(chunk, steps_left) if outputs is None and probes is None else steps_in_window(step, steps_left, StepOutputs.CHUNK)
+                    window(step)
+                    sess.decode_steps(n)
+                    steps_left -= n
+                    step += n
+                    if steps_left > 0 and int(sess.state[1].item()) == 0:
+                        break
+        finally:
+            if probes is not None:
+                sess.set_probes()   # the session keeps no window (nor the chunks) past this call, whatever happens in it
         cur_len = int(sess.state[0].item())
         if outputs is not None:
             sess.set_outputs(None, None)   # the session keeps no reference to the chunks
@@ -1024,7 +1187,8 @@ class ParlerTTSForConditionalGeneration:
     @torch.no_grad()
     def forward(self, input_ids=None, attention_mask=None, input_values=None, padding_mask=None, decoder_input_ids=None,
                 decoder_attention_mask=None, encoder_outputs=None, prompt_input_ids=None, prompt_attention_mask=None,
-                prompt_hidden_states=None, labels=None, loss_reduction: str = "mean", return_logits: bool = False, **kwargs):
+                prompt_hidden_states=None, labels=None, loss_reduction: str = "mean", return_logits: bool = False,
+                output_attentions: bool = False, output_hidden_states: bool = False, **kwargs):
         """The reference's model call (:2695-2880) for inference-time scoring: the decoder over the prompt prefix and the T decoder
         input columns in one prefill pass, the K lm heads over the T positions, and the loss of :1922-1974.
 
@@ -1035,7 +1199,11 @@ class ParlerTTSForConditionalGeneration:
         sums per utterance).  One deviation: with labels, `logits` [B * K, T, V] is filled only if return_logits=True (otherwise
         None), because the fused kernel exists so that tensor (0.5-3 GB) is never built; without labels it is always filled.
         decoder_attention_mask must be right padding, which changes nothing the loss keeps under the causal mask.  Training
-        (backward) is out of scope."""
+        (backward) is out of scope.
+
+        output_attentions / output_hidden_states add decoder_attentions (L x [B, heads, P+T, P+T]), cross_attentions
+        (L x [B, heads, P+T, S]) and decoder_hidden_states (L+1 x [B, P+T, H]) in the model dtype, written by the same pass (the
+        weights by the reference's eager definition, see generate()); the loss, token_losses and logits do not change."""
         if kwargs:
             raise ValueError(f"forward() got arguments this path does not take: {sorted(kwargs)}")
         if loss_reduction not in ("mean", "sum"):
@@ -1083,12 +1251,22 @@ class ParlerTTSForConditionalGeneration:
         n_shards = (B + self._SCORE_SHARD - 1) // self._SCORE_SHARD
         sums = None if labels is None else torch.empty(n_shards, K, 2, dtype=torch.float32, device=dev)
         cut = lambda t, sl: None if t is None else t[sl]
+        probes = None
+        if output_attentions or output_hidden_states:
+            probes = StepProbes(d.num_hidden_layers, B, d.num_attention_heads, S, d.hidden_size, P, T, self.dtype, dev,
+                                output_attentions, output_hidden_states)
         for i, b0 in enumerate(range(0, B, self._SCORE_SHARD)):
             sl = slice(b0, min(B, b0 + self._SCORE_SHARD))
             sess = self.decoder.engine.session(sl.stop - sl.start, P, S, P + T, max_input_len=T)
-            sess.score(cut(prompt_hidden, sl), cut(prompt_mask, sl), enc_hidden[sl], cut(attention_mask, sl),
-                       dec[sl.start * K:sl.stop * K], cut(labels, sl), cut(token_nll, sl),
-                       None if logits is None else logits[sl.start * K:sl.stop * K], None if sums is None else sums[i])
+            try:
+                if probes is not None:
+                    probes.set_prefill(sess, b0)
+                sess.score(cut(prompt_hidden, sl), cut(prompt_mask, sl), enc_hidden[sl], cut(attention_mask, sl),
+                           dec[sl.start * K:sl.stop * K], cut(labels, sl), cut(token_nll, sl),
+                           None if logits is None else logits[sl.start * K:sl.stop * K], None if sums is None else sums[i])
+            finally:
+                if probes is not None:
+                    sess.set_probes()   # the cached session keeps no window (nor a reference to the buffers) past this call
         loss = per_codebook = None
         if labels is not None:
             # per codebook: sum (and count) over the shards, then the reference's reduction; a mean over no cell is NaN as in torch
@@ -1101,8 +1279,11 @@ class ParlerTTSForConditionalGeneration:
             else:
                 loss = (per.sum() / K).float()
             per_codebook = [per[k].float() for k in range(K)]
-        return ParlerTTSSeq2SeqLMOutput(loss=loss, logits=logits, per_codebook_losses=per_codebook, token_losses=token_nll,
-                                        encoder_last_hidden_state=enc_hidden)
+        out = ParlerTTSSeq2SeqLMOutput(loss=loss, logits=logits, per_codebook_losses=per_codebook, token_losses=token_nll,
+                                       encoder_last_hidden_state=enc_hidden)
+        if probes is not None:
+            out.update(probes.entry(0))
+        return out
 
     __call__ = forward
 
@@ -1118,7 +1299,20 @@ class ParlerTTSForConditionalGeneration:
         tuple with one fp32 [B * K, V] entry per generated column (column n0 + t was drawn from entry t), the processed scores the
         token was drawn from (-inf where removed) and the raw logits.  Rows that finished keep being recorded while the session
         runs.  Deviation: a batch above 32 utterances runs as shards of 32, and a shard that ended holds NaN in both up to the
-        longest shard's end.  output_attentions / output_hidden_states are accepted and ignored.
+        longest shard's end.
+
+        output_attentions / output_hidden_states (with return_dict_in_generate=True) add transformers' `decoder_attentions`,
+        `cross_attentions` and `decoder_hidden_states`, one entry per generated column indexed like `scores`: entry 0 is the
+        prefill (q = P + n0 rows: the prompt prefix, then BOS or the code prefix), entry t >= 1 has q = 1 and T_kv = P + n0 + t
+        keys.  Attention entries are tuples of L [B, heads, q, T_kv] (cross: [B, heads, q, S]) tensors, hidden-state entries
+        tuples of L + 1 [B, q, H] (the embeddings, the outputs of layers 0 .. L-2, the final LayerNorm of the last layer's output),
+        all in the model dtype.  When generate() runs the text encoder itself, `encoder_attentions` / `encoder_hidden_states`
+        come from an eager call of it with the same flags (None with `encoder_outputs`).  The weights follow the reference's eager
+        attention (model-dtype scores, fp32 softmax), computed from the q and K the session holds.  Deviations: in the reference,
+        asking for attentions switches its own attention to that eager path and can change its tokens; here the tokens, scores
+        and audio are bit-identical with and without the flags, while the decode steps run the multi-kernel path (not the fused
+        step kernel) for as long as anything is recorded.  A shard that ended holds NaN, as in `scores`.  Memory: see
+        StepProbes.
         """
         import copy
         gc = copy.deepcopy(generation_config if generation_config is not None else self.generation_config)
@@ -1133,7 +1327,7 @@ class ParlerTTSForConditionalGeneration:
         if unknown:
             raise ValueError(f"The following `model_kwargs` are not used by the model: {unknown} (note: typos in the generate "
                              "arguments will also show up in this list)")
-        for k in ("use_cache", "cache_implementation", "output_attentions", "output_hidden_states"):
+        for k in ("use_cache", "cache_implementation"):
             mk.pop(k, None)   # accepted for call compatibility: the device loop always uses its static cache
         unsupported = {k: getattr(gc, k) for k, neutral in self._NEUTRAL_GENERATION_KNOBS.items() if getattr(gc, k, neutral) != neutral}
         if unsupported:
@@ -1152,6 +1346,17 @@ class ParlerTTSForConditionalGeneration:
         else:
             if input_ids is None:
                 raise ValueError("generate() needs `input_ids` (description) or `encoder_outputs`")
+            enc_hidden = None
+        # decoder_attentions / cross_attentions / decoder_hidden_states exist only in the dict return, as in transformers
+        want_attn = bool(gc.return_dict_in_generate and gc.output_attentions)
+        want_hidden = bool(gc.return_dict_in_generate and gc.output_hidden_states)
+        enc_probe = {}
+        if enc_hidden is None and (want_attn or want_hidden):   # the encoder's own tuples: one eager call with the flags
+            enc_hidden, eo = self._encode_text_eager(input_ids, attention_mask, dict(output_attentions=want_attn,
+                                                                                     output_hidden_states=want_hidden))
+            enc_probe = dict(encoder_attentions=getattr(eo, "attentions", None) if want_attn else None,
+                             encoder_hidden_states=getattr(eo, "hidden_states", None) if want_hidden else None)
+        elif enc_hidden is None:
             enc_hidden = self._encode_text(input_ids, attention_mask)   # encoder + enc_to_dec_proj + mask multiply, one CUDA graph
         enc_hidden = enc_hidden.to(self.device, self.dtype)
         B, S, _ = enc_hidden.shape
@@ -1196,6 +1401,10 @@ class ParlerTTSForConditionalGeneration:
         want_scores = bool(gc.return_dict_in_generate and gc.output_scores)
         want_logits = bool(gc.return_dict_in_generate and gc.output_logits)
         outputs = StepOutputs(B * K, d.vocab_size, self.device, want_scores, want_logits) if (want_scores or want_logits) else None
+        probes = None
+        if want_attn or want_hidden:
+            probes = StepProbes(d.num_hidden_layers, B, d.num_attention_heads, S, d.hidden_size, P, n0, self.dtype, self.device,
+                                want_attn, want_hidden)
         limit = self._fused_batch_limit()
         if limit is not None and B > limit and not custom_loop and streamer is None:
             # The fused decode-step kernels hold one 32-row tile: a larger batch runs as consecutive shards of <= 32 utterances through
@@ -1208,13 +1417,13 @@ class ParlerTTSForConditionalGeneration:
                                                   None if prompt_hidden is None else prompt_hidden[sl],
                                                   None if prompt_mask is None else prompt_mask[sl], row_base=row_base + b0 * K,
                                                   input_ids=None if dec_ids is None else dec_ids[sl.start * K:sl.stop * K],
-                                                  outputs=outputs, out_row=b0 * K, **run))
+                                                  outputs=outputs, out_row=b0 * K, probes=probes, **run))
             n = max(t.shape[1] for t in parts)
             output_ids = torch.cat([torch.nn.functional.pad(t, (0, n - t.shape[1]), value=d.pad_token_id) for t in parts], dim=0)
         else:
             output_ids = self._run_token_loop(enc_hidden, attention_mask, prompt_hidden, prompt_mask, row_base=row_base, streamer=streamer,
                                               custom=(logits_processor or [], stopping_criteria or []) if custom_loop else None,
-                                              input_ids=dec_ids, outputs=outputs, **run)
+                                              input_ids=dec_ids, outputs=outputs, probes=probes, **run)
 
         # apply the stashed delay mask, then keep only the free cells (:3586-3597); both masks come from the whole decoder input,
         # so a continuation's codes begin with its prefix frames
@@ -1253,6 +1462,12 @@ class ParlerTTSForConditionalGeneration:
             if outputs is not None:   # one entry per generated column: column n0 + t was drawn from entry t
                 rec = outputs.result(output_ids.shape[1] - n0)
                 out.update(scores=rec.get("scores"), logits=rec.get("logits"))
+            if probes is not None:
+                out.update(probes.result(output_ids.shape[1] - n0))
+                if want_attn:
+                    out.update(encoder_attentions=enc_probe.get("encoder_attentions"))
+                if want_hidden:
+                    out.update(encoder_hidden_states=enc_probe.get("encoder_hidden_states"))
             if gc.return_dict_in_generate:
                 return out
             return output_values, out
