@@ -274,6 +274,14 @@ int ptts_delay_apply(const int64_t* input_ids, int32_t BK, int32_t seq_len, int6
 int ptts_logits_processor(const int64_t* input_ids, int32_t BK, int32_t seq_len, int64_t ld_ids,
                           float* scores, int32_t V, int64_t eos, int32_t num_codebooks,
                           int64_t* first_unfinished, void* stream);
+/* The fused step kernels' sampling phase (sample_all_rows_cta: each of n_ctas CTAs takes rows cta, cta + n_ctas, ..., one row
+ * per pass while B*K <= n_ctas, otherwise passes of three) on the session's current logits, as a kernel of its own.  Test hook
+ * for the three-row passes: it computes what ptts_sample computes (scores, the token at column cur_len and the per-row state)
+ * but leaves cur_len where it is.  The per-row state it writes (unfinished, eos_seen, the next input) is the state after this
+ * column, so a second launch at the same column, or a ptts_sample after it, repeats the result only while no row finished
+ * there (drew EOS or reached max_length): such a row then gets PAD instead of its draw.  PTTS_ESTATE before ptts_prefill; PTTS_EINVAL for n_ctas < 1, vocab_size > 2304, or while a
+ * ptts_sampling_ext stage or a ptts_generate_set_outputs window is active (the step kernels run neither). */
+int ptts_op_sample_phase(ptts_session* s, int32_t n_ctas, void* stream);
 /* y[M,N] = epi(LN?(x[M,K]) @ W^T): W taken from a packed blob slot (the whole fused matrix it belongs to).  Test hook for the
  * GEMM kernels.  path 0: the decode GEMM (launch_linear, every dtype); path 1: the wgmma prefill GEMM (launch_linear_tc) over
  * the matrix's row-major copy, with the same eligibility rule and the same blob lookup as the prefill -- PTTS_EINVAL when it

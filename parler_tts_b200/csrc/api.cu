@@ -784,6 +784,15 @@ int ptts_logits_processor(const int64_t* input_ids, int32_t BK, int32_t seq_len,
   return launch_logits_processor(input_ids, BK, seq_len, ld_ids, scores, V, eos, num_codebooks, first_unfinished, (cudaStream_t)stream);
 }
 
+int ptts_op_sample_phase(ptts_session* s, int32_t n_ctas, void* stream) {
+  PTTS_REQUIRE(s, "null argument");
+  if (!s->prefilled) return fail(PTTS_ESTATE, "ptts_op_sample_phase called before ptts_prefill");
+  PTTS_REQUIRE(sampler_ext(s) == nullptr, "op_sample_phase: the step kernels' sampling phase has no ptts_sampling_ext stages and "
+                                          "records no per-step outputs; switch them off first");
+  s->launches++;
+  return launch_sample_phase(sample_args(s), n_ctas, (cudaStream_t)stream);
+}
+
 int ptts_op_linear2(const ptts_decoder_config* cfg, const void* blob, int32_t tensor_id, int32_t index, const void* x, int32_t M,
                     int32_t use_ln, int32_t epilogue, const void* residual, void* y, int32_t path, float* row_stats, void* stream) {
   PTTS_REQUIRE(cfg && blob && x && y, "null argument");

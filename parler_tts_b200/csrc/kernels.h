@@ -110,6 +110,8 @@ struct SampleOut {
 // set); out != nullptr (needs ext): that sampler also records the raw logits and the processed scores of the steps in its window
 int launch_sample(const SampleArgs& a, const int64_t* forced, cudaStream_t st, bool pdl, const ptts_sampling_ext* ext = nullptr,
                   const SampleOut* out = nullptr);
+// the fused step kernels' sampling phase over n_ctas CTAs (passes of up to three rows per CTA), as a kernel of its own; no EXT
+int launch_sample_phase(const SampleArgs& a, int n_ctas, cudaStream_t st);
 // ids == nullptr: the BOS column (n0 = 1); otherwise the BOS-led [B*K][n0] input the generation continues from
 int launch_generate_begin(const SampleArgs& a, const int64_t* ids, int n0, int max_length, cudaStream_t st);
 int launch_delay_build(const int64_t* ids, int BK, int seq, int K, int64_t bos, int64_t pad, int L, int64_t* mask, cudaStream_t st);

@@ -85,6 +85,34 @@ int launch_sample(const SampleArgs& a, const int64_t* forced, cudaStream_t st, b
   return PTTS_OK;
 }
 
+// ptts_op_sample_phase: the step kernels' sampling phase (sample_all_rows_cta, passes of up to three rows per CTA) over a grid of
+// n_ctas CTAs, on the session's logits.  cur_len stays where it is; the last CTA clears the counters the rows add to.
+template <int ITEMS>
+__global__ void __launch_bounds__(SMP_THREADS) sample_phase_kernel(SampleArgs p) {
+  if (p.ctrl->active == 0) return;
+  const int cur_len = p.ctrl->cur_len;
+  const ptts_gen_params g = *p.gen;
+  sample_all_rows_cta<ITEMS>(p, g, (int)blockIdx.x, (int)gridDim.x, p.B * p.K, cur_len);
+  __threadfence();
+  __syncthreads();
+  if (threadIdx.x == 0 && atomicAdd(&p.ctrl->done_blocks, 1) == (int)gridDim.x - 1) {
+    p.ctrl->n_unfinished = 0;
+    p.ctrl->done_blocks = 0;
+    __threadfence();
+  }
+}
+
+int launch_sample_phase(const SampleArgs& a, int n_ctas, cudaStream_t st) {
+  const int items = (a.V + SMP_THREADS - 1) / SMP_THREADS;
+  PTTS_REQUIRE(items <= 9, "sample: vocab_size %d > 2304 not supported", a.V);
+  PTTS_REQUIRE(n_ctas >= 1, "op_sample_phase: n_ctas must be positive, got %d", n_ctas);
+  if (items <= 1) sample_phase_kernel<1><<<n_ctas, SMP_THREADS, 0, st>>>(a);
+  else if (items <= 5) sample_phase_kernel<5><<<n_ctas, SMP_THREADS, 0, st>>>(a);
+  else sample_phase_kernel<9><<<n_ctas, SMP_THREADS, 0, st>>>(a);
+  PTTS_LAUNCH_CHECK();
+  return PTTS_OK;
+}
+
 // build_delay_pattern_mask (modeling_parler_tts.py:214-276), cell c of row `row` (codebook k) for the BOS-led ids [B*K][seq]: the
 // id shifted by k, BOS over the lower triangle, PAD over the upper one (:261); -1 = free (predicted).  No pattern below 2K-1 columns.
 __device__ __forceinline__ int64_t delay_pattern_cell(const int64_t* ids, int row, int seq, int k, int K, int64_t bos, int64_t pad, int L, int c) {
