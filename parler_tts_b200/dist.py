@@ -50,11 +50,14 @@ def broadcast_blob(blob: torch.Tensor, src: int = 0, group=None) -> torch.Tensor
 def model_weight_tensors(model) -> list[torch.Tensor]:
     """Every device tensor that holds weights, in a fixed order that depends on the CONFIG only (never on what a rank has
     loaded): the packed decoder blob, the packed DAC blob, the prompt embedding table, when the text encoder's width
-    differs from the decoder's, enc_to_dec_proj (modeling_parler_tts.py:2388-2392), and the DAC encoder blob when the codec
-    config has an encoder.  All exist from construction on."""
+    differs from the decoder's, enc_to_dec_proj (modeling_parler_tts.py:2388-2392), with config.prompt_cross_attention the
+    prompt's position table (:2397-2402), and the DAC encoder blob when the codec config has an encoder.  All exist from
+    construction on."""
     ts = [model.decoder.engine.blob, model.audio_encoder.blob, model.embed_prompts_weight]
     if model.enc_to_dec_proj is not None:
         ts += list(model.enc_to_dec_proj)
+    if getattr(model, "embed_positions_weight", None) is not None:
+        ts.append(model.embed_positions_weight)
     enc_blob = getattr(model.audio_encoder, "encoder_blob", None)
     if enc_blob is not None:
         ts.append(enc_blob)

@@ -161,6 +161,33 @@ def check_scoring_inputs(labels, decoder_input_ids, decoder_attention_mask, *, b
     return labels, dec
 
 
+def prompt_cross_states(enc_hidden: torch.Tensor, enc_mask: Optional[torch.Tensor], prompt: torch.Tensor,
+                        prompt_mask: Optional[torch.Tensor], embed_prompts: torch.Tensor, positions: torch.Tensor):
+    """config.prompt_cross_attention: the transcript prompt as cross-attention keys after the description (reference :3099-3130,
+    forward :2791-2811) -> (states [B, S + P, H], mask [B, S + P] or None).
+
+    prompt: ids [B, P] (looked up in embed_prompts) or states [B, P, H]; positions: the [max_position_embeddings, H] sinusoidal
+    table.  The prompt becomes prompt + positions[0:P] in the tables' dtype; it is not multiplied by its mask.  If only one of the
+    two masks is given, the other becomes ones; with neither there is no mask.  Raises ValueError when P exceeds the table."""
+    B, S = enc_hidden.shape[:2]
+    P = prompt.shape[1]
+    if P > positions.shape[0]:
+        raise ValueError(f"the prompt has {P} tokens, more than max_position_embeddings = {positions.shape[0]} positions")
+    if prompt.shape[0] != B or prompt.dim() not in (2, 3) or (prompt_mask is not None and tuple(prompt_mask.shape) != (B, P)):
+        raise ValueError(f"the prompt must be [{B}, P] ids or [{B}, P, H] states with a [{B}, P] mask, got {tuple(prompt.shape)}"
+                         f" and {None if prompt_mask is None else tuple(prompt_mask.shape)}")
+    if prompt.dim() == 2:
+        prompt = torch.nn.functional.embedding(prompt.to(embed_prompts.device), embed_prompts)
+    prompt = prompt.to(device=positions.device, dtype=positions.dtype) + positions[:P]
+    if prompt_mask is not None and enc_mask is None:
+        enc_mask = torch.ones(B, S, dtype=prompt_mask.dtype, device=prompt_mask.device)
+    elif enc_mask is not None and prompt_mask is None:
+        prompt_mask = torch.ones(B, P, dtype=enc_mask.dtype, device=enc_mask.device)
+    states = torch.cat([enc_hidden.to(prompt.device, prompt.dtype), prompt], dim=1)
+    mask = None if prompt_mask is None else torch.cat([enc_mask, prompt_mask.to(enc_mask.device)], dim=1)
+    return states, mask
+
+
 def resolve_sampling_ext(gc, n0: int):
     """The further processors of transformers' `_get_logits_processor` from a GenerationConfig -> (ext, min_new_tokens).
 
@@ -888,14 +915,17 @@ class ParlerTTSForConditionalGeneration:
         self.decoder = ParlerTTSForCausalLM(config.decoder, device, dtype)
         self.audio_encoder = DACModel(config.audio_encoder, device, dtype)
         self.text_encoder = text_encoder  # a torch module (T5 encoder) or None; not part of the replaced path
-        self.prompt_cross_attention = config.prompt_cross_attention
-        if self.prompt_cross_attention:
-            raise ValueError("prompt_cross_attention=True checkpoints are not supported by this path yet")
+        self.prompt_cross_attention = bool(config.prompt_cross_attention)
         # Side-input parameters exist (zero-filled) from construction on, with shapes that depend on the config only, so every
         # rank of a sharded run issues the SAME list of broadcasts at init (dist.broadcast_model_weights); `_side_loaded`
         # says whether they hold real weights.  enc_to_dec_proj exists iff the text encoder's width differs (:2388-2392).
         dd = config.decoder
         self.embed_prompts_weight: torch.Tensor = torch.zeros(config.vocab_size, dd.hidden_size, device=self.device, dtype=dtype)
+        # prompt_cross_attention: the prompt's sinusoidal positions (embed_positions.weights, :2397-2402), valid from construction
+        # on; a checkpoint's own table replaces it at load_state_dict
+        self.embed_positions_weight: Optional[torch.Tensor] = None
+        if self.prompt_cross_attention:
+            self.embed_positions_weight = _sinusoidal_table(dd.max_position_embeddings, dd.hidden_size).to(self.device, dtype)
         te_hidden = (config.text_encoder or {}).get("d_model", (config.text_encoder or {}).get("hidden_size"))
         self.enc_to_dec_proj: Optional[tuple] = None
         if te_hidden is not None and int(te_hidden) != dd.hidden_size:
@@ -925,6 +955,12 @@ class ParlerTTSForConditionalGeneration:
                 self.enc_to_dec_proj[0].copy_(w); self.enc_to_dec_proj[1].copy_(b)
             else:
                 self.enc_to_dec_proj = (w.contiguous(), b.contiguous())
+        if self.embed_positions_weight is not None and "embed_positions.weights" in sd:
+            w = sd["embed_positions.weights"]
+            if tuple(w.shape) != tuple(self.embed_positions_weight.shape):
+                raise ValueError(f"embed_positions.weights must be {tuple(self.embed_positions_weight.shape)} "
+                                 f"(max_position_embeddings x hidden_size), got {tuple(w.shape)}")
+            self.embed_positions_weight.copy_(w.to(self.device, self.dtype))
         ae = {k[len("audio_encoder."):]: v for k, v in sd.items() if k.startswith("audio_encoder.")}
         if dac_state_dict is not None:
             ae = dac_state_dict
@@ -1203,7 +1239,11 @@ class ParlerTTSForConditionalGeneration:
 
         output_attentions / output_hidden_states add decoder_attentions (L x [B, heads, P+T, P+T]), cross_attentions
         (L x [B, heads, P+T, S]) and decoder_hidden_states (L+1 x [B, P+T, H]) in the model dtype, written by the same pass (the
-        weights by the reference's eager definition, see generate()); the loss, token_losses and logits do not change."""
+        weights by the reference's eager definition, see generate()); the loss, token_losses and logits do not change.
+
+        config.prompt_cross_attention: when forward() runs the text encoder, `prompt_input_ids` or `prompt_hidden_states` plus
+        their positions join the description as cross-attention keys (prompt_cross_states, :2791-2811) and P = 0; with
+        `encoder_outputs` a prompt raises ValueError."""
         if kwargs:
             raise ValueError(f"forward() got arguments this path does not take: {sorted(kwargs)}")
         if loss_reduction not in ("mean", "sum"):
@@ -1213,7 +1253,12 @@ class ParlerTTSForConditionalGeneration:
                 raise ValueError("forward(input_values=...) without labels or decoder_input_ids: encode the audio with "
                                  "audio_encoder.encode(...) and pass its codes as decoder_input_ids")
             raise ValueError("forward() needs `labels` or `decoder_input_ids`")
+        cross_prompt = self.prompt_cross_attention and (prompt_input_ids is not None or prompt_hidden_states is not None)
         if encoder_outputs is not None:
+            if cross_prompt:
+                # the reference would make the prompt a self-attention prefix without positions: the other model
+                raise ValueError("a prompt_cross_attention model joins the prompt to the description only when forward() runs the "
+                                 "text encoder: pass `input_ids` instead of `encoder_outputs`, or no prompt")
             enc = encoder_outputs
             enc_hidden = enc[0] if isinstance(enc, (tuple, list)) else getattr(enc, "last_hidden_state", enc)
         else:
@@ -1221,6 +1266,14 @@ class ParlerTTSForConditionalGeneration:
                 raise ValueError("forward() needs `input_ids` (description) or `encoder_outputs`")
             enc_hidden = self._encode_text(input_ids, attention_mask)
         enc_hidden = enc_hidden.to(self.device, self.dtype)
+        if cross_prompt:
+            # the prompt joins the description as cross-attention keys (:2791-2811); the decoder then has no prompt prefix
+            prompt = prompt_hidden_states if prompt_hidden_states is not None else prompt_input_ids
+            if prompt.dim() == 2 and not self._side_loaded:
+                raise ValueError("no embed_prompts weights loaded")
+            enc_hidden, attention_mask = prompt_cross_states(enc_hidden, attention_mask, prompt, prompt_attention_mask,
+                                                             self.embed_prompts_weight, self.embed_positions_weight)
+            prompt_input_ids = prompt_hidden_states = prompt_attention_mask = None
         if enc_hidden.dim() != 3 or enc_hidden.shape[2] != self.config.decoder.hidden_size:
             raise ValueError(f"encoder states must be [batch, length, {self.config.decoder.hidden_size}], got {tuple(enc_hidden.shape)}")
         B, S, _ = enc_hidden.shape
@@ -1313,6 +1366,10 @@ class ParlerTTSForConditionalGeneration:
         and audio are bit-identical with and without the flags, while the decode steps run the multi-kernel path (not the fused
         step kernel) for as long as anything is recorded.  A shard that ended holds NaN, as in `scores`.  Memory: see
         StepProbes.
+
+        config.prompt_cross_attention: `prompt_input_ids` plus their sinusoidal positions are appended to the description states
+        as cross-attention keys (prompt_cross_states, reference :3099-3130), also after `encoder_outputs`; the decoder then has no
+        prompt prefix (P = 0), and `cross_attentions` have S + P keys.  `prompt_hidden_states` raise ValueError in this mode.
         """
         import copy
         gc = copy.deepcopy(generation_config if generation_config is not None else self.generation_config)
@@ -1337,6 +1394,9 @@ class ParlerTTSForConditionalGeneration:
         if gc.num_beams != 1:
             raise ValueError("Got incompatible mode for generation, should be one of greedy or sampling. "
                              "Ensure that beam search is de-activated by setting `num_beams=1` and `num_beam_groups=1`.")
+        if self.prompt_cross_attention and mk.get("prompt_hidden_states") is not None:
+            # the reference would put these states in front of the decoder while counting its cache positions without them
+            raise ValueError("a prompt_cross_attention model takes the transcript as `prompt_input_ids`, not `prompt_hidden_states`")
         custom_loop = bool(logits_processor) or bool(stopping_criteria)   # merged with the built-in ones like :3540-3552
         input_ids = mk.get("input_ids", inputs)
         attention_mask = mk.get("attention_mask")
@@ -1359,14 +1419,20 @@ class ParlerTTSForConditionalGeneration:
         elif enc_hidden is None:
             enc_hidden = self._encode_text(input_ids, attention_mask)   # encoder + enc_to_dec_proj + mask multiply, one CUDA graph
         enc_hidden = enc_hidden.to(self.device, self.dtype)
-        B, S, _ = enc_hidden.shape
         prompt_hidden = mk.get("prompt_hidden_states")
-        if prompt_hidden is None and mk.get("prompt_input_ids") is not None:
+        if self.prompt_cross_attention and mk.get("prompt_input_ids") is not None:
+            # the prompt joins the description as cross-attention keys (:3099-3130); everything below runs with P = 0
+            if not self._side_loaded:
+                raise ValueError("no embed_prompts weights loaded")
+            enc_hidden, attention_mask = prompt_cross_states(enc_hidden, attention_mask, mk["prompt_input_ids"], mk.get("prompt_attention_mask"),
+                                                             self.embed_prompts_weight, self.embed_positions_weight)
+        elif prompt_hidden is None and mk.get("prompt_input_ids") is not None:
             if not self._side_loaded:
                 raise ValueError("no embed_prompts weights loaded")
             prompt_hidden = torch.nn.functional.embedding(mk["prompt_input_ids"].to(self.device), self.embed_prompts_weight)
         prompt_mask = mk.get("prompt_attention_mask") if prompt_hidden is not None else None
         P = 0 if prompt_hidden is None else prompt_hidden.shape[1]
+        B, S, _ = enc_hidden.shape
 
         d = self.config.decoder
         K = d.num_codebooks
