@@ -132,6 +132,13 @@ int ptts_workspace_bytes(const ptts_decoder_config* cfg, int32_t B, int32_t P, i
 int ptts_workspace_bytes2(const ptts_decoder_config* cfg, int32_t B, int32_t P, int32_t S, int32_t max_cache_len,
                           int32_t max_input_len, int64_t* out_bytes);
 
+/* Same, for a session whose B rows are B / takes descriptions with `takes` consecutive takes each (generate(num_return_sequences=
+ * takes), modeling_parler_tts.py:3556): row b reads the cross-attention K/V and encoder mask of description b / takes, so the
+ * workspace holds those for B / takes descriptions only.  takes must divide B (PTTS_EINVAL otherwise); takes = 1 gives exactly
+ * ptts_workspace_bytes2. */
+int ptts_workspace_bytes3(const ptts_decoder_config* cfg, int32_t B, int32_t P, int32_t S, int32_t max_cache_len,
+                          int32_t max_input_len, int32_t takes, int64_t* out_bytes);
+
 typedef struct ptts_session ptts_session; /* host-side object: pointers into blob/workspace + CUDA graphs */
 
 int ptts_session_create(const ptts_decoder_config* cfg, const void* blob, void* workspace,
@@ -141,6 +148,12 @@ int ptts_session_create(const ptts_decoder_config* cfg, const void* blob, void* 
 int ptts_session_create2(const ptts_decoder_config* cfg, const void* blob, void* workspace,
                          int64_t workspace_bytes, int32_t B, int32_t P, int32_t S, int32_t max_cache_len,
                          int32_t max_input_len, ptts_session** out);
+/* Same, with the takes of ptts_workspace_bytes3 (= ptts_session_create2 when 1).  On such a session ptts_prefill and ptts_score
+ * take enc_hidden [B / takes, S, H] and enc_mask [B / takes, S]: the cross-attention K/V are projected once per description and
+ * shared by its takes in every decode path.  Everything else (prompt prefix, decoder input, outputs, probes) has B rows. */
+int ptts_session_create3(const ptts_decoder_config* cfg, const void* blob, void* workspace,
+                         int64_t workspace_bytes, int32_t B, int32_t P, int32_t S, int32_t max_cache_len,
+                         int32_t max_input_len, int32_t takes, ptts_session** out);
 int ptts_session_destroy(ptts_session* s);
 
 /* Start a generate() call: reset per-call state (ids history = BOS column, processor state,

@@ -61,6 +61,8 @@ _SIGS = {
     "ptts_session_create": (C.c_int, [C.POINTER(DecoderConfigC), _VP, _VP, _I64, _I32, _I32, _I32, _I32, C.POINTER(_VP)]),
     "ptts_workspace_bytes2": (C.c_int, [C.POINTER(DecoderConfigC), _I32, _I32, _I32, _I32, _I32, C.POINTER(_I64)]),
     "ptts_session_create2": (C.c_int, [C.POINTER(DecoderConfigC), _VP, _VP, _I64, _I32, _I32, _I32, _I32, _I32, C.POINTER(_VP)]),
+    "ptts_workspace_bytes3": (C.c_int, [C.POINTER(DecoderConfigC), _I32, _I32, _I32, _I32, _I32, _I32, C.POINTER(_I64)]),
+    "ptts_session_create3": (C.c_int, [C.POINTER(DecoderConfigC), _VP, _VP, _I64, _I32, _I32, _I32, _I32, _I32, _I32, C.POINTER(_VP)]),
     "ptts_session_destroy": (C.c_int, [_VP]),
     "ptts_generate_begin": (C.c_int, [_VP, C.POINTER(GenParamsC), _VP]),
     "ptts_generate_begin_ids": (C.c_int, [_VP, C.POINTER(GenParamsC), _VP, _I32, _VP]),

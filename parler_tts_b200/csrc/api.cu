@@ -193,14 +193,20 @@ int ptts_decoder_finalize(const ptts_decoder_config* cfg, void* blob, void* stre
   return PTTS_OK;
 }
 
-int ptts_workspace_bytes2(const ptts_decoder_config* cfg, int32_t B, int32_t P, int32_t S, int32_t max_cache_len, int32_t max_input_len,
-                          int64_t* out_bytes) {
+int ptts_workspace_bytes3(const ptts_decoder_config* cfg, int32_t B, int32_t P, int32_t S, int32_t max_cache_len, int32_t max_input_len,
+                          int32_t takes, int64_t* out_bytes) {
   PTTS_REQUIRE(cfg && out_bytes, "null argument");
   if (int e = validate_config(*cfg)) return e;
   PTTS_REQUIRE(B > 0 && P >= 0 && S > 0 && max_cache_len > P, "workspace: need B>0, P>=0, S>0, max_cache_len>P (got %d %d %d %d)", B, P, S, max_cache_len);
   PTTS_REQUIRE(max_input_len >= 1 && max_input_len < max_cache_len - P + 1, "workspace: max_input_len %d must be in [1, max_cache_len - P]", max_input_len);
-  *out_bytes = make_workspace(*cfg, B, P, S, max_cache_len, max_input_len).total;
+  PTTS_REQUIRE(takes >= 1 && B % takes == 0, "workspace: takes %d must be >= 1 and divide B = %d", takes, B);
+  *out_bytes = make_workspace(*cfg, B, P, S, max_cache_len, max_input_len, takes).total;
   return PTTS_OK;
+}
+
+int ptts_workspace_bytes2(const ptts_decoder_config* cfg, int32_t B, int32_t P, int32_t S, int32_t max_cache_len, int32_t max_input_len,
+                          int64_t* out_bytes) {
+  return ptts_workspace_bytes3(cfg, B, P, S, max_cache_len, max_input_len, 1, out_bytes);
 }
 
 int ptts_workspace_bytes(const ptts_decoder_config* cfg, int32_t B, int32_t P, int32_t S, int32_t max_cache_len, int64_t* out_bytes) {
@@ -208,18 +214,19 @@ int ptts_workspace_bytes(const ptts_decoder_config* cfg, int32_t B, int32_t P, i
 }
 
 // ---- session ------------------------------------------------------------------------------------
-int ptts_session_create2(const ptts_decoder_config* cfg, const void* blob, void* workspace, int64_t workspace_bytes,
-                         int32_t B, int32_t P, int32_t S, int32_t max_cache_len, int32_t max_input_len, ptts_session** out) {
+int ptts_session_create3(const ptts_decoder_config* cfg, const void* blob, void* workspace, int64_t workspace_bytes,
+                         int32_t B, int32_t P, int32_t S, int32_t max_cache_len, int32_t max_input_len, int32_t takes, ptts_session** out) {
   PTTS_REQUIRE(cfg && blob && workspace && out, "null argument");
   if (int e = validate_config(*cfg)) return e;
   PTTS_REQUIRE(B > 0 && P >= 0 && S > 0 && max_cache_len > P, "session: bad shape B=%d P=%d S=%d Tmax=%d", B, P, S, max_cache_len);
   PTTS_REQUIRE(max_cache_len <= cfg->max_positions, "session: cache length %d exceeds max_position_embeddings %d", max_cache_len, cfg->max_positions);
   PTTS_REQUIRE(max_input_len >= 1 && max_input_len < max_cache_len - P + 1, "session: max_input_len %d must be in [1, max_cache_len - P]", max_input_len);
+  PTTS_REQUIRE(takes >= 1 && B % takes == 0, "session: takes %d must be >= 1 and divide B = %d", takes, B);
   ptts_session* s = new (std::nothrow) ptts_session();
   PTTS_REQUIRE(s, "out of host memory");
   s->cfg = *cfg;
   s->L = make_layout(*cfg);
-  s->W = make_workspace(*cfg, B, P, S, max_cache_len, max_input_len);
+  s->W = make_workspace(*cfg, B, P, S, max_cache_len, max_input_len, takes);
   s->n0 = 1;
   s->ext = kExtOff;
   s->out = SampleOut{};
@@ -245,6 +252,11 @@ int ptts_session_create2(const ptts_decoder_config* cfg, const void* blob, void*
   s->launches = 0;
   *out = s;
   return PTTS_OK;
+}
+
+int ptts_session_create2(const ptts_decoder_config* cfg, const void* blob, void* workspace, int64_t workspace_bytes,
+                         int32_t B, int32_t P, int32_t S, int32_t max_cache_len, int32_t max_input_len, ptts_session** out) {
+  return ptts_session_create3(cfg, blob, workspace, workspace_bytes, B, P, S, max_cache_len, max_input_len, 1, out);
 }
 
 int ptts_session_create(const ptts_decoder_config* cfg, const void* blob, void* workspace, int64_t workspace_bytes,
@@ -303,7 +315,7 @@ static DecodePath choose_decode_path(ptts_session* s) {
   StepParams& p = s->sp;
   memset(&p, 0, sizeof(p));
   p.B = W.B; p.H = L.H; p.F = L.F; p.V = L.V; p.K = L.K; p.L = L.L; p.nh = L.nh; p.nkv = L.nkv; p.nckv = L.nckv;
-  p.S = W.S; p.P = W.P; p.Tmax = W.Tmax; p.rope = c.rope; p.act = c.activation; p.qkv_rows = L.qkv_rows; p.ckv_rows = L.ckv_rows;
+  p.S = W.S; p.P = W.P; p.Tmax = W.Tmax; p.takes = W.takes; p.rope = c.rope; p.act = c.activation; p.qkv_rows = L.qkv_rows; p.ckv_rows = L.ckv_rows;
   p.eps = c.layer_norm_eps; p.scale = 0.125f;
   p.blob = s->blob;
   p.lay = L;
@@ -435,6 +447,7 @@ static int run_forward(ptts_session* s, cudaStream_t st, bool prefill, const voi
   const DecoderLayout& L = s->L;
   const WorkspaceLayout& W = s->W;
   const int B = W.B, P = W.P, S = W.S, H = L.H, D = PTTS_HEAD_DIM;
+  const int n_desc = B / W.takes;   // descriptions: the cross K/V and the encoder mask hold one item each
   const int q_len = prefill ? P + s->n0 : 1;
   const int M = B * q_len;
   const bool pdl = !prefill;  // the one-off prefill stays on plain stream order
@@ -480,7 +493,7 @@ static int run_forward(ptts_session* s, cudaStream_t st, bool prefill, const voi
     if (base == nullptr) return PTTS_OK;
     AttnProbeArgs p{};
     p.q = at.q; p.ldq = at.ldq; p.q_col0 = at.q_col0;
-    p.kcache = at.kcache; p.kv_b_stride = at.kv_b_stride; p.kv_h_stride = at.kv_h_stride;
+    p.kcache = at.kcache; p.kv_b_stride = at.kv_b_stride; p.kv_h_stride = at.kv_h_stride; p.kv_b_div = at.kv_b_div;
     p.key_mask = at.key_mask; p.mask_len = at.mask_len; p.mask_ld = at.mask_ld;
     p.B = B; p.nh = L.nh; p.nkv = at.nkv; p.q_len = q_len; p.cross = at.cross;
     const int64_t ld = at.cross ? S : pw->self_ld;
@@ -495,8 +508,9 @@ static int run_forward(ptts_session* s, cudaStream_t st, bool prefill, const voi
   };
   if (int e = probe_rows(0, false)) return e;
 
+  // plan_rows: the row count that picks the kernel (default Mrows); the GEMMs' per-row results do not depend on M otherwise
   auto lin = [&](const void* X, int64_t ldx, int64_t woff, int N, int K, const float* lw, const float* lb, int epi,
-                 const void* R, void* Y, int64_t ldy, int Mrows, int64_t coff = -1) -> int {
+                 const void* R, void* Y, int64_t ldy, int Mrows, int64_t coff = -1, int plan_rows = 0) -> int {
     LinearArgs a{};
     a.X = X; a.ldx = ldx; a.W = blob + woff; a.Y = Y; a.ldy = ldy; a.R = R; a.ldr = ldy;
     a.ln_w = lw; a.ln_b = lb; a.eps = c.layer_norm_eps;
@@ -508,7 +522,9 @@ static int run_forward(ptts_session* s, cudaStream_t st, bool prefill, const voi
     s->launches++;
     // the same matrix, row-major: M = B*(P+n0) or B*S rows are tensor-core work (wgmma, gemm_tc.cu)
     const int64_t rm = prefill ? rowmajor_offset(L, woff) : -1;
-    if (rm >= 0 && linear_tc_supported(a)) {
+    LinearArgs plan = a;
+    if (plan_rows > 0) plan.M = plan_rows;
+    if (rm >= 0 && linear_tc_supported(plan)) {
       if (a.c1 != nullptr) s->launches++;  // row statistics kernel
       return launch_linear_tc(a, blob + rm, (float*)(ws + W.row_stats), st);
     }
@@ -518,10 +534,12 @@ static int run_forward(ptts_session* s, cudaStream_t st, bool prefill, const voi
   for (int i = 0; i < L.L; i++) {
     const int64_t lb = L.layer0 + L.layer_stride * i;
     char* x = ws + W.x;
-    if (prefill) {  // cross-attention K/V of the encoder states, once per generate() (:872-878)
+    if (prefill) {  // cross-attention K/V of the encoder states, once per generate() and description (:872-878)
+      // the kernel is the one B * S rows take, so that the takes of a description get the bits B expanded rows would get (the
+      // wgmma GEMM zero-fills the rows of a partial 128-row tile, also below 128 rows)
       if (int e = lin(enc_hidden, H, lb + L.wkvc, L.ckv_rows, H, nullptr, nullptr, EPI_STORE, nullptr,
-                      ws + W.cross_tmp, L.ckv_rows, B * S)) return e;
-      if (int e = launch_cross_kv_relayout(ws + W.cross_tmp, ws + W.cross_kv + W.cross_layer_stride * i, B, S, L.nckv, c.dtype, st)) return e;
+                      ws + W.cross_tmp, L.ckv_rows, n_desc * S, -1, B * S)) return e;
+      if (int e = launch_cross_kv_relayout(ws + W.cross_tmp, ws + W.cross_kv + W.cross_layer_stride * i, n_desc, S, L.nckv, c.dtype, st)) return e;
       s->launches++;
     }
     if (int e = lin(x, H, lb + L.wqkv, L.qkv_rows, H, (const float*)(blob + lb + L.ln1_w), (const float*)(blob + lb + L.ln1_b),
@@ -531,7 +549,7 @@ static int run_forward(ptts_session* s, cudaStream_t st, bool prefill, const voi
     at.knew = ws + W.qkv; at.vnew = ws + W.qkv; at.ldkv = L.qkv_rows; at.k_col0 = L.nh * D; at.v_col0 = (L.nh + L.nkv) * D;
     char* kc = ws + W.self_kv + W.self_layer_stride * i;
     at.kcache = kc; at.vcache = kc + (int64_t)B * L.nkv * W.Tmax * D * es;
-    at.kv_b_stride = (int64_t)L.nkv * W.Tmax * D; at.kv_h_stride = (int64_t)W.Tmax * D; at.kv_t_stride = D;
+    at.kv_b_stride = (int64_t)L.nkv * W.Tmax * D; at.kv_h_stride = (int64_t)W.Tmax * D; at.kv_t_stride = D; at.kv_b_div = 1;
     at.out = ws + W.attn; at.ldo = H;
     at.key_mask = s->has_prompt_mask ? (const int*)(ws + W.prompt_mask) : nullptr; at.mask_len = P; at.mask_ld = P;
     at.ctrl = ctrl; at.B = B; at.nh = L.nh; at.nkv = L.nkv; at.q_len = q_len;
@@ -550,8 +568,8 @@ static int run_forward(ptts_session* s, cudaStream_t st, bool prefill, const voi
     ct.q = ws + W.qc; ct.ldq = H; ct.q_col0 = 0;
     ct.knew = ct.vnew = nullptr;
     char* ck = ws + W.cross_kv + W.cross_layer_stride * i;
-    ct.kcache = ck; ct.vcache = ck + (int64_t)B * L.nckv * S * D * es;   // item-major: K [B][nckv][S][64] | V [...]
-    ct.kv_b_stride = (int64_t)L.nckv * S * D; ct.kv_h_stride = (int64_t)S * D; ct.kv_t_stride = D;
+    ct.kcache = ck; ct.vcache = ck + (int64_t)n_desc * L.nckv * S * D * es;   // item-major: K [B/takes][nckv][S][64] | V [...]
+    ct.kv_b_stride = (int64_t)L.nckv * S * D; ct.kv_h_stride = (int64_t)S * D; ct.kv_t_stride = D; ct.kv_b_div = W.takes;
     ct.key_mask = s->has_enc_mask ? (const int*)(ws + W.enc_mask) : nullptr; ct.mask_len = S; ct.mask_ld = S;
     ct.nkv = L.nckv; ct.cross = 1; ct.kv_len = S; ct.kv_capacity = S;
     if (int e = launch_attention(ct, c.dtype, st, pdl, true)) return e;
@@ -579,7 +597,7 @@ int ptts_prefill(ptts_session* s, const void* prompt_hidden, const int64_t* prom
   s->has_prompt_mask = (prompt_mask != nullptr && s->W.P > 0);
   s->has_enc_mask = (enc_mask != nullptr);
   if (s->has_prompt_mask) { if (int e = launch_mask_convert(prompt_mask, s->W.B * s->W.P, (int*)(s->ws + s->W.prompt_mask), st)) return e; }
-  if (s->has_enc_mask) { if (int e = launch_mask_convert(enc_mask, s->W.B * s->W.S, (int*)(s->ws + s->W.enc_mask), st)) return e; }
+  if (s->has_enc_mask) { if (int e = launch_mask_convert(enc_mask, s->W.B / s->W.takes * s->W.S, (int*)(s->ws + s->W.enc_mask), st)) return e; }
   if (int e = run_forward(s, st, true, prompt_hidden, enc_hidden)) return e;
   s->prefilled = true;
   s->path = choose_decode_path(s);
@@ -625,7 +643,7 @@ int ptts_score(ptts_session* s, const void* prompt_hidden, const int64_t* prompt
   s->has_prompt_mask = (prompt_mask != nullptr && W.P > 0);
   s->has_enc_mask = (enc_mask != nullptr);
   if (s->has_prompt_mask) { if (int e = launch_mask_convert(prompt_mask, W.B * W.P, (int*)(s->ws + W.prompt_mask), st)) return e; }
-  if (s->has_enc_mask) { if (int e = launch_mask_convert(enc_mask, W.B * W.S, (int*)(s->ws + W.enc_mask), st)) return e; }
+  if (s->has_enc_mask) { if (int e = launch_mask_convert(enc_mask, W.B / W.takes * W.S, (int*)(s->ws + W.enc_mask), st)) return e; }
   s->n0 = T;
   s->begun = s->prefilled = false;  // the caches now hold this call's positions: a generation has to begin again
   if (int e = run_forward(s, st, true, prompt_hidden, enc_hidden, false)) return e;
@@ -874,7 +892,7 @@ int ptts_op_attention(int32_t dtype, int32_t B, int32_t nh, int32_t nkv, int32_t
     a.ldq = a.ldkv = (int64_t)(nh + 2 * nkv) * D; a.k_col0 = nh * D; a.v_col0 = (nh + nkv) * D;
   }
   a.kcache = kcache; a.vcache = vcache;
-  a.kv_b_stride = (int64_t)nkv * capacity * D; a.kv_h_stride = (int64_t)capacity * D; a.kv_t_stride = D;
+  a.kv_b_stride = (int64_t)nkv * capacity * D; a.kv_h_stride = (int64_t)capacity * D; a.kv_t_stride = D; a.kv_b_div = 1;
   a.out = out; a.ldo = (int64_t)nh * D;
   a.key_mask = key_mask; a.mask_len = mask_len; a.mask_ld = mask_len;
   a.B = B; a.nh = nh; a.nkv = nkv; a.q_len = q_len;
@@ -899,6 +917,7 @@ int ptts_op_attention_probs(int32_t dtype, int32_t B, int32_t nh, int32_t nkv, i
   AttnProbeArgs a{};
   a.q = q; a.ldq = ldq; a.q_col0 = 0;
   a.kcache = kcache; a.kv_b_stride = (int64_t)nkv * capacity * PTTS_HEAD_DIM; a.kv_h_stride = (int64_t)capacity * PTTS_HEAD_DIM;
+  a.kv_b_div = 1;
   a.key_mask = key_mask; a.mask_len = mask_len; a.mask_ld = mask_len;
   a.B = B; a.nh = nh; a.nkv = nkv; a.q_len = q_len; a.cross = cross ? 1 : 0;
   a.kv_len = kv_len; a.pos0 = past_len; a.kv_cap = kv_len;

@@ -65,8 +65,9 @@ __global__ void __launch_bounds__(PRE_TC_WARPS * 32) attention_prefill_tc_kernel
   if (p.ctrl != nullptr && p.ctrl->active == 0) return;
   const int b = blockIdx.y, h = blockIdx.x;
   const int past = p.past_len;
-  bf16* kc = reinterpret_cast<bf16*>(p.kcache) + (size_t)b * p.kv_b_stride + (size_t)h * p.kv_h_stride;
-  bf16* vc = reinterpret_cast<bf16*>(p.vcache) + (size_t)b * p.kv_b_stride + (size_t)h * p.kv_h_stride;
+  const int kvb = b / p.kv_b_div;   // batch index of the K/V rows and the key mask
+  bf16* kc = reinterpret_cast<bf16*>(p.kcache) + (size_t)kvb * p.kv_b_stride + (size_t)h * p.kv_h_stride;
+  bf16* vc = reinterpret_cast<bf16*>(p.vcache) + (size_t)kvb * p.kv_b_stride + (size_t)h * p.kv_h_stride;
   if (!p.cross) {   // append the new rows (same arithmetic as attention_item's phase A)
     const bf16* rope_cos = reinterpret_cast<const bf16*>(p.rope_cos);
     const bf16* rope_sin = reinterpret_cast<const bf16*>(p.rope_sin);
@@ -98,7 +99,7 @@ __global__ void __launch_bounds__(PRE_TC_WARPS * 32) attention_prefill_tc_kernel
     it.q = reinterpret_cast<const bf16*>(p.q) + r * p.ldq + p.q_col0 + (size_t)h * HD;
     it.knew = nullptr; it.vnew = nullptr;
     it.kc = kc; it.vc = vc;
-    it.km = p.key_mask ? p.key_mask + (size_t)b * p.mask_ld : nullptr; it.mask_len = p.mask_len;
+    it.km = p.key_mask ? p.key_mask + (size_t)kvb * p.mask_ld : nullptr; it.mask_len = p.mask_len;
     it.n_cached = p.cross ? p.kv_len : past + j + 1;   // causal: the rows up to and including this position (already in the cache)
     it.pos = past + j; it.cross = 1;                    // (no separate "own key" step)
     it.rope = p.rope; it.rope_cos = reinterpret_cast<const bf16*>(p.rope_cos); it.rope_sin = reinterpret_cast<const bf16*>(p.rope_sin);

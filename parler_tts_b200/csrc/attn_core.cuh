@@ -48,8 +48,9 @@ __device__ __forceinline__ void attention_item(const AttnArgs& p, int b, int kvh
   int past = p.past_len;
   if (p.past_from_ctrl) past = p.prefix + p.ctrl->cur_len - 1;
 
-  T* kc = reinterpret_cast<T*>(p.kcache) + (size_t)b * p.kv_b_stride + (size_t)kvh * p.kv_h_stride;
-  T* vc = reinterpret_cast<T*>(p.vcache) + (size_t)b * p.kv_b_stride + (size_t)kvh * p.kv_h_stride;
+  const int kvb = b / p.kv_b_div;   // batch index of the K/V rows and the key mask
+  T* kc = reinterpret_cast<T*>(p.kcache) + (size_t)kvb * p.kv_b_stride + (size_t)kvh * p.kv_h_stride;
+  T* vc = reinterpret_cast<T*>(p.vcache) + (size_t)kvb * p.kv_b_stride + (size_t)kvh * p.kv_h_stride;
 
   // ---- phase A: append the new K/V rows (self-attention only) ----
   if (!p.cross) {
@@ -77,7 +78,7 @@ __device__ __forceinline__ void attention_item(const AttnArgs& p, int b, int kvh
   const int grp = lane >> 3;           // key group inside the warp (4 keys per warp per iteration)
   const int d0 = (lane & 7) * 8;       // this lane's 8 dims
   const int kslot = warp * 4 + grp;    // 0..15
-  const int* km = p.key_mask ? p.key_mask + (size_t)b * p.mask_ld : nullptr;
+  const int* km = p.key_mask ? p.key_mask + (size_t)kvb * p.mask_ld : nullptr;
 
   // [q_lo, q_hi): the query positions this group sweeps (the prefill kernel cuts the positions over blockIdx.z; every group appends
   // ALL new K/V rows itself above -- identical values, so the duplicate global writes are benign -- and reads only what it wrote)
@@ -238,8 +239,9 @@ __device__ __forceinline__ void attn_decode_issue_chunk(const T* kc, const T* vc
 template <typename T, int CH = AttChunk<T>::CH>
 __device__ __forceinline__ void attention_decode_request(const AttnArgs& p, int b, int kvh, int pos, unsigned char* stage0, uint64_t* bars, int lane,
                                                          int part, int nparts) {
-  const T* kc = reinterpret_cast<const T*>(p.kcache) + (size_t)b * p.kv_b_stride + (size_t)kvh * p.kv_h_stride;
-  const T* vc = reinterpret_cast<const T*>(p.vcache) + (size_t)b * p.kv_b_stride + (size_t)kvh * p.kv_h_stride;
+  const int kvb = b / p.kv_b_div;
+  const T* kc = reinterpret_cast<const T*>(p.kcache) + (size_t)kvb * p.kv_b_stride + (size_t)kvh * p.kv_h_stride;
+  const T* vc = reinterpret_cast<const T*>(p.vcache) + (size_t)kvb * p.kv_b_stride + (size_t)kvh * p.kv_h_stride;
   const int n_cached = p.cross ? p.kv_len : pos;
   if (attn_decode_warp_chunks(n_cached, CH, part, nparts) > 0)
     attn_decode_issue_chunk<T, CH>(kc, vc, n_cached, 0, part, nparts, reinterpret_cast<T*>(stage0), &bars[0], lane);
@@ -266,8 +268,9 @@ __device__ __forceinline__ void attention_decode_sweep(const AttnArgs& p, int b,
   const T* __restrict__ rope_cos = reinterpret_cast<const T*>(p.rope_cos) + (size_t)pos * HD;
   const T* __restrict__ rope_sin = reinterpret_cast<const T*>(p.rope_sin) + (size_t)pos * HD;
   const int rep = p.nh / p.nkv;
-  T* kc = reinterpret_cast<T*>(p.kcache) + (size_t)b * p.kv_b_stride + (size_t)kvh * p.kv_h_stride;
-  T* vc = reinterpret_cast<T*>(p.vcache) + (size_t)b * p.kv_b_stride + (size_t)kvh * p.kv_h_stride;
+  const int kvb = b / p.kv_b_div;   // batch index of the K/V rows and the key mask
+  T* kc = reinterpret_cast<T*>(p.kcache) + (size_t)kvb * p.kv_b_stride + (size_t)kvh * p.kv_h_stride;
+  T* vc = reinterpret_cast<T*>(p.vcache) + (size_t)kvb * p.kv_b_stride + (size_t)kvh * p.kv_h_stride;
   const int lo = lane, hi = lane + HD / 2;
   const int n_cached = p.cross ? p.kv_len : pos;  // keys that come from the cache
   const int n_chunks = attn_decode_warp_chunks(n_cached, CH, part, nparts);  // chunks of THIS warp
@@ -319,7 +322,7 @@ __device__ __forceinline__ void attention_decode_sweep(const AttnArgs& p, int b,
     vn[lo] = DT<T>::to_f(v0); vn[hi] = DT<T>::to_f(v1);
   }
   const int grp = lane >> 3, d0 = (lane & 7) * 8;
-  const int* km = p.key_mask ? p.key_mask + (size_t)b * p.mask_ld : nullptr;
+  const int* km = p.key_mask ? p.key_mask + (size_t)kvb * p.mask_ld : nullptr;
 
   for (int rr = 0; rr < rep; rr++) {
     const int h = kvh * rep + rr;

@@ -33,6 +33,8 @@ struct AttnArgs {
   const void* knew; const void* vnew; int64_t ldkv; int k_col0, v_col0;  // self: new K/V rows (same matrix as q)
   void* kcache; void* vcache;                   // self: [B][nkv][Tmax][64]; cross: strided view
   int64_t kv_b_stride, kv_h_stride, kv_t_stride; // element strides of (batch, kv head, token)
+  int kv_b_div;         // row b reads the K/V and key-mask rows of batch index b / kv_b_div (cross-attention of a session whose
+                        // consecutive rows share one description, ptts_session_create3); 1: its own
   void* out; int64_t ldo;                       // [B*q_len, H]
   const int* key_mask; int mask_len, mask_ld;   // keys t < mask_len with key_mask[b*mask_ld+t]==0 are excluded
   const Ctrl* ctrl;
@@ -54,6 +56,7 @@ int launch_attention(const AttnArgs& a, int dtype, cudaStream_t st, bool pdl, bo
 struct AttnProbeArgs {
   const void* q; int64_t ldq; int q_col0;          // row b*q_len + j, head h at columns q_col0 + h*64 (before RoPE and scaling)
   const void* kcache; int64_t kv_b_stride, kv_h_stride;  // K rows [..][64], swizzled (kv_swz)
+  int kv_b_div;                                    // row b reads K rows and key mask of batch index b / kv_b_div (AttnArgs)
   const int* key_mask; int mask_len, mask_ld;      // keys t < mask_len with key_mask[b*mask_ld+t] == 0 are masked
   int B, nh, nkv, q_len;
   int cross;                                       // 1: kv_len keys, no causal mask

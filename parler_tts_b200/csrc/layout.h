@@ -4,7 +4,7 @@
 //   blob      : [embed tables K x (V+1) x H][pos table][L x layer][final LN][lm heads (K*V) x H]
 //               GEMM matrices are stored in mma.m16n8k16 B-fragment order (bf16) so a warp's 512 B
 //               load is one fully coalesced request and needs no shared-memory staging.
-//   workspace : control block, token history, activations, cross K/V [L][B*S][2*nckv*64],
+//   workspace : control block, token history, activations, cross K/V [L][(B/takes)*S][2*nckv*64],
 //               self K/V cache [L][2][B][nkv][Tmax][64].
 #pragma once
 #include "common.cuh"
@@ -155,6 +155,7 @@ static inline bool matrix_slot(const DecoderLayout& l, int tensor_id, int index,
 // ---- workspace ----------------------------------------------------------------------------------
 struct WorkspaceLayout {
   int B, P, S, Tmax, Mmax, BK;
+  int takes;                       // consecutive rows per description: cross K/V and enc_mask hold B / takes descriptions
   int max_input;                   // largest decoder input (BOS column + code prefix) a generate() call may continue from
   int64_t ctrl, progress, gen, raw_ids, cur_ids, eos_seen, unfinished, first_unf, prompt_mask, enc_mask;
   int64_t prefix_cells;            // [BK][K-1] int64: delay-pattern cells just past the input (max_input > 1 only; -1 = none)
@@ -168,10 +169,13 @@ struct WorkspaceLayout {
 };
 
 // max_input = 1: the BOS column only; the layout is then the same as before continuation existed (prefix_cells takes no bytes).
-static inline WorkspaceLayout make_workspace(const ptts_decoder_config& c, int B, int P, int S, int Tmax, int max_input = 1) {
+// takes (divides B): rows b .. b + takes - 1 of each group are takes of one description and read its cross K/V; takes = 1 is the
+// layout of one description per row.  Only the cross K/V (and its re-layout buffer) and enc_mask depend on it.
+static inline WorkspaceLayout make_workspace(const ptts_decoder_config& c, int B, int P, int S, int Tmax, int max_input = 1, int takes = 1) {
   DecoderLayout l = make_layout(c);
   WorkspaceLayout w{};
   w.B = B; w.P = P; w.S = S; w.Tmax = Tmax; w.BK = B * c.num_codebooks;
+  w.takes = takes;
   w.max_input = max_input;
   w.Mmax = B * (P + max_input);
   int64_t o = 0;
@@ -186,10 +190,10 @@ static inline WorkspaceLayout make_workspace(const ptts_decoder_config& c, int B
   w.unfinished = take((int64_t)w.BK * 4);
   w.first_unf = take((int64_t)2 * B * 4);
   w.prompt_mask = take((int64_t)B * (P > 0 ? P : 1) * 4);
-  w.enc_mask = take((int64_t)B * S * 4);
+  w.enc_mask = take((int64_t)(B / takes) * S * 4);
   w.prefix_cells = -1;
   if (max_input > 1 && c.num_codebooks > 1) w.prefix_cells = take((int64_t)w.BK * (c.num_codebooks - 1) * 8);
-  int64_t rows_enc = (int64_t)B * S;
+  const int64_t rows_enc = (int64_t)B * S, rows_cross = (int64_t)(B / takes) * S;
   w.x = take((int64_t)w.Mmax * l.H * l.es);
   w.qkv = take((int64_t)w.Mmax * l.qkv_rows * l.es);
   w.attn = take((int64_t)w.Mmax * l.H * l.es);
@@ -205,7 +209,7 @@ static inline WorkspaceLayout make_workspace(const ptts_decoder_config& c, int B
   w.cl_h = take((int64_t)4 * 32 * (l.F / 4 + 8) * 2);
   w.logits = take((int64_t)w.BK * l.V * 4);
   w.scores = take((int64_t)w.BK * l.V * 4);
-  w.cross_layer_stride = align_up(rows_enc * l.ckv_rows * l.es, 256);
+  w.cross_layer_stride = align_up(rows_cross * l.ckv_rows * l.es, 256);
   w.cross_tmp = take(w.cross_layer_stride);   // GEMM output of one layer before the item-major re-layout
   w.cross_kv = take(w.cross_layer_stride * l.L);
   w.self_layer_stride = align_up((int64_t)2 * B * l.nkv * Tmax * PTTS_HEAD_DIM * l.es, 256);

@@ -49,10 +49,11 @@ __global__ void __launch_bounds__(QT * 32) attention_probs_kernel(AttnProbeArgs 
   const int pos0 = a.ctrl != nullptr ? a.prefix + cur_len - 1 : a.pos0;   // position of query row 0
   const int T_kv = a.cross ? a.kv_len : (a.ctrl != nullptr ? pos0 + 1 : a.kv_len);
   const int kvh = h / (a.nh / a.nkv);
-  const T* kc = reinterpret_cast<const T*>(a.kcache) + (size_t)b * a.kv_b_stride + (size_t)kvh * a.kv_h_stride;
+  const int kvb = b / a.kv_b_div;   // batch index of the K rows and the key mask
+  const T* kc = reinterpret_cast<const T*>(a.kcache) + (size_t)kvb * a.kv_b_stride + (size_t)kvh * a.kv_h_stride;
   const T* rope_cos = reinterpret_cast<const T*>(a.rope_cos);
   const T* rope_sin = reinterpret_cast<const T*>(a.rope_sin);
-  const int* km = a.key_mask ? a.key_mask + (size_t)b * a.mask_ld : nullptr;
+  const int* km = a.key_mask ? a.key_mask + (size_t)kvb * a.mask_ld : nullptr;
   const int nq = min(QT, a.q_len - j0);
 
   for (int i = threadIdx.x; i < QT * HD; i += blockDim.x) {

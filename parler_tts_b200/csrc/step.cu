@@ -124,8 +124,9 @@ __device__ __forceinline__ void prefetch_kv(const StepParams& p, int l, int pos)
   }
   if (lane == 0) {  // cross K/V of this CTA's items (item-major, contiguous)
     const char* ck = p.cross_kv + p.cross_layer_stride * l;
-    const size_t vofs = (size_t)p.B * p.nckv * p.S * HD * 2;
-    for (int it = blockIdx.x + gridDim.x * pw; it < p.B * p.nckv; it += gridDim.x * 4) {
+    const int items = (p.B / p.takes) * p.nckv;   // one per (description, kv head)
+    const size_t vofs = (size_t)items * p.S * HD * 2;
+    for (int it = blockIdx.x + gridDim.x * pw; it < items; it += gridDim.x * 4) {
       const char* k = ck + (size_t)it * p.S * HD * 2;
       l2_prefetch(k, (uint32_t)(p.S * HD * 2));
       l2_prefetch(k + vofs, (uint32_t)(p.S * HD * 2));

@@ -9,6 +9,7 @@ namespace ptts {
 struct StepParams {
   // shapes
   int B, H, F, V, K, L, nh, nkv, nckv, S, P, Tmax, rope, act, qkv_rows, ckv_rows;
+  int takes;               // consecutive rows that share one description's cross K/V and encoder mask (B / takes of each)
   float eps, scale;
   // packed weights: blob offsets from the session's layout (the cluster kernel's weight slices: lay.cp, lay.cp_slice)
   const char* blob;

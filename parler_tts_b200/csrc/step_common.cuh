@@ -39,13 +39,13 @@ __device__ __forceinline__ AttnArgs decode_attn_args(const StepParams& p, int l,
   if (!cross) {
     char* kc = p.self_kv + p.self_layer_stride * l;
     a.kcache = kc; a.vcache = kc + (size_t)p.B * p.nkv * p.Tmax * HD * 2;
-    a.kv_b_stride = (int64_t)p.nkv * p.Tmax * HD; a.kv_h_stride = (int64_t)p.Tmax * HD; a.kv_t_stride = HD;
+    a.kv_b_stride = (int64_t)p.nkv * p.Tmax * HD; a.kv_h_stride = (int64_t)p.Tmax * HD; a.kv_t_stride = HD; a.kv_b_div = 1;
     a.key_mask = p.prompt_mask; a.mask_len = p.P; a.mask_ld = p.P;
     a.nkv = p.nkv; a.cross = 0; a.kv_len = 0; a.kv_capacity = p.Tmax;
   } else {
     char* ck = p.cross_kv + p.cross_layer_stride * l;
-    a.kcache = ck; a.vcache = ck + (size_t)p.B * p.nckv * p.S * HD * 2;
-    a.kv_b_stride = (int64_t)p.nckv * p.S * HD; a.kv_h_stride = (int64_t)p.S * HD; a.kv_t_stride = HD;
+    a.kcache = ck; a.vcache = ck + (size_t)(p.B / p.takes) * p.nckv * p.S * HD * 2;   // one K/V item per description
+    a.kv_b_stride = (int64_t)p.nckv * p.S * HD; a.kv_h_stride = (int64_t)p.S * HD; a.kv_t_stride = HD; a.kv_b_div = p.takes;
     a.key_mask = p.enc_mask; a.mask_len = p.S; a.mask_ld = p.S;
     a.nkv = p.nckv; a.cross = 1; a.kv_len = p.S; a.kv_capacity = p.S;
   }

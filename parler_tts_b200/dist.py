@@ -19,7 +19,9 @@ def shard_range(n: int, rank: int, world: int) -> tuple[int, int]:
 
 
 def shard_row_base(n: int, rank: int, world: int, num_codebooks: int) -> int:
-    """Global (utterance, codebook) row index of this rank's first row: the `row_base` to pass to generate()."""
+    """Global (utterance, codebook) row index of this rank's first row: the `row_base` to pass to generate().  row_base counts
+    takes: with generate(num_return_sequences=N) pass shard_row_base(...) * N, so that take j of description b draws the
+    substreams of global row (b * N + j) * num_codebooks + k whatever the number of ranks."""
     return shard_range(n, rank, world)[0] * num_codebooks
 
 

@@ -88,6 +88,37 @@ def check_continuation_length(n0: int, prompt_len: int, max_length: int, max_pos
         raise ValueError(f"{prompt_len} prompt positions + max_length {max_length} exceed max_position_embeddings {max_position_embeddings}")
 
 
+def resolve_num_return_sequences(gc) -> int:
+    """generate()'s takes per description, validated as transformers does (GenerationConfig.validate): an int >= 1, and > 1 only
+    with sampling."""
+    n = gc.num_return_sequences
+    if isinstance(n, bool) or not isinstance(n, int) or n < 1:
+        raise ValueError(f"`num_return_sequences` has to be a strictly positive integer, got {n!r}")
+    if n > 1 and not gc.do_sample:
+        raise ValueError(f"Greedy methods without beam search do not support `num_return_sequences` different than 1 (got {n}).")
+    return n
+
+
+def expand_takes(ids: torch.Tensor, batch_size: int, num_codebooks: int, takes: int) -> torch.Tensor:
+    """[B * K, n] utterance-major code rows -> [B * takes * K, n]: the K rows of utterance b, as one group, once for each of its
+    takes, so that take j of utterance b is utterance b * takes + j (never a repeat of single [B * K] rows)."""
+    return ids.reshape(batch_size, num_codebooks, -1).repeat_interleave(takes, dim=0).reshape(batch_size * takes * num_codebooks, -1)
+
+
+def take_shards(batch_size: int, takes: int, limit: Optional[int]) -> list[tuple[int, int, int, int]]:
+    """The sessions generate() runs for batch_size descriptions x `takes` takes: (first description, end, first output row, end)
+    each, every session's rows whole groups of takes of its descriptions (its takes = rows / descriptions).  limit: the rows one
+    session may hold (None: one session).  takes <= limit: floor(limit / takes) descriptions per session; takes > limit: up to
+    `limit` takes of one description per session."""
+    n = batch_size * takes
+    if limit is None or n <= limit:
+        return [(0, batch_size, 0, n)]
+    if takes <= limit:
+        g = limit // takes
+        return [(d0, min(batch_size, d0 + g), d0 * takes, min(batch_size, d0 + g) * takes) for d0 in range(0, batch_size, g)]
+    return [(b, b + 1, b * takes + j0, b * takes + min(takes, j0 + limit)) for b in range(batch_size) for j0 in range(0, takes, limit)]
+
+
 def shift_tokens_right(input_ids: torch.Tensor, pad_token_id: int, decoder_start_token_id: int):
     """The reference's shift_tokens_right (:308-323): one position to the right along dim 1, decoder_start_token_id first, -100
     replaced by pad_token_id.  Host-side integer work: labels [B, T, K] -> the decoder input [B, T, K]."""
@@ -418,31 +449,33 @@ class DecoderEngine:
             return sd[f"{prefix}lm_heads.weight"][k * V:(k + 1) * V]
         raise ValueError(f"missing weight {prefix}lm_heads.{k}.weight")
 
-    def session(self, B: int, P: int, S: int, max_cache_len: int, max_input_len: int = 1) -> "GenSession":
-        """max_input_len: the most decoder input columns (BOS column + code prefix) a generate() call on it may continue from."""
+    def session(self, B: int, P: int, S: int, max_cache_len: int, max_input_len: int = 1, takes: int = 1) -> "GenSession":
+        """max_input_len: the most decoder input columns (BOS column + code prefix) a generate() call on it may continue from.
+        takes: consecutive rows that are takes of one description and share its cross-attention K/V (ptts_session_create3)."""
         key = (B, P, S)
         s = self._sessions.get(key)
-        if s is None or s.max_cache_len < max_cache_len or s.max_input_len < max_input_len:
+        if s is None or s.max_cache_len < max_cache_len or s.max_input_len < max_input_len or s.takes != takes:
             if s is not None:
                 s.close()
-            s = GenSession(self, B, P, S, max_cache_len, max_input_len)
+            s = GenSession(self, B, P, S, max_cache_len, max_input_len, takes)
             self._sessions = {key: s}  # keep one live session (the reference keeps one `_cache`, :3254-3309)
         return s
 
 
 class GenSession:
-    """Device-resident generation state for (B, P, S): KV caches, token history, processor state."""
+    """Device-resident generation state for (B, P, S): KV caches, token history, processor state.  With takes > 1 the B rows are
+    B / takes descriptions with `takes` consecutive takes each: prefill / score take B / takes encoder rows, everything else B."""
 
-    def __init__(self, eng: DecoderEngine, B: int, P: int, S: int, max_cache_len: int, max_input_len: int = 1):
+    def __init__(self, eng: DecoderEngine, B: int, P: int, S: int, max_cache_len: int, max_input_len: int = 1, takes: int = 1):
         self.eng, self.B, self.P, self.S, self.max_cache_len = eng, B, P, S, max_cache_len
-        self.max_input_len = int(max_input_len)
+        self.max_input_len, self.takes = int(max_input_len), int(takes)
         lib = _lib.lib()
         n = C.c_int64()
-        _lib.check(lib.ptts_workspace_bytes2(C.byref(eng.c), B, P, S, max_cache_len, self.max_input_len, C.byref(n)))
+        _lib.check(lib.ptts_workspace_bytes3(C.byref(eng.c), B, P, S, max_cache_len, self.max_input_len, self.takes, C.byref(n)))
         self.ws = torch.zeros(n.value, dtype=torch.uint8, device=eng.device)
         h = C.c_void_p()
-        _lib.check(lib.ptts_session_create2(C.byref(eng.c), _lib.ptr(eng.blob), _lib.ptr(self.ws), n.value, B, P, S,
-                                            max_cache_len, self.max_input_len, C.byref(h)))
+        _lib.check(lib.ptts_session_create3(C.byref(eng.c), _lib.ptr(eng.blob), _lib.ptr(self.ws), n.value, B, P, S,
+                                            max_cache_len, self.max_input_len, self.takes, C.byref(h)))
         self.h = h
         self.K, self.V = eng.cfg.num_codebooks, eng.cfg.vocab_size
         self._keep: list[Any] = []
@@ -533,8 +566,8 @@ class GenSession:
         dt, dev = self.eng.dtype, self.eng.device
         H = self.eng.cfg.hidden_size
         enc_hidden = enc_hidden.to(device=dev, dtype=dt).contiguous()
-        if tuple(enc_hidden.shape) != (self.B, self.S, H):
-            raise ValueError(f"encoder states must be [{self.B}, {self.S}, {H}], got {tuple(enc_hidden.shape)}")
+        if tuple(enc_hidden.shape) != (self.B // self.takes, self.S, H):
+            raise ValueError(f"encoder states must be [{self.B // self.takes}, {self.S}, {H}], got {tuple(enc_hidden.shape)}")
         if self.P > 0:
             if prompt_hidden is None:
                 raise ValueError("prompt_hidden_states are required for a session created with P > 0")
@@ -553,8 +586,8 @@ class GenSession:
         dt, dev = self.eng.dtype, self.eng.device
         H = self.eng.cfg.hidden_size
         enc_hidden = enc_hidden.to(device=dev, dtype=dt).contiguous()
-        if tuple(enc_hidden.shape) != (self.B, self.S, H):
-            raise ValueError(f"encoder states must be [{self.B}, {self.S}, {H}], got {tuple(enc_hidden.shape)}")
+        if tuple(enc_hidden.shape) != (self.B // self.takes, self.S, H):
+            raise ValueError(f"encoder states must be [{self.B // self.takes}, {self.S}, {H}], got {tuple(enc_hidden.shape)}")
         if self.P > 0:
             prompt_hidden = prompt_hidden.to(device=dev, dtype=dt).contiguous()
             if tuple(prompt_hidden.shape) != (self.B, self.P, H):
@@ -904,7 +937,7 @@ class ParlerTTSForConditionalGeneration:
                                "encoder_outputs", "input_values", "decoder_input_ids", "padding_mask", "use_cache",
                                "cache_implementation", "output_attentions", "output_hidden_states"})
     # GenerationConfig fields the device loop does not implement, with the value that means "off"
-    _NEUTRAL_GENERATION_KNOBS = {"num_return_sequences": 1, "num_beam_groups": 1, "repetition_penalty": 1.0, "length_penalty": 1.0,
+    _NEUTRAL_GENERATION_KNOBS = {"num_beam_groups": 1, "repetition_penalty": 1.0, "length_penalty": 1.0,
                                  "penalty_alpha": None, "bad_words_ids": None, "force_words_ids": None, "guidance_scale": None}
 
     def __init__(self, config: ParlerTTSConfig, device="cuda", dtype=torch.bfloat16, text_encoder=None):
@@ -1138,8 +1171,10 @@ class ParlerTTSForConditionalGeneration:
         return 32
 
     def _run_token_loop(self, enc_hidden, attention_mask, prompt_hidden, prompt_mask, *, gc, max_length, seed, suppress_special, row_base,
-                        ext, min_new_tokens, streamer=None, custom=None, input_ids=None, outputs=None, out_row=0, probes=None):
+                        ext, min_new_tokens, streamer=None, custom=None, input_ids=None, outputs=None, out_row=0, probes=None, takes=1):
         """begin + prefill + the token loop of one session; returns the raw token matrix [B * K, generated length].
+        takes: the session's B rows are `takes` consecutive takes of each of the enc_hidden.shape[0] descriptions (B / takes);
+        prompt_hidden, prompt_mask and input_ids have B rows.
         input_ids: None, or the BOS-led decoder input [B * K, n0] this shard continues from.
         outputs: None, or the StepOutputs this session's rows (from row out_row of the batch) are recorded into.  The device
         loop then sets the sampler's window before every call and keeps each call inside one chunk.
@@ -1147,10 +1182,11 @@ class ParlerTTSForConditionalGeneration:
         its windows follow the same chunks, and the decode steps then run the multi-kernel path (ptts_generate_set_probes)."""
         d = self.config.decoder
         K = d.num_codebooks
-        B, S, _ = enc_hidden.shape
+        S = enc_hidden.shape[1]
+        B = enc_hidden.shape[0] * takes
         P = 0 if prompt_hidden is None else prompt_hidden.shape[1]
         n0 = 1 if input_ids is None else int(input_ids.shape[1])
-        sess = self.decoder.engine.session(B, P, S, P + max_length, max_input_len=n0)
+        sess = self.decoder.engine.session(B, P, S, P + max_length, max_input_len=n0, takes=takes)
         sess.begin(max_length, do_sample=gc.do_sample, temperature=gc.temperature, top_k=gc.top_k if gc.do_sample else 0,
                    top_p=gc.top_p, min_new_tokens=min_new_tokens, seed=seed, suppress_special=suppress_special,
                    codebook_size=self.config.audio_encoder.codebook_size, row_base=row_base, input_ids=input_ids,
@@ -1370,6 +1406,14 @@ class ParlerTTSForConditionalGeneration:
         config.prompt_cross_attention: `prompt_input_ids` plus their sinusoidal positions are appended to the description states
         as cross-attention keys (prompt_cross_states, reference :3099-3130), also after `encoder_outputs`; the decoder then has no
         prompt prefix (P = 0), and `cross_attentions` have S + P keys.  `prompt_hidden_states` raise ValueError in this mode.
+
+        num_return_sequences = N (an int >= 1; > 1 needs do_sample=True, as in transformers) draws N takes per description: every
+        per-utterance output has B * N rows, take n of description b at row b * N + n (`sequences`, `audio_codes`, `audios_length`,
+        `raw_ids`, the streamer's rows, the [B * N * K, V] `scores` / `logits` entries, the batch index of the decoder probes), and
+        it draws exactly what row b * N + n of the hand-expanded batch would (Philox substream (b * N + n) * K + k + row_base).  The
+        text encoder runs once per description (`encoder_attentions` / `encoder_hidden_states` stay B-sized) and the takes of a
+        description share one copy of its cross-attention K/V; a self-attention prompt prefix and a continuation's codes
+        (`decoder_input_ids` / `input_values`, encoded once) are repeated per take, as one group of K code rows per utterance.
         """
         import copy
         gc = copy.deepcopy(generation_config if generation_config is not None else self.generation_config)
@@ -1394,6 +1438,7 @@ class ParlerTTSForConditionalGeneration:
         if gc.num_beams != 1:
             raise ValueError("Got incompatible mode for generation, should be one of greedy or sampling. "
                              "Ensure that beam search is de-activated by setting `num_beams=1` and `num_beam_groups=1`.")
+        N = resolve_num_return_sequences(gc)
         if self.prompt_cross_attention and mk.get("prompt_hidden_states") is not None:
             # the reference would put these states in front of the decoder while counting its cache positions without them
             raise ValueError("a prompt_cross_attention model takes the transcript as `prompt_input_ids`, not `prompt_hidden_states`")
@@ -1451,6 +1496,15 @@ class ParlerTTSForConditionalGeneration:
             start = gc.decoder_start_token_id if gc.decoder_start_token_id is not None else d.bos_token_id
             dec_ids = prepare_decoder_input_ids(mk["decoder_input_ids"], B, K, d.vocab_size, start, self.device)
         n0 = 1 if dec_ids is None else dec_ids.shape[1]
+        # num_return_sequences: the output batch is B * N, take n of description b at row b * N + n.  The encoder ran (and the
+        # cross-attention K/V are projected) once per description; what is per row -- a self-attention prompt prefix, the code
+        # prefix of a continuation -- is expanded per take.
+        if N > 1:
+            if prompt_hidden is not None:
+                prompt_hidden = prompt_hidden.repeat_interleave(N, dim=0)
+                prompt_mask = None if prompt_mask is None else prompt_mask.repeat_interleave(N, dim=0)
+            if dec_ids is not None:
+                dec_ids = expand_takes(dec_ids, B, K, N)
 
         # generated length (:3458-3469): max_new_tokens wins over max_length (both count the n0 input columns)
         if gc.max_new_tokens is not None:
@@ -1466,30 +1520,33 @@ class ParlerTTSForConditionalGeneration:
         # output_scores / output_logits exist only in the dict return, as in transformers; without it nothing is recorded
         want_scores = bool(gc.return_dict_in_generate and gc.output_scores)
         want_logits = bool(gc.return_dict_in_generate and gc.output_logits)
-        outputs = StepOutputs(B * K, d.vocab_size, self.device, want_scores, want_logits) if (want_scores or want_logits) else None
+        BN = B * N
+        outputs = StepOutputs(BN * K, d.vocab_size, self.device, want_scores, want_logits) if (want_scores or want_logits) else None
         probes = None
         if want_attn or want_hidden:
-            probes = StepProbes(d.num_hidden_layers, B, d.num_attention_heads, S, d.hidden_size, P, n0, self.dtype, self.device,
+            probes = StepProbes(d.num_hidden_layers, BN, d.num_attention_heads, S, d.hidden_size, P, n0, self.dtype, self.device,
                                 want_attn, want_hidden)
         limit = self._fused_batch_limit()
-        if limit is not None and B > limit and not custom_loop and streamer is None:
-            # The fused decode-step kernels hold one 32-row tile: a larger batch runs as consecutive shards of <= 32 utterances through
-            # the same session.  The result is the one the whole batch would give: the Philox draw is keyed by the global row
-            # (row_base), the processors' state is per utterance, and a finished utterance emits pad ids until the longest one ends.
+        if limit is not None and BN > limit and not custom_loop and streamer is None:
+            # The fused decode-step kernels hold one 32-row tile: a larger batch runs as consecutive shards of <= 32 rows through the
+            # same session, each whole groups of takes (take_shards).  The result is the one the whole batch would give: the Philox
+            # draw is keyed by the global row (row_base), the processors' state is per utterance, and a finished utterance emits pad
+            # ids until the longest one ends.
             parts = []
-            for b0 in range(0, B, limit):
-                sl = slice(b0, min(B, b0 + limit))
-                parts.append(self._run_token_loop(enc_hidden[sl], None if attention_mask is None else attention_mask[sl],
-                                                  None if prompt_hidden is None else prompt_hidden[sl],
-                                                  None if prompt_mask is None else prompt_mask[sl], row_base=row_base + b0 * K,
-                                                  input_ids=None if dec_ids is None else dec_ids[sl.start * K:sl.stop * K],
-                                                  outputs=outputs, out_row=b0 * K, probes=probes, **run))
+            for d0, d1, r0, r1 in take_shards(B, N, limit):
+                rs = slice(r0, r1)
+                parts.append(self._run_token_loop(enc_hidden[d0:d1], None if attention_mask is None else attention_mask[d0:d1],
+                                                  None if prompt_hidden is None else prompt_hidden[rs],
+                                                  None if prompt_mask is None else prompt_mask[rs], row_base=row_base + r0 * K,
+                                                  input_ids=None if dec_ids is None else dec_ids[r0 * K:r1 * K],
+                                                  outputs=outputs, out_row=r0 * K, probes=probes, takes=(r1 - r0) // (d1 - d0), **run))
             n = max(t.shape[1] for t in parts)
             output_ids = torch.cat([torch.nn.functional.pad(t, (0, n - t.shape[1]), value=d.pad_token_id) for t in parts], dim=0)
         else:
             output_ids = self._run_token_loop(enc_hidden, attention_mask, prompt_hidden, prompt_mask, row_base=row_base, streamer=streamer,
                                               custom=(logits_processor or [], stopping_criteria or []) if custom_loop else None,
-                                              input_ids=dec_ids, outputs=outputs, probes=probes, **run)
+                                              input_ids=dec_ids, outputs=outputs, probes=probes, takes=N, **run)
+        B = BN   # from here on the batch is the B * N takes
 
         # apply the stashed delay mask, then keep only the free cells (:3586-3597); both masks come from the whole decoder input,
         # so a continuation's codes begin with its prefix frames
