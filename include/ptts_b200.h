@@ -356,6 +356,13 @@ int ptts_dac_workspace_bytes(const ptts_dac_config* cfg, int32_t B, int32_t T, i
  * audio [B, 1, hop*T] in cfg->dtype.  = quantizer.from_codes (:138) + model.decode (:139). */
 int ptts_dac_decode(const ptts_dac_config* cfg, const void* blob, void* workspace, int64_t workspace_bytes,
                     const int64_t* codes, int32_t B, int32_t T, void* audio_out, void* stream);
+/* Same, over a ragged batch: row b holds frame_lengths[b] frames (device int32 [B]; NULL = every row has T, which is
+ * ptts_dac_decode).  Row b of audio_out equals the decode of codes[b, :, :n_b] alone, bit for bit, in samples
+ * [0, hop*n_b) and is 0 in [hop*n_b, hop*T); codes at frames >= n_b are never read and may hold any value.  The
+ * kernels clamp each length to [0, T]; the caller validates them.  The workspace is ptts_dac_workspace_bytes(B, T). */
+int ptts_dac_decode2(const ptts_dac_config* cfg, const void* blob, void* workspace, int64_t workspace_bytes,
+                     const int64_t* codes, int32_t B, int32_t T, const int32_t* frame_lengths, void* audio_out,
+                     void* stream);
 
 /* ---- DAC encode ------------------------------------------------------------------------------ */
 /* The encoder weights (encoder convs and snake alphas, quantizer in_proj, unit-normalised codebooks) live in a second blob

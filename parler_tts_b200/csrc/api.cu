@@ -963,6 +963,13 @@ int ptts_dac_workspace_bytes(const ptts_dac_config* cfg, int32_t B, int32_t T, i
 
 int ptts_dac_decode(const ptts_dac_config* cfg, const void* blob, void* workspace, int64_t workspace_bytes, const int64_t* codes,
                     int32_t B, int32_t T, void* audio_out, void* stream) {
+  return ptts_dac_decode2(cfg, blob, workspace, workspace_bytes, codes, B, T, nullptr, audio_out, stream);
+}
+
+// frame_lengths (device, [B], or NULL): every kernel clamps each value to [0, T], reads no code at or past it and writes zeros
+// there (RowLengths in dac.h).  Each layer gets the time steps per code frame so far (Tlen / T) to place each row's end.
+int ptts_dac_decode2(const ptts_dac_config* cfg, const void* blob, void* workspace, int64_t workspace_bytes, const int64_t* codes,
+                     int32_t B, int32_t T, const int32_t* frame_lengths, void* audio_out, void* stream) {
   PTTS_REQUIRE(cfg && blob && workspace && codes && audio_out, "null argument");
   if (int e = validate_dac(*cfg)) return e;
   PTTS_REQUIRE(B > 0 && T > 0, "dac decode: empty input B=%d T=%d", B, T);
@@ -984,7 +991,8 @@ int ptts_dac_decode(const ptts_dac_config* cfg, const void* blob, void* workspac
     char* bufB = bufA + half;
     char* bufX = bufB + half;
     char* bufZ = bufX + half;
-    FromCodesArgs fz{codes, bl + L.codebooks, bl + L.proj_w, bl + L.proj_b, bufZ, K, cfg->codebook_dim, cfg->latent_dim, T, cfg->codebook_size};
+    FromCodesArgs fz{codes, bl + L.codebooks, bl + L.proj_w, bl + L.proj_b, bufZ, K, cfg->codebook_dim, cfg->latent_dim, T, cfg->codebook_size,
+                     frame_lengths};
     if (int e = launch_from_codes(fz, cfg->dtype, B, st)) return e;
     int ti = 3 * K;
     auto tpk = [&](int i) { return bl + L.t[i].off_k; };
@@ -995,7 +1003,7 @@ int ptts_dac_decode(const ptts_dac_config* cfg, const void* blob, void* workspac
       a.Cin = Cin; a.Cout = Cout; a.Tin = Tlen; a.Tout = Tlen; a.q_count = Tlen;
       a.n_taps = ks; a.off_base = -((ks - 1) / 2) * dil; a.off_step = dil; a.wt_base = 0; a.wt_step = 1;
       a.n_phase = 1; a.wt_phase_step = 0; a.o_mul = 1; a.o_add = 0; a.o_phase_step = 0;
-      return launch_conv_tc(a, tpk(w_i), ks, alpha_next, out_raw, out_act, B, st);
+      return launch_conv_tc(a, tpk(w_i), ks, alpha_next, out_raw, out_act, B, st, RowLengths{frame_lengths, T, Tlen / T, Tlen / T});
     };
     const int C = cfg->decoder_dim;
     char* act = bufA;   // snake'd input of the next conv
@@ -1013,7 +1021,7 @@ int ptts_dac_decode(const ptts_dac_config* cfg, const void* blob, void* workspac
       a.n_taps = 2; a.off_base = 0; a.off_step = -1; a.wt_base = 0; a.wt_step = sd;
       a.n_phase = sd; a.wt_phase_step = 1; a.o_mul = sd; a.o_add = -pad; a.o_phase_step = 1;
       // raw -> X (residual stream of the block), snake_{res1.snake1}(x) -> the other activation buffer
-      if (int e = launch_conv_tc(a, tpk(ti + 1), 2 * sd, tpp(ti + 3), bufX, oth2, B, st)) return e;
+      if (int e = launch_conv_tc(a, tpk(ti + 1), 2 * sd, tpp(ti + 3), bufX, oth2, B, st, RowLengths{frame_lengths, T, Tlen / T, Tlen / T * sd})) return e;
       ti += 3;
       std::swap(act, oth2);
       Tlen *= sd;
@@ -1028,15 +1036,16 @@ int ptts_dac_decode(const ptts_dac_config* cfg, const void* blob, void* workspac
     }
     const int cl = C >> cfg->n_blocks;
     if (final_conv_supported(cl))   // one thread per output sample (dac.cu)
-      return launch_final_conv_tanh(act, tpp(ti + 1), tpp(ti + 2), audio_out, cl, Tlen, B, st);
+      return launch_final_conv_tanh(act, tpp(ti + 1), tpp(ti + 2), audio_out, cl, Tlen, B, frame_lengths, T, st);
     ConvArgs f{};  // final conv (Cout = 1) + tanh on the already snake'd tensor: generic kernel
     f.x = act; f.w = tpp(ti + 1); f.bias = tpp(ti + 2); f.alpha = nullptr; f.res = nullptr; f.out = audio_out;
     f.Cin = cl; f.Cout = 1; f.Tin = Tlen; f.Tout = Tlen; f.q_count = Tlen;
     f.n_taps = 7; f.off_base = -3; f.off_step = 1; f.wt_base = 0; f.wt_step = 1;
     f.n_phase = 1; f.wt_phase_step = 0; f.o_mul = 1; f.o_add = 0; f.o_phase_step = 0; f.tanh_out = 1;
-    return launch_conv(f, cfg->dtype, B, st);
+    return launch_conv(f, cfg->dtype, B, st, RowLengths{frame_lengths, T, Tlen / T, Tlen / T});
   }
-  FromCodesArgs fc{codes, bl + L.codebooks, bl + L.proj_w, bl + L.proj_b, cur, K, cfg->codebook_dim, cfg->latent_dim, T, cfg->codebook_size};
+  FromCodesArgs fc{codes, bl + L.codebooks, bl + L.proj_w, bl + L.proj_b, cur, K, cfg->codebook_dim, cfg->latent_dim, T, cfg->codebook_size,
+                   frame_lengths};
   if (int e = launch_from_codes(fc, cfg->dtype, B, st)) return e;
   int ti = 3 * K;  // tensor cursor (see make_dac_layout order)
   auto tp = [&](int i) { return bl + L.t[i].off; };
@@ -1046,7 +1055,7 @@ int ptts_dac_decode(const ptts_dac_config* cfg, const void* blob, void* workspac
     a.Cin = Cin; a.Cout = Cout; a.Tin = Tlen; a.Tout = Tlen; a.q_count = Tlen;
     a.n_taps = ks; a.off_base = -((ks - 1) / 2) * dil; a.off_step = dil; a.wt_base = 0; a.wt_step = 1;
     a.n_phase = 1; a.wt_phase_step = 0; a.o_mul = 1; a.o_add = 0; a.o_phase_step = 0; a.tanh_out = tanh_out;
-    return launch_conv(a, cfg->dtype, B, st);
+    return launch_conv(a, cfg->dtype, B, st, RowLengths{frame_lengths, T, Tlen / T, Tlen / T});
   };
   const int C = cfg->decoder_dim;
   if (int e = conv(cur, ti, ti + 1, nullptr, nullptr, oth, cfg->latent_dim, C, T, 7, 1, 0)) return e;
@@ -1061,7 +1070,7 @@ int ptts_dac_decode(const ptts_dac_config* cfg, const void* blob, void* workspac
     a.Cin = cin; a.Cout = cout; a.Tin = Tlen; a.Tout = Tlen * sd; a.q_count = Tlen + 1;
     a.n_taps = 2; a.off_base = 0; a.off_step = -1; a.wt_base = 0; a.wt_step = sd;
     a.n_phase = sd; a.wt_phase_step = 1; a.o_mul = sd; a.o_add = -pad; a.o_phase_step = 1; a.tanh_out = 0;
-    if (int e = launch_conv(a, cfg->dtype, B, st)) return e;
+    if (int e = launch_conv(a, cfg->dtype, B, st, RowLengths{frame_lengths, T, Tlen / T, Tlen / T * sd})) return e;
     ti += 3;
     std::swap(cur, oth);
     Tlen *= sd;

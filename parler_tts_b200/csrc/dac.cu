@@ -26,7 +26,7 @@ __device__ __forceinline__ float snake_fn(float x, float alpha, float inv) {
 constexpr int CT_M = 64, CT_N = 64, CT_K = 16, CT_AROWS = 128, CT_MAXTAPS = 7;
 
 template <typename T>
-__global__ void __launch_bounds__(256) conv_kernel(ConvArgs p) {
+__global__ void __launch_bounds__(256) conv_kernel(ConvArgs p, RowLengths rl) {
   __shared__ float As[CT_K][CT_AROWS];
   __shared__ __align__(16) float Bs[CT_MAXTAPS][CT_K][CT_N];
   const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
@@ -36,6 +36,13 @@ __global__ void __launch_bounds__(256) conv_kernel(ConvArgs p) {
   // input row window of this tile: q0 + off_lo .. q0 + CT_M - 1 + off_hi
   const int off_last = p.off_base + (p.n_taps - 1) * p.off_step;
   const int off_lo = min(p.off_base, off_last);
+  // this row's lengths: a ragged decode loads its input as if the buffer ended at the row's end (the zero padding a standalone
+  // decode sees) and writes 0 past its output end; a tile wholly past the end skips the K loop
+  int t_in = p.Tin, t_out = p.Tout, q_end = p.q_count;
+  if (rl.frame_lengths != nullptr) {
+    const int n = row_frames(rl.frame_lengths, b, rl.frames);
+    t_in = n * rl.up_in; t_out = n * rl.up_out; q_end = p.q_count - p.Tin + t_in;
+  }
   const T* __restrict__ x = reinterpret_cast<const T*>(p.x) + (size_t)b * p.Tin * p.Cin;
   const T* __restrict__ w = reinterpret_cast<const T*>(p.w);
   const T* __restrict__ alpha = reinterpret_cast<const T*>(p.alpha);
@@ -47,14 +54,14 @@ __global__ void __launch_bounds__(256) conv_kernel(ConvArgs p) {
 #pragma unroll
     for (int j = 0; j < 4; j++) acc[i][j] = 0.f;
 
-  for (int ci0 = 0; ci0 < p.Cin; ci0 += CT_K) {
+  for (int ci0 = 0; q0 < q_end && ci0 < p.Cin; ci0 += CT_K) {
     __syncthreads();
     // A tile: (snake of) x[q0+off_lo+r][ci0+c], zero outside [0,Tin) -- conv zero padding
     for (int e = tid; e < arows * CT_K; e += 256) {
       const int r = e / CT_K, c = e - r * CT_K;
       const int t = q0 + off_lo + r, ci = ci0 + c;
       float v = 0.f;
-      if (t >= 0 && t < p.Tin && ci < p.Cin) {
+      if (t >= 0 && t < t_in && ci < p.Cin) {
         v = DT<T>::to_f(x[(size_t)t * p.Cin + ci]);
         if (alpha != nullptr) {
           const float a = DT<T>::to_f(alpha[ci]);
@@ -103,8 +110,9 @@ __global__ void __launch_bounds__(256) conv_kernel(ConvArgs p) {
     for (int j = 0; j < 4; j++) {
       const int co = co0 + tx * 4 + j;
       if (co >= p.Cout) continue;
-      float v = DT<T>::rnd(acc[i][j] + DT<T>::to_f(bias[co]));
       const size_t o = ((size_t)b * p.Tout + to) * p.Cout + co;
+      if (to >= t_out) { out[o] = DT<T>::from_f(0.f); continue; }
+      float v = DT<T>::rnd(acc[i][j] + DT<T>::to_f(bias[co]));
       if (res != nullptr) v = DT<T>::rnd(DT<T>::to_f(res[o]) + v);
       if (p.tanh_out) v = tanhf(v);
       out[o] = DT<T>::from_f(v);
@@ -112,12 +120,12 @@ __global__ void __launch_bounds__(256) conv_kernel(ConvArgs p) {
   }
 }
 
-int launch_conv(const ConvArgs& a, int dtype, int B, cudaStream_t st) {
+int launch_conv(const ConvArgs& a, int dtype, int B, cudaStream_t st, const RowLengths& rl) {
   PTTS_REQUIRE(a.n_taps >= 1 && a.n_taps <= CT_MAXTAPS, "conv: n_taps %d out of range", a.n_taps);
   PTTS_REQUIRE(CT_M + abs((a.n_taps - 1) * a.off_step) <= CT_AROWS, "conv: receptive field too wide");
   dim3 grid((a.q_count + CT_M - 1) / CT_M, (a.Cout + CT_N - 1) / CT_N, B * a.n_phase);
-  if (dtype == PTTS_BF16) conv_kernel<bf16><<<grid, 256, 0, st>>>(a);
-  else conv_kernel<float><<<grid, 256, 0, st>>>(a);
+  if (dtype == PTTS_BF16) conv_kernel<bf16><<<grid, 256, 0, st>>>(a, rl);
+  else conv_kernel<float><<<grid, 256, 0, st>>>(a, rl);
   PTTS_LAUNCH_CHECK();
   return PTTS_OK;
 }
@@ -129,6 +137,11 @@ __global__ void __launch_bounds__(256) from_codes_kernel(FromCodesArgs p) {
   __shared__ float e[32][16];  // [k][d] for this (b, t)
   const int t = blockIdx.x, b = blockIdx.y;
   const int K = p.K, D = p.D;
+  if (p.frame_lengths != nullptr && t >= row_frames(p.frame_lengths, b, p.T)) {   // past a ragged row's end: a zero latent
+    T* __restrict__ z = reinterpret_cast<T*>(p.z) + ((size_t)b * p.T + t) * p.C;
+    for (int c = threadIdx.x; c < p.C; c += blockDim.x) z[c] = DT<T>::from_f(0.f);
+    return;
+  }
   if (threadIdx.x < K * D) {
     const int k = threadIdx.x / D, d = threadIdx.x - k * D;
     const int64_t code = p.codes[((size_t)b * K + k) * p.T + t];
@@ -195,12 +208,20 @@ int pack_conv(const void* src, int src_dtype, void* dst, int dst_dtype, int d0, 
 // bf16 inputs, fp32 accumulation in tap-major / channel order, one rounding of acc + bias, tanh, one rounding (torch's ops).
 constexpr int FC_T = 128;   // outputs per block
 __global__ void __launch_bounds__(FC_T) final_conv_tanh_kernel(const bf16* __restrict__ x, const bf16* __restrict__ w, const bf16* __restrict__ bias,
-                                                               bf16* __restrict__ out, int C, int T) {
+                                                               bf16* __restrict__ out, int C, int T,
+                                                               const int32_t* __restrict__ frame_lengths, int frames) {
   extern __shared__ __align__(16) unsigned char fsm[];
   const int pitch = C + 8;                                   // elements
   bf16* xs = reinterpret_cast<bf16*>(fsm);                   // [FC_T + 6][pitch]
   float* ws = reinterpret_cast<float*>(fsm + (size_t)(FC_T + 6) * pitch * 2);   // [7][C]
   const int b = blockIdx.y, t0 = blockIdx.x * FC_T, tid = threadIdx.x;
+  // a ragged row's samples end at n_b * hop: later samples are 0 (not tanh(bias)); a block wholly past the end loads nothing.
+  // Inputs up to 3 rows past the end are read by kept samples: the zero band the last conv wrote there.
+  const int t_end = frame_lengths != nullptr ? row_frames(frame_lengths, b, frames) * (T / frames) : T;
+  if (t0 >= t_end) {
+    if (t0 + tid < T) out[(size_t)b * T + t0 + tid] = __float2bfloat16_rn(0.f);
+    return;
+  }
   const bf16* xb = x + (size_t)b * T * C;
   const int vec_per_row = C / 8;
   for (int e = tid; e < (FC_T + 6) * vec_per_row; e += FC_T) {
@@ -226,15 +247,17 @@ __global__ void __launch_bounds__(FC_T) final_conv_tanh_kernel(const bf16* __res
     }
   }
   const float y = DT<bf16>::rnd(acc + __bfloat162float(bias[0]));
-  out[(size_t)b * T + t] = __float2bfloat16_rn(tanhf(y));
+  out[(size_t)b * T + t] = __float2bfloat16_rn(t < t_end ? tanhf(y) : 0.f);
 }
 
 bool final_conv_supported(int C) { return C % 8 == 0 && C <= 512; }
-int launch_final_conv_tanh(const void* x, const void* w, const void* bias, void* out, int C, int T, int B, cudaStream_t st) {
+int launch_final_conv_tanh(const void* x, const void* w, const void* bias, void* out, int C, int T, int B, const int32_t* frame_lengths,
+                           int frames, cudaStream_t st) {
   const size_t smem = (size_t)(FC_T + 6) * (C + 8) * 2 + (size_t)7 * C * 4;
   static bool attr = false;
   if (!attr) { PTTS_CHECK_CUDA(cudaFuncSetAttribute(final_conv_tanh_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024)); attr = true; }
-  final_conv_tanh_kernel<<<dim3((T + FC_T - 1) / FC_T, B), FC_T, smem, st>>>((const bf16*)x, (const bf16*)w, (const bf16*)bias, (bf16*)out, C, T);
+  final_conv_tanh_kernel<<<dim3((T + FC_T - 1) / FC_T, B), FC_T, smem, st>>>((const bf16*)x, (const bf16*)w, (const bf16*)bias, (bf16*)out, C, T,
+                                                                                 frame_lengths, frames);
   PTTS_LAUNCH_CHECK();
   return PTTS_OK;
 }

@@ -16,23 +16,39 @@ struct ConvArgs {
   int n_phase, wt_phase_step, o_mul, o_add, o_phase_step;
   int tanh_out;
 };
-int launch_conv(const ConvArgs& a, int dtype, int B, cudaStream_t st);
+// Ragged decode: row b holds frame_lengths[b] code frames (clamped to [0, frames]) and ends at frame_lengths[b] * up_in on a
+// conv's input axis, * up_out on its output axis.  Outputs past a row's end are written as 0, so that the buffers hold the zero
+// padding a standalone decode of the row sees.  frame_lengths == nullptr: every row is full (equal lengths, and the encoder).
+struct RowLengths {
+  const int32_t* frame_lengths;
+  int frames, up_in, up_out;
+};
+int launch_conv(const ConvArgs& a, int dtype, int B, cudaStream_t st, const RowLengths& rl = RowLengths{});
+
+// code frames of row b of a ragged decode, clamped to [0, frames] so that no value can move a kernel outside its row
+__device__ __forceinline__ int row_frames(const int32_t* frame_lengths, int b, int frames) {
+  return min(max(__ldg(frame_lengths + b), 0), frames);
+}
 
 struct FromCodesArgs {
   const int64_t* codes;  // [B][K][T]
   const void* codebooks; const void* proj_w; const void* proj_b;  // [K][cs][D], [K][C][D], [K][C]
   void* z;               // [B][T][C]
   int K, D, C, T, codebook_size;
+  const int32_t* frame_lengths;  // [B] or nullptr: frames at or past row b's length are zero latents and read no code
 };
 int launch_from_codes(const FromCodesArgs& a, int dtype, int B, cudaStream_t st);
 int pack_conv(const void* src, int src_dtype, void* dst, int dst_dtype, int d0, int d1, int k, int transposed, cudaStream_t st);
 // tensor-core path (dac_tc.cu, wgmma)
 bool conv_tc_supported(int Cin, int Cout);
-int launch_conv_tc(const ConvArgs& a, const void* w_kmajor, int taps_total, const void* alpha_next, void* out_raw, void* out_act, int B, cudaStream_t st);
+int launch_conv_tc(const ConvArgs& a, const void* w_kmajor, int taps_total, const void* alpha_next, void* out_raw, void* out_act, int B, cudaStream_t st,
+                   const RowLengths& rl = RowLengths{});
 int pack_conv_kmajor(const void* src, int src_dtype, void* dst, int d0, int d1, int k, int transposed, cudaStream_t st);
 // output convolution (C -> 1, k = 7) + tanh on the already snake'd channels-last tensor, bf16 (dac.cu)
 bool final_conv_supported(int C);
-int launch_final_conv_tanh(const void* x, const void* w, const void* bias, void* out, int C, int T, int B, cudaStream_t st);
+// frame_lengths (nullptr: none) as in RowLengths, `frames` code frames of T / frames samples each: samples past a row's end are 0
+int launch_final_conv_tanh(const void* x, const void* w, const void* bias, void* out, int C, int T, int B, const int32_t* frame_lengths,
+                           int frames, cudaStream_t st);
 
 enum { DK_PLAIN = 0, DK_CONV = 1, DK_CONVT = 2 };
 struct DacTensor {

@@ -15,6 +15,7 @@
 //     for the NEXT layer, so every layer's A operand is a ready-to-MMA bf16 tensor (snake is x + sin^2(alpha x)/(alpha + 1e-9),
 //     rounded like torch's bf16 ops).
 // ConvTranspose1d(k = 2s, stride s) = s output phases x 2 taps (dac.cu explains the mapping).
+#include <algorithm>
 #include <mutex>
 #include <vector>
 
@@ -36,6 +37,8 @@ struct ConvTcArgs {
   bf16* out_raw;           // raw result or nullptr
   bf16* out_act;           // snake_{alpha_next}(result) for the next layer or nullptr
   const bf16* alpha_next;  // [Cout]
+  const int32_t* frame_lengths;  // ragged decode (RowLengths in dac.h); nullptr: every row is full
+  int frames, up_in, up_out;
 };
 
 template <int NT>
@@ -48,6 +51,16 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant_
   const int phase = blockIdx.z % p.n_phase, b = blockIdx.z / p.n_phase;
   const int q0 = blockIdx.x * TC_M, n0 = blockIdx.y * NT;
   const int k_chunks = (p.Cin + TC_K - 1) / TC_K;
+  // Ragged decode.  The TMA map zero-fills only past the whole buffer, so a row's zero padding is written instead: every output
+  // past the row's end is 0, in the tile that holds the end (q_end) and in the whole tile after it -- a band of more than TC_M
+  // positions, wider than any following conv's reach past the end (host-checked).  Tiles past the band exit at once, tiles
+  // wholly inside it skip the K loop: the work follows each row's frames, not B * T.
+  int n_iter = p.n_taps * k_chunks;
+  if (p.frame_lengths != nullptr) {
+    const int q_end = p.q_count - p.Tin + row_frames(p.frame_lengths, b, p.frames) * p.up_in;
+    if ((int)blockIdx.x > q_end / TC_M + 1) return;
+    if (q0 >= q_end) n_iter = 0;
+  }
 
   if (threadIdx.x == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(&map_x) : "memory");
@@ -72,8 +85,22 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant_
     wg::tma_load_3d(a_dst, &map_x, kc * TC_K, q0 + p.off_base + j * p.off_step, b, bar);
     wg::tma_load_3d(b_dst, &map_w, kc * TC_K, n0, p.wt_base + phase * p.wt_phase_step + j * p.wt_step, bar);
   };
-  wg::mainloop<NT>(pipe, p.n_taps * k_chunks, load, acc);
-  if ((threadIdx.x >> 5) == wg::PRODUCER_WARP) return;
+  wg::mainloop<NT>(pipe, n_iter, load, acc);
+  const int to_end = p.frame_lengths != nullptr ? row_frames(p.frame_lengths, b, p.frames) * p.up_out : p.Tout;
+  if ((threadIdx.x >> 5) == wg::PRODUCER_WARP) {
+    // the producer warp, idle now, writes this tile's rows past the row's end: raw 0 (conv(0) + bias is not) and snake(0) = 0
+    if (to_end < p.Tout) {
+      for (int e = threadIdx.x & 31; e < TC_M * (NT / 8); e += 32) {
+        const int q = q0 + e / (NT / 8), c = 8 * (e % (NT / 8));
+        const int to = q * p.o_mul + p.o_add + phase * p.o_phase_step;
+        if (q >= p.q_count || to < to_end || to >= p.Tout) continue;
+        const size_t o = ((size_t)b * p.Tout + to) * p.Cout + n0 + c;
+        if (p.out_raw != nullptr) *reinterpret_cast<uint4*>(p.out_raw + o) = make_uint4(0u, 0u, 0u, 0u);
+        if (p.out_act != nullptr) *reinterpret_cast<uint4*>(p.out_act + o) = make_uint4(0u, 0u, 0u, 0u);
+      }
+    }
+    return;
+  }
 
   // ===== epilogue: each register pair is two adjacent channels of one time row =====
   const __nv_bfloat162* bias2 = reinterpret_cast<const __nv_bfloat162*>(chan);
@@ -84,7 +111,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant_
   for (int h = 0; h < 2; h++) {
     const int q = qrow + wg::frag_row(2 * h);
     const int to = q * p.o_mul + p.o_add + phase * p.o_phase_step;
-    if (q >= p.q_count || to < 0 || to >= p.Tout) continue;
+    if (q >= p.q_count || to < 0 || to >= to_end) continue;   // to_end <= Tout; the producer warp writes the rows past it
     const size_t orow = ((size_t)b * p.Tout + to) * p.Cout + n0;
 #pragma unroll
     for (int j = 0; j < NT / 8; j++) {
@@ -175,13 +202,22 @@ static int launch_conv_tile(const CUtensorMap& mx, const CUtensorMap& mw, const 
 }
 
 // x: [B][Tin][Cin] bf16, w: [taps_total][Cout][Cin] bf16
-int launch_conv_tc(const ConvArgs& a, const void* w_kmajor, int taps_total, const void* alpha_next, void* out_raw, void* out_act, int B, cudaStream_t st) {
+int launch_conv_tc(const ConvArgs& a, const void* w_kmajor, int taps_total, const void* alpha_next, void* out_raw, void* out_act, int B, cudaStream_t st,
+                   const RowLengths& rl) {
   ConvTcArgs p{};
   p.Cin = a.Cin; p.Cout = a.Cout; p.Tin = a.Tin; p.Tout = a.Tout; p.q_count = a.q_count;
   p.n_taps = a.n_taps; p.off_base = a.off_base; p.off_step = a.off_step; p.wt_base = a.wt_base; p.wt_step = a.wt_step;
   p.n_phase = a.n_phase; p.wt_phase_step = a.wt_phase_step; p.o_mul = a.o_mul; p.o_add = a.o_add; p.o_phase_step = a.o_phase_step;
   const int n_tile = conv_tc_ntile(a.Cout);
   p.bias = (const bf16*)a.bias; p.res = (const bf16*)a.res; p.out_raw = (bf16*)out_raw; p.out_act = (bf16*)out_act; p.alpha_next = (const bf16*)alpha_next;
+  p.frame_lengths = rl.frame_lengths; p.frames = rl.frames; p.up_in = rl.up_in; p.up_out = rl.up_out;
+  if (rl.frame_lengths != nullptr) {
+    // a kept output reads this far past its row's end: the highest tap offset, plus the row the transposed conv's extra q reads.
+    // The producer of x wrote zeros over more than TC_M positions past the end.
+    const int reach = std::max(std::max(a.off_base, a.off_base + (a.n_taps - 1) * a.off_step), 0) + (a.q_count - a.Tin);
+    PTTS_REQUIRE(reach <= TC_M, "conv_tc: a ragged decode reads %d rows past a row's end, more than the %d-row zero band", reach, TC_M);
+    PTTS_REQUIRE(rl.frames > 0 && a.Tin == rl.frames * rl.up_in && a.Tout == rl.frames * rl.up_out, "conv_tc: ragged lengths do not match the shape");
+  }
   CUtensorMap mx, mw;
   if (int e = make_map(&mx, a.x, (uint64_t)a.Cin, (uint64_t)a.Tin, (uint64_t)B, TC_M)) return e;
   if (int e = make_map(&mw, w_kmajor, (uint64_t)a.Cin, (uint64_t)a.Cout, (uint64_t)taps_total, (uint32_t)n_tile)) return e;

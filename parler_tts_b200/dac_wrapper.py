@@ -2,7 +2,8 @@
 
 Mirrors parler_tts/dac_wrapper/modeling_dac.py:14-164:
   DACModel.encode(input_values, padding_mask=None, bandwidth=None, return_dict=None, n_quantizers=None, sample_rate=None) (:33-104)
-  DACModel.decode(audio_codes, audio_scales, padding_mask=None, return_dict=None)   (:106-142)
+  DACModel.decode(audio_codes, audio_scales, padding_mask=None, return_dict=None)   (:106-142), plus frame_lengths= for ragged
+  batches (one codec call for utterances of different lengths)
 Weights: either folded tensors under transformers-DacModel style keys (decoder.conv1.weight, encoder.block.0.res_unit1..., ...)
 or descript-audio-codec checkpoint keys with weight-norm parameters (weight_g / weight_v, or
 parametrizations.weight.original0/1), folded here as w = g * v / ||v|| (reference :148-157).  The encoder's weights go to a
@@ -11,6 +12,7 @@ blob of their own; a state dict without them (decode only) stays valid, and enco
 from __future__ import annotations
 import ctypes as C
 import math
+import numbers
 import re
 from dataclasses import dataclass
 
@@ -178,6 +180,24 @@ def _encoder_state_dict(sd: dict[str, torch.Tensor], n_blocks: int) -> dict[str,
     return out
 
 
+def _frame_lengths(frame_lengths, B: int, T: int) -> torch.Tensor:
+    """DACModel.decode's frame_lengths -> int32 [B] on the host; ValueError for a wrong shape, dtype or value outside [0, T]."""
+    if isinstance(frame_lengths, torch.Tensor):
+        if frame_lengths.is_floating_point() or frame_lengths.is_complex() or frame_lengths.dtype == torch.bool:
+            raise ValueError(f"frame_lengths must hold integers, got {frame_lengths.dtype}")
+        n = frame_lengths.detach().cpu()
+    else:
+        vals = list(frame_lengths)
+        if not all(isinstance(v, numbers.Integral) and not isinstance(v, bool) for v in vals):
+            raise ValueError(f"frame_lengths must hold integers, got {vals}")
+        n = torch.tensor([int(v) for v in vals], dtype=torch.int64)
+    if n.shape != (B,):
+        raise ValueError(f"frame_lengths must have shape [{B}] (one length per batch row), got {tuple(n.shape)}")
+    if bool(((n < 0) | (n > T)).any()):
+        raise ValueError(f"frame_lengths must lie in [0, {T}], got {n.tolist()}")
+    return n.to(torch.int32)
+
+
 class DACModel:
     config_class = DACConfig
     main_input_name = "input_values"
@@ -341,8 +361,13 @@ class DACModel:
         return codes, latents
 
     @torch.no_grad()
-    def decode(self, audio_codes, audio_scales=None, padding_mask=None, return_dict=None):
-        """audio_codes [1, B, K, T] int64 (CUDA) -> DACDecoderOutput(audio_values [B, 1, hop*T])."""
+    def decode(self, audio_codes, audio_scales=None, padding_mask=None, return_dict=None, frame_lengths=None):
+        """audio_codes [1, B, K, T] int64 (CUDA) -> DACDecoderOutput(audio_values [B, 1, hop*T]).
+
+        frame_lengths (ints or an integer tensor of shape [B], each in [0, T]) decodes a ragged batch in one call: row b equals
+        the decode of audio_codes[:, b:b+1, :, :frame_lengths[b]] alone, bit for bit, in samples [0, hop*frame_lengths[b]) and is
+        0 after them.  Codes at frames >= frame_lengths[b] are never read and may hold anything (EOS / pad ids included).
+        `padding_mask` is accepted and unused, as in the reference."""
         if not self.loaded:
             raise RuntimeError("DACModel has no weights loaded")
         if len(audio_codes) != 1:
@@ -354,7 +379,12 @@ class DACModel:
         B, K, T = codes.shape
         if T == 0 or B == 0:
             raise ValueError("audio_codes is empty")
-        if bool(((codes < 0) | (codes >= self.config.codebook_size)).any()):
+        lengths = None if frame_lengths is None else _frame_lengths(frame_lengths, B, T)
+        bad = (codes < 0) | (codes >= self.config.codebook_size)
+        if lengths is not None:
+            lengths = lengths.to(self.device)
+            bad &= torch.arange(T, device=self.device) < lengths[:, None, None]   # only frames inside each row are read
+        if bool(bad.any()):
             raise IndexError("audio code out of range for the codebook (the reference's embedding lookup raises too)")
         lib = _lib.lib()
         need = C.c_int64()
@@ -362,8 +392,8 @@ class DACModel:
         if self._ws is None or self._ws.numel() < need.value:
             self._ws = torch.empty(need.value, dtype=torch.uint8, device=self.device)
         audio = torch.empty(B, 1, T * self.hop_length, dtype=self.dtype, device=self.device)
-        _lib.check(lib.ptts_dac_decode(C.byref(self._c), _lib.ptr(self.blob), _lib.ptr(self._ws), self._ws.numel(),
-                                       _lib.ptr(codes), B, T, _lib.ptr(audio), _lib.stream_ptr()))
+        _lib.check(lib.ptts_dac_decode2(C.byref(self._c), _lib.ptr(self.blob), _lib.ptr(self._ws), self._ws.numel(),
+                                        _lib.ptr(codes), B, T, _lib.ptr(lengths), _lib.ptr(audio), _lib.stream_ptr()))
         if return_dict is False:
             return (audio,)
         return DACDecoderOutput(audio)

@@ -119,6 +119,35 @@ def take_shards(batch_size: int, takes: int, limit: Optional[int]) -> list[tuple
     return [(b, b + 1, b * takes + j0, b * takes + min(takes, j0 + limit)) for b in range(batch_size) for j0 in range(0, takes, limit)]
 
 
+def compact_valid_frames(codes: torch.Tensor, codebook_size: int) -> tuple[torch.Tensor, torch.Tensor]:
+    """codes [B, K, T] -> (codes with each row's valid frames moved to the front in order, valid count [B] int64).
+
+    A frame is valid when all K of its ids are < codebook_size: the frames the reference's per-sample branch keeps with its
+    boolean gather (:3631-3633).  Invalid frames can sit mid-row (untrained weights, quirk Q5), so this is a stable sort of
+    the frame order by validity; what lies past a row's count is left over and never decoded."""
+    valid = (codes < codebook_size).all(dim=1)                                       # [B, T]
+    order = torch.sort((~valid).to(torch.uint8), dim=1, stable=True).indices          # valid frames first, in order
+    packed = torch.gather(codes, 2, order[:, None, :].expand_as(codes))
+    return packed, valid.sum(dim=1)
+
+
+def codes_to_waveform(audio_encoder: DACModel, codes: torch.Tensor, codebook_size: int, dtype: torch.dtype):
+    """generate()'s codes -> waveform step for codes [B, K, T] that may hold ids >= codebook_size (EOS / pad after an
+    utterance's end): each row decodes its valid frames alone (:3615-3641), here in one ragged codec call.
+
+    Returns (audio [B, hop * max n_b] zero-padded after each row, lengths: hop * n_b, or 1 for a row without a valid frame).
+    A batch with no valid frame at all gives [B, 1] zeros in `dtype`, like the reference's pad_sequence of 1-sample rows."""
+    B = codes.shape[0]
+    packed, n = compact_valid_frames(codes, codebook_size)
+    n_host = n.tolist()
+    T = max(n_host, default=0)
+    if T == 0:
+        return torch.zeros(B, 1, device=codes.device, dtype=dtype), [1] * B
+    audio = audio_encoder.decode(audio_codes=packed[None, :, :, :T], audio_scales=[None] * B, frame_lengths=n_host).audio_values
+    hop = audio_encoder.hop_length
+    return audio.squeeze(1), [hop * v if v > 0 else 1 for v in n_host]
+
+
 def shift_tokens_right(input_ids: torch.Tensor, pad_token_id: int, decoder_start_token_id: int):
     """The reference's shift_tokens_right (:308-323): one position to the right along dim 1, decoder_start_token_id first, -100
     replaced by pad_token_id.  Host-side integer work: labels [B, T, K] -> the decoder input [B, T, K]."""
@@ -1568,18 +1597,8 @@ class ParlerTTSForConditionalGeneration:
             lengths = [vals.shape[1]] * B
             output_values = vals
         else:
-            outs = []
-            for b in range(B):
-                sample = audio_codes[:, b]
-                ok = (sample >= cs).sum(dim=(0, 1)) == 0
-                if int(ok.sum()) > 0:
-                    sample = sample[:, :, ok]
-                    a = self.audio_encoder.decode(audio_codes=sample[None, ...], audio_scales=[None]).audio_values
-                    outs.append(a.reshape(-1))
-                else:
-                    outs.append(torch.zeros(1, device=self.device, dtype=self.dtype))  # :3641
-            lengths = [o.shape[0] for o in outs]
-            output_values = torch.nn.utils.rnn.pad_sequence(outs, batch_first=True, padding_value=0)
+            # the reference's per-sample loop (:3620-3647) as one ragged codec call over each row's valid frames
+            output_values, lengths = codes_to_waveform(self.audio_encoder, codes, cs, self.dtype)
         if gc.return_dict_in_generate or return_codes:
             out = GenerateOutput(sequences=output_values, audios_length=lengths, audio_codes=codes, raw_ids=output_ids)
             if outputs is not None:   # one entry per generated column: column n0 + t was drawn from entry t
