@@ -87,6 +87,36 @@ typedef struct ptts_sampling_ext {
   float eta_cutoff;             /* [0, 1): remove p < min(eta, sqrt(eta) exp(-entropy)) (sampling only; 0 = off) */
 } ptts_sampling_ext;
 
+/* The remaining processors of transformers' _get_logits_processor (modeling_parler_tts.py:3540-3547), greedy and sampling.  On
+ * each step's fp32 row, with cur_len = the column being drawn (the history's length), they run in transformers' order:
+ *   SequenceBias, [NoRepeatNGram], [MinNewTokens], ForcedBOS, ForcedEOS, InfNanRemove, ExponentialDecayLengthPenalty, Suppress,
+ *   SuppressAtBegin, [ParlerTTSLogitsProcessor], [temperature .. eta], LogitNormalization.
+ * Every table is caller-owned device memory that must stay valid while the generation runs; a NULL table (or a negative id) is
+ * that stage off.  All off = every pointer NULL, both ids -1, both flags 0. */
+#define PTTS_SEQ_BIAS_MAX 64       /* multi-id sequences of sequence_bias */
+#define PTTS_SEQ_BIAS_MAX_LEN 16   /* ids per sequence */
+typedef struct ptts_logits_ext {
+  /* SequenceBiasLogitsProcessor: row[i] += (0 + bias1[i]) + the bias of every sequence in `seq` whose last id is i and whose
+   * other ids equal the last len-1 history ids, added in table order (sequences longer than cur_len are skipped) */
+  const float* bias1;           /* [V] the single-id biases (0 where none), or NULL */
+  const int32_t* seq;           /* [n_seq][1 + PTTS_SEQ_BIAS_MAX_LEN]: len, then the len ids (oldest first) */
+  const float* seq_bias;        /* [n_seq] */
+  int32_t n_seq;                /* [0, PTTS_SEQ_BIAS_MAX] */
+  int32_t forced_bos_token_id;  /* ForcedBOSTokenLogitsProcessor: at cur_len == 1, every id -inf but this one, which gets 0; -1 = off */
+  int32_t forced_eos_token_id;  /* ForcedEOSTokenLogitsProcessor: the same at cur_len == max_length - 1; -1 = off */
+  int32_t remove_invalid_values; /* InfNanRemoveLogitsProcessor: NaN -> 0, +-inf -> +-FLT_MAX; 0 = off */
+  /* ExponentialDecayLengthPenalty: at cur_len > decay_start (= start + n0), row[eos] += |row[eos]| * decay[cur_len], where the
+   * caller fills decay[c] = (float)(factor^(c - decay_start) - 1) in double precision; the other ids get + 0 */
+  const float* decay;           /* [max_length], or NULL */
+  int32_t decay_start;
+  const uint32_t* suppress;     /* SuppressTokensLogitsProcessor: bitmap of ids, [ceil(V / 32)] words, bit i % 32 of word i / 32 */
+  const uint32_t* begin_suppress; /* SuppressTokensAtBeginLogitsProcessor: bitmap, applied at cur_len == begin_index only */
+  int32_t begin_index;          /* n0, or 2 when n0 == 1 and forced_bos_token_id is set (_get_logits_processor) */
+  int32_t renormalize_logits;   /* LogitNormalization: the recorded scores are log_softmax of the final row; the token is drawn
+                                 * from the same distribution as without it (softmax(log_softmax(x)) = softmax(x)), and greedy's
+                                 * argmax is taken before the normalization; 0 = off */
+} ptts_logits_ext;
+
 /* Tensor ids for ptts_decoder_pack(). `index` = layer (per-layer tensors) or codebook (EMBED/LM_HEAD). */
 enum {
   PTTS_T_EMBED_TOKENS = 0, /* [vocab+1, H]  decoder.model.decoder.embed_tokens.N.weight (:1354) */
@@ -229,6 +259,14 @@ int ptts_decode_steps(ptts_session* s, int32_t n_steps, void* stream);
  * sampling phase followed by that sampler: one launch pair per token instead of the step kernel's many tokens per launch.
  * A row left with no candidate gets token 0 (the reference's torch.multinomial raises there). */
 int ptts_generate_set_sampling_ext(ptts_session* s, const ptts_sampling_ext* ext);
+
+/* The processors of ptts_logits_ext for the generation begun last (ptts_generate_begin* resets them to off; NULL = off).  The
+ * struct is copied; the tables it points to are read by every step.  PTTS_EINVAL for n_seq outside [0, PTTS_SEQ_BIAS_MAX], n_seq > 0
+ * with a NULL seq or seq_bias, a forced id outside [-1, vocab_size), decay_start < 0 or begin_index < 1.  The sequence table is not
+ * read on the host: the sampler skips a sequence whose len is outside [2, PTTS_SEQ_BIAS_MAX_LEN], and ids are only compared, so
+ * one outside [0, V) never matches (the Python shim rejects both first).  While any stage is active, ptts_sample and
+ * ptts_decode_steps take the split path of ptts_generate_set_sampling_ext. */
+int ptts_generate_set_logits_ext(ptts_session* s, const ptts_logits_ext* ext);
 
 /* generate()'s output_logits / output_scores for the generation begun last: the sampler records, for every step (step =
  * cur_len - n0, the column it draws minus the decoder input's columns) inside [first_step, first_step + n_steps), the raw f32

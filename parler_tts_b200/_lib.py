@@ -38,6 +38,16 @@ class SamplingExtC(C.Structure):
                 ("epsilon_cutoff", C.c_float), ("eta_cutoff", C.c_float)]
 
 
+class LogitsExtC(C.Structure):
+    _fields_ = [("bias1", C.c_void_p), ("seq", C.c_void_p), ("seq_bias", C.c_void_p), ("n_seq", C.c_int32),
+                ("forced_bos_token_id", C.c_int32), ("forced_eos_token_id", C.c_int32), ("remove_invalid_values", C.c_int32),
+                ("decay", C.c_void_p), ("decay_start", C.c_int32), ("suppress", C.c_void_p), ("begin_suppress", C.c_void_p),
+                ("begin_index", C.c_int32), ("renormalize_logits", C.c_int32)]
+
+
+SEQ_BIAS_MAX, SEQ_BIAS_MAX_LEN = 64, 16   # PTTS_SEQ_BIAS_MAX, PTTS_SEQ_BIAS_MAX_LEN
+
+
 class DacConfigC(C.Structure):
     _fields_ = [("n_codebooks", C.c_int32), ("codebook_size", C.c_int32), ("codebook_dim", C.c_int32),
                 ("latent_dim", C.c_int32), ("decoder_dim", C.c_int32), ("n_blocks", C.c_int32),
@@ -67,6 +77,7 @@ _SIGS = {
     "ptts_generate_begin": (C.c_int, [_VP, C.POINTER(GenParamsC), _VP]),
     "ptts_generate_begin_ids": (C.c_int, [_VP, C.POINTER(GenParamsC), _VP, _I32, _VP]),
     "ptts_generate_set_sampling_ext": (C.c_int, [_VP, C.POINTER(SamplingExtC)]),
+    "ptts_generate_set_logits_ext": (C.c_int, [_VP, C.POINTER(LogitsExtC)]),
     "ptts_generate_set_outputs": (C.c_int, [_VP, _VP, _VP, _I32, _I32, _I64]),
     "ptts_generate_set_probes": (C.c_int, [_VP, _VP, _VP, _VP, _I32, _I32, _I64, _I64, _I64, _I64]),
     "ptts_prefill": (C.c_int, [_VP, _VP, _VP, _VP, _VP, _VP]),

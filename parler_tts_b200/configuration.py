@@ -101,7 +101,9 @@ class GenerationConfig(_Record):
                  num_return_sequences=1, repetition_penalty=1.0, no_repeat_ngram_size=0, length_penalty=1.0, typical_p=1.0,
                  epsilon_cutoff=0.0, eta_cutoff=0.0, min_length=0, penalty_alpha=None, bad_words_ids=None, force_words_ids=None,
                  guidance_scale=None, min_p=None, output_scores=False, output_logits=False,
-                 output_attentions=False, output_hidden_states=False, **kwargs):
+                 output_attentions=False, output_hidden_states=False, sequence_bias=None, suppress_tokens=None,
+                 begin_suppress_tokens=None, exponential_decay_length_penalty=None, forced_bos_token_id=None,
+                 forced_eos_token_id=None, remove_invalid_values=False, renormalize_logits=False, **kwargs):
         self.max_length = max_length
         self.max_new_tokens = max_new_tokens
         self.min_new_tokens = min_new_tokens
@@ -123,6 +125,11 @@ class GenerationConfig(_Record):
         # sampling, the min_p / typical_p / epsilon_cutoff / eta_cutoff warpers with sampling
         self.no_repeat_ngram_size, self.min_length, self.min_p = no_repeat_ngram_size, min_length, min_p
         self.typical_p, self.epsilon_cutoff, self.eta_cutoff = typical_p, epsilon_cutoff, eta_cutoff
+        # the remaining processors of transformers' _get_logits_processor (modeling.resolve_logits_ext), greedy and sampling
+        self.sequence_bias, self.suppress_tokens, self.begin_suppress_tokens = sequence_bias, suppress_tokens, begin_suppress_tokens
+        self.exponential_decay_length_penalty = exponential_decay_length_penalty
+        self.forced_bos_token_id, self.forced_eos_token_id = forced_bos_token_id, forced_eos_token_id
+        self.remove_invalid_values, self.renormalize_logits = remove_invalid_values, renormalize_logits
         # knobs the device loop does not implement: kept so that generate() can REJECT a non-neutral value instead of
         # silently ignoring it (modeling.py::_NEUTRAL_GENERATION_KNOBS)
         self.num_beam_groups, self.num_return_sequences = num_beam_groups, num_return_sequences

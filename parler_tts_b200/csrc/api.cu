@@ -64,6 +64,7 @@ struct ptts_session {
   DecodePath path;
   StepParams sp;     // the step kernels' parameters (DECODE_STEP, DECODE_CLUSTER)
   ptts_sampling_ext ext;  // ptts_generate_set_sampling_ext; off after every ptts_generate_begin*
+  ptts_logits_ext lext;   // ptts_generate_set_logits_ext; off after every ptts_generate_begin*
   SampleOut out;          // ptts_generate_set_outputs; off (both pointers null) after every ptts_generate_begin*
   ProbeWindow probe;      // ptts_generate_set_probes; off (all pointers null) after every ptts_generate_begin*
   int64_t graph_launches; // kernels of one replay of the captured decode graph
@@ -75,6 +76,14 @@ static const ptts_sampling_ext* active_ext(const ptts_session* s) {
   const ptts_sampling_ext& x = s->ext;
   const bool warp = s->gen.do_sample && (x.min_p > 0.f || x.typical_p < 1.f || x.epsilon_cutoff > 0.f || x.eta_cutoff > 0.f);
   return (x.no_repeat_ngram_size > 0 || warp) ? &s->ext : nullptr;
+}
+// the ptts_logits_ext stages, or nullptr while none is set
+static const ptts_logits_ext* active_lext(const ptts_session* s) {
+  const ptts_logits_ext& x = s->lext;
+  const bool on = x.bias1 != nullptr || x.n_seq > 0 || x.forced_bos_token_id >= 0 || x.forced_eos_token_id >= 0 ||
+                  x.remove_invalid_values || x.decay != nullptr || x.suppress != nullptr || x.begin_suppress != nullptr ||
+                  x.renormalize_logits;
+  return on ? &s->lext : nullptr;
 }
 // the per-step outputs, or nullptr while none is set
 static const SampleOut* active_out(const ptts_session* s) {
@@ -88,11 +97,11 @@ static const ProbeWindow* active_probe(const ptts_session* s) {
 // the path decode steps take now: a probe window needs the per-layer kernels of the multi-kernel path
 static DecodePath decode_path(const ptts_session* s) { return active_probe(s) != nullptr ? DECODE_MULTI_KERNEL : s->path; }
 
-// the knobs of the EXT sampler, or nullptr for the plain one: the outputs are recorded by the EXT sampler, with every stage off
-// when none is active (it then computes what the plain sampler computes)
+// the knobs of the EXT sampler, or nullptr for the plain one: the outputs and the ptts_logits_ext stages run on the EXT sampler,
+// with every ptts_sampling_ext stage off when none is active (it then computes what the plain sampler computes)
 static const ptts_sampling_ext* sampler_ext(const ptts_session* s) {
   const ptts_sampling_ext* x = active_ext(s);
-  return (x == nullptr && active_out(s) != nullptr) ? &kExtOff : x;
+  return (x == nullptr && (active_out(s) != nullptr || active_lext(s) != nullptr)) ? &kExtOff : x;
 }
 
 extern "C" {
@@ -229,6 +238,7 @@ int ptts_session_create3(const ptts_decoder_config* cfg, const void* blob, void*
   s->W = make_workspace(*cfg, B, P, S, max_cache_len, max_input_len, takes);
   s->n0 = 1;
   s->ext = kExtOff;
+  s->lext = kLogitsExtOff;
   s->out = SampleOut{};
   s->probe = ProbeWindow{};
   s->graph_launches = 0;
@@ -353,6 +363,7 @@ int ptts_generate_begin_ids(ptts_session* s, const ptts_gen_params* gen, const i
   s->gen.input_len = n0;
   s->n0 = n0;
   s->ext = kExtOff;
+  s->lext = kLogitsExtOff;
   s->out = SampleOut{};
   if (active_probe(s) && s->exec) { cudaGraphExecDestroy(s->exec); s->exec = nullptr; s->graph_ready = false; }
   s->probe = ProbeWindow{};
@@ -378,6 +389,23 @@ int ptts_generate_set_sampling_ext(ptts_session* s, const ptts_sampling_ext* ext
   PTTS_REQUIRE(x.eta_cutoff >= 0.f && x.eta_cutoff < 1.f, "`eta_cutoff` has to be a float in [0, 1) (0 = off), got %f", x.eta_cutoff);
   s->ext = x;
   // the knobs are a by-value argument of the captured graph's sampler node: capture again
+  if (s->exec) { cudaGraphExecDestroy(s->exec); s->exec = nullptr; s->graph_ready = false; }
+  return PTTS_OK;
+}
+
+int ptts_generate_set_logits_ext(ptts_session* s, const ptts_logits_ext* ext) {
+  PTTS_REQUIRE(s, "null argument");
+  if (!s->begun) return fail(PTTS_ESTATE, "ptts_generate_set_logits_ext called before ptts_generate_begin");
+  const ptts_logits_ext x = ext ? *ext : kLogitsExtOff;
+  const int V = s->cfg.vocab_size;
+  PTTS_REQUIRE(x.n_seq >= 0 && x.n_seq <= PTTS_SEQ_BIAS_MAX, "`sequence_bias`: %d sequences of two or more ids, at most %d are supported", x.n_seq, PTTS_SEQ_BIAS_MAX);
+  PTTS_REQUIRE(x.n_seq == 0 || (x.seq != nullptr && x.seq_bias != nullptr), "`sequence_bias`: n_seq > 0 needs the seq and seq_bias tables");
+  PTTS_REQUIRE(x.forced_bos_token_id >= -1 && x.forced_bos_token_id < V, "`forced_bos_token_id` %d is outside the vocabulary [0, %d)", x.forced_bos_token_id, V);
+  PTTS_REQUIRE(x.forced_eos_token_id >= -1 && x.forced_eos_token_id < V, "`forced_eos_token_id` %d is outside the vocabulary [0, %d)", x.forced_eos_token_id, V);
+  PTTS_REQUIRE(x.decay == nullptr || x.decay_start >= 0, "`exponential_decay_length_penalty`: regulation start %d must be >= 0", x.decay_start);
+  PTTS_REQUIRE(x.begin_suppress == nullptr || x.begin_index >= 1, "`begin_suppress_tokens`: begin index %d must be >= 1", x.begin_index);
+  s->lext = x;
+  // the struct is a by-value argument of the captured graph's sampler node: capture again
   if (s->exec) { cudaGraphExecDestroy(s->exec); s->exec = nullptr; s->graph_ready = false; }
   return PTTS_OK;
 }
@@ -696,7 +724,7 @@ int ptts_sample(ptts_session* s, const int64_t* forced_tokens, void* stream) {
   PTTS_REQUIRE(s, "null argument");
   if (!s->prefilled) return fail(PTTS_ESTATE, "ptts_sample called before ptts_prefill");
   s->launches++;
-  return launch_sample(sample_args(s), forced_tokens, (cudaStream_t)stream, false, sampler_ext(s), active_out(s));
+  return launch_sample(sample_args(s), forced_tokens, (cudaStream_t)stream, false, sampler_ext(s), active_out(s), active_lext(s));
 }
 
 int ptts_decode_steps(ptts_session* s, int32_t n_steps, void* stream) {
@@ -705,6 +733,7 @@ int ptts_decode_steps(ptts_session* s, int32_t n_steps, void* stream) {
   cudaStream_t st = (cudaStream_t)stream;
   const ptts_sampling_ext* ext = sampler_ext(s);
   const SampleOut* out = active_out(s);
+  const ptts_logits_ext* lext = active_lext(s);
   const DecodePath path = decode_path(s);
   if (ext != nullptr && path != DECODE_MULTI_KERNEL) {
     // an EXT stage is active or the outputs are set: the step kernel stops at the logits and the EXT sampler follows, token by
@@ -714,7 +743,7 @@ int ptts_decode_steps(ptts_session* s, int32_t n_steps, void* stream) {
     for (int i = 0; i < n_steps; i++) {
       const int e = path == DECODE_CLUSTER ? launch_decode_step_cluster(p, st) : launch_decode_step(p, s->sm_count, st);
       if (e) return e;
-      if (int e2 = launch_sample(sample_args(s), nullptr, st, false, ext, out)) return e2;
+      if (int e2 = launch_sample(sample_args(s), nullptr, st, false, ext, out, lext)) return e2;
     }
     s->launches += 2 * (int64_t)n_steps;
     return PTTS_OK;
@@ -746,7 +775,7 @@ int ptts_decode_steps(ptts_session* s, int32_t n_steps, void* stream) {
     const int64_t before = s->launches;
     PTTS_CHECK_CUDA(cudaStreamBeginCapture(s->cap_stream, cudaStreamCaptureModeThreadLocal));
     int e = run_forward(s, s->cap_stream, false, nullptr, nullptr);
-    if (!e) { s->launches++; e = launch_sample(sample_args(s), nullptr, s->cap_stream, true, ext, out); }
+    if (!e) { s->launches++; e = launch_sample(sample_args(s), nullptr, s->cap_stream, true, ext, out, lext); }
     cudaGraph_t graph = nullptr;
     cudaError_t ce = cudaStreamEndCapture(s->cap_stream, &graph);
     s->graph_launches = s->launches - before;   // embed + 8 kernels per layer + heads + sample (+ the probe kernels)
@@ -805,8 +834,8 @@ int ptts_logits_processor(const int64_t* input_ids, int32_t BK, int32_t seq_len,
 int ptts_op_sample_phase(ptts_session* s, int32_t n_ctas, void* stream) {
   PTTS_REQUIRE(s, "null argument");
   if (!s->prefilled) return fail(PTTS_ESTATE, "ptts_op_sample_phase called before ptts_prefill");
-  PTTS_REQUIRE(sampler_ext(s) == nullptr, "op_sample_phase: the step kernels' sampling phase has no ptts_sampling_ext stages and "
-                                          "records no per-step outputs; switch them off first");
+  PTTS_REQUIRE(sampler_ext(s) == nullptr, "op_sample_phase: the step kernels' sampling phase has no ptts_sampling_ext or "
+                                          "ptts_logits_ext stages and records no per-step outputs; switch them off first");
   s->launches++;
   return launch_sample_phase(sample_args(s), n_ctas, (cudaStream_t)stream);
 }

@@ -111,8 +111,11 @@ struct SampleOut {
 };
 // ext != nullptr: the sampler with the ptts_sampling_ext stages (the caller passes it while one is active, or all off while out is
 // set); out != nullptr (needs ext): that sampler also records the raw logits and the processed scores of the steps in its window
+// lext: the ptts_logits_ext stages (needs ext; nullptr = all off)
 int launch_sample(const SampleArgs& a, const int64_t* forced, cudaStream_t st, bool pdl, const ptts_sampling_ext* ext = nullptr,
-                  const SampleOut* out = nullptr);
+                  const SampleOut* out = nullptr, const ptts_logits_ext* lext = nullptr);
+// every ptts_logits_ext stage off
+constexpr ptts_logits_ext kLogitsExtOff = {nullptr, nullptr, nullptr, 0, -1, -1, 0, nullptr, 0, nullptr, nullptr, 1, 0};
 // the fused step kernels' sampling phase over n_ctas CTAs (passes of up to three rows per CTA), as a kernel of its own; no EXT
 int launch_sample_phase(const SampleArgs& a, int n_ctas, cudaStream_t st);
 // ids == nullptr: the BOS column (n0 = 1); otherwise the BOS-led [B*K][n0] input the generation continues from

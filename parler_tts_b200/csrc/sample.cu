@@ -18,14 +18,14 @@ namespace ptts {
 
 template <int ITEMS, bool EXT>
 __device__ __forceinline__ void sample_kernel_body(const SampleArgs& p, const int64_t* __restrict__ forced, const ptts_sampling_ext& x,
-                                                   const SampleOut& o) {
+                                                   const SampleOut& o, const ptts_logits_ext& lx) {
   pdl_launch_dependents();
   pdl_wait();
   if (p.ctrl->active == 0) return;
   const int row = blockIdx.x;           // one CTA per (utterance, codebook) row
   const int cur_len = p.ctrl->cur_len;  // the new token becomes column `cur_len`
   const ptts_gen_params g = *p.gen;
-  sample_rows_cta<ITEMS, 1, EXT>(p, g, forced, row, 0, row + 1, cur_len, x, o);
+  sample_rows_cta<ITEMS, 1, EXT>(p, g, forced, row, 0, row + 1, cur_len, x, o, lx);
   // last block advances the control block
   __threadfence();
   __syncthreads();
@@ -46,19 +46,19 @@ __device__ __forceinline__ void sample_kernel_body(const SampleArgs& p, const in
 
 template <int ITEMS>
 __global__ void __launch_bounds__(SMP_THREADS) sample_kernel(SampleArgs p, const int64_t* __restrict__ forced) {
-  sample_kernel_body<ITEMS, false>(p, forced, ptts_sampling_ext{}, SampleOut{});
+  sample_kernel_body<ITEMS, false>(p, forced, ptts_sampling_ext{}, SampleOut{}, ptts_logits_ext{});
 }
 
-// the ptts_sampling_ext stages and the per-step outputs (sample_core.cuh, EXT = true); the knobs and the output window come by
-// value, so a captured graph holds them
+// the ptts_sampling_ext and ptts_logits_ext stages and the per-step outputs (sample_core.cuh, EXT = true); the knobs, the table
+// pointers and the output window come by value, so a captured graph holds them
 template <int ITEMS, bool EXT>
 __global__ void __launch_bounds__(SMP_THREADS) sample_kernel(SampleArgs p, const int64_t* __restrict__ forced, ptts_sampling_ext x,
-                                                             SampleOut o) {
-  sample_kernel_body<ITEMS, EXT>(p, forced, x, o);
+                                                             SampleOut o, ptts_logits_ext lx) {
+  sample_kernel_body<ITEMS, EXT>(p, forced, x, o, lx);
 }
 
 int launch_sample(const SampleArgs& a, const int64_t* forced, cudaStream_t st, bool pdl, const ptts_sampling_ext* ext,
-                  const SampleOut* out) {
+                  const SampleOut* out, const ptts_logits_ext* lext) {
   const int BK = a.B * a.K;
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = dim3(BK);
@@ -71,12 +71,13 @@ int launch_sample(const SampleArgs& a, const int64_t* forced, cudaStream_t st, b
   cfg.numAttrs = pdl ? 1 : 0;
   const int items = (a.V + SMP_THREADS - 1) / SMP_THREADS;
   PTTS_REQUIRE(items <= 9, "sample: vocab_size %d > 2304 not supported", a.V);
-  PTTS_REQUIRE(out == nullptr || ext != nullptr, "sample: the per-step outputs need the EXT sampler");
+  PTTS_REQUIRE((out == nullptr && lext == nullptr) || ext != nullptr, "sample: the per-step outputs and the ptts_logits_ext stages need the EXT sampler");
   if (ext != nullptr) {
     const SampleOut o = out ? *out : SampleOut{};
-    if (items <= 1) PTTS_CHECK_CUDA(cudaLaunchKernelEx(&cfg, sample_kernel<1, true>, a, forced, *ext, o));
-    else if (items <= 5) PTTS_CHECK_CUDA(cudaLaunchKernelEx(&cfg, sample_kernel<5, true>, a, forced, *ext, o));
-    else PTTS_CHECK_CUDA(cudaLaunchKernelEx(&cfg, sample_kernel<9, true>, a, forced, *ext, o));
+    const ptts_logits_ext lx = lext ? *lext : kLogitsExtOff;
+    if (items <= 1) PTTS_CHECK_CUDA(cudaLaunchKernelEx(&cfg, sample_kernel<1, true>, a, forced, *ext, o, lx));
+    else if (items <= 5) PTTS_CHECK_CUDA(cudaLaunchKernelEx(&cfg, sample_kernel<5, true>, a, forced, *ext, o, lx));
+    else PTTS_CHECK_CUDA(cudaLaunchKernelEx(&cfg, sample_kernel<9, true>, a, forced, *ext, o, lx));
     return PTTS_OK;
   }
   if (items <= 1) PTTS_CHECK_CUDA(cudaLaunchKernelEx(&cfg, sample_kernel<1>, a, forced));

@@ -1,5 +1,6 @@
 // sample_core.cuh -- one row of logits -> next token (shared by sample_kernel and the fused step kernel).
 #pragma once
+#include <cfloat>
 #include "common.cuh"
 #include "kernels.h"
 
@@ -52,16 +53,30 @@ __device__ __forceinline__ uint32_t (&smp_bans())[SMP_MAX_ROWS][SMP_BAN_WORDS] {
   __shared__ uint32_t ban[SMP_MAX_ROWS][SMP_BAN_WORDS];
   return ban;
 }
+// EXT: the sequence_bias sequences of each row whose prefix matches the history: the id they bias (-1: no match), and their biases
+struct SmpSeq {
+  int last[SMP_MAX_ROWS][PTTS_SEQ_BIAS_MAX];
+  float bias[PTTS_SEQ_BIAS_MAX];
+};
+__device__ __forceinline__ SmpSeq& smp_seq() {
+  __shared__ SmpSeq sq;
+  return sq;
+}
+__device__ __forceinline__ bool bitmap_has(const uint32_t* __restrict__ bits, int i) { return (__ldg(bits + (i >> 5)) >> (i & 31)) & 1u; }
 
 // EXT = true adds the ptts_sampling_ext stages (sample_kernel's second set of instantiations): the n-gram bans join the EOS masks,
 // and MinP, Typical, Epsilon and Eta run after top-p on the same arrays, each a fixed-order CTA reduction or a bitwise threshold
 // search, so draws stay bit-reproducible.  With every stage off it computes what EXT = false computes.  EXT = true also records
 // generate()'s per-step outputs when the step (cur_len - input_len) lies in o's window: the raw row as loaded, and the final
 // processed row where p.scores gets it.
+// EXT = true also runs the ptts_logits_ext stages (lx; the caller passes the off values of ptts_generate_set_logits_ext when none
+// is set, not a zeroed struct).  The masks among them (suppress, begin-suppress) join the single mask pass; while an additive,
+// forcing or InfNan stage acts on this step, the pass applies every stage per id in transformers' order instead (they do not
+// commute with the masks).  Additions and the decay product use __fadd_rn / __fmul_rn so that no FMA changes their rounding.
 template <int ITEMS, int R, bool EXT = false>
 __device__ __forceinline__ void sample_rows_cta(const SampleArgs& p, const ptts_gen_params& g, const int64_t* __restrict__ forced,
                                                 int row0, int stride, int n_rows, int cur_len, ptts_sampling_ext x = {},
-                                                SampleOut o = {}) {
+                                                SampleOut o = {}, ptts_logits_ext lx = {}) {
   static_assert(R >= 1 && R <= SMP_MAX_ROWS, "rows per pass");
   SmpScratch& sc = smp_scratch();   // one static buffer for every instantiation inlined into a kernel
   float (&s_f)[2][SMP_MAX_ROWS][SMP_WARPS] = sc.f;
@@ -178,12 +193,43 @@ __device__ __forceinline__ void sample_rows_cta(const SampleArgs& p, const ptts_
       __syncthreads();
     }
   }
+  // ptts_logits_ext: which stages act on this column
+  const bool seq_bias = EXT && (lx.bias1 != nullptr || lx.n_seq > 0);
+  const bool forced_bos = EXT && lx.forced_bos_token_id >= 0 && cur_len == 1;
+  const bool forced_eos = EXT && lx.forced_eos_token_id >= 0 && cur_len == g.max_length - 1;
+  const bool decay = EXT && lx.decay != nullptr && cur_len > lx.decay_start;
+  const bool begin_sup = EXT && lx.begin_suppress != nullptr && cur_len == lx.begin_index;
+  const bool chain = seq_bias || forced_bos || forced_eos || decay || (EXT && lx.remove_invalid_values);
+  if constexpr (EXT) {
+    if (lx.n_seq > 0) {  // one thread per (row, sequence): does the history end with the sequence's first len - 1 ids?
+      SmpSeq& sq = smp_seq();
+#pragma unroll
+      for (int r = 0; r < R; r++) {
+        for (int q = tid; q < lx.n_seq; q += SMP_THREADS) {
+          const int32_t* e = lx.seq + q * (1 + PTTS_SEQ_BIAS_MAX_LEN);
+          const int len = e[0];
+          int last = -1;
+          if (valid[r] && len >= 2 && len <= PTTS_SEQ_BIAS_MAX_LEN && len <= cur_len) {
+            const int64_t* h = p.raw_ids + (size_t)row[r] * p.raw_ld + cur_len - (len - 1);
+            bool match = true;
+            for (int t = 0; t < len - 1 && match; t++) match = h[t] == e[1 + t];
+            if (match) last = e[len];
+          }
+          sq.last[r][q] = last;
+          if (r == 0) sq.bias[q] = lx.seq_bias[q];
+        }
+      }
+      __syncthreads();
+    }
+  }
 #pragma unroll
   for (int r = 0; r < R; r++) {
     const int b = row[r] / p.K, k = row[r] - b * p.K;
     bool mask_eos = false;
     // MinNewTokensLength: prompt_length_to_skip = the decoder input's columns (the BOS column, or n0 when continuing)
     if (cur_len - (g.input_len > 1 ? g.input_len : 1) < g.min_new_tokens) mask_eos = true;
+    const bool mask_min = mask_eos;   // (EXT's ordered pass applies the two EOS masks at their own places)
+    bool mask_par = false;
     // ParlerTTSLogitsProcessor (stateful; state double-buffered on the column parity)
     if (valid[r]) {
       const int par = cur_len & 1;
@@ -194,20 +240,54 @@ __device__ __forceinline__ void sample_rows_cta(const SampleArgs& p, const ptts_
       const int es = __ldcg(p.eos_seen + fu);
       if (es > 0 && es <= cur_len && fu < b * p.K + p.K - 1) fu++;
       if (k == 0 && tid == 0) p.first_unf[(par ^ 1) * p.B + b] = fu;
-      if (row[r] > fu) mask_eos = true;
+      if (row[r] > fu) mask_eos = mask_par = true;
+    }
+    if (chain) {
+      // transformers' order: SequenceBias, NoRepeatNGram, MinNewTokens, ForcedBOS, ForcedEOS, InfNan, ExponentialDecay, Suppress,
+      // SuppressAtBegin, ParlerTTS (the custom list is merged last); suppress_special (a bench aid) goes with the last mask
+      const float mult = decay ? __ldg(lx.decay + cur_len) : 0.f;
+#pragma unroll
+      for (int j = 0; j < ITEMS; j++) {
+        const int i = tid + SMP_THREADS * j;
+        if (i >= p.V) continue;   // padding slots stay -inf (InfNan would lift them)
+        float y = v[r][j];
+        if (seq_bias) {   // bias = (0 + bias1[i]) + each matching sequence ending in i, in table order; then scores + bias
+          float bs = lx.bias1 != nullptr ? __fadd_rn(0.f, __ldg(lx.bias1 + i)) : 0.f;
+          for (int q = 0; q < lx.n_seq; q++)
+            if (smp_seq().last[r][q] == i) bs = __fadd_rn(bs, smp_seq().bias[q]);
+          y = __fadd_rn(y, bs);
+        }
+        if (bans && ((smp_bans()[r][i >> 5] >> (i & 31)) & 1u)) y = -INFINITY;
+        if (mask_min && i == p.eos) y = -INFINITY;
+        if (forced_bos) y = (i == lx.forced_bos_token_id) ? 0.f : -INFINITY;
+        if (forced_eos) y = (i == lx.forced_eos_token_id) ? 0.f : -INFINITY;
+        if (lx.remove_invalid_values) y = (y != y) ? 0.f : (y == INFINITY ? FLT_MAX : (y == -INFINITY ? -FLT_MAX : y));
+        if (decay) y = __fadd_rn(y, i == p.eos ? __fmul_rn(fabsf(y), mult) : 0.f);   // scores + penalties (0 off EOS)
+        if (lx.suppress != nullptr && bitmap_has(lx.suppress, i)) y = -INFINITY;
+        if (begin_sup && bitmap_has(lx.begin_suppress, i)) y = -INFINITY;
+        if (mask_par && i == p.eos) y = -INFINITY;
+        if (g.suppress_special && i >= g.codebook_size) y = -INFINITY;
+        v[r][j] = y;
+      }
+      continue;
     }
 #pragma unroll
     for (int j = 0; j < ITEMS; j++) {
       const int i = tid + SMP_THREADS * j;
       if (mask_eos && i == p.eos) v[r][j] = -INFINITY;
       if (g.suppress_special && i >= g.codebook_size) v[r][j] = -INFINITY;
-      if constexpr (EXT)
+      if constexpr (EXT) {
         if (bans && ((smp_bans()[r][i >> 5] >> (i & 31)) & 1u)) v[r][j] = -INFINITY;
+        if (i < p.V && lx.suppress != nullptr && bitmap_has(lx.suppress, i)) v[r][j] = -INFINITY;
+        if (i < p.V && begin_sup && bitmap_has(lx.begin_suppress, i)) v[r][j] = -INFINITY;
+      }
     }
   }
   int tok[R];
 #pragma unroll
   for (int r = 0; r < R; r++) tok[r] = 0;
+  const bool renorm = EXT && lx.renormalize_logits;
+  float n_max[R], n_log[R];  // LogitNormalization: the final row's max and log of its softmax sum
   if (g.do_sample) {
     if (g.temperature != 1.0f) {
 #pragma unroll
@@ -422,8 +502,11 @@ __device__ __forceinline__ void sample_rows_cta(const SampleArgs& p, const ptts_
     for (int r = 0; r < R; r++) tok[r] = found[r] >= 0 ? found[r] : last_nz[r];
     if constexpr (EXT) {  // every id removed (the bans can do that): token 0, as greedy's argmax gives
 #pragma unroll
-      for (int r = 0; r < R; r++)
+      for (int r = 0; r < R; r++) {
         if (tok[r] < 0) tok[r] = 0;
+        n_max[r] = m[r];          // the warpers never remove the max
+        n_log[r] = logf(s[r]);
+      }
     }
   } else {
     // argmax, smallest index on ties
@@ -458,6 +541,30 @@ __device__ __forceinline__ void sample_rows_cta(const SampleArgs& p, const ptts_
       tok[r] = mi;
     }
     buf ^= 1;
+    if (renorm) {  // greedy: the argmax above is taken before the normalization
+#pragma unroll
+      for (int r = 0; r < R; r++) {
+        n_max[r] = -INFINITY;
+#pragma unroll
+        for (int j = 0; j < ITEMS; j++) n_max[r] = fmaxf(n_max[r], v[r][j]);
+      }
+      cta_max_f(n_max);
+#pragma unroll
+      for (int r = 0; r < R; r++) {
+        n_log[r] = 0.f;
+#pragma unroll
+        for (int j = 0; j < ITEMS; j++) n_log[r] += expf(v[r][j] - n_max[r]);
+      }
+      cta_sum_f(n_log);
+#pragma unroll
+      for (int r = 0; r < R; r++) n_log[r] = logf(n_log[r]);
+    }
+  }
+  if (renorm) {  // log_softmax = (x - max) - log(sum exp(x - max))
+#pragma unroll
+    for (int r = 0; r < R; r++)
+#pragma unroll
+      for (int j = 0; j < ITEMS; j++) v[r][j] = (v[r][j] - n_max[r]) - n_log[r];
   }
 #pragma unroll
   for (int r = 0; r < R; r++) {

@@ -15,6 +15,7 @@ import math
 import os
 from typing import Any, Optional
 
+import numpy as np
 import torch
 
 from . import _lib
@@ -334,6 +335,197 @@ def sampling_ext_warpers(scores: torch.Tensor, ext: dict) -> torch.Tensor:
     return scores
 
 
+def _sequence_bias_dict(sb) -> dict:
+    """SequenceBiasLogitsProcessor's argument checks (dict {tuple(ids): float} or list [[ids], float]) -> the dict it uses."""
+    if not isinstance(sb, (dict, list)) or len(sb) == 0:
+        raise ValueError(f"`sequence_bias` has to be a non-empty dictionary, or non-empty list of lists but is {sb}.")
+    is_id = lambda t: isinstance(t, (int, np.integer)) and not isinstance(t, bool)
+    if isinstance(sb, dict):
+        if any(not isinstance(ids, tuple) for ids in sb):
+            raise ValueError(f"`sequence_bias` has to be a dict with tuples as keys, but is {sb}.")
+        if any(len(ids) == 0 or any(not is_id(t) or t < 0 for t in ids) for ids in sb):
+            raise ValueError(f"Each key in `sequence_bias` has to be a non-empty tuple of positive integers, but is {sb}.")
+        if any(not isinstance(b, float) for b in sb.values()):
+            raise ValueError(f"`sequence_bias` has to be a dict with floats as values, but is {sb}.")
+        return dict(sb)
+    ok = lambda e: (isinstance(e, list) and len(e) == 2 and isinstance(e[0], list) and all(is_id(t) and t > 0 for t in e[0])
+                    and isinstance(e[1], float))
+    if any(not ok(e) for e in sb):
+        raise ValueError(f"Each element in `sequence_bias` has to be a non-empty list of lists of positive integers and float, "
+                         f"but is {sb}.")
+    return {tuple(e[0]): e[1] for e in sb}
+
+
+def _token_id(v, name: str, V: int) -> int:
+    if isinstance(v, (list, tuple)) or (isinstance(v, torch.Tensor) and v.dim() > 0):
+        if len(v) != 1:
+            raise ValueError(f"`{name}` takes one id here, got {v}")
+        v = v[0]
+    if isinstance(v, torch.Tensor):
+        if torch.is_floating_point(v):
+            raise ValueError(f"`{name}` has to be a list of positive integers, but is {v}")
+        v = int(v)
+    if not isinstance(v, (int, np.integer)) or isinstance(v, bool) or v < 0:
+        raise ValueError(f"`{name}` has to be a list of positive integers, but is {v}")
+    if v >= V:
+        raise ValueError(f"`{name}` {v} is outside the vocabulary of size {V}")
+    return int(v)
+
+
+def _id_list(v, name: str) -> list[int]:
+    ids = list(v.tolist() if isinstance(v, torch.Tensor) else v)
+    if any(not isinstance(t, (int, np.integer)) or isinstance(t, bool) for t in ids):
+        raise ValueError(f"`{name}` has to be a list of integer ids, but is {v}")
+    return [int(t) for t in ids]
+
+
+class LogitsExt:
+    """The ptts_logits_ext processors of one generate() call (resolve_logits_ext): their values, the device tables built from
+    them once per call, and the same stages as torch ops for the host-driven loop.  In transformers' order: sequence_bias
+    (before the n-gram bans and MinNewTokens), then forced BOS, forced EOS, InfNan, exponential decay, suppress, begin-suppress
+    (before the Parler EOS processor), and LogitNormalization after the warpers."""
+
+    def __init__(self, V: int, eos: int, max_length: int):
+        self.V, self.eos, self.max_length = V, eos, max_length
+        self.bias1 = None                   # np.float32 [V], or None
+        self.seqs: list[tuple[tuple[int, ...], float]] = []   # the multi-id sequences in dict order (bias rounded to fp32)
+        self.forced_bos = self.forced_eos = -1
+        self.remove_invalid_values = self.renormalize_logits = False
+        self.decay = None                   # np.float32 [max_length]: decay[c] = fp32(factor^(c - decay_start) - 1)
+        self.decay_start = 0
+        self.suppress = self.begin_suppress = None   # sorted in-vocabulary ids, or None
+        self.begin_index = 1
+        self._dev = None
+
+    def active(self) -> bool:
+        return (self.bias1 is not None or bool(self.seqs) or self.forced_bos >= 0 or self.forced_eos >= 0 or self.remove_invalid_values
+                or self.decay is not None or self.suppress is not None or self.begin_suppress is not None or self.renormalize_logits)
+
+    def c_struct(self, device) -> "_lib.LogitsExtC":
+        """The C struct over device tables built once (they live as long as this object)."""
+        if self._dev is None:
+            W = (self.V + 31) // 32
+
+            def bitmap(ids):
+                if ids is None:
+                    return None
+                words = np.zeros(W, dtype=np.uint32)
+                for t in ids:
+                    words[t >> 5] |= np.uint32(1 << (t & 31))
+                return torch.from_numpy(words.view(np.int32)).to(device)
+            seq = np.zeros((max(1, len(self.seqs)), 1 + _lib.SEQ_BIAS_MAX_LEN), dtype=np.int32)
+            for q, (ids, _) in enumerate(self.seqs):
+                seq[q, 0] = len(ids)
+                seq[q, 1:1 + len(ids)] = ids
+            t = lambda a: None if a is None else torch.from_numpy(np.ascontiguousarray(a)).to(device)
+            self._dev = dict(bias1=t(self.bias1), seq=t(seq) if self.seqs else None,
+                             seq_bias=t(np.array([b for _, b in self.seqs], dtype=np.float32)) if self.seqs else None,
+                             decay=t(self.decay), suppress=bitmap(self.suppress), begin_suppress=bitmap(self.begin_suppress))
+        d = self._dev
+        return _lib.LogitsExtC(bias1=_lib.ptr(d["bias1"]), seq=_lib.ptr(d["seq"]), seq_bias=_lib.ptr(d["seq_bias"]),
+                               n_seq=len(self.seqs), forced_bos_token_id=self.forced_bos, forced_eos_token_id=self.forced_eos,
+                               remove_invalid_values=int(self.remove_invalid_values), decay=_lib.ptr(d["decay"]),
+                               decay_start=self.decay_start, suppress=_lib.ptr(d["suppress"]),
+                               begin_suppress=_lib.ptr(d["begin_suppress"]), begin_index=self.begin_index,
+                               renormalize_logits=int(self.renormalize_logits))
+
+    # -- the stages as torch ops (the host-driven loop); ids [R, cur_len] is the history, scores fp32 [R, V] --------------------
+    def sequence_bias(self, ids: torch.Tensor, scores: torch.Tensor) -> torch.Tensor:
+        if self.bias1 is None and not self.seqs:
+            return scores
+        bias = torch.zeros_like(scores)
+        if self.bias1 is not None:
+            bias += torch.from_numpy(self.bias1).to(scores.device)
+        for seq, b in self.seqs:
+            if len(seq) > ids.shape[1]:
+                continue
+            match = (ids[:, ids.shape[1] - len(seq) + 1:] == torch.tensor(seq[:-1], device=ids.device)).all(1)
+            bias[:, seq[-1]] += torch.where(match, torch.tensor(b, device=scores.device), torch.tensor(0.0, device=scores.device))
+        return scores + bias
+
+    def before_parler(self, ids: torch.Tensor, scores: torch.Tensor) -> torch.Tensor:
+        """forced BOS, forced EOS, InfNan, exponential decay, suppress, begin-suppress."""
+        cur, ninf = ids.shape[1], -float("inf")
+        for fid, col in ((self.forced_bos, 1), (self.forced_eos, self.max_length - 1)):
+            if fid >= 0 and cur == col:
+                scores = torch.full_like(scores, ninf)
+                scores[:, fid] = 0
+        if self.remove_invalid_values:
+            fmax = torch.finfo(scores.dtype).max
+            out = torch.where(scores != scores, 0.0, scores)
+            out = torch.where(scores == float("inf"), fmax, out)
+            scores = torch.where(scores == ninf, -fmax, out)
+        if self.decay is not None and cur > self.decay_start:
+            pen = torch.zeros_like(scores)
+            pen[:, self.eos] = scores[:, self.eos].abs() * float(self.decay[cur])
+            scores = scores + pen
+        for ids_, on in ((self.suppress, True), (self.begin_suppress, cur == self.begin_index)):
+            if ids_ is not None and on:
+                scores = scores.masked_fill(torch.isin(torch.arange(scores.shape[1], device=scores.device),
+                                                       torch.tensor(ids_, device=scores.device, dtype=torch.long)), ninf)
+        return scores
+
+    def normalize(self, scores: torch.Tensor) -> torch.Tensor:
+        return scores.log_softmax(-1) if self.renormalize_logits else scores
+
+
+def resolve_logits_ext(gc, n0: int, max_length: int, vocab_size: int, eos_token_id: int) -> Optional[LogitsExt]:
+    """sequence_bias, suppress_tokens, begin_suppress_tokens, exponential_decay_length_penalty, forced_bos_token_id,
+    forced_eos_token_id, remove_invalid_values and renormalize_logits from a GenerationConfig -> a LogitsExt, or None when none
+    is set.  Greedy and sampling alike, as transformers builds them.  Raises ValueError where transformers raises (sequence_bias's
+    format checks; a negative or float forced_eos_token_id), and up front for ids transformers only rejects when its processor
+    first runs (sequence_bias or forced ids >= vocab_size).  Beyond transformers: more than PTTS_SEQ_BIAS_MAX multi-id sequences,
+    one longer than PTTS_SEQ_BIAS_MAX_LEN, a forced_eos_token_id list of several ids, and a non-integer suppress id raise too.
+    Suppress ids outside the vocabulary are ignored, as torch.isin ignores them."""
+    V = int(vocab_size)
+    lx = LogitsExt(V, int(eos_token_id), int(max_length))
+    sb = getattr(gc, "sequence_bias", None)
+    if sb is not None:
+        sb = _sequence_bias_dict(sb)
+        bad = [t for ids in sb for t in ids if t >= V]
+        if bad:
+            raise ValueError(f"The model vocabulary size is {V}, but the following tokens were being biased: {bad}")
+        singles = {ids[0]: b for ids, b in sb.items() if len(ids) == 1}
+        if singles:
+            lx.bias1 = np.zeros(V, dtype=np.float32)
+            for t, b in singles.items():
+                lx.bias1[t] = np.float32(b)
+        lx.seqs = [(tuple(int(t) for t in ids), float(np.float32(b))) for ids, b in sb.items() if len(ids) > 1]
+        if len(lx.seqs) > _lib.SEQ_BIAS_MAX or any(len(s) > _lib.SEQ_BIAS_MAX_LEN for s, _ in lx.seqs):
+            raise ValueError(f"`sequence_bias`: at most {_lib.SEQ_BIAS_MAX} sequences of 2 .. {_lib.SEQ_BIAS_MAX_LEN} ids are "
+                             "supported by the device loop")
+    fb = getattr(gc, "forced_bos_token_id", None)
+    if fb is not None:
+        lx.forced_bos = _token_id(fb, "forced_bos_token_id", V)
+    fe = getattr(gc, "forced_eos_token_id", None)
+    if fe is not None:
+        lx.forced_eos = _token_id(fe, "forced_eos_token_id", V)
+    lx.remove_invalid_values = getattr(gc, "remove_invalid_values", False) is True
+    decay = getattr(gc, "exponential_decay_length_penalty", None)
+    if decay is not None:
+        if (not isinstance(decay, (tuple, list)) or len(decay) != 2 or not isinstance(decay[0], (int, np.integer))
+                or not isinstance(decay[1], (int, float, np.number))):
+            raise ValueError(f"`exponential_decay_length_penalty` has to be an (int start, float factor) pair, but is {decay}")
+        lx.decay_start = int(decay[0]) + int(n0)   # regulation_start
+        table = np.zeros(int(max_length), dtype=np.float32)
+        with np.errstate(over="ignore"):
+            for c in range(lx.decay_start + 1, int(max_length)):
+                try:
+                    table[c] = np.float32(pow(decay[1], c - lx.decay_start) - 1)   # Python's pow in double, rounded once
+                except OverflowError:
+                    table[c] = np.float32(np.inf)
+        lx.decay = table
+    for name in ("suppress_tokens", "begin_suppress_tokens"):
+        v = getattr(gc, name, None)
+        if v is not None:
+            ids = sorted({t for t in _id_list(v, name) if 0 <= t < V})
+            setattr(lx, "suppress" if name == "suppress_tokens" else "begin_suppress", ids if ids else None)
+    # begin_index: the first generated column, one later when a forced BOS takes column 1 (_get_logits_processor)
+    lx.begin_index = int(n0) + (1 if int(n0) == 1 and fb is not None else 0)
+    lx.renormalize_logits = getattr(gc, "renormalize_logits", False) is True
+    return lx if lx.active() else None
+
+
 class ParlerTTSLogitsProcessor:
     """Stateful EOS gating across codebooks; HF LogitsProcessor protocol (__call__(input_ids, scores))."""
 
@@ -568,10 +760,11 @@ class GenSession:
 
     def begin(self, max_length: int, do_sample=False, temperature=1.0, top_k=0, top_p=1.0, min_new_tokens=0, seed=0,
               suppress_special=False, codebook_size=1024, row_base=0, input_ids: Optional[torch.Tensor] = None,
-              ext: Optional[dict] = None):
+              ext: Optional[dict] = None, lext: Optional[LogitsExt] = None):
         """input_ids: None (the BOS column) or the BOS-led decoder input [B*K, n0] the generation continues from; the history
         then starts with its delayed form and the first sampled column is n0 (ptts_generate_begin_ids).
-        ext: None, or the ptts_sampling_ext values (resolve_sampling_ext) for this generation."""
+        ext: None, or the ptts_sampling_ext values (resolve_sampling_ext) for this generation.
+        lext: None, or the ptts_logits_ext processors (resolve_logits_ext); the session keeps it, and so its device tables, alive."""
         g = _lib.GenParamsC()
         g.max_length, g.min_new_tokens, g.do_sample = int(max_length), int(min_new_tokens or 0), int(bool(do_sample))
         g.top_k, g.top_p, g.temperature = int(top_k or 0), float(1.0 if top_p is None else top_p), float(temperature or 1.0)
@@ -588,6 +781,9 @@ class GenSession:
             _lib.check(_lib.lib().ptts_generate_begin_ids(self.h, C.byref(g), _lib.ptr(ids), self.n0, _lib.stream_ptr()))
         if ext is not None:
             _lib.check(_lib.lib().ptts_generate_set_sampling_ext(self.h, C.byref(_lib.SamplingExtC(**ext))))
+        self._lext = lext
+        if lext is not None:
+            _lib.check(_lib.lib().ptts_generate_set_logits_ext(self.h, C.byref(lext.c_struct(self.eng.device))))
         self._outputs = None   # the begin calls switch the per-step outputs off
         self.max_length = int(max_length)
 
@@ -1129,14 +1325,16 @@ class ParlerTTSForConditionalGeneration:
 
     # -- generate with user-supplied processors / stopping criteria --------------------------------
     def _host_driven_loop(self, sess: "GenSession", gc, max_length, user_processors, user_criteria, streamer, seed, stream_col, ext,
-                          min_new_tokens, outputs=None, out_row=0, probe_window=None):
+                          min_new_tokens, outputs=None, out_row=0, probe_window=None, lext=None):
         """One host iteration per token, like GenerationMixin._sample: the decoder step still runs on the fused kernel
         (ptts_decode_forward), the built-in processors run as their device operators (MinNewTokens as a mask,
         ParlerTTSLogitsProcessor = ptts_logits_processor), then the caller's `logits_processor` list, the HF warpers and the draw
         as torch ops on the device scores, and the token is appended with ptts_sample(forced).  Used only when the caller passes
         processors or criteria the device loop does not know (the reference merges such lists at :3540-3552).  `ext`
         (resolve_sampling_ext) adds the n-gram bans before the EOS masks and the MinP / Typical / Epsilon / Eta warpers after
-        top-p, in transformers' order.  `outputs` (StepOutputs) records each step's raw logits and final scores before the draw;
+        top-p, in transformers' order; `lext` (resolve_logits_ext) adds sequence_bias first, forced BOS / EOS, InfNan, the decay
+        and the suppress lists before the Parler EOS processor, and LogitNormalization last (greedy's argmax and the draw use the
+        scores before it, as the device loop does).  `outputs` (StepOutputs) records each step's raw logits and final scores before the draw;
         `probe_window(step)` (StepProbes) points the decoder's attention / hidden-state outputs at the next step's slot."""
         d = self.config.decoder
         K, BK = d.num_codebooks, sess.B * d.num_codebooks
@@ -1147,10 +1345,14 @@ class ParlerTTSForConditionalGeneration:
         while True:
             ids = sess.raw_ids[:, :cur]
             scores = sess.logits.clone()
+            if lext is not None:
+                scores = lext.sequence_bias(ids, scores)
             if ext is not None:
                 scores = no_repeat_ngram_mask(ids, scores, ext["no_repeat_ngram_size"])
             if min_new_tokens > 0 and cur - sess.n0 < min_new_tokens:
                 scores[:, d.eos_token_id] = -float("inf")
+            if lext is not None:
+                scores = lext.before_parler(ids, scores).contiguous()
             scores = parler(ids, scores)
             for proc in user_processors:
                 scores = proc(ids, scores)
@@ -1167,8 +1369,9 @@ class ParlerTTSForConditionalGeneration:
                     scores = scores.masked_fill(rem.scatter(1, si, rem), -float("inf"))
                 if ext is not None:
                     scores = sampling_ext_warpers(scores, ext)
+            final = scores if lext is None else lext.normalize(scores)   # what transformers' _sample records and passes on
             if outputs is not None:
-                outputs.put(cur - sess.n0, out_row, sess.logits, scores)
+                outputs.put(cur - sess.n0, out_row, sess.logits, final)
             if gc.do_sample:
                 nxt = torch.multinomial(scores.softmax(-1), 1, generator=gen).squeeze(1)
             else:
@@ -1181,7 +1384,7 @@ class ParlerTTSForConditionalGeneration:
             unfinished = unfinished & ~((nxt == d.eos_token_id) | (cur >= max_length)).long()
             stop = unfinished.max().item() == 0
             for crit in user_criteria:
-                r = crit(sess.raw_ids[:, :cur], scores)
+                r = crit(sess.raw_ids[:, :cur], final)
                 r = r if isinstance(r, torch.Tensor) else torch.full((BK,), bool(r), device=self.device)
                 unfinished = unfinished & ~r.long()
                 stop = stop or unfinished.max().item() == 0
@@ -1200,7 +1403,7 @@ class ParlerTTSForConditionalGeneration:
         return 32
 
     def _run_token_loop(self, enc_hidden, attention_mask, prompt_hidden, prompt_mask, *, gc, max_length, seed, suppress_special, row_base,
-                        ext, min_new_tokens, streamer=None, custom=None, input_ids=None, outputs=None, out_row=0, probes=None, takes=1):
+                        ext, min_new_tokens, lext=None, streamer=None, custom=None, input_ids=None, outputs=None, out_row=0, probes=None, takes=1):
         """begin + prefill + the token loop of one session; returns the raw token matrix [B * K, generated length].
         takes: the session's B rows are `takes` consecutive takes of each of the enc_hidden.shape[0] descriptions (B / takes);
         prompt_hidden, prompt_mask and input_ids have B rows.
@@ -1219,7 +1422,8 @@ class ParlerTTSForConditionalGeneration:
         sess.begin(max_length, do_sample=gc.do_sample, temperature=gc.temperature, top_k=gc.top_k if gc.do_sample else 0,
                    top_p=gc.top_p, min_new_tokens=min_new_tokens, seed=seed, suppress_special=suppress_special,
                    codebook_size=self.config.audio_encoder.codebook_size, row_base=row_base, input_ids=input_ids,
-                   ext=None if custom is not None else ext)   # the host-driven loop applies them as torch ops
+                   ext=None if custom is not None else ext,    # the host-driven loop applies them as torch ops
+                   lext=None if custom is not None else lext)
         stream_col = lambda col, v: v
         if streamer is not None:
             if input_ids is None:
@@ -1244,7 +1448,7 @@ class ParlerTTSForConditionalGeneration:
                     probe_window(step)
             if custom is not None:
                 self._host_driven_loop(sess, gc, max_length, custom[0], custom[1], streamer, seed, stream_col, ext, min_new_tokens,
-                                       outputs, out_row, probe_window)
+                                       outputs, out_row, probe_window, lext)
             elif streamer is not None:
                 window(0)
                 sess.sample()
@@ -1463,7 +1667,9 @@ class ParlerTTSForConditionalGeneration:
         if unsupported:
             raise ValueError(f"generation options {unsupported} are not supported by the device loop (greedy / sampling with "
                              "temperature, top_k, top_p, min_p, typical_p, epsilon_cutoff, eta_cutoff, no_repeat_ngram_size, "
-                             "min_length and min_new_tokens only)")
+                             "min_length, min_new_tokens, sequence_bias, suppress_tokens, begin_suppress_tokens, "
+                             "exponential_decay_length_penalty, forced_bos_token_id, forced_eos_token_id, remove_invalid_values and "
+                             "renormalize_logits only)")
         if gc.num_beams != 1:
             raise ValueError("Got incompatible mode for generation, should be one of greedy or sampling. "
                              "Ensure that beam search is de-activated by setting `num_beams=1` and `num_beam_groups=1`.")
@@ -1545,7 +1751,9 @@ class ParlerTTSForConditionalGeneration:
         if dec_ids is not None:
             check_continuation_length(n0, P, max_length, d.max_position_embeddings)
         ext, min_new_tokens = resolve_sampling_ext(gc, n0)
-        run = dict(gc=gc, max_length=max_length, seed=seed, suppress_special=suppress_special, ext=ext, min_new_tokens=min_new_tokens)
+        lext = resolve_logits_ext(gc, n0, max_length, d.vocab_size, d.eos_token_id)   # its device tables serve every shard
+        run = dict(gc=gc, max_length=max_length, seed=seed, suppress_special=suppress_special, ext=ext, min_new_tokens=min_new_tokens,
+                   lext=lext)
         # output_scores / output_logits exist only in the dict return, as in transformers; without it nothing is recorded
         want_scores = bool(gc.return_dict_in_generate and gc.output_scores)
         want_logits = bool(gc.return_dict_in_generate and gc.output_logits)
