@@ -300,6 +300,28 @@ int ptts_generate_set_outputs(ptts_session* s, float* logits, float* scores, int
 int ptts_generate_set_probes(ptts_session* s, void* self_attn, void* cross_attn, void* hidden, int32_t first_step, int32_t n_steps,
                              int64_t self_ld, int64_t self_step, int64_t cross_step, int64_t hidden_step);
 
+/* return_token_timestamps: each decode step writes the transcript alignment of its query into a caller-owned fp32 buffer.  The
+ * step whose input is column c (its query; the prefill writes nothing) writes row r = c - n0 when r lies in [first_step,
+ * first_step + n_steps), at out + ((r - first_step) * B + b) * key_len floats: the mean over the n_heads listed heads (heads:
+ * device int32 [n_heads][2] = (layer, head)) of each head's attention weights over keys [key0, key0 + key_len), renormalized
+ * over those keys (a key whose mask is 0 gets weight 0).  The keys are the self-attention prompt prefix of a session with P > 0,
+ * else its cross-attention keys.  Scores follow ptts_generate_set_probes' eager definition from the same q and K; the kernel
+ * reads only the key_len transcript keys of each listed head.  out NULL = off, which ptts_generate_begin* restores; while set,
+ * decode steps run the multi-kernel path as with probes.  The head list is copied to the host once here (a synchronous copy).
+ * PTTS_EINVAL for an empty list, a head outside the model or listed twice, keys outside the session or a negative window. */
+int ptts_generate_set_alignment(ptts_session* s, const int32_t* heads, int32_t n_heads, int32_t key0, int32_t key_len, float* out,
+                                int32_t first_step, int32_t n_steps);
+
+/* Token timestamps from alignments [B][T][P] fp32 (openai-whisper's recipe as transformers' generation_whisper states it): per
+ * utterance b, the median of width 7 along its first n_frames[b] frames (reflect padding; <= 3 frames are left as they are)
+ * into filtered [B][T][P], then the DTW of -filtered over those frames and the keys with key_mask[b][p] != 0 (masked keys are
+ * removed, not given a cost; key_mask NULL = none masked), with _dynamic_time_warping's recurrence, fp32 sums and tie order
+ * (diagonal, then previous key, then previous frame).  jumps [B][P] int32: the first frame of each key on the path, -1 for a
+ * masked key, 0 for every key of an utterance without frames.  n_frames and key_mask are device int32 arrays; trace is
+ * B * (P + 1) * (T + 1) bytes of device scratch.  Rows of filtered past n_frames[b] are not written. */
+int ptts_align_dtw(const float* alignment, int32_t B, int32_t T, int32_t P, const int32_t* n_frames, const int32_t* key_mask,
+                   float* filtered, uint8_t* trace, int32_t* jumps, void* stream);
+
 /* Device pointers into the workspace (valid for the session lifetime). */
 int ptts_session_logits(ptts_session* s, float** out);          /* [B*K, V] f32, last step's raw logits */
 int ptts_session_scores(ptts_session* s, float** out);          /* [B*K, V] f32, processed scores      */

@@ -80,6 +80,8 @@ _SIGS = {
     "ptts_generate_set_logits_ext": (C.c_int, [_VP, C.POINTER(LogitsExtC)]),
     "ptts_generate_set_outputs": (C.c_int, [_VP, _VP, _VP, _I32, _I32, _I64]),
     "ptts_generate_set_probes": (C.c_int, [_VP, _VP, _VP, _VP, _I32, _I32, _I64, _I64, _I64, _I64]),
+    "ptts_generate_set_alignment": (C.c_int, [_VP, _VP, _I32, _I32, _I32, _VP, _I32, _I32]),
+    "ptts_align_dtw": (C.c_int, [_VP, _I32, _I32, _I32, _VP, _VP, _VP, _VP, _VP, _VP]),
     "ptts_prefill": (C.c_int, [_VP, _VP, _VP, _VP, _VP, _VP]),
     "ptts_lm_heads_rowmajor_bytes": (C.c_int, [C.POINTER(DecoderConfigC), C.POINTER(_I64)]),
     "ptts_lm_heads_rowmajor_pack": (C.c_int, [C.POINTER(DecoderConfigC), _VP, _VP, _VP]),

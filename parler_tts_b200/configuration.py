@@ -103,7 +103,8 @@ class GenerationConfig(_Record):
                  guidance_scale=None, min_p=None, output_scores=False, output_logits=False,
                  output_attentions=False, output_hidden_states=False, sequence_bias=None, suppress_tokens=None,
                  begin_suppress_tokens=None, exponential_decay_length_penalty=None, forced_bos_token_id=None,
-                 forced_eos_token_id=None, remove_invalid_values=False, renormalize_logits=False, **kwargs):
+                 forced_eos_token_id=None, remove_invalid_values=False, renormalize_logits=False, return_token_timestamps=False,
+                 alignment_heads=None, **kwargs):
         self.max_length = max_length
         self.max_new_tokens = max_new_tokens
         self.min_new_tokens = min_new_tokens
@@ -130,6 +131,10 @@ class GenerationConfig(_Record):
         self.exponential_decay_length_penalty = exponential_decay_length_penalty
         self.forced_bos_token_id, self.forced_eos_token_id = forced_bos_token_id, forced_eos_token_id
         self.remove_invalid_values, self.renormalize_logits = remove_invalid_values, renormalize_logits
+        # with return_dict_in_generate: per generated column, the transcript alignment of the alignment heads ([layer, head]
+        # pairs; None = every head of the last ceil(L / 2) decoder layers) and each transcript token's start time
+        # (modeling.resolve_alignment_heads, modeling.align_dtw)
+        self.return_token_timestamps, self.alignment_heads = return_token_timestamps, alignment_heads
         # knobs the device loop does not implement: kept so that generate() can REJECT a non-neutral value instead of
         # silently ignoring it (modeling.py::_NEUTRAL_GENERATION_KNOBS)
         self.num_beam_groups, self.num_return_sequences = num_beam_groups, num_return_sequences

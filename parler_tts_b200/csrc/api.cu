@@ -4,6 +4,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <new>
+#include <vector>
 
 #include "common.cuh"
 #include "dac.h"
@@ -46,6 +47,15 @@ struct ProbeWindow {
   int64_t self_ld, self_step, cross_step, hidden_step;
 };
 
+// ptts_generate_set_alignment: rows [first_row, first_row + n_rows) of out [n_rows][B][key_len] fp32
+struct AlignWindow {
+  const int32_t* heads; int n_heads;   // device [n_heads][2] (layer, head)
+  std::vector<int> layer_heads;        // entries per layer (host copy of the list's layers)
+  int key0, key_len;
+  float* out;
+  int first_row, n_rows;
+};
+
 struct ptts_session {
   ptts_decoder_config cfg;
   DecoderLayout L;
@@ -67,6 +77,7 @@ struct ptts_session {
   ptts_logits_ext lext;   // ptts_generate_set_logits_ext; off after every ptts_generate_begin*
   SampleOut out;          // ptts_generate_set_outputs; off (both pointers null) after every ptts_generate_begin*
   ProbeWindow probe;      // ptts_generate_set_probes; off (all pointers null) after every ptts_generate_begin*
+  AlignWindow align;      // ptts_generate_set_alignment; off (out null) after every ptts_generate_begin*
   int64_t graph_launches; // kernels of one replay of the captured decode graph
 };
 
@@ -94,8 +105,12 @@ static const ProbeWindow* active_probe(const ptts_session* s) {
   const ProbeWindow& w = s->probe;
   return (w.self_attn != nullptr || w.cross_attn != nullptr || w.hidden != nullptr) ? &w : nullptr;
 }
-// the path decode steps take now: a probe window needs the per-layer kernels of the multi-kernel path
-static DecodePath decode_path(const ptts_session* s) { return active_probe(s) != nullptr ? DECODE_MULTI_KERNEL : s->path; }
+// the alignment window, or nullptr while none is set
+static const AlignWindow* active_align(const ptts_session* s) { return s->align.out != nullptr ? &s->align : nullptr; }
+// the path decode steps take now: a probe or alignment window needs the per-layer kernels of the multi-kernel path
+static DecodePath decode_path(const ptts_session* s) {
+  return (active_probe(s) != nullptr || active_align(s) != nullptr) ? DECODE_MULTI_KERNEL : s->path;
+}
 
 // the knobs of the EXT sampler, or nullptr for the plain one: the outputs and the ptts_logits_ext stages run on the EXT sampler,
 // with every ptts_sampling_ext stage off when none is active (it then computes what the plain sampler computes)
@@ -365,8 +380,9 @@ int ptts_generate_begin_ids(ptts_session* s, const ptts_gen_params* gen, const i
   s->ext = kExtOff;
   s->lext = kLogitsExtOff;
   s->out = SampleOut{};
-  if (active_probe(s) && s->exec) { cudaGraphExecDestroy(s->exec); s->exec = nullptr; s->graph_ready = false; }
+  if ((active_probe(s) || active_align(s)) && s->exec) { cudaGraphExecDestroy(s->exec); s->exec = nullptr; s->graph_ready = false; }
   s->probe = ProbeWindow{};
+  s->align = AlignWindow{};
   PTTS_CHECK_CUDA(cudaMemcpyAsync(s->ws + s->W.gen, &s->gen, sizeof(ptts_gen_params), cudaMemcpyHostToDevice, st));
   if (int e = launch_generate_begin(sample_args(s), input_ids, n0, gen->max_length, st)) return e;
   s->begun = true;
@@ -456,6 +472,41 @@ int ptts_generate_set_probes(ptts_session* s, void* self_attn, void* cross_attn,
   return PTTS_OK;
 }
 
+int ptts_generate_set_alignment(ptts_session* s, const int32_t* heads, int32_t n_heads, int32_t key0, int32_t key_len, float* out,
+                                int32_t first_step, int32_t n_steps) {
+  PTTS_REQUIRE(s, "null argument");
+  PTTS_REQUIRE(first_step >= 0 && n_steps >= 0, "alignment: the window needs first_step >= 0 and n_steps >= 0, got %d and %d", first_step, n_steps);
+  AlignWindow w{};
+  if (out != nullptr) {
+    const DecoderLayout& L = s->L;
+    // a session with a self-attention prompt prefix aligns to it; one without (prompt_cross_attention) to its cross keys
+    const int keys = s->W.P > 0 ? s->W.P : s->W.S;
+    PTTS_REQUIRE(heads != nullptr && n_heads > 0, "alignment: the head list is empty");
+    PTTS_REQUIRE(key0 >= 0 && key_len > 0 && key0 + key_len <= keys, "alignment: keys [%d, %d) are outside the session's %d %s keys",
+                 key0, key0 + key_len, keys, s->W.P > 0 ? "prompt-prefix" : "cross-attention");
+    std::vector<int32_t> h(2 * (size_t)n_heads);
+    PTTS_CHECK_CUDA(cudaMemcpy(h.data(), heads, h.size() * sizeof(int32_t), cudaMemcpyDeviceToHost));
+    w.layer_heads.assign(L.L, 0);
+    std::vector<char> seen((size_t)L.L * L.nh, 0);
+    for (int e = 0; e < n_heads; e++) {
+      const int l = h[2 * e], hd = h[2 * e + 1];
+      PTTS_REQUIRE(l >= 0 && l < L.L && hd >= 0 && hd < L.nh, "alignment: head [%d, %d] is outside %d layers x %d heads", l, hd, L.L, L.nh);
+      PTTS_REQUIRE(!seen[(size_t)l * L.nh + hd], "alignment: head [%d, %d] is listed twice", l, hd);
+      seen[(size_t)l * L.nh + hd] = 1;
+      w.layer_heads[l]++;
+    }
+    w.heads = heads; w.n_heads = n_heads; w.key0 = key0; w.key_len = key_len; w.out = out;
+    w.first_row = first_step; w.n_rows = n_steps;
+  }
+  const AlignWindow& o = s->align;
+  const bool same = w.out == o.out && w.heads == o.heads && w.n_heads == o.n_heads && w.layer_heads == o.layer_heads &&
+                    w.key0 == o.key0 && w.key_len == o.key_len && w.first_row == o.first_row && w.n_rows == o.n_rows;
+  s->align = w;
+  // the window is a by-value argument of the captured graph's alignment nodes (and it switches the path): capture again
+  if (!same && s->exec) { cudaGraphExecDestroy(s->exec); s->exec = nullptr; s->graph_ready = false; }
+  return PTTS_OK;
+}
+
 // Blob offset of the row-major copy (layout.h rm[]) of the layer matrix stored at blob offset woff, which the wgmma GEMM
 // (gemm_tc.cu) reads; -1 when there is none (f32 model dtype, or not a layer matrix: the lm heads).
 static int64_t rowmajor_offset(const DecoderLayout& L, int64_t woff) {
@@ -535,6 +586,24 @@ static int run_forward(ptts_session* s, cudaStream_t st, bool prefill, const voi
     return launch_attention_probs(p, c.dtype, st);
   };
   if (int e = probe_rows(0, false)) return e;
+  // return_token_timestamps (ptts_generate_set_alignment): decode steps only, after the attention whose keys hold the transcript
+  const AlignWindow* aw = prefill ? nullptr : active_align(s);
+  int align_done = 0;   // alignment heads written so far this step
+  auto align_probe = [&](const AttnArgs& at, int layer) -> int {
+    if (aw == nullptr || aw->layer_heads[layer] == 0 || (at.cross != 0) != (P == 0)) return PTTS_OK;
+    AlignProbeArgs g{};
+    g.q = at.q; g.ldq = at.ldq; g.q_col0 = at.q_col0;
+    g.kcache = at.kcache; g.kv_b_stride = at.kv_b_stride; g.kv_h_stride = at.kv_h_stride; g.kv_b_div = at.kv_b_div;
+    g.key_mask = at.key_mask; g.mask_ld = at.mask_ld;
+    g.B = B; g.nh = L.nh; g.nkv = at.nkv; g.key0 = aw->key0; g.key_len = aw->key_len;
+    g.heads = aw->heads; g.n_heads = aw->n_heads; g.layer = layer; g.layer_heads = aw->layer_heads[layer];
+    g.weight = 1.0f / (float)aw->n_heads; g.accumulate = align_done > 0;
+    g.rope = at.rope; g.rope_cos = at.rope_cos; g.rope_sin = at.rope_sin; g.scale = at.scale;
+    g.out = aw->out; g.ctrl = ctrl; g.n0 = s->n0; g.prefix = P; g.first_row = aw->first_row; g.n_rows = aw->n_rows;
+    align_done += g.layer_heads;
+    s->launches++;
+    return launch_alignment_probe(g, c.dtype, st);
+  };
 
   // plan_rows: the row count that picks the kernel (default Mrows); the GEMMs' per-row results do not depend on M otherwise
   auto lin = [&](const void* X, int64_t ldx, int64_t woff, int N, int K, const float* lw, const float* lb, int epi,
@@ -589,6 +658,7 @@ static int run_forward(ptts_session* s, cudaStream_t st, bool prefill, const voi
     if (int e = launch_attention(at, c.dtype, st, pdl, true)) return e;
     s->launches++;
     if (pw != nullptr) { if (int e = probe_attn(at, i)) return e; }
+    if (int e = align_probe(at, i)) return e;
     if (int e = lin(ws + W.attn, H, lb + L.wo, H, H, nullptr, nullptr, EPI_RESIDUAL, x, x, H, M)) return e;
     if (int e = lin(x, H, lb + L.wqc, H, H, (const float*)(blob + lb + L.ln2_w), (const float*)(blob + lb + L.ln2_b),
                     EPI_STORE, nullptr, ws + W.qc, H, M, lb + L.c_qc)) return e;
@@ -603,6 +673,7 @@ static int run_forward(ptts_session* s, cudaStream_t st, bool prefill, const voi
     if (int e = launch_attention(ct, c.dtype, st, pdl, true)) return e;
     s->launches++;
     if (pw != nullptr) { if (int e = probe_attn(ct, i)) return e; }
+    if (int e = align_probe(ct, i)) return e;
     if (int e = lin(ws + W.attn, H, lb + L.woc, H, H, nullptr, nullptr, EPI_RESIDUAL, x, x, H, M)) return e;
     if (int e = lin(x, H, lb + L.fc1, L.F, H, (const float*)(blob + lb + L.ln3_w), (const float*)(blob + lb + L.ln3_b),
                     EPI_ACT, nullptr, ws + W.hbuf, L.F, M, lb + L.c_fc1)) return e;
@@ -790,6 +861,12 @@ int ptts_decode_steps(ptts_session* s, int32_t n_steps, void* stream) {
   for (int i = 0; i < n_steps; i++) PTTS_CHECK_CUDA(cudaGraphLaunch(s->exec, st));
   s->launches += s->graph_launches * n_steps;
   return PTTS_OK;
+}
+
+int ptts_align_dtw(const float* alignment, int32_t B, int32_t T, int32_t P, const int32_t* n_frames, const int32_t* key_mask,
+                   float* filtered, uint8_t* trace, int32_t* jumps, void* stream) {
+  PTTS_REQUIRE(alignment && n_frames && filtered && trace && jumps, "null argument");
+  return launch_align_dtw(alignment, B, T, P, n_frames, key_mask, filtered, trace, jumps, (cudaStream_t)stream);
 }
 
 int ptts_session_logits(ptts_session* s, float** out) { PTTS_REQUIRE(s && out, "null"); *out = (float*)(s->ws + s->W.logits); return PTTS_OK; }

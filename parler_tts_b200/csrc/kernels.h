@@ -76,6 +76,32 @@ struct ProbeRowsArgs {
   const Ctrl* ctrl; int n0, first_step, n_steps; int64_t step_bytes;
 };
 int launch_probe_rows(const ProbeRowsArgs& a, int dtype, cudaStream_t st);
+// return_token_timestamps (ptts_generate_set_alignment): one layer's share of the alignment row of a decode step.  The step's
+// query is column c = ctrl->cur_len - 1; it writes row c - n0 - first_row of out ([n_rows][B][key_len] fp32) when that lies in
+// [0, n_rows), nothing otherwise or once ctrl->active is 0.
+struct AlignProbeArgs {
+  const void* q; int64_t ldq; int q_col0;          // as AttnProbeArgs (decode: one query row per batch row)
+  const void* kcache; int64_t kv_b_stride, kv_h_stride; int kv_b_div;
+  const int* key_mask; int mask_ld;                // key t with key_mask[(b / kv_b_div) * mask_ld + t] == 0 gets weight 0
+  int B, nh, nkv;
+  int key0, key_len;                               // the transcript keys [key0, key0 + key_len)
+  const int* heads; int n_heads; int layer;        // device [n_heads][2] (layer, head): the entries of `layer` are this launch's
+  int layer_heads;                                 // how many entries belong to `layer`
+  float weight;                                    // 1 / n_heads: the mean
+  int accumulate;                                  // 0: the first layer with alignment heads stores, later layers add
+  int rope; const void* rope_cos; const void* rope_sin;
+  float scale;
+  float* out;
+  const Ctrl* ctrl; int n0, prefix, first_row, n_rows;
+};
+int launch_alignment_probe(const AlignProbeArgs& a, int dtype, cudaStream_t st);
+
+// ---- token timestamps (align.cu) ----------------------------------------------------------------
+// x [B][T][P] fp32 -> y (the width-7 median along frames of each utterance's first n_frames[b] rows), then per utterance the DTW
+// of -y over its unmasked keys and frames; jumps [B][P] = the first frame of each key on the path (-1 for a masked key).
+// trace: B * (P + 1) * (T + 1) bytes of scratch.
+int launch_align_dtw(const float* x, int B, int T, int P, const int* n_frames, const int* key_mask, float* y, unsigned char* trace,
+                     int* jumps, cudaStream_t st);
 
 // ---- embedding (embed.cu) -----------------------------------------------------------------------
 struct EmbedArgs {

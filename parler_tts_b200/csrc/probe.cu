@@ -165,6 +165,103 @@ int launch_attention_probs(const AttnProbeArgs& a, int dtype, cudaStream_t st) {
   return dtype == PTTS_BF16 ? launch_probs_t<bf16, 1>(a, st) : launch_probs_t<float, 1>(a, st);
 }
 
+// One CTA per batch row, one warp per alignment head of this layer (warp w takes the layer's entries w, w + nw, ...).  A head's
+// scores are attention_probs_kernel's (the same q load, RoPE, scale, fp32 dot products in the same order, rounded to the model
+// dtype), over the key_len transcript keys only; the softmax over those keys alone is the eager weights restricted to them and
+// renormalized, before any rounding.  Each warp sums its heads' distributions; the CTA adds the warps in order and scales by
+// `weight`.  Cost per row: (heads of the layer) x key_len K rows, independent of the cache length.
+template <typename T>
+__global__ void __launch_bounds__(256) alignment_probe_kernel(AlignProbeArgs a) {
+  extern __shared__ __align__(16) float sma[];
+  const int nw = blockDim.x >> 5, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int b = blockIdx.x, P = a.key_len;
+  if (a.ctrl->active == 0) return;
+  const int cl = a.ctrl->cur_len;
+  const int row = cl - 1 - a.n0 - a.first_row;
+  if (row < 0 || row >= a.n_rows) return;
+  float* qs = sma + (size_t)warp * (HD + 2 * P);   // [64] the head's scaled, rotated query
+  float* sc = qs + HD;                             // [P] its rounded scores (-inf: masked key)
+  float* acc = sc + P;                             // [P] this warp's sum of distributions
+  for (int p = lane; p < P; p += 32) acc[p] = 0.f;
+  const int pos = a.prefix + cl - 1;
+  const int kvb = b / a.kv_b_div;
+  const int* km = a.key_mask ? a.key_mask + (size_t)kvb * a.mask_ld : nullptr;
+  const T* rope_cos = reinterpret_cast<const T*>(a.rope_cos);
+  const T* rope_sin = reinterpret_cast<const T*>(a.rope_sin);
+  int k = 0;   // index of the entry among this layer's
+  for (int e = 0; e < a.n_heads; e++) {
+    if (a.heads[2 * e] != a.layer) continue;
+    if (k++ % nw != warp) continue;
+    const int h = a.heads[2 * e + 1];
+    const T* src = reinterpret_cast<const T*>(a.q) + (size_t)b * a.ldq + a.q_col0 + (size_t)h * HD;
+    for (int d = lane; d < HD; d += 32) {
+      float x = DT<T>::to_f(src[d]);
+      if (a.rope) {
+        const float xp = DT<T>::to_f(src[d < HD / 2 ? d + HD / 2 : d - HD / 2]);
+        x = rope_elem<T>(x, xp, d, rope_cos + (size_t)pos * HD, rope_sin + (size_t)pos * HD);
+      }
+      qs[d] = DT<T>::rnd(x * a.scale);
+    }
+    __syncwarp();
+    const T* kc = reinterpret_cast<const T*>(a.kcache) + (size_t)kvb * a.kv_b_stride + (size_t)(h / (a.nh / a.nkv)) * a.kv_h_stride;
+    float m = -INFINITY;
+    for (int p = lane; p < P; p += 32) {
+      const int t = a.key0 + p;
+      float s = -INFINITY;
+      if (km == nullptr || km[t] != 0) {
+        const T* krow = kc + (size_t)t * HD;
+        float dot = 0.f;
+#pragma unroll
+        for (int c = 0; c < HD / 8; c++) {
+          float kv[8];
+          load8(krow + kv_swz(t, 8 * c), kv);
+#pragma unroll
+          for (int i = 0; i < 8; i++) dot = fmaf(qs[8 * c + i], kv[i], dot);
+        }
+        s = DT<T>::rnd(dot);
+      }
+      sc[p] = s;
+      m = fmaxf(m, s);
+    }
+    m = warp_max(m);
+    if (m != -INFINITY) {   // every transcript key masked: the head adds nothing
+      float l = 0.f;
+      for (int p = lane; p < P; p += 32) l += expf(sc[p] - m);
+      l = warp_sum(l);
+      for (int p = lane; p < P; p += 32) acc[p] += expf(sc[p] - m) / l;
+    }
+    __syncwarp();
+  }
+  __syncthreads();
+  float* out = a.out + ((size_t)row * a.B + b) * P;
+  for (int p = threadIdx.x; p < P; p += blockDim.x) {
+    float v = 0.f;
+    for (int w = 0; w < nw; w++) v += sma[(size_t)w * (HD + 2 * P) + HD + P + p];
+    v *= a.weight;
+    out[p] = a.accumulate ? out[p] + v : v;
+  }
+}
+
+int launch_alignment_probe(const AlignProbeArgs& a, int dtype, cudaStream_t st) {
+  PTTS_REQUIRE(a.B > 0 && a.nh > 0 && a.nkv > 0 && a.nh % a.nkv == 0 && a.key_len > 0 && a.layer_heads > 0 && a.ctrl != nullptr,
+               "alignment_probe: bad shape");
+  const int nw = a.layer_heads < 8 ? a.layer_heads : 8;
+  const size_t smem = (size_t)nw * (HD + 2 * a.key_len) * sizeof(float);
+  PTTS_REQUIRE(smem <= 200 * 1024, "alignment_probe: %d transcript keys need %zu B of shared memory (> 200 KB)", a.key_len, smem);
+  static bool attr[2] = {false, false};
+  if (!attr[dtype == PTTS_BF16]) {
+    if (dtype == PTTS_BF16)
+      PTTS_CHECK_CUDA(cudaFuncSetAttribute(alignment_probe_kernel<bf16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    else
+      PTTS_CHECK_CUDA(cudaFuncSetAttribute(alignment_probe_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    attr[dtype == PTTS_BF16] = true;
+  }
+  if (dtype == PTTS_BF16) alignment_probe_kernel<bf16><<<a.B, nw * 32, smem, st>>>(a);
+  else alignment_probe_kernel<float><<<a.B, nw * 32, smem, st>>>(a);
+  PTTS_CHECK_CUDA(cudaGetLastError());
+  return PTTS_OK;
+}
+
 int launch_probe_rows(const ProbeRowsArgs& a, int dtype, cudaStream_t st) {
   const int blocks = (a.rows * 32 + 255) / 256;
   if (dtype == PTTS_BF16) probe_rows_kernel<bf16><<<blocks, 256, 0, st>>>(a);

@@ -871,6 +871,20 @@ class GenSession:
         _lib.check(_lib.lib().ptts_generate_set_probes(self.h, addr(self_attn), addr(cross_attn), addr(hidden), int(first_step),
                                                        int(n_steps), int(self_ld), step(self_attn), step(cross_attn), step(hidden)))
 
+    def set_alignment(self, heads: Optional[torch.Tensor] = None, key0: int = 0, key_len: int = 0, out: Optional[torch.Tensor] = None,
+                      first_row: int = 0, n_rows: int = 0):
+        """ptts_generate_set_alignment: decode steps write the alignment rows [first_row, first_row + n_rows) of the [n_heads, 2]
+        int32 (layer, head) list over keys [key0, key0 + key_len) into out [n_rows, B, key_len] fp32.  out None switches it off."""
+        if out is None:
+            self._align = None
+            _lib.check(_lib.lib().ptts_generate_set_alignment(self.h, None, 0, 0, 0, None, 0, 0))
+            return
+        if out.dtype != torch.float32 or tuple(out.shape) != (n_rows, self.B, key_len):
+            raise ValueError(f"the alignment buffer must be float32 [{n_rows}, {self.B}, {key_len}]")
+        self._align = (heads, out)   # the list and the buffer stay alive while the kernels may read / write them
+        _lib.check(_lib.lib().ptts_generate_set_alignment(self.h, _lib.ptr(heads), int(heads.shape[0]), int(key0), int(key_len),
+                                                          _lib.ptr(out), int(first_row), int(n_rows)))
+
 
 def output_window(step: int, chunk: int) -> tuple[int, int]:
     """The chunk of generate()'s per-step outputs that holds `step`: (index, first step)."""
@@ -1015,6 +1029,83 @@ class StepProbes:
 
 
 # ---- model classes -------------------------------------------------------------------------------
+def resolve_alignment_heads(heads, n_layers: int, n_heads: int) -> list[list[int]]:
+    """GenerationConfig.alignment_heads -> the [layer, head] pairs return_token_timestamps averages.  None: every head of the last
+    ceil(n_layers / 2) layers (openai-whisper's choice when a model has no known alignment heads; no Parler checkpoint has any).
+    An empty list, a pair outside the decoder or a pair listed twice raises ValueError."""
+    if heads is None:
+        return [[l, h] for l in range(n_layers // 2, n_layers) for h in range(n_heads)]
+    try:
+        pairs = [list(p) for p in heads]
+    except TypeError:
+        raise ValueError(f"`alignment_heads` must be a list of [layer, head] pairs, got {heads!r}") from None
+    if not pairs:
+        raise ValueError("`alignment_heads` is empty: list at least one [layer, head] pair, or None for the default heads")
+    seen = set()
+    for p in pairs:
+        if len(p) != 2 or not all(isinstance(v, int) and not isinstance(v, bool) for v in p):
+            raise ValueError(f"`alignment_heads` must be a list of [layer, head] integer pairs, got {p!r}")
+        l, h = p
+        if not (0 <= l < n_layers and 0 <= h < n_heads):
+            raise ValueError(f"`alignment_heads` pair {p} is outside the decoder's {n_layers} layers x {n_heads} heads")
+        if (l, h) in seen:
+            raise ValueError(f"`alignment_heads` lists {p} twice")
+        seen.add((l, h))
+    return pairs
+
+
+def token_frames(raw_ids: torch.Tensor, n0: int, num_codebooks: int, codebook_size: int) -> torch.Tensor:
+    """raw_ids [B * K, T] -> int32 [B]: the generated frames of each utterance that token timestamps align to.  Generated frame f
+    is codebook 0's id at column n0 + f and codebook k's at column n0 + f + k (the delay pattern); the frames counted are the
+    leading ones whose K ids are all codes (< codebook_size, as the audio decode requires), so they end at the utterance's EOS,
+    at the last frame every codebook reaches (T - n0 - K + 1) and at the last column that got an alignment row (T - n0 - 1)."""
+    K = num_codebooks
+    T = raw_ids.shape[1] - n0
+    F = max(0, min(T - K + 1, T - 1))
+    r = raw_ids.view(-1, K, raw_ids.shape[1])
+    ok = torch.ones(r.shape[0], F, dtype=torch.bool, device=raw_ids.device)
+    for k in range(K):
+        ok &= r[:, k, n0 + k:n0 + k + F] < codebook_size
+    return ok.int().cumprod(dim=1).sum(dim=1).to(torch.int32)
+
+
+def align_dtw(alignment: torch.Tensor, n_frames: torch.Tensor, key_mask: Optional[torch.Tensor] = None):
+    """ptts_align_dtw: alignment [B, T, P] fp32 (CUDA) -> (filtered [B, T, P]: the width-7 median along each utterance's first
+    n_frames[b] frames, NaN past them; jumps [B, P] int32: the first frame of each unmasked key on the DTW path of -filtered,
+    -1 for a masked key).  openai-whisper's median filter and DTW as transformers' generation_whisper runs them."""
+    B, T, P = alignment.shape
+    dev = alignment.device
+    x = alignment.to(torch.float32).contiguous()
+    nf = n_frames.to(device=dev, dtype=torch.int32).contiguous()
+    km = None if key_mask is None else key_mask.to(device=dev, dtype=torch.int32).contiguous()
+    filtered = torch.full_like(x, float("nan"))
+    trace = torch.empty(B * (P + 1) * (T + 1), dtype=torch.uint8, device=dev)
+    jumps = torch.empty(B, P, dtype=torch.int32, device=dev)
+    _lib.check(_lib.lib().ptts_align_dtw(_lib.ptr(x), B, T, P, _lib.ptr(nf), _lib.ptr(km), _lib.ptr(filtered), _lib.ptr(trace),
+                                         _lib.ptr(jumps), _lib.stream_ptr()))
+    return filtered, jumps
+
+
+class StepAlignment:
+    """generate()'s return_token_timestamps recorder: row t of utterance b (alignment[b, t]) is the alignment heads' mean
+    distribution over the key_len transcript keys for the query of generated column n0 + t, written by the decode step whose
+    input is that column (ptts_generate_set_alignment).  The last generated column is never a decode step's input, so its row,
+    and the rows of a shard that ended before the longest one, stay NaN.  One [rows, B_shard, key_len] buffer per session."""
+
+    def __init__(self, heads: list[list[int]], batch: int, rows: int, key0: int, key_len: int, device):
+        self.heads = torch.tensor(heads, dtype=torch.int32, device=device).reshape(-1, 2).contiguous()
+        self.rows, self.key0, self.key_len = rows, key0, key_len
+        self.alignment = torch.full((batch, rows, key_len), float("nan"), dtype=torch.float32, device=device)
+
+    def set(self, sess: "GenSession") -> torch.Tensor:
+        buf = torch.full((self.rows, sess.B, self.key_len), float("nan"), dtype=torch.float32, device=self.alignment.device)
+        sess.set_alignment(self.heads, self.key0, self.key_len, buf, 0, self.rows)
+        return buf
+
+    def put(self, buf: torch.Tensor, b0: int):
+        self.alignment[b0:b0 + buf.shape[1]] = buf.permute(1, 0, 2)
+
+
 class GenerateOutput(dict):
     """Stands in for HF's GenerateEncoderDecoderOutput: .sequences plus ["audios_length"] (:3648-3651)."""
 
@@ -1403,7 +1494,8 @@ class ParlerTTSForConditionalGeneration:
         return 32
 
     def _run_token_loop(self, enc_hidden, attention_mask, prompt_hidden, prompt_mask, *, gc, max_length, seed, suppress_special, row_base,
-                        ext, min_new_tokens, lext=None, streamer=None, custom=None, input_ids=None, outputs=None, out_row=0, probes=None, takes=1):
+                        ext, min_new_tokens, lext=None, streamer=None, custom=None, input_ids=None, outputs=None, out_row=0, probes=None, takes=1,
+                        align=None):
         """begin + prefill + the token loop of one session; returns the raw token matrix [B * K, generated length].
         takes: the session's B rows are `takes` consecutive takes of each of the enc_hidden.shape[0] descriptions (B / takes);
         prompt_hidden, prompt_mask and input_ids have B rows.
@@ -1411,7 +1503,8 @@ class ParlerTTSForConditionalGeneration:
         outputs: None, or the StepOutputs this session's rows (from row out_row of the batch) are recorded into.  The device
         loop then sets the sampler's window before every call and keeps each call inside one chunk.
         probes: None, or the StepProbes this session's attention weights / hidden states (from utterance out_row // K) go to;
-        its windows follow the same chunks, and the decode steps then run the multi-kernel path (ptts_generate_set_probes)."""
+        its windows follow the same chunks, and the decode steps then run the multi-kernel path (ptts_generate_set_probes).
+        align: None, or the StepAlignment this session's utterances (from out_row // K) go to; one window spans the whole call."""
         d = self.config.decoder
         K = d.num_codebooks
         S = enc_hidden.shape[1]
@@ -1435,7 +1528,10 @@ class ParlerTTSForConditionalGeneration:
                 _, pm = build_delay_pattern_mask(input_ids, d.bos_token_id, d.pad_token_id, max_length, K)
                 cells = pm[:, n0:n0 + K - 1]
                 stream_col = lambda col, v: (torch.where(cells[:, col - n0] == -1, v, cells[:, col - n0]) if col - n0 < cells.shape[1] else v)
+        align_buf = None
         try:
+            if align is not None:
+                align_buf = align.set(sess)
             if probes is not None:
                 probes.set_prefill(sess, out_row // K)
             sess.prefill(prompt_hidden, prompt_mask, enc_hidden, attention_mask)
@@ -1481,10 +1577,28 @@ class ParlerTTSForConditionalGeneration:
         finally:
             if probes is not None:
                 sess.set_probes()   # the session keeps no window (nor the chunks) past this call, whatever happens in it
+            if align_buf is not None:
+                sess.set_alignment()
+        if align_buf is not None:
+            align.put(align_buf, out_row // K)
         cur_len = int(sess.state[0].item())
         if outputs is not None:
             sess.set_outputs(None, None)   # the session keeps no reference to the chunks
         return sess.raw_ids[:, :cur_len].clone()
+
+    def _token_timestamps(self, align: StepAlignment, raw_ids: torch.Tensor, n0: int, text_mask, takes: int) -> dict:
+        """generate()'s `alignment` [B * N, T_gen, P] and `token_timestamps` [B * N, P] (seconds from the first generated frame,
+        NaN at masked transcript positions): the recorded rows, then ptts_align_dtw over each utterance's token_frames."""
+        K, cs = self.config.decoder.num_codebooks, self.config.audio_encoder.codebook_size
+        alignment = align.alignment[:, :raw_ids.shape[1] - n0].contiguous()
+        mask = None
+        if text_mask is not None:
+            mask = text_mask.to(self.device)
+            if mask.shape[0] != alignment.shape[0]:
+                mask = mask.repeat_interleave(takes, dim=0)
+        _, jumps = align_dtw(alignment, token_frames(raw_ids, n0, K, cs), mask)
+        seconds = jumps.double() * self.audio_encoder.hop_length / self.config.audio_encoder.sampling_rate
+        return dict(alignment=alignment, token_timestamps=torch.where(jumps >= 0, seconds, float("nan")).float())
 
     # -- teacher-forced forward (scoring) ------------------------------------------------------------
     _SCORE_SHARD = 32   # utterances per ptts_score call: the workspace is sized for one shard
@@ -1636,6 +1750,15 @@ class ParlerTTSForConditionalGeneration:
         step kernel) for as long as anything is recorded.  A shard that ended holds NaN, as in `scores`.  Memory: see
         StepProbes.
 
+        return_token_timestamps=True (with return_dict_in_generate=True, else ValueError) adds `alignment` [B * N, T_gen, P] fp32,
+        row t the mean over `alignment_heads` ([layer, head] pairs; None = every head of the last ceil(L / 2) layers) of each
+        head's weights over the P transcript tokens, renormalized over them (masked tokens 0), for the query of generated column
+        n0 + t (the last row, never a decode step's input, is NaN), and `token_timestamps` [B * N, P] fp32: each transcript
+        token's start in seconds, counted from the first generated frame (after a continuation's prefix audio), NaN where the
+        prompt is masked (StepAlignment, align_dtw).  The transcript is the prompt prefix, or the prompt's cross-attention keys
+        in prompt_cross_attention mode; without one the flag raises ValueError.  The tokens and audio do not change; the decode
+        steps run the multi-kernel path while it is set.
+
         config.prompt_cross_attention: `prompt_input_ids` plus their sinusoidal positions are appended to the description states
         as cross-attention keys (prompt_cross_states, reference :3099-3130), also after `encoder_outputs`; the decoder then has no
         prompt prefix (P = 0), and `cross_attentions` have S + P keys.  `prompt_hidden_states` raise ValueError in this mode.
@@ -1674,6 +1797,14 @@ class ParlerTTSForConditionalGeneration:
             raise ValueError("Got incompatible mode for generation, should be one of greedy or sampling. "
                              "Ensure that beam search is de-activated by setting `num_beams=1` and `num_beam_groups=1`.")
         N = resolve_num_return_sequences(gc)
+        want_ts = bool(gc.return_token_timestamps)
+        if want_ts and not gc.return_dict_in_generate:
+            raise ValueError("`return_token_timestamps=True` needs `return_dict_in_generate=True`: the alignment and the "
+                             "timestamps exist only in the dict return")
+        align_heads = None
+        if want_ts or gc.alignment_heads is not None:
+            align_heads = resolve_alignment_heads(gc.alignment_heads, self.config.decoder.num_hidden_layers,
+                                                  self.config.decoder.num_attention_heads)
         if self.prompt_cross_attention and mk.get("prompt_hidden_states") is not None:
             # the reference would put these states in front of the decoder while counting its cache positions without them
             raise ValueError("a prompt_cross_attention model takes the transcript as `prompt_input_ids`, not `prompt_hidden_states`")
@@ -1700,10 +1831,12 @@ class ParlerTTSForConditionalGeneration:
             enc_hidden = self._encode_text(input_ids, attention_mask)   # encoder + enc_to_dec_proj + mask multiply, one CUDA graph
         enc_hidden = enc_hidden.to(self.device, self.dtype)
         prompt_hidden = mk.get("prompt_hidden_states")
+        text_key0, text_len, text_mask = 0, 0, None   # the transcript keys token timestamps align to
         if self.prompt_cross_attention and mk.get("prompt_input_ids") is not None:
             # the prompt joins the description as cross-attention keys (:3099-3130); everything below runs with P = 0
             if not self._side_loaded:
                 raise ValueError("no embed_prompts weights loaded")
+            text_key0, text_len, text_mask = enc_hidden.shape[1], mk["prompt_input_ids"].shape[1], mk.get("prompt_attention_mask")
             enc_hidden, attention_mask = prompt_cross_states(enc_hidden, attention_mask, mk["prompt_input_ids"], mk.get("prompt_attention_mask"),
                                                              self.embed_prompts_weight, self.embed_positions_weight)
         elif prompt_hidden is None and mk.get("prompt_input_ids") is not None:
@@ -1713,6 +1846,11 @@ class ParlerTTSForConditionalGeneration:
         prompt_mask = mk.get("prompt_attention_mask") if prompt_hidden is not None else None
         P = 0 if prompt_hidden is None else prompt_hidden.shape[1]
         B, S, _ = enc_hidden.shape
+        if P > 0:
+            text_len, text_mask = P, prompt_mask
+        if want_ts and text_len == 0:
+            raise ValueError("`return_token_timestamps=True` needs a transcript to align: pass `prompt_input_ids` or "
+                             "`prompt_hidden_states` with at least one token")
 
         d = self.config.decoder
         K = d.num_codebooks
@@ -1763,6 +1901,8 @@ class ParlerTTSForConditionalGeneration:
         if want_attn or want_hidden:
             probes = StepProbes(d.num_hidden_layers, BN, d.num_attention_heads, S, d.hidden_size, P, n0, self.dtype, self.device,
                                 want_attn, want_hidden)
+        if want_ts:
+            run["align"] = StepAlignment(align_heads, BN, max_length - n0, text_key0, text_len, self.device)
         limit = self._fused_batch_limit()
         if limit is not None and BN > limit and not custom_loop and streamer is None:
             # The fused decode-step kernels hold one 32-row tile: a larger batch runs as consecutive shards of <= 32 rows through the
@@ -1818,6 +1958,8 @@ class ParlerTTSForConditionalGeneration:
                     out.update(encoder_attentions=enc_probe.get("encoder_attentions"))
                 if want_hidden:
                     out.update(encoder_hidden_states=enc_probe.get("encoder_hidden_states"))
+            if want_ts:
+                out.update(self._token_timestamps(run["align"], output_ids, n0, text_mask, N))
             if gc.return_dict_in_generate:
                 return out
             return output_values, out
