@@ -297,6 +297,14 @@ int ptts_session_destroy(ptts_session* s) {
   return PTTS_OK;
 }
 
+// The captured decode graph holds the session's settings and windows by value: drop it, and the next ptts_decode_steps captures
+// again.
+static void drop_graph(ptts_session* s) {
+  if (s->exec) cudaGraphExecDestroy(s->exec);
+  s->exec = nullptr;
+  s->graph_ready = false;
+}
+
 static SampleArgs sample_args(ptts_session* s) {
   SampleArgs a{};
   const WorkspaceLayout& W = s->W;
@@ -380,7 +388,7 @@ int ptts_generate_begin_ids(ptts_session* s, const ptts_gen_params* gen, const i
   s->ext = kExtOff;
   s->lext = kLogitsExtOff;
   s->out = SampleOut{};
-  if ((active_probe(s) || active_align(s)) && s->exec) { cudaGraphExecDestroy(s->exec); s->exec = nullptr; s->graph_ready = false; }
+  if (active_probe(s) || active_align(s)) drop_graph(s);
   s->probe = ProbeWindow{};
   s->align = AlignWindow{};
   PTTS_CHECK_CUDA(cudaMemcpyAsync(s->ws + s->W.gen, &s->gen, sizeof(ptts_gen_params), cudaMemcpyHostToDevice, st));
@@ -405,7 +413,7 @@ int ptts_generate_set_sampling_ext(ptts_session* s, const ptts_sampling_ext* ext
   PTTS_REQUIRE(x.eta_cutoff >= 0.f && x.eta_cutoff < 1.f, "`eta_cutoff` has to be a float in [0, 1) (0 = off), got %f", x.eta_cutoff);
   s->ext = x;
   // the knobs are a by-value argument of the captured graph's sampler node: capture again
-  if (s->exec) { cudaGraphExecDestroy(s->exec); s->exec = nullptr; s->graph_ready = false; }
+  drop_graph(s);
   return PTTS_OK;
 }
 
@@ -422,7 +430,7 @@ int ptts_generate_set_logits_ext(ptts_session* s, const ptts_logits_ext* ext) {
   PTTS_REQUIRE(x.begin_suppress == nullptr || x.begin_index >= 1, "`begin_suppress_tokens`: begin index %d must be >= 1", x.begin_index);
   s->lext = x;
   // the struct is a by-value argument of the captured graph's sampler node: capture again
-  if (s->exec) { cudaGraphExecDestroy(s->exec); s->exec = nullptr; s->graph_ready = false; }
+  drop_graph(s);
   return PTTS_OK;
 }
 
@@ -440,7 +448,7 @@ int ptts_generate_set_outputs(ptts_session* s, float* logits, float* scores, int
                     o.n_steps == s->out.n_steps && o.step_stride == s->out.step_stride;
   s->out = o;
   // the window is a by-value argument of the captured graph's sampler node: capture again when it moved
-  if (!same && s->exec) { cudaGraphExecDestroy(s->exec); s->exec = nullptr; s->graph_ready = false; }
+  if (!same) drop_graph(s);
   return PTTS_OK;
 }
 
@@ -468,7 +476,7 @@ int ptts_generate_set_probes(ptts_session* s, void* self_attn, void* cross_attn,
                     w.hidden_step == o.hidden_step;
   s->probe = w;
   // the window is a by-value argument of the captured graph's probe nodes (and it switches the path): capture again when it moved
-  if (!same && s->exec) { cudaGraphExecDestroy(s->exec); s->exec = nullptr; s->graph_ready = false; }
+  if (!same) drop_graph(s);
   return PTTS_OK;
 }
 
@@ -503,7 +511,7 @@ int ptts_generate_set_alignment(ptts_session* s, const int32_t* heads, int32_t n
                     w.key0 == o.key0 && w.key_len == o.key_len && w.first_row == o.first_row && w.n_rows == o.n_rows;
   s->align = w;
   // the window is a by-value argument of the captured graph's alignment nodes (and it switches the path): capture again
-  if (!same && s->exec) { cudaGraphExecDestroy(s->exec); s->exec = nullptr; s->graph_ready = false; }
+  if (!same) drop_graph(s);
   return PTTS_OK;
 }
 
@@ -701,7 +709,7 @@ int ptts_prefill(ptts_session* s, const void* prompt_hidden, const int64_t* prom
   s->prefilled = true;
   s->path = choose_decode_path(s);
   // mask presence is baked into the captured graph: re-capture if it changed
-  if (s->exec) { cudaGraphExecDestroy(s->exec); s->exec = nullptr; s->graph_ready = false; }
+  drop_graph(s);
   return PTTS_OK;
 }
 

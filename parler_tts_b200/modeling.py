@@ -9,11 +9,12 @@ PyTorch is used for device memory, streams and the one-off side inputs the path 
 (text encoder, prompt embedding lookup: SURVEY.md section 1).
 """
 from __future__ import annotations
+import contextlib
 import ctypes as C
 import json
 import math
 import os
-from typing import Any, Optional
+from typing import Any, NamedTuple, Optional
 
 import numpy as np
 import torch
@@ -913,12 +914,18 @@ class StepOutputs:
                 lst.append(torch.full((self.CHUNK, self.rows, self.V), float("nan"), dtype=torch.float32, device=self.device))
         return {k: lst[c] for k, lst in self.chunks.items()}
 
-    def set_window(self, sess: "GenSession", step: int, row0: int):
-        """Points the session's sampler at the chunk holding `step`, at this shard's first row row0."""
+    def attach_prefill(self, sess: "GenSession", b0: int):
+        pass   # the prefill records no row: step 0 is the sample after it
+
+    def attach_window(self, sess: "GenSession", step: int, b0: int):
+        """Points the session's sampler at the chunk holding `step`, at the rows of batch row b0 on."""
         c, first = output_window(step, self.CHUNK)
         ch = self.chunk(c)
-        at = lambda k: ch[k][0, row0] if k in ch else None
+        at = lambda k: ch[k][0, b0 * sess.K] if k in ch else None
         sess.set_outputs(at("logits"), at("scores"), first, self.CHUNK, self.rows * self.V)
+
+    def detach(self, sess: "GenSession", b0: int):
+        sess.set_outputs(None, None)   # the session keeps no reference to the chunks
 
     def put(self, step: int, row0: int, logits: torch.Tensor, scores: torch.Tensor):
         """Stores one step's rows from torch (the host-driven loop)."""
@@ -987,19 +994,24 @@ class StepProbes:
             self.chunks[c] = ch
         return self.chunks[c]
 
-    def set_prefill(self, sess: "GenSession", b0: int):
+    def attach_prefill(self, sess: "GenSession", b0: int):
         """Points the session's prefill at entry 0, from batch row b0 on."""
         e = self._entry0()
         at = lambda k: e[k][:, b0] if k in e else None
         sess.set_probes(at("self"), at("cross"), at("hidden"), 0, 1, self.P + self.n0)
 
-    def set_window(self, sess: "GenSession", step: int, b0: int):
-        """Points the session's decode steps at the chunk holding `step` (>= 1), from batch row b0 on."""
+    def attach_window(self, sess: "GenSession", step: int, b0: int):
+        """Points the session's decode steps at the chunk holding `step`, from batch row b0 on (step 0 is entry 0: nothing)."""
+        if step == 0:
+            return
         c, first = output_window(step, self.CHUNK)
         f = max(first, 1)   # (slot 0 of chunk 0 stays unused: step 0 is entry 0)
         ch = self.chunk(c)
         at = lambda k: ch[k][f - first:, b0] if k in ch else None
         sess.set_probes(at("self"), at("cross"), at("hidden"), f, first + self.CHUNK - f, self.t_hi(c))
+
+    def detach(self, sess: "GenSession", b0: int):
+        sess.set_probes()   # the session keeps no window (nor the chunks) past the call
 
     def entry(self, t: int) -> dict:
         """Entry t: decoder_attentions / cross_attentions (tuples of L [B, heads, q, T_kv] / [B, heads, q, S]) and
@@ -1090,20 +1102,64 @@ class StepAlignment:
     """generate()'s return_token_timestamps recorder: row t of utterance b (alignment[b, t]) is the alignment heads' mean
     distribution over the key_len transcript keys for the query of generated column n0 + t, written by the decode step whose
     input is that column (ptts_generate_set_alignment).  The last generated column is never a decode step's input, so its row,
-    and the rows of a shard that ended before the longest one, stay NaN.  One [rows, B_shard, key_len] buffer per session."""
+    and the rows of a shard that ended before the longest one, stay NaN.  One [rows, B_shard, key_len] buffer and window per session."""
+    CHUNK = None   # the window spans the whole call
 
     def __init__(self, heads: list[list[int]], batch: int, rows: int, key0: int, key_len: int, device):
         self.heads = torch.tensor(heads, dtype=torch.int32, device=device).reshape(-1, 2).contiguous()
         self.rows, self.key0, self.key_len = rows, key0, key_len
         self.alignment = torch.full((batch, rows, key_len), float("nan"), dtype=torch.float32, device=device)
 
-    def set(self, sess: "GenSession") -> torch.Tensor:
-        buf = torch.full((self.rows, sess.B, self.key_len), float("nan"), dtype=torch.float32, device=self.alignment.device)
-        sess.set_alignment(self.heads, self.key0, self.key_len, buf, 0, self.rows)
-        return buf
+    def attach_prefill(self, sess: "GenSession", b0: int):
+        self.buf = torch.full((self.rows, sess.B, self.key_len), float("nan"), dtype=torch.float32, device=self.alignment.device)
+        sess.set_alignment(self.heads, self.key0, self.key_len, self.buf, 0, self.rows)
 
-    def put(self, buf: torch.Tensor, b0: int):
-        self.alignment[b0:b0 + buf.shape[1]] = buf.permute(1, 0, 2)
+    def attach_window(self, sess: "GenSession", step: int, b0: int):
+        pass
+
+    def detach(self, sess: "GenSession", b0: int):
+        sess.set_alignment()
+        self.alignment[b0:b0 + self.buf.shape[1]] = self.buf.permute(1, 0, 2)
+        self.buf = None
+
+
+@contextlib.contextmanager
+def recording(sess: "GenSession", recorders, b0: int, step: int = 0):
+    """Attaches the recorders (StepOutputs, StepProbes, StepAlignment; rows from batch row b0 on) for the prefill / score pass
+    (step 0) or for the decode step `step`, and detaches them and collects their rows when the block ends, whatever happens in it
+    (in reverse order).  A token loop in the block moves their windows: attach_window(sess, t, b0) before the steps from t on."""
+    attached = []
+    try:
+        for r in recorders:
+            if step == 0:
+                r.attach_prefill(sess, b0)
+            else:
+                r.attach_window(sess, step, b0)
+            attached.append(r)
+        yield
+    finally:
+        for r in reversed(attached):
+            r.detach(sess, b0)
+
+
+class Sampling(NamedTuple):
+    """One generate() call's sampling settings (ParlerTTSForConditionalGeneration._sampling): what GenSession.begin takes (a
+    shard begins at row_base + its first row * K), and the caller's logits processors and stopping criteria (the host-driven
+    loop runs the call when there are any)."""
+    max_length: int
+    do_sample: bool
+    temperature: float
+    top_k: int
+    top_p: float
+    min_new_tokens: int
+    seed: int
+    suppress_special: bool
+    codebook_size: int
+    row_base: int
+    ext: Optional[dict]           # resolve_sampling_ext
+    lext: Optional[LogitsExt]     # resolve_logits_ext
+    processors: list
+    criteria: list
 
 
 class GenerateOutput(dict):
@@ -1195,13 +1251,8 @@ class ParlerTTSForCausalLM:
             if not bool((ids == self.config.bos_token_id).all()):
                 raise ValueError("the first call must feed the decoder start (BOS) column")
             probes = self._probes(B, P, S, output_attentions, output_hidden_states)
-            try:
-                if probes is not None:
-                    probes.set_prefill(sess, 0)
+            with recording(sess, [] if probes is None else [probes], 0):
                 sess.prefill(prompt_hidden_states, prompt_attention_mask if P > 0 else None, encoder_hidden_states, encoder_attention_mask)
-            finally:
-                if probes is not None:
-                    sess.set_probes()   # the window never outlives the call, whatever happens in it
             past_key_values = ParlerTTSCache(sess)
         else:
             if not isinstance(past_key_values, ParlerTTSCache) or past_key_values.session.B != B:
@@ -1210,13 +1261,8 @@ class ParlerTTSForCausalLM:
             sess.sample(forced=ids)
             step = past_key_values.steps + 1
             probes = self._probes(B, sess.P, sess.S, output_attentions, output_hidden_states)
-            try:
-                if probes is not None:
-                    probes.set_window(sess, step, 0)
+            with recording(sess, [] if probes is None else [probes], 0, step):
                 sess.decode_forward()
-            finally:
-                if probes is not None:
-                    sess.set_probes()
             past_key_values.steps += 1
         logits = sess.logits.clone().unsqueeze(1)   # [B*K, 1, V] fp32
         if not return_dict:
@@ -1414,23 +1460,73 @@ class ParlerTTSForConditionalGeneration:
         graph.replay()
         return s_out.clone()
 
-    # -- generate with user-supplied processors / stopping criteria --------------------------------
-    def _host_driven_loop(self, sess: "GenSession", gc, max_length, user_processors, user_criteria, streamer, seed, stream_col, ext,
-                          min_new_tokens, outputs=None, out_row=0, probe_window=None, lext=None):
+    # -- conditioning (forward and generate) --------------------------------------------------------
+    def _conditioning(self, caller: str, input_ids, attention_mask, encoder_outputs, prompt_input_ids, prompt_attention_mask,
+                      prompt_hidden_states, cross_prompt_after_encoder_outputs: bool, encoder_flags: Optional[dict] = None):
+        """forward()'s and generate()'s inputs -> (encoder states [B, S, H], their mask, the prompt prefix [B, P, H] or None, its
+        mask, the transcript keys as (first key, count, mask), the text encoder's output if encoder_flags ran it eagerly, else None).
+        On a prompt_cross_attention checkpoint the prompt joins the description as cross-attention keys (prompt_cross_states,
+        :2791-2811 / :3099-3130) and there is no prefix; with `encoder_outputs` only if cross_prompt_after_encoder_outputs."""
+        cross_prompt = self.prompt_cross_attention and (prompt_input_ids is not None or prompt_hidden_states is not None)
+        eo = None
+        if encoder_outputs is not None:
+            if cross_prompt and not cross_prompt_after_encoder_outputs:
+                # the reference would make the prompt a self-attention prefix without positions: the other model
+                raise ValueError("a prompt_cross_attention model joins the prompt to the description only when forward() runs the "
+                                 "text encoder: pass `input_ids` instead of `encoder_outputs`, or no prompt")
+            enc = encoder_outputs
+            enc_hidden = enc[0] if isinstance(enc, (tuple, list)) else getattr(enc, "last_hidden_state", enc)
+        elif input_ids is None:
+            raise ValueError(f"{caller}() needs `input_ids` (description) or `encoder_outputs`")
+        elif encoder_flags:
+            enc_hidden, eo = self._encode_text_eager(input_ids, attention_mask, encoder_flags)
+        else:
+            enc_hidden = self._encode_text(input_ids, attention_mask)   # encoder + enc_to_dec_proj + mask multiply, one CUDA graph
+        enc_hidden = enc_hidden.to(self.device, self.dtype)
+        if cross_prompt:
+            prompt = prompt_hidden_states if prompt_hidden_states is not None else prompt_input_ids
+            if prompt.dim() == 2 and not self._side_loaded:
+                raise ValueError("no embed_prompts weights loaded")
+            text = (enc_hidden.shape[1], prompt.shape[1], prompt_attention_mask)
+            enc_hidden, attention_mask = prompt_cross_states(enc_hidden, attention_mask, prompt, prompt_attention_mask,
+                                                             self.embed_prompts_weight, self.embed_positions_weight)
+            return enc_hidden, attention_mask, None, None, text, eo
+        prompt_hidden = prompt_hidden_states
+        if prompt_hidden is None and prompt_input_ids is not None:
+            if not self._side_loaded:
+                raise ValueError("no embed_prompts weights loaded")
+            prompt_hidden = torch.nn.functional.embedding(prompt_input_ids.to(self.device), self.embed_prompts_weight)
+        prompt_mask = prompt_attention_mask if prompt_hidden is not None else None
+        text = (0, 0 if prompt_hidden is None else prompt_hidden.shape[1], prompt_mask)
+        return enc_hidden, attention_mask, prompt_hidden, prompt_mask, text, eo
+
+    # -- the token loop ------------------------------------------------------------------------------
+    def _sampling(self, gc, n0: int, max_length: int, seed=0, suppress_special=False, row_base=0, logits_processor=None,
+                  stopping_criteria=None) -> Sampling:
+        """A generate() call's Sampling for n0 decoder input columns; resolve_sampling_ext / resolve_logits_ext raise here."""
+        d = self.config.decoder
+        ext, min_new_tokens = resolve_sampling_ext(gc, n0)
+        lext = resolve_logits_ext(gc, n0, max_length, d.vocab_size, d.eos_token_id)
+        return Sampling(max_length, gc.do_sample, gc.temperature, gc.top_k if gc.do_sample else 0, gc.top_p, min_new_tokens, seed,
+                        suppress_special, self.config.audio_encoder.codebook_size, row_base, ext, lext, list(logits_processor or []),
+                        list(stopping_criteria or []))
+
+    def _host_driven_loop(self, sess: "GenSession", s: Sampling, streamer, stream_col, outputs, out_row, window):
         """One host iteration per token, like GenerationMixin._sample: the decoder step still runs on the fused kernel
         (ptts_decode_forward), the built-in processors run as their device operators (MinNewTokens as a mask,
         ParlerTTSLogitsProcessor = ptts_logits_processor), then the caller's `logits_processor` list, the HF warpers and the draw
         as torch ops on the device scores, and the token is appended with ptts_sample(forced).  Used only when the caller passes
-        processors or criteria the device loop does not know (the reference merges such lists at :3540-3552).  `ext`
+        processors or criteria the device loop does not know (the reference merges such lists at :3540-3552).  `s.ext`
         (resolve_sampling_ext) adds the n-gram bans before the EOS masks and the MinP / Typical / Epsilon / Eta warpers after
-        top-p, in transformers' order; `lext` (resolve_logits_ext) adds sequence_bias first, forced BOS / EOS, InfNan, the decay
+        top-p, in transformers' order; `s.lext` (resolve_logits_ext) adds sequence_bias first, forced BOS / EOS, InfNan, the decay
         and the suppress lists before the Parler EOS processor, and LogitNormalization last (greedy's argmax and the draw use the
-        scores before it, as the device loop does).  `outputs` (StepOutputs) records each step's raw logits and final scores before the draw;
-        `probe_window(step)` (StepProbes) points the decoder's attention / hidden-state outputs at the next step's slot."""
+        scores before it, as the device loop does).  `outputs` (StepOutputs) records each step's raw logits and final scores
+        before the draw, from row out_row on; `window(step)` attaches the other recorders before each decoder step."""
         d = self.config.decoder
         K, BK = d.num_codebooks, sess.B * d.num_codebooks
+        ext, lext = s.ext, s.lext
         parler = ParlerTTSLogitsProcessor(d.eos_token_id, K, sess.B, self.device)
-        gen = torch.Generator(device=self.device).manual_seed(int(seed))
+        gen = torch.Generator(device=self.device).manual_seed(int(s.seed))
         unfinished = torch.ones(BK, dtype=torch.long, device=self.device)
         cur = sess.n0   # the first new column follows the decoder input (the BOS column, or BOS + code prefix)
         while True:
@@ -1440,22 +1536,22 @@ class ParlerTTSForConditionalGeneration:
                 scores = lext.sequence_bias(ids, scores)
             if ext is not None:
                 scores = no_repeat_ngram_mask(ids, scores, ext["no_repeat_ngram_size"])
-            if min_new_tokens > 0 and cur - sess.n0 < min_new_tokens:
+            if s.min_new_tokens > 0 and cur - sess.n0 < s.min_new_tokens:
                 scores[:, d.eos_token_id] = -float("inf")
             if lext is not None:
                 scores = lext.before_parler(ids, scores).contiguous()
             scores = parler(ids, scores)
-            for proc in user_processors:
+            for proc in s.processors:
                 scores = proc(ids, scores)
-            if gc.do_sample:
-                if gc.temperature and gc.temperature != 1.0:
-                    scores = scores / gc.temperature
-                if gc.top_k:
-                    kth = torch.topk(scores, min(int(gc.top_k), scores.shape[-1]))[0][..., -1, None]
+            if s.do_sample:
+                if s.temperature and s.temperature != 1.0:
+                    scores = scores / s.temperature
+                if s.top_k:
+                    kth = torch.topk(scores, min(int(s.top_k), scores.shape[-1]))[0][..., -1, None]
                     scores = scores.masked_fill(scores < kth, -float("inf"))
-                if gc.top_p is not None and gc.top_p < 1.0:
+                if s.top_p is not None and s.top_p < 1.0:
                     ss, si = torch.sort(scores, descending=False)
-                    rem = ss.softmax(-1).cumsum(-1) <= (1 - gc.top_p)
+                    rem = ss.softmax(-1).cumsum(-1) <= (1 - s.top_p)
                     rem[..., -1:] = False
                     scores = scores.masked_fill(rem.scatter(1, si, rem), -float("inf"))
                 if ext is not None:
@@ -1463,7 +1559,7 @@ class ParlerTTSForConditionalGeneration:
             final = scores if lext is None else lext.normalize(scores)   # what transformers' _sample records and passes on
             if outputs is not None:
                 outputs.put(cur - sess.n0, out_row, sess.logits, final)
-            if gc.do_sample:
+            if s.do_sample:
                 nxt = torch.multinomial(scores.softmax(-1), 1, generator=gen).squeeze(1)
             else:
                 nxt = scores.argmax(-1)
@@ -1472,20 +1568,17 @@ class ParlerTTSForConditionalGeneration:
             if streamer is not None:
                 streamer.put(stream_col(cur, nxt).cpu())
             cur += 1
-            unfinished = unfinished & ~((nxt == d.eos_token_id) | (cur >= max_length)).long()
+            unfinished = unfinished & ~((nxt == d.eos_token_id) | (cur >= s.max_length)).long()
             stop = unfinished.max().item() == 0
-            for crit in user_criteria:
+            for crit in s.criteria:
                 r = crit(sess.raw_ids[:, :cur], final)
                 r = r if isinstance(r, torch.Tensor) else torch.full((BK,), bool(r), device=self.device)
                 unfinished = unfinished & ~r.long()
                 stop = stop or unfinished.max().item() == 0
             if stop:
                 break
-            if probe_window is not None:
-                probe_window(cur - sess.n0)
+            window(cur - sess.n0)
             sess.decode_forward()
-        if streamer is not None:
-            streamer.end()
 
     def _fused_batch_limit(self):
         """Rows one fused decode-step launch covers (None: the fused kernels are not in play, the batch runs as one session)."""
@@ -1493,30 +1586,27 @@ class ParlerTTSForConditionalGeneration:
             return None
         return 32
 
-    def _run_token_loop(self, enc_hidden, attention_mask, prompt_hidden, prompt_mask, *, gc, max_length, seed, suppress_special, row_base,
-                        ext, min_new_tokens, lext=None, streamer=None, custom=None, input_ids=None, outputs=None, out_row=0, probes=None, takes=1,
-                        align=None):
-        """begin + prefill + the token loop of one session; returns the raw token matrix [B * K, generated length].
-        takes: the session's B rows are `takes` consecutive takes of each of the enc_hidden.shape[0] descriptions (B / takes);
-        prompt_hidden, prompt_mask and input_ids have B rows.
-        input_ids: None, or the BOS-led decoder input [B * K, n0] this shard continues from.
-        outputs: None, or the StepOutputs this session's rows (from row out_row of the batch) are recorded into.  The device
-        loop then sets the sampler's window before every call and keeps each call inside one chunk.
-        probes: None, or the StepProbes this session's attention weights / hidden states (from utterance out_row // K) go to;
-        its windows follow the same chunks, and the decode steps then run the multi-kernel path (ptts_generate_set_probes).
-        align: None, or the StepAlignment this session's utterances (from out_row // K) go to; one window spans the whole call."""
+    def _run_token_loop(self, enc_hidden, enc_mask, prompt_hidden, prompt_mask, input_ids, sampling: Sampling, shard, recorders=(),
+                        streamer=None):
+        """begin + prefill + the token loop of one shard's session -> its raw token matrix [rows * K, generated length].
+        The inputs are the whole call's: enc_hidden / enc_mask per description, prompt_hidden / prompt_mask per take, input_ids
+        None or the BOS-led decoder input [takes * K, n0].  shard: (first description, end, first take, end) (take_shards).
+        recorders (see recording): the device loop keeps each decode_steps call inside one chunk of those that have chunks."""
         d = self.config.decoder
-        K = d.num_codebooks
-        S = enc_hidden.shape[1]
-        B = enc_hidden.shape[0] * takes
+        K, s = d.num_codebooks, sampling
+        d0, d1, r0, r1 = shard
+        cut = lambda t, a, b: None if t is None else t[a:b]
+        enc_hidden, enc_mask = enc_hidden[d0:d1], cut(enc_mask, d0, d1)
+        prompt_hidden, prompt_mask, input_ids = cut(prompt_hidden, r0, r1), cut(prompt_mask, r0, r1), cut(input_ids, r0 * K, r1 * K)
+        B, S = r1 - r0, enc_hidden.shape[1]
         P = 0 if prompt_hidden is None else prompt_hidden.shape[1]
         n0 = 1 if input_ids is None else int(input_ids.shape[1])
-        sess = self.decoder.engine.session(B, P, S, P + max_length, max_input_len=n0, takes=takes)
-        sess.begin(max_length, do_sample=gc.do_sample, temperature=gc.temperature, top_k=gc.top_k if gc.do_sample else 0,
-                   top_p=gc.top_p, min_new_tokens=min_new_tokens, seed=seed, suppress_special=suppress_special,
-                   codebook_size=self.config.audio_encoder.codebook_size, row_base=row_base, input_ids=input_ids,
-                   ext=None if custom is not None else ext,    # the host-driven loop applies them as torch ops
-                   lext=None if custom is not None else lext)
+        sess = self.decoder.engine.session(B, P, S, P + s.max_length, max_input_len=n0, takes=B // (d1 - d0))
+        host = bool(s.processors or s.criteria)
+        sess.begin(s.max_length, do_sample=s.do_sample, temperature=s.temperature, top_k=s.top_k, top_p=s.top_p,
+                   min_new_tokens=s.min_new_tokens, seed=s.seed, suppress_special=s.suppress_special, codebook_size=s.codebook_size,
+                   row_base=s.row_base + r0 * K, input_ids=input_ids,
+                   ext=None if host else s.ext, lext=None if host else s.lext)    # the host-driven loop applies them as torch ops
         stream_col = lambda col, v: v
         if streamer is not None:
             if input_ids is None:
@@ -1525,65 +1615,45 @@ class ParlerTTSForConditionalGeneration:
                 streamer.put(sess.raw_ids[:, :n0].cpu())   # the whole delayed input first (:3534)
                 # Codebook k's prefix ids reach K-1 columns past the delayed input; generate()'s result takes them there
                 # (the pattern mask, :3586), so the streamed columns carry them too.
-                _, pm = build_delay_pattern_mask(input_ids, d.bos_token_id, d.pad_token_id, max_length, K)
+                _, pm = build_delay_pattern_mask(input_ids, d.bos_token_id, d.pad_token_id, s.max_length, K)
                 cells = pm[:, n0:n0 + K - 1]
                 stream_col = lambda col, v: (torch.where(cells[:, col - n0] == -1, v, cells[:, col - n0]) if col - n0 < cells.shape[1] else v)
-        align_buf = None
-        try:
-            if align is not None:
-                align_buf = align.set(sess)
-            if probes is not None:
-                probes.set_prefill(sess, out_row // K)
-            sess.prefill(prompt_hidden, prompt_mask, enc_hidden, attention_mask)
-            probe_window = (lambda step: probes.set_window(sess, step, out_row // K)) if probes is not None else None
+        # The host-driven loop draws the token in torch and copies the outputs from there (StepOutputs.put): the sampler records
+        # none, so only the other recorders get windows.
+        outputs = next((r for r in recorders if isinstance(r, StepOutputs)), None) if host else None
+        windows = [r for r in recorders if r is not outputs]
 
-            def window(step):
-                if outputs is not None:
-                    outputs.set_window(sess, step, out_row)
-                if probe_window is not None and step > 0:
-                    probe_window(step)
-            if custom is not None:
-                self._host_driven_loop(sess, gc, max_length, custom[0], custom[1], streamer, seed, stream_col, ext, min_new_tokens,
-                                       outputs, out_row, probe_window, lext)
-            elif streamer is not None:
-                window(0)
-                sess.sample()
-                steps_left = max_length - n0 - 1
-                # the streamer contract is one host-visible token column per step (_sample -> streamer.put(next.cpu()))
-                col = n0
-                streamer.put(stream_col(col, sess.raw_ids[:, col]).cpu())
-                while steps_left > 0 and int(sess.state[1].item()) == 1:
-                    window(col + 1 - n0)
-                    sess.decode_steps(1)
-                    col += 1
-                    steps_left -= 1
-                    streamer.put(stream_col(col, sess.raw_ids[:, col]).cpu())
-                streamer.end()
+        def window(step):
+            for r in windows:
+                r.attach_window(sess, step, r0)
+        with recording(sess, recorders, r0):
+            sess.prefill(prompt_hidden, prompt_mask, enc_hidden, enc_mask)
+            if host:
+                self._host_driven_loop(sess, s, streamer, stream_col, outputs, r0 * K, window)
             else:
                 window(0)
                 sess.sample()
-                steps_left = max_length - n0 - 1
-                # no per-step host sync: enqueue graph replays in chunks and poll the device `active` flag between chunks
-                chunk = 64
-                step = 1
+                step, steps_left = 1, s.max_length - n0 - 1
+                chunked = any(r.CHUNK for r in windows)
+                if streamer is not None:
+                    streamer.put(stream_col(n0, sess.raw_ids[:, n0]).cpu())
+                # Without a streamer there is no per-step host sync: decode_steps enqueues up to 64 tokens (one cluster kernel
+                # launch) and the device `active` flag is read between calls.  A streamer gets one host-visible column per step
+                # (_sample -> streamer.put(next.cpu())), and none after the session went inactive.
                 while steps_left > 0:
-                    n = min(chunk, steps_left) if outputs is None and probes is None else steps_in_window(step, steps_left, StepOutputs.CHUNK)
+                    if streamer is not None and int(sess.state[1].item()) != 1:
+                        break
+                    n = 1 if streamer is not None else steps_in_window(step, steps_left, StepOutputs.CHUNK) if chunked else min(64, steps_left)
                     window(step)
                     sess.decode_steps(n)
-                    steps_left -= n
-                    step += n
-                    if steps_left > 0 and int(sess.state[1].item()) == 0:
+                    step, steps_left = step + n, steps_left - n
+                    if streamer is not None:
+                        streamer.put(stream_col(n0 + step - 1, sess.raw_ids[:, n0 + step - 1]).cpu())
+                    elif steps_left > 0 and int(sess.state[1].item()) == 0:
                         break
-        finally:
-            if probes is not None:
-                sess.set_probes()   # the session keeps no window (nor the chunks) past this call, whatever happens in it
-            if align_buf is not None:
-                sess.set_alignment()
-        if align_buf is not None:
-            align.put(align_buf, out_row // K)
+            if streamer is not None:
+                streamer.end()
         cur_len = int(sess.state[0].item())
-        if outputs is not None:
-            sess.set_outputs(None, None)   # the session keeps no reference to the chunks
         return sess.raw_ids[:, :cur_len].clone()
 
     def _token_timestamps(self, align: StepAlignment, raw_ids: torch.Tensor, n0: int, text_mask, takes: int) -> dict:
@@ -1636,39 +1706,15 @@ class ParlerTTSForConditionalGeneration:
                 raise ValueError("forward(input_values=...) without labels or decoder_input_ids: encode the audio with "
                                  "audio_encoder.encode(...) and pass its codes as decoder_input_ids")
             raise ValueError("forward() needs `labels` or `decoder_input_ids`")
-        cross_prompt = self.prompt_cross_attention and (prompt_input_ids is not None or prompt_hidden_states is not None)
-        if encoder_outputs is not None:
-            if cross_prompt:
-                # the reference would make the prompt a self-attention prefix without positions: the other model
-                raise ValueError("a prompt_cross_attention model joins the prompt to the description only when forward() runs the "
-                                 "text encoder: pass `input_ids` instead of `encoder_outputs`, or no prompt")
-            enc = encoder_outputs
-            enc_hidden = enc[0] if isinstance(enc, (tuple, list)) else getattr(enc, "last_hidden_state", enc)
-        else:
-            if input_ids is None:
-                raise ValueError("forward() needs `input_ids` (description) or `encoder_outputs`")
-            enc_hidden = self._encode_text(input_ids, attention_mask)
-        enc_hidden = enc_hidden.to(self.device, self.dtype)
-        if cross_prompt:
-            # the prompt joins the description as cross-attention keys (:2791-2811); the decoder then has no prompt prefix
-            prompt = prompt_hidden_states if prompt_hidden_states is not None else prompt_input_ids
-            if prompt.dim() == 2 and not self._side_loaded:
-                raise ValueError("no embed_prompts weights loaded")
-            enc_hidden, attention_mask = prompt_cross_states(enc_hidden, attention_mask, prompt, prompt_attention_mask,
-                                                             self.embed_prompts_weight, self.embed_positions_weight)
-            prompt_input_ids = prompt_hidden_states = prompt_attention_mask = None
+        enc_hidden, attention_mask, prompt_hidden, prompt_mask, _, _ = self._conditioning(
+            "forward", input_ids, attention_mask, encoder_outputs, prompt_input_ids, prompt_attention_mask, prompt_hidden_states,
+            cross_prompt_after_encoder_outputs=False)
         if enc_hidden.dim() != 3 or enc_hidden.shape[2] != self.config.decoder.hidden_size:
             raise ValueError(f"encoder states must be [batch, length, {self.config.decoder.hidden_size}], got {tuple(enc_hidden.shape)}")
         B, S, _ = enc_hidden.shape
         if attention_mask is not None and tuple(attention_mask.shape) != (B, S):
             raise ValueError(f"attention_mask must be [{B}, {S}], got {tuple(attention_mask.shape)}")
-        prompt_hidden = prompt_hidden_states
-        if prompt_hidden is None and prompt_input_ids is not None:
-            if not self._side_loaded:
-                raise ValueError("no embed_prompts weights loaded")
-            prompt_hidden = torch.nn.functional.embedding(prompt_input_ids.to(self.device), self.embed_prompts_weight)
         P = 0 if prompt_hidden is None else prompt_hidden.shape[1]
-        prompt_mask = prompt_attention_mask if prompt_hidden is not None else None
         if prompt_hidden is not None and (prompt_hidden.dim() != 3 or prompt_hidden.shape[0] != B):
             raise ValueError(f"prompt states must be [{B}, P, H], got {tuple(prompt_hidden.shape)}")
         if prompt_mask is not None and tuple(prompt_mask.shape) != (B, P):
@@ -1694,15 +1740,10 @@ class ParlerTTSForConditionalGeneration:
         for i, b0 in enumerate(range(0, B, self._SCORE_SHARD)):
             sl = slice(b0, min(B, b0 + self._SCORE_SHARD))
             sess = self.decoder.engine.session(sl.stop - sl.start, P, S, P + T, max_input_len=T)
-            try:
-                if probes is not None:
-                    probes.set_prefill(sess, b0)
+            with recording(sess, [] if probes is None else [probes], b0):
                 sess.score(cut(prompt_hidden, sl), cut(prompt_mask, sl), enc_hidden[sl], cut(attention_mask, sl),
                            dec[sl.start * K:sl.stop * K], cut(labels, sl), cut(token_nll, sl),
                            None if logits is None else logits[sl.start * K:sl.stop * K], None if sums is None else sums[i])
-            finally:
-                if probes is not None:
-                    sess.set_probes()   # the cached session keeps no window (nor a reference to the buffers) past this call
         loss = per_codebook = None
         if labels is not None:
             # per codebook: sum (and count) over the shards, then the reference's reduction; a mean over no cell is NaN as in torch
@@ -1808,46 +1849,16 @@ class ParlerTTSForConditionalGeneration:
         if self.prompt_cross_attention and mk.get("prompt_hidden_states") is not None:
             # the reference would put these states in front of the decoder while counting its cache positions without them
             raise ValueError("a prompt_cross_attention model takes the transcript as `prompt_input_ids`, not `prompt_hidden_states`")
-        custom_loop = bool(logits_processor) or bool(stopping_criteria)   # merged with the built-in ones like :3540-3552
-        input_ids = mk.get("input_ids", inputs)
-        attention_mask = mk.get("attention_mask")
-        enc = mk.get("encoder_outputs")
-        if enc is not None:
-            enc_hidden = enc[0] if isinstance(enc, (tuple, list)) else getattr(enc, "last_hidden_state", enc)
-        else:
-            if input_ids is None:
-                raise ValueError("generate() needs `input_ids` (description) or `encoder_outputs`")
-            enc_hidden = None
         # decoder_attentions / cross_attentions / decoder_hidden_states exist only in the dict return, as in transformers
         want_attn = bool(gc.return_dict_in_generate and gc.output_attentions)
         want_hidden = bool(gc.return_dict_in_generate and gc.output_hidden_states)
-        enc_probe = {}
-        if enc_hidden is None and (want_attn or want_hidden):   # the encoder's own tuples: one eager call with the flags
-            enc_hidden, eo = self._encode_text_eager(input_ids, attention_mask, dict(output_attentions=want_attn,
-                                                                                     output_hidden_states=want_hidden))
-            enc_probe = dict(encoder_attentions=getattr(eo, "attentions", None) if want_attn else None,
-                             encoder_hidden_states=getattr(eo, "hidden_states", None) if want_hidden else None)
-        elif enc_hidden is None:
-            enc_hidden = self._encode_text(input_ids, attention_mask)   # encoder + enc_to_dec_proj + mask multiply, one CUDA graph
-        enc_hidden = enc_hidden.to(self.device, self.dtype)
-        prompt_hidden = mk.get("prompt_hidden_states")
-        text_key0, text_len, text_mask = 0, 0, None   # the transcript keys token timestamps align to
-        if self.prompt_cross_attention and mk.get("prompt_input_ids") is not None:
-            # the prompt joins the description as cross-attention keys (:3099-3130); everything below runs with P = 0
-            if not self._side_loaded:
-                raise ValueError("no embed_prompts weights loaded")
-            text_key0, text_len, text_mask = enc_hidden.shape[1], mk["prompt_input_ids"].shape[1], mk.get("prompt_attention_mask")
-            enc_hidden, attention_mask = prompt_cross_states(enc_hidden, attention_mask, mk["prompt_input_ids"], mk.get("prompt_attention_mask"),
-                                                             self.embed_prompts_weight, self.embed_positions_weight)
-        elif prompt_hidden is None and mk.get("prompt_input_ids") is not None:
-            if not self._side_loaded:
-                raise ValueError("no embed_prompts weights loaded")
-            prompt_hidden = torch.nn.functional.embedding(mk["prompt_input_ids"].to(self.device), self.embed_prompts_weight)
-        prompt_mask = mk.get("prompt_attention_mask") if prompt_hidden is not None else None
+        enc_hidden, attention_mask, prompt_hidden, prompt_mask, (text_key0, text_len, text_mask), eo = self._conditioning(
+            "generate", mk.get("input_ids", inputs), mk.get("attention_mask"), mk.get("encoder_outputs"), mk.get("prompt_input_ids"),
+            mk.get("prompt_attention_mask"), mk.get("prompt_hidden_states"), cross_prompt_after_encoder_outputs=True,
+            # the encoder's own tuples: one eager call with the flags
+            encoder_flags=dict(output_attentions=want_attn, output_hidden_states=want_hidden) if want_attn or want_hidden else None)
         P = 0 if prompt_hidden is None else prompt_hidden.shape[1]
         B, S, _ = enc_hidden.shape
-        if P > 0:
-            text_len, text_mask = P, prompt_mask
         if want_ts and text_len == 0:
             raise ValueError("`return_token_timestamps=True` needs a transcript to align: pass `prompt_input_ids` or "
                              "`prompt_hidden_states` with at least one token")
@@ -1888,41 +1899,28 @@ class ParlerTTSForConditionalGeneration:
             raise ValueError(f"max_length must allow at least one new token, got {max_length}")
         if dec_ids is not None:
             check_continuation_length(n0, P, max_length, d.max_position_embeddings)
-        ext, min_new_tokens = resolve_sampling_ext(gc, n0)
-        lext = resolve_logits_ext(gc, n0, max_length, d.vocab_size, d.eos_token_id)   # its device tables serve every shard
-        run = dict(gc=gc, max_length=max_length, seed=seed, suppress_special=suppress_special, ext=ext, min_new_tokens=min_new_tokens,
-                   lext=lext)
+        # the caller's processors / criteria are merged with the built-in ones like :3540-3552, on the host-driven loop
+        sampling = self._sampling(gc, n0, max_length, seed, suppress_special, row_base, logits_processor, stopping_criteria)
         # output_scores / output_logits exist only in the dict return, as in transformers; without it nothing is recorded
         want_scores = bool(gc.return_dict_in_generate and gc.output_scores)
         want_logits = bool(gc.return_dict_in_generate and gc.output_logits)
         BN = B * N
         outputs = StepOutputs(BN * K, d.vocab_size, self.device, want_scores, want_logits) if (want_scores or want_logits) else None
-        probes = None
-        if want_attn or want_hidden:
-            probes = StepProbes(d.num_hidden_layers, BN, d.num_attention_heads, S, d.hidden_size, P, n0, self.dtype, self.device,
-                                want_attn, want_hidden)
-        if want_ts:
-            run["align"] = StepAlignment(align_heads, BN, max_length - n0, text_key0, text_len, self.device)
-        limit = self._fused_batch_limit()
-        if limit is not None and BN > limit and not custom_loop and streamer is None:
-            # The fused decode-step kernels hold one 32-row tile: a larger batch runs as consecutive shards of <= 32 rows through the
-            # same session, each whole groups of takes (take_shards).  The result is the one the whole batch would give: the Philox
-            # draw is keyed by the global row (row_base), the processors' state is per utterance, and a finished utterance emits pad
-            # ids until the longest one ends.
-            parts = []
-            for d0, d1, r0, r1 in take_shards(B, N, limit):
-                rs = slice(r0, r1)
-                parts.append(self._run_token_loop(enc_hidden[d0:d1], None if attention_mask is None else attention_mask[d0:d1],
-                                                  None if prompt_hidden is None else prompt_hidden[rs],
-                                                  None if prompt_mask is None else prompt_mask[rs], row_base=row_base + r0 * K,
-                                                  input_ids=None if dec_ids is None else dec_ids[r0 * K:r1 * K],
-                                                  outputs=outputs, out_row=r0 * K, probes=probes, takes=(r1 - r0) // (d1 - d0), **run))
+        probes = StepProbes(d.num_hidden_layers, BN, d.num_attention_heads, S, d.hidden_size, P, n0, self.dtype, self.device, want_attn,
+                            want_hidden) if want_attn or want_hidden else None
+        align = StepAlignment(align_heads, BN, max_length - n0, text_key0, text_len, self.device) if want_ts else None
+        recorders = [r for r in (outputs, align, probes) if r is not None]
+        # The fused decode-step kernels hold one 32-row tile: a larger batch runs as consecutive shards of <= 32 rows through the
+        # same session, each whole groups of takes (take_shards).  The result is the one the whole batch would give: the Philox
+        # draw is keyed by the global row (row_base), the processors' state is per utterance, and a finished utterance emits pad
+        # ids until the longest one ends.  The host-driven loop and a streamer run the batch as one session.
+        limit = None if sampling.processors or sampling.criteria or streamer is not None else self._fused_batch_limit()
+        parts = [self._run_token_loop(enc_hidden, attention_mask, prompt_hidden, prompt_mask, dec_ids, sampling, shard, recorders, streamer)
+                 for shard in take_shards(B, N, limit)]
+        output_ids = parts[0]
+        if len(parts) > 1:
             n = max(t.shape[1] for t in parts)
             output_ids = torch.cat([torch.nn.functional.pad(t, (0, n - t.shape[1]), value=d.pad_token_id) for t in parts], dim=0)
-        else:
-            output_ids = self._run_token_loop(enc_hidden, attention_mask, prompt_hidden, prompt_mask, row_base=row_base, streamer=streamer,
-                                              custom=(logits_processor or [], stopping_criteria or []) if custom_loop else None,
-                                              input_ids=dec_ids, outputs=outputs, probes=probes, takes=N, **run)
         B = BN   # from here on the batch is the B * N takes
 
         # apply the stashed delay mask, then keep only the free cells (:3586-3597); both masks come from the whole decoder input,
@@ -1955,11 +1953,11 @@ class ParlerTTSForConditionalGeneration:
             if probes is not None:
                 out.update(probes.result(output_ids.shape[1] - n0))
                 if want_attn:
-                    out.update(encoder_attentions=enc_probe.get("encoder_attentions"))
+                    out.update(encoder_attentions=getattr(eo, "attentions", None))
                 if want_hidden:
-                    out.update(encoder_hidden_states=enc_probe.get("encoder_hidden_states"))
+                    out.update(encoder_hidden_states=getattr(eo, "hidden_states", None))
             if want_ts:
-                out.update(self._token_timestamps(run["align"], output_ids, n0, text_mask, N))
+                out.update(self._token_timestamps(align, output_ids, n0, text_mask, N))
             if gc.return_dict_in_generate:
                 return out
             return output_values, out

@@ -37,7 +37,7 @@ def main():
     from oracle.config import mini_cfg, tiny_dac_cfg
     from oracle.weights import make_dac_weights, make_decoder_weights
     from parler_tts_b200.configuration import GenerationConfig
-    from parler_tts_b200.modeling import StepOutputs, resolve_sampling_ext
+    from parler_tts_b200.modeling import StepOutputs
     from tests.helpers import build_product_model, synth_inputs
     cfg = mini_cfg()
     w = make_decoder_weights(cfg, seed=1, head_std=0.1)
@@ -55,11 +55,10 @@ def main():
     def codes_only(extra, outputs):
         # generate()'s token loop without the DAC decode; with outputs, the storage generate() would pass
         gc = GenerationConfig(**{k: v for k, v in {**base, **extra}.items() if k in GenerationConfig().__dict__})
-        ext, mnt = resolve_sampling_ext(gc, 1)
         rec = StepOutputs(B * K, V, model.device, True, True) if outputs else None
         ids = model._run_token_loop(base["encoder_outputs"][0], base["attention_mask"], base["prompt_hidden_states"],
-                                    base["prompt_attention_mask"], gc=gc, max_length=L, seed=1, suppress_special=False, row_base=0,
-                                    ext=ext, min_new_tokens=mnt, outputs=rec)
+                                    base["prompt_attention_mask"], None, model._sampling(gc, 1, L, seed=1), (0, B, 0, B),
+                                    [rec] if outputs else [])
         return ids, rec
 
     gpu = card()

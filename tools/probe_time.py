@@ -36,7 +36,7 @@ def main():
     from oracle.config import mini_cfg, tiny_dac_cfg
     from oracle.weights import make_dac_weights, make_decoder_weights
     from parler_tts_b200.configuration import GenerationConfig
-    from parler_tts_b200.modeling import StepProbes, resolve_sampling_ext
+    from parler_tts_b200.modeling import StepProbes
     from tests.helpers import build_product_model, synth_inputs
     cfg = mini_cfg()
     w = make_decoder_weights(cfg, seed=1, head_std=0.1)
@@ -51,8 +51,7 @@ def main():
         enc, em, prompt, pm = synth_inputs(cfg, B, S, P, seed=0)
         enc, prompt = enc.cuda().bfloat16(), prompt.cuda().bfloat16()
         em, pm = em.cuda(), pm.cuda()
-        gc = GenerationConfig(do_sample=True, top_k=50, max_length=L, min_new_tokens=steps)
-        ext, mnt = resolve_sampling_ext(gc, 1)
+        sampling = model._sampling(GenerationConfig(do_sample=True, top_k=50, max_length=L, min_new_tokens=steps), 1, L, seed=1)
 
         def loop(mode):
             probe = mode == "probes"
@@ -61,8 +60,7 @@ def main():
             rec = StepProbes(cfg.num_hidden_layers, B, cfg.num_attention_heads, S, cfg.hidden_size, P, 1, torch.bfloat16,
                              model.device, True, True) if probe else None
             try:
-                ids = model._run_token_loop(enc, em, prompt, pm, gc=gc, max_length=L, seed=1, suppress_special=False, row_base=0,
-                                            ext=ext, min_new_tokens=mnt, probes=rec)
+                ids = model._run_token_loop(enc, em, prompt, pm, None, sampling, (0, B, 0, B), [rec] if probe else [])
             finally:
                 os.environ.pop("PTTS_FUSED", None)
             return ids, rec

@@ -55,12 +55,9 @@ def main():
     def codes_only(extra):
         # generate()'s token loop without the DAC decode: the part the processors change
         from parler_tts_b200.configuration import GenerationConfig
-        from parler_tts_b200.modeling import resolve_sampling_ext
         gc = GenerationConfig(**{k: v for k, v in {**base, **extra}.items() if k in GenerationConfig().__dict__})
-        ext, mnt = resolve_sampling_ext(gc, 1)
         return model._run_token_loop(base["encoder_outputs"][0], base["attention_mask"], base["prompt_hidden_states"],
-                                     base["prompt_attention_mask"], gc=gc, max_length=L, seed=1, suppress_special=False, row_base=0,
-                                     ext=ext, min_new_tokens=mnt)
+                                     base["prompt_attention_mask"], None, model._sampling(gc, 1, L, seed=1), (0, B, 0, B))
 
     gpu = card()
     print(f"card: {gpu}")

@@ -38,7 +38,7 @@ def main():
     from oracle.config import mini_cfg, tiny_dac_cfg
     from oracle.weights import make_dac_weights, make_decoder_weights
     from parler_tts_b200.configuration import GenerationConfig
-    from parler_tts_b200.modeling import StepAlignment, align_dtw, resolve_alignment_heads, resolve_sampling_ext
+    from parler_tts_b200.modeling import StepAlignment, align_dtw, resolve_alignment_heads
     from tests.helpers import build_product_model, synth_inputs
     cfg = mini_cfg()
     w = make_decoder_weights(cfg, seed=1, head_std=0.1)
@@ -53,16 +53,14 @@ def main():
     rows = []
     for steps in (256, 1024):
         L = steps + 1
-        gc = GenerationConfig(do_sample=True, top_k=50, max_length=L, min_new_tokens=steps)
-        ext, mnt = resolve_sampling_ext(gc, 1)
+        sampling = model._sampling(GenerationConfig(do_sample=True, top_k=50, max_length=L, min_new_tokens=steps), 1, L, seed=1)
 
         def loop(mode):
             if mode == "multi":
                 os.environ["PTTS_FUSED"] = "0"   # read when the session picks its path at the prefill
             rec = StepAlignment(heads, B, L - 1, 0, P, model.device) if mode == "align" else None
             try:
-                ids = model._run_token_loop(enc, em, prompt, pm, gc=gc, max_length=L, seed=1, suppress_special=False, row_base=0,
-                                            ext=ext, min_new_tokens=mnt, align=rec)
+                ids = model._run_token_loop(enc, em, prompt, pm, None, sampling, (0, B, 0, B), [] if rec is None else [rec])
             finally:
                 os.environ.pop("PTTS_FUSED", None)
             return ids, rec
