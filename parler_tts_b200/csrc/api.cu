@@ -1,5 +1,5 @@
 // api.cu -- the C ABI (include/ptts_b200.h): argument validation, weight packing, the generation
-// session (prefill / decode step / sample / CUDA-graph replay) and DAC decode / encode orchestration.
+// session (prefill / decode step / sample / CUDA-graph replay); the DAC entry points call the codec walks of dac.cu / dac_enc.cu.
 #include <cstdarg>
 #include <cstdlib>
 #include <cstring>
@@ -145,11 +145,10 @@ int ptts_decoder_pack(const ptts_decoder_config* cfg, void* blob, int32_t tensor
   if (per_layer) PTTS_REQUIRE(index >= 0 && index < L.L, "pack: layer %d out of range", index);
   if (matrix_slot(L, tensor_id, index, &ms)) {
     if (tensor_id == PTTS_T_LM_HEAD) PTTS_REQUIRE(index >= 0 && index < L.K, "pack: codebook %d out of range", index);
-    PTTS_REQUIRE(cols == ms.K, "pack: tensor %d expects %d columns, got %lld", tensor_id, ms.K, (long long)cols);
-    PTTS_REQUIRE(rows > 0 && ms.row_off + rows <= ms.N, "pack: tensor %d rows %lld do not fit fused matrix of %d rows", tensor_id, (long long)rows, ms.N);
-    return pack_matrix(src, src_dtype, rows, cols, ms.row_off, ms.K, base + ms.off, cfg->dtype, st);
+    PTTS_REQUIRE(cols == ms.m.K, "pack: tensor %d expects %d columns, got %lld", tensor_id, ms.m.K, (long long)cols);
+    PTTS_REQUIRE(rows > 0 && ms.row_off + rows <= ms.m.N, "pack: tensor %d rows %lld do not fit fused matrix of %d rows", tensor_id, (long long)rows, ms.m.N);
+    return pack_matrix(src, src_dtype, rows, cols, ms.row_off, ms.m.K, base + ms.m.w, cfg->dtype, st);
   }
-  const int64_t lb = L.layer0 + L.layer_stride * index;
   const int H = L.H;
   switch (tensor_id) {
     case PTTS_T_EMBED_TOKENS:
@@ -162,22 +161,14 @@ int ptts_decoder_pack(const ptts_decoder_config* cfg, void* blob, int32_t tensor
     case PTTS_T_ROPE_SIN:
       PTTS_REQUIRE(cfg->rope && rows == cfg->max_positions && cols == PTTS_HEAD_DIM, "pack: rope table shape");
       return pack_plain(src, src_dtype, rows * cols, base + (tensor_id == PTTS_T_ROPE_COS ? L.rope_cos : L.rope_sin), cfg->dtype, st);
-    case PTTS_T_LN1_W: case PTTS_T_LN1_B: case PTTS_T_LN2_W: case PTTS_T_LN2_B: case PTTS_T_LN3_W: case PTTS_T_LN3_B: {
+    case PTTS_T_LN1_W: case PTTS_T_LN1_B: case PTTS_T_LN2_W: case PTTS_T_LN2_B: case PTTS_T_LN3_W: case PTTS_T_LN3_B:
+    case PTTS_T_FINAL_LN_W: case PTTS_T_FINAL_LN_B: {   // the LayerNorm in front of a matrix
       PTTS_REQUIRE(rows * cols == H, "pack: LayerNorm parameter must have %d elements", H);
-      const int64_t off[6] = {L.ln1_w, L.ln1_b, 0, 0, 0, 0};
-      (void)off;
-      int64_t o = 0;
-      switch (tensor_id) {
-        case PTTS_T_LN1_W: o = L.ln1_w; break; case PTTS_T_LN1_B: o = L.ln1_b; break;
-        case PTTS_T_LN2_W: o = L.ln2_w; break; case PTTS_T_LN2_B: o = L.ln2_b; break;
-        case PTTS_T_LN3_W: o = L.ln3_w; break; default: o = L.ln3_b; break;
-      }
-      return pack_plain(src, src_dtype, H, base + lb + o, PTTS_F32, st);
+      const int m = tensor_id <= PTTS_T_LN1_B ? MAT_QKV : tensor_id <= PTTS_T_LN2_B ? MAT_Q_CROSS : tensor_id <= PTTS_T_LN3_B ? MAT_FC1 : MAT_HEADS;
+      const DecoderMatrix dm = decoder_matrix(L, m, index);
+      const bool gamma = tensor_id == PTTS_T_LN1_W || tensor_id == PTTS_T_LN2_W || tensor_id == PTTS_T_LN3_W || tensor_id == PTTS_T_FINAL_LN_W;
+      return pack_plain(src, src_dtype, H, base + (gamma ? dm.ln_w : dm.ln_b), PTTS_F32, st);
     }
-    case PTTS_T_FINAL_LN_W:
-    case PTTS_T_FINAL_LN_B:
-      PTTS_REQUIRE(rows * cols == H, "pack: LayerNorm parameter must have %d elements", H);
-      return pack_plain(src, src_dtype, H, base + (tensor_id == PTTS_T_FINAL_LN_W ? L.final_ln_w : L.final_ln_b), PTTS_F32, st);
     default:
       return fail(PTTS_EINVAL, "pack: unknown tensor id %d", tensor_id);
   }
@@ -190,26 +181,17 @@ int ptts_decoder_finalize(const ptts_decoder_config* cfg, void* blob, void* stre
   const DecoderLayout L = make_layout(*cfg);
   cudaStream_t st = (cudaStream_t)stream;
   char* b = (char*)blob;
-  for (int i = 0; i < L.L; i++) {
-    char* lb = b + L.layer0 + L.layer_stride * i;
-    float* cq = (float*)(lb + L.c_qkv);
-    if (int e = fold_layernorm(lb + L.wqkv, L.qkv_rows, L.H, (const float*)(lb + L.ln1_w), (const float*)(lb + L.ln1_b), cq, cq + L.qkv_rows, st)) return e;
-    float* cc = (float*)(lb + L.c_qc);
-    if (int e = fold_layernorm(lb + L.wqc, L.H, L.H, (const float*)(lb + L.ln2_w), (const float*)(lb + L.ln2_b), cc, cc + L.H, st)) return e;
-    float* cf = (float*)(lb + L.c_fc1);
-    if (int e = fold_layernorm(lb + L.fc1, L.F, L.H, (const float*)(lb + L.ln3_w), (const float*)(lb + L.ln3_b), cf, cf + L.F, st)) return e;
-  }
-  float* ch = (float*)(b + L.c_heads);
-  if (int e = fold_layernorm(b + L.heads, L.K * L.V, L.H, (const float*)(b + L.final_ln_w), (const float*)(b + L.final_ln_b), ch, ch + L.K * L.V, st)) return e;
-  {  // row-major copies for the wgmma prefill GEMM (gemm_tc.cu), unpacked AFTER the LayerNorm fold
-    const struct { int64_t off; int64_t N; int K; } mats[7] = {{L.wqkv, L.qkv_rows, L.H}, {L.wo, L.H, L.H}, {L.wqc, L.H, L.H}, {L.wkvc, L.ckv_rows, L.H},
-                                                               {L.woc, L.H, L.H}, {L.fc1, L.F, L.H}, {L.fc2, L.H, L.F}};
-    for (int i = 0; i < L.L; i++) {
-      char* lb = b + L.layer0 + L.layer_stride * i;
-      for (int m = 0; m < 7; m++)
-        if (int e = unpack_fragments(lb + mats[m].off, lb + L.rm[m], mats[m].N, mats[m].K, st)) return e;
+  for (int m = 0; m < MAT_COUNT; m++)
+    for (int i = 0; i < (m == MAT_HEADS ? 1 : L.L); i++) {
+      const DecoderMatrix d = decoder_matrix(L, m, i);
+      if (d.ln_w >= 0) {
+        float* c = (float*)(b + d.c);
+        if (int e = fold_layernorm(b + d.w, d.N, d.K, (const float*)(b + d.ln_w), (const float*)(b + d.ln_b), c, c + d.N, st)) return e;
+      }
+      // the row-major copy for the wgmma prefill GEMM (gemm_tc.cu) is unpacked after the fold
+      if (d.rm >= 0)
+        if (int e = unpack_fragments(b + d.w, b + d.rm, d.N, d.K, st)) return e;
     }
-  }
   if (L.cl_NC > 0) {  // second copy of the layer matrices, sliced per (phase, cluster, rank) for the cluster step kernel (step2.cu)
     for (int i = 0; i < L.L; i++)
       if (int e = cluster_pack_layer(L, b + L.layer0 + L.layer_stride * i, st)) return e;
@@ -515,17 +497,6 @@ int ptts_generate_set_alignment(ptts_session* s, const int32_t* heads, int32_t n
   return PTTS_OK;
 }
 
-// Blob offset of the row-major copy (layout.h rm[]) of the layer matrix stored at blob offset woff, which the wgmma GEMM
-// (gemm_tc.cu) reads; -1 when there is none (f32 model dtype, or not a layer matrix: the lm heads).
-static int64_t rowmajor_offset(const DecoderLayout& L, int64_t woff) {
-  if (L.es != 2 || woff < L.layer0 || woff >= L.layer0 + L.layer_stride * L.L) return -1;
-  const int64_t in_layer = (woff - L.layer0) % L.layer_stride, lbase = woff - in_layer;
-  const int64_t frag[7] = {L.wqkv, L.wo, L.wqc, L.wkvc, L.woc, L.fc1, L.fc2};
-  for (int m = 0; m < 7; m++)
-    if (in_layer == frag[m]) return lbase + L.rm[m];
-  return -1;
-}
-
 // one decoder pass over q_len new positions per batch row (q_len = P+n0 at prefill, 1 at decode); heads == false stops after
 // the last layer and leaves the residual stream x [B][q_len][H] for the caller (ptts_score)
 static int run_forward(ptts_session* s, cudaStream_t st, bool prefill, const void* prompt_hidden, const void* enc_hidden,
@@ -613,42 +584,41 @@ static int run_forward(ptts_session* s, cudaStream_t st, bool prefill, const voi
     return launch_alignment_probe(g, c.dtype, st);
   };
 
+  // matrix `mat` of layer `layer` (decoder_matrix), with the LayerNorm in front of it where it has one.
   // plan_rows: the row count that picks the kernel (default Mrows); the GEMMs' per-row results do not depend on M otherwise
-  auto lin = [&](const void* X, int64_t ldx, int64_t woff, int N, int K, const float* lw, const float* lb, int epi,
-                 const void* R, void* Y, int64_t ldy, int Mrows, int64_t coff = -1, int plan_rows = 0) -> int {
+  auto lin = [&](const void* X, int64_t ldx, int mat, int layer, int epi, const void* R, void* Y, int64_t ldy, int Mrows,
+                 int plan_rows = 0) -> int {
+    const DecoderMatrix m = decoder_matrix(L, mat, layer);
     LinearArgs a{};
-    a.X = X; a.ldx = ldx; a.W = blob + woff; a.Y = Y; a.ldy = ldy; a.R = R; a.ldr = ldy;
-    a.ln_w = lw; a.ln_b = lb; a.eps = c.layer_norm_eps;
-    if (lw != nullptr && c.dtype == PTTS_BF16) {  // bf16: LayerNorm folded into the weights at load (ptts_decoder_finalize)
-      a.c1 = (const float*)(blob + coff); a.c2 = a.c1 + N;
+    a.X = X; a.ldx = ldx; a.W = blob + m.w; a.Y = Y; a.ldy = ldy; a.R = R; a.ldr = ldy;
+    a.eps = c.layer_norm_eps;
+    if (m.ln_w >= 0) {
+      a.ln_w = (const float*)(blob + m.ln_w); a.ln_b = (const float*)(blob + m.ln_b);
+      if (c.dtype == PTTS_BF16) { a.c1 = (const float*)(blob + m.c); a.c2 = a.c1 + m.N; }   // folded at load (ptts_decoder_finalize)
     }
-    a.M = Mrows; a.N = N; a.K = K; a.Kc = (K > H && K % H == 0) ? H : K;
+    a.M = Mrows; a.N = m.N; a.K = m.K; a.Kc = (m.K > H && m.K % H == 0) ? H : m.K;
     a.epi = epi; a.act = c.activation; a.ctrl = ctrl;
     s->launches++;
     // the same matrix, row-major: M = B*(P+n0) or B*S rows are tensor-core work (wgmma, gemm_tc.cu)
-    const int64_t rm = prefill ? rowmajor_offset(L, woff) : -1;
     LinearArgs plan = a;
     if (plan_rows > 0) plan.M = plan_rows;
-    if (rm >= 0 && linear_tc_supported(plan)) {
+    if (prefill && m.rm >= 0 && linear_tc_supported(plan)) {
       if (a.c1 != nullptr) s->launches++;  // row statistics kernel
-      return launch_linear_tc(a, blob + rm, (float*)(ws + W.row_stats), st);
+      return launch_linear_tc(a, blob + m.rm, (float*)(ws + W.row_stats), st);
     }
     return launch_linear(a, c.dtype, st, pdl, s->sm_count);
   };
 
   for (int i = 0; i < L.L; i++) {
-    const int64_t lb = L.layer0 + L.layer_stride * i;
     char* x = ws + W.x;
     if (prefill) {  // cross-attention K/V of the encoder states, once per generate() and description (:872-878)
       // the kernel is the one B * S rows take, so that the takes of a description get the bits B expanded rows would get (the
       // wgmma GEMM zero-fills the rows of a partial 128-row tile, also below 128 rows)
-      if (int e = lin(enc_hidden, H, lb + L.wkvc, L.ckv_rows, H, nullptr, nullptr, EPI_STORE, nullptr,
-                      ws + W.cross_tmp, L.ckv_rows, n_desc * S, -1, B * S)) return e;
+      if (int e = lin(enc_hidden, H, MAT_KV_CROSS, i, EPI_STORE, nullptr, ws + W.cross_tmp, L.ckv_rows, n_desc * S, B * S)) return e;
       if (int e = launch_cross_kv_relayout(ws + W.cross_tmp, ws + W.cross_kv + W.cross_layer_stride * i, n_desc, S, L.nckv, c.dtype, st)) return e;
       s->launches++;
     }
-    if (int e = lin(x, H, lb + L.wqkv, L.qkv_rows, H, (const float*)(blob + lb + L.ln1_w), (const float*)(blob + lb + L.ln1_b),
-                    EPI_STORE, nullptr, ws + W.qkv, L.qkv_rows, M, lb + L.c_qkv)) return e;
+    if (int e = lin(x, H, MAT_QKV, i, EPI_STORE, nullptr, ws + W.qkv, L.qkv_rows, M)) return e;
     AttnArgs at{};
     at.q = ws + W.qkv; at.ldq = L.qkv_rows; at.q_col0 = 0;
     at.knew = ws + W.qkv; at.vnew = ws + W.qkv; at.ldkv = L.qkv_rows; at.k_col0 = L.nh * D; at.v_col0 = (L.nh + L.nkv) * D;
@@ -667,9 +637,8 @@ static int run_forward(ptts_session* s, cudaStream_t st, bool prefill, const voi
     s->launches++;
     if (pw != nullptr) { if (int e = probe_attn(at, i)) return e; }
     if (int e = align_probe(at, i)) return e;
-    if (int e = lin(ws + W.attn, H, lb + L.wo, H, H, nullptr, nullptr, EPI_RESIDUAL, x, x, H, M)) return e;
-    if (int e = lin(x, H, lb + L.wqc, H, H, (const float*)(blob + lb + L.ln2_w), (const float*)(blob + lb + L.ln2_b),
-                    EPI_STORE, nullptr, ws + W.qc, H, M, lb + L.c_qc)) return e;
+    if (int e = lin(ws + W.attn, H, MAT_O, i, EPI_RESIDUAL, x, x, H, M)) return e;
+    if (int e = lin(x, H, MAT_Q_CROSS, i, EPI_STORE, nullptr, ws + W.qc, H, M)) return e;
     AttnArgs ct = at;
     ct.q = ws + W.qc; ct.ldq = H; ct.q_col0 = 0;
     ct.knew = ct.vnew = nullptr;
@@ -682,17 +651,15 @@ static int run_forward(ptts_session* s, cudaStream_t st, bool prefill, const voi
     s->launches++;
     if (pw != nullptr) { if (int e = probe_attn(ct, i)) return e; }
     if (int e = align_probe(ct, i)) return e;
-    if (int e = lin(ws + W.attn, H, lb + L.woc, H, H, nullptr, nullptr, EPI_RESIDUAL, x, x, H, M)) return e;
-    if (int e = lin(x, H, lb + L.fc1, L.F, H, (const float*)(blob + lb + L.ln3_w), (const float*)(blob + lb + L.ln3_b),
-                    EPI_ACT, nullptr, ws + W.hbuf, L.F, M, lb + L.c_fc1)) return e;
-    if (int e = lin(ws + W.hbuf, L.F, lb + L.fc2, H, L.F, nullptr, nullptr, EPI_RESIDUAL, x, x, H, M)) return e;
+    if (int e = lin(ws + W.attn, H, MAT_O_CROSS, i, EPI_RESIDUAL, x, x, H, M)) return e;
+    if (int e = lin(x, H, MAT_FC1, i, EPI_ACT, nullptr, ws + W.hbuf, L.F, M)) return e;
+    if (int e = lin(ws + W.hbuf, L.F, MAT_FC2, i, EPI_RESIDUAL, x, x, H, M)) return e;
     if (int e = probe_rows(i + 1, i == L.L - 1)) return e;   // entry L: the final LayerNorm of the last layer's output
   }
   if (!heads) return PTTS_OK;
   // final LayerNorm + K lm heads on the last position of every batch row -> f32 logits [B, K*V] == [B*K, V]
   const char* xlast = ws + W.x + (int64_t)(q_len - 1) * H * es;
-  return lin(xlast, (int64_t)q_len * H, L.heads, L.K * L.V, H, (const float*)(blob + L.final_ln_w), (const float*)(blob + L.final_ln_b),
-             EPI_F32, nullptr, ws + W.logits, (int64_t)L.K * L.V, B, L.c_heads);
+  return lin(xlast, (int64_t)q_len * H, MAT_HEADS, 0, EPI_F32, nullptr, ws + W.logits, (int64_t)L.K * L.V, B);
 }
 
 int ptts_prefill(ptts_session* s, const void* prompt_hidden, const int64_t* prompt_mask, const void* enc_hidden,
@@ -760,18 +727,19 @@ int ptts_score(ptts_session* s, const void* prompt_hidden, const int64_t* prompt
   a.M = W.B * T; a.B = W.B; a.T = T; a.K = L.K; a.V = L.V; a.H = L.H;
   a.bos = c.bos_token_id; a.eos = c.eos_token_id;
   const int q_len = W.P + T;
+  const DecoderMatrix hm = decoder_matrix(L, MAT_HEADS, 0);
   if (fused) {
-    a.c1 = (const float*)(s->blob + L.c_heads); a.c2 = a.c1 + (int64_t)L.K * L.V;
+    a.c1 = (const float*)(s->blob + hm.c); a.c2 = a.c1 + hm.N;
     s->launches += 2;
     if (int e = launch_score_fused(a, s->ws + W.x, W.P, c.layer_norm_eps, s->ws + W.qc, (float*)(s->ws + W.row_stats), heads_rm, st)) return e;
   } else {  // the decoder's heads GEMM over the B rows of one frame at a time, into the workspace logits [B*K][V]
     for (int t = 0; t < T; t++) {
       LinearArgs h{};
       h.X = s->ws + W.x + (int64_t)(W.P + t) * L.H * L.es; h.ldx = (int64_t)q_len * L.H;
-      h.W = s->blob + L.heads; h.Y = s->ws + W.logits; h.ldy = (int64_t)L.K * L.V; h.ldr = h.ldy;
-      h.ln_w = (const float*)(s->blob + L.final_ln_w); h.ln_b = (const float*)(s->blob + L.final_ln_b); h.eps = c.layer_norm_eps;
-      if (c.dtype == PTTS_BF16) { h.c1 = (const float*)(s->blob + L.c_heads); h.c2 = h.c1 + (int64_t)L.K * L.V; }
-      h.M = W.B; h.N = L.K * L.V; h.K = L.H; h.Kc = L.H;
+      h.W = s->blob + hm.w; h.Y = s->ws + W.logits; h.ldy = hm.N; h.ldr = h.ldy;
+      h.ln_w = (const float*)(s->blob + hm.ln_w); h.ln_b = (const float*)(s->blob + hm.ln_b); h.eps = c.layer_norm_eps;
+      if (c.dtype == PTTS_BF16) { h.c1 = (const float*)(s->blob + hm.c); h.c2 = h.c1 + hm.N; }
+      h.M = W.B; h.N = hm.N; h.K = hm.K; h.Kc = hm.K;
       h.epi = EPI_F32; h.act = c.activation;
       if (int e = launch_linear(h, c.dtype, st, false, s->sm_count)) return e;
       if (int e = launch_score_rows(a, (const float*)(s->ws + W.logits), t, out_logits, st)) return e;
@@ -934,45 +902,28 @@ int ptts_op_linear2(const ptts_decoder_config* cfg, const void* blob, int32_t te
   const DecoderLayout L = make_layout(*cfg);
   MatSlot ms;
   PTTS_REQUIRE(matrix_slot(L, tensor_id, index, &ms), "op_linear: tensor %d is not a matrix", tensor_id);
-  const int64_t lb = L.layer0 + L.layer_stride * index;
+  const DecoderMatrix& m = ms.m;
+  const char* bl = (const char*)blob;
   LinearArgs a{};
-  a.X = x; a.ldx = ms.K; a.W = (const char*)blob + ms.off; a.Y = y; a.ldy = ms.N; a.R = residual; a.ldr = ms.N;
+  a.X = x; a.ldx = m.K; a.W = bl + m.w; a.Y = y; a.ldy = m.N; a.R = residual; a.ldr = m.N;
   if (use_ln) {
-    PTTS_REQUIRE(ms.K == L.H, "op_linear: LayerNorm needs K == hidden_size");
-    int64_t w = 0, b = 0;
-    switch (tensor_id) {
-      case PTTS_T_SELF_Q: case PTTS_T_SELF_K: case PTTS_T_SELF_V: w = lb + L.ln1_w; b = lb + L.ln1_b; break;
-      case PTTS_T_CROSS_Q: w = lb + L.ln2_w; b = lb + L.ln2_b; break;
-      case PTTS_T_FC1: w = lb + L.ln3_w; b = lb + L.ln3_b; break;
-      case PTTS_T_LM_HEAD: w = L.final_ln_w; b = L.final_ln_b; break;
-      default: return fail(PTTS_EINVAL, "op_linear: tensor %d has no LayerNorm in front", tensor_id);
-    }
-    a.ln_w = (const float*)((const char*)blob + w);
-    a.ln_b = (const float*)((const char*)blob + b);
-    if (cfg->dtype == PTTS_BF16) {
-      int64_t co = 0;
-      switch (tensor_id) {
-        case PTTS_T_SELF_Q: case PTTS_T_SELF_K: case PTTS_T_SELF_V: co = lb + L.c_qkv; break;
-        case PTTS_T_CROSS_Q: co = lb + L.c_qc; break;
-        case PTTS_T_FC1: co = lb + L.c_fc1; break;
-        default: co = L.c_heads; break;
-      }
-      a.c1 = (const float*)((const char*)blob + co);
-      a.c2 = a.c1 + ms.N;
-    }
+    PTTS_REQUIRE(m.K == L.H, "op_linear: LayerNorm needs K == hidden_size");
+    PTTS_REQUIRE(m.ln_w >= 0, "op_linear: tensor %d has no LayerNorm in front", tensor_id);
+    a.ln_w = (const float*)(bl + m.ln_w);
+    a.ln_b = (const float*)(bl + m.ln_b);
+    if (cfg->dtype == PTTS_BF16) { a.c1 = (const float*)(bl + m.c); a.c2 = a.c1 + m.N; }
   }
   a.eps = cfg->layer_norm_eps;
-  a.M = M; a.N = ms.N; a.K = ms.K; a.Kc = (ms.K > L.H && ms.K % L.H == 0) ? L.H : ms.K;
+  a.M = M; a.N = m.N; a.K = m.K; a.Kc = (m.K > L.H && m.K % L.H == 0) ? L.H : m.K;
   a.epi = epilogue; a.act = cfg->activation; a.ctrl = nullptr;
   PTTS_REQUIRE(epilogue >= 0 && epilogue <= 3, "op_linear: bad epilogue");
   PTTS_REQUIRE(epilogue != EPI_RESIDUAL || residual, "op_linear: residual required");
   if (path == 1) {  // the prefill's rule: bf16, linear_tc_supported, a row-major copy
     PTTS_REQUIRE(cfg->dtype == PTTS_BF16 && linear_tc_supported(a), "op_linear: the wgmma GEMM does not take this problem (dtype %d, M %d, N %d, K %d, epilogue %d)",
-                 cfg->dtype, M, ms.N, ms.K, epilogue);
-    const int64_t rm = rowmajor_offset(L, ms.off);
-    PTTS_REQUIRE(rm >= 0, "op_linear: tensor %d has no row-major copy for the wgmma GEMM", tensor_id);
+                 cfg->dtype, M, m.N, m.K, epilogue);
+    PTTS_REQUIRE(m.rm >= 0, "op_linear: tensor %d has no row-major copy for the wgmma GEMM", tensor_id);
     PTTS_REQUIRE(a.c1 == nullptr || row_stats, "op_linear: row_stats scratch required with LayerNorm");
-    return launch_linear_tc(a, (const char*)blob + rm, row_stats, (cudaStream_t)stream);
+    return launch_linear_tc(a, bl + m.rm, row_stats, (cudaStream_t)stream);
   }
   int sm = 132, dev = 0;
   cudaGetDevice(&dev);
@@ -1071,7 +1022,7 @@ int ptts_dac_pack(const ptts_dac_config* cfg, void* blob, int32_t name_id, const
 int ptts_dac_workspace_bytes(const ptts_dac_config* cfg, int32_t B, int32_t T, int64_t* out_bytes) {
   PTTS_REQUIRE(cfg && out_bytes && B > 0 && T > 0, "bad argument");
   if (int e = validate_dac(*cfg)) return e;
-  *out_bytes = 3 * align_up(dac_max_act_per_frame(*cfg) * B * T * dtype_size(cfg->dtype), 1024) + align_up((int64_t)cfg->latent_dim * B * T * dtype_size(cfg->dtype), 1024);
+  *out_bytes = dac_decode_workspace(*cfg, B, T).bytes();
   return PTTS_OK;
 }
 
@@ -1081,123 +1032,14 @@ int ptts_dac_decode(const ptts_dac_config* cfg, const void* blob, void* workspac
 }
 
 // frame_lengths (device, [B], or NULL): every kernel clamps each value to [0, T], reads no code at or past it and writes zeros
-// there (RowLengths in dac.h).  Each layer gets the time steps per code frame so far (Tlen / T) to place each row's end.
+// there (RowLengths in dac.h).
 int ptts_dac_decode2(const ptts_dac_config* cfg, const void* blob, void* workspace, int64_t workspace_bytes, const int64_t* codes,
                      int32_t B, int32_t T, const int32_t* frame_lengths, void* audio_out, void* stream) {
   PTTS_REQUIRE(cfg && blob && workspace && codes && audio_out, "null argument");
   if (int e = validate_dac(*cfg)) return e;
   PTTS_REQUIRE(B > 0 && T > 0, "dac decode: empty input B=%d T=%d", B, T);
-  const DacLayout L = make_dac_layout(*cfg);
-  const int es = L.es;
-  const int64_t half = align_up(dac_max_act_per_frame(*cfg) * B * T * es, 1024);
-  const int64_t zbytes = align_up((int64_t)cfg->latent_dim * B * T * es, 1024);
-  PTTS_REQUIRE(workspace_bytes >= 3 * half + zbytes, "dac decode: workspace too small");
-  cudaStream_t st = (cudaStream_t)stream;
-  const char* bl = (const char*)blob;
-  char* cur = (char*)workspace;
-  char* oth = cur + half;
-  const int K = cfg->n_codebooks;
-  // ---- tensor-core path: bf16 storage, every conv but the last (Cout = 1) as a wgmma implicit GEMM ----
-  bool use_tc = (cfg->dtype == PTTS_BF16) && env_flag("PTTS_DAC_TC", true) && conv_tc_supported(cfg->latent_dim, cfg->decoder_dim);
-  for (int bi = 0; bi < cfg->n_blocks && use_tc; bi++) use_tc = conv_tc_supported(cfg->decoder_dim >> bi, cfg->decoder_dim >> (bi + 1)) && conv_tc_supported(cfg->decoder_dim >> (bi + 1), cfg->decoder_dim >> (bi + 1));
-  if (use_tc) {
-    char* bufA = (char*)workspace;
-    char* bufB = bufA + half;
-    char* bufX = bufB + half;
-    char* bufZ = bufX + half;
-    FromCodesArgs fz{codes, bl + L.codebooks, bl + L.proj_w, bl + L.proj_b, bufZ, K, cfg->codebook_dim, cfg->latent_dim, T, cfg->codebook_size,
-                     frame_lengths};
-    if (int e = launch_from_codes(fz, cfg->dtype, B, st)) return e;
-    int ti = 3 * K;
-    auto tpk = [&](int i) { return bl + L.t[i].off_k; };
-    auto tpp = [&](int i) { return bl + L.t[i].off; };
-    auto convk = [&](const void* x, int w_i, int b_i, const void* res, void* out_raw, void* out_act, const void* alpha_next, int Cin, int Cout, int Tlen, int ks, int dil) {
-      ConvArgs a{};
-      a.x = x; a.bias = tpp(b_i); a.res = res;
-      a.Cin = Cin; a.Cout = Cout; a.Tin = Tlen; a.Tout = Tlen; a.q_count = Tlen;
-      a.n_taps = ks; a.off_base = -((ks - 1) / 2) * dil; a.off_step = dil; a.wt_base = 0; a.wt_step = 1;
-      a.n_phase = 1; a.wt_phase_step = 0; a.o_mul = 1; a.o_add = 0; a.o_phase_step = 0;
-      return launch_conv_tc(a, tpk(w_i), ks, alpha_next, out_raw, out_act, B, st, RowLengths{frame_lengths, T, Tlen / T, Tlen / T});
-    };
-    const int C = cfg->decoder_dim;
-    char* act = bufA;   // snake'd input of the next conv
-    char* oth2 = bufB;
-    // conv1: latent -> C, output only as snake_{block0.snake1}(y)
-    if (int e = convk(bufZ, ti, ti + 1, nullptr, nullptr, act, tpp(ti + 2), cfg->latent_dim, C, T, 7, 1)) return e;
-    ti += 2;
-    int Tlen = T;
-    for (int bi = 0; bi < cfg->n_blocks; bi++) {
-      const int cin = C >> bi, cout = C >> (bi + 1), sd = cfg->strides[bi];
-      const int pad = (sd + 1) / 2;
-      ConvArgs a{};
-      a.x = act; a.bias = tpp(ti + 2); a.res = nullptr;
-      a.Cin = cin; a.Cout = cout; a.Tin = Tlen; a.Tout = Tlen * sd; a.q_count = Tlen + 1;
-      a.n_taps = 2; a.off_base = 0; a.off_step = -1; a.wt_base = 0; a.wt_step = sd;
-      a.n_phase = sd; a.wt_phase_step = 1; a.o_mul = sd; a.o_add = -pad; a.o_phase_step = 1;
-      // raw -> X (residual stream of the block), snake_{res1.snake1}(x) -> the other activation buffer
-      if (int e = launch_conv_tc(a, tpk(ti + 1), 2 * sd, tpp(ti + 3), bufX, oth2, B, st, RowLengths{frame_lengths, T, Tlen / T, Tlen / T * sd})) return e;
-      ti += 3;
-      std::swap(act, oth2);
-      Tlen *= sd;
-      const int dil[3] = {1, 3, 9};
-      for (int r = 0; r < 3; r++) {
-        // y = conv7(snake1(x)) -> only snake2(y) is stored; x += conv1(snake2(y)), plus snake_next(x) for the next unit
-        if (int e = convk(act, ti + 1, ti + 2, nullptr, nullptr, oth2, tpp(ti + 3), cout, cout, Tlen, 7, dil[r])) return e;
-        const int next_alpha = ti + 6;  // next unit's snake1, next block's snake1, or the decoder's final snake1
-        if (int e = convk(oth2, ti + 4, ti + 5, bufX, bufX, act, tpp(next_alpha), cout, cout, Tlen, 1, 1)) return e;
-        ti += 6;
-      }
-    }
-    const int cl = C >> cfg->n_blocks;
-    if (final_conv_supported(cl))   // one thread per output sample (dac.cu)
-      return launch_final_conv_tanh(act, tpp(ti + 1), tpp(ti + 2), audio_out, cl, Tlen, B, frame_lengths, T, st);
-    ConvArgs f{};  // final conv (Cout = 1) + tanh on the already snake'd tensor: generic kernel
-    f.x = act; f.w = tpp(ti + 1); f.bias = tpp(ti + 2); f.alpha = nullptr; f.res = nullptr; f.out = audio_out;
-    f.Cin = cl; f.Cout = 1; f.Tin = Tlen; f.Tout = Tlen; f.q_count = Tlen;
-    f.n_taps = 7; f.off_base = -3; f.off_step = 1; f.wt_base = 0; f.wt_step = 1;
-    f.n_phase = 1; f.wt_phase_step = 0; f.o_mul = 1; f.o_add = 0; f.o_phase_step = 0; f.tanh_out = 1;
-    return launch_conv(f, cfg->dtype, B, st, RowLengths{frame_lengths, T, Tlen / T, Tlen / T});
-  }
-  FromCodesArgs fc{codes, bl + L.codebooks, bl + L.proj_w, bl + L.proj_b, cur, K, cfg->codebook_dim, cfg->latent_dim, T, cfg->codebook_size,
-                   frame_lengths};
-  if (int e = launch_from_codes(fc, cfg->dtype, B, st)) return e;
-  int ti = 3 * K;  // tensor cursor (see make_dac_layout order)
-  auto tp = [&](int i) { return bl + L.t[i].off; };
-  auto conv = [&](const void* x, int w_i, int b_i, const void* alpha, const void* res, void* out, int Cin, int Cout, int Tlen, int ks, int dil, int tanh_out) {
-    ConvArgs a{};
-    a.x = x; a.w = tp(w_i); a.bias = tp(b_i); a.alpha = alpha; a.res = res; a.out = out;
-    a.Cin = Cin; a.Cout = Cout; a.Tin = Tlen; a.Tout = Tlen; a.q_count = Tlen;
-    a.n_taps = ks; a.off_base = -((ks - 1) / 2) * dil; a.off_step = dil; a.wt_base = 0; a.wt_step = 1;
-    a.n_phase = 1; a.wt_phase_step = 0; a.o_mul = 1; a.o_add = 0; a.o_phase_step = 0; a.tanh_out = tanh_out;
-    return launch_conv(a, cfg->dtype, B, st, RowLengths{frame_lengths, T, Tlen / T, Tlen / T});
-  };
-  const int C = cfg->decoder_dim;
-  if (int e = conv(cur, ti, ti + 1, nullptr, nullptr, oth, cfg->latent_dim, C, T, 7, 1, 0)) return e;
-  ti += 2;
-  std::swap(cur, oth);
-  int Tlen = T;
-  for (int bi = 0; bi < cfg->n_blocks; bi++) {
-    const int cin = C >> bi, cout = C >> (bi + 1), sd = cfg->strides[bi];
-    const int pad = (sd + 1) / 2;
-    ConvArgs a{};
-    a.x = cur; a.alpha = tp(ti); a.w = tp(ti + 1); a.bias = tp(ti + 2); a.res = nullptr; a.out = oth;
-    a.Cin = cin; a.Cout = cout; a.Tin = Tlen; a.Tout = Tlen * sd; a.q_count = Tlen + 1;
-    a.n_taps = 2; a.off_base = 0; a.off_step = -1; a.wt_base = 0; a.wt_step = sd;
-    a.n_phase = sd; a.wt_phase_step = 1; a.o_mul = sd; a.o_add = -pad; a.o_phase_step = 1; a.tanh_out = 0;
-    if (int e = launch_conv(a, cfg->dtype, B, st, RowLengths{frame_lengths, T, Tlen / T, Tlen / T * sd})) return e;
-    ti += 3;
-    std::swap(cur, oth);
-    Tlen *= sd;
-    const int dil[3] = {1, 3, 9};
-    for (int r = 0; r < 3; r++) {
-      // y = conv7(snake1(x)) -> oth ; x = x + conv1(snake2(y)) in place
-      if (int e = conv(cur, ti + 1, ti + 2, tp(ti), nullptr, oth, cout, cout, Tlen, 7, dil[r], 0)) return e;
-      if (int e = conv(oth, ti + 4, ti + 5, tp(ti + 3), cur, cur, cout, cout, Tlen, 1, 1, 0)) return e;
-      ti += 6;
-    }
-  }
-  const int cl = C >> cfg->n_blocks;
-  return conv(cur, ti + 1, ti + 2, tp(ti), nullptr, audio_out, cl, 1, Tlen, 7, 1, 1);
+  PTTS_REQUIRE(workspace_bytes >= dac_decode_workspace(*cfg, B, T).bytes(), "dac decode: workspace too small");
+  return dac_decode(*cfg, blob, workspace, codes, B, T, frame_lengths, audio_out, env_flag("PTTS_DAC_TC", true), (cudaStream_t)stream);
 }
 
 // ---- DAC encode -----------------------------------------------------------------------------------
@@ -1245,8 +1087,7 @@ int ptts_dac_encoder_pack(const ptts_dac_config* cfg, void* enc_blob, int32_t na
 int ptts_dac_encode_workspace_bytes(const ptts_dac_config* cfg, int32_t B, int32_t samples, int64_t* out_bytes) {
   PTTS_REQUIRE(cfg && out_bytes && B > 0 && samples > 0, "bad argument");
   if (int e = validate_dac_encoder(*cfg)) return e;
-  const int64_t T = (samples + dac_hop(*cfg) - 1) / dac_hop(*cfg), es = dtype_size(cfg->dtype);
-  *out_bytes = 3 * align_up(dac_enc_max_act_per_frame(*cfg) * B * T * es, 1024) + align_up((int64_t)cfg->latent_dim * B * T * es, 1024);
+  *out_bytes = dac_encode_workspace(*cfg, B, samples).bytes();
   return PTTS_OK;
 }
 
@@ -1256,95 +1097,9 @@ int ptts_dac_encode(const ptts_dac_config* cfg, const void* dec_blob, const void
   if (int e = validate_dac_encoder(*cfg)) return e;
   PTTS_REQUIRE(B > 0 && samples > 0, "dac encode: empty input B=%d samples=%d", B, samples);
   PTTS_REQUIRE(n_q >= 1 && n_q <= cfg->n_codebooks, "dac encode: n_q %d outside 1..%d", n_q, cfg->n_codebooks);
-  const DacEncLayout L = make_dac_enc_layout(*cfg);
-  const DacLayout DL = make_dac_layout(*cfg);
-  const int es = L.es, hop = dac_hop(*cfg), T = (samples + hop - 1) / hop, Tp = T * hop, Z = cfg->latent_dim;
-  const int64_t half = align_up(dac_enc_max_act_per_frame(*cfg) * B * T * es, 1024);
-  PTTS_REQUIRE(workspace_bytes >= 3 * half + align_up((int64_t)Z * B * T * es, 1024), "dac encode: workspace too small");
-  cudaStream_t st = (cudaStream_t)stream;
-  const char* bl = (const char*)enc_blob;
-  char* bufX = (char*)workspace;   // residual stream of the current block
-  char* act = bufX + half;         // activation the next conv reads
-  char* oth = act + half;
-  void* z = latents_out ? latents_out : (void*)(oth + half);
-  auto tp = [&](int i) { return bl + L.t[i].off; };
-  const int nb = cfg->n_enc_blocks, C0 = cfg->encoder_dim, cf = C0 << nb;
-  const int dil[3] = {1, 3, 9};
-  int ti = 2;   // tensor cursor (make_dac_enc_layout order): past the input conv
-  int Tlen = Tp;
-  // ---- tensor-core path: bf16, every conv after the input conv as a wgmma implicit GEMM (strided ones over the s*C view) ----
-  bool use_tc = cfg->dtype == PTTS_BF16 && env_flag("PTTS_DAC_TC", true) && C0 % 2 == 0 && conv_tc_supported(cf, Z);
-  for (int bi = 0; bi < nb && use_tc; bi++)
-    use_tc = conv_tc_supported(C0 << bi, C0 << bi) && conv_tc_supported(cfg->encoder_rates[bi] * (C0 << bi), 2 * (C0 << bi));
-  if (use_tc) {
-    auto tpk = [&](int i) { return bl + L.t[i].off_k; };
-    auto convk = [&](const void* x, int w_i, int b_i, const void* res, void* out_raw, void* out_act, const void* alpha_next, int Cin, int Cout,
-                     int Tl, int ks, int dl) {
-      ConvArgs a{};
-      a.x = x; a.bias = tp(b_i); a.res = res;
-      a.Cin = Cin; a.Cout = Cout; a.Tin = Tl; a.Tout = Tl; a.q_count = Tl;
-      a.n_taps = ks; a.off_base = -((ks - 1) / 2) * dl; a.off_step = dl; a.wt_base = 0; a.wt_step = 1;
-      a.n_phase = 1; a.wt_phase_step = 0; a.o_mul = 1; a.o_add = 0; a.o_phase_step = 0;
-      return launch_conv_tc(a, tpk(w_i), ks, alpha_next, out_raw, out_act, B, st);
-    };
-    // input conv: raw -> X, snake_{block0.res_unit1.snake1}(x) -> act
-    if (int e = launch_enc_input_conv(audio, tp(0), tp(1), tp(ti), bufX, act, C0, samples, Tp, B, st)) return e;
-    for (int bi = 0; bi < nb; bi++) {
-      const int C = C0 << bi, s = cfg->encoder_rates[bi];
-      for (int r = 0; r < 3; r++) {
-        // y = conv7(snake1(x)) -> only snake2(y) is stored; x += conv1(snake2(y)), plus snake_next(x): the next unit's snake1 or
-        // the block's snake1 (ti + 6 either way)
-        if (int e = convk(act, ti + 1, ti + 2, nullptr, nullptr, oth, tp(ti + 3), C, C, Tlen, 7, dil[r])) return e;
-        if (int e = convk(oth, ti + 4, ti + 5, bufX, bufX, act, tp(ti + 6), C, C, Tlen, 1, 1)) return e;
-        ti += 6;
-      }
-      // strided conv over super-rows of s time steps: 3 taps at rows q-1, q, q+1 of the [B][T/s][s*C] view; TMA zero fill of
-      // rows -1 and T/s is the conv padding.  Raw -> X (the next block's residual stream; not needed after the last block),
-      // snake of the next layer (next block's res_unit1.snake1 or the encoder's snake1, both at ti + 3) -> the other buffer
-      ConvArgs a{};
-      a.x = act; a.bias = tp(ti + 2); a.res = nullptr;
-      a.Cin = s * C; a.Cout = 2 * C; a.Tin = Tlen / s; a.Tout = Tlen / s; a.q_count = Tlen / s;
-      a.n_taps = 3; a.off_base = -1; a.off_step = 1; a.wt_base = 0; a.wt_step = 1;
-      a.n_phase = 1; a.wt_phase_step = 0; a.o_mul = 1; a.o_add = 0; a.o_phase_step = 0;
-      if (int e = launch_conv_tc(a, tpk(ti + 1), 3, tp(ti + 3), bi + 1 < nb ? bufX : nullptr, oth, B, st)) return e;
-      std::swap(act, oth);
-      Tlen /= s;
-      ti += 3;
-    }
-    if (int e = convk(act, ti + 1, ti + 2, nullptr, z, nullptr, nullptr, cf, Z, Tlen, 3, 1)) return e;
-  } else {
-    // ---- generic path (f32, or widths the wgmma kernel does not take): snake applied on the fly to each conv's input ----
-    auto conv = [&](const void* x, const void* w, const void* bias, const void* alpha, const void* res, void* out, int Cin, int Cout,
-                    int Tin, int Tout, int ks, int dl, int off_base) {
-      ConvArgs a{};
-      a.x = x; a.w = w; a.bias = bias; a.alpha = alpha; a.res = res; a.out = out;
-      a.Cin = Cin; a.Cout = Cout; a.Tin = Tin; a.Tout = Tout; a.q_count = Tout;
-      a.n_taps = ks; a.off_base = off_base; a.off_step = dl; a.wt_base = 0; a.wt_step = 1;
-      a.n_phase = 1; a.wt_phase_step = 0; a.o_mul = 1; a.o_add = 0; a.o_phase_step = 0; a.tanh_out = 0;
-      return launch_conv(a, cfg->dtype, B, st);
-    };
-    char* cur = bufX;
-    // input conv: rows past `samples` read zeros (the pad to the hop)
-    if (int e = conv(audio, tp(0), tp(1), nullptr, nullptr, cur, 1, C0, samples, Tp, 7, 1, -3)) return e;
-    for (int bi = 0; bi < nb; bi++) {
-      const int C = C0 << bi, s = cfg->encoder_rates[bi];
-      for (int r = 0; r < 3; r++) {
-        if (int e = conv(cur, tp(ti + 1), tp(ti + 2), tp(ti), nullptr, oth, C, C, Tlen, Tlen, 7, dil[r], -3 * dil[r])) return e;
-        if (int e = conv(oth, tp(ti + 4), tp(ti + 5), tp(ti + 3), cur, cur, C, C, Tlen, Tlen, 1, 1, 0)) return e;
-        ti += 6;
-      }
-      // strided conv over the super-row view; the block's snake1 alpha is tiled s times to match its s*C input channels
-      if (int e = conv(cur, tp(ti + 1), tp(ti + 2), bl + L.t[ti].off_t, nullptr, oth, s * C, 2 * C, Tlen / s, Tlen / s, 3, 1, -1)) return e;
-      std::swap(cur, oth);
-      Tlen /= s;
-      ti += 3;
-    }
-    if (int e = conv(cur, tp(ti + 1), tp(ti + 2), tp(ti), nullptr, z, cf, Z, Tlen, Tlen, 3, 1, -1)) return e;
-  }
-  const char* dbl = (const char*)dec_blob;
-  QuantizeArgs q{z, bl + L.in_w, bl + L.in_b, (const float*)(bl + L.cb_norm), dbl + DL.codebooks, dbl + DL.proj_w, dbl + DL.proj_b,
-                 codes_out, n_q, cfg->codebook_dim, Z, T, cfg->codebook_size};
-  return launch_quantize(q, cfg->dtype, B, st);
+  PTTS_REQUIRE(workspace_bytes >= dac_encode_workspace(*cfg, B, samples).bytes(), "dac encode: workspace too small");
+  return dac_encode(*cfg, dec_blob, enc_blob, workspace, audio, B, samples, n_q, codes_out, latents_out, env_flag("PTTS_DAC_TC", true),
+                    (cudaStream_t)stream);
 }
 
 }  // extern "C"

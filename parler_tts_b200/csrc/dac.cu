@@ -11,6 +11,9 @@
 // one kernel covers Conv1d(k=7, dilated), Conv1d(k=1) and ConvTranspose1d(k=2s, stride s) by
 // describing each as "n_taps shifted input rows x per-tap weight slice"; snake on the input, bias,
 // residual add and tanh are fused.  Roofline: tensor/FMA-bound (1.608 GFLOP per code frame, SURVEY 8d).
+// dac_decode at the end walks the codec's layers by name (dac.h) on this path or on the wgmma one (dac_tc.cu).
+#include <utility>
+
 #include "common.cuh"
 #include "dac.h"
 
@@ -260,6 +263,94 @@ int launch_final_conv_tanh(const void* x, const void* w, const void* bias, void*
                                                                                  frame_lengths, frames);
   PTTS_LAUNCH_CHECK();
   return PTTS_OK;
+}
+
+// ---- decode walk: from_codes into the latent buffer, then conv1, the decoder blocks and the output conv ----------------------
+// Each conv gets its row lengths as time steps per code frame so far (Tin / T, Tout / T), which place each ragged row's end.
+static const int kDilation[3] = {1, 3, 9};
+
+// bf16, every conv but the last (Cout = 1) as a wgmma implicit GEMM.  Snake moves into the epilogue of the conv before it: a conv
+// writes its raw output where a residual needs it and snake_{alpha of the next layer}(output) for the next conv to read.
+static int decode_tc(const ptts_dac_config& c, const DacLayout& L, const char* bl, const DacWorkspace& W, void* ws, int B, int T,
+                     const int32_t* fl, void* audio, cudaStream_t st) {
+  auto P = [&](int i) { return (const void*)(bl + L.t[i].off); };
+  auto conv = [&](ConvArgs a, const void* x, int w, int b, const void* res, void* out_raw, void* out_act, const void* alpha_next) {
+    a.x = x; a.bias = P(b); a.res = res;
+    return launch_conv_tc(a, bl + L.t[w].off_k, a.n_taps * a.n_phase, alpha_next, out_raw, out_act, B, st, RowLengths{fl, T, a.Tin / T, a.Tout / T});
+  };
+  char* act = W.buf(ws, 0);   // snake'd input of the next conv
+  char* oth = W.buf(ws, 1);
+  char* res = W.buf(ws, 2);   // residual stream of the current block
+  const int C = c.decoder_dim, nb = c.n_blocks;
+  if (int e = conv(conv_same(c.latent_dim, C, T, 7, 1), W.buf(ws, 3), L.conv1_w, L.conv1_b, nullptr, nullptr, act, P(L.block[0].snake1))) return e;
+  int Tl = T;
+  for (int bi = 0; bi < nb; bi++) {
+    const DacDecBlock& blk = L.block[bi];
+    const int cout = C >> (bi + 1), s = c.strides[bi];
+    if (int e = conv(conv_up(C >> bi, cout, Tl, s), act, blk.conv_t1_w, blk.conv_t1_b, nullptr, res, oth, P(blk.res[0].snake1))) return e;
+    std::swap(act, oth);
+    Tl *= s;
+    for (int r = 0; r < 3; r++) {
+      const DacResUnit& u = blk.res[r];
+      const int next = r < 2 ? blk.res[r + 1].snake1 : bi + 1 < nb ? L.block[bi + 1].snake1 : L.snake1;
+      // y = conv7(snake1(x)): only snake2(y) is stored; x += conv1(snake2(y)), and snake_next(x) for the next layer
+      if (int e = conv(conv_same(cout, cout, Tl, 7, kDilation[r]), act, u.conv1_w, u.conv1_b, nullptr, nullptr, oth, P(u.snake2))) return e;
+      if (int e = conv(conv_same(cout, cout, Tl, 1, 1), oth, u.conv2_w, u.conv2_b, res, res, act, P(next))) return e;
+    }
+  }
+  const int cl = C >> nb;
+  if (final_conv_supported(cl))   // one thread per output sample
+    return launch_final_conv_tanh(act, P(L.conv2_w), P(L.conv2_b), audio, cl, Tl, B, fl, T, st);
+  ConvArgs f = conv_same(cl, 1, Tl, 7, 1);   // the input is already snake'd
+  f.x = act; f.w = P(L.conv2_w); f.bias = P(L.conv2_b); f.out = audio; f.tanh_out = 1;
+  return launch_conv(f, c.dtype, B, st, RowLengths{fl, T, Tl / T, Tl / T});
+}
+
+// Any dtype and width: snake applied on the fly to each conv's input, the residual added in place.
+static int decode_generic(const ptts_dac_config& c, const DacLayout& L, const char* bl, const DacWorkspace& W, void* ws, int B, int T,
+                          const int32_t* fl, void* audio, cudaStream_t st) {
+  auto P = [&](int i) { return (const void*)(bl + L.t[i].off); };
+  auto conv = [&](ConvArgs a, const void* x, const void* alpha, int w, int b, const void* res, void* out) {
+    a.x = x; a.alpha = alpha; a.w = P(w); a.bias = P(b); a.res = res; a.out = out;
+    return launch_conv(a, c.dtype, B, st, RowLengths{fl, T, a.Tin / T, a.Tout / T});
+  };
+  char* cur = W.buf(ws, 0);
+  char* oth = W.buf(ws, 1);
+  const int C = c.decoder_dim;
+  if (int e = conv(conv_same(c.latent_dim, C, T, 7, 1), W.buf(ws, 3), nullptr, L.conv1_w, L.conv1_b, nullptr, cur)) return e;
+  int Tl = T;
+  for (int bi = 0; bi < c.n_blocks; bi++) {
+    const DacDecBlock& blk = L.block[bi];
+    const int cout = C >> (bi + 1), s = c.strides[bi];
+    if (int e = conv(conv_up(C >> bi, cout, Tl, s), cur, P(blk.snake1), blk.conv_t1_w, blk.conv_t1_b, nullptr, oth)) return e;
+    std::swap(cur, oth);
+    Tl *= s;
+    for (int r = 0; r < 3; r++) {
+      const DacResUnit& u = blk.res[r];
+      // y = conv7(snake1(x)) -> oth; x = x + conv1(snake2(y)) in place
+      if (int e = conv(conv_same(cout, cout, Tl, 7, kDilation[r]), cur, P(u.snake1), u.conv1_w, u.conv1_b, nullptr, oth)) return e;
+      if (int e = conv(conv_same(cout, cout, Tl, 1, 1), oth, P(u.snake2), u.conv2_w, u.conv2_b, cur, cur)) return e;
+    }
+  }
+  ConvArgs f = conv_same(C >> c.n_blocks, 1, Tl, 7, 1);
+  f.tanh_out = 1;
+  return conv(f, cur, P(L.snake1), L.conv2_w, L.conv2_b, nullptr, audio);
+}
+
+int dac_decode(const ptts_dac_config& c, const void* blob, void* ws, const int64_t* codes, int B, int T, const int32_t* frame_lengths,
+               void* audio, bool allow_tc, cudaStream_t st) {
+  const DacLayout L = make_dac_layout(c);
+  const DacWorkspace W = dac_decode_workspace(c, B, T);
+  const char* bl = (const char*)blob;
+  FromCodesArgs fz{codes, bl + L.codebooks, bl + L.proj_w, bl + L.proj_b, W.buf(ws, 3), c.n_codebooks, c.codebook_dim, c.latent_dim, T,
+                   c.codebook_size, frame_lengths};
+  if (int e = launch_from_codes(fz, c.dtype, B, st)) return e;
+  bool tc = allow_tc && c.dtype == PTTS_BF16 && conv_tc_supported(c.latent_dim, c.decoder_dim);
+  for (int bi = 0; bi < c.n_blocks && tc; bi++) {
+    const int cin = c.decoder_dim >> bi, cout = c.decoder_dim >> (bi + 1);
+    tc = conv_tc_supported(cin, cout) && conv_tc_supported(cout, cout);
+  }
+  return (tc ? decode_tc : decode_generic)(c, L, bl, W, ws, B, T, frame_lengths, audio, st);
 }
 
 }  // namespace ptts

@@ -16,6 +16,28 @@ struct ConvArgs {
   int n_phase, wt_phase_step, o_mul, o_add, o_phase_step;
   int tanh_out;
 };
+// The codec's three conv shapes: geometry only, the caller sets the pointers.  Their weights hold n_taps * n_phase taps.
+// Stride-1 Conv1d(k = taps, dilation dil, "same" padding) over T rows.
+static inline ConvArgs conv_same(int Cin, int Cout, int T, int taps, int dil) {
+  ConvArgs a{};
+  a.Cin = Cin; a.Cout = Cout; a.Tin = T; a.Tout = T; a.q_count = T;
+  a.n_taps = taps; a.off_base = -((taps - 1) / 2) * dil; a.off_step = dil; a.wt_base = 0; a.wt_step = 1;
+  a.n_phase = 1; a.wt_phase_step = 0; a.o_mul = 1; a.o_add = 0; a.o_phase_step = 0;
+  return a;
+}
+// ConvTranspose1d(k = 2s, stride s, pad ceil(s/2)) from T rows to T*s: phase p of output row q*s - pad + p takes taps p and
+// p + s at input rows q and q - 1.
+static inline ConvArgs conv_up(int Cin, int Cout, int T, int s) {
+  ConvArgs a{};
+  a.Cin = Cin; a.Cout = Cout; a.Tin = T; a.Tout = T * s; a.q_count = T + 1;
+  a.n_taps = 2; a.off_base = 0; a.off_step = -1; a.wt_base = 0; a.wt_step = s;
+  a.n_phase = s; a.wt_phase_step = 1; a.o_mul = s; a.o_add = -((s + 1) / 2); a.o_phase_step = 1;
+  return a;
+}
+// The encoder's strided Conv1d(C -> Cout, k = 2s, stride s) over T rows: the 3-tap conv over super-rows q-1, q, q+1 of the
+// [B][T/s][s*C] view (pack_strided_conv below).
+static inline ConvArgs conv_super_rows(int C, int Cout, int T, int s) { return conv_same(s * C, Cout, T / s, 3, 1); }
+
 // Ragged decode: row b holds frame_lengths[b] code frames (clamped to [0, frames]) and ends at frame_lengths[b] * up_in on a
 // conv's input axis, * up_out on its output axis.  Outputs past a row's end are written as 0, so that the buffers hold the zero
 // padding a standalone decode of the row sees.  frame_lengths == nullptr: every row is full (equal lengths, and the encoder).
@@ -59,9 +81,18 @@ struct DacTensor {
   int64_t off_k;   // conv weights: second copy [tap][Cout][Cin] bf16 for the tensor-core path (-1: none)
 };
 
+// Tensor ids (indices into a layout's t) under the state-dict names of dac_wrapper._dac_tensor_list /
+// _dac_encoder_tensor_list; the ids themselves are the push order of make_dac_layout / make_dac_enc_layout.
+struct DacResUnit { int snake1, conv1_w, conv1_b, snake2, conv2_w, conv2_b; };
+struct DacDecBlock { int snake1, conv_t1_w, conv_t1_b; DacResUnit res[3]; };
+struct DacEncBlock { DacResUnit res[3]; int snake1, conv1_w, conv1_b; };
+
 struct DacLayout {
   std::vector<DacTensor> t;
   int64_t codebooks, proj_w, proj_b;
+  int conv1_w, conv1_b;
+  DacDecBlock block[8];
+  int snake1, conv2_w, conv2_b;
   int64_t total;
   int es;
 };
@@ -85,6 +116,7 @@ static inline DacLayout make_dac_layout(const ptts_dac_config& c) {
     o = align_up(o + t.numel * L.es, 256);
     if (kind != DK_PLAIN && c.dtype == PTTS_BF16) { t.off_k = o; o = align_up(o + t.numel * 2, 1024); }
     L.t.push_back(t);
+    return (int)L.t.size() - 1;
   };
   const int K = c.n_codebooks, D = c.codebook_dim, Z = c.latent_dim;
   // from_codes tensors are laid out as three contiguous arrays; ids interleave per codebook
@@ -98,21 +130,22 @@ static inline DacLayout make_dac_layout(const ptts_dac_config& c) {
     L.t.push_back({DK_PLAIN, Z, 1, 1, L.proj_b + (int64_t)k * Z * L.es, (int64_t)Z, -1});
   }
   const int C = c.decoder_dim;
-  add(DK_CONV, C, Z, 7); add(DK_PLAIN, C, 1, 1);
+  L.conv1_w = add(DK_CONV, C, Z, 7); L.conv1_b = add(DK_PLAIN, C, 1, 1);
   for (int bi = 0; bi < c.n_blocks; bi++) {
     const int cin = C >> bi, cout = C >> (bi + 1), s = c.strides[bi];
-    add(DK_PLAIN, cin, 1, 1);
-    add(DK_CONVT, cin, cout, 2 * s); add(DK_PLAIN, cout, 1, 1);
-    for (int r = 0; r < 3; r++) {
-      add(DK_PLAIN, cout, 1, 1);
-      add(DK_CONV, cout, cout, 7); add(DK_PLAIN, cout, 1, 1);
-      add(DK_PLAIN, cout, 1, 1);
-      add(DK_CONV, cout, cout, 1); add(DK_PLAIN, cout, 1, 1);
+    DacDecBlock& b = L.block[bi];
+    b.snake1 = add(DK_PLAIN, cin, 1, 1);
+    b.conv_t1_w = add(DK_CONVT, cin, cout, 2 * s); b.conv_t1_b = add(DK_PLAIN, cout, 1, 1);
+    for (DacResUnit& u : b.res) {
+      u.snake1 = add(DK_PLAIN, cout, 1, 1);
+      u.conv1_w = add(DK_CONV, cout, cout, 7); u.conv1_b = add(DK_PLAIN, cout, 1, 1);
+      u.snake2 = add(DK_PLAIN, cout, 1, 1);
+      u.conv2_w = add(DK_CONV, cout, cout, 1); u.conv2_b = add(DK_PLAIN, cout, 1, 1);
     }
   }
   const int cl = C >> c.n_blocks;
-  add(DK_PLAIN, cl, 1, 1);
-  add(DK_CONV, 1, cl, 7); add(DK_PLAIN, 1, 1, 1);
+  L.snake1 = add(DK_PLAIN, cl, 1, 1);
+  L.conv2_w = add(DK_CONV, 1, cl, 7); L.conv2_b = add(DK_PLAIN, 1, 1, 1);
   L.total = o;
   return L;
 }
@@ -161,6 +194,9 @@ struct DacEncTensor {
 struct DacEncLayout {
   std::vector<DacEncTensor> t;
   int64_t in_w, in_b, cb_norm;   // quantizer arrays, contiguous over codebooks
+  int conv1_w, conv1_b;
+  DacEncBlock block[8];
+  int snake1, conv2_w, conv2_b;
   int64_t total;
   int es;
 };
@@ -197,22 +233,24 @@ static inline DacEncLayout make_dac_enc_layout(const ptts_dac_config& c) {
     if (tc && (kind == EK_SCONV || (kind == EK_CONV && d1 > 1))) { t.off_k = o; o = align_up(o + stored * 2, 1024); }
     if (tile > 1) { t.off_t = o; o = align_up(o + t.numel * tile * L.es, 256); }
     L.t.push_back(t);
+    return (int)L.t.size() - 1;
   };
-  add(EK_CONV, c.encoder_dim, 1, 7, 1); add(EK_PLAIN, c.encoder_dim, 1, 1, 1);
+  L.conv1_w = add(EK_CONV, c.encoder_dim, 1, 7, 1); L.conv1_b = add(EK_PLAIN, c.encoder_dim, 1, 1, 1);
   for (int bi = 0; bi < c.n_enc_blocks; bi++) {
     const int C = c.encoder_dim << bi, s = c.encoder_rates[bi];
-    for (int r = 0; r < 3; r++) {
-      add(EK_PLAIN, C, 1, 1, 1);
-      add(EK_CONV, C, C, 7, 1); add(EK_PLAIN, C, 1, 1, 1);
-      add(EK_PLAIN, C, 1, 1, 1);
-      add(EK_CONV, C, C, 1, 1); add(EK_PLAIN, C, 1, 1, 1);
+    DacEncBlock& b = L.block[bi];
+    for (DacResUnit& u : b.res) {
+      u.snake1 = add(EK_PLAIN, C, 1, 1, 1);
+      u.conv1_w = add(EK_CONV, C, C, 7, 1); u.conv1_b = add(EK_PLAIN, C, 1, 1, 1);
+      u.snake2 = add(EK_PLAIN, C, 1, 1, 1);
+      u.conv2_w = add(EK_CONV, C, C, 1, 1); u.conv2_b = add(EK_PLAIN, C, 1, 1, 1);
     }
-    add(EK_PLAIN, C, 1, 1, s);
-    add(EK_SCONV, 2 * C, C, 2 * s, 1); add(EK_PLAIN, 2 * C, 1, 1, 1);
+    b.snake1 = add(EK_PLAIN, C, 1, 1, s);
+    b.conv1_w = add(EK_SCONV, 2 * C, C, 2 * s, 1); b.conv1_b = add(EK_PLAIN, 2 * C, 1, 1, 1);
   }
   const int cf = c.encoder_dim << c.n_enc_blocks;
-  add(EK_PLAIN, cf, 1, 1, 1);
-  add(EK_CONV, Z, cf, 3, 1); add(EK_PLAIN, Z, 1, 1, 1);
+  L.snake1 = add(EK_PLAIN, cf, 1, 1, 1);
+  L.conv2_w = add(EK_CONV, Z, cf, 3, 1); L.conv2_b = add(EK_PLAIN, Z, 1, 1, 1);
   for (int k = 0; k < K; k++) {
     L.t.push_back({EK_PLAIN, D * Z, 1, 1, 1, L.in_w + (int64_t)k * D * Z * L.es, (int64_t)D * Z, -1, -1});
     L.t.push_back({EK_PLAIN, D, 1, 1, 1, L.in_b + (int64_t)k * D * L.es, (int64_t)D, -1, -1});
@@ -222,26 +260,43 @@ static inline DacEncLayout make_dac_enc_layout(const ptts_dac_config& c) {
   return L;
 }
 
-// elements per (batch, code frame) of the largest encoder activation
-static inline int64_t dac_enc_max_act_per_frame(const ptts_dac_config& c) {
+// Codec workspace: three activation buffers, each of the largest activation (per_frame elements per batch row and code frame),
+// then the latent [B][T][latent_dim].  T: code frames (encode: samples rounded up to the hop).
+struct DacWorkspace {
+  int64_t act, z;   // bytes of one activation buffer, of the latent buffer
+  int64_t bytes() const { return 3 * act + z; }
+  char* buf(void* ws, int i) const { return (char*)ws + i * act; }   // activation buffer i; i = 3: the latent
+};
+static inline DacWorkspace dac_workspace(const ptts_dac_config& c, int64_t per_frame, int B, int64_t T) {
+  const int64_t es = dtype_size(c.dtype);
+  return {align_up(per_frame * B * T * es, 1024), align_up((int64_t)c.latent_dim * B * T * es, 1024)};
+}
+static inline DacWorkspace dac_decode_workspace(const ptts_dac_config& c, int B, int T) {
+  int64_t m = c.latent_dim > c.decoder_dim ? c.latent_dim : c.decoder_dim, up = 1;
+  for (int i = 0; i < c.n_blocks; i++) {
+    up *= c.strides[i];
+    const int64_t e = up * (c.decoder_dim >> (i + 1));
+    if (e > m) m = e;
+  }
+  return dac_workspace(c, m, B, T);
+}
+static inline DacWorkspace dac_encode_workspace(const ptts_dac_config& c, int B, int samples) {
   int64_t per = dac_hop(c), m = (int64_t)c.latent_dim;
   for (int bi = 0; bi <= c.n_enc_blocks; bi++) {
     const int64_t e = per * ((int64_t)c.encoder_dim << bi);
     if (e > m) m = e;
     if (bi < c.n_enc_blocks) per /= c.encoder_rates[bi];
   }
-  return m;
+  return dac_workspace(c, m, B, (samples + dac_hop(c) - 1) / dac_hop(c));
 }
-// elements per (batch, code frame) of the largest activation
-static inline int64_t dac_max_act_per_frame(const ptts_dac_config& c) {
-  int64_t m = c.latent_dim > c.decoder_dim ? c.latent_dim : c.decoder_dim;
-  int64_t up = 1;
-  for (int i = 0; i < c.n_blocks; i++) {
-    up *= c.strides[i];
-    int64_t e = up * (c.decoder_dim >> (i + 1));
-    if (e > m) m = e;
-  }
-  return m;
-}
+
+// codes [B][K][T] -> waveform [B][T * hop] (dac.cu).  frame_lengths as in RowLengths.  allow_tc: the wgmma path where the config
+// is bf16 and conv_tc_supported takes every width; the generic conv_kernel path otherwise.
+int dac_decode(const ptts_dac_config& c, const void* blob, void* ws, const int64_t* codes, int B, int T, const int32_t* frame_lengths,
+               void* audio, bool allow_tc, cudaStream_t st);
+// waveform [B][samples] -> codes [B][n_q][T] and, when latents != nullptr, the encoder output [B][T][latent_dim] (dac_enc.cu).
+// allow_tc as for dac_decode.
+int dac_encode(const ptts_dac_config& c, const void* dec_blob, const void* enc_blob, void* ws, const void* audio, int B, int samples,
+               int n_q, int64_t* codes, void* latents, bool allow_tc, cudaStream_t st);
 
 }  // namespace ptts

@@ -7,8 +7,11 @@
 // (conv_tc_kernel in dac_tc.cu, conv_kernel in dac.cu); this file adds what those cannot do:
 //   * the input conv (Cin = 1; the wgmma kernel needs Cin >= 64),
 //   * the weight packs of the strided convs, which run as 3-tap convs over the [B][T/s][s*C] view (dac.h),
-//   * the residual vector quantizer.
+//   * the residual vector quantizer,
+//   * dac_encode, the walk over the encoder's layers by name (dac.h).
 #include <math.h>
+
+#include <utility>
 
 #include "common.cuh"
 #include "dac.h"
@@ -221,6 +224,95 @@ static int launch_quantize_t(const QuantizeArgs& a, int B, cudaStream_t st) {
 int launch_quantize(const QuantizeArgs& a, int dtype, int B, cudaStream_t st) {
   PTTS_REQUIRE(quantize_supported(a.Z, a.D), "dac encode: quantizer shape latent %d / codebook_dim %d unsupported", a.Z, a.D);
   return dtype == PTTS_BF16 ? launch_quantize_t<bf16>(a, B, st) : launch_quantize_t<float>(a, B, st);
+}
+
+// ---- encode walk: the input conv, the encoder blocks, the output conv, the quantizer ---------------------------------------
+static const int kDilation[3] = {1, 3, 9};
+
+// bf16, every conv after the input conv as a wgmma implicit GEMM (the strided ones over the s*C view).  Snake moves into the
+// epilogue of the conv before it, as in the decode walk (dac.cu).
+static int encode_tc(const ptts_dac_config& c, const DacEncLayout& L, const char* bl, const DacWorkspace& W, void* ws, const void* audio,
+                     int B, int samples, int Tp, void* z, cudaStream_t st) {
+  auto P = [&](int i) { return (const void*)(bl + L.t[i].off); };
+  auto conv = [&](ConvArgs a, const void* x, int w, int b, const void* res, void* out_raw, void* out_act, const void* alpha_next) {
+    a.x = x; a.bias = P(b); a.res = res;
+    return launch_conv_tc(a, bl + L.t[w].off_k, a.n_taps * a.n_phase, alpha_next, out_raw, out_act, B, st);
+  };
+  char* res = W.buf(ws, 0);   // residual stream of the current block
+  char* act = W.buf(ws, 1);   // snake'd input of the next conv
+  char* oth = W.buf(ws, 2);
+  const int nb = c.n_enc_blocks, C0 = c.encoder_dim;
+  int Tl = Tp;   // samples padded to the hop
+  // input conv: raw -> res, snake_{block 0's first snake1}(x) -> act
+  if (int e = launch_enc_input_conv(audio, P(L.conv1_w), P(L.conv1_b), P(L.block[0].res[0].snake1), res, act, C0, samples, Tl, B, st)) return e;
+  for (int bi = 0; bi < nb; bi++) {
+    const DacEncBlock& blk = L.block[bi];
+    const int C = C0 << bi, s = c.encoder_rates[bi];
+    for (int r = 0; r < 3; r++) {
+      const DacResUnit& u = blk.res[r];
+      const int next = r < 2 ? blk.res[r + 1].snake1 : blk.snake1;
+      // y = conv7(snake1(x)): only snake2(y) is stored; x += conv1(snake2(y)), and snake_next(x) for the next layer
+      if (int e = conv(conv_same(C, C, Tl, 7, kDilation[r]), act, u.conv1_w, u.conv1_b, nullptr, nullptr, oth, P(u.snake2))) return e;
+      if (int e = conv(conv_same(C, C, Tl, 1, 1), oth, u.conv2_w, u.conv2_b, res, res, act, P(next))) return e;
+    }
+    // strided conv; the TMA zero fill of super-rows -1 and T/s is its padding.  Raw -> res (the next block's residual stream; not
+    // needed after the last block), snake of the next layer -> oth
+    const bool last = bi + 1 == nb;
+    const void* alpha_next = P(last ? L.snake1 : L.block[bi + 1].res[0].snake1);
+    if (int e = conv(conv_super_rows(C, 2 * C, Tl, s), act, blk.conv1_w, blk.conv1_b, nullptr, last ? nullptr : res, oth, alpha_next)) return e;
+    std::swap(act, oth);
+    Tl /= s;
+  }
+  return conv(conv_same(C0 << nb, c.latent_dim, Tl, 3, 1), act, L.conv2_w, L.conv2_b, nullptr, z, nullptr, nullptr);
+}
+
+// Any dtype and width: snake applied on the fly to each conv's input, the residual added in place.
+static int encode_generic(const ptts_dac_config& c, const DacEncLayout& L, const char* bl, const DacWorkspace& W, void* ws, const void* audio,
+                          int B, int samples, int Tp, void* z, cudaStream_t st) {
+  auto P = [&](int i) { return (const void*)(bl + L.t[i].off); };
+  auto conv = [&](ConvArgs a, const void* x, const void* alpha, int w, int b, const void* res, void* out) {
+    a.x = x; a.alpha = alpha; a.w = P(w); a.bias = P(b); a.res = res; a.out = out;
+    return launch_conv(a, c.dtype, B, st);
+  };
+  char* cur = W.buf(ws, 0);
+  char* oth = W.buf(ws, 2);
+  const int nb = c.n_enc_blocks, C0 = c.encoder_dim;
+  int Tl = Tp;   // samples padded to the hop
+  ConvArgs in = conv_same(1, C0, Tl, 7, 1);
+  in.Tin = samples;   // rows past `samples` read zeros: the pad to the hop
+  if (int e = conv(in, audio, nullptr, L.conv1_w, L.conv1_b, nullptr, cur)) return e;
+  for (int bi = 0; bi < nb; bi++) {
+    const DacEncBlock& blk = L.block[bi];
+    const int C = C0 << bi, s = c.encoder_rates[bi];
+    for (int r = 0; r < 3; r++) {
+      const DacResUnit& u = blk.res[r];
+      if (int e = conv(conv_same(C, C, Tl, 7, kDilation[r]), cur, P(u.snake1), u.conv1_w, u.conv1_b, nullptr, oth)) return e;
+      if (int e = conv(conv_same(C, C, Tl, 1, 1), oth, P(u.snake2), u.conv2_w, u.conv2_b, cur, cur)) return e;
+    }
+    // strided conv over the super-row view: the block's snake1 alpha tiled s times matches its s*C input channels
+    if (int e = conv(conv_super_rows(C, 2 * C, Tl, s), cur, bl + L.t[blk.snake1].off_t, blk.conv1_w, blk.conv1_b, nullptr, oth)) return e;
+    std::swap(cur, oth);
+    Tl /= s;
+  }
+  return conv(conv_same(C0 << nb, c.latent_dim, Tl, 3, 1), cur, P(L.snake1), L.conv2_w, L.conv2_b, nullptr, z);
+}
+
+int dac_encode(const ptts_dac_config& c, const void* dec_blob, const void* enc_blob, void* ws, const void* audio, int B, int samples,
+               int n_q, int64_t* codes, void* latents, bool allow_tc, cudaStream_t st) {
+  const DacEncLayout L = make_dac_enc_layout(c);
+  const DacLayout DL = make_dac_layout(c);
+  const DacWorkspace W = dac_encode_workspace(c, B, samples);
+  const int nb = c.n_enc_blocks, C0 = c.encoder_dim, Z = c.latent_dim;
+  bool tc = allow_tc && c.dtype == PTTS_BF16 && C0 % 2 == 0 && conv_tc_supported(C0 << nb, Z);
+  for (int bi = 0; bi < nb && tc; bi++) tc = conv_tc_supported(C0 << bi, C0 << bi) && conv_tc_supported(c.encoder_rates[bi] * (C0 << bi), 2 * (C0 << bi));
+  const char* bl = (const char*)enc_blob;
+  void* z = latents ? latents : (void*)W.buf(ws, 3);
+  const int T = (samples + dac_hop(c) - 1) / dac_hop(c);
+  if (int e = (tc ? encode_tc : encode_generic)(c, L, bl, W, ws, audio, B, samples, T * dac_hop(c), z, st)) return e;
+  const char* dbl = (const char*)dec_blob;
+  QuantizeArgs q{z, bl + L.in_w, bl + L.in_b, (const float*)(bl + L.cb_norm), dbl + DL.codebooks, dbl + DL.proj_w, dbl + DL.proj_b,
+                 codes, n_q, c.codebook_dim, Z, T, c.codebook_size};
+  return launch_quantize(q, c.dtype, B, st);
 }
 
 }  // namespace ptts

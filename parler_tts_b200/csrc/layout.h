@@ -11,12 +11,6 @@
 
 namespace ptts {
 
-struct MatSlot {
-  int64_t off;  // byte offset in blob
-  int N, K;     // fused matrix shape (rows = output features)
-  int row_off;  // row offset of this tensor inside the fused matrix
-};
-
 struct DecoderLayout {
   int es;  // element size of model dtype
   int H, F, V, K, L, nh, nkv, nckv, qkv_rows, ckv_rows;
@@ -29,7 +23,7 @@ struct DecoderLayout {
   // (phase, cluster, rank): the n-tiles the cluster owns x the K range the rank reduces.  cl_NC == 0: shape not covered.
   int cl_C, cl_NC;          // CTAs per cluster (2), clusters (4 per head)
   int64_t rm[7];            // per layer (bf16 only): ROW-MAJOR copies of wqkv, wo, wqc, wkvc, woc, fc1, fc2 for the wgmma prefill
-                            // GEMM (gemm_tc.cu: TMA-tiled K-major operands); same order as rm_src()
+                            // GEMM (gemm_tc.cu: TMA-tiled K-major operands); indexed by DecoderMatrixId
   int64_t cp[6];            // per layer: offset of phase p's slices (A qkv | B o | C q_cross | D o_cross | E fc1 | F fc2)
   int64_t cp_slice[6];      // bytes of one (cluster, rank) slice of phase p
   int64_t total;
@@ -132,22 +126,52 @@ static inline int validate_config(const ptts_decoder_config& c) {
   return PTTS_OK;
 }
 
-// Resolve (tensor_id, index) -> fused matrix slot.  Returns false for non-matrix tensors.
+// The decoder's GEMM matrices: the seven of each layer (fused where the reference has several projections) and the lm heads.
+enum DecoderMatrixId { MAT_QKV, MAT_O, MAT_Q_CROSS, MAT_KV_CROSS, MAT_O_CROSS, MAT_FC1, MAT_FC2, MAT_HEADS, MAT_COUNT };
+struct DecoderMatrix {
+  int64_t w;           // blob offset of the fragment-order weights
+  int N, K;            // rows = output features, columns
+  int64_t ln_w, ln_b;  // blob offsets of the fp32 gamma / beta of the LayerNorm in front; -1: none
+  int64_t c;           // blob offset of the folded LayerNorm vectors c1 | c2 (fp32, N each; bf16 only, ptts_decoder_finalize); -1: none
+  int64_t rm;          // blob offset of the row-major copy the wgmma prefill GEMM reads; -1: none (f32, or the lm heads)
+};
+// Matrix m of `layer` (ignored for the lm heads).
+static inline DecoderMatrix decoder_matrix(const DecoderLayout& l, int m, int layer) {
+  const int64_t lb = l.layer0 + l.layer_stride * layer;
+  const int64_t rm = l.es == 2 && m != MAT_HEADS ? lb + l.rm[m] : -1;
+  switch (m) {
+    case MAT_QKV: return {lb + l.wqkv, l.qkv_rows, l.H, lb + l.ln1_w, lb + l.ln1_b, lb + l.c_qkv, rm};
+    case MAT_O: return {lb + l.wo, l.H, l.H, -1, -1, -1, rm};
+    case MAT_Q_CROSS: return {lb + l.wqc, l.H, l.H, lb + l.ln2_w, lb + l.ln2_b, lb + l.c_qc, rm};
+    case MAT_KV_CROSS: return {lb + l.wkvc, l.ckv_rows, l.H, -1, -1, -1, rm};
+    case MAT_O_CROSS: return {lb + l.woc, l.H, l.H, -1, -1, -1, rm};
+    case MAT_FC1: return {lb + l.fc1, l.F, l.H, lb + l.ln3_w, lb + l.ln3_b, lb + l.c_fc1, rm};
+    case MAT_FC2: return {lb + l.fc2, l.H, l.F, -1, -1, -1, rm};
+    default: return {l.heads, l.K * l.V, l.H, l.final_ln_w, l.final_ln_b, l.c_heads, -1};
+  }
+}
+
+// An ABI tensor id's place in the matrix table: the fused matrix and the tensor's first row in it.
+struct MatSlot {
+  DecoderMatrix m;
+  int row_off;
+};
+// Resolve (tensor_id, index) -> fused matrix slot (index: the layer, or the lm head's codebook).  Returns false for non-matrix tensors.
 static inline bool matrix_slot(const DecoderLayout& l, int tensor_id, int index, MatSlot* s) {
-  int64_t lb = l.layer0 + l.layer_stride * index;
   const int D = PTTS_HEAD_DIM;
+  auto slot = [&](int m, int row_off) { *s = {decoder_matrix(l, m, index), row_off}; return true; };
   switch (tensor_id) {
-    case PTTS_T_SELF_Q: *s = {lb + l.wqkv, l.qkv_rows, l.H, 0}; return true;
-    case PTTS_T_SELF_K: *s = {lb + l.wqkv, l.qkv_rows, l.H, l.nh * D}; return true;
-    case PTTS_T_SELF_V: *s = {lb + l.wqkv, l.qkv_rows, l.H, (l.nh + l.nkv) * D}; return true;
-    case PTTS_T_SELF_O: *s = {lb + l.wo, l.H, l.H, 0}; return true;
-    case PTTS_T_CROSS_Q: *s = {lb + l.wqc, l.H, l.H, 0}; return true;
-    case PTTS_T_CROSS_K: *s = {lb + l.wkvc, l.ckv_rows, l.H, 0}; return true;
-    case PTTS_T_CROSS_V: *s = {lb + l.wkvc, l.ckv_rows, l.H, l.nckv * D}; return true;
-    case PTTS_T_CROSS_O: *s = {lb + l.woc, l.H, l.H, 0}; return true;
-    case PTTS_T_FC1: *s = {lb + l.fc1, l.F, l.H, 0}; return true;
-    case PTTS_T_FC2: *s = {lb + l.fc2, l.H, l.F, 0}; return true;
-    case PTTS_T_LM_HEAD: *s = {l.heads, l.K * l.V, l.H, index * l.V}; return true;
+    case PTTS_T_SELF_Q: return slot(MAT_QKV, 0);
+    case PTTS_T_SELF_K: return slot(MAT_QKV, l.nh * D);
+    case PTTS_T_SELF_V: return slot(MAT_QKV, (l.nh + l.nkv) * D);
+    case PTTS_T_SELF_O: return slot(MAT_O, 0);
+    case PTTS_T_CROSS_Q: return slot(MAT_Q_CROSS, 0);
+    case PTTS_T_CROSS_K: return slot(MAT_KV_CROSS, 0);
+    case PTTS_T_CROSS_V: return slot(MAT_KV_CROSS, l.nckv * D);
+    case PTTS_T_CROSS_O: return slot(MAT_O_CROSS, 0);
+    case PTTS_T_FC1: return slot(MAT_FC1, 0);
+    case PTTS_T_FC2: return slot(MAT_FC2, 0);
+    case PTTS_T_LM_HEAD: return slot(MAT_HEADS, index * l.V);
     default: return false;
   }
 }
