@@ -201,6 +201,17 @@ int ptts_generate_begin(ptts_session* s, const ptts_gen_params* gen, void* strea
  * columns in one pass (:3033-3044); gen->input_len is set to n0. */
 int ptts_generate_begin_ids(ptts_session* s, const ptts_gen_params* gen, const int64_t* input_ids, int32_t n0, void* stream);
 
+/* Same, for a batch whose rows continue from inputs of different lengths (ragged prefixes).
+ *   input_lens [B] int32 device, or NULL (= ptts_generate_begin_ids): row b's input is the first n0_b = input_lens[b] columns of
+ *              its input_ids row, 1 <= n0_b <= n0 (the columns past it are never read).  Checked with one host sync.  With
+ *              n0 == 1 every length is 1: the call is ptts_generate_begin_ids (any session takes it).
+ * Row b then computes exactly what it would as a batch of its own, continuing from its n0_b columns with max_length
+ * gen->max_length - (n0 - n0_b): its history, cache slots and positions start at 0 as they would alone, and every decode step,
+ * sampler stage and Philox draw uses its own column cur_len - (n0 - n0_b).  All rows reach their limit at the same step.  The
+ * probe windows (ptts_generate_set_probes, ptts_generate_set_alignment) are refused while such a call runs. */
+int ptts_generate_begin_ids2(ptts_session* s, const ptts_gen_params* gen, const int64_t* input_ids, int32_t n0, const int32_t* input_lens,
+                             void* stream);
+
 /* Step 0 (prefill): prompt prefix + the n0 delayed input columns (the BOS column unless the call began with
  * ptts_generate_begin_ids) through the decoder, cross-attention K/V projected once,
  * self-attention cache filled at positions [0, P + n0).  Leaves f32 logits [B*K, V] in the workspace.

@@ -76,6 +76,7 @@ _SIGS = {
     "ptts_session_destroy": (C.c_int, [_VP]),
     "ptts_generate_begin": (C.c_int, [_VP, C.POINTER(GenParamsC), _VP]),
     "ptts_generate_begin_ids": (C.c_int, [_VP, C.POINTER(GenParamsC), _VP, _I32, _VP]),
+    "ptts_generate_begin_ids2": (C.c_int, [_VP, C.POINTER(GenParamsC), _VP, _I32, _VP, _VP]),
     "ptts_generate_set_sampling_ext": (C.c_int, [_VP, C.POINTER(SamplingExtC)]),
     "ptts_generate_set_logits_ext": (C.c_int, [_VP, C.POINTER(LogitsExtC)]),
     "ptts_generate_set_outputs": (C.c_int, [_VP, _VP, _VP, _I32, _I32, _I64]),

@@ -66,6 +66,7 @@ struct ptts_session {
   bool has_prompt_mask, has_enc_mask, begun, prefilled;
   ptts_gen_params gen;
   int n0;            // decoder input columns of the current generate() call (1: the BOS column; > 1: continuing from codes)
+  bool ragged;       // the call's rows continue from inputs of different lengths (ptts_generate_begin_ids2): W.row_shift is live
   cudaStream_t cap_stream;
   cudaGraphExec_t exec;
   bool graph_ready;
@@ -234,6 +235,7 @@ int ptts_session_create3(const ptts_decoder_config* cfg, const void* blob, void*
   s->L = make_layout(*cfg);
   s->W = make_workspace(*cfg, B, P, S, max_cache_len, max_input_len, takes);
   s->n0 = 1;
+  s->ragged = false;
   s->ext = kExtOff;
   s->lext = kLogitsExtOff;
   s->out = SampleOut{};
@@ -301,6 +303,7 @@ static SampleArgs sample_args(ptts_session* s) {
   a.ctrl = (Ctrl*)(s->ws + W.ctrl);
   a.gen = (const ptts_gen_params*)(s->ws + W.gen);
   a.prefix_cells = W.prefix_cells >= 0 ? (int64_t*)(s->ws + W.prefix_cells) : nullptr;
+  a.shift = s->ragged ? (int*)(s->ws + W.row_shift) : nullptr;
   a.B = W.B; a.K = s->cfg.num_codebooks; a.V = s->cfg.vocab_size;
   a.bos = s->cfg.bos_token_id; a.pad = s->cfg.pad_token_id; a.eos = s->cfg.eos_token_id;
   return a;
@@ -353,7 +356,8 @@ static DecodePath choose_decode_path(ptts_session* s) {
   return DECODE_STEP;
 }
 
-int ptts_generate_begin_ids(ptts_session* s, const ptts_gen_params* gen, const int64_t* input_ids, int32_t n0, void* stream) {
+int ptts_generate_begin_ids2(ptts_session* s, const ptts_gen_params* gen, const int64_t* input_ids, int32_t n0, const int32_t* input_lens,
+                             void* stream) {
   PTTS_REQUIRE(s && gen, "null argument");
   PTTS_REQUIRE(n0 >= 1 && n0 <= s->W.max_input, "generate: %d decoder input columns, the session takes 1 .. %d", n0, s->W.max_input);
   PTTS_REQUIRE(input_ids != nullptr || n0 == 1, "generate: input_ids is required for %d input columns", n0);
@@ -364,6 +368,16 @@ int ptts_generate_begin_ids(ptts_session* s, const ptts_gen_params* gen, const i
   PTTS_REQUIRE(s->cfg.eos_token_id >= 0 && s->cfg.eos_token_id < s->cfg.vocab_size, "eos_token_id out of vocabulary");
   PTTS_REQUIRE(n0 < gen->max_length, "generate: %d input columns leave nothing to generate within max_length %d", n0, gen->max_length);
   cudaStream_t st = (cudaStream_t)stream;
+  if (input_lens != nullptr) {   // checked here, once per call: every kernel after the begin trusts the shifts it derives
+    PTTS_REQUIRE(input_ids != nullptr, "generate: input_lens needs input_ids");
+    std::vector<int32_t> lens(s->W.B);
+    PTTS_CHECK_CUDA(cudaMemcpyAsync(lens.data(), input_lens, lens.size() * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+    PTTS_CHECK_CUDA(cudaStreamSynchronize(st));
+    for (int b = 0; b < s->W.B; b++)
+      PTTS_REQUIRE(lens[b] >= 1 && lens[b] <= n0, "generate: input_lens[%d] = %d is outside [1, n0 = %d]", b, lens[b], n0);
+  }
+  // n0 == 1: every length is 1 and every offset 0 -- a uniform batch (and a session without max_input_len > 1 has no row_shift)
+  s->ragged = input_lens != nullptr && n0 > 1;
   s->gen = *gen;
   s->gen.input_len = n0;
   s->n0 = n0;
@@ -374,10 +388,14 @@ int ptts_generate_begin_ids(ptts_session* s, const ptts_gen_params* gen, const i
   s->probe = ProbeWindow{};
   s->align = AlignWindow{};
   PTTS_CHECK_CUDA(cudaMemcpyAsync(s->ws + s->W.gen, &s->gen, sizeof(ptts_gen_params), cudaMemcpyHostToDevice, st));
-  if (int e = launch_generate_begin(sample_args(s), input_ids, n0, gen->max_length, st)) return e;
+  if (int e = launch_generate_begin(sample_args(s), input_ids, n0, gen->max_length, s->ragged ? input_lens : nullptr, st)) return e;
   s->begun = true;
   s->prefilled = false;
   return PTTS_OK;
+}
+
+int ptts_generate_begin_ids(ptts_session* s, const ptts_gen_params* gen, const int64_t* input_ids, int32_t n0, void* stream) {
+  return ptts_generate_begin_ids2(s, gen, input_ids, n0, nullptr, stream);
 }
 
 int ptts_generate_begin(ptts_session* s, const ptts_gen_params* gen, void* stream) {
@@ -440,6 +458,7 @@ int ptts_generate_set_probes(ptts_session* s, void* self_attn, void* cross_attn,
   PTTS_REQUIRE(first_step >= 0 && n_steps >= 0, "probes: the window needs first_step >= 0 and n_steps >= 0, got %d and %d", first_step, n_steps);
   ProbeWindow w{};
   if (self_attn != nullptr || cross_attn != nullptr || hidden != nullptr) {
+    PTTS_REQUIRE(!s->ragged, "probes: the probe kernels take one position for the whole batch, not a ragged continuation's");
     const WorkspaceLayout& W = s->W;
     const DecoderLayout& L = s->L;
     // (the prefill slot's row count P + n0 is only known when ptts_prefill / ptts_score runs: run_forward checks self_ld there)
@@ -468,6 +487,7 @@ int ptts_generate_set_alignment(ptts_session* s, const int32_t* heads, int32_t n
   PTTS_REQUIRE(first_step >= 0 && n_steps >= 0, "alignment: the window needs first_step >= 0 and n_steps >= 0, got %d and %d", first_step, n_steps);
   AlignWindow w{};
   if (out != nullptr) {
+    PTTS_REQUIRE(!s->ragged, "alignment: the probe kernels take one position for the whole batch, not a ragged continuation's");
     const DecoderLayout& L = s->L;
     // a session with a self-attention prompt prefix aligns to it; one without (prompt_cross_attention) to its cross keys
     const int keys = s->W.P > 0 ? s->W.P : s->W.S;
@@ -524,6 +544,9 @@ static int run_forward(ptts_session* s, cudaStream_t st, bool prefill, const voi
   ea.ctrl = ctrl;
   ea.B = B; ea.K = L.K; ea.V1 = L.V + 1; ea.H = H; ea.P = prefill ? P : 0; ea.n_cols = prefill ? s->n0 : 1;
   ea.pos_from_ctrl = prefill ? 0 : 1; ea.pos0 = 0; ea.prefix_len = P;
+  // a ragged continuation's decode positions are per row; at prefill every row's column j sits at position P + j, as alone
+  const int* shift = prefill ? nullptr : sample_args(s).shift;
+  ea.shift = shift;
   if (int e = launch_embed(ea, c.dtype, st, pdl)) return e;
   s->launches++;
 
@@ -628,7 +651,7 @@ static int run_forward(ptts_session* s, cudaStream_t st, bool prefill, const voi
     at.out = ws + W.attn; at.ldo = H;
     at.key_mask = s->has_prompt_mask ? (const int*)(ws + W.prompt_mask) : nullptr; at.mask_len = P; at.mask_ld = P;
     at.ctrl = ctrl; at.B = B; at.nh = L.nh; at.nkv = L.nkv; at.q_len = q_len;
-    at.past_from_ctrl = prefill ? 0 : 1; at.past_len = 0; at.prefix = P;
+    at.past_from_ctrl = prefill ? 0 : 1; at.past_len = 0; at.prefix = P; at.shift = shift;
     at.cross = 0; at.kv_len = 0;
     at.rope = c.rope; at.rope_cos = blob + L.rope_cos; at.rope_sin = blob + L.rope_sin;
     at.kv_capacity = prefill ? q_len : W.Tmax;
@@ -658,6 +681,14 @@ static int run_forward(ptts_session* s, cudaStream_t st, bool prefill, const voi
   }
   if (!heads) return PTTS_OK;
   // final LayerNorm + K lm heads on the last position of every batch row -> f32 logits [B, K*V] == [B*K, V]
+  if (prefill && s->ragged) {
+    // a ragged continuation's row b ends at its own last input column, row P + n0_b - 1 = q_len - 1 - shift[b].  Its padded
+    // columns past it were embedded and wrote K/V into cache slots >= P + n0_b, which no query has seen: the causal mask keeps
+    // the row's own queries off them, and decode step t appends slot P + n0_b + t before its query reads keys up to it.
+    if (int e = launch_gather_rows(ws + W.x, H, q_len - 1, q_len, sample_args(s).shift, ws + W.hidden, B, H, c.dtype, st)) return e;
+    s->launches++;
+    return lin(ws + W.hidden, H, MAT_HEADS, 0, EPI_F32, nullptr, ws + W.logits, (int64_t)L.K * L.V, B);
+  }
   const char* xlast = ws + W.x + (int64_t)(q_len - 1) * H * es;
   return lin(xlast, (int64_t)q_len * H, MAT_HEADS, 0, EPI_F32, nullptr, ws + W.logits, (int64_t)L.K * L.V, B);
 }
@@ -719,6 +750,7 @@ int ptts_score(ptts_session* s, const void* prompt_hidden, const int64_t* prompt
   if (s->has_prompt_mask) { if (int e = launch_mask_convert(prompt_mask, W.B * W.P, (int*)(s->ws + W.prompt_mask), st)) return e; }
   if (s->has_enc_mask) { if (int e = launch_mask_convert(enc_mask, W.B / W.takes * W.S, (int*)(s->ws + W.enc_mask), st)) return e; }
   s->n0 = T;
+  s->ragged = false;
   s->begun = s->prefilled = false;  // the caches now hold this call's positions: a generation has to begin again
   if (int e = run_forward(s, st, true, prompt_hidden, enc_hidden, false)) return e;
 

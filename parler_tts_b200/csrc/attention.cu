@@ -26,8 +26,9 @@ __global__ void __launch_bounds__(ATT_THREADS) attention_kernel(AttnArgs p) {
   attention_item<T>(p, blockIdx.y, blockIdx.x, sm, threadIdx.x, [] { __syncthreads(); }, (int)blockIdx.z * per, (int)(blockIdx.z + 1) * per);
 }
 
-// decode (q_len == 1): 8 items per CTA, one warp each (TMA-staged K/V ring per warp)
-template <typename T>
+// decode (q_len == 1): 8 items per CTA, one warp each (TMA-staged K/V ring per warp).  RAGGED (p.shift != nullptr): each row's
+// own position; false is the code of a uniform batch
+template <typename T, bool RAGGED>
 __global__ void __launch_bounds__(256) attention_decode_kernel(AttnArgs p) {
   extern __shared__ __align__(128) unsigned char smd[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -41,7 +42,7 @@ __global__ void __launch_bounds__(256) attention_decode_kernel(AttnArgs p) {
   const int it = blockIdx.x * 4 + pair;
   if (it >= p.B * p.nkv) return;
   int past = p.past_len;
-  if (p.past_from_ctrl) past = p.prefix + p.ctrl->cur_len - 1;
+  if (p.past_from_ctrl) past = p.prefix + p.ctrl->cur_len - 1 - (RAGGED ? row_shift(p.shift, it / p.nkv) : 0);
   uint32_t parity = 0;
   float* xch = reinterpret_cast<float*>(smd + 128 + (size_t)8 * attn_decode_smem_per_warp<T>()) + pair * 128;
   attention_decode_item_warp<T>(p, it / p.nkv, it % p.nkv, past, sm_warp, bars, lane, parity, part, 2, xch, pair + 1);
@@ -136,8 +137,10 @@ int launch_attention(const AttnArgs& a, int dtype, cudaStream_t st, bool pdl, bo
     const size_t smem_d = 128 + (size_t)8 * (dtype == PTTS_BF16 ? attn_decode_smem_per_warp<bf16>() : attn_decode_smem_per_warp<float>()) + 4 * 128 * sizeof(float);
     static bool attr_d = false;
     if (!attr_d) {
-      PTTS_CHECK_CUDA(cudaFuncSetAttribute(attention_decode_kernel<bf16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-      PTTS_CHECK_CUDA(cudaFuncSetAttribute(attention_decode_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+      PTTS_CHECK_CUDA(cudaFuncSetAttribute(attention_decode_kernel<bf16, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+      PTTS_CHECK_CUDA(cudaFuncSetAttribute(attention_decode_kernel<float, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+      PTTS_CHECK_CUDA(cudaFuncSetAttribute(attention_decode_kernel<bf16, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+      PTTS_CHECK_CUDA(cudaFuncSetAttribute(attention_decode_kernel<float, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
       attr_d = true;
     }
     cudaLaunchConfig_t cfg{};
@@ -150,8 +153,9 @@ int launch_attention(const AttnArgs& a, int dtype, cudaStream_t st, bool pdl, bo
     at[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = at;
     cfg.numAttrs = pdl ? 1 : 0;
-    if (dtype == PTTS_BF16) PTTS_CHECK_CUDA(cudaLaunchKernelEx(&cfg, attention_decode_kernel<bf16>, a));
-    else PTTS_CHECK_CUDA(cudaLaunchKernelEx(&cfg, attention_decode_kernel<float>, a));
+    const bool rg = a.shift != nullptr;
+    if (dtype == PTTS_BF16) PTTS_CHECK_CUDA(cudaLaunchKernelEx(&cfg, rg ? attention_decode_kernel<bf16, true> : attention_decode_kernel<bf16, false>, a));
+    else PTTS_CHECK_CUDA(cudaLaunchKernelEx(&cfg, rg ? attention_decode_kernel<float, true> : attention_decode_kernel<float, false>, a));
     return PTTS_OK;
   }
   const int kv_capacity = a.kv_capacity;

@@ -47,6 +47,11 @@ struct Ctrl {
 };
 static_assert(sizeof(Ctrl) == 256, "Ctrl layout");
 
+// Ragged continuation (ptts_generate_begin_ids2): batch row b continues from shift[b] fewer input columns than the longest row,
+// so its history column and cache position are the batch's minus shift[b] -- what the row alone would have.  The array is
+// written once by the begin kernel; shift == nullptr (every row at the batch's own column) reads nothing.
+__device__ __forceinline__ int row_shift(const int* shift, int b) { return shift != nullptr ? shift[b] : 0; }
+
 // ---- dtype traits -------------------------------------------------------------------------------
 template <typename T> struct DT;
 template <> struct DT<bf16> {

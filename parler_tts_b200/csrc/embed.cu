@@ -10,14 +10,15 @@
 
 namespace ptts {
 
-template <typename T>
+// RAGGED (a.shift != nullptr): decode positions per row; false is the code of a uniform batch
+template <typename T, bool RAGGED>
 __global__ void __launch_bounds__(128) embed_kernel(EmbedArgs p) {
   pdl_launch_dependents();
   pdl_wait();
   if (p.ctrl != nullptr && p.ctrl->active == 0) return;
   const int rows_per_b = p.P + p.n_cols;
   const int b = blockIdx.x / rows_per_b, j = blockIdx.x - b * rows_per_b;
-  const int position = p.pos_from_ctrl ? (p.prefix_len + p.ctrl->cur_len - 1) : (p.pos0 + j);
+  const int position = p.pos_from_ctrl ? (p.prefix_len + p.ctrl->cur_len - 1 - (RAGGED ? row_shift(p.shift, b) : 0)) : (p.pos0 + j);
   const T* tables = reinterpret_cast<const T*>(p.tables);
   const T* pos = reinterpret_cast<const T*>(p.pos);
   T* x = reinterpret_cast<T*>(p.x) + (size_t)blockIdx.x * p.H;
@@ -48,8 +49,9 @@ int launch_embed(const EmbedArgs& a, int dtype, cudaStream_t st, bool pdl) {
   at[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = at;
   cfg.numAttrs = pdl ? 1 : 0;
-  if (dtype == PTTS_BF16) PTTS_CHECK_CUDA(cudaLaunchKernelEx(&cfg, embed_kernel<bf16>, a));
-  else PTTS_CHECK_CUDA(cudaLaunchKernelEx(&cfg, embed_kernel<float>, a));
+  const bool rg = a.shift != nullptr;
+  if (dtype == PTTS_BF16) PTTS_CHECK_CUDA(cudaLaunchKernelEx(&cfg, rg ? embed_kernel<bf16, true> : embed_kernel<bf16, false>, a));
+  else PTTS_CHECK_CUDA(cudaLaunchKernelEx(&cfg, rg ? embed_kernel<float, true> : embed_kernel<float, false>, a));
   return PTTS_OK;
 }
 
@@ -66,13 +68,15 @@ int launch_mask_convert(const int64_t* src, int n, int* dst, cudaStream_t st) {
 }
 
 template <typename T>
-__global__ void gather_rows_kernel(const T* src, int64_t ld_src, int64_t row0, int64_t row_step, T* dst, int rows, int cols) {
+__global__ void gather_rows_kernel(const T* src, int64_t ld_src, int64_t row0, int64_t row_step, const int* shift, T* dst, int rows, int cols) {
   int r = blockIdx.x;
-  for (int c = threadIdx.x; c < cols; c += blockDim.x) dst[(size_t)r * cols + c] = src[(size_t)(row0 + r * row_step) * ld_src + c];
+  const int64_t s = row0 + r * row_step - row_shift(shift, r);
+  for (int c = threadIdx.x; c < cols; c += blockDim.x) dst[(size_t)r * cols + c] = src[(size_t)s * ld_src + c];
 }
-int launch_gather_rows(const void* src, int64_t ld_src, int64_t row0, int64_t row_step, void* dst, int rows, int cols, int dtype, cudaStream_t st) {
-  if (dtype == PTTS_BF16) gather_rows_kernel<bf16><<<rows, 128, 0, st>>>((const bf16*)src, ld_src, row0, row_step, (bf16*)dst, rows, cols);
-  else gather_rows_kernel<float><<<rows, 128, 0, st>>>((const float*)src, ld_src, row0, row_step, (float*)dst, rows, cols);
+int launch_gather_rows(const void* src, int64_t ld_src, int64_t row0, int64_t row_step, const int* shift, void* dst, int rows, int cols,
+                       int dtype, cudaStream_t st) {
+  if (dtype == PTTS_BF16) gather_rows_kernel<bf16><<<rows, 128, 0, st>>>((const bf16*)src, ld_src, row0, row_step, shift, (bf16*)dst, rows, cols);
+  else gather_rows_kernel<float><<<rows, 128, 0, st>>>((const float*)src, ld_src, row0, row_step, shift, (float*)dst, rows, cols);
   PTTS_LAUNCH_CHECK();
   return PTTS_OK;
 }

@@ -39,8 +39,9 @@ struct AttnArgs {
   const int* key_mask; int mask_len, mask_ld;   // keys t < mask_len with key_mask[b*mask_ld+t]==0 are excluded
   const Ctrl* ctrl;
   int B, nh, nkv, q_len;
-  int past_from_ctrl;   // 1: past = prefix + ctrl->cur_len - 1 (decode); 0: past = past_len (prefill)
+  int past_from_ctrl;   // 1: past = prefix + ctrl->cur_len - 1 (decode, less row_shift(shift, b) in attention_decode_kernel); 0: past_len
   int past_len, prefix; // cache position of the first new row
+  const int* shift;     // decode: per-row position offsets of a ragged continuation (SampleArgs::shift), or nullptr
   int cross;            // 1: keys = kv_len encoder positions, no append, no causal structure
   int kv_len;
   int rope; const void* rope_cos; const void* rope_sin;  // [max_pos][64] tables in the model dtype (Q3)
@@ -114,7 +115,8 @@ struct EmbedArgs {
   const Ctrl* ctrl;
   int B, K, V1, H, P;  // P = prefix rows per batch in THIS call (0 at decode)
   int n_cols;          // code columns per batch row after the prefix (1 at decode)
-  int pos_from_ctrl, pos0, prefix_len;  // decode: position = prefix_len + cur_len - 1
+  int pos_from_ctrl, pos0, prefix_len;  // decode: position = prefix_len + cur_len - 1 - row_shift(shift, b)
+  const int* shift;    // decode: per-row position offsets of a ragged continuation (SampleArgs::shift), or nullptr
 };
 int launch_embed(const EmbedArgs& a, int dtype, cudaStream_t st, bool pdl);
 
@@ -126,6 +128,9 @@ struct SampleArgs {
   Ctrl* ctrl;
   const ptts_gen_params* gen;  // device copy
   int64_t* prefix_cells;       // [B*K][K-1] pattern cells past a multi-column input (nullptr: the session takes the BOS column only)
+  // [B] ragged continuation (ptts_generate_begin_ids2): row b's input is shift[b] columns shorter than the longest, and every
+  // column it reads or writes is the batch's cur_len - shift[b] (its own, starting at 0); nullptr: all rows share cur_len
+  int* shift;
   int B, K, V;
   int bos, pad, eos;
 };
@@ -144,14 +149,17 @@ int launch_sample(const SampleArgs& a, const int64_t* forced, cudaStream_t st, b
 constexpr ptts_logits_ext kLogitsExtOff = {nullptr, nullptr, nullptr, 0, -1, -1, 0, nullptr, 0, nullptr, nullptr, 1, 0};
 // the fused step kernels' sampling phase over n_ctas CTAs (passes of up to three rows per CTA), as a kernel of its own; no EXT
 int launch_sample_phase(const SampleArgs& a, int n_ctas, cudaStream_t st);
-// ids == nullptr: the BOS column (n0 = 1); otherwise the BOS-led [B*K][n0] input the generation continues from
-int launch_generate_begin(const SampleArgs& a, const int64_t* ids, int n0, int max_length, cudaStream_t st);
+// ids == nullptr: the BOS column (n0 = 1); otherwise the BOS-led [B*K][n0] input the generation continues from.  lens (with
+// a.shift): row b's input is its first lens[b] columns (in [1, n0]); the kernel writes a.shift[b] = n0 - lens[b]
+int launch_generate_begin(const SampleArgs& a, const int64_t* ids, int n0, int max_length, const int* lens, cudaStream_t st);
 int launch_delay_build(const int64_t* ids, int BK, int seq, int K, int64_t bos, int64_t pad, int L, int64_t* mask, cudaStream_t st);
 int launch_delay_apply(const int64_t* ids, int BK, int seq, int64_t ld_ids, const int64_t* mask, int64_t ld_mask, int64_t* out, cudaStream_t st);
 int launch_logits_processor(const int64_t* ids, int BK, int seq, int64_t ld_ids, float* scores, int V, int64_t eos, int K, int64_t* first_unf, cudaStream_t st);
 int launch_mask_convert(const int64_t* src, int n, int* dst, cudaStream_t st);  // int64 0/1 -> int32; src==nullptr -> ones
 int launch_cross_kv_relayout(const void* src, void* dst, int B, int S, int nckv, int dtype, cudaStream_t st);
-int launch_gather_rows(const void* src, int64_t ld_src, int64_t row0, int64_t row_step, void* dst, int rows, int cols, int dtype, cudaStream_t st);
+// dst row r = src row row0 + r * row_step - row_shift(shift, r)
+int launch_gather_rows(const void* src, int64_t ld_src, int64_t row0, int64_t row_step, const int* shift, void* dst, int rows, int cols,
+                       int dtype, cudaStream_t st);
 
 // ---- teacher-forced scoring (score.cu) ----------------------------------------------------------
 struct ScoreArgs {

@@ -183,6 +183,7 @@ struct WorkspaceLayout {
   int max_input;                   // largest decoder input (BOS column + code prefix) a generate() call may continue from
   int64_t ctrl, progress, gen, raw_ids, cur_ids, eos_seen, unfinished, first_unf, prompt_mask, enc_mask;
   int64_t prefix_cells;            // [BK][K-1] int64: delay-pattern cells just past the input (max_input > 1 only; -1 = none)
+  int64_t row_shift;               // [B] int32: per-row offsets of a ragged continuation (max_input > 1 only; -1 = none)
   int64_t x, qkv, attn, qc, hbuf, hidden, logits, scores, cross_tmp, cross_kv, self_kv;
   int64_t img_x, img_attn, img_h;  // fused step kernel: activations as tile images [chunk][32][H + 8] (step.cu stage_tile)
   int64_t cl_x, cl_attn, cl_h;     // cluster step kernel: K-sliced images [2][32][H/2 + 8], fc2's in quarters [4][32][F/4 + 8] (step2.cu)
@@ -217,6 +218,7 @@ static inline WorkspaceLayout make_workspace(const ptts_decoder_config& c, int B
   w.enc_mask = take((int64_t)(B / takes) * S * 4);
   w.prefix_cells = -1;
   if (max_input > 1 && c.num_codebooks > 1) w.prefix_cells = take((int64_t)w.BK * (c.num_codebooks - 1) * 8);
+  w.row_shift = max_input > 1 ? take((int64_t)B * 4) : -1;
   const int64_t rows_enc = (int64_t)B * S, rows_cross = (int64_t)(B / takes) * S;
   w.x = take((int64_t)w.Mmax * l.H * l.es);
   w.qkv = take((int64_t)w.Mmax * l.qkv_rows * l.es);

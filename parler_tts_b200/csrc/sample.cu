@@ -16,7 +16,7 @@
 
 namespace ptts {
 
-template <int ITEMS, bool EXT>
+template <int ITEMS, bool EXT, bool RAGGED>
 __device__ __forceinline__ void sample_kernel_body(const SampleArgs& p, const int64_t* __restrict__ forced, const ptts_sampling_ext& x,
                                                    const SampleOut& o, const ptts_logits_ext& lx) {
   pdl_launch_dependents();
@@ -25,7 +25,7 @@ __device__ __forceinline__ void sample_kernel_body(const SampleArgs& p, const in
   const int row = blockIdx.x;           // one CTA per (utterance, codebook) row
   const int cur_len = p.ctrl->cur_len;  // the new token becomes column `cur_len`
   const ptts_gen_params g = *p.gen;
-  sample_rows_cta<ITEMS, 1, EXT>(p, g, forced, row, 0, row + 1, cur_len, x, o, lx);
+  sample_rows_cta<ITEMS, 1, EXT, RAGGED>(p, g, forced, row, 0, row + 1, cur_len, x, o, lx);
   // last block advances the control block
   __threadfence();
   __syncthreads();
@@ -44,17 +44,17 @@ __device__ __forceinline__ void sample_kernel_body(const SampleArgs& p, const in
   }
 }
 
-template <int ITEMS>
+template <int ITEMS, bool RAGGED>
 __global__ void __launch_bounds__(SMP_THREADS) sample_kernel(SampleArgs p, const int64_t* __restrict__ forced) {
-  sample_kernel_body<ITEMS, false>(p, forced, ptts_sampling_ext{}, SampleOut{}, ptts_logits_ext{});
+  sample_kernel_body<ITEMS, false, RAGGED>(p, forced, ptts_sampling_ext{}, SampleOut{}, ptts_logits_ext{});
 }
 
 // the ptts_sampling_ext and ptts_logits_ext stages and the per-step outputs (sample_core.cuh, EXT = true); the knobs, the table
 // pointers and the output window come by value, so a captured graph holds them
-template <int ITEMS, bool EXT>
+template <int ITEMS, bool EXT, bool RAGGED>
 __global__ void __launch_bounds__(SMP_THREADS) sample_kernel(SampleArgs p, const int64_t* __restrict__ forced, ptts_sampling_ext x,
                                                              SampleOut o, ptts_logits_ext lx) {
-  sample_kernel_body<ITEMS, EXT>(p, forced, x, o, lx);
+  sample_kernel_body<ITEMS, EXT, RAGGED>(p, forced, x, o, lx);
 }
 
 int launch_sample(const SampleArgs& a, const int64_t* forced, cudaStream_t st, bool pdl, const ptts_sampling_ext* ext,
@@ -72,28 +72,31 @@ int launch_sample(const SampleArgs& a, const int64_t* forced, cudaStream_t st, b
   const int items = (a.V + SMP_THREADS - 1) / SMP_THREADS;
   PTTS_REQUIRE(items <= 9, "sample: vocab_size %d > 2304 not supported", a.V);
   PTTS_REQUIRE((out == nullptr && lext == nullptr) || ext != nullptr, "sample: the per-step outputs and the ptts_logits_ext stages need the EXT sampler");
+  const bool rg = a.shift != nullptr;
   if (ext != nullptr) {
     const SampleOut o = out ? *out : SampleOut{};
     const ptts_logits_ext lx = lext ? *lext : kLogitsExtOff;
-    if (items <= 1) PTTS_CHECK_CUDA(cudaLaunchKernelEx(&cfg, sample_kernel<1, true>, a, forced, *ext, o, lx));
-    else if (items <= 5) PTTS_CHECK_CUDA(cudaLaunchKernelEx(&cfg, sample_kernel<5, true>, a, forced, *ext, o, lx));
-    else PTTS_CHECK_CUDA(cudaLaunchKernelEx(&cfg, sample_kernel<9, true>, a, forced, *ext, o, lx));
+    auto fn = items <= 1 ? (rg ? sample_kernel<1, true, true> : sample_kernel<1, true, false>)
+            : items <= 5 ? (rg ? sample_kernel<5, true, true> : sample_kernel<5, true, false>)
+                         : (rg ? sample_kernel<9, true, true> : sample_kernel<9, true, false>);
+    PTTS_CHECK_CUDA(cudaLaunchKernelEx(&cfg, fn, a, forced, *ext, o, lx));
     return PTTS_OK;
   }
-  if (items <= 1) PTTS_CHECK_CUDA(cudaLaunchKernelEx(&cfg, sample_kernel<1>, a, forced));
-  else if (items <= 5) PTTS_CHECK_CUDA(cudaLaunchKernelEx(&cfg, sample_kernel<5>, a, forced));
-  else PTTS_CHECK_CUDA(cudaLaunchKernelEx(&cfg, sample_kernel<9>, a, forced));
+  auto fn = items <= 1 ? (rg ? sample_kernel<1, true> : sample_kernel<1, false>)
+          : items <= 5 ? (rg ? sample_kernel<5, true> : sample_kernel<5, false>)
+                       : (rg ? sample_kernel<9, true> : sample_kernel<9, false>);
+  PTTS_CHECK_CUDA(cudaLaunchKernelEx(&cfg, fn, a, forced));
   return PTTS_OK;
 }
 
 // ptts_op_sample_phase: the step kernels' sampling phase (sample_all_rows_cta, passes of up to three rows per CTA) over a grid of
 // n_ctas CTAs, on the session's logits.  cur_len stays where it is; the last CTA clears the counters the rows add to.
-template <int ITEMS>
+template <int ITEMS, bool RAGGED>
 __global__ void __launch_bounds__(SMP_THREADS) sample_phase_kernel(SampleArgs p) {
   if (p.ctrl->active == 0) return;
   const int cur_len = p.ctrl->cur_len;
   const ptts_gen_params g = *p.gen;
-  sample_all_rows_cta<ITEMS>(p, g, (int)blockIdx.x, (int)gridDim.x, p.B * p.K, cur_len);
+  sample_all_rows_cta<ITEMS, RAGGED>(p, g, (int)blockIdx.x, (int)gridDim.x, p.B * p.K, cur_len);
   __threadfence();
   __syncthreads();
   if (threadIdx.x == 0 && atomicAdd(&p.ctrl->done_blocks, 1) == (int)gridDim.x - 1) {
@@ -107,27 +110,34 @@ int launch_sample_phase(const SampleArgs& a, int n_ctas, cudaStream_t st) {
   const int items = (a.V + SMP_THREADS - 1) / SMP_THREADS;
   PTTS_REQUIRE(items <= 9, "sample: vocab_size %d > 2304 not supported", a.V);
   PTTS_REQUIRE(n_ctas >= 1, "op_sample_phase: n_ctas must be positive, got %d", n_ctas);
-  if (items <= 1) sample_phase_kernel<1><<<n_ctas, SMP_THREADS, 0, st>>>(a);
-  else if (items <= 5) sample_phase_kernel<5><<<n_ctas, SMP_THREADS, 0, st>>>(a);
-  else sample_phase_kernel<9><<<n_ctas, SMP_THREADS, 0, st>>>(a);
+  const bool rg = a.shift != nullptr;
+  auto fn = items <= 1 ? (rg ? sample_phase_kernel<1, true> : sample_phase_kernel<1, false>)
+          : items <= 5 ? (rg ? sample_phase_kernel<5, true> : sample_phase_kernel<5, false>)
+                       : (rg ? sample_phase_kernel<9, true> : sample_phase_kernel<9, false>);
+  fn<<<n_ctas, SMP_THREADS, 0, st>>>(a);
   PTTS_LAUNCH_CHECK();
   return PTTS_OK;
 }
 
-// build_delay_pattern_mask (modeling_parler_tts.py:214-276), cell c of row `row` (codebook k) for the BOS-led ids [B*K][seq]: the
-// id shifted by k, BOS over the lower triangle, PAD over the upper one (:261); -1 = free (predicted).  No pattern below 2K-1 columns.
-__device__ __forceinline__ int64_t delay_pattern_cell(const int64_t* ids, int row, int seq, int k, int K, int64_t bos, int64_t pad, int L, int c) {
+// build_delay_pattern_mask (modeling_parler_tts.py:214-276), cell c of row `row` (codebook k) for the BOS-led ids [B*K][ld], of
+// which the first seq columns are the row's input: the id shifted by k, BOS over the lower triangle, PAD over the upper one (:261);
+// -1 = free (predicted).  No pattern below 2K-1 columns.
+__device__ __forceinline__ int64_t delay_pattern_cell(const int64_t* ids, int row, int ld, int seq, int k, int K, int64_t bos, int64_t pad,
+                                                      int L, int c) {
   if (L < 2 * K - 1) return -1;
   const bool bos_pat = c <= k;
   const bool eos_pat = (c - k) >= (L - K + 1);
-  const int64_t shifted = (c >= k && c < seq + k) ? ids[(size_t)row * seq + (c - k)] : -1;
+  const int64_t shifted = (c >= k && c < seq + k) ? ids[(size_t)row * ld + (c - k)] : -1;
   return ((!bos_pat && !eos_pat) ? shifted : 0) + (bos_pat ? bos : 0) + (eos_pat ? pad : 0);
 }
 
 // ids == nullptr: the BOS column.  Otherwise the history starts with the delayed input: the first n0 columns of the pattern (:3523;
 // where the pattern is free -- max_length < 2K-1 -- the ids themselves), the K-1 cells after it are kept for the sampler's next-input
 // override, and eos_seen records the first EOS inside the input (ParlerTTSLogitsProcessor counts the whole history, :46).
-__global__ void generate_begin_kernel(SampleArgs p, const int64_t* __restrict__ ids, int n0, int L) {
+// lens != nullptr (ragged): row b does all of this with its own n0_b = lens[b] columns and its own limit L - (n0 - n0_b), exactly
+// as the row alone would; its history columns [n0_b, n0) get PAD (the prefill embeds them, and the decode steps overwrite their
+// K/V before any query reaches them), and shift[b] = n0 - n0_b.
+__global__ void generate_begin_kernel(SampleArgs p, const int64_t* __restrict__ ids, int n0, int L, const int* __restrict__ lens) {
   const int BK = p.B * p.K;
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i == 0) {
@@ -142,26 +152,33 @@ __global__ void generate_begin_kernel(SampleArgs p, const int64_t* __restrict__ 
       p.eos_seen[i] = 0;
     } else {
       const int k = i % p.K;
+      const int nb = lens != nullptr ? lens[i / p.K] : n0;   // this row's input columns
+      const int Lb = L - (n0 - nb);
       int64_t v = 0;
       int es = 0;
-      for (int c = 0; c < n0; c++) {
-        const int64_t m = delay_pattern_cell(ids, i, n0, k, p.K, p.bos, p.pad, L, c);
+      for (int c = 0; c < nb; c++) {
+        const int64_t m = delay_pattern_cell(ids, i, n0, nb, k, p.K, p.bos, p.pad, Lb, c);
         v = (m == -1) ? ids[(size_t)i * n0 + c] : m;
         p.raw_ids[(size_t)i * p.raw_ld + c] = v;
         if (v == p.eos && es == 0) es = c + 1;
       }
+      for (int c = nb; c < n0; c++) p.raw_ids[(size_t)i * p.raw_ld + c] = p.pad;
       p.cur_ids[i] = (int)v;
       p.eos_seen[i] = es;
       if (p.prefix_cells != nullptr)
-        for (int c = 0; c < p.K - 1; c++) p.prefix_cells[(size_t)i * (p.K - 1) + c] = delay_pattern_cell(ids, i, n0, k, p.K, p.bos, p.pad, L, n0 + c);
+        for (int c = 0; c < p.K - 1; c++)
+          p.prefix_cells[(size_t)i * (p.K - 1) + c] = delay_pattern_cell(ids, i, n0, nb, k, p.K, p.bos, p.pad, Lb, nb + c);
     }
     p.unfinished[i] = 1;
   }
-  if (i < p.B) { p.first_unf[i] = i * p.K; p.first_unf[p.B + i] = i * p.K; }
+  if (i < p.B) {
+    p.first_unf[i] = i * p.K; p.first_unf[p.B + i] = i * p.K;
+    if (lens != nullptr) p.shift[i] = n0 - lens[i];
+  }
 }
-int launch_generate_begin(const SampleArgs& a, const int64_t* ids, int n0, int max_length, cudaStream_t st) {
+int launch_generate_begin(const SampleArgs& a, const int64_t* ids, int n0, int max_length, const int* lens, cudaStream_t st) {
   const int n = a.B * a.K;
-  generate_begin_kernel<<<(n + 127) / 128, 128, 0, st>>>(a, ids, ids == nullptr ? 1 : n0, max_length);
+  generate_begin_kernel<<<(n + 127) / 128, 128, 0, st>>>(a, ids, ids == nullptr ? 1 : n0, max_length, lens);
   PTTS_LAUNCH_CHECK();
   return PTTS_OK;
 }
@@ -171,7 +188,7 @@ int launch_generate_begin(const SampleArgs& a, const int64_t* ids, int n0, int m
 __global__ void delay_build_kernel(const int64_t* ids, int BK, int seq, int K, int64_t bos, int64_t pad, int L, int64_t* mask) {
   const int row = blockIdx.x;
   const int k = row % K;
-  for (int c = threadIdx.x; c < L; c += blockDim.x) mask[(size_t)row * L + c] = delay_pattern_cell(ids, row, seq, k, K, bos, pad, L, c);
+  for (int c = threadIdx.x; c < L; c += blockDim.x) mask[(size_t)row * L + c] = delay_pattern_cell(ids, row, seq, seq, k, K, bos, pad, L, c);
 }
 int launch_delay_build(const int64_t* ids, int BK, int seq, int K, int64_t bos, int64_t pad, int L, int64_t* mask, cudaStream_t st) {
   delay_build_kernel<<<BK, 128, 0, st>>>(ids, BK, seq, K, bos, pad, L, mask);

@@ -73,7 +73,9 @@ __device__ __forceinline__ bool bitmap_has(const uint32_t* __restrict__ bits, in
 // is set, not a zeroed struct).  The masks among them (suppress, begin-suppress) join the single mask pass; while an additive,
 // forcing or InfNan stage acts on this step, the pass applies every stage per id in transformers' order instead (they do not
 // commute with the masks).  Additions and the decay product use __fadd_rn / __fmul_rn so that no FMA changes their rounding.
-template <int ITEMS, int R, bool EXT = false>
+// RAGGED = true reads each row's column from p.shift (a ragged continuation); RAGGED = false is the code of a uniform batch, in
+// which every row samples column cur_len (the callers pick the instantiation by p.shift != nullptr).
+template <int ITEMS, int R, bool EXT = false, bool RAGGED = false>
 __device__ __forceinline__ void sample_rows_cta(const SampleArgs& p, const ptts_gen_params& g, const int64_t* __restrict__ forced,
                                                 int row0, int stride, int n_rows, int cur_len, ptts_sampling_ext x = {},
                                                 SampleOut o = {}, ptts_logits_ext lx = {}) {
@@ -135,11 +137,13 @@ __device__ __forceinline__ void sample_rows_cta(const SampleArgs& p, const ptts_
 
   int row[R];
   bool valid[R];
+  int col[R];   // the column row r samples: its own history's (cur_len less the row's shift in a ragged continuation)
   float v[R][ITEMS];
 #pragma unroll
   for (int r = 0; r < R; r++) {
     row[r] = row0 + r * stride;
     valid[r] = row[r] < n_rows;
+    col[r] = cur_len - ((RAGGED && valid[r]) ? row_shift(p.shift, row[r] / p.K) : 0);
 #pragma unroll
     for (int j = 0; j < ITEMS; j++) {
       const int i = tid + SMP_THREADS * j;
@@ -167,8 +171,8 @@ __device__ __forceinline__ void sample_rows_cta(const SampleArgs& p, const ptts_
   // the tail's inputs (thread r finishes row r): requested now, consumed after the draw
   int t_unf = 0, t_es = 0;
   if (tid < R && row0 + tid * stride < n_rows) { t_unf = p.unfinished[row0 + tid * stride]; t_es = p.eos_seen[row0 + tid * stride]; }
-  // NoRepeatNGram over the row's history, columns [0, cur_len): every i in [0, cur_len - n] whose ids[i, i + n - 1) equal the last
-  // n - 1 ids bans ids[i + n - 1].  Nothing is banned while cur_len + 1 < n.
+  // NoRepeatNGram over the row's history, columns [0, col): every i in [0, col - n] whose ids[i, i + n - 1) equal the last
+  // n - 1 ids bans ids[i + n - 1].  Nothing is banned while col + 1 < n (cur_len is the largest col of the batch).
   const int ngram = EXT ? x.no_repeat_ngram_size : 0;
   const bool bans = EXT && ngram > 0 && cur_len + 1 >= ngram;
   if constexpr (EXT) {
@@ -180,10 +184,10 @@ __device__ __forceinline__ void sample_rows_cta(const SampleArgs& p, const ptts_
       __syncthreads();
 #pragma unroll
       for (int r = 0; r < R; r++) {
-        if (!valid[r]) continue;
+        if (!valid[r] || col[r] + 1 < ngram) continue;
         const int64_t* h = p.raw_ids + (size_t)row[r] * p.raw_ld;
-        const int64_t* tail = h + cur_len - ngram + 1;
-        for (int i = tid; i <= cur_len - ngram; i += SMP_THREADS) {
+        const int64_t* tail = h + col[r] - ngram + 1;
+        for (int i = tid; i <= col[r] - ngram; i += SMP_THREADS) {
           bool match = true;
           for (int q = 0; q < ngram - 1 && match; q++) match = h[i + q] == tail[q];
           const int64_t t = h[i + ngram - 1];
@@ -193,13 +197,21 @@ __device__ __forceinline__ void sample_rows_cta(const SampleArgs& p, const ptts_
       __syncthreads();
     }
   }
-  // ptts_logits_ext: which stages act on this column
+  // ptts_logits_ext: which stages act on this column.  ForcedEOS, the decay and MinNewTokens count from the input's end or the
+  // limit, which a ragged row has at the same batch column as every other row (its n0 and max_length are the batch's less its
+  // shift), so they stay on cur_len; ForcedBOS and begin-suppress test the row's own column.
   const bool seq_bias = EXT && (lx.bias1 != nullptr || lx.n_seq > 0);
-  const bool forced_bos = EXT && lx.forced_bos_token_id >= 0 && cur_len == 1;
   const bool forced_eos = EXT && lx.forced_eos_token_id >= 0 && cur_len == g.max_length - 1;
   const bool decay = EXT && lx.decay != nullptr && cur_len > lx.decay_start;
-  const bool begin_sup = EXT && lx.begin_suppress != nullptr && cur_len == lx.begin_index;
-  const bool chain = seq_bias || forced_bos || forced_eos || decay || (EXT && lx.remove_invalid_values);
+  bool forced_bos[R], begin_sup[R];
+#pragma unroll
+  for (int r = 0; r < R; r++) {
+    forced_bos[r] = EXT && lx.forced_bos_token_id >= 0 && col[r] == 1;
+    // a ragged row continuing from the BOS column alone begins one column later under a forced BOS, as it would alone
+    const int sh = cur_len - col[r];
+    const int begin = lx.begin_index - sh + ((sh > 0 && g.input_len - sh == 1 && lx.forced_bos_token_id >= 0) ? 1 : 0);
+    begin_sup[r] = EXT && lx.begin_suppress != nullptr && col[r] == begin;
+  }
   if constexpr (EXT) {
     if (lx.n_seq > 0) {  // one thread per (row, sequence): does the history end with the sequence's first len - 1 ids?
       SmpSeq& sq = smp_seq();
@@ -209,8 +221,8 @@ __device__ __forceinline__ void sample_rows_cta(const SampleArgs& p, const ptts_
           const int32_t* e = lx.seq + q * (1 + PTTS_SEQ_BIAS_MAX_LEN);
           const int len = e[0];
           int last = -1;
-          if (valid[r] && len >= 2 && len <= PTTS_SEQ_BIAS_MAX_LEN && len <= cur_len) {
-            const int64_t* h = p.raw_ids + (size_t)row[r] * p.raw_ld + cur_len - (len - 1);
+          if (valid[r] && len >= 2 && len <= PTTS_SEQ_BIAS_MAX_LEN && len <= col[r]) {
+            const int64_t* h = p.raw_ids + (size_t)row[r] * p.raw_ld + col[r] - (len - 1);
             bool match = true;
             for (int t = 0; t < len - 1 && match; t++) match = h[t] == e[1 + t];
             if (match) last = e[len];
@@ -235,14 +247,14 @@ __device__ __forceinline__ void sample_rows_cta(const SampleArgs& p, const ptts_
       const int par = cur_len & 1;
       int fu = p.first_unf[par * p.B + b];
       // eos_seen[r] = 1 + column of row r's first EOS (0 = none).  The reference counts EOS over input_ids, i.e. columns
-      // < cur_len (logits_processors.py:46): an EOS written by another CTA during THIS step (column cur_len) must not count,
+      // < col (logits_processors.py:46): an EOS written by another CTA during THIS step (column col) must not count,
       // so the test is on the column, not on a flag (rows of one batch item are sampled by different CTAs).
       const int es = __ldcg(p.eos_seen + fu);
-      if (es > 0 && es <= cur_len && fu < b * p.K + p.K - 1) fu++;
+      if (es > 0 && es <= col[r] && fu < b * p.K + p.K - 1) fu++;
       if (k == 0 && tid == 0) p.first_unf[(par ^ 1) * p.B + b] = fu;
       if (row[r] > fu) mask_eos = mask_par = true;
     }
-    if (chain) {
+    if (seq_bias || forced_bos[r] || forced_eos || decay || (EXT && lx.remove_invalid_values)) {
       // transformers' order: SequenceBias, NoRepeatNGram, MinNewTokens, ForcedBOS, ForcedEOS, InfNan, ExponentialDecay, Suppress,
       // SuppressAtBegin, ParlerTTS (the custom list is merged last); suppress_special (a bench aid) goes with the last mask
       const float mult = decay ? __ldg(lx.decay + cur_len) : 0.f;
@@ -259,12 +271,12 @@ __device__ __forceinline__ void sample_rows_cta(const SampleArgs& p, const ptts_
         }
         if (bans && ((smp_bans()[r][i >> 5] >> (i & 31)) & 1u)) y = -INFINITY;
         if (mask_min && i == p.eos) y = -INFINITY;
-        if (forced_bos) y = (i == lx.forced_bos_token_id) ? 0.f : -INFINITY;
+        if (forced_bos[r]) y = (i == lx.forced_bos_token_id) ? 0.f : -INFINITY;
         if (forced_eos) y = (i == lx.forced_eos_token_id) ? 0.f : -INFINITY;
         if (lx.remove_invalid_values) y = (y != y) ? 0.f : (y == INFINITY ? FLT_MAX : (y == -INFINITY ? -FLT_MAX : y));
         if (decay) y = __fadd_rn(y, i == p.eos ? __fmul_rn(fabsf(y), mult) : 0.f);   // scores + penalties (0 off EOS)
         if (lx.suppress != nullptr && bitmap_has(lx.suppress, i)) y = -INFINITY;
-        if (begin_sup && bitmap_has(lx.begin_suppress, i)) y = -INFINITY;
+        if (begin_sup[r] && bitmap_has(lx.begin_suppress, i)) y = -INFINITY;
         if (mask_par && i == p.eos) y = -INFINITY;
         if (g.suppress_special && i >= g.codebook_size) y = -INFINITY;
         v[r][j] = y;
@@ -279,7 +291,7 @@ __device__ __forceinline__ void sample_rows_cta(const SampleArgs& p, const ptts_
       if constexpr (EXT) {
         if (bans && ((smp_bans()[r][i >> 5] >> (i & 31)) & 1u)) v[r][j] = -INFINITY;
         if (i < p.V && lx.suppress != nullptr && bitmap_has(lx.suppress, i)) v[r][j] = -INFINITY;
-        if (i < p.V && begin_sup && bitmap_has(lx.begin_suppress, i)) v[r][j] = -INFINITY;
+        if (i < p.V && begin_sup[r] && bitmap_has(lx.begin_suppress, i)) v[r][j] = -INFINITY;
       }
     }
   }
@@ -450,7 +462,7 @@ __device__ __forceinline__ void sample_rows_cta(const SampleArgs& p, const ptts_
     int found[R], last_nz[R];
 #pragma unroll
     for (int r = 0; r < R; r++) {
-      target[r] = philox_uniform(g.seed, (uint32_t)(row[r] + g.row_base), (uint32_t)cur_len) * s[r];
+      target[r] = philox_uniform(g.seed, (uint32_t)(row[r] + g.row_base), (uint32_t)col[r]) * s[r];
       carry[r] = 0.f; found[r] = -1; last_nz[r] = -1;
     }
 #pragma unroll
@@ -585,30 +597,34 @@ __device__ __forceinline__ void sample_rows_cta(const SampleArgs& p, const ptts_
     }
   }
   // thread r finishes row r (the rows are independent: each owns its entries of every array below)
-  int my_tok = 0, my_row = 0;
+  int my_tok = 0, my_row = 0, my_col = 0;
   bool my_valid = false;
 #pragma unroll
   for (int r = 0; r < R; r++)
-    if (tid == r) { my_tok = tok[r]; my_row = row[r]; my_valid = valid[r]; }
+    if (tid == r) { my_tok = tok[r]; my_row = row[r]; my_valid = valid[r]; my_col = col[r]; }
   if (tid < R && my_valid) {
     const int b = my_row / p.K, k = my_row - b * p.K;
     int t = my_tok;
     if (forced != nullptr) t = (int)forced[my_row];
     if (!t_unf) t = p.pad;  // next_tokens * unfinished + pad * (1 - unfinished)
-    p.raw_ids[(size_t)my_row * p.raw_ld + cur_len] = t;
-    if (t == p.eos && t_es == 0) p.eos_seen[my_row] = cur_len + 1;
+    p.raw_ids[(size_t)my_row * p.raw_ld + my_col] = t;
+    if (t == p.eos && t_es == 0) p.eos_seen[my_row] = my_col + 1;
+    // the row's own limit max_length - shift is reached at the batch's max_length
     const int new_len = cur_len + 1;
     const int done = (t == p.eos) || (new_len >= g.max_length);
     const int still_unfinished = t_unf && !done;
     p.unfinished[my_row] = still_unfinished;
-    // delay-pattern override of the NEXT model input (column `cur_len`), build_delay_pattern_mask :252-261
+    // delay-pattern override of the NEXT model input (column `my_col`), build_delay_pattern_mask :252-261, with the row's own
+    // limit Lb and input length nb
+    const int sh = cur_len - my_col;
+    const int Lb = g.max_length - sh, nb = g.input_len - sh;
     int nxt = t;
-    if (g.max_length >= 2 * p.K - 1) {
-      const bool is_bos = cur_len <= k;
-      const bool is_pad = (cur_len - k) >= (g.max_length - p.K + 1);
+    if (Lb >= 2 * p.K - 1) {
+      const bool is_bos = my_col <= k;
+      const bool is_pad = (my_col - k) >= (Lb - p.K + 1);
       if (is_bos || is_pad) nxt = (is_bos ? p.bos : 0) + (is_pad ? p.pad : 0);
       // continuing from n0 input columns: codebook k's prefix ids reach up to column n0-1+k, past the delayed input (:246-248)
-      else if (g.input_len > 1 && cur_len - g.input_len < k) nxt = (int)p.prefix_cells[(size_t)my_row * (p.K - 1) + (cur_len - g.input_len)];
+      else if (nb > 1 && my_col - nb < k) nxt = (int)p.prefix_cells[(size_t)my_row * (p.K - 1) + (my_col - nb)];
     }
     p.cur_ids[my_row] = nxt;
     if (still_unfinished) atomicAdd(&p.ctrl->n_unfinished, 1);
@@ -623,12 +639,12 @@ __device__ __forceinline__ void sample_row_cta(const SampleArgs& p, const ptts_g
 }
 
 // all rows of the token over the CTAs of a fused step kernel: passes of up to three rows per CTA
-template <int ITEMS>
+template <int ITEMS, bool RAGGED = false>
 __device__ __forceinline__ void sample_all_rows_cta(const SampleArgs& p, const ptts_gen_params& g, int cta, int n_ctas, int n_rows, int cur_len) {
   if (n_rows <= n_ctas) {
-    if (cta < n_rows) sample_rows_cta<ITEMS, 1>(p, g, nullptr, cta, n_ctas, n_rows, cur_len);
+    if (cta < n_rows) sample_rows_cta<ITEMS, 1, false, RAGGED>(p, g, nullptr, cta, n_ctas, n_rows, cur_len);
   } else {
-    for (int row0 = cta; row0 < n_rows; row0 += 3 * n_ctas) sample_rows_cta<ITEMS, 3>(p, g, nullptr, row0, n_ctas, n_rows, cur_len);
+    for (int row0 = cta; row0 < n_rows; row0 += 3 * n_ctas) sample_rows_cta<ITEMS, 3, false, RAGGED>(p, g, nullptr, row0, n_ctas, n_rows, cur_len);
   }
 }
 

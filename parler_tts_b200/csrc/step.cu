@@ -118,6 +118,7 @@ __device__ __forceinline__ void prefetch_kv(const StepParams& p, int l, int pos)
     const size_t vofs = (size_t)p.B * p.nkv * p.Tmax * HD * 2;
     for (int it = blockIdx.x + gridDim.x * pw; it < p.B * p.nkv; it += gridDim.x * 4) {  // (any warp may prefetch any item)
       const char* k = kc + (size_t)it * p.Tmax * HD * 2;  // [B][nkv][Tmax][64]: item-major
+      // (a ragged continuation's shorter rows get the batch's length: a hint inside the row's cache, never read as keys)
       l2_prefetch(k, (uint32_t)(pos * HD * 2));
       l2_prefetch(k + vofs, (uint32_t)(pos * HD * 2));
     }
@@ -321,6 +322,7 @@ __device__ __forceinline__ void run_gemm(const StepParams& p, Smem& sm, const Ge
 
 // Attention phase: one warp per (batch row, kv head) item, TMA-staged K/V.  Items are dealt round-robin over
 // CTAs first (item i -> CTA i % grid, warp i / grid) so all SMs pull K/V, 3-4 warps each at Mini/B=32.
+template <bool RAGGED>
 __device__ __forceinline__ void attn_phase(const StepParams& p, Smem& sm, const AttnArgs& a, int nkv, int pos, uint32_t& att_parity, int ph) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   unsigned char* region = sm.scratch + (size_t)warp * attn_decode_smem_per_warp<bf16>();
@@ -330,10 +332,10 @@ __device__ __forceinline__ void attn_phase(const StepParams& p, Smem& sm, const 
   float* xch = reinterpret_cast<float*>(sm.scratch + (size_t)ST_WARPS * attn_decode_smem_per_warp<bf16>()) + pair * 128;
   __syncthreads();  // the tile / reduction scratch of the previous GEMM phase is dead
   for (int it = blockIdx.x + gridDim.x * pair; it < items; it += gridDim.x * (ST_WARPS / 2))
-    attention_decode_item_warp<bf16>(a, it / nkv, it % nkv, pos, region, bars, lane, att_parity, part, 2, xch, pair + 1);
+    attention_decode_item_warp<bf16>(a, it / nkv, it % nkv, row_pos<RAGGED>(p, it / nkv, pos), region, bars, lane, att_parity, part, 2, xch, pair + 1);
 }
 
-template <int ITEMS>
+template <int ITEMS, bool RAGGED>
 __global__ void __launch_bounds__(ST_THREADS, 1) decode_step_kernel(const __grid_constant__ StepParams p) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   Ctrl* ctrl = p.sa.ctrl;
@@ -395,7 +397,7 @@ __global__ void __launch_bounds__(ST_THREADS, 1) decode_step_kernel(const __grid
     for (int it = blockIdx.x; it < p.B * cpr; it += gridDim.x) {
       const int b = it / cpr, c = (it - b * cpr) * ST_THREADS + tid;
       if (c >= H) continue;
-      p.x[(size_t)b * sm.pitch + c] = __float2bfloat16_rn(embed_value(p, b, c, pos));
+      p.x[(size_t)b * sm.pitch + c] = __float2bfloat16_rn(embed_value(p, b, c, row_pos<RAGGED>(p, b, pos)));
     }
   }
   prof_mark(sm.prof, 6);
@@ -418,7 +420,7 @@ __global__ void __launch_bounds__(ST_THREADS, 1) decode_step_kernel(const __grid
       } else {         // cross-attention over the cached encoder K/V
         a.q = p.qc; a.ldq = H;
       }
-      attn_phase(p, sm, a, a.nkv, pos, att_parity, ph);
+      attn_phase<RAGGED>(p, sm, a, a.nkv, pos, att_parity, ph);
     } else {
       // Activations live in tile images (row pitch H + 8, see stage_tile).  Each GEMM phase also pulls the matrix the
       // SAME phase of the next layer will use into L2 (PrefetchJob), so the HBM stream is spread over the layer;
@@ -498,7 +500,7 @@ __global__ void __launch_bounds__(ST_THREADS, 1) decode_step_kernel(const __grid
   if (p.do_sample_phase) {
     const ptts_gen_params gp = *p.sa.gen;
     const int BK = p.B * p.K;
-    sample_phase<ITEMS>(p.sa, gp, BK, cur_len);
+    sample_phase<ITEMS, RAGGED>(p.sa, gp, BK, cur_len);
     prof_mark(sm.prof, 1);
     bar_target = grid_sync(bar_ctr, bar_target, 0, true);
     prof_mark(sm.prof, 2);
@@ -553,11 +555,12 @@ int launch_decode_step(const StepParams& p, int grid, cudaStream_t st) {
   const int smem = (int)(ST_HEADER + p.tile_region_bytes);
   void* args[] = {(void*)&p};
   const void* fn;
-  if (p.sample_items <= 1) fn = (const void*)decode_step_kernel<1>;
-  else if (p.sample_items <= 5) fn = (const void*)decode_step_kernel<5>;
-  else fn = (const void*)decode_step_kernel<9>;
-  static int attr_done[3] = {0, 0, 0};
-  const int fi = p.sample_items <= 1 ? 0 : (p.sample_items <= 5 ? 1 : 2);
+  const bool rg = p.sa.shift != nullptr;
+  if (p.sample_items <= 1) fn = rg ? (const void*)decode_step_kernel<1, true> : (const void*)decode_step_kernel<1, false>;
+  else if (p.sample_items <= 5) fn = rg ? (const void*)decode_step_kernel<5, true> : (const void*)decode_step_kernel<5, false>;
+  else fn = rg ? (const void*)decode_step_kernel<9, true> : (const void*)decode_step_kernel<9, false>;
+  static int attr_done[6] = {0, 0, 0, 0, 0, 0};
+  const int fi = (p.sample_items <= 1 ? 0 : (p.sample_items <= 5 ? 1 : 2)) + (rg ? 3 : 0);
   if (!attr_done[fi]) {
     PTTS_CHECK_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, ST_SMEM_LIMIT));
     attr_done[fi] = 1;

@@ -200,7 +200,7 @@ __device__ __forceinline__ bool weight_job(const StepParams& p, int j, int cta, 
   return true;
 }
 
-template <int ITEMS>
+template <int ITEMS, bool RAGGED>
 __global__ void __launch_bounds__(THREADS, 1) decode_step_cluster_kernel(const __grid_constant__ StepParams p) {
   extern __shared__ __align__(128) unsigned char smem[];
   Ctrl* ctrl = p.sa.ctrl;
@@ -287,7 +287,7 @@ __global__ void __launch_bounds__(THREADS, 1) decode_step_cluster_kernel(const _
   // ---- embeddings: this CTA's 32 x 8 slice of sum_k embed_k[id] (+ position) -> residual slice + x image -----------------
   {
     const int row = tid >> 3, f = tid & 7, n = cta * 8 + f;
-    const float v = row < B ? embed_value(p, row, n, pos) : 0.f;
+    const float v = row < B ? embed_value(p, row, n, row_pos<RAGGED>(p, row, pos)) : 0.f;
     res_s[row * 8 + f] = v;
     x_img[(size_t)xo_slice * x_slice_elems + row * pitch + xo_col + f] = __float2bfloat16_rn(v);
   }
@@ -366,8 +366,10 @@ __global__ void __launch_bounds__(THREADS, 1) decode_step_cluster_kernel(const _
       if (sub == PH_QC) return Rg + ATT_S0_QC + warp * ATT_STAGE;
       return warp < 6 ? Rg + ATT_S0_QKV + warp * ATT_STAGE : smem + HDR + (warp - 6) * WB_BYTES + ATT_S0_WB;
     };
+    // The request is sized by the row's own position (row_pos): a ragged continuation's shorter rows never read the slots past it.
     if (rowpart && att_row < B)
-      attention_decode_request<bf16>(decode_attn_args(p, l, pos, sub == PH_QC), att_row, head, pos, att_stage0(), attbars + 2 * warp, lane, warp & 1, 2);
+      attention_decode_request<bf16>(decode_attn_args(p, l, pos, sub == PH_QC), att_row, head, row_pos<RAGGED>(p, att_row, pos), att_stage0(),
+                                     attbars + 2 * warp, lane, warp & 1, 2);
 
     // folded-LayerNorm vectors of this phase's features: requested now, parked in shared memory after the MMA loop (a global
     // load followed at once by its shared-memory store would park the warp for an L2 round trip in front of the MMAs)
@@ -606,7 +608,7 @@ __global__ void __launch_bounds__(THREADS, 1) decode_step_cluster_kernel(const _
         unsigned char* rest = warp < 2 ? Rg + (size_t)warp * ATT_REST : held + (size_t)(warp - 2) * ATT_REST;
         float* xr = reinterpret_cast<float*>(other + 16384) + (warp >> 1) * 128;
         prof_mark(prof, 10);
-        attention_decode_sweep<bf16>(att, att_row, head, pos, att_stage0(), rest, attbars + 2 * warp, lane, att_parity, warp & 1, 2, xr, (warp >> 1) + 1,
+        attention_decode_sweep<bf16>(att, att_row, head, row_pos<RAGGED>(p, att_row, pos), att_stage0(), rest, attbars + 2 * warp, lane, att_parity, warp & 1, 2, xr, (warp >> 1) + 1,
                                      true, tid == 0 ? prof : nullptr);
       }
       prof_mark(prof, 5);
@@ -742,7 +744,7 @@ __global__ void __launch_bounds__(THREADS, 1) decode_step_cluster_kernel(const _
   if (p.do_sample_phase) {
     const ptts_gen_params gp = *p.sa.gen;
     const int BK = B * p.K;
-    sample_phase<ITEMS>(p.sa, gp, BK, cur_len);
+    sample_phase<ITEMS, RAGGED>(p.sa, gp, BK, cur_len);
     prof_mark(prof, 1);
     // every CTA learns whether any row is still unfinished: thread 0 reads the counter the moment the barrier opens (after its
     // acquire fence); the counter is reset only when the launch ends, so a step's count is the growth since the previous step
@@ -806,9 +808,10 @@ int cluster_pack_layer(const DecoderLayout& L, char* layer, cudaStream_t st) {
 }
 
 static const void* cluster_kernel_fn(const StepParams& p) {
-  if (p.sample_items <= 1) return (const void*)cl::decode_step_cluster_kernel<1>;
-  if (p.sample_items <= 5) return (const void*)cl::decode_step_cluster_kernel<5>;
-  return (const void*)cl::decode_step_cluster_kernel<9>;
+  const bool rg = p.sa.shift != nullptr;
+  if (p.sample_items <= 1) return rg ? (const void*)cl::decode_step_cluster_kernel<1, true> : (const void*)cl::decode_step_cluster_kernel<1, false>;
+  if (p.sample_items <= 5) return rg ? (const void*)cl::decode_step_cluster_kernel<5, true> : (const void*)cl::decode_step_cluster_kernel<5, false>;
+  return rg ? (const void*)cl::decode_step_cluster_kernel<9, true> : (const void*)cl::decode_step_cluster_kernel<9, false>;
 }
 
 static void cluster_launch_config(const StepParams& p, cudaLaunchConfig_t& cfg, cudaLaunchAttribute* at, cudaStream_t st) {

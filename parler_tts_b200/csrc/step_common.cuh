@@ -8,6 +8,13 @@
 
 namespace ptts {
 
+// Cache position of batch row b's token when the batch's is `pos` (a ragged continuation's rows run SampleArgs::shift behind).
+// Every per-row use of the position -- embedding, K/V append slot, causal key count, RoPE, K/V chunk requests -- goes through it.
+// The step kernels are instantiated with RAGGED = false (a uniform batch: the code without any offset) and true, launched by
+// p.sa.shift != nullptr.
+template <bool RAGGED>
+__device__ __forceinline__ int row_pos(const StepParams& p, int b, int pos) { return RAGGED ? pos - row_shift(p.sa.shift, b) : pos; }
+
 // Input embedding of batch row `row`, column `col`, for the token fed at cache position `pos`: the K codebook embeddings of the
 // row's current ids added left to right with a bf16 rounding after each add, then the position embedding (models without
 // rope).  Codebooks go in groups of 8: the loads of a group are in flight together, and the group's values are all that is live.
@@ -54,9 +61,9 @@ __device__ __forceinline__ AttnArgs decode_attn_args(const StepParams& p, int l,
 
 // Sampling phase: logits -> next token of every (utterance, codebook) row, one CTA per row (sample_core.cuh).  Not inlined: the
 // sampler's registers then do not add to the decode phases' in the kernel's allocation.
-template <int ITEMS>
+template <int ITEMS, bool RAGGED>
 __device__ __noinline__ void sample_phase(const SampleArgs& sa, const ptts_gen_params& gp, int BK, int cur_len) {
-  sample_all_rows_cta<ITEMS>(sa, gp, (int)blockIdx.x, (int)gridDim.x, BK, cur_len);
+  sample_all_rows_cta<ITEMS, RAGGED>(sa, gp, (int)blockIdx.x, (int)gridDim.x, BK, cur_len);
 }
 
 }  // namespace ptts

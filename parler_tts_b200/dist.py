@@ -27,7 +27,7 @@ def shard_row_base(n: int, rank: int, world: int, num_codebooks: int) -> int:
 
 def shard_batch(tensors: dict, rank: int, world: int) -> dict:
     """Slice every [B, ...] tensor of a generate() kwarg dict to this rank's utterances.  `decoder_input_ids` ([B * K, N] audio
-    codes) is split by its K-row groups, one group per utterance."""
+    codes) is split by its K-row groups, one group per utterance, and a list of `input_values` clips by its items."""
     B = next(v.shape[0] for k, v in tensors.items() if isinstance(v, torch.Tensor) and k != "decoder_input_ids")
     lo, hi = shard_range(B, rank, world)
     out = {}
@@ -37,6 +37,8 @@ def shard_batch(tensors: dict, rank: int, world: int) -> dict:
                 raise ValueError(f"decoder_input_ids has {v.shape[0]} rows, not a multiple of the batch size {B}")
             K = v.shape[0] // B
             out[k] = v[lo * K:hi * K]
+        elif k == "input_values" and isinstance(v, (list, tuple)):   # one clip per utterance (a ragged continuation)
+            out[k] = list(v[lo:hi])
         else:
             out[k] = v[lo:hi] if isinstance(v, torch.Tensor) and v.shape[0] == B else v
     return out

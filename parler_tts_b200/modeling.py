@@ -80,6 +80,56 @@ def prepare_decoder_input_ids(decoder_input_ids, batch_size: int, num_codebooks:
     return ids.contiguous()
 
 
+def prepare_ragged_decoder_input_ids(decoder_input_ids, decoder_attention_mask, batch_size: int, num_codebooks: int, vocab_size: int,
+                                     decoder_start_token_id: int, device) -> tuple[torch.Tensor, torch.Tensor]:
+    """generate()'s `decoder_input_ids` with a `decoder_attention_mask` [B, N] (code prefixes of different lengths) -> (the
+    BOS-led decoder input [B * K, n0] int64 on `device`, input_lens [B] int32 on `device`: row b's own columns n0_b, BOS included).
+
+    The mask must be right padding (ones, then zeros); row b's prefix is its first m_b frames, 0 <= m_b <= N, and the ids past it
+    are never read.  The BOS column is prepended as prepare_decoder_input_ids does, deciding on the rows that have frames (all
+    rows when none has), and a one goes in front of the mask with it (:3025-3031): n0_b = m_b + 1, so a row with m_b = 0 is the
+    BOS column alone.  Without the prepended column every row needs m_b >= 1.  n0 = max n0_b; ids in the valid region must lie
+    in [0, vocab_size]."""
+    B, K, V = int(batch_size), int(num_codebooks), int(vocab_size)
+    ids = torch.as_tensor(decoder_input_ids)
+    if ids.is_floating_point() or ids.is_complex() or ids.dtype == torch.bool:
+        raise ValueError(f"decoder_input_ids must hold integer audio codes, got {ids.dtype}")
+    N = ids.shape[-1] if ids.dim() >= 1 else 0
+    if N < 1 or ids.numel() != B * K * N:
+        raise ValueError(f"decoder_input_ids must have batch_size * num_codebooks = {B * K} rows of codes, got shape {tuple(ids.shape)}")
+    m = torch.as_tensor(decoder_attention_mask)
+    if m.dim() != 2 or tuple(m.shape) != (B, N):
+        raise ValueError(f"decoder_attention_mask must be [batch_size, frames] = [{B}, {N}], got {tuple(m.shape)}")
+    m = m.to(device="cpu")
+    if m.is_floating_point() or m.is_complex():
+        raise ValueError(f"decoder_attention_mask must hold 0 / 1 integers, got {m.dtype}")
+    m = m.to(torch.int64)
+    if bool(((m != 0) & (m != 1)).any()) or bool((m[:, 1:] > m[:, :-1]).any()):
+        raise ValueError("decoder_attention_mask must be right padding: ones, then zeros, in every row")
+    frames = m.sum(dim=1)                                                          # m_b
+    ids = ids.reshape(B * K, N).to(dtype=torch.int64)
+    valid = (torch.arange(N)[None, :] < frames.repeat_interleave(K)[:, None]).to(ids.device)
+    if bool(valid.any()):
+        lo, hi = int(ids[valid].min()), int(ids[valid].max())
+        if lo < 0 or hi > V:
+            raise ValueError(f"decoder_input_ids must lie in [0, vocab_size = {V}] inside the mask, got values in [{lo}, {hi}]")
+    with_frames = (frames > 0).repeat_interleave(K).to(ids.device)
+    prepend = not bool(with_frames.any()) or bool((ids[with_frames, 0] != decoder_start_token_id).all())
+    if prepend:
+        ids = torch.cat([torch.full((B * K, 1), int(decoder_start_token_id), dtype=torch.int64, device=ids.device), ids], dim=1)
+        frames = frames + 1
+    elif bool((frames == 0).any()):
+        raise ValueError("decoder_attention_mask: a row without frames needs the BOS column, but the codes already start with it "
+                         "(pass the rows without their BOS column)")
+    n0 = int(frames.max())
+    return ids[:, :n0].to(device).contiguous(), frames.to(device=device, dtype=torch.int32)
+
+
+def ragged_offsets(input_lens: torch.Tensor) -> torch.Tensor:
+    """Per-row offsets s_b = n0 - n0_b of a ragged continuation: row b's columns run s_b behind the batch's."""
+    return input_lens.max() - input_lens
+
+
 def check_continuation_length(n0: int, prompt_len: int, max_length: int, max_position_embeddings: int):
     """A continuation from n0 input columns must leave a new column within max_length, and the prompt prefix plus max_length
     positions must fit the position table."""
@@ -105,6 +155,28 @@ def expand_takes(ids: torch.Tensor, batch_size: int, num_codebooks: int, takes: 
     """[B * K, n] utterance-major code rows -> [B * takes * K, n]: the K rows of utterance b, as one group, once for each of its
     takes, so that take j of utterance b is utterance b * takes + j (never a repeat of single [B * K] rows)."""
     return ids.reshape(batch_size, num_codebooks, -1).repeat_interleave(takes, dim=0).reshape(batch_size * takes * num_codebooks, -1)
+
+
+def check_ragged_generate(streamer, logits_processor, stopping_criteria, gc):
+    """What generate() refuses with code prefixes of different lengths (a decoder_attention_mask or a list of input_values): the
+    streamer and the caller's processors / criteria (the host-driven loop hands them one rectangular input_ids),
+    output_attentions / output_hidden_states / return_token_timestamps (their probes take one position for the batch), and
+    min_length without min_new_tokens (it counts each row's own prefix, which one min_new_tokens for the batch cannot)."""
+    bad = []
+    if streamer is not None:
+        bad.append("streamer")
+    if logits_processor:
+        bad.append("logits_processor")
+    if stopping_criteria:
+        bad.append("stopping_criteria")
+    for k in ("output_attentions", "output_hidden_states", "return_token_timestamps"):
+        if getattr(gc, k, False):
+            bad.append(k)
+    if gc.min_new_tokens is None and (getattr(gc, "min_length", 0) or 0) > 0:
+        bad.append("min_length (pass min_new_tokens)")
+    if bad:
+        raise ValueError(f"code prefixes of different lengths (decoder_attention_mask, or a list of input_values) do not support "
+                         f"{', '.join(bad)}")
 
 
 def take_shards(batch_size: int, takes: int, limit: Optional[int]) -> list[tuple[int, int, int, int]]:
@@ -761,9 +833,11 @@ class GenSession:
 
     def begin(self, max_length: int, do_sample=False, temperature=1.0, top_k=0, top_p=1.0, min_new_tokens=0, seed=0,
               suppress_special=False, codebook_size=1024, row_base=0, input_ids: Optional[torch.Tensor] = None,
-              ext: Optional[dict] = None, lext: Optional[LogitsExt] = None):
+              ext: Optional[dict] = None, lext: Optional[LogitsExt] = None, input_lens: Optional[torch.Tensor] = None):
         """input_ids: None (the BOS column) or the BOS-led decoder input [B*K, n0] the generation continues from; the history
         then starts with its delayed form and the first sampled column is n0 (ptts_generate_begin_ids).
+        input_lens: None, or [B] int32: row b continues from its first input_lens[b] columns (ptts_generate_begin_ids2); None
+        when every row takes all n0.
         ext: None, or the ptts_sampling_ext values (resolve_sampling_ext) for this generation.
         lext: None, or the ptts_logits_ext processors (resolve_logits_ext); the session keeps it, and so its device tables, alive."""
         g = _lib.GenParamsC()
@@ -779,7 +853,14 @@ class GenSession:
             if ids.dim() != 2 or ids.shape[0] != self.B * self.K:
                 raise ValueError(f"input_ids must be [{self.B * self.K}, n0], got {tuple(ids.shape)}")
             self._input_ids, self.n0 = ids, int(ids.shape[1])   # kept alive until the asynchronous begin kernel has read it
-            _lib.check(_lib.lib().ptts_generate_begin_ids(self.h, C.byref(g), _lib.ptr(ids), self.n0, _lib.stream_ptr()))
+            if input_lens is None:
+                _lib.check(_lib.lib().ptts_generate_begin_ids(self.h, C.byref(g), _lib.ptr(ids), self.n0, _lib.stream_ptr()))
+            else:
+                lens = input_lens.to(device=self.eng.device, dtype=torch.int32).contiguous()
+                if tuple(lens.shape) != (self.B,):
+                    raise ValueError(f"input_lens must be [{self.B}], got {tuple(lens.shape)}")
+                _lib.check(_lib.lib().ptts_generate_begin_ids2(self.h, C.byref(g), _lib.ptr(ids), self.n0, _lib.ptr(lens),
+                                                               _lib.stream_ptr()))
         if ext is not None:
             _lib.check(_lib.lib().ptts_generate_set_sampling_ext(self.h, C.byref(_lib.SamplingExtC(**ext))))
         self._lext = lext
@@ -1296,8 +1377,8 @@ class ParlerTTSForConditionalGeneration:
     main_input_name = "input_ids"
     # model kwargs generate() understands (reference: _validate_model_kwargs over forward()'s signature)
     _MODEL_KWARGS = frozenset({"input_ids", "attention_mask", "prompt_input_ids", "prompt_attention_mask", "prompt_hidden_states",
-                               "encoder_outputs", "input_values", "decoder_input_ids", "padding_mask", "use_cache",
-                               "cache_implementation", "output_attentions", "output_hidden_states"})
+                               "encoder_outputs", "input_values", "decoder_input_ids", "decoder_attention_mask", "padding_mask",
+                               "use_cache", "cache_implementation", "output_attentions", "output_hidden_states"})
     # GenerationConfig fields the device loop does not implement, with the value that means "off"
     _NEUTRAL_GENERATION_KNOBS = {"num_beam_groups": 1, "repetition_penalty": 1.0, "length_penalty": 1.0,
                                  "penalty_alpha": None, "bad_words_ids": None, "force_words_ids": None, "guidance_scale": None}
@@ -1500,6 +1581,70 @@ class ParlerTTSForConditionalGeneration:
         text = (0, 0 if prompt_hidden is None else prompt_hidden.shape[1], prompt_mask)
         return enc_hidden, attention_mask, prompt_hidden, prompt_mask, text, eo
 
+    def _encode_clips(self, clips, B: int):
+        """generate(input_values=[w_0, ..]): each clip [1, samples_b] or [samples_b] through DACModel.encode (clips of one length
+        together) -> the codes right-padded to the longest, [B, K, N_max], and their frame mask [B, N_max]."""
+        K = self.config.decoder.num_codebooks
+        if len(clips) != B:
+            raise ValueError(f"input_values must hold batch_size = {B} clips, got {len(clips)}")
+        if self.config.audio_encoder.num_codebooks != K:
+            raise ValueError(f"the codec has {self.config.audio_encoder.num_codebooks} codebooks, the decoder {K}: "
+                             "its codes cannot continue this decoder")
+        wavs = []
+        for i, w in enumerate(clips):
+            w = torch.as_tensor(w)
+            if w.dim() == 2 and w.shape[0] == 1:
+                w = w[0]
+            if w.dim() != 1 or w.shape[0] < 1:
+                raise ValueError(f"input_values[{i}] must be [1, samples] or [samples], got {tuple(w.shape)}")
+            wavs.append(w)
+        codes = [None] * B
+        for n in sorted({w.shape[0] for w in wavs}):
+            idx = [i for i, w in enumerate(wavs) if w.shape[0] == n]
+            c = self.audio_encoder.encode(torch.stack([wavs[i] for i in idx])[:, None, :].to(self.device)).audio_codes
+            for j, i in enumerate(idx):
+                codes[i] = c.reshape(len(idx), K, -1)[j]
+        F = max(c.shape[-1] for c in codes)
+        ids = torch.zeros(B, K, F, dtype=torch.int64, device=self.device)
+        mask = torch.zeros(B, F, dtype=torch.int64)
+        for i, c in enumerate(codes):
+            ids[i, :, :c.shape[-1]] = c
+            mask[i, :c.shape[-1]] = 1
+        return ids, mask
+
+    def _codes_from_raw(self, output_ids, mask_src, max_length: int):
+        """The raw token matrix [B * K, T] of one decoder input mask_src [B * K, n0] -> (the de-delayed matrix, codes [B, K, F])."""
+        d = self.config.decoder
+        K = d.num_codebooks
+        _, full_mask = build_delay_pattern_mask(mask_src, d.bos_token_id, d.pad_token_id, max_length, K)
+        output_ids = apply_delay_pattern_mask(output_ids, full_mask)
+        _, mask = build_delay_pattern_mask(mask_src, d.bos_token_id, d.pad_token_id, output_ids.shape[1], K)
+        keep = (mask != d.bos_token_id) & (mask != d.pad_token_id)
+        return output_ids, output_ids[keep].reshape(output_ids.shape[0] // K, K, -1)
+
+    def _ragged_codes_from_raw(self, output_ids, dec_ids, input_lens, max_length: int):
+        """A ragged continuation's raw token matrix [B * K, T] -> (de-delayed matrix, codes [B, K, F_max]).  Row b holds its own
+        columns [0, T - s_b) with s_b = n0 - n0_b, and gets its own delay pattern (its input's first n0_b columns, max_length - s_b),
+        what the row alone would get; past its columns (and its frames in `codes`) the rows are filled with pad_token_id."""
+        d = self.config.decoder
+        K, T, n0 = d.num_codebooks, output_ids.shape[1], dec_ids.shape[1]
+        B = output_ids.shape[0] // K
+        shift = (n0 - input_lens).cpu()
+        out = torch.full_like(output_ids, d.pad_token_id)
+        rows_codes = [None] * B
+        for s in sorted(set(shift.tolist())):
+            idx = torch.nonzero(shift == s).flatten()
+            rows = (idx[:, None] * K + torch.arange(K)[None, :]).flatten().to(output_ids.device)
+            o, c = self._codes_from_raw(output_ids[rows, :T - s].contiguous(), dec_ids[rows, :n0 - s].contiguous(), max_length - s)
+            out[rows, :T - s] = o
+            for j, b in enumerate(idx.tolist()):
+                rows_codes[b] = c[j]
+        F = max(c.shape[-1] for c in rows_codes)
+        codes = torch.full((B, K, F), d.pad_token_id, dtype=torch.int64, device=output_ids.device)
+        for b, c in enumerate(rows_codes):
+            codes[b, :, :c.shape[-1]] = c
+        return out, codes
+
     # -- the token loop ------------------------------------------------------------------------------
     def _sampling(self, gc, n0: int, max_length: int, seed=0, suppress_special=False, row_base=0, logits_processor=None,
                   stopping_criteria=None) -> Sampling:
@@ -1587,10 +1732,12 @@ class ParlerTTSForConditionalGeneration:
         return 32
 
     def _run_token_loop(self, enc_hidden, enc_mask, prompt_hidden, prompt_mask, input_ids, sampling: Sampling, shard, recorders=(),
-                        streamer=None):
+                        streamer=None, input_lens=None):
         """begin + prefill + the token loop of one shard's session -> its raw token matrix [rows * K, generated length].
         The inputs are the whole call's: enc_hidden / enc_mask per description, prompt_hidden / prompt_mask per take, input_ids
-        None or the BOS-led decoder input [takes * K, n0].  shard: (first description, end, first take, end) (take_shards).
+        None or the BOS-led decoder input [takes * K, n0], input_lens None or each take's own column count [takes] (a ragged
+        continuation; the shard passes its slice, or None when all of it is n0).  shard: (first description, end, first take,
+        end) (take_shards).
         recorders (see recording): the device loop keeps each decode_steps call inside one chunk of those that have chunks."""
         d = self.config.decoder
         K, s = d.num_codebooks, sampling
@@ -1601,11 +1748,14 @@ class ParlerTTSForConditionalGeneration:
         B, S = r1 - r0, enc_hidden.shape[1]
         P = 0 if prompt_hidden is None else prompt_hidden.shape[1]
         n0 = 1 if input_ids is None else int(input_ids.shape[1])
+        input_lens = cut(input_lens, r0, r1)
+        if input_lens is not None and bool((input_lens == n0).all()):
+            input_lens = None
         sess = self.decoder.engine.session(B, P, S, P + s.max_length, max_input_len=n0, takes=B // (d1 - d0))
         host = bool(s.processors or s.criteria)
         sess.begin(s.max_length, do_sample=s.do_sample, temperature=s.temperature, top_k=s.top_k, top_p=s.top_p,
                    min_new_tokens=s.min_new_tokens, seed=s.seed, suppress_special=s.suppress_special, codebook_size=s.codebook_size,
-                   row_base=s.row_base + r0 * K, input_ids=input_ids,
+                   row_base=s.row_base + r0 * K, input_ids=input_ids, input_lens=input_lens,
                    ext=None if host else s.ext, lext=None if host else s.lext)    # the host-driven loop applies them as torch ops
         stream_col = lambda col, v: v
         if streamer is not None:
@@ -1865,8 +2015,17 @@ class ParlerTTSForConditionalGeneration:
 
         d = self.config.decoder
         K = d.num_codebooks
-        dec_ids = None
-        if mk.get("decoder_input_ids") is None and mk.get("input_values") is not None:
+        dec_ids = input_lens = None
+        # code prefixes of different lengths: a decoder_attention_mask, or the clips of a list of input_values (ragged mode)
+        ragged = mk.get("decoder_attention_mask") is not None or (mk.get("decoder_input_ids") is None and
+                                                                  isinstance(mk.get("input_values"), (list, tuple)))
+        if ragged:
+            check_ragged_generate(streamer, logits_processor, stopping_criteria, gc)
+            if mk.get("decoder_input_ids") is None and mk.get("input_values") is None:
+                raise ValueError("decoder_attention_mask needs decoder_input_ids (or input_values) to apply to")
+        if mk.get("decoder_input_ids") is None and isinstance(mk.get("input_values"), (list, tuple)):
+            mk["decoder_input_ids"], mk["decoder_attention_mask"] = self._encode_clips(mk["input_values"], B)
+        elif mk.get("decoder_input_ids") is None and mk.get("input_values") is not None:
             # audio prompt (:3442-3446, :3136-3194): encoded once, with every codebook; its codes continue like decoder_input_ids.
             # padding_mask does not reach the encoder, as in the reference.
             wav = mk["input_values"]
@@ -1878,7 +2037,11 @@ class ParlerTTSForConditionalGeneration:
             mk["decoder_input_ids"] = self.audio_encoder.encode(wav).audio_codes
         if mk.get("decoder_input_ids") is not None:   # -> the BOS-led [B * K, n0] on the device (:3012-3024)
             start = gc.decoder_start_token_id if gc.decoder_start_token_id is not None else d.bos_token_id
-            dec_ids = prepare_decoder_input_ids(mk["decoder_input_ids"], B, K, d.vocab_size, start, self.device)
+            if ragged:   # + each row's own column count n0_b
+                dec_ids, input_lens = prepare_ragged_decoder_input_ids(mk["decoder_input_ids"], mk["decoder_attention_mask"], B, K,
+                                                                       d.vocab_size, start, self.device)
+            else:
+                dec_ids = prepare_decoder_input_ids(mk["decoder_input_ids"], B, K, d.vocab_size, start, self.device)
         n0 = 1 if dec_ids is None else dec_ids.shape[1]
         # num_return_sequences: the output batch is B * N, take n of description b at row b * N + n.  The encoder ran (and the
         # cross-attention K/V are projected) once per description; what is per row -- a self-attention prompt prefix, the code
@@ -1889,6 +2052,8 @@ class ParlerTTSForConditionalGeneration:
                 prompt_mask = None if prompt_mask is None else prompt_mask.repeat_interleave(N, dim=0)
             if dec_ids is not None:
                 dec_ids = expand_takes(dec_ids, B, K, N)
+            if input_lens is not None:
+                input_lens = input_lens.repeat_interleave(N)
 
         # generated length (:3458-3469): max_new_tokens wins over max_length (both count the n0 input columns)
         if gc.max_new_tokens is not None:
@@ -1915,7 +2080,8 @@ class ParlerTTSForConditionalGeneration:
         # draw is keyed by the global row (row_base), the processors' state is per utterance, and a finished utterance emits pad
         # ids until the longest one ends.  The host-driven loop and a streamer run the batch as one session.
         limit = None if sampling.processors or sampling.criteria or streamer is not None else self._fused_batch_limit()
-        parts = [self._run_token_loop(enc_hidden, attention_mask, prompt_hidden, prompt_mask, dec_ids, sampling, shard, recorders, streamer)
+        parts = [self._run_token_loop(enc_hidden, attention_mask, prompt_hidden, prompt_mask, dec_ids, sampling, shard, recorders, streamer,
+                                      input_lens)
                  for shard in take_shards(B, N, limit)]
         output_ids = parts[0]
         if len(parts) > 1:
@@ -1925,12 +2091,11 @@ class ParlerTTSForConditionalGeneration:
 
         # apply the stashed delay mask, then keep only the free cells (:3586-3597); both masks come from the whole decoder input,
         # so a continuation's codes begin with its prefix frames
-        mask_src = output_ids[:, :1] if dec_ids is None else dec_ids
-        _, full_mask = build_delay_pattern_mask(mask_src, d.bos_token_id, d.pad_token_id, max_length, K)
-        output_ids = apply_delay_pattern_mask(output_ids, full_mask)
-        _, mask = build_delay_pattern_mask(mask_src, d.bos_token_id, d.pad_token_id, output_ids.shape[1], K)
-        keep = (mask != d.bos_token_id) & (mask != d.pad_token_id)
-        codes = output_ids[keep].reshape(B, K, -1)
+        if input_lens is None:
+            mask_src = output_ids[:, :1] if dec_ids is None else dec_ids
+            output_ids, codes = self._codes_from_raw(output_ids, mask_src, max_length)
+        else:
+            output_ids, codes = self._ragged_codes_from_raw(output_ids, dec_ids, input_lens, max_length)
         audio_codes = codes[None, ...]  # frame dim (:3600)
 
         # The reference decodes sample by sample when any bos/pad/eos id survived (:3615-3619).  Ids in
