@@ -333,11 +333,39 @@ int ptts_generate_set_alignment(ptts_session* s, const int32_t* heads, int32_t n
 int ptts_align_dtw(const float* alignment, int32_t B, int32_t T, int32_t P, const int32_t* n_frames, const int32_t* key_mask,
                    float* filtered, uint8_t* trace, int32_t* jumps, void* stream);
 
+/* ---- continuous batching ---------------------------------------------------------------------- */
+/* Copy n request rows out of src into slots of dst: row src_rows[i] of src becomes row dst_rows[i] of dst (host int32 arrays; the
+ * destination rows distinct).  src has run ptts_generate_begin (the BOS column), ptts_prefill and exactly one ptts_sample since, and
+ * no decode step (PTTS_EINVAL otherwise: its cache holds positions [0, P + 1) and its history columns [0, 2) only then);
+ * dst is prefilled, typically live in slot mode.  Both run the same model with the same config, P and S, takes = 1, the same
+ * max_input_len class (1, or >= 2) and the same masks given at their prefills.  Every per-row region the decode path reads is
+ * copied: the self K/V of positions [0, P + 1) of every layer and head, the cross K/V, the encoder and prompt masks, the history
+ * columns [0, 2), the next input, the EOS and stopping state, the ParlerTTSLogitsProcessor state (into the parity
+ * buffer dst's next step reads: keep dst's cur_len parity until then, see ptts_generate_set_slots) and the prefix cells.  One
+ * kernel on `stream`, no host sync.  PTTS_ESTATE before either prefill; PTTS_EINVAL for sessions that do not match or rows out
+ * of range. */
+int ptts_session_import_rows(ptts_session* dst, const ptts_session* src, const int32_t* src_rows, const int32_t* dst_rows, int32_t n,
+                             void* stream);
+
+/* Slot mode: every row b is a request of its own that started from the BOS column, at its own column col_b = cur_len - row_shift[b]
+ * (>= 1), with Philox key row_key[b] (its draws use substream row_key[b] * K + k, what row row_key[b] of a generate() call with
+ * row_base 0 uses).  Each decode step then stops a row at col_b + 1 >= max_length or its EOS, masks EOS while col_b - 1 <
+ * min_new_tokens and applies the delay pattern of max_length in the row's own column; the decode kernels put the row at position
+ * P + col_b - 1.  Sets ctrl cur_len, reactivates a session that went inactive and clears the sampler's counters; row_shift and
+ * row_key are host int32 [B] arrays, passed to the kernel by value (no host sync).  Call it again at every rebase.
+ * Needs a prefilled session created with max_input_len >= 2 (it holds the per-row offsets), takes = 1, a generation begun from
+ * the BOS column, no probe, alignment or per-step output window, and none of forced_eos_token_id, the decay penalty or
+ * begin_suppress_tokens (they count from one batch column); every token then takes the split path's EXT sampler.  The caller
+ * runs at most raw_ld - max(col_b) steps before the next call (ptts_session_raw_ids gives raw_ld), and keeps each row's
+ * cur_len parity where it was when it imported rows.  Slot mode lasts until the next ptts_generate_begin*. */
+int ptts_generate_set_slots(ptts_session* s, int32_t cur_len, const int32_t* row_shift, const int32_t* row_key, void* stream);
+
 /* Device pointers into the workspace (valid for the session lifetime). */
 int ptts_session_logits(ptts_session* s, float** out);          /* [B*K, V] f32, last step's raw logits */
 int ptts_session_scores(ptts_session* s, float** out);          /* [B*K, V] f32, processed scores      */
 int ptts_session_raw_ids(ptts_session* s, int64_t** out, int32_t* ld); /* [B*K, ld] raw (un-masked) history */
 int ptts_session_state(ptts_session* s, int32_t** out);         /* int32[8]: {cur_len, n_unfinished, ...} */
+int ptts_session_eos_seen(ptts_session* s, int32_t** out);      /* [B*K] int32: 1 + the column of each row's first EOS, 0 = none */
 int ptts_session_launches(ptts_session* s, int64_t* out);       /* kernels launched through this session  */
 /* After ptts_prefill: 0 = decode steps run the multi-kernel path (shape outside the fused kernel's range; a warning is printed
  * once), 1 = the fused persistent step kernel (one launch per token, step.cu), 2 = its cluster variant (step2.cu). */

@@ -90,10 +90,13 @@ _SIGS = {
     "ptts_decode_forward": (C.c_int, [_VP, _VP]),
     "ptts_sample": (C.c_int, [_VP, _VP, _VP]),
     "ptts_decode_steps": (C.c_int, [_VP, _I32, _VP]),
+    "ptts_session_import_rows": (C.c_int, [_VP, _VP, C.POINTER(_I32), C.POINTER(_I32), _I32, _VP]),
+    "ptts_generate_set_slots": (C.c_int, [_VP, _I32, C.POINTER(_I32), C.POINTER(_I32), _VP]),
     "ptts_session_logits": (C.c_int, [_VP, C.POINTER(_VP)]),
     "ptts_session_scores": (C.c_int, [_VP, C.POINTER(_VP)]),
     "ptts_session_raw_ids": (C.c_int, [_VP, C.POINTER(_VP), C.POINTER(_I32)]),
     "ptts_session_state": (C.c_int, [_VP, C.POINTER(_VP)]),
+    "ptts_session_eos_seen": (C.c_int, [_VP, C.POINTER(_VP)]),
     "ptts_session_launches": (C.c_int, [_VP, C.POINTER(_I64)]),
     "ptts_session_fused": (C.c_int, [_VP, C.POINTER(_I32)]),
     "ptts_session_set_profile": (C.c_int, [_VP, _VP]),

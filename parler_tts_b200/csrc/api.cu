@@ -67,6 +67,9 @@ struct ptts_session {
   ptts_gen_params gen;
   int n0;            // decoder input columns of the current generate() call (1: the BOS column; > 1: continuing from codes)
   bool ragged;       // the call's rows continue from inputs of different lengths (ptts_generate_begin_ids2): W.row_shift is live
+  int sampled;       // ptts_sample / ptts_op_sample_phase calls since the last ptts_prefill
+  bool decoded;      // a decode step ran since the last ptts_prefill (the cache holds positions past P + n0)
+  bool slots;        // slot mode (ptts_generate_set_slots): ragged, and every row is a request with its own column and Philox key
   cudaStream_t cap_stream;
   cudaGraphExec_t exec;
   bool graph_ready;
@@ -113,12 +116,14 @@ static DecodePath decode_path(const ptts_session* s) {
   return (active_probe(s) != nullptr || active_align(s) != nullptr) ? DECODE_MULTI_KERNEL : s->path;
 }
 
-// the knobs of the EXT sampler, or nullptr for the plain one: the outputs and the ptts_logits_ext stages run on the EXT sampler,
-// with every ptts_sampling_ext stage off when none is active (it then computes what the plain sampler computes)
+// the knobs of the EXT sampler, or nullptr for the plain one: the outputs, the ptts_logits_ext stages and slot mode run on the EXT
+// sampler, with every ptts_sampling_ext stage off when none is active (it then computes what the plain sampler computes)
 static const ptts_sampling_ext* sampler_ext(const ptts_session* s) {
   const ptts_sampling_ext* x = active_ext(s);
-  return (x == nullptr && (active_out(s) != nullptr || active_lext(s) != nullptr)) ? &kExtOff : x;
+  return (x == nullptr && (active_out(s) != nullptr || active_lext(s) != nullptr || s->slots)) ? &kExtOff : x;
 }
+// slot mode's per-row Philox keys, or nullptr
+static const int* slot_keys(const ptts_session* s) { return s->slots ? (const int*)(s->ws + s->W.row_key) : nullptr; }
 
 extern "C" {
 
@@ -235,7 +240,7 @@ int ptts_session_create3(const ptts_decoder_config* cfg, const void* blob, void*
   s->L = make_layout(*cfg);
   s->W = make_workspace(*cfg, B, P, S, max_cache_len, max_input_len, takes);
   s->n0 = 1;
-  s->ragged = false;
+  s->ragged = s->slots = false;
   s->ext = kExtOff;
   s->lext = kLogitsExtOff;
   s->out = SampleOut{};
@@ -378,6 +383,7 @@ int ptts_generate_begin_ids2(ptts_session* s, const ptts_gen_params* gen, const 
   }
   // n0 == 1: every length is 1 and every offset 0 -- a uniform batch (and a session without max_input_len > 1 has no row_shift)
   s->ragged = input_lens != nullptr && n0 > 1;
+  s->slots = false;
   s->gen = *gen;
   s->gen.input_len = n0;
   s->n0 = n0;
@@ -705,6 +711,8 @@ int ptts_prefill(ptts_session* s, const void* prompt_hidden, const int64_t* prom
   if (s->has_enc_mask) { if (int e = launch_mask_convert(enc_mask, s->W.B / s->W.takes * s->W.S, (int*)(s->ws + s->W.enc_mask), st)) return e; }
   if (int e = run_forward(s, st, true, prompt_hidden, enc_hidden)) return e;
   s->prefilled = true;
+  s->sampled = 0;
+  s->decoded = false;
   s->path = choose_decode_path(s);
   // mask presence is baked into the captured graph: re-capture if it changed
   drop_graph(s);
@@ -750,7 +758,7 @@ int ptts_score(ptts_session* s, const void* prompt_hidden, const int64_t* prompt
   if (s->has_prompt_mask) { if (int e = launch_mask_convert(prompt_mask, W.B * W.P, (int*)(s->ws + W.prompt_mask), st)) return e; }
   if (s->has_enc_mask) { if (int e = launch_mask_convert(enc_mask, W.B / W.takes * W.S, (int*)(s->ws + W.enc_mask), st)) return e; }
   s->n0 = T;
-  s->ragged = false;
+  s->ragged = s->slots = false;
   s->begun = s->prefilled = false;  // the caches now hold this call's positions: a generation has to begin again
   if (int e = run_forward(s, st, true, prompt_hidden, enc_hidden, false)) return e;
 
@@ -789,6 +797,7 @@ int ptts_decode_forward(ptts_session* s, void* stream) {
   PTTS_REQUIRE(s, "null argument");
   if (!s->prefilled) return fail(PTTS_ESTATE, "ptts_decode_forward called before ptts_prefill");
   cudaStream_t st = (cudaStream_t)stream;
+  s->decoded = true;
   StepParams p = s->sp;
   p.do_sample_phase = 0;
   switch (decode_path(s)) {
@@ -803,13 +812,16 @@ int ptts_sample(ptts_session* s, const int64_t* forced_tokens, void* stream) {
   PTTS_REQUIRE(s, "null argument");
   if (!s->prefilled) return fail(PTTS_ESTATE, "ptts_sample called before ptts_prefill");
   s->launches++;
-  return launch_sample(sample_args(s), forced_tokens, (cudaStream_t)stream, false, sampler_ext(s), active_out(s), active_lext(s));
+  s->sampled++;
+  return launch_sample(sample_args(s), forced_tokens, (cudaStream_t)stream, false, sampler_ext(s), active_out(s), active_lext(s),
+                       slot_keys(s));
 }
 
 int ptts_decode_steps(ptts_session* s, int32_t n_steps, void* stream) {
   PTTS_REQUIRE(s && n_steps >= 0, "bad argument");
   if (!s->prefilled) return fail(PTTS_ESTATE, "ptts_decode_steps called before ptts_prefill");
   cudaStream_t st = (cudaStream_t)stream;
+  if (n_steps > 0) s->decoded = true;
   const ptts_sampling_ext* ext = sampler_ext(s);
   const SampleOut* out = active_out(s);
   const ptts_logits_ext* lext = active_lext(s);
@@ -822,7 +834,7 @@ int ptts_decode_steps(ptts_session* s, int32_t n_steps, void* stream) {
     for (int i = 0; i < n_steps; i++) {
       const int e = path == DECODE_CLUSTER ? launch_decode_step_cluster(p, st) : launch_decode_step(p, s->sm_count, st);
       if (e) return e;
-      if (int e2 = launch_sample(sample_args(s), nullptr, st, false, ext, out, lext)) return e2;
+      if (int e2 = launch_sample(sample_args(s), nullptr, st, false, ext, out, lext, slot_keys(s))) return e2;
     }
     s->launches += 2 * (int64_t)n_steps;
     return PTTS_OK;
@@ -854,7 +866,7 @@ int ptts_decode_steps(ptts_session* s, int32_t n_steps, void* stream) {
     const int64_t before = s->launches;
     PTTS_CHECK_CUDA(cudaStreamBeginCapture(s->cap_stream, cudaStreamCaptureModeThreadLocal));
     int e = run_forward(s, s->cap_stream, false, nullptr, nullptr);
-    if (!e) { s->launches++; e = launch_sample(sample_args(s), nullptr, s->cap_stream, true, ext, out, lext); }
+    if (!e) { s->launches++; e = launch_sample(sample_args(s), nullptr, s->cap_stream, true, ext, out, lext, slot_keys(s)); }
     cudaGraph_t graph = nullptr;
     cudaError_t ce = cudaStreamEndCapture(s->cap_stream, &graph);
     s->graph_launches = s->launches - before;   // embed + 8 kernels per layer + heads + sample (+ the probe kernels)
@@ -871,6 +883,76 @@ int ptts_decode_steps(ptts_session* s, int32_t n_steps, void* stream) {
   return PTTS_OK;
 }
 
+// ---- continuous batching ------------------------------------------------------------------------
+int ptts_session_import_rows(ptts_session* dst, const ptts_session* src, const int32_t* src_rows, const int32_t* dst_rows, int32_t n,
+                             void* stream) {
+  PTTS_REQUIRE(dst && src && (n == 0 || (src_rows && dst_rows)) && n >= 0, "bad argument");
+  if (!src->prefilled || !dst->prefilled) return fail(PTTS_ESTATE, "import_rows: both sessions must have run ptts_prefill");
+  PTTS_REQUIRE(dst != src, "import_rows: the source and the destination are one session");
+  PTTS_REQUIRE(memcmp(&src->cfg, &dst->cfg, sizeof(src->cfg)) == 0 && src->blob == dst->blob, "import_rows: the sessions run different models");
+  PTTS_REQUIRE(src->W.P == dst->W.P && src->W.S == dst->W.S, "import_rows: P and S must match (source %d, %d; destination %d, %d)",
+               src->W.P, src->W.S, dst->W.P, dst->W.S);
+  PTTS_REQUIRE(src->W.takes == 1 && dst->W.takes == 1, "import_rows: sessions with takes > 1 share cross K/V between rows");
+  PTTS_REQUIRE(src->has_prompt_mask == dst->has_prompt_mask && src->has_enc_mask == dst->has_enc_mask,
+               "import_rows: both sessions must have been prefilled with the same masks given (or both without)");
+  PTTS_REQUIRE(!src->ragged && src->n0 == 1, "import_rows: the source rows must start from the BOS column (a uniform generation)");
+  // the cache holds positions [0, P + 1) and the history columns [0, 2) only then
+  PTTS_REQUIRE(src->sampled == 1 && !src->decoded, "import_rows: the source must have run ptts_prefill and exactly one ptts_sample "
+               "since (%d samples%s)", src->sampled, src->decoded ? " and decode steps" : "");
+  const int kv_len = src->W.P + src->n0;
+  PTTS_REQUIRE(kv_len <= dst->W.Tmax, "import_rows: %d cache positions do not fit the destination's %d", kv_len, dst->W.Tmax);
+  RowImportArgs a{};
+  RowRegion tmp[kMaxRowRegions];
+  a.n_regions = row_regions(src->cfg, src->W, kv_len, a.src);
+  PTTS_REQUIRE(row_regions(dst->cfg, dst->W, kv_len, tmp) == a.n_regions, "import_rows: the sessions hold different per-row state "
+               "(create both with the same max_input_len class: 1, or >= 2)");
+  for (int r = 0; r < a.n_regions; r++) a.dst[r] = tmp[r];
+  a.src_ws = src->ws; a.dst_ws = dst->ws; a.K = src->cfg.num_codebooks;
+  a.src_ctrl = (const Ctrl*)(src->ws + src->W.ctrl); a.dst_ctrl = (const Ctrl*)(dst->ws + dst->W.ctrl);
+  std::vector<char> taken(dst->W.B, 0);
+  for (int i = 0; i < n; i++) {
+    PTTS_REQUIRE(src_rows[i] >= 0 && src_rows[i] < src->W.B, "import_rows: source row %d outside [0, %d)", src_rows[i], src->W.B);
+    PTTS_REQUIRE(dst_rows[i] >= 0 && dst_rows[i] < dst->W.B, "import_rows: destination row %d outside [0, %d)", dst_rows[i], dst->W.B);
+    PTTS_REQUIRE(!taken[dst_rows[i]], "import_rows: destination row %d is listed twice", dst_rows[i]);
+    taken[dst_rows[i]] = 1;
+  }
+  for (int i0 = 0; i0 < n; i0 += kMaxImportRows) {
+    const int m = n - i0 < kMaxImportRows ? n - i0 : kMaxImportRows;
+    for (int i = 0; i < m; i++) { a.src_row[i] = src_rows[i0 + i]; a.dst_row[i] = dst_rows[i0 + i]; }
+    if (int e = launch_import_rows(a, m, (cudaStream_t)stream)) return e;
+    dst->launches++;
+  }
+  return PTTS_OK;
+}
+
+int ptts_generate_set_slots(ptts_session* s, int32_t cur_len, const int32_t* row_shift, const int32_t* row_key, void* stream) {
+  PTTS_REQUIRE(s && row_shift && row_key, "null argument");
+  if (!s->prefilled) return fail(PTTS_ESTATE, "set_slots called before ptts_prefill");
+  const WorkspaceLayout& W = s->W;
+  PTTS_REQUIRE(W.row_shift >= 0, "set_slots: the session has no per-row offsets (create it with max_input_len >= 2)");
+  PTTS_REQUIRE(W.takes == 1, "set_slots: a session with takes > 1 shares cross K/V between rows");
+  PTTS_REQUIRE(s->n0 == 1 && (!s->ragged || s->slots), "set_slots: slot mode takes requests that start from the BOS column");
+  PTTS_REQUIRE(active_probe(s) == nullptr && active_align(s) == nullptr && active_out(s) == nullptr,
+               "set_slots: the probe and per-step output windows count one batch step, not a slot's column");
+  const ptts_logits_ext& lx = s->lext;
+  PTTS_REQUIRE(lx.forced_eos_token_id < 0 && lx.decay == nullptr && lx.begin_suppress == nullptr,
+               "set_slots: forced_eos_token_id, the decay penalty and begin_suppress_tokens count from one batch column");
+  PTTS_REQUIRE(cur_len >= 1 && cur_len < W.raw_ld, "set_slots: cur_len %d outside [1, %lld)", cur_len, (long long)W.raw_ld);
+  for (int b = 0; b < W.B; b++) {
+    PTTS_REQUIRE(row_shift[b] >= 0 && row_shift[b] < cur_len, "set_slots: row_shift[%d] = %d outside [0, cur_len = %d)", b, row_shift[b], cur_len);
+    PTTS_REQUIRE(row_key[b] >= 0, "set_slots: row_key[%d] = %d is negative", b, row_key[b]);
+  }
+  if (int e = launch_set_slots((Ctrl*)(s->ws + W.ctrl), cur_len, (int*)(s->ws + W.row_shift), (int*)(s->ws + W.row_key), row_shift, row_key,
+                               W.B, (cudaStream_t)stream)) return e;
+  s->launches += (W.B + kMaxSlotRows - 1) / kMaxSlotRows;
+  if (!s->slots) {   // the decode kernels switch to their ragged instantiations (set up anew) and the sampler to slot mode
+    s->ragged = s->slots = true;
+    s->path = choose_decode_path(s);
+    drop_graph(s);
+  }
+  return PTTS_OK;
+}
+
 int ptts_align_dtw(const float* alignment, int32_t B, int32_t T, int32_t P, const int32_t* n_frames, const int32_t* key_mask,
                    float* filtered, uint8_t* trace, int32_t* jumps, void* stream) {
   PTTS_REQUIRE(alignment && n_frames && filtered && trace && jumps, "null argument");
@@ -883,6 +965,11 @@ int ptts_session_raw_ids(ptts_session* s, int64_t** out, int32_t* ld) {
   PTTS_REQUIRE(s && out && ld, "null");
   *out = (int64_t*)(s->ws + s->W.raw_ids);
   *ld = (int32_t)s->W.raw_ld;
+  return PTTS_OK;
+}
+int ptts_session_eos_seen(ptts_session* s, int32_t** out) {
+  PTTS_REQUIRE(s && out, "null");
+  *out = (int32_t*)(s->ws + s->W.eos_seen);
   return PTTS_OK;
 }
 int ptts_session_state(ptts_session* s, int32_t** out) { PTTS_REQUIRE(s && out, "null"); *out = (int32_t*)(s->ws + s->W.ctrl); return PTTS_OK; }
@@ -922,6 +1009,7 @@ int ptts_op_sample_phase(ptts_session* s, int32_t n_ctas, void* stream) {
   PTTS_REQUIRE(sampler_ext(s) == nullptr, "op_sample_phase: the step kernels' sampling phase has no ptts_sampling_ext or "
                                           "ptts_logits_ext stages and records no per-step outputs; switch them off first");
   s->launches++;
+  s->sampled++;
   return launch_sample_phase(sample_args(s), n_ctas, (cudaStream_t)stream);
 }
 

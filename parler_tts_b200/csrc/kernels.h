@@ -1,6 +1,7 @@
 // kernels.h -- host-side launch interface of the kernel translation units.
 #pragma once
 #include "common.cuh"
+#include "layout.h"
 
 namespace ptts {
 
@@ -143,8 +144,9 @@ struct SampleOut {
 // ext != nullptr: the sampler with the ptts_sampling_ext stages (the caller passes it while one is active, or all off while out is
 // set); out != nullptr (needs ext): that sampler also records the raw logits and the processed scores of the steps in its window
 // lext: the ptts_logits_ext stages (needs ext; nullptr = all off)
+// slot_key (needs ext and a.shift): slot mode (ptts_generate_set_slots), with the per-row Philox keys [B] on the device
 int launch_sample(const SampleArgs& a, const int64_t* forced, cudaStream_t st, bool pdl, const ptts_sampling_ext* ext = nullptr,
-                  const SampleOut* out = nullptr, const ptts_logits_ext* lext = nullptr);
+                  const SampleOut* out = nullptr, const ptts_logits_ext* lext = nullptr, const int* slot_key = nullptr);
 // every ptts_logits_ext stage off
 constexpr ptts_logits_ext kLogitsExtOff = {nullptr, nullptr, nullptr, 0, -1, -1, 0, nullptr, 0, nullptr, nullptr, 1, 0};
 // the fused step kernels' sampling phase over n_ctas CTAs (passes of up to three rows per CTA), as a kernel of its own; no EXT
@@ -160,6 +162,23 @@ int launch_cross_kv_relayout(const void* src, void* dst, int B, int S, int nckv,
 // dst row r = src row row0 + r * row_step - row_shift(shift, r)
 int launch_gather_rows(const void* src, int64_t ld_src, int64_t row0, int64_t row_step, const int* shift, void* dst, int rows, int cols,
                        int dtype, cudaStream_t st);
+
+// ---- continuous batching (rows.cu) --------------------------------------------------------------
+// ptts_session_import_rows: row src_row[p] of the source workspace -> slot dst_row[p] of the destination, over the row_regions
+// lists of both sessions (same config, P and S: the lists match entry for entry)
+constexpr int kMaxImportRows = 32;   // row pairs per launch
+struct RowImportArgs {
+  const char* src_ws; char* dst_ws;
+  const Ctrl* src_ctrl; const Ctrl* dst_ctrl;   // the history's length, and each side's first_unf parity
+  RowRegion src[kMaxRowRegions], dst[kMaxRowRegions];
+  int n_regions, K;   // K: codebooks (first_unf holds row indices b * K + k)
+  int src_row[kMaxImportRows], dst_row[kMaxImportRows];
+};
+int launch_import_rows(const RowImportArgs& a, int n_pairs, cudaStream_t st);
+// slot mode (ptts_generate_set_slots): the host arrays row_shift / row_key [B] into the workspace's shift / key, then the new cur_len,
+// active = 1 and the sampler's counters cleared
+constexpr int kMaxSlotRows = 256;    // rows per launch
+int launch_set_slots(Ctrl* ctrl, int cur_len, int* shift, int* key, const int* row_shift, const int* row_key, int B, cudaStream_t st);
 
 // ---- teacher-forced scoring (score.cu) ----------------------------------------------------------
 struct ScoreArgs {

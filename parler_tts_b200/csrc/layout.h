@@ -184,6 +184,7 @@ struct WorkspaceLayout {
   int64_t ctrl, progress, gen, raw_ids, cur_ids, eos_seen, unfinished, first_unf, prompt_mask, enc_mask;
   int64_t prefix_cells;            // [BK][K-1] int64: delay-pattern cells just past the input (max_input > 1 only; -1 = none)
   int64_t row_shift;               // [B] int32: per-row offsets of a ragged continuation (max_input > 1 only; -1 = none)
+  int64_t row_key;                 // [B] int32: slot mode's per-row Philox keys (ptts_generate_set_slots; with row_shift)
   int64_t x, qkv, attn, qc, hbuf, hidden, logits, scores, cross_tmp, cross_kv, self_kv;
   int64_t img_x, img_attn, img_h;  // fused step kernel: activations as tile images [chunk][32][H + 8] (step.cu stage_tile)
   int64_t cl_x, cl_attn, cl_h;     // cluster step kernel: K-sliced images [2][32][H/2 + 8], fc2's in quarters [4][32][F/4 + 8] (step2.cu)
@@ -219,6 +220,7 @@ static inline WorkspaceLayout make_workspace(const ptts_decoder_config& c, int B
   w.prefix_cells = -1;
   if (max_input > 1 && c.num_codebooks > 1) w.prefix_cells = take((int64_t)w.BK * (c.num_codebooks - 1) * 8);
   w.row_shift = max_input > 1 ? take((int64_t)B * 4) : -1;
+  w.row_key = max_input > 1 ? take((int64_t)B * 4) : -1;
   const int64_t rows_enc = (int64_t)B * S, rows_cross = (int64_t)(B / takes) * S;
   w.x = take((int64_t)w.Mmax * l.H * l.es);
   w.qkv = take((int64_t)w.Mmax * l.qkv_rows * l.es);
@@ -242,6 +244,46 @@ static inline WorkspaceLayout make_workspace(const ptts_decoder_config& c, int B
   w.self_kv = take(w.self_layer_stride * l.L);
   w.total = o;
   return w;
+}
+
+// ---- per-row state ------------------------------------------------------------------------------
+// Every workspace region a decode step or the sampler reads for batch row b, so that ptts_session_import_rows moves a row from
+// one session into a slot of another by copying exactly these (a region added to make_workspace that holds per-row state
+// belongs here too).  A region is n[0] x n[1] x n[2] blocks of `bytes` bytes; block (i, j, l) of row b starts at
+// off + i * stride[0] + j * stride[1] + l * stride[2] + b * row_stride.
+enum RowRegionKind {
+  ROW_PLAIN = 0,
+  ROW_HISTORY = 1,   // raw_ids: only the columns [0, cur_len) of the source are copied (bytes is the row's capacity)
+  ROW_FIRST_UNF = 2, // first_unf: one int32 per row, double-buffered on cur_len & 1 (each side adds (its cur_len & 1) * parity
+                     // to the offset), holding a row index b * K + k: moved from row b to row b' it gains (b' - b) * K
+};
+struct RowRegion {
+  int64_t off, row_stride, stride[3], parity, bytes;
+  int n[3];
+  int kind;
+};
+constexpr int kMaxRowRegions = 12;
+// kv_len: the self-attention positions [0, kv_len) that hold the row's keys and values (P + n0 after a prefill)
+static inline int row_regions(const ptts_decoder_config& c, const WorkspaceLayout& w, int kv_len, RowRegion* r) {
+  const DecoderLayout l = make_layout(c);
+  const int64_t D = PTTS_HEAD_DIM, es = l.es, K = c.num_codebooks;
+  const int64_t head = (int64_t)w.Tmax * D * es, desc = (int64_t)l.nckv * w.S * D * es;
+  int n = 0;
+  auto add = [&](int64_t off, int64_t row_stride, int64_t bytes, int n0 = 1, int64_t s0 = 0, int n1 = 1, int64_t s1 = 0, int n2 = 1,
+                 int64_t s2 = 0, int kind = ROW_PLAIN, int64_t parity = 0) {
+    r[n++] = RowRegion{off, row_stride, {s0, s1, s2}, parity, bytes, {n0, n1, n2}, kind};
+  };
+  add(w.self_kv, l.nkv * head, kv_len * D * es, l.L, w.self_layer_stride, 2, (int64_t)w.B * l.nkv * head, l.nkv, head);   // [L][K|V][B][nkv][Tmax][64]
+  add(w.cross_kv, desc, desc, l.L, w.cross_layer_stride, 2, (int64_t)(w.B / w.takes) * desc);                          // [L][K|V][B][nckv][S][64]
+  add(w.enc_mask, (int64_t)w.S * 4, (int64_t)w.S * 4);
+  if (w.P > 0) add(w.prompt_mask, (int64_t)w.P * 4, (int64_t)w.P * 4);
+  add(w.raw_ids, K * w.raw_ld * 8, w.raw_ld * 8, (int)K, w.raw_ld * 8, 1, 0, 1, 0, ROW_HISTORY);
+  add(w.cur_ids, K * 4, K * 4);
+  add(w.eos_seen, K * 4, K * 4);
+  add(w.unfinished, K * 4, K * 4);
+  add(w.first_unf, 4, 4, 1, 0, 1, 0, 1, 0, ROW_FIRST_UNF, (int64_t)w.B * 4);
+  if (w.prefix_cells >= 0) add(w.prefix_cells, K * (K - 1) * 8, K * (K - 1) * 8);
+  return n;
 }
 
 }  // namespace ptts

@@ -75,10 +75,14 @@ __device__ __forceinline__ bool bitmap_has(const uint32_t* __restrict__ bits, in
 // commute with the masks).  Additions and the decay product use __fadd_rn / __fmul_rn so that no FMA changes their rounding.
 // RAGGED = true reads each row's column from p.shift (a ragged continuation); RAGGED = false is the code of a uniform batch, in
 // which every row samples column cur_len (the callers pick the instantiation by p.shift != nullptr).
-template <int ITEMS, int R, bool EXT = false, bool RAGGED = false>
+// SLOT = true (with RAGGED and EXT; ptts_generate_set_slots) is slot mode: every row is a request of its own that started from
+// the BOS column at its own column 0, so its stop, MinNewTokens and delay pattern count in its column col = cur_len - shift[b]
+// and its draws use the Philox substream key[b] * K + k.
+template <int ITEMS, int R, bool EXT = false, bool RAGGED = false, bool SLOT = false>
 __device__ __forceinline__ void sample_rows_cta(const SampleArgs& p, const ptts_gen_params& g, const int64_t* __restrict__ forced,
                                                 int row0, int stride, int n_rows, int cur_len, ptts_sampling_ext x = {},
-                                                SampleOut o = {}, ptts_logits_ext lx = {}) {
+                                                SampleOut o = {}, ptts_logits_ext lx = {}, const int* __restrict__ key = nullptr) {
+  static_assert(!SLOT || (RAGGED && EXT), "slot mode runs on the ragged EXT sampler");
   static_assert(R >= 1 && R <= SMP_MAX_ROWS, "rows per pass");
   SmpScratch& sc = smp_scratch();   // one static buffer for every instantiation inlined into a kernel
   float (&s_f)[2][SMP_MAX_ROWS][SMP_WARPS] = sc.f;
@@ -238,8 +242,9 @@ __device__ __forceinline__ void sample_rows_cta(const SampleArgs& p, const ptts_
   for (int r = 0; r < R; r++) {
     const int b = row[r] / p.K, k = row[r] - b * p.K;
     bool mask_eos = false;
-    // MinNewTokensLength: prompt_length_to_skip = the decoder input's columns (the BOS column, or n0 when continuing)
-    if (cur_len - (g.input_len > 1 ? g.input_len : 1) < g.min_new_tokens) mask_eos = true;
+    // MinNewTokensLength: prompt_length_to_skip = the decoder input's columns (the BOS column, or n0 when continuing); a slot's
+    // request has the BOS column only
+    if ((SLOT ? col[r] - 1 : cur_len - (g.input_len > 1 ? g.input_len : 1)) < g.min_new_tokens) mask_eos = true;
     const bool mask_min = mask_eos;   // (EXT's ordered pass applies the two EOS masks at their own places)
     bool mask_par = false;
     // ParlerTTSLogitsProcessor (stateful; state double-buffered on the column parity)
@@ -462,7 +467,8 @@ __device__ __forceinline__ void sample_rows_cta(const SampleArgs& p, const ptts_
     int found[R], last_nz[R];
 #pragma unroll
     for (int r = 0; r < R; r++) {
-      target[r] = philox_uniform(g.seed, (uint32_t)(row[r] + g.row_base), (uint32_t)col[r]) * s[r];
+      const uint32_t stream = !SLOT ? (uint32_t)(row[r] + g.row_base) : valid[r] ? (uint32_t)(key[row[r] / p.K] * p.K + row[r] % p.K) : 0u;
+      target[r] = philox_uniform(g.seed, stream, (uint32_t)col[r]) * s[r];
       carry[r] = 0.f; found[r] = -1; last_nz[r] = -1;
     }
 #pragma unroll
@@ -609,15 +615,15 @@ __device__ __forceinline__ void sample_rows_cta(const SampleArgs& p, const ptts_
     if (!t_unf) t = p.pad;  // next_tokens * unfinished + pad * (1 - unfinished)
     p.raw_ids[(size_t)my_row * p.raw_ld + my_col] = t;
     if (t == p.eos && t_es == 0) p.eos_seen[my_row] = my_col + 1;
-    // the row's own limit max_length - shift is reached at the batch's max_length
-    const int new_len = cur_len + 1;
+    // the row's own limit max_length - shift is reached at the batch's max_length; a slot's limit is max_length in its column
+    const int new_len = (SLOT ? my_col : cur_len) + 1;
     const int done = (t == p.eos) || (new_len >= g.max_length);
     const int still_unfinished = t_unf && !done;
     p.unfinished[my_row] = still_unfinished;
     // delay-pattern override of the NEXT model input (column `my_col`), build_delay_pattern_mask :252-261, with the row's own
     // limit Lb and input length nb
     const int sh = cur_len - my_col;
-    const int Lb = g.max_length - sh, nb = g.input_len - sh;
+    const int Lb = SLOT ? g.max_length : g.max_length - sh, nb = SLOT ? 1 : g.input_len - sh;
     int nxt = t;
     if (Lb >= 2 * p.K - 1) {
       const bool is_bos = my_col <= k;

@@ -211,15 +211,105 @@ def codes_to_waveform(audio_encoder: DACModel, codes: torch.Tensor, codebook_siz
 
     Returns (audio [B, hop * max n_b] zero-padded after each row, lengths: hop * n_b, or 1 for a row without a valid frame).
     A batch with no valid frame at all gives [B, 1] zeros in `dtype`, like the reference's pad_sequence of 1-sample rows."""
-    B = codes.shape[0]
     packed, n = compact_valid_frames(codes, codebook_size)
-    n_host = n.tolist()
+    return packed_to_waveform(audio_encoder, packed, n.tolist(), dtype)
+
+
+def packed_to_waveform(audio_encoder: DACModel, packed: torch.Tensor, n_host: list[int], dtype: torch.dtype):
+    """codes_to_waveform after the compaction: packed [B, K, T] with row b's n_host[b] valid frames first."""
+    B = packed.shape[0]
     T = max(n_host, default=0)
     if T == 0:
-        return torch.zeros(B, 1, device=codes.device, dtype=dtype), [1] * B
+        return torch.zeros(B, 1, device=packed.device, dtype=dtype), [1] * B
     audio = audio_encoder.decode(audio_codes=packed[None, :, :, :T], audio_scales=[None] * B, frame_lengths=n_host).audio_values
     hop = audio_encoder.hop_length
     return audio.squeeze(1), [hop * v if v > 0 else 1 for v in n_host]
+
+
+# ---- continuous batching (generate_continuous) --------------------------------------------------------------------------------
+def check_continuous_generate(gc, mk: dict, streamer=None, logits_processor=None, stopping_criteria=None):
+    """What generate_continuous() refuses: whatever counts from one batch column for all rows (forced_eos_token_id,
+    exponential_decay_length_penalty, begin_suppress_tokens), the per-step outputs and probes (output_scores, output_logits,
+    output_attentions, output_hidden_states, return_token_timestamps), a streamer, the caller's processors and criteria (the
+    host-driven loop), continuations (decoder_input_ids, decoder_attention_mask, input_values) and num_return_sequences > 1."""
+    bad = []
+    if streamer is not None:
+        bad.append("streamer")
+    if logits_processor:
+        bad.append("logits_processor")
+    if stopping_criteria:
+        bad.append("stopping_criteria")
+    for k in ("decoder_input_ids", "decoder_attention_mask", "input_values"):
+        if mk.get(k) is not None:
+            bad.append(k)
+    for k in ("output_scores", "output_logits", "output_attentions", "output_hidden_states", "return_token_timestamps"):
+        if getattr(gc, k, False):
+            bad.append(k)
+    for k in ("forced_eos_token_id", "exponential_decay_length_penalty", "begin_suppress_tokens"):
+        if getattr(gc, k, None) is not None:
+            bad.append(k)
+    if gc.num_return_sequences != 1:
+        bad.append("num_return_sequences > 1")
+    if bad:
+        raise ValueError(f"generate_continuous() does not support {', '.join(bad)}")
+
+
+def slot_outputs(raw: torch.Tensor, eos_last: torch.Tensor, cur_len, shift: torch.Tensor, max_length: int, codebook_size: int):
+    """Every slot's state at a refill boundary, on the device (nothing here waits for it).  raw [B, K, ld] the history, eos_last [B]
+    = 1 + the column of the last codebook's first EOS (0: none; a row stopped by max_length records the PAD it writes after, when
+    pad == eos: hence the clamp), cur_len and shift [B] the slot columns.  Returns (finished [B], frames F [B], codes [B, K,
+    max_length] with the F de-delayed frames first, the same with the valid frames compacted to the front as codes_to_waveform
+    does, and their count [B]).  A request that ended with n history columns gets generate()'s cut (_codes_from_raw over its own columns): frame f
+    of codebook k is column f + k + 1, F = n - K, once n reaches the delay pattern's 2K - 1 columns; below that every column, F = n."""
+    B, K, ld = raw.shape
+    L = int(max_length)
+    finished = (eos_last > 0) | (cur_len - shift >= L)
+    n = torch.where(eos_last > 0, eos_last.clamp(max=L), torch.full_like(eos_last, L))
+    pattern = n >= 2 * K - 1
+    frames = torch.where(pattern, n - K, n)
+    f = torch.arange(L, device=raw.device)
+    off = pattern[:, None].long() * torch.arange(1, K + 1, device=raw.device)[None, :]
+    codes = torch.gather(raw, 2, (f[None, None, :] + off[:, :, None]).clamp(max=ld - 1))
+    valid = (codes < codebook_size).all(dim=1) & (f[None, :] < frames[:, None])
+    order = torch.sort((~valid).to(torch.uint8), dim=1, stable=True).indices
+    packed = torch.gather(codes, 2, order[:, None, :].expand_as(codes))
+    return finished, frames, codes, packed, valid.sum(dim=1)
+
+
+def refill_rows(t: Optional[torch.Tensor], first: int, count: int, rows: int) -> Optional[torch.Tensor]:
+    """Rows [first, first + count) of a per-request input, padded to `rows` rows by repeating the last one: a refill prefills a
+    session of batch_size rows, so its GEMMs take the kernels a batch_size-row generate() shard takes (the padding rows are never
+    imported)."""
+    if t is None:
+        return None
+    last = t[first + count - 1:first + count]
+    return torch.cat([t[first:first + count], last.expand(rows - count, *t.shape[1:])])
+
+
+def rebase_slots(cur_len: int, cols: list) -> tuple[int, list[int]]:
+    """A refill boundary's new batch column and row offsets.  cols[b]: the column slot b draws next, None for an idle slot.  The
+    batch column becomes the largest live column, one more when that keeps cur_len's parity (the ParlerTTSLogitsProcessor state
+    is double-buffered on it), and row b's offset is cur_len - cols[b] >= 0; idle slots are parked at column 1."""
+    top = max((c for c in cols if c is not None), default=1)
+    new = top + ((top - cur_len) & 1)
+    return new, [new - (1 if c is None else c) for c in cols]
+
+
+class ContinuousRun:
+    """generate_continuous()'s iterator of (request index, waveform[, codes]) in completion order.  `refills` logs every request
+    put into a slot at a boundary as (slot, request, batch column of that boundary); `boundaries` and `steps` count the
+    boundaries and the decode steps enqueued."""
+
+    def __init__(self):
+        self.refills: list[tuple[int, int, int]] = []
+        self.boundaries = self.steps = 0
+        self._it = None
+
+    def __iter__(self):
+        return self
+
+    def __next__(self):
+        return next(self._it)
 
 
 def shift_tokens_right(input_ids: torch.Tensor, pad_token_id: int, decoder_start_token_id: int):
@@ -818,6 +908,11 @@ class GenSession:
         return self._view(_lib.lib().ptts_session_state, (8,), torch.int32)
 
     @property
+    def eos_seen(self) -> torch.Tensor:
+        """int32 [B * K]: 1 + the column of each row's first EOS, 0 while it has none."""
+        return self._view(_lib.lib().ptts_session_eos_seen, (self.B * self.K,), torch.int32)
+
+    @property
     def launches(self) -> int:
         n = C.c_int64()
         _lib.check(_lib.lib().ptts_session_launches(self.h, C.byref(n)))
@@ -919,6 +1014,22 @@ class GenSession:
 
     def decode_steps(self, n: int):
         _lib.check(_lib.lib().ptts_decode_steps(self.h, int(n), _lib.stream_ptr()))
+
+    def import_rows(self, src: "GenSession", src_rows: list[int], dst_rows: list[int]):
+        """ptts_session_import_rows: row src_rows[i] of `src` (begun from the BOS column, prefilled, sampled) becomes slot
+        dst_rows[i] of this session."""
+        n = len(src_rows)
+        if len(dst_rows) != n:
+            raise ValueError(f"{n} source rows and {len(dst_rows)} destination rows")
+        arr = lambda v: (C.c_int32 * max(n, 1))(*[int(x) for x in v])
+        _lib.check(_lib.lib().ptts_session_import_rows(self.h, src.h, arr(src_rows), arr(dst_rows), n, _lib.stream_ptr()))
+
+    def set_slots(self, cur_len: int, row_shift: list[int], row_key: list[int]):
+        """ptts_generate_set_slots: slot mode, row b at its own column cur_len - row_shift[b] with Philox key row_key[b]."""
+        if len(row_shift) != self.B or len(row_key) != self.B:
+            raise ValueError(f"row_shift and row_key must hold {self.B} entries")
+        arr = lambda v: (C.c_int32 * self.B)(*[int(x) for x in v])
+        _lib.check(_lib.lib().ptts_generate_set_slots(self.h, int(cur_len), arr(row_shift), arr(row_key), _lib.stream_ptr()))
 
     def set_outputs(self, logits: Optional[torch.Tensor], scores: Optional[torch.Tensor], first_step: int = 0, n_steps: int = 0,
                     step_stride: int = 0):
@@ -2127,3 +2238,131 @@ class ParlerTTSForConditionalGeneration:
                 return out
             return output_values, out
         return output_values
+
+    # -- continuous batching -----------------------------------------------------------------------
+    @torch.no_grad()
+    def generate_continuous(self, input_ids=None, attention_mask=None, prompt_input_ids=None, prompt_attention_mask=None,
+                            batch_size: int = 32, refill_every: int = 16, seed=0, return_codes: bool = False, streamer=None,
+                            logits_processor=None, stopping_criteria=None, **kwargs) -> ContinuousRun:
+        """Generate N requests through `batch_size` slots of one live session, refilling a finished request's slot with the next
+        request while the others keep decoding.  Returns a ContinuousRun that yields (request index, waveform) as requests finish,
+        (request index, waveform, codes [K, T_i]) with return_codes=True.
+
+        The requests come as one generate() call's inputs (padded descriptions or `encoder_outputs`, prompts, masks) and share its
+        generation settings; max_length / max_new_tokens count in each request's own columns.  Request i draws with Philox key i
+        (substream i * K + k), the key generate() over the whole list gives row i.  Its codes and waveform equal that row's bit
+        for bit when generate()'s shards take the prefill kernels a batch_size-row batch takes: always in fp32; in bf16 when every
+        shard of generate() (32 rows, and the remainder) and a batch_size-row batch are all at or all below the wgmma GEMM's 128
+        rows, for both (P + 1) and S rows per request.  With N = 33 and P < 127, for example, generate() runs the last request in a
+        1-row shard below 128 rows, so its bits differ, as they would between generate() calls of different batch sizes.  The text
+        encoder runs once over the whole list before the first step, as in generate(): the first audio waits for all N
+        descriptions, and the encoder states of all N stay in memory (N x S x H in the model dtype).
+
+        Every `refill_every` decode steps a boundary reads every slot's outcome, computed on the device, in one host sync.  It cuts
+        the finished requests' codes out of the history (the delay pattern undone as generate() does), prefills the next requests
+        on a second session of batch_size rows (padded with the last request, so one prefill serves the whole refill and its GEMMs
+        take a batch_size-row batch's kernels), draws their first column there and imports them into the free slots
+        (ptts_session_import_rows).  The batch column is then rebased (rebase_slots, ptts_generate_set_slots), the next interval
+        is enqueued, and the finished requests' valid frames go through one ragged codec call behind it (the codec's range check
+        waits for that interval, which the next boundary waits for anyway).  Finished rows keep
+        decoding PAD until their boundary, so the live session holds max_length + refill_every columns.  Raises ValueError for what
+        check_continuous_generate lists."""
+        import copy
+        if isinstance(batch_size, bool) or not isinstance(batch_size, int) or batch_size < 1:
+            raise ValueError(f"batch_size must be a positive int, got {batch_size!r}")
+        if isinstance(refill_every, bool) or not isinstance(refill_every, int) or refill_every < 1:
+            raise ValueError(f"refill_every must be a positive int, got {refill_every!r}")
+        gc = copy.deepcopy(self.generation_config)
+        suppress_special = kwargs.pop("_suppress_special", False)
+        user_max_length = kwargs.get("max_length")
+        mk = gc.update(**kwargs)
+        unknown = sorted(k for k in mk if k not in self._MODEL_KWARGS)
+        if unknown:
+            raise ValueError(f"The following `model_kwargs` are not used by the model: {unknown}")
+        unsupported = {k: getattr(gc, k) for k, neutral in self._NEUTRAL_GENERATION_KNOBS.items() if getattr(gc, k, neutral) != neutral}
+        if unsupported or gc.num_beams != 1:
+            raise ValueError(f"generation options {unsupported or {'num_beams': gc.num_beams}} are not supported by the device loop")
+        for k in ("output_attentions", "output_hidden_states"):   # model kwargs in generate(); here refused like the config fields
+            if mk.get(k):
+                setattr(gc, k, True)
+        check_continuous_generate(gc, mk, streamer, logits_processor, stopping_criteria)
+        if gc.max_new_tokens is not None:
+            max_length = int(gc.max_new_tokens) + 1
+        else:
+            max_length = int(user_max_length if user_max_length is not None else gc.max_length)
+        if max_length < 2:
+            raise ValueError(f"max_length must allow at least one new token, got {max_length}")
+        enc_hidden, enc_mask, prompt_hidden, prompt_mask, _, _ = self._conditioning(
+            "generate_continuous", input_ids, attention_mask, mk.get("encoder_outputs"), prompt_input_ids, prompt_attention_mask,
+            mk.get("prompt_hidden_states"), cross_prompt_after_encoder_outputs=True)
+        sampling = self._sampling(gc, 1, max_length, seed, suppress_special)
+        run = ContinuousRun()
+        run._it = self._continuous_loop(run, enc_hidden, enc_mask, prompt_hidden, prompt_mask, sampling, batch_size, refill_every,
+                                        bool(return_codes))
+        return run
+
+    def _continuous_loop(self, run: ContinuousRun, enc_hidden, enc_mask, prompt_hidden, prompt_mask, s: Sampling, batch_size: int,
+                         refill_every: int, return_codes: bool):
+        d = self.config.decoder
+        K, eng, cs = d.num_codebooks, self.decoder.engine, self.config.audio_encoder.codebook_size
+        N, S = enc_hidden.shape[0], enc_hidden.shape[1]
+        P = 0 if prompt_hidden is None else prompt_hidden.shape[1]
+        Bl = min(batch_size, N)
+
+        def start(sess, first, count, row_base):   # begin + prefill + the first column, as a generate() shard does
+            sess.begin(s.max_length, do_sample=s.do_sample, temperature=s.temperature, top_k=s.top_k, top_p=s.top_p,
+                       min_new_tokens=s.min_new_tokens, seed=s.seed, suppress_special=s.suppress_special,
+                       codebook_size=s.codebook_size, row_base=row_base, ext=s.ext, lext=s.lext)
+            rows = lambda t: refill_rows(t, first, count, Bl)
+            sess.prefill(rows(prompt_hidden), rows(prompt_mask), rows(enc_hidden), rows(enc_mask))
+            sess.sample()
+
+        # Sessions of our own (DecoderEngine.session keeps one live session); max_input_len 2 gives both the per-row offsets.  The
+        # refill session has the live session's rows, so one prefill serves a whole refill.
+        live = GenSession(eng, Bl, P, S, P + s.max_length + refill_every, max_input_len=2)
+        fill = GenSession(eng, Bl, P, S, P + s.max_length, max_input_len=2) if N > Bl else None
+        start(live, 0, Bl, 0)            # requests 0 .. Bl-1: the first shard generate() would run
+        slot_req: list = list(range(Bl))
+        nxt, cur_len = Bl, 2
+        shift = [0] * Bl
+        live.set_slots(cur_len, shift, slot_req)
+        live.decode_steps(refill_every)
+        run.steps += refill_every
+        while True:
+            run.boundaries += 1
+            # every slot's outcome is computed on the device, then read in the boundary's one host sync
+            shift_dev = torch.tensor(shift, dtype=torch.int32).pin_memory().to(self.device, non_blocking=True)
+            fin, frames, codes, packed, n_valid = slot_outputs(live.raw_ids.view(Bl, K, -1), live.eos_seen.view(Bl, K)[:, K - 1],
+                                                               live.state[0], shift_dev, s.max_length, cs)
+            status = torch.cat([live.state[:1].long(), fin.long(), frames.long(), n_valid.long()]).cpu().tolist()
+            cur_len = status[0]
+            fin, frames, n_valid = status[1:1 + Bl], status[1 + Bl:1 + 2 * Bl], status[1 + 2 * Bl:]
+            cols = [cur_len - sh for sh in shift]
+            done = [b for b, r in enumerate(slot_req) if r is not None and fin[b]]
+            done_req = [slot_req[b] for b in done]
+            for b in done:
+                slot_req[b] = None
+            free = [b for b, r in enumerate(slot_req) if r is None]
+            g = min(len(free), N - nxt)
+            if g > 0:   # one prefill of Bl rows: the next g requests, padded with the last one
+                start(fill, nxt, g, nxt * K)
+                live.import_rows(fill, list(range(g)), free[:g])
+                for j, b in enumerate(free[:g]):
+                    slot_req[b], cols[b] = nxt + j, 2
+                    run.refills.append((b, nxt + j, cur_len))
+                nxt += g
+            last = all(r is None for r in slot_req)
+            if not last:
+                cur_len, shift = rebase_slots(cur_len, [c if r is not None else None for c, r in zip(cols, slot_req)])
+                live.set_slots(cur_len, shift, [0 if r is None else r for r in slot_req])
+                live.decode_steps(refill_every)   # enqueued before the finished requests' codec call and the caller's turn
+                run.steps += refill_every
+            if done:
+                # the codes were cut before any import overwrote their slots; the codec call queues behind the next interval
+                audio, lengths = packed_to_waveform(self.audio_encoder, torch.stack([packed[b] for b in done]),
+                                                    [n_valid[b] for b in done], self.dtype)
+                for j, (b, r) in enumerate(zip(done, done_req)):
+                    wav = audio[j, :lengths[j]]
+                    yield (r, wav, codes[b, :, :frames[b]]) if return_codes else (r, wav)
+            if last:
+                return
