@@ -483,6 +483,30 @@ int ptts_dac_encode(const ptts_dac_config* cfg, const void* dec_blob, const void
                     int64_t workspace_bytes, const void* audio, int32_t B, int32_t samples, int32_t n_q, int64_t* codes_out,
                     void* latents_out, void* stream);
 
+/* One codec convolution as the decode and encode walks launch it (test hook for the DAC conv kernels).  Activations are
+ * channels-last [B][rows][C] in dtype; every buffer belongs to the caller.
+ *   kernel 0: conv_kernel (bf16 or f32): out_raw = conv(snake_alpha(x)) + bias (+ res) (tanh when tanh_out); alpha [Cin] or
+ *             NULL (no input snake).  samples > 0 (conv_same only): the input has `samples` rows, zeros past them (the
+ *             generic encode walk's input conv).
+ *   kernel 1: conv_tc_kernel (bf16; PTTS_EINVAL where conv_tc_supported refuses): out_raw = conv(x) + bias (+ res) and/or
+ *             out_act = snake_{alpha_next}(that), alpha_next [Cout].  res may equal out_raw (in place).
+ *   kernel 2: final_conv_tanh_kernel (bf16, kind 0, Cout 1, taps 7, dil 1, final_conv_supported(Cin)): out_raw = tanh(conv + bias).
+ *   kernel 3: enc_input_conv_kernel (bf16, kind 0, Cin 1, taps 7, dil 1): T rows from `samples` <= T waveform samples x [B][samples];
+ *             out_raw and out_act = snake_{alpha_next}(out_raw), both required.
+ * kind (dil_or_stride = dilation for kind 0, the even stride s otherwise):
+ *   0 conv_same(Cin, Cout, T, taps, dil):  Conv1d(k = taps, dilation, "same"), weight [Cout][Cin][taps], T rows in and out;
+ *   1 conv_up(Cin, Cout, T, s):            ConvTranspose1d(k = 2s, stride s, pad ceil(s/2)), weight [Cin][Cout][2s], T -> T*s rows;
+ *   2 conv_super_rows(Cin, Cout, T, s):    Conv1d(k = 2s, stride s, pad s/2), weight [Cout][Cin][2s], T -> T/s rows (T % s == 0).
+ * frame_lengths (device int32 [B], or NULL) and frames: a ragged batch as in ptts_dac_decode2, input and output rows being whole
+ * frames (kernels 0-2).  The weight is packed into `scratch` by the blob's pack for that tensor; scratch holds at least
+ * (2 * Cin * Cout * k + k * Cin) * dtype size + 256 bytes (k = taps, or 2s).  PTTS_EINVAL for what the kernel or its launcher
+ * refuses: taps > 7 or a receptive field wider than conv_kernel's tile, a ragged reach past conv_tc_kernel's zero band, a
+ * kernel / dtype / argument combination it does not take. */
+int ptts_op_dac_conv(int32_t dtype, int32_t kernel, int32_t kind, int32_t B, int32_t Cin, int32_t Cout, int32_t T, int32_t taps,
+                     int32_t dil_or_stride, int32_t samples, const void* weight, const void* bias, const void* alpha,
+                     const void* alpha_next, const void* x, const void* res, void* out_raw, void* out_act, int32_t tanh_out,
+                     const int32_t* frame_lengths, int32_t frames, void* scratch, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -1222,4 +1222,80 @@ int ptts_dac_encode(const ptts_dac_config* cfg, const void* dec_blob, const void
                     (cudaStream_t)stream);
 }
 
+// One codec conv launch (test hook).  The geometry comes from the dac.h constructors and the weights go through the packs the
+// blobs use, so that both are under test with the kernel.
+int ptts_op_dac_conv(int32_t dtype, int32_t kernel, int32_t kind, int32_t B, int32_t Cin, int32_t Cout, int32_t T, int32_t taps,
+                     int32_t dil_or_stride, int32_t samples, const void* weight, const void* bias, const void* alpha,
+                     const void* alpha_next, const void* x, const void* res, void* out_raw, void* out_act, int32_t tanh_out,
+                     const int32_t* frame_lengths, int32_t frames, void* scratch, void* stream) {
+  PTTS_REQUIRE(weight && bias && x && scratch && (out_raw || out_act), "null argument");
+  PTTS_REQUIRE(dtype == PTTS_BF16 || dtype == PTTS_F32, "op_dac_conv: dtype must be bf16 or f32");
+  PTTS_REQUIRE(kernel >= 0 && kernel <= 3, "op_dac_conv: kernel is 0 (conv_kernel), 1 (conv_tc_kernel), 2 (final conv) or 3 (input conv)");
+  PTTS_REQUIRE(kind >= 0 && kind <= 2, "op_dac_conv: kind is 0 (conv_same), 1 (conv_up) or 2 (conv_super_rows)");
+  PTTS_REQUIRE(B > 0 && Cin > 0 && Cout > 0 && T > 0 && taps > 0 && dil_or_stride > 0, "op_dac_conv: bad shape");
+  PTTS_REQUIRE(kernel == 0 || dtype == PTTS_BF16, "op_dac_conv: kernel %d is bf16 only", kernel);
+  PTTS_REQUIRE(kind == 0 || dil_or_stride % 2 == 0, "op_dac_conv: stride %d must be even", dil_or_stride);
+  PTTS_REQUIRE(kind != 2 || T % dil_or_stride == 0, "op_dac_conv: conv_super_rows needs T %% s == 0");
+  PTTS_REQUIRE(frame_lengths == nullptr || frames > 0, "op_dac_conv: frame_lengths needs frames > 0");
+  const int s = dil_or_stride;
+  ConvArgs a = kind == 0 ? conv_same(Cin, Cout, T, taps, dil_or_stride) : kind == 1 ? conv_up(Cin, Cout, T, s) : conv_super_rows(Cin, Cout, T, s);
+  a.x = x; a.bias = bias; a.res = res;
+  const int k_src = kind == 0 ? taps : 2 * s;   // taps of the PyTorch weight
+  cudaStream_t st = (cudaStream_t)stream;
+  auto ragged = [&](const ConvArgs& c) {
+    if (frame_lengths == nullptr) return RowLengths{};
+    return RowLengths{frame_lengths, frames, c.Tin / frames, c.Tout / frames};
+  };
+  PTTS_REQUIRE(frame_lengths == nullptr || (a.Tin % frames == 0 && a.Tout % frames == 0), "op_dac_conv: %d / %d rows are not whole frames of %d",
+               a.Tin, a.Tout, frames);
+  switch (kernel) {
+    case 0: {   // conv_kernel, snake_alpha on the input; alpha of a strided conv tiled s times over the super-row channels
+      PTTS_REQUIRE(!alpha_next && !out_act && out_raw, "op_dac_conv: conv_kernel writes out_raw only");
+      PTTS_REQUIRE(samples == 0 || (kind == 0 && samples > 0 && samples <= T), "op_dac_conv: samples is for conv_same only, 1..T");
+      if (samples > 0) a.Tin = samples;   // the encoder's input conv: rows past `samples` read zeros
+      const int es = dtype_size(dtype);
+      if (kind == 2) {
+        if (int e = pack_strided_conv(weight, dtype, scratch, dtype, Cout, Cin, s, 0, st)) return e;
+      } else if (int e = pack_conv(weight, dtype, scratch, dtype, kind == 1 ? Cin : Cout, kind == 1 ? Cout : Cin, k_src, kind == 1, st)) {
+        return e;
+      }
+      a.w = scratch;
+      a.alpha = alpha;
+      if (kind == 2 && alpha != nullptr) {
+        char* tiled = (char*)scratch + align_up((int64_t)3 * s * Cin * Cout * es, 256);
+        for (int i = 0; i < s; i++)
+          if (int e = pack_plain(alpha, dtype, Cin, tiled + (int64_t)i * Cin * es, dtype, st)) return e;
+        a.alpha = tiled;
+      }
+      a.out = out_raw; a.tanh_out = tanh_out ? 1 : 0;
+      return launch_conv(a, dtype, B, st, ragged(a));
+    }
+    case 1: {   // conv_tc_kernel: snake_{alpha_next} of the output
+      PTTS_REQUIRE(conv_tc_supported(a.Cin, a.Cout), "op_dac_conv: conv_tc_kernel does not take Cin %d, Cout %d", a.Cin, a.Cout);
+      PTTS_REQUIRE(!alpha && !tanh_out && samples == 0, "op_dac_conv: conv_tc_kernel has no input snake, tanh or samples");
+      PTTS_REQUIRE(!out_act == !alpha_next, "op_dac_conv: out_act and alpha_next go together");
+      if (kind == 2) {
+        if (int e = pack_strided_conv(weight, dtype, scratch, PTTS_BF16, Cout, Cin, s, 1, st)) return e;
+      } else if (int e = pack_conv_kmajor(weight, dtype, scratch, kind == 1 ? Cin : Cout, kind == 1 ? Cout : Cin, k_src, kind == 1, st)) {
+        return e;
+      }
+      return launch_conv_tc(a, scratch, a.n_taps * a.n_phase, alpha_next, out_raw, out_act, B, st, ragged(a));
+    }
+    case 2: {   // final_conv_tanh_kernel over an already snake'd input
+      PTTS_REQUIRE(kind == 0 && Cout == 1 && taps == 7 && dil_or_stride == 1 && final_conv_supported(Cin),
+                   "op_dac_conv: the final conv is conv_same(C, 1, T, 7, 1) with final_conv_supported(C), got Cin %d Cout %d taps %d", Cin, Cout, taps);
+      PTTS_REQUIRE(!alpha && !alpha_next && !res && !out_act && out_raw && tanh_out && samples == 0, "op_dac_conv: the final conv writes tanh to out_raw only");
+      if (int e = pack_conv(weight, dtype, scratch, dtype, Cout, Cin, 7, 0, st)) return e;
+      return launch_final_conv_tanh(x, scratch, bias, out_raw, Cin, T, B, frame_lengths, frames, st);
+    }
+    default: {  // enc_input_conv_kernel: T rows from `samples` waveform samples, raw and snake_{alpha_next}
+      PTTS_REQUIRE(kind == 0 && Cin == 1 && taps == 7 && dil_or_stride == 1 && samples > 0 && samples <= T,
+                   "op_dac_conv: the input conv is conv_same(1, C, T, 7, 1) over 1..T samples");
+      PTTS_REQUIRE(!alpha && !res && !tanh_out && !frame_lengths && alpha_next && out_raw && out_act, "op_dac_conv: the input conv writes raw and snake_{alpha_next}");
+      if (int e = pack_conv(weight, dtype, scratch, dtype, Cout, 1, 7, 0, st)) return e;
+      return launch_enc_input_conv(x, scratch, bias, alpha_next, out_raw, out_act, Cout, samples, T, B, st);
+    }
+  }
+}
+
 }  // extern "C"

@@ -116,7 +116,8 @@ __global__ void __launch_bounds__(256) enc_input_conv_kernel(const bf16* __restr
     const __nv_bfloat162 ax = __hmul2(chan[half + cp], r2);
     const float2 axf = __bfloat1622float2(ax);
     const __nv_bfloat162 sn = __floats2bfloat162_rn(__sinf(axf.x), __sinf(axf.y));
-    *reinterpret_cast<__nv_bfloat162*>(out_act + o) = __hadd2(r2, __hmul2(chan[2 * half + cp], __hmul2(sn, sn)));
+    // __hmul2_rn keeps the product's own rounding (torch's): a plain __hmul2 followed by __hadd2 is contracted into an fma
+    *reinterpret_cast<__nv_bfloat162*>(out_act + o) = __hadd2(r2, __hmul2_rn(chan[2 * half + cp], __hmul2(sn, sn)));
   }
 }
 int launch_enc_input_conv(const void* audio, const void* w, const void* bias, const void* alpha_next, void* out_raw, void* out_act,

@@ -127,7 +127,8 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant_
         const float2 axf = __bfloat1622float2(ax);
         const __nv_bfloat162 sn = __floats2bfloat162_rn(__sinf(axf.x), __sinf(axf.y));  // sin(.)  (MUFU; bf16 result)
         const __nv_bfloat162 sq = __hmul2(sn, sn);                                    // ^2
-        *reinterpret_cast<__nv_bfloat162*>(p.out_act + orow + c) = __hadd2(r2, __hmul2(inv2[c >> 1], sq));  // x + inv * sin^2
+        *reinterpret_cast<__nv_bfloat162*>(p.out_act + orow + c) = __hadd2(r2, __hmul2_rn(inv2[c >> 1], sq));  // x + inv * sin^2
+        // (_rn: the product is rounded before the add, as in torch -- a plain __hmul2 would be contracted into an fma)
       }
     }
   }
