@@ -482,6 +482,14 @@ int ptts_dac_encode_workspace_bytes(const ptts_dac_config* cfg, int32_t B, int32
 int ptts_dac_encode(const ptts_dac_config* cfg, const void* dec_blob, const void* enc_blob, void* workspace,
                     int64_t workspace_bytes, const void* audio, int32_t B, int32_t samples, int32_t n_q, int64_t* codes_out,
                     void* latents_out, void* stream);
+/* Same, over a ragged batch: row b holds sample_lengths[b] = n_b samples (device int32 [B]; NULL = every row has `samples`,
+ * which is ptts_dac_encode).  Row b of codes_out and latents_out equals the encode of audio[b, :n_b] alone, bit for bit, in
+ * frames [0, ceil(n_b / hop)); later frames hold codebook_size in every codebook and zero latents.  Samples at or past n_b are
+ * never read and may hold any value.  The kernels clamp each length to [1, samples]; the caller validates them.  The
+ * workspace is ptts_dac_encode_workspace_bytes(B, samples). */
+int ptts_dac_encode2(const ptts_dac_config* cfg, const void* dec_blob, const void* enc_blob, void* workspace,
+                     int64_t workspace_bytes, const void* audio, int32_t B, int32_t samples, const int32_t* sample_lengths,
+                     int32_t n_q, int64_t* codes_out, void* latents_out, void* stream);
 
 /* One codec convolution as the decode and encode walks launch it (test hook for the DAC conv kernels).  Activations are
  * channels-last [B][rows][C] in dtype; every buffer belongs to the caller.

@@ -121,6 +121,7 @@ _SIGS = {
     "ptts_dac_encoder_pack": (C.c_int, [C.POINTER(DacConfigC), _VP, _I32, _VP, _I32, _I64, _VP]),
     "ptts_dac_encode_workspace_bytes": (C.c_int, [C.POINTER(DacConfigC), _I32, _I32, C.POINTER(_I64)]),
     "ptts_dac_encode": (C.c_int, [C.POINTER(DacConfigC), _VP, _VP, _VP, _I64, _VP, _I32, _I32, _I32, _VP, _VP, _VP]),
+    "ptts_dac_encode2": (C.c_int, [C.POINTER(DacConfigC), _VP, _VP, _VP, _I64, _VP, _I32, _I32, _VP, _I32, _VP, _VP, _VP]),
     "ptts_op_dac_conv": (C.c_int, [_I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _VP, _VP, _VP, _VP, _VP, _VP, _VP,
                                    _VP, _I32, _VP, _I32, _VP, _VP]),
 }

@@ -1213,13 +1213,22 @@ int ptts_dac_encode_workspace_bytes(const ptts_dac_config* cfg, int32_t B, int32
 
 int ptts_dac_encode(const ptts_dac_config* cfg, const void* dec_blob, const void* enc_blob, void* workspace, int64_t workspace_bytes,
                     const void* audio, int32_t B, int32_t samples, int32_t n_q, int64_t* codes_out, void* latents_out, void* stream) {
+  return ptts_dac_encode2(cfg, dec_blob, enc_blob, workspace, workspace_bytes, audio, B, samples, nullptr, n_q, codes_out, latents_out,
+                          stream);
+}
+
+// sample_lengths (device, [B], or NULL): every kernel clamps each value to [1, samples], reads no sample at or past it, and the
+// frames past the row's ceil(n_b / hop) hold codebook_size and zero latents (RowLengths in dac.h).
+int ptts_dac_encode2(const ptts_dac_config* cfg, const void* dec_blob, const void* enc_blob, void* workspace, int64_t workspace_bytes,
+                     const void* audio, int32_t B, int32_t samples, const int32_t* sample_lengths, int32_t n_q, int64_t* codes_out,
+                     void* latents_out, void* stream) {
   PTTS_REQUIRE(cfg && dec_blob && enc_blob && workspace && audio && codes_out, "null argument");
   if (int e = validate_dac_encoder(*cfg)) return e;
   PTTS_REQUIRE(B > 0 && samples > 0, "dac encode: empty input B=%d samples=%d", B, samples);
   PTTS_REQUIRE(n_q >= 1 && n_q <= cfg->n_codebooks, "dac encode: n_q %d outside 1..%d", n_q, cfg->n_codebooks);
   PTTS_REQUIRE(workspace_bytes >= dac_encode_workspace(*cfg, B, samples).bytes(), "dac encode: workspace too small");
-  return dac_encode(*cfg, dec_blob, enc_blob, workspace, audio, B, samples, n_q, codes_out, latents_out, env_flag("PTTS_DAC_TC", true),
-                    (cudaStream_t)stream);
+  return dac_encode(*cfg, dec_blob, enc_blob, workspace, audio, B, samples, sample_lengths, n_q, codes_out, latents_out,
+                    env_flag("PTTS_DAC_TC", true), (cudaStream_t)stream);
 }
 
 // One codec conv launch (test hook).  The geometry comes from the dac.h constructors and the weights go through the packs the
@@ -1293,7 +1302,7 @@ int ptts_op_dac_conv(int32_t dtype, int32_t kernel, int32_t kind, int32_t B, int
                    "op_dac_conv: the input conv is conv_same(1, C, T, 7, 1) over 1..T samples");
       PTTS_REQUIRE(!alpha && !res && !tanh_out && !frame_lengths && alpha_next && out_raw && out_act, "op_dac_conv: the input conv writes raw and snake_{alpha_next}");
       if (int e = pack_conv(weight, dtype, scratch, dtype, Cout, 1, 7, 0, st)) return e;
-      return launch_enc_input_conv(x, scratch, bias, alpha_next, out_raw, out_act, Cout, samples, T, B, st);
+      return launch_enc_input_conv(x, scratch, bias, alpha_next, out_raw, out_act, Cout, samples, T, B, nullptr, 0, st);
     }
   }
 }

@@ -28,7 +28,7 @@ __device__ __forceinline__ float snake_fn(float x, float alpha, float inv) {
 
 constexpr int CT_M = 64, CT_N = 64, CT_K = 16, CT_AROWS = 128, CT_MAXTAPS = 7;
 
-template <typename T>
+template <typename T, bool SAMPLES>   // SAMPLES: a ragged encode's lengths (RowLengths, hop > 0)
 __global__ void __launch_bounds__(256) conv_kernel(ConvArgs p, RowLengths rl) {
   __shared__ float As[CT_K][CT_AROWS];
   __shared__ __align__(16) float Bs[CT_MAXTAPS][CT_K][CT_N];
@@ -43,7 +43,7 @@ __global__ void __launch_bounds__(256) conv_kernel(ConvArgs p, RowLengths rl) {
   // decode sees) and writes 0 past its output end; a tile wholly past the end skips the K loop
   int t_in = p.Tin, t_out = p.Tout, q_end = p.q_count;
   if (rl.frame_lengths != nullptr) {
-    const int n = row_frames(rl.frame_lengths, b, rl.frames);
+    const int n = row_frames<SAMPLES>(rl.frame_lengths, b, rl.frames, rl.hop);
     t_in = n * rl.up_in; t_out = n * rl.up_out; q_end = p.q_count - p.Tin + t_in;
   }
   const T* __restrict__ x = reinterpret_cast<const T*>(p.x) + (size_t)b * p.Tin * p.Cin;
@@ -127,8 +127,9 @@ int launch_conv(const ConvArgs& a, int dtype, int B, cudaStream_t st, const RowL
   PTTS_REQUIRE(a.n_taps >= 1 && a.n_taps <= CT_MAXTAPS, "conv: n_taps %d out of range", a.n_taps);
   PTTS_REQUIRE(CT_M + abs((a.n_taps - 1) * a.off_step) <= CT_AROWS, "conv: receptive field too wide");
   dim3 grid((a.q_count + CT_M - 1) / CT_M, (a.Cout + CT_N - 1) / CT_N, B * a.n_phase);
-  if (dtype == PTTS_BF16) conv_kernel<bf16><<<grid, 256, 0, st>>>(a, rl);
-  else conv_kernel<float><<<grid, 256, 0, st>>>(a, rl);
+  const bool samples = rl.frame_lengths != nullptr && rl.hop > 0;
+  if (dtype == PTTS_BF16) (samples ? conv_kernel<bf16, true> : conv_kernel<bf16, false>)<<<grid, 256, 0, st>>>(a, rl);
+  else (samples ? conv_kernel<float, true> : conv_kernel<float, false>)<<<grid, 256, 0, st>>>(a, rl);
   PTTS_LAUNCH_CHECK();
   return PTTS_OK;
 }

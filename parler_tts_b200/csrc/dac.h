@@ -38,18 +38,32 @@ static inline ConvArgs conv_up(int Cin, int Cout, int T, int s) {
 // [B][T/s][s*C] view (pack_strided_conv below).
 static inline ConvArgs conv_super_rows(int C, int Cout, int T, int s) { return conv_same(s * C, Cout, T / s, 3, 1); }
 
-// Ragged decode: row b holds frame_lengths[b] code frames (clamped to [0, frames]) and ends at frame_lengths[b] * up_in on a
-// conv's input axis, * up_out on its output axis.  Outputs past a row's end are written as 0, so that the buffers hold the zero
-// padding a standalone decode of the row sees.  frame_lengths == nullptr: every row is full (equal lengths, and the encoder).
+// Ragged batch: row b holds n_b code frames and ends at n_b * up_in on a conv's input axis, * up_out on its output axis.  Outputs
+// past a row's end are written as 0, so that the buffers hold the zero padding a standalone run of the row sees.
+//   hop == 0 (decode): n_b = frame_lengths[b], clamped to [0, frames];
+//   hop > 0 (encode):  frame_lengths[b] counts waveform samples, clamped to [1, frames * hop]; n_b = ceil(samples / hop).
+// frame_lengths == nullptr: every row is full (equal lengths).
 struct RowLengths {
   const int32_t* frame_lengths;
   int frames, up_in, up_out;
+  int hop;
 };
 int launch_conv(const ConvArgs& a, int dtype, int B, cudaStream_t st, const RowLengths& rl = RowLengths{});
 
 // code frames of row b of a ragged decode, clamped to [0, frames] so that no value can move a kernel outside its row
 __device__ __forceinline__ int row_frames(const int32_t* frame_lengths, int b, int frames) {
   return min(max(__ldg(frame_lengths + b), 0), frames);
+}
+// waveform samples of row b of a ragged encode, clamped to [1, samples]
+__device__ __forceinline__ int row_samples(const int32_t* sample_lengths, int b, int samples) {
+  return min(max(__ldg(sample_lengths + b), 1), samples);
+}
+// code frames of row b, lengths counting samples (SAMPLES: a ragged encode, hop > 0) or frames.  The kernels that take both are
+// instantiated once per reading, so that the decode's instantiations stay the code they were before the encode's.
+template <bool SAMPLES>
+__device__ __forceinline__ int row_frames(const int32_t* lengths, int b, int frames, int hop) {
+  if constexpr (SAMPLES) return (row_samples(lengths, b, frames * hop) + hop - 1) / hop;
+  else return row_frames(lengths, b, frames);
 }
 
 struct FromCodesArgs {
@@ -164,11 +178,13 @@ int pack_strided_conv(const void* src, int src_dtype, void* dst, int dst_dtype, 
 // codebook [n][D] (rounded to bf16 first when round_bf16) -> rows / max(||row||, 1e-12) in fp32 (F.normalize)
 int pack_normalized_codebook(const void* src, int src_dtype, float* dst, int n, int D, int round_bf16, cudaStream_t st);
 // Conv1d(1 -> C, k = 7, pad 3) over the waveform [B][samples] (zero beyond `samples`, T rows out, bf16): raw [B][T][C] and
-// snake_{alpha_next}(raw) for the next layer -- the wgmma kernel needs Cin >= 64.
+// snake_{alpha_next}(raw) for the next layer -- the wgmma kernel needs Cin >= 64.  sample_lengths (nullptr: none), a ragged
+// encode as in RowLengths with T / hop frames: row b reads no sample past its own count and ends at ceil(count / hop) * hop rows;
+// it writes zeros over more than conv_tc_kernel's 128-row zero band past that end.
 int launch_enc_input_conv(const void* audio, const void* w, const void* bias, const void* alpha_next, void* out_raw, void* out_act,
-                          int C, int samples, int T, int B, cudaStream_t st);
+                          int C, int samples, int T, int B, const int32_t* sample_lengths, int hop, cudaStream_t st);
 struct QuantizeArgs {
-  const void* z;          // [B][T][Z] encoder output
+  void* z;                // [B][T][Z] encoder output (frames past a ragged row's end are set to 0)
   const void* in_w;       // [K][D][Z]
   const void* in_b;       // [K][D]
   const float* cb_norm;   // [K][cs][D] fp32, unit rows
@@ -177,6 +193,8 @@ struct QuantizeArgs {
   const void* out_b;      // [K][Z]   (decode blob)
   int64_t* codes;         // [B][n_q][T]
   int n_q, D, Z, T, codebook_size;
+  const int32_t* sample_lengths;   // [B] or nullptr: a ragged encode (RowLengths, hop > 0); frames past a row's end code as
+  int hop;                         // codebook_size and read no latent
 };
 bool quantize_supported(int Z, int D);
 int launch_quantize(const QuantizeArgs& a, int dtype, int B, cudaStream_t st);
@@ -295,8 +313,10 @@ static inline DacWorkspace dac_encode_workspace(const ptts_dac_config& c, int B,
 int dac_decode(const ptts_dac_config& c, const void* blob, void* ws, const int64_t* codes, int B, int T, const int32_t* frame_lengths,
                void* audio, bool allow_tc, cudaStream_t st);
 // waveform [B][samples] -> codes [B][n_q][T] and, when latents != nullptr, the encoder output [B][T][latent_dim] (dac_enc.cu).
-// allow_tc as for dac_decode.
+// sample_lengths (device [B], or nullptr: every row has `samples`): a ragged encode whose row b equals the encode of its first
+// sample_lengths[b] samples alone in its first ceil(sample_lengths[b] / hop) frames; later frames hold codebook_size and zero
+// latents.  allow_tc as for dac_decode.
 int dac_encode(const ptts_dac_config& c, const void* dec_blob, const void* enc_blob, void* ws, const void* audio, int B, int samples,
-               int n_q, int64_t* codes, void* latents, bool allow_tc, cudaStream_t st);
+               const int32_t* sample_lengths, int n_q, int64_t* codes, void* latents, bool allow_tc, cudaStream_t st);
 
 }  // namespace ptts

@@ -37,11 +37,11 @@ struct ConvTcArgs {
   bf16* out_raw;           // raw result or nullptr
   bf16* out_act;           // snake_{alpha_next}(result) for the next layer or nullptr
   const bf16* alpha_next;  // [Cout]
-  const int32_t* frame_lengths;  // ragged decode (RowLengths in dac.h); nullptr: every row is full
-  int frames, up_in, up_out;
+  const int32_t* frame_lengths;  // ragged batch (RowLengths in dac.h); nullptr: every row is full
+  int frames, up_in, up_out, hop;
 };
 
-template <int NT>
+template <int NT, bool SAMPLES>   // SAMPLES: a ragged encode's lengths (RowLengths, hop > 0)
 __global__ void __launch_bounds__(wg::THREADS, 2)
 conv_tc_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_w, const ConvTcArgs p) {
   extern __shared__ unsigned char smem_raw[];
@@ -51,13 +51,13 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant_
   const int phase = blockIdx.z % p.n_phase, b = blockIdx.z / p.n_phase;
   const int q0 = blockIdx.x * TC_M, n0 = blockIdx.y * NT;
   const int k_chunks = (p.Cin + TC_K - 1) / TC_K;
-  // Ragged decode.  The TMA map zero-fills only past the whole buffer, so a row's zero padding is written instead: every output
+  // Ragged batch.  The TMA map zero-fills only past the whole buffer, so a row's zero padding is written instead: every output
   // past the row's end is 0, in the tile that holds the end (q_end) and in the whole tile after it -- a band of more than TC_M
   // positions, wider than any following conv's reach past the end (host-checked).  Tiles past the band exit at once, tiles
   // wholly inside it skip the K loop: the work follows each row's frames, not B * T.
   int n_iter = p.n_taps * k_chunks;
   if (p.frame_lengths != nullptr) {
-    const int q_end = p.q_count - p.Tin + row_frames(p.frame_lengths, b, p.frames) * p.up_in;
+    const int q_end = p.q_count - p.Tin + row_frames<SAMPLES>(p.frame_lengths, b, p.frames, p.hop) * p.up_in;
     if ((int)blockIdx.x > q_end / TC_M + 1) return;
     if (q0 >= q_end) n_iter = 0;
   }
@@ -86,7 +86,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant_
     wg::tma_load_3d(b_dst, &map_w, kc * TC_K, n0, p.wt_base + phase * p.wt_phase_step + j * p.wt_step, bar);
   };
   wg::mainloop<NT>(pipe, n_iter, load, acc);
-  const int to_end = p.frame_lengths != nullptr ? row_frames(p.frame_lengths, b, p.frames) * p.up_out : p.Tout;
+  const int to_end = p.frame_lengths != nullptr ? row_frames<SAMPLES>(p.frame_lengths, b, p.frames, p.hop) * p.up_out : p.Tout;
   if ((threadIdx.x >> 5) == wg::PRODUCER_WARP) {
     // the producer warp, idle now, writes this tile's rows past the row's end: raw 0 (conv(0) + bias is not) and snake(0) = 0
     if (to_end < p.Tout) {
@@ -188,18 +188,22 @@ int conv_tc_ntile(int Cout) {
   return 32;
 }
 
-template <int NT>
-static int launch_conv_tile(const CUtensorMap& mx, const CUtensorMap& mw, const ConvTcArgs& p, int B, cudaStream_t st) {
+template <int NT, bool SAMPLES>
+static int launch_conv_tile_t(const CUtensorMap& mx, const CUtensorMap& mw, const ConvTcArgs& p, int B, cudaStream_t st) {
   const size_t smem = wg::smem_bytes<NT>(3 * NT * (int)sizeof(bf16));
   static bool attr = false;
   if (!attr) {
-    PTTS_CHECK_CUDA(cudaFuncSetAttribute(conv_tc_kernel<NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    PTTS_CHECK_CUDA(cudaFuncSetAttribute(conv_tc_kernel<NT, SAMPLES>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     attr = true;
   }
   dim3 grid((p.q_count + TC_M - 1) / TC_M, p.Cout / NT, B * p.n_phase);
-  conv_tc_kernel<NT><<<grid, wg::THREADS, smem, st>>>(mx, mw, p);
+  conv_tc_kernel<NT, SAMPLES><<<grid, wg::THREADS, smem, st>>>(mx, mw, p);
   PTTS_LAUNCH_CHECK();
   return PTTS_OK;
+}
+template <int NT>
+static int launch_conv_tile(const CUtensorMap& mx, const CUtensorMap& mw, const ConvTcArgs& p, int B, cudaStream_t st) {
+  return p.frame_lengths != nullptr && p.hop > 0 ? launch_conv_tile_t<NT, true>(mx, mw, p, B, st) : launch_conv_tile_t<NT, false>(mx, mw, p, B, st);
 }
 
 // x: [B][Tin][Cin] bf16, w: [taps_total][Cout][Cin] bf16
@@ -211,12 +215,13 @@ int launch_conv_tc(const ConvArgs& a, const void* w_kmajor, int taps_total, cons
   p.n_phase = a.n_phase; p.wt_phase_step = a.wt_phase_step; p.o_mul = a.o_mul; p.o_add = a.o_add; p.o_phase_step = a.o_phase_step;
   const int n_tile = conv_tc_ntile(a.Cout);
   p.bias = (const bf16*)a.bias; p.res = (const bf16*)a.res; p.out_raw = (bf16*)out_raw; p.out_act = (bf16*)out_act; p.alpha_next = (const bf16*)alpha_next;
-  p.frame_lengths = rl.frame_lengths; p.frames = rl.frames; p.up_in = rl.up_in; p.up_out = rl.up_out;
+  p.frame_lengths = rl.frame_lengths; p.frames = rl.frames; p.up_in = rl.up_in; p.up_out = rl.up_out; p.hop = rl.hop;
   if (rl.frame_lengths != nullptr) {
     // a kept output reads this far past its row's end: the highest tap offset, plus the row the transposed conv's extra q reads.
-    // The producer of x wrote zeros over more than TC_M positions past the end.
+    // The producer of x wrote zeros over more than TC_M positions past the end (for the encoder's super-row convs, more than
+    // TC_M rows of the full-rate view, which is more than TC_M / s super-rows: reach 1 needs s <= TC_M, and s <= 32).
     const int reach = std::max(std::max(a.off_base, a.off_base + (a.n_taps - 1) * a.off_step), 0) + (a.q_count - a.Tin);
-    PTTS_REQUIRE(reach <= TC_M, "conv_tc: a ragged decode reads %d rows past a row's end, more than the %d-row zero band", reach, TC_M);
+    PTTS_REQUIRE(reach <= TC_M, "conv_tc: a ragged batch reads %d rows past a row's end, more than the %d-row zero band", reach, TC_M);
     PTTS_REQUIRE(rl.frames > 0 && a.Tin == rl.frames * rl.up_in && a.Tout == rl.frames * rl.up_out, "conv_tc: ragged lengths do not match the shape");
   }
   CUtensorMap mx, mw;

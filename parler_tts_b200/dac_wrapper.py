@@ -180,22 +180,34 @@ def _encoder_state_dict(sd: dict[str, torch.Tensor], n_blocks: int) -> dict[str,
     return out
 
 
-def _frame_lengths(frame_lengths, B: int, T: int) -> torch.Tensor:
-    """DACModel.decode's frame_lengths -> int32 [B] on the host; ValueError for a wrong shape, dtype or value outside [0, T]."""
-    if isinstance(frame_lengths, torch.Tensor):
-        if frame_lengths.is_floating_point() or frame_lengths.is_complex() or frame_lengths.dtype == torch.bool:
-            raise ValueError(f"frame_lengths must hold integers, got {frame_lengths.dtype}")
-        n = frame_lengths.detach().cpu()
+def _row_lengths(lengths, B: int, lo: int, hi: int, name: str) -> torch.Tensor:
+    """Per-row lengths (ints or an integer tensor) -> int32 [B] on the host; ValueError for a wrong shape, dtype or a value
+    outside [lo, hi]."""
+    if isinstance(lengths, torch.Tensor):
+        if lengths.is_floating_point() or lengths.is_complex() or lengths.dtype == torch.bool:
+            raise ValueError(f"{name} must hold integers, got {lengths.dtype}")
+        n = lengths.detach().cpu()
     else:
-        vals = list(frame_lengths)
+        vals = list(lengths)
         if not all(isinstance(v, numbers.Integral) and not isinstance(v, bool) for v in vals):
-            raise ValueError(f"frame_lengths must hold integers, got {vals}")
+            raise ValueError(f"{name} must hold integers, got {vals}")
         n = torch.tensor([int(v) for v in vals], dtype=torch.int64)
     if n.shape != (B,):
-        raise ValueError(f"frame_lengths must have shape [{B}] (one length per batch row), got {tuple(n.shape)}")
-    if bool(((n < 0) | (n > T)).any()):
-        raise ValueError(f"frame_lengths must lie in [0, {T}], got {n.tolist()}")
+        raise ValueError(f"{name} must have shape [{B}] (one length per batch row), got {tuple(n.shape)}")
+    if bool(((n < lo) | (n > hi)).any()):
+        raise ValueError(f"{name} must lie in [{lo}, {hi}], got {n.tolist()}")
     return n.to(torch.int32)
+
+
+def _frame_lengths(frame_lengths, B: int, T: int) -> torch.Tensor:
+    """DACModel.decode's frame_lengths -> int32 [B] on the host; ValueError for a wrong shape, dtype or value outside [0, T]."""
+    return _row_lengths(frame_lengths, B, 0, T, "frame_lengths")
+
+
+def _sample_lengths(sample_lengths, B: int, samples: int) -> torch.Tensor:
+    """DACModel.encode's sample_lengths -> int32 [B] on the host; ValueError for a wrong shape, dtype or value outside
+    [1, samples]."""
+    return _row_lengths(sample_lengths, B, 1, samples, "sample_lengths")
 
 
 class DACModel:
@@ -309,12 +321,18 @@ class DACModel:
 
     # -- reference surface -------------------------------------------------------------------------
     @torch.no_grad()
-    def encode(self, input_values, padding_mask=None, bandwidth=None, return_dict=None, n_quantizers=None, sample_rate=None):
+    def encode(self, input_values, padding_mask=None, bandwidth=None, return_dict=None, n_quantizers=None, sample_rate=None,
+               sample_lengths=None):
         """input_values [B, 1, samples] -> DACEncoderOutput(audio_codes [1, B, n_q, ceil(samples / hop)] int64, audio_scales [None]).
 
         One chunk, right zero-padded to the hop like model.preprocess (:64); n_q = n_quantizers or every codebook.
         `padding_mask` and `bandwidth` are unused, as in the reference.  Float32 or model-dtype audio; it is rounded to the
-        model dtype before the first conv."""
+        model dtype before the first conv.
+
+        sample_lengths (ints or an integer tensor of shape [B], each in [1, samples]) encodes a ragged batch in one call: row b
+        equals the encode of input_values[b:b+1, :, :sample_lengths[b]] alone, bit for bit, in its first
+        F_b = ceil(sample_lengths[b] / hop) frames, and holds codebook_size (no frame) after them.  Samples past a row's length
+        are never read and may hold anything."""
         if not isinstance(input_values, torch.Tensor) or input_values.dim() != 3:
             raise ValueError(f"input_values must be [batch, channels, samples], got {getattr(input_values, 'shape', type(input_values))}")
         B, channels, n = input_values.shape
@@ -332,14 +350,17 @@ class DACModel:
         n_q = K if n_quantizers is None else int(n_quantizers)
         if not 1 <= n_q <= K:
             raise ValueError(f"n_quantizers must lie in 1..{K}, got {n_quantizers}")
-        codes, _ = self._encode(input_values[:, 0, :], n_q)
+        lengths = None if sample_lengths is None else _sample_lengths(sample_lengths, B, n)
+        codes, _ = self._encode(input_values[:, 0, :], n_q, sample_lengths=lengths)
         codes = codes[None]
         if return_dict is False:
             return (codes, [None])
         return DACEncoderOutput(codes, [None])
 
-    def _encode(self, audio: torch.Tensor, n_q: int, return_latents: bool = False):
-        """audio [B, samples] -> (codes [B, n_q, T] int64, encoder output [B, T, latent_dim] in the model dtype or None)."""
+    def _encode(self, audio: torch.Tensor, n_q: int, return_latents: bool = False, sample_lengths=None):
+        """audio [B, samples] -> (codes [B, n_q, T] int64, encoder output [B, T, latent_dim] in the model dtype or None).
+        sample_lengths: None, or an integer tensor [B] already checked to lie in [1, samples] (encode's ragged batch; the
+        latents past a row's frames are 0)."""
         if self.encoder_blob is None:
             raise ValueError(f"DACModel.encode is not available for this config: {self._encoder_error}")
         if not (self.encoder_loaded and self.loaded):
@@ -355,9 +376,10 @@ class DACModel:
             self._enc_ws = torch.empty(need.value, dtype=torch.uint8, device=self.device)
         codes = torch.empty(B, n_q, T, dtype=torch.int64, device=self.device)
         latents = torch.empty(B, T, self.config.latent_dim, dtype=self.dtype, device=self.device) if return_latents else None
-        _lib.check(lib.ptts_dac_encode(C.byref(self._c), _lib.ptr(self.blob), _lib.ptr(self.encoder_blob), _lib.ptr(self._enc_ws),
-                                       self._enc_ws.numel(), _lib.ptr(audio), B, n, n_q, _lib.ptr(codes), _lib.ptr(latents),
-                                       _lib.stream_ptr()))
+        lengths = None if sample_lengths is None else sample_lengths.to(device=self.device, dtype=torch.int32).contiguous()
+        _lib.check(lib.ptts_dac_encode2(C.byref(self._c), _lib.ptr(self.blob), _lib.ptr(self.encoder_blob), _lib.ptr(self._enc_ws),
+                                        self._enc_ws.numel(), _lib.ptr(audio), B, n, _lib.ptr(lengths), n_q, _lib.ptr(codes),
+                                        _lib.ptr(latents), _lib.stream_ptr()))
         return codes, latents
 
     @torch.no_grad()

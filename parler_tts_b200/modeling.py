@@ -11,6 +11,7 @@ PyTorch is used for device memory, streams and the one-off side inputs the path 
 from __future__ import annotations
 import contextlib
 import ctypes as C
+import functools
 import json
 import math
 import os
@@ -1693,8 +1694,9 @@ class ParlerTTSForConditionalGeneration:
         return enc_hidden, attention_mask, prompt_hidden, prompt_mask, text, eo
 
     def _encode_clips(self, clips, B: int):
-        """generate(input_values=[w_0, ..]): each clip [1, samples_b] or [samples_b] through DACModel.encode (clips of one length
-        together) -> the codes right-padded to the longest, [B, K, N_max], and their frame mask [B, N_max]."""
+        """generate(input_values=[w_0, ..]): each clip [1, samples_b] or [samples_b] through one ragged DACModel.encode call
+        (the clips right-padded to the longest, sample_lengths = their lengths) -> the codes right-padded to the longest,
+        [B, K, N_max] with 0 past each clip's frames, and their frame mask [B, N_max]."""
         K = self.config.decoder.num_codebooks
         if len(clips) != B:
             raise ValueError(f"input_values must hold batch_size = {B} clips, got {len(clips)}")
@@ -1709,18 +1711,20 @@ class ParlerTTSForConditionalGeneration:
             if w.dim() != 1 or w.shape[0] < 1:
                 raise ValueError(f"input_values[{i}] must be [1, samples] or [samples], got {tuple(w.shape)}")
             wavs.append(w)
-        codes = [None] * B
-        for n in sorted({w.shape[0] for w in wavs}):
-            idx = [i for i, w in enumerate(wavs) if w.shape[0] == n]
-            c = self.audio_encoder.encode(torch.stack([wavs[i] for i in idx])[:, None, :].to(self.device)).audio_codes
-            for j, i in enumerate(idx):
-                codes[i] = c.reshape(len(idx), K, -1)[j]
-        F = max(c.shape[-1] for c in codes)
-        ids = torch.zeros(B, K, F, dtype=torch.int64, device=self.device)
-        mask = torch.zeros(B, F, dtype=torch.int64)
-        for i, c in enumerate(codes):
-            ids[i, :, :c.shape[-1]] = c
-            mask[i, :c.shape[-1]] = 1
+        for i, w in enumerate(wavs):
+            if not w.is_floating_point():
+                raise ValueError(f"input_values[{i}] must be a floating-point waveform, got {w.dtype}")
+        # one dtype every clip widens to exactly, so that each is rounded to the model dtype as it would be on its own
+        dtype = functools.reduce(torch.promote_types, [w.dtype for w in wavs])
+        lens = [w.shape[0] for w in wavs]
+        wav = torch.zeros(B, max(lens), dtype=dtype, device=self.device)
+        for i, w in enumerate(wavs):
+            wav[i, :lens[i]] = w.to(self.device)
+        codes = self.audio_encoder.encode(wav[:, None, :], sample_lengths=lens).audio_codes.reshape(B, K, -1)
+        hop = self.audio_encoder.hop_length
+        frames = torch.tensor([-(-n // hop) for n in lens])
+        mask = (torch.arange(codes.shape[-1])[None, :] < frames[:, None]).to(torch.int64)
+        ids = codes.masked_fill(mask.to(self.device)[:, None, :] == 0, 0)
         return ids, mask
 
     def _codes_from_raw(self, output_ids, mask_src, max_length: int):
