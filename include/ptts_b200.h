@@ -462,6 +462,17 @@ int ptts_dac_decode(const ptts_dac_config* cfg, const void* blob, void* workspac
 int ptts_dac_decode2(const ptts_dac_config* cfg, const void* blob, void* workspace, int64_t workspace_bytes,
                      const int64_t* codes, int32_t B, int32_t T, const int32_t* frame_lengths, void* audio_out,
                      void* stream);
+/* Windowed decode, for streaming: row b's window is codes[b, :, s_b : s_b + n_b] of codes [B, K, T_codes] (s_b =
+ * frame_start[b], n_b = frame_lengths[b]; device int32 [B] each; n_b <= T <= T_codes, s_b + n_b <= T_codes).  It is decoded
+ * as ptts_dac_decode2 decodes that window copied alone to frame 0, and audio_out [B, 1, hop*T] holds, bit for bit, that decode's
+ * samples [hop*lo_b, hop*hi_b) (lo_b = emit_lo[b], hi_b = emit_hi[b], device int32 [B], 0 <= lo_b <= hi_b <= n_b) and 0
+ * everywhere else.  Each layer computes only the rows those samples depend on, so the cost follows the emit ranges, not the
+ * windows.  The kernels clamp the values; the caller guarantees that the ids inside the windows are in range.  The workspace
+ * is ptts_dac_workspace_bytes(B, T). */
+int ptts_dac_decode3(const ptts_dac_config* cfg, const void* blob, void* workspace, int64_t workspace_bytes,
+                     const int64_t* codes, int32_t B, int32_t T_codes, int32_t T,
+                     const int32_t* frame_start, const int32_t* frame_lengths,
+                     const int32_t* emit_lo, const int32_t* emit_hi, void* audio_out, void* stream);
 
 /* ---- DAC encode ------------------------------------------------------------------------------ */
 /* The encoder weights (encoder convs and snake alphas, quantizer in_proj, unit-normalised codebooks) live in a second blob

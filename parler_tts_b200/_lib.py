@@ -116,6 +116,7 @@ _SIGS = {
     "ptts_dac_workspace_bytes": (C.c_int, [C.POINTER(DacConfigC), _I32, _I32, C.POINTER(_I64)]),
     "ptts_dac_decode": (C.c_int, [C.POINTER(DacConfigC), _VP, _VP, _I64, _VP, _I32, _I32, _VP, _VP]),
     "ptts_dac_decode2": (C.c_int, [C.POINTER(DacConfigC), _VP, _VP, _I64, _VP, _I32, _I32, _VP, _VP, _VP]),
+    "ptts_dac_decode3": (C.c_int, [C.POINTER(DacConfigC), _VP, _VP, _I64, _VP, _I32, _I32, _I32, _VP, _VP, _VP, _VP, _VP, _VP]),
     "ptts_dac_encoder_blob_bytes": (C.c_int, [C.POINTER(DacConfigC), C.POINTER(_I64)]),
     "ptts_dac_encoder_num_tensors": (C.c_int, [C.POINTER(DacConfigC), C.POINTER(_I32)]),
     "ptts_dac_encoder_pack": (C.c_int, [C.POINTER(DacConfigC), _VP, _I32, _VP, _I32, _I64, _VP]),

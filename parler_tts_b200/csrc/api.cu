@@ -1162,6 +1162,20 @@ int ptts_dac_decode2(const ptts_dac_config* cfg, const void* blob, void* workspa
   return dac_decode(*cfg, blob, workspace, codes, B, T, frame_lengths, audio_out, env_flag("PTTS_DAC_TC", true), (cudaStream_t)stream);
 }
 
+// Windowed decode: row b decodes codes[b, :, s_b : s_b + n_b] as ptts_dac_decode2 decodes that window alone at frame 0 and keeps the
+// samples of window frames [emit_lo[b], emit_hi[b]); each layer computes only the rows those samples depend on (dac.cu).  The
+// kernels clamp n_b to [0, T], the emit range to [0, n_b] and s_b to [0, T_codes - n_b].
+int ptts_dac_decode3(const ptts_dac_config* cfg, const void* blob, void* workspace, int64_t workspace_bytes, const int64_t* codes,
+                     int32_t B, int32_t T_codes, int32_t T, const int32_t* frame_start, const int32_t* frame_lengths,
+                     const int32_t* emit_lo, const int32_t* emit_hi, void* audio_out, void* stream) {
+  PTTS_REQUIRE(cfg && blob && workspace && codes && audio_out && frame_start && frame_lengths && emit_lo && emit_hi, "null argument");
+  if (int e = validate_dac(*cfg)) return e;
+  PTTS_REQUIRE(B > 0 && T > 0 && T <= T_codes, "dac decode3: bad shape B=%d T=%d T_codes=%d (0 < T <= T_codes)", B, T, T_codes);
+  PTTS_REQUIRE(workspace_bytes >= dac_decode_workspace(*cfg, B, T).bytes(), "dac decode: workspace too small");
+  return dac_decode_window(*cfg, blob, workspace, codes, B, T, frame_lengths, DacWindow{frame_start, emit_lo, emit_hi, T_codes}, audio_out,
+                           env_flag("PTTS_DAC_TC", true), (cudaStream_t)stream);
+}
+
 // ---- DAC encode -----------------------------------------------------------------------------------
 int ptts_dac_encoder_blob_bytes(const ptts_dac_config* cfg, int64_t* out_bytes) {
   PTTS_REQUIRE(cfg && out_bytes, "null argument");

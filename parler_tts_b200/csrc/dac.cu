@@ -13,6 +13,7 @@
 // residual add and tanh are fused.  Roofline: tensor/FMA-bound (1.608 GFLOP per code frame, SURVEY 8d).
 // dac_decode at the end walks the codec's layers by name (dac.h) on this path or on the wgmma one (dac_tc.cu).
 #include <utility>
+#include <vector>
 
 #include "common.cuh"
 #include "dac.h"
@@ -28,7 +29,9 @@ __device__ __forceinline__ float snake_fn(float x, float alpha, float inv) {
 
 constexpr int CT_M = 64, CT_N = 64, CT_K = 16, CT_AROWS = 128, CT_MAXTAPS = 7;
 
-template <typename T, bool SAMPLES>   // SAMPLES: a ragged encode's lengths (RowLengths, hop > 0)
+// SAMPLES: a ragged encode's lengths (RowLengths, hop > 0).  WINDOW: a windowed decode (RowLengths::emit_lo), whose rows outside
+// needed_rows are written as 0 and whose tiles without a needed row skip the K loop.
+template <typename T, bool SAMPLES, bool WINDOW = false>
 __global__ void __launch_bounds__(256) conv_kernel(ConvArgs p, RowLengths rl) {
   __shared__ float As[CT_K][CT_AROWS];
   __shared__ __align__(16) float Bs[CT_MAXTAPS][CT_K][CT_N];
@@ -45,6 +48,12 @@ __global__ void __launch_bounds__(256) conv_kernel(ConvArgs p, RowLengths rl) {
   if (rl.frame_lengths != nullptr) {
     const int n = row_frames<SAMPLES>(rl.frame_lengths, b, rl.frames, rl.hop);
     t_in = n * rl.up_in; t_out = n * rl.up_out; q_end = p.q_count - p.Tin + t_in;
+  }
+  int2 need = make_int2(0, 0);
+  if constexpr (WINDOW) {
+    need = needed_rows(rl.emit_lo, rl.emit_hi, b, row_frames(rl.frame_lengths, b, rl.frames), rl.up_out, rl.m_lo, rl.m_hi);
+    const int to0 = q0 * p.o_mul + p.o_add + phase * p.o_phase_step;
+    if (to0 + (CT_M - 1) * p.o_mul < need.x || to0 >= need.y) q_end = q0;
   }
   const T* __restrict__ x = reinterpret_cast<const T*>(p.x) + (size_t)b * p.Tin * p.Cin;
   const T* __restrict__ w = reinterpret_cast<const T*>(p.w);
@@ -114,7 +123,7 @@ __global__ void __launch_bounds__(256) conv_kernel(ConvArgs p, RowLengths rl) {
       const int co = co0 + tx * 4 + j;
       if (co >= p.Cout) continue;
       const size_t o = ((size_t)b * p.Tout + to) * p.Cout + co;
-      if (to >= t_out) { out[o] = DT<T>::from_f(0.f); continue; }
+      if (to >= t_out || (WINDOW && (to < need.x || to >= need.y))) { out[o] = DT<T>::from_f(0.f); continue; }
       float v = DT<T>::rnd(acc[i][j] + DT<T>::to_f(bias[co]));
       if (res != nullptr) v = DT<T>::rnd(DT<T>::to_f(res[o]) + v);
       if (p.tanh_out) v = tanhf(v);
@@ -128,7 +137,10 @@ int launch_conv(const ConvArgs& a, int dtype, int B, cudaStream_t st, const RowL
   PTTS_REQUIRE(CT_M + abs((a.n_taps - 1) * a.off_step) <= CT_AROWS, "conv: receptive field too wide");
   dim3 grid((a.q_count + CT_M - 1) / CT_M, (a.Cout + CT_N - 1) / CT_N, B * a.n_phase);
   const bool samples = rl.frame_lengths != nullptr && rl.hop > 0;
-  if (dtype == PTTS_BF16) (samples ? conv_kernel<bf16, true> : conv_kernel<bf16, false>)<<<grid, 256, 0, st>>>(a, rl);
+  if (rl.emit_lo != nullptr) {
+    PTTS_REQUIRE(rl.frame_lengths != nullptr && !samples, "conv: a windowed decode needs frame lengths");
+    (dtype == PTTS_BF16 ? conv_kernel<bf16, false, true> : conv_kernel<float, false, true>)<<<grid, 256, 0, st>>>(a, rl);
+  } else if (dtype == PTTS_BF16) (samples ? conv_kernel<bf16, true> : conv_kernel<bf16, false>)<<<grid, 256, 0, st>>>(a, rl);
   else (samples ? conv_kernel<float, true> : conv_kernel<float, false>)<<<grid, 256, 0, st>>>(a, rl);
   PTTS_LAUNCH_CHECK();
   return PTTS_OK;
@@ -136,11 +148,18 @@ int launch_conv(const ConvArgs& a, int dtype, int B, cudaStream_t st, const RowL
 
 // quantizer.from_codes: z[b][t][c] = sum_k ( out_proj_k.bias[c] + sum_d out_proj_k.w[c][d] * codebook_k[code][d] )
 // accumulated codebook by codebook in the storage dtype (quantized_representation += ..., :367).
-template <typename T>
+template <typename T, bool WINDOW = false>   // WINDOW: a windowed decode (FromCodesArgs::emit_lo)
 __global__ void __launch_bounds__(256) from_codes_kernel(FromCodesArgs p) {
   __shared__ float e[32][16];  // [k][d] for this (b, t)
   const int t = blockIdx.x, b = blockIdx.y;
   const int K = p.K, D = p.D;
+  int src = t;   // code frame of latent frame t
+  if constexpr (WINDOW) {
+    const int n = row_frames(p.frame_lengths, b, p.T);
+    const int2 need = needed_rows(p.emit_lo, p.emit_hi, b, n, 1, p.m_lo, p.m_hi);
+    if (t < need.x || t >= need.y) return;                                  // not needed: left as it is
+    src = min(max(__ldg(p.frame_start + b), 0), p.codes_T - n) + t;         // n <= T <= codes_T (host-checked)
+  }
   if (p.frame_lengths != nullptr && t >= row_frames(p.frame_lengths, b, p.T)) {   // past a ragged row's end: a zero latent
     T* __restrict__ z = reinterpret_cast<T*>(p.z) + ((size_t)b * p.T + t) * p.C;
     for (int c = threadIdx.x; c < p.C; c += blockDim.x) z[c] = DT<T>::from_f(0.f);
@@ -148,7 +167,7 @@ __global__ void __launch_bounds__(256) from_codes_kernel(FromCodesArgs p) {
   }
   if (threadIdx.x < K * D) {
     const int k = threadIdx.x / D, d = threadIdx.x - k * D;
-    const int64_t code = p.codes[((size_t)b * K + k) * p.T + t];
+    const int64_t code = p.codes[((size_t)b * K + k) * (WINDOW ? p.codes_T : p.T) + src];
     e[k][d] = DT<T>::to_f(reinterpret_cast<const T*>(p.codebooks)[((size_t)k * p.codebook_size + code) * D + d]);
   }
   __syncthreads();
@@ -169,7 +188,10 @@ __global__ void __launch_bounds__(256) from_codes_kernel(FromCodesArgs p) {
 int launch_from_codes(const FromCodesArgs& a, int dtype, int B, cudaStream_t st) {
   PTTS_REQUIRE(a.K <= 32 && a.D <= 16 && a.K * a.D <= 256, "from_codes: K=%d D=%d unsupported", a.K, a.D);
   dim3 grid(a.T, B);
-  if (dtype == PTTS_BF16) from_codes_kernel<bf16><<<grid, 256, 0, st>>>(a);
+  if (a.emit_lo != nullptr) {
+    PTTS_REQUIRE(a.frame_lengths != nullptr && a.frame_start != nullptr && a.T <= a.codes_T, "from_codes: bad window arguments");
+    (dtype == PTTS_BF16 ? from_codes_kernel<bf16, true> : from_codes_kernel<float, true>)<<<grid, 256, 0, st>>>(a);
+  } else if (dtype == PTTS_BF16) from_codes_kernel<bf16><<<grid, 256, 0, st>>>(a);
   else from_codes_kernel<float><<<grid, 256, 0, st>>>(a);
   PTTS_LAUNCH_CHECK();
   return PTTS_OK;
@@ -211,9 +233,11 @@ int pack_conv(const void* src, int src_dtype, void* dst, int dst_dtype, int d0, 
 // C + 8 elements so that 8 consecutive threads' 16-byte reads hit 8 different bank groups), weights [7][C] as fp32.
 // bf16 inputs, fp32 accumulation in tap-major / channel order, one rounding of acc + bias, tanh, one rounding (torch's ops).
 constexpr int FC_T = 128;   // outputs per block
+template <bool WINDOW = false>   // WINDOW: a windowed decode, samples outside the emit range [emit_lo, emit_hi) are 0
 __global__ void __launch_bounds__(FC_T) final_conv_tanh_kernel(const bf16* __restrict__ x, const bf16* __restrict__ w, const bf16* __restrict__ bias,
                                                                bf16* __restrict__ out, int C, int T,
-                                                               const int32_t* __restrict__ frame_lengths, int frames) {
+                                                               const int32_t* __restrict__ frame_lengths, int frames,
+                                                               const int32_t* __restrict__ emit_lo, const int32_t* __restrict__ emit_hi) {
   extern __shared__ __align__(16) unsigned char fsm[];
   const int pitch = C + 8;                                   // elements
   bf16* xs = reinterpret_cast<bf16*>(fsm);                   // [FC_T + 6][pitch]
@@ -221,8 +245,13 @@ __global__ void __launch_bounds__(FC_T) final_conv_tanh_kernel(const bf16* __res
   const int b = blockIdx.y, t0 = blockIdx.x * FC_T, tid = threadIdx.x;
   // a ragged row's samples end at n_b * hop: later samples are 0 (not tanh(bias)); a block wholly past the end loads nothing.
   // Inputs up to 3 rows past the end are read by kept samples: the zero band the last conv wrote there.
-  const int t_end = frame_lengths != nullptr ? row_frames(frame_lengths, b, frames) * (T / frames) : T;
-  if (t0 >= t_end) {
+  int t_end = frame_lengths != nullptr ? row_frames(frame_lengths, b, frames) * (T / frames) : T;
+  int t_beg = 0;
+  if constexpr (WINDOW) {   // the emit range: the only samples computed, and they read only rows the convs before computed
+    const int2 need = needed_rows(emit_lo, emit_hi, b, row_frames(frame_lengths, b, frames), T / frames, 0, 0);
+    t_beg = need.x; t_end = need.y;
+  }
+  if (t0 >= t_end || (WINDOW && t0 + FC_T <= t_beg)) {
     if (t0 + tid < T) out[(size_t)b * T + t0 + tid] = __float2bfloat16_rn(0.f);
     return;
   }
@@ -251,17 +280,23 @@ __global__ void __launch_bounds__(FC_T) final_conv_tanh_kernel(const bf16* __res
     }
   }
   const float y = DT<bf16>::rnd(acc + __bfloat162float(bias[0]));
-  out[(size_t)b * T + t] = __float2bfloat16_rn(t < t_end ? tanhf(y) : 0.f);
+  out[(size_t)b * T + t] = __float2bfloat16_rn(t < t_end && (!WINDOW || t >= t_beg) ? tanhf(y) : 0.f);
 }
 
 bool final_conv_supported(int C) { return C % 8 == 0 && C <= 512; }
 int launch_final_conv_tanh(const void* x, const void* w, const void* bias, void* out, int C, int T, int B, const int32_t* frame_lengths,
-                           int frames, cudaStream_t st) {
+                           int frames, cudaStream_t st, const int32_t* emit_lo, const int32_t* emit_hi) {
   const size_t smem = (size_t)(FC_T + 6) * (C + 8) * 2 + (size_t)7 * C * 4;
   static bool attr = false;
-  if (!attr) { PTTS_CHECK_CUDA(cudaFuncSetAttribute(final_conv_tanh_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024)); attr = true; }
-  final_conv_tanh_kernel<<<dim3((T + FC_T - 1) / FC_T, B), FC_T, smem, st>>>((const bf16*)x, (const bf16*)w, (const bf16*)bias, (bf16*)out, C, T,
-                                                                                 frame_lengths, frames);
+  if (!attr) {
+    PTTS_CHECK_CUDA(cudaFuncSetAttribute(final_conv_tanh_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
+    PTTS_CHECK_CUDA(cudaFuncSetAttribute(final_conv_tanh_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
+    attr = true;
+  }
+  const bool window = emit_lo != nullptr;
+  PTTS_REQUIRE(!window || (frame_lengths != nullptr && emit_hi != nullptr), "final conv: a windowed decode needs frame lengths");
+  (window ? final_conv_tanh_kernel<true> : final_conv_tanh_kernel<false>)<<<dim3((T + FC_T - 1) / FC_T, B), FC_T, smem, st>>>(
+      (const bf16*)x, (const bf16*)w, (const bf16*)bias, (bf16*)out, C, T, frame_lengths, frames, emit_lo, emit_hi);
   PTTS_LAUNCH_CHECK();
   return PTTS_OK;
 }
@@ -270,14 +305,53 @@ int launch_final_conv_tanh(const void* x, const void* w, const void* bias, void*
 // Each conv gets its row lengths as time steps per code frame so far (Tin / T, Tout / T), which place each ragged row's end.
 static const int kDilation[3] = {1, 3, 9};
 
+// Windowed decode: the rows each layer must compute beyond [lo * up, hi * up) on its output axis, so that the samples of the emit
+// frames [lo, hi) come out as in a whole decode.  Walked backwards from the output conv (margins 0): a stride-1 conv with taps k,
+// dilation d reads (k - 1) / 2 * d rows on each side; the transposed conv's output row q * s - pad + p reads input rows q and
+// q - 1 (conv_up), so output rows [A, C) read input rows [floor((A + pad) / s) - 1, floor((C - 1 + pad) / s)].  The residual
+// path adds nothing (its reach is 0).  Same interval arithmetic as incremental.dac_dependency_radius; exact up to the transposed
+// conv's rounding, which only widens.  Returns [from_codes (latent frames), conv 1, ..., output conv], in walk order.
+struct Margin { int lo, hi; };
+static int floor_div(int a, int b) { return a >= 0 ? a / b : -((-a + b - 1) / b); }
+static std::vector<Margin> window_margins(const ptts_dac_config& c) {
+  std::vector<Margin> m;
+  Margin cur{0, 0};
+  auto same = [&](int taps, int dil) { m.push_back(cur); cur = {cur.lo + (taps - 1) / 2 * dil, cur.hi + (taps - 1) / 2 * dil}; };
+  same(7, 1);                                              // output conv
+  for (int bi = c.n_blocks - 1; bi >= 0; bi--) {
+    const int s = c.strides[bi], pad = (s + 1) / 2;
+    for (int r = 2; r >= 0; r--) { same(1, 1); same(7, kDilation[r]); }
+    m.push_back(cur);                                      // transposed conv
+    cur = {1 - floor_div(pad - cur.lo, s), floor_div(cur.hi - 1 + pad, s) + 1};
+  }
+  same(7, 1);                                              // conv 1
+  m.push_back(cur);                                        // from_codes
+  return std::vector<Margin>(m.rbegin(), m.rend());
+}
+
+// Each conv's RowLengths in walk order; in a windowed decode (win != nullptr) with its margins.
+struct WalkRows {
+  const int32_t* fl;
+  int T;
+  const DacWindow* win;
+  std::vector<Margin> m;
+  size_t i = 1;   // m[0] is from_codes'
+  RowLengths next(int up_in, int up_out) {
+    RowLengths r{fl, T, up_in, up_out};
+    if (win != nullptr) { r.emit_lo = win->emit_lo; r.emit_hi = win->emit_hi; r.m_lo = m[i].lo; r.m_hi = m[i].hi; }
+    i++;
+    return r;
+  }
+};
+
 // bf16, every conv but the last (Cout = 1) as a wgmma implicit GEMM.  Snake moves into the epilogue of the conv before it: a conv
 // writes its raw output where a residual needs it and snake_{alpha of the next layer}(output) for the next conv to read.
 static int decode_tc(const ptts_dac_config& c, const DacLayout& L, const char* bl, const DacWorkspace& W, void* ws, int B, int T,
-                     const int32_t* fl, void* audio, cudaStream_t st) {
+                     WalkRows& rows, void* audio, cudaStream_t st) {
   auto P = [&](int i) { return (const void*)(bl + L.t[i].off); };
   auto conv = [&](ConvArgs a, const void* x, int w, int b, const void* res, void* out_raw, void* out_act, const void* alpha_next) {
     a.x = x; a.bias = P(b); a.res = res;
-    return launch_conv_tc(a, bl + L.t[w].off_k, a.n_taps * a.n_phase, alpha_next, out_raw, out_act, B, st, RowLengths{fl, T, a.Tin / T, a.Tout / T});
+    return launch_conv_tc(a, bl + L.t[w].off_k, a.n_taps * a.n_phase, alpha_next, out_raw, out_act, B, st, rows.next(a.Tin / T, a.Tout / T));
   };
   char* act = W.buf(ws, 0);   // snake'd input of the next conv
   char* oth = W.buf(ws, 1);
@@ -300,20 +374,21 @@ static int decode_tc(const ptts_dac_config& c, const DacLayout& L, const char* b
     }
   }
   const int cl = C >> nb;
+  const RowLengths rl = rows.next(Tl / T, Tl / T);
   if (final_conv_supported(cl))   // one thread per output sample
-    return launch_final_conv_tanh(act, P(L.conv2_w), P(L.conv2_b), audio, cl, Tl, B, fl, T, st);
+    return launch_final_conv_tanh(act, P(L.conv2_w), P(L.conv2_b), audio, cl, Tl, B, rl.frame_lengths, T, st, rl.emit_lo, rl.emit_hi);
   ConvArgs f = conv_same(cl, 1, Tl, 7, 1);   // the input is already snake'd
   f.x = act; f.w = P(L.conv2_w); f.bias = P(L.conv2_b); f.out = audio; f.tanh_out = 1;
-  return launch_conv(f, c.dtype, B, st, RowLengths{fl, T, Tl / T, Tl / T});
+  return launch_conv(f, c.dtype, B, st, rl);
 }
 
 // Any dtype and width: snake applied on the fly to each conv's input, the residual added in place.
 static int decode_generic(const ptts_dac_config& c, const DacLayout& L, const char* bl, const DacWorkspace& W, void* ws, int B, int T,
-                          const int32_t* fl, void* audio, cudaStream_t st) {
+                          WalkRows& rows, void* audio, cudaStream_t st) {
   auto P = [&](int i) { return (const void*)(bl + L.t[i].off); };
   auto conv = [&](ConvArgs a, const void* x, const void* alpha, int w, int b, const void* res, void* out) {
     a.x = x; a.alpha = alpha; a.w = P(w); a.bias = P(b); a.res = res; a.out = out;
-    return launch_conv(a, c.dtype, B, st, RowLengths{fl, T, a.Tin / T, a.Tout / T});
+    return launch_conv(a, c.dtype, B, st, rows.next(a.Tin / T, a.Tout / T));
   };
   char* cur = W.buf(ws, 0);
   char* oth = W.buf(ws, 1);
@@ -338,20 +413,35 @@ static int decode_generic(const ptts_dac_config& c, const DacLayout& L, const ch
   return conv(f, cur, P(L.snake1), L.conv2_w, L.conv2_b, nullptr, audio);
 }
 
-int dac_decode(const ptts_dac_config& c, const void* blob, void* ws, const int64_t* codes, int B, int T, const int32_t* frame_lengths,
-               void* audio, bool allow_tc, cudaStream_t st) {
+static int decode_walk(const ptts_dac_config& c, const void* blob, void* ws, const int64_t* codes, int B, int T, const int32_t* frame_lengths,
+                       const DacWindow* win, void* audio, bool allow_tc, cudaStream_t st) {
   const DacLayout L = make_dac_layout(c);
   const DacWorkspace W = dac_decode_workspace(c, B, T);
   const char* bl = (const char*)blob;
+  WalkRows rows{frame_lengths, T, win, win != nullptr ? window_margins(c) : std::vector<Margin>{}};
   FromCodesArgs fz{codes, bl + L.codebooks, bl + L.proj_w, bl + L.proj_b, W.buf(ws, 3), c.n_codebooks, c.codebook_dim, c.latent_dim, T,
                    c.codebook_size, frame_lengths};
+  if (win != nullptr) {
+    fz.frame_start = win->frame_start; fz.emit_lo = win->emit_lo; fz.emit_hi = win->emit_hi;
+    fz.codes_T = win->codes_T; fz.m_lo = rows.m[0].lo; fz.m_hi = rows.m[0].hi;
+  }
   if (int e = launch_from_codes(fz, c.dtype, B, st)) return e;
   bool tc = allow_tc && c.dtype == PTTS_BF16 && conv_tc_supported(c.latent_dim, c.decoder_dim);
   for (int bi = 0; bi < c.n_blocks && tc; bi++) {
     const int cin = c.decoder_dim >> bi, cout = c.decoder_dim >> (bi + 1);
     tc = conv_tc_supported(cin, cout) && conv_tc_supported(cout, cout);
   }
-  return (tc ? decode_tc : decode_generic)(c, L, bl, W, ws, B, T, frame_lengths, audio, st);
+  return (tc ? decode_tc : decode_generic)(c, L, bl, W, ws, B, T, rows, audio, st);
+}
+
+int dac_decode(const ptts_dac_config& c, const void* blob, void* ws, const int64_t* codes, int B, int T, const int32_t* frame_lengths,
+               void* audio, bool allow_tc, cudaStream_t st) {
+  return decode_walk(c, blob, ws, codes, B, T, frame_lengths, nullptr, audio, allow_tc, st);
+}
+
+int dac_decode_window(const ptts_dac_config& c, const void* blob, void* ws, const int64_t* codes, int B, int T, const int32_t* frame_lengths,
+                      const DacWindow& win, void* audio, bool allow_tc, cudaStream_t st) {
+  return decode_walk(c, blob, ws, codes, B, T, frame_lengths, &win, audio, allow_tc, st);
 }
 
 }  // namespace ptts

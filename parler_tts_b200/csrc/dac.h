@@ -43,10 +43,14 @@ static inline ConvArgs conv_super_rows(int C, int Cout, int T, int s) { return c
 //   hop == 0 (decode): n_b = frame_lengths[b], clamped to [0, frames];
 //   hop > 0 (encode):  frame_lengths[b] counts waveform samples, clamped to [1, frames * hop]; n_b = ceil(samples / hop).
 // frame_lengths == nullptr: every row is full (equal lengths).
+// Windowed decode (emit_lo != nullptr, hop == 0): the conv computes only the output rows [lo_b * up_out - m_lo, hi_b * up_out + m_hi)
+// of row b, the rows the samples of frames [lo_b, hi_b) depend on through the layers after it (needed_rows).
 struct RowLengths {
   const int32_t* frame_lengths;
   int frames, up_in, up_out;
   int hop;
+  const int32_t* emit_lo; const int32_t* emit_hi;
+  int m_lo, m_hi;
 };
 int launch_conv(const ConvArgs& a, int dtype, int B, cudaStream_t st, const RowLengths& rl = RowLengths{});
 
@@ -65,6 +69,14 @@ __device__ __forceinline__ int row_frames(const int32_t* lengths, int b, int fra
   if constexpr (SAMPLES) return (row_samples(lengths, b, frames * hop) + hop - 1) / hop;
   else return row_frames(lengths, b, frames);
 }
+// The output rows [x, y) of row b (n frames) that a windowed decode needs from a layer with up_out rows per frame: the emit range
+// [lo_b, hi_b), clamped to [0, n], widened by the layer's margins.  Rows past n * up_out in it are the zero padding later layers
+// read.  An empty emit range needs nothing (x == y).
+__device__ __forceinline__ int2 needed_rows(const int32_t* emit_lo, const int32_t* emit_hi, int b, int n, int up_out, int m_lo, int m_hi) {
+  const int lo = min(max(__ldg(emit_lo + b), 0), n), hi = min(max(__ldg(emit_hi + b), lo), n);
+  if (lo == hi) return make_int2(0, 0);
+  return make_int2(lo * up_out - m_lo, hi * up_out + m_hi);
+}
 
 struct FromCodesArgs {
   const int64_t* codes;  // [B][K][T]
@@ -72,6 +84,10 @@ struct FromCodesArgs {
   void* z;               // [B][T][C]
   int K, D, C, T, codebook_size;
   const int32_t* frame_lengths;  // [B] or nullptr: frames at or past row b's length are zero latents and read no code
+  // windowed decode (emit_lo != nullptr): codes are [B][K][codes_T] and latent frame t of row b is code frame frame_start[b] + t;
+  // only the frames of needed_rows(m_lo, m_hi) are written
+  const int32_t* frame_start; const int32_t* emit_lo; const int32_t* emit_hi;
+  int codes_T, m_lo, m_hi;
 };
 int launch_from_codes(const FromCodesArgs& a, int dtype, int B, cudaStream_t st);
 int pack_conv(const void* src, int src_dtype, void* dst, int dst_dtype, int d0, int d1, int k, int transposed, cudaStream_t st);
@@ -82,9 +98,10 @@ int launch_conv_tc(const ConvArgs& a, const void* w_kmajor, int taps_total, cons
 int pack_conv_kmajor(const void* src, int src_dtype, void* dst, int d0, int d1, int k, int transposed, cudaStream_t st);
 // output convolution (C -> 1, k = 7) + tanh on the already snake'd channels-last tensor, bf16 (dac.cu)
 bool final_conv_supported(int C);
-// frame_lengths (nullptr: none) as in RowLengths, `frames` code frames of T / frames samples each: samples past a row's end are 0
+// frame_lengths (nullptr: none) as in RowLengths, `frames` code frames of T / frames samples each: samples past a row's end are 0.
+// emit_lo / emit_hi (nullptr: none): a windowed decode, samples outside the emit frames [lo_b, hi_b) are 0.
 int launch_final_conv_tanh(const void* x, const void* w, const void* bias, void* out, int C, int T, int B, const int32_t* frame_lengths,
-                           int frames, cudaStream_t st);
+                           int frames, cudaStream_t st, const int32_t* emit_lo = nullptr, const int32_t* emit_hi = nullptr);
 
 enum { DK_PLAIN = 0, DK_CONV = 1, DK_CONVT = 2 };
 struct DacTensor {
@@ -312,6 +329,15 @@ static inline DacWorkspace dac_encode_workspace(const ptts_dac_config& c, int B,
 // is bf16 and conv_tc_supported takes every width; the generic conv_kernel path otherwise.
 int dac_decode(const ptts_dac_config& c, const void* blob, void* ws, const int64_t* codes, int B, int T, const int32_t* frame_lengths,
                void* audio, bool allow_tc, cudaStream_t st);
+// Windowed decode (ptts_dac_decode3): row b decodes code frames [frame_start[b], + frame_lengths[b]) of codes [B][K][codes_T] as
+// dac_decode decodes them alone at frame 0, and keeps the samples of frames [emit_lo[b], emit_hi[b]) (the rest are 0).  Each
+// layer computes only the rows those samples depend on (window_margins in dac.cu).
+struct DacWindow {
+  const int32_t* frame_start; const int32_t* emit_lo; const int32_t* emit_hi;
+  int codes_T;
+};
+int dac_decode_window(const ptts_dac_config& c, const void* blob, void* ws, const int64_t* codes, int B, int T, const int32_t* frame_lengths,
+                      const DacWindow& win, void* audio, bool allow_tc, cudaStream_t st);
 // waveform [B][samples] -> codes [B][n_q][T] and, when latents != nullptr, the encoder output [B][T][latent_dim] (dac_enc.cu).
 // sample_lengths (device [B], or nullptr: every row has `samples`): a ragged encode whose row b equals the encode of its first
 // sample_lengths[b] samples alone in its first ceil(sample_lengths[b] / hop) frames; later frames hold codebook_size and zero

@@ -16,6 +16,7 @@
 //     rounded like torch's bf16 ops).
 // ConvTranspose1d(k = 2s, stride s) = s output phases x 2 taps (dac.cu explains the mapping).
 #include <algorithm>
+#include <type_traits>
 #include <mutex>
 #include <vector>
 
@@ -40,10 +41,19 @@ struct ConvTcArgs {
   const int32_t* frame_lengths;  // ragged batch (RowLengths in dac.h); nullptr: every row is full
   int frames, up_in, up_out, hop;
 };
+// A windowed decode's launch (RowLengths in dac.h).  A type of its own, so that the other instantiations keep their arguments.
+struct ConvTcWindowArgs : ConvTcArgs {
+  const int32_t* emit_lo; const int32_t* emit_hi;
+  int m_lo, m_hi;
+};
 
-template <int NT, bool SAMPLES>   // SAMPLES: a ragged encode's lengths (RowLengths, hop > 0)
+// SAMPLES: a ragged encode's lengths (RowLengths, hop > 0).  Args = ConvTcWindowArgs: a windowed decode, whose tiles without a
+// row of needed_rows exit before any load.  The rows a kept tile computes outside needed_rows may read stale workspace rows:
+// no needed row reads them.
+template <int NT, bool SAMPLES, typename Args = ConvTcArgs>
 __global__ void __launch_bounds__(wg::THREADS, 2)
-conv_tc_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_w, const ConvTcArgs p) {
+conv_tc_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_w, const Args p) {
+  constexpr bool WINDOW = std::is_same_v<Args, ConvTcWindowArgs>;
   extern __shared__ unsigned char smem_raw[];
   const wg::Pipe pipe = wg::pipe_setup<NT>(smem_raw);
   bf16* chan = reinterpret_cast<bf16*>(pipe.extra);  // [3][NT]: bias | alpha | 1/(alpha+1e-9)
@@ -60,6 +70,11 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant_
     const int q_end = p.q_count - p.Tin + row_frames<SAMPLES>(p.frame_lengths, b, p.frames, p.hop) * p.up_in;
     if ((int)blockIdx.x > q_end / TC_M + 1) return;
     if (q0 >= q_end) n_iter = 0;
+  }
+  if constexpr (WINDOW) {
+    const int2 need = needed_rows(p.emit_lo, p.emit_hi, b, row_frames(p.frame_lengths, b, p.frames), p.up_out, p.m_lo, p.m_hi);
+    const int to0 = q0 * p.o_mul + p.o_add + phase * p.o_phase_step;
+    if (to0 + (TC_M - 1) * p.o_mul < need.x || to0 >= need.y) return;
   }
 
   if (threadIdx.x == 0) {
@@ -188,34 +203,42 @@ int conv_tc_ntile(int Cout) {
   return 32;
 }
 
-template <int NT, bool SAMPLES>
-static int launch_conv_tile_t(const CUtensorMap& mx, const CUtensorMap& mw, const ConvTcArgs& p, int B, cudaStream_t st) {
+template <int NT, bool SAMPLES, typename Args>
+static int launch_conv_tile_t(const CUtensorMap& mx, const CUtensorMap& mw, const Args& p, int B, cudaStream_t st) {
   const size_t smem = wg::smem_bytes<NT>(3 * NT * (int)sizeof(bf16));
   static bool attr = false;
   if (!attr) {
-    PTTS_CHECK_CUDA(cudaFuncSetAttribute(conv_tc_kernel<NT, SAMPLES>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    PTTS_CHECK_CUDA(cudaFuncSetAttribute(conv_tc_kernel<NT, SAMPLES, Args>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     attr = true;
   }
   dim3 grid((p.q_count + TC_M - 1) / TC_M, p.Cout / NT, B * p.n_phase);
-  conv_tc_kernel<NT, SAMPLES><<<grid, wg::THREADS, smem, st>>>(mx, mw, p);
+  conv_tc_kernel<NT, SAMPLES, Args><<<grid, wg::THREADS, smem, st>>>(mx, mw, p);
   PTTS_LAUNCH_CHECK();
   return PTTS_OK;
 }
 template <int NT>
-static int launch_conv_tile(const CUtensorMap& mx, const CUtensorMap& mw, const ConvTcArgs& p, int B, cudaStream_t st) {
-  return p.frame_lengths != nullptr && p.hop > 0 ? launch_conv_tile_t<NT, true>(mx, mw, p, B, st) : launch_conv_tile_t<NT, false>(mx, mw, p, B, st);
+static int launch_conv_tile(const CUtensorMap& mx, const CUtensorMap& mw, const ConvTcWindowArgs& p, int B, cudaStream_t st) {
+  if (p.emit_lo != nullptr) return launch_conv_tile_t<NT, false>(mx, mw, p, B, st);
+  const ConvTcArgs& q = p;
+  return p.frame_lengths != nullptr && p.hop > 0 ? launch_conv_tile_t<NT, true>(mx, mw, q, B, st) : launch_conv_tile_t<NT, false>(mx, mw, q, B, st);
 }
 
 // x: [B][Tin][Cin] bf16, w: [taps_total][Cout][Cin] bf16
 int launch_conv_tc(const ConvArgs& a, const void* w_kmajor, int taps_total, const void* alpha_next, void* out_raw, void* out_act, int B, cudaStream_t st,
                    const RowLengths& rl) {
-  ConvTcArgs p{};
+  ConvTcWindowArgs p{};
   p.Cin = a.Cin; p.Cout = a.Cout; p.Tin = a.Tin; p.Tout = a.Tout; p.q_count = a.q_count;
   p.n_taps = a.n_taps; p.off_base = a.off_base; p.off_step = a.off_step; p.wt_base = a.wt_base; p.wt_step = a.wt_step;
   p.n_phase = a.n_phase; p.wt_phase_step = a.wt_phase_step; p.o_mul = a.o_mul; p.o_add = a.o_add; p.o_phase_step = a.o_phase_step;
   const int n_tile = conv_tc_ntile(a.Cout);
   p.bias = (const bf16*)a.bias; p.res = (const bf16*)a.res; p.out_raw = (bf16*)out_raw; p.out_act = (bf16*)out_act; p.alpha_next = (const bf16*)alpha_next;
   p.frame_lengths = rl.frame_lengths; p.frames = rl.frames; p.up_in = rl.up_in; p.up_out = rl.up_out; p.hop = rl.hop;
+  p.emit_lo = rl.emit_lo; p.emit_hi = rl.emit_hi; p.m_lo = rl.m_lo; p.m_hi = rl.m_hi;
+  if (rl.emit_lo != nullptr) {
+    // needed rows past a row's end lie in the zero band the producer warps write (more than TC_M rows): the margin must not pass it
+    PTTS_REQUIRE(rl.frame_lengths != nullptr && rl.hop == 0 && rl.emit_hi != nullptr, "conv_tc: a windowed decode needs frame lengths");
+    PTTS_REQUIRE(rl.m_hi <= TC_M, "conv_tc: window margin %d rows is wider than the %d-row zero band", rl.m_hi, TC_M);
+  }
   if (rl.frame_lengths != nullptr) {
     // a kept output reads this far past its row's end: the highest tap offset, plus the row the transposed conv's extra q reads.
     // The producer of x wrote zeros over more than TC_M positions past the end (for the encoder's super-row convs, more than

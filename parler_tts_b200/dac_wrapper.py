@@ -420,5 +420,25 @@ class DACModel:
             return (audio,)
         return DACDecoderOutput(audio)
 
+    def _decode_windows(self, codes: torch.Tensor, windows: list) -> torch.Tensor:
+        """Streamed decode of one window per row: codes [B, K, T_codes] int64 (CUDA, contiguous), windows [(start, n, lo, hi)] * B.
+        Row b's samples of window frames [lo, hi) equal, bit for bit, those of decode() on codes[b, :, start:start + n] alone;
+        the rest of the row is 0.  Returns a fresh [B, hop * max n] tensor.  Each layer computes only the rows those samples
+        depend on (ptts_dac_decode3).  No range check (it would wait for the device): the ids inside the windows must be
+        codebook ids."""
+        B, _, T_codes = codes.shape
+        T = max(w[1] for w in windows)
+        lib = _lib.lib()
+        need = C.c_int64()
+        _lib.check(lib.ptts_dac_workspace_bytes(C.byref(self._c), B, T, C.byref(need)))
+        if self._ws is None or self._ws.numel() < need.value:
+            self._ws = torch.empty(need.value, dtype=torch.uint8, device=self.device)
+        ranges = torch.tensor(windows, dtype=torch.int32).t().contiguous().pin_memory().to(self.device, non_blocking=True)   # [4, B]
+        audio = torch.empty(B, T * self.hop_length, dtype=self.dtype, device=self.device)
+        _lib.check(lib.ptts_dac_decode3(C.byref(self._c), _lib.ptr(self.blob), _lib.ptr(self._ws), self._ws.numel(), _lib.ptr(codes), B,
+                                        T_codes, T, _lib.ptr(ranges[0]), _lib.ptr(ranges[1]), _lib.ptr(ranges[2]), _lib.ptr(ranges[3]),
+                                        _lib.ptr(audio), _lib.stream_ptr()))
+        return audio
+
     def forward(self, tensor):
         raise ValueError("`DACModel.forward` not implemented yet")

@@ -23,6 +23,7 @@ import torch
 from . import _lib
 from .configuration import DACConfig, GenerationConfig, ParlerTTSConfig, ParlerTTSDecoderConfig
 from .dac_wrapper import DACModel
+from .incremental import dac_dependency_radius
 
 _ACT = {"gelu": 0, "relu": 1, "silu": 2, "swish": 2, "gelu_new": 3, "gelu_pytorch_tanh": 3}
 
@@ -255,19 +256,27 @@ def check_continuous_generate(gc, mk: dict, streamer=None, logits_processor=None
         raise ValueError(f"generate_continuous() does not support {', '.join(bad)}")
 
 
-def slot_outputs(raw: torch.Tensor, eos_last: torch.Tensor, cur_len, shift: torch.Tensor, max_length: int, codebook_size: int):
+def slot_outputs(raw: torch.Tensor, eos_last: torch.Tensor, cur_len, shift: torch.Tensor, max_length: int, codebook_size: int,
+                 live: bool = False):
     """Every slot's state at a refill boundary, on the device (nothing here waits for it).  raw [B, K, ld] the history, eos_last [B]
     = 1 + the column of the last codebook's first EOS (0: none; a row stopped by max_length records the PAD it writes after, when
     pad == eos: hence the clamp), cur_len and shift [B] the slot columns.  Returns (finished [B], frames F [B], codes [B, K,
     max_length] with the F de-delayed frames first, the same with the valid frames compacted to the front as codes_to_waveform
     does, and their count [B]).  A request that ended with n history columns gets generate()'s cut (_codes_from_raw over its own columns): frame f
-    of codebook k is column f + k + 1, F = n - K, once n reaches the delay pattern's 2K - 1 columns; below that every column, F = n."""
+    of codebook k is column f + k + 1, F = n - K, once n reaches the delay pattern's 2K - 1 columns; below that every column, F = n.
+    live: an unfinished slot with col = cur_len - shift columns also gets its complete frames, F = col - K (the last codebook of
+    frame f is column f + K), and none while col < 2K - 1, where the row may still end under the cut without the pattern.  Its
+    compacted frames are then a prefix of those its finished cut will hold (the compaction keeps the frame order)."""
     B, K, ld = raw.shape
     L = int(max_length)
     finished = (eos_last > 0) | (cur_len - shift >= L)
     n = torch.where(eos_last > 0, eos_last.clamp(max=L), torch.full_like(eos_last, L))
     pattern = n >= 2 * K - 1
     frames = torch.where(pattern, n - K, n)
+    if live:
+        col = cur_len - shift
+        pattern = pattern | ~finished
+        frames = torch.where(finished, frames, torch.where(col >= 2 * K - 1, col - K, torch.zeros_like(col)).to(frames.dtype))
     f = torch.arange(L, device=raw.device)
     off = pattern[:, None].long() * torch.arange(1, K + 1, device=raw.device)[None, :]
     codes = torch.gather(raw, 2, (f[None, None, :] + off[:, :, None]).clamp(max=ld - 1))
@@ -275,6 +284,25 @@ def slot_outputs(raw: torch.Tensor, eos_last: torch.Tensor, cur_len, shift: torc
     order = torch.sort((~valid).to(torch.uint8), dim=1, stable=True).indices
     packed = torch.gather(codes, 2, order[:, None, :].expand_as(codes))
     return finished, frames, codes, packed, valid.sum(dim=1)
+
+
+def stream_windows(n_valid: list, emitted: list, finishing: list, radius: int) -> list[tuple[int, int, int, int]]:
+    """A streamed boundary's codec windows, one (start, n, lo, hi) per slot: decode valid frames [start, start + n) and emit the
+    samples of window frames [lo, hi), i.e. of frames [start + lo, start + hi).  n_valid: each slot's valid frames so far,
+    emitted: the frames already played (None: no request in the slot), finishing: the slot's request ends at this boundary.
+    Frame f's samples depend on frames [f - radius, f + radius] (incremental.dac_dependency_radius), so a live slot emits up
+    to n_valid - radius, once that passes `emitted`, from a window that starts radius frames before `emitted` (or at frame 0).
+    A finishing slot emits up to n_valid: its end is the true end, which the decode's zero padding stands for.  Every other slot
+    gets n = 0."""
+    out = []
+    for n, e, fin in zip(n_valid, emitted, finishing):
+        upto = n if fin else n - radius
+        if e is None or not (fin or upto > e):
+            out.append((0, 0, 0, 0))
+            continue
+        start = max(0, e - radius)
+        out.append((start, n - start, e - start, upto - start))
+    return out
 
 
 def refill_rows(t: Optional[torch.Tensor], first: int, count: int, rows: int) -> Optional[torch.Tensor]:
@@ -297,7 +325,8 @@ def rebase_slots(cur_len: int, cols: list) -> tuple[int, list[int]]:
 
 
 class ContinuousRun:
-    """generate_continuous()'s iterator of (request index, waveform[, codes]) in completion order.  `refills` logs every request
+    """generate_continuous()'s iterator of (request index, waveform[, codes]) in completion order, or with stream=True of
+    (request index, chunk, final[, codes]) events.  `refills` logs every request
     put into a slot at a boundary as (slot, request, batch column of that boundary); `boundaries` and `steps` count the
     boundaries and the decode steps enqueued."""
 
@@ -2247,7 +2276,7 @@ class ParlerTTSForConditionalGeneration:
     @torch.no_grad()
     def generate_continuous(self, input_ids=None, attention_mask=None, prompt_input_ids=None, prompt_attention_mask=None,
                             batch_size: int = 32, refill_every: int = 16, seed=0, return_codes: bool = False, streamer=None,
-                            logits_processor=None, stopping_criteria=None, **kwargs) -> ContinuousRun:
+                            logits_processor=None, stopping_criteria=None, stream: bool = False, **kwargs) -> ContinuousRun:
         """Generate N requests through `batch_size` slots of one live session, refilling a finished request's slot with the next
         request while the others keep decoding.  Returns a ContinuousRun that yields (request index, waveform) as requests finish,
         (request index, waveform, codes [K, T_i]) with return_codes=True.
@@ -2270,8 +2299,20 @@ class ParlerTTSForConditionalGeneration:
         is enqueued, and the finished requests' valid frames go through one ragged codec call behind it (the codec's range check
         waits for that interval, which the next boundary waits for anyway).  Finished rows keep
         decoding PAD until their boundary, so the live session holds max_length + refill_every columns.  Raises ValueError for what
-        check_continuous_generate lists."""
+        check_continuous_generate lists.
+
+        stream=True yields each request's audio while it is generated: events (request index, chunk, final), or (request index,
+        chunk, final, codes) with return_codes=True, where codes is the [K, T_i] tensor on the final event and None before it.
+        Chunks are 1-D device tensors in the model dtype; a request's chunks, in the order yielded, concatenate to the waveform
+        stream=False yields for it, bit for bit, and its one final event is its last.  At every boundary each slot's complete
+        valid frames so far (slot_outputs(live=True)) give a codec window (stream_windows): the frames whose samples no later
+        frame can change are emitted, the rest wait for their right context; a request that ends emits its remainder.  The
+        windows of all slots go through one windowed codec call (DACModel._decode_windows), enqueued before the refill and the
+        next interval, and the events are yielded in slot order.  A request's first chunk comes at the first boundary that has
+        more than dac_dependency_radius (10 for the 44.1 kHz codec) valid frames of it."""
         import copy
+        if not isinstance(stream, bool):
+            raise ValueError(f"stream must be a bool, got {stream!r}")
         if isinstance(batch_size, bool) or not isinstance(batch_size, int) or batch_size < 1:
             raise ValueError(f"batch_size must be a positive int, got {batch_size!r}")
         if isinstance(refill_every, bool) or not isinstance(refill_every, int) or refill_every < 1:
@@ -2302,11 +2343,11 @@ class ParlerTTSForConditionalGeneration:
         sampling = self._sampling(gc, 1, max_length, seed, suppress_special)
         run = ContinuousRun()
         run._it = self._continuous_loop(run, enc_hidden, enc_mask, prompt_hidden, prompt_mask, sampling, batch_size, refill_every,
-                                        bool(return_codes))
+                                        bool(return_codes), stream)
         return run
 
     def _continuous_loop(self, run: ContinuousRun, enc_hidden, enc_mask, prompt_hidden, prompt_mask, s: Sampling, batch_size: int,
-                         refill_every: int, return_codes: bool):
+                         refill_every: int, return_codes: bool, stream: bool):
         d = self.config.decoder
         K, eng, cs = d.num_codebooks, self.decoder.engine, self.config.audio_encoder.codebook_size
         N, S = enc_hidden.shape[0], enc_hidden.shape[1]
@@ -2329,6 +2370,8 @@ class ParlerTTSForConditionalGeneration:
         slot_req: list = list(range(Bl))
         nxt, cur_len = Bl, 2
         shift = [0] * Bl
+        emitted = [0] * Bl   # stream: valid frames of each slot's request already played
+        radius = dac_dependency_radius(self.audio_encoder.config.decoder_rates)
         live.set_slots(cur_len, shift, slot_req)
         live.decode_steps(refill_every)
         run.steps += refill_every
@@ -2337,11 +2380,13 @@ class ParlerTTSForConditionalGeneration:
             # every slot's outcome is computed on the device, then read in the boundary's one host sync
             shift_dev = torch.tensor(shift, dtype=torch.int32).pin_memory().to(self.device, non_blocking=True)
             fin, frames, codes, packed, n_valid = slot_outputs(live.raw_ids.view(Bl, K, -1), live.eos_seen.view(Bl, K)[:, K - 1],
-                                                               live.state[0], shift_dev, s.max_length, cs)
+                                                               live.state[0], shift_dev, s.max_length, cs, live=stream)
             status = torch.cat([live.state[:1].long(), fin.long(), frames.long(), n_valid.long()]).cpu().tolist()
             cur_len = status[0]
             fin, frames, n_valid = status[1:1 + Bl], status[1 + Bl:1 + 2 * Bl], status[1 + 2 * Bl:]
             cols = [cur_len - sh for sh in shift]
+            if stream:   # the codec call goes ahead of the refill and the next interval: the chunks are ready one call after the sync
+                events = self._stream_events(packed, codes, slot_req, fin, frames, n_valid, emitted, radius, return_codes)
             done = [b for b, r in enumerate(slot_req) if r is not None and fin[b]]
             done_req = [slot_req[b] for b in done]
             for b in done:
@@ -2352,7 +2397,7 @@ class ParlerTTSForConditionalGeneration:
                 start(fill, nxt, g, nxt * K)
                 live.import_rows(fill, list(range(g)), free[:g])
                 for j, b in enumerate(free[:g]):
-                    slot_req[b], cols[b] = nxt + j, 2
+                    slot_req[b], cols[b], emitted[b] = nxt + j, 2, 0
                     run.refills.append((b, nxt + j, cur_len))
                 nxt += g
             last = all(r is None for r in slot_req)
@@ -2361,7 +2406,9 @@ class ParlerTTSForConditionalGeneration:
                 live.set_slots(cur_len, shift, [0 if r is None else r for r in slot_req])
                 live.decode_steps(refill_every)   # enqueued before the finished requests' codec call and the caller's turn
                 run.steps += refill_every
-            if done:
+            if stream:
+                yield from events
+            elif done:
                 # the codes were cut before any import overwrote their slots; the codec call queues behind the next interval
                 audio, lengths = packed_to_waveform(self.audio_encoder, torch.stack([packed[b] for b in done]),
                                                     [n_valid[b] for b in done], self.dtype)
@@ -2370,3 +2417,28 @@ class ParlerTTSForConditionalGeneration:
                     yield (r, wav, codes[b, :, :frames[b]]) if return_codes else (r, wav)
             if last:
                 return
+
+    def _stream_events(self, packed, codes, slot_req, fin, frames, n_valid, emitted, radius, return_codes):
+        """One streamed boundary: every slot's window through one windowed codec call (enqueued here, waited for by nobody), and
+        the events to yield, in slot order.  Advances `emitted`."""
+        wins = stream_windows(n_valid, [e if r is not None else None for e, r in zip(emitted, slot_req)],
+                              [r is not None and bool(f) for r, f in zip(slot_req, fin)], radius)
+        # a fresh buffer per boundary: the chunks yielded are views into it
+        audio = self.audio_encoder._decode_windows(packed, wins) if any(w[1] > 0 for w in wins) else None
+        hop, events = self.audio_encoder.hop_length, []
+        for b, (r, (start, n, lo, hi)) in enumerate(zip(slot_req, wins)):
+            final = r is not None and bool(fin[b])
+            if r is None or not (final or hi > lo):
+                continue
+            if final and n_valid[b] == 0:      # no valid frame: the [1] zero waveform, as stream=False gives
+                chunk = torch.zeros(1, device=self.device, dtype=self.dtype)
+            elif hi > lo:
+                chunk = audio[b, lo * hop:hi * hop]
+                emitted[b] = start + hi
+            else:
+                chunk = torch.zeros(0, device=self.device, dtype=self.dtype)
+            if return_codes:
+                events.append((r, chunk, final, codes[b, :, :frames[b]] if final else None))
+            else:
+                events.append((r, chunk, final))
+        return events
