@@ -357,8 +357,18 @@ int ptts_session_import_rows(ptts_session* dst, const ptts_session* src, const i
  * the BOS column, no probe, alignment or per-step output window, and none of forced_eos_token_id, the decay penalty or
  * begin_suppress_tokens (they count from one batch column); every token then takes the split path's EXT sampler.  The caller
  * runs at most raw_ld - max(col_b) steps before the next call (ptts_session_raw_ids gives raw_ld), and keeps each row's
- * cur_len parity where it was when it imported rows.  Slot mode lasts until the next ptts_generate_begin*. */
+ * cur_len parity where it was when it imported rows.  Slot mode lasts until the next ptts_generate_begin*.
+ * Same as ptts_generate_set_slots2 with row_max_length NULL. */
 int ptts_generate_set_slots(ptts_session* s, int32_t cur_len, const int32_t* row_shift, const int32_t* row_key, void* stream);
+
+/* ptts_generate_set_slots with a length limit per row: row b stops at col_b + 1 >= row_max_length[b] (or its EOS) and takes the
+ * delay pattern of row_max_length[b] in its own column, what a generate() call with max_length = row_max_length[b] gives it.
+ * row_max_length: host int32 [B], passed by value like the others, each in [max(2K - 1, 2), the generation's max_length]
+ * (PTTS_EINVAL otherwise); NULL gives every row the generation's max_length.  The lower bound keeps a request's first column,
+ * drawn before slot mode under the generation's max_length (ptts_sample of the session it is imported from), the one its own
+ * limit gives: both limits are then on the same side of the delay pattern's 2K - 1 gate, and neither stops or pads column 1. */
+int ptts_generate_set_slots2(ptts_session* s, int32_t cur_len, const int32_t* row_shift, const int32_t* row_key,
+                             const int32_t* row_max_length, void* stream);
 
 /* Device pointers into the workspace (valid for the session lifetime). */
 int ptts_session_logits(ptts_session* s, float** out);          /* [B*K, V] f32, last step's raw logits */

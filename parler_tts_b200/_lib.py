@@ -92,6 +92,7 @@ _SIGS = {
     "ptts_decode_steps": (C.c_int, [_VP, _I32, _VP]),
     "ptts_session_import_rows": (C.c_int, [_VP, _VP, C.POINTER(_I32), C.POINTER(_I32), _I32, _VP]),
     "ptts_generate_set_slots": (C.c_int, [_VP, _I32, C.POINTER(_I32), C.POINTER(_I32), _VP]),
+    "ptts_generate_set_slots2": (C.c_int, [_VP, _I32, C.POINTER(_I32), C.POINTER(_I32), C.POINTER(_I32), _VP]),
     "ptts_session_logits": (C.c_int, [_VP, C.POINTER(_VP)]),
     "ptts_session_scores": (C.c_int, [_VP, C.POINTER(_VP)]),
     "ptts_session_raw_ids": (C.c_int, [_VP, C.POINTER(_VP), C.POINTER(_I32)]),

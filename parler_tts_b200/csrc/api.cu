@@ -124,6 +124,7 @@ static const ptts_sampling_ext* sampler_ext(const ptts_session* s) {
 }
 // slot mode's per-row Philox keys, or nullptr
 static const int* slot_keys(const ptts_session* s) { return s->slots ? (const int*)(s->ws + s->W.row_key) : nullptr; }
+static const int* slot_max_lens(const ptts_session* s) { return s->slots ? (const int*)(s->ws + s->W.row_max_len) : nullptr; }
 
 extern "C" {
 
@@ -814,7 +815,7 @@ int ptts_sample(ptts_session* s, const int64_t* forced_tokens, void* stream) {
   s->launches++;
   s->sampled++;
   return launch_sample(sample_args(s), forced_tokens, (cudaStream_t)stream, false, sampler_ext(s), active_out(s), active_lext(s),
-                       slot_keys(s));
+                       slot_keys(s), slot_max_lens(s));
 }
 
 int ptts_decode_steps(ptts_session* s, int32_t n_steps, void* stream) {
@@ -834,7 +835,7 @@ int ptts_decode_steps(ptts_session* s, int32_t n_steps, void* stream) {
     for (int i = 0; i < n_steps; i++) {
       const int e = path == DECODE_CLUSTER ? launch_decode_step_cluster(p, st) : launch_decode_step(p, s->sm_count, st);
       if (e) return e;
-      if (int e2 = launch_sample(sample_args(s), nullptr, st, false, ext, out, lext, slot_keys(s))) return e2;
+      if (int e2 = launch_sample(sample_args(s), nullptr, st, false, ext, out, lext, slot_keys(s), slot_max_lens(s))) return e2;
     }
     s->launches += 2 * (int64_t)n_steps;
     return PTTS_OK;
@@ -866,7 +867,7 @@ int ptts_decode_steps(ptts_session* s, int32_t n_steps, void* stream) {
     const int64_t before = s->launches;
     PTTS_CHECK_CUDA(cudaStreamBeginCapture(s->cap_stream, cudaStreamCaptureModeThreadLocal));
     int e = run_forward(s, s->cap_stream, false, nullptr, nullptr);
-    if (!e) { s->launches++; e = launch_sample(sample_args(s), nullptr, s->cap_stream, true, ext, out, lext, slot_keys(s)); }
+    if (!e) { s->launches++; e = launch_sample(sample_args(s), nullptr, s->cap_stream, true, ext, out, lext, slot_keys(s), slot_max_lens(s)); }
     cudaGraph_t graph = nullptr;
     cudaError_t ce = cudaStreamEndCapture(s->cap_stream, &graph);
     s->graph_launches = s->launches - before;   // embed + 8 kernels per layer + heads + sample (+ the probe kernels)
@@ -926,6 +927,11 @@ int ptts_session_import_rows(ptts_session* dst, const ptts_session* src, const i
 }
 
 int ptts_generate_set_slots(ptts_session* s, int32_t cur_len, const int32_t* row_shift, const int32_t* row_key, void* stream) {
+  return ptts_generate_set_slots2(s, cur_len, row_shift, row_key, nullptr, stream);
+}
+
+int ptts_generate_set_slots2(ptts_session* s, int32_t cur_len, const int32_t* row_shift, const int32_t* row_key,
+                             const int32_t* row_max_length, void* stream) {
   PTTS_REQUIRE(s && row_shift && row_key, "null argument");
   if (!s->prefilled) return fail(PTTS_ESTATE, "set_slots called before ptts_prefill");
   const WorkspaceLayout& W = s->W;
@@ -942,8 +948,18 @@ int ptts_generate_set_slots(ptts_session* s, int32_t cur_len, const int32_t* row
     PTTS_REQUIRE(row_shift[b] >= 0 && row_shift[b] < cur_len, "set_slots: row_shift[%d] = %d outside [0, cur_len = %d)", b, row_shift[b], cur_len);
     PTTS_REQUIRE(row_key[b] >= 0, "set_slots: row_key[%d] = %d is negative", b, row_key[b]);
   }
-  if (int e = launch_set_slots((Ctrl*)(s->ws + W.ctrl), cur_len, (int*)(s->ws + W.row_shift), (int*)(s->ws + W.row_key), row_shift, row_key,
-                               W.B, (cudaStream_t)stream)) return e;
+  // a row's first column was drawn under gen.max_length before slot mode: a limit of at least 2K - 1 (and 2) is on the same side
+  // of the delay pattern's gate and neither stops nor pads that column, so the row holds what its own limit gives it
+  const int lo = 2 * s->cfg.num_codebooks - 1 > 2 ? 2 * s->cfg.num_codebooks - 1 : 2, hi = s->gen.max_length;
+  std::vector<int32_t> lims(W.B, hi);
+  if (row_max_length != nullptr)
+    for (int b = 0; b < W.B; b++) {
+      PTTS_REQUIRE(row_max_length[b] >= lo && row_max_length[b] <= hi, "set_slots: row_max_length[%d] = %d outside [%d, max_length = %d]",
+                   b, row_max_length[b], lo, hi);
+      lims[b] = row_max_length[b];
+    }
+  if (int e = launch_set_slots((Ctrl*)(s->ws + W.ctrl), cur_len, (int*)(s->ws + W.row_shift), (int*)(s->ws + W.row_key),
+                               (int*)(s->ws + W.row_max_len), row_shift, row_key, lims.data(), W.B, (cudaStream_t)stream)) return e;
   s->launches += (W.B + kMaxSlotRows - 1) / kMaxSlotRows;
   if (!s->slots) {   // the decode kernels switch to their ragged instantiations (set up anew) and the sampler to slot mode
     s->ragged = s->slots = true;

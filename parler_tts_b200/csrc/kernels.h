@@ -144,9 +144,11 @@ struct SampleOut {
 // ext != nullptr: the sampler with the ptts_sampling_ext stages (the caller passes it while one is active, or all off while out is
 // set); out != nullptr (needs ext): that sampler also records the raw logits and the processed scores of the steps in its window
 // lext: the ptts_logits_ext stages (needs ext; nullptr = all off)
-// slot_key (needs ext and a.shift): slot mode (ptts_generate_set_slots), with the per-row Philox keys [B] on the device
+// slot_key (needs ext and a.shift): slot mode (ptts_generate_set_slots2), with the per-row Philox keys [B] and slot_max_len, the
+// per-row length limits [B], on the device
 int launch_sample(const SampleArgs& a, const int64_t* forced, cudaStream_t st, bool pdl, const ptts_sampling_ext* ext = nullptr,
-                  const SampleOut* out = nullptr, const ptts_logits_ext* lext = nullptr, const int* slot_key = nullptr);
+                  const SampleOut* out = nullptr, const ptts_logits_ext* lext = nullptr, const int* slot_key = nullptr,
+                  const int* slot_max_len = nullptr);
 // every ptts_logits_ext stage off
 constexpr ptts_logits_ext kLogitsExtOff = {nullptr, nullptr, nullptr, 0, -1, -1, 0, nullptr, 0, nullptr, nullptr, 1, 0};
 // the fused step kernels' sampling phase over n_ctas CTAs (passes of up to three rows per CTA), as a kernel of its own; no EXT
@@ -175,10 +177,11 @@ struct RowImportArgs {
   int src_row[kMaxImportRows], dst_row[kMaxImportRows];
 };
 int launch_import_rows(const RowImportArgs& a, int n_pairs, cudaStream_t st);
-// slot mode (ptts_generate_set_slots): the host arrays row_shift / row_key [B] into the workspace's shift / key, then the new cur_len,
-// active = 1 and the sampler's counters cleared
+// slot mode (ptts_generate_set_slots2): the host arrays row_shift / row_key / row_max_len [B] into the workspace's shift / key /
+// max_len, then the new cur_len, active = 1 and the sampler's counters cleared
 constexpr int kMaxSlotRows = 256;    // rows per launch
-int launch_set_slots(Ctrl* ctrl, int cur_len, int* shift, int* key, const int* row_shift, const int* row_key, int B, cudaStream_t st);
+int launch_set_slots(Ctrl* ctrl, int cur_len, int* shift, int* key, int* max_len, const int* row_shift, const int* row_key,
+                     const int* row_max_len, int B, cudaStream_t st);
 
 // ---- teacher-forced scoring (score.cu) ----------------------------------------------------------
 struct ScoreArgs {

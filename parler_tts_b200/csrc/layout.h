@@ -184,7 +184,8 @@ struct WorkspaceLayout {
   int64_t ctrl, progress, gen, raw_ids, cur_ids, eos_seen, unfinished, first_unf, prompt_mask, enc_mask;
   int64_t prefix_cells;            // [BK][K-1] int64: delay-pattern cells just past the input (max_input > 1 only; -1 = none)
   int64_t row_shift;               // [B] int32: per-row offsets of a ragged continuation (max_input > 1 only; -1 = none)
-  int64_t row_key;                 // [B] int32: slot mode's per-row Philox keys (ptts_generate_set_slots; with row_shift)
+  int64_t row_key;                 // [B] int32: slot mode's per-row Philox keys (ptts_generate_set_slots2; with row_shift)
+  int64_t row_max_len;             // [B] int32: slot mode's per-row length limits (ptts_generate_set_slots2; with row_shift)
   int64_t x, qkv, attn, qc, hbuf, hidden, logits, scores, cross_tmp, cross_kv, self_kv;
   int64_t img_x, img_attn, img_h;  // fused step kernel: activations as tile images [chunk][32][H + 8] (step.cu stage_tile)
   int64_t cl_x, cl_attn, cl_h;     // cluster step kernel: K-sliced images [2][32][H/2 + 8], fc2's in quarters [4][32][F/4 + 8] (step2.cu)
@@ -221,6 +222,7 @@ static inline WorkspaceLayout make_workspace(const ptts_decoder_config& c, int B
   if (max_input > 1 && c.num_codebooks > 1) w.prefix_cells = take((int64_t)w.BK * (c.num_codebooks - 1) * 8);
   w.row_shift = max_input > 1 ? take((int64_t)B * 4) : -1;
   w.row_key = max_input > 1 ? take((int64_t)B * 4) : -1;
+  w.row_max_len = max_input > 1 ? take((int64_t)B * 4) : -1;
   const int64_t rows_enc = (int64_t)B * S, rows_cross = (int64_t)(B / takes) * S;
   w.x = take((int64_t)w.Mmax * l.H * l.es);
   w.qkv = take((int64_t)w.Mmax * l.qkv_rows * l.es);

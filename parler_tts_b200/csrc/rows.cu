@@ -1,5 +1,5 @@
 // rows.cu -- moving batch rows between sessions (continuous batching): the per-row state of row_regions (layout.h) copied from
-// the rows of one session into slots of another, and the control-block rewrite of ptts_generate_set_slots.
+// the rows of one session into slots of another, and the control-block rewrite of ptts_generate_set_slots2.
 #include "common.cuh"
 #include "kernels.h"
 
@@ -43,12 +43,14 @@ int launch_import_rows(const RowImportArgs& a, int n_pairs, cudaStream_t st) {
 
 // the rows come by value (the host's arrays need no staging copy and no stream sync); the first launch also writes the control block
 struct SlotRows {
-  int* shift; int* key;   // the workspace's row_shift and row_key
+  int* shift; int* key; int* max_len;   // the workspace's row_shift, row_key and row_max_len
   int b0, n;
-  int v_shift[kMaxSlotRows], v_key[kMaxSlotRows];
+  int v_shift[kMaxSlotRows], v_key[kMaxSlotRows], v_max_len[kMaxSlotRows];
 };
 __global__ void set_slots_kernel(Ctrl* ctrl, int cur_len, SlotRows r) {
-  for (int i = threadIdx.x; i < r.n; i += blockDim.x) { r.shift[r.b0 + i] = r.v_shift[i]; r.key[r.b0 + i] = r.v_key[i]; }
+  for (int i = threadIdx.x; i < r.n; i += blockDim.x) {
+    r.shift[r.b0 + i] = r.v_shift[i]; r.key[r.b0 + i] = r.v_key[i]; r.max_len[r.b0 + i] = r.v_max_len[i];
+  }
   if (r.b0 == 0 && threadIdx.x == 0) {
     ctrl->cur_len = cur_len;
     ctrl->active = 1;
@@ -57,11 +59,12 @@ __global__ void set_slots_kernel(Ctrl* ctrl, int cur_len, SlotRows r) {
   }
 }
 
-int launch_set_slots(Ctrl* ctrl, int cur_len, int* shift, int* key, const int* row_shift, const int* row_key, int B, cudaStream_t st) {
+int launch_set_slots(Ctrl* ctrl, int cur_len, int* shift, int* key, int* max_len, const int* row_shift, const int* row_key,
+                     const int* row_max_len, int B, cudaStream_t st) {
   for (int b0 = 0; b0 < B; b0 += kMaxSlotRows) {
     SlotRows r{};
-    r.shift = shift; r.key = key; r.b0 = b0; r.n = B - b0 < kMaxSlotRows ? B - b0 : kMaxSlotRows;
-    for (int i = 0; i < r.n; i++) { r.v_shift[i] = row_shift[b0 + i]; r.v_key[i] = row_key[b0 + i]; }
+    r.shift = shift; r.key = key; r.max_len = max_len; r.b0 = b0; r.n = B - b0 < kMaxSlotRows ? B - b0 : kMaxSlotRows;
+    for (int i = 0; i < r.n; i++) { r.v_shift[i] = row_shift[b0 + i]; r.v_key[i] = row_key[b0 + i]; r.v_max_len[i] = row_max_len[b0 + i]; }
     set_slots_kernel<<<1, 256, 0, st>>>(ctrl, cur_len, r);
     PTTS_LAUNCH_CHECK();
   }

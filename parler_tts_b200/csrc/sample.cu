@@ -18,14 +18,15 @@ namespace ptts {
 
 template <int ITEMS, bool EXT, bool RAGGED, bool SLOT = false>
 __device__ __forceinline__ void sample_kernel_body(const SampleArgs& p, const int64_t* __restrict__ forced, const ptts_sampling_ext& x,
-                                                   const SampleOut& o, const ptts_logits_ext& lx, const int* key = nullptr) {
+                                                   const SampleOut& o, const ptts_logits_ext& lx, const int* key = nullptr,
+                                                   const int* max_len = nullptr) {
   pdl_launch_dependents();
   pdl_wait();
   if (p.ctrl->active == 0) return;
   const int row = blockIdx.x;           // one CTA per (utterance, codebook) row
   const int cur_len = p.ctrl->cur_len;  // the new token becomes column `cur_len`
   const ptts_gen_params g = *p.gen;
-  sample_rows_cta<ITEMS, 1, EXT, RAGGED, SLOT>(p, g, forced, row, 0, row + 1, cur_len, x, o, lx, key);
+  sample_rows_cta<ITEMS, 1, EXT, RAGGED, SLOT>(p, g, forced, row, 0, row + 1, cur_len, x, o, lx, key, max_len);
   // last block advances the control block
   __threadfence();
   __syncthreads();
@@ -57,15 +58,17 @@ __global__ void __launch_bounds__(SMP_THREADS) sample_kernel(SampleArgs p, const
   sample_kernel_body<ITEMS, EXT, RAGGED>(p, forced, x, o, lx);
 }
 
-// slot mode (ptts_generate_set_slots): the EXT sampler with each row's own column and Philox key (key [B], in the workspace)
+// slot mode (ptts_generate_set_slots2): the EXT sampler with each row's own column, Philox key and length limit (key and max_len
+// [B], in the workspace)
 template <int ITEMS>
 __global__ void __launch_bounds__(SMP_THREADS) sample_slot_kernel(SampleArgs p, const int64_t* __restrict__ forced, ptts_sampling_ext x,
-                                                                  SampleOut o, ptts_logits_ext lx, const int* __restrict__ key) {
-  sample_kernel_body<ITEMS, true, true, true>(p, forced, x, o, lx, key);
+                                                                  SampleOut o, ptts_logits_ext lx, const int* __restrict__ key,
+                                                                  const int* __restrict__ max_len) {
+  sample_kernel_body<ITEMS, true, true, true>(p, forced, x, o, lx, key, max_len);
 }
 
 int launch_sample(const SampleArgs& a, const int64_t* forced, cudaStream_t st, bool pdl, const ptts_sampling_ext* ext,
-                  const SampleOut* out, const ptts_logits_ext* lext, const int* slot_key) {
+                  const SampleOut* out, const ptts_logits_ext* lext, const int* slot_key, const int* slot_max_len) {
   const int BK = a.B * a.K;
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = dim3(BK);
@@ -80,13 +83,14 @@ int launch_sample(const SampleArgs& a, const int64_t* forced, cudaStream_t st, b
   PTTS_REQUIRE(items <= 9, "sample: vocab_size %d > 2304 not supported", a.V);
   PTTS_REQUIRE((out == nullptr && lext == nullptr) || ext != nullptr, "sample: the per-step outputs and the ptts_logits_ext stages need the EXT sampler");
   const bool rg = a.shift != nullptr;
-  PTTS_REQUIRE(slot_key == nullptr || (ext != nullptr && rg), "sample: slot mode needs the EXT sampler and per-row offsets");
+  PTTS_REQUIRE(slot_key == nullptr || (ext != nullptr && rg && slot_max_len != nullptr),
+               "sample: slot mode needs the EXT sampler, per-row offsets and per-row limits");
   if (ext != nullptr) {
     const SampleOut o = out ? *out : SampleOut{};
     const ptts_logits_ext lx = lext ? *lext : kLogitsExtOff;
     if (slot_key != nullptr) {
       auto fn = items <= 1 ? sample_slot_kernel<1> : items <= 5 ? sample_slot_kernel<5> : sample_slot_kernel<9>;
-      PTTS_CHECK_CUDA(cudaLaunchKernelEx(&cfg, fn, a, forced, *ext, o, lx, slot_key));
+      PTTS_CHECK_CUDA(cudaLaunchKernelEx(&cfg, fn, a, forced, *ext, o, lx, slot_key, slot_max_len));
       return PTTS_OK;
     }
     auto fn = items <= 1 ? (rg ? sample_kernel<1, true, true> : sample_kernel<1, true, false>)

@@ -77,11 +77,11 @@ __device__ __forceinline__ bool bitmap_has(const uint32_t* __restrict__ bits, in
 // which every row samples column cur_len (the callers pick the instantiation by p.shift != nullptr).
 // SLOT = true (with RAGGED and EXT; ptts_generate_set_slots) is slot mode: every row is a request of its own that started from
 // the BOS column at its own column 0, so its stop, MinNewTokens and delay pattern count in its column col = cur_len - shift[b]
-// and its draws use the Philox substream key[b] * K + k.
+// (stop and pattern at its own limit max_len[b], not max_length) and its draws use the Philox substream key[b] * K + k.
 template <int ITEMS, int R, bool EXT = false, bool RAGGED = false, bool SLOT = false>
 __device__ __forceinline__ void sample_rows_cta(const SampleArgs& p, const ptts_gen_params& g, const int64_t* __restrict__ forced,
                                                 int row0, int stride, int n_rows, int cur_len, ptts_sampling_ext x = {},
-                                                SampleOut o = {}, ptts_logits_ext lx = {}, const int* __restrict__ key = nullptr) {
+                                                SampleOut o = {}, ptts_logits_ext lx = {}, const int* __restrict__ key = nullptr, const int* __restrict__ max_len = nullptr) {
   static_assert(!SLOT || (RAGGED && EXT), "slot mode runs on the ragged EXT sampler");
   static_assert(R >= 1 && R <= SMP_MAX_ROWS, "rows per pass");
   SmpScratch& sc = smp_scratch();   // one static buffer for every instantiation inlined into a kernel
@@ -615,15 +615,15 @@ __device__ __forceinline__ void sample_rows_cta(const SampleArgs& p, const ptts_
     if (!t_unf) t = p.pad;  // next_tokens * unfinished + pad * (1 - unfinished)
     p.raw_ids[(size_t)my_row * p.raw_ld + my_col] = t;
     if (t == p.eos && t_es == 0) p.eos_seen[my_row] = my_col + 1;
-    // the row's own limit max_length - shift is reached at the batch's max_length; a slot's limit is max_length in its column
+    // the row's own limit max_length - shift is reached at the batch's max_length; a slot's limit is max_len[b] in its column
     const int new_len = (SLOT ? my_col : cur_len) + 1;
-    const int done = (t == p.eos) || (new_len >= g.max_length);
+    const int done = (t == p.eos) || (new_len >= (SLOT ? max_len[b] : g.max_length));
     const int still_unfinished = t_unf && !done;
     p.unfinished[my_row] = still_unfinished;
     // delay-pattern override of the NEXT model input (column `my_col`), build_delay_pattern_mask :252-261, with the row's own
     // limit Lb and input length nb
     const int sh = cur_len - my_col;
-    const int Lb = SLOT ? g.max_length : g.max_length - sh, nb = SLOT ? 1 : g.input_len - sh;
+    const int Lb = SLOT ? max_len[b] : g.max_length - sh, nb = SLOT ? 1 : g.input_len - sh;
     int nxt = t;
     if (Lb >= 2 * p.K - 1) {
       const bool is_bos = my_col <= k;

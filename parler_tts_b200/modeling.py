@@ -9,6 +9,7 @@ PyTorch is used for device memory, streams and the one-off side inputs the path 
 (text encoder, prompt embedding lookup: SURVEY.md section 1).
 """
 from __future__ import annotations
+import collections
 import contextlib
 import ctypes as C
 import functools
@@ -256,7 +257,44 @@ def check_continuous_generate(gc, mk: dict, streamer=None, logits_processor=None
         raise ValueError(f"generate_continuous() does not support {', '.join(bad)}")
 
 
-def slot_outputs(raw: torch.Tensor, eos_last: torch.Tensor, cur_len, shift: torch.Tensor, max_length: int, codebook_size: int,
+def check_continuous_counts(stream, batch_size, refill_every):
+    """generate_continuous()'s and continuous_engine()'s first checks, before anything touches the model."""
+    if not isinstance(stream, bool):
+        raise ValueError(f"stream must be a bool, got {stream!r}")
+    if isinstance(batch_size, bool) or not isinstance(batch_size, int) or batch_size < 1:
+        raise ValueError(f"batch_size must be a positive int, got {batch_size!r}")
+    if isinstance(refill_every, bool) or not isinstance(refill_every, int) or refill_every < 1:
+        raise ValueError(f"refill_every must be a positive int, got {refill_every!r}")
+
+
+def continuous_settings(model, kwargs: dict, streamer, logits_processor, stopping_criteria):
+    """generate_continuous()'s and continuous_engine()'s generation settings -> (config, model kwargs, max_length in each
+    request's own columns, suppress_special), with the device loop's and check_continuous_generate's rejections."""
+    import copy
+    gc = copy.deepcopy(model.generation_config)
+    suppress_special = kwargs.pop("_suppress_special", False)
+    user_max_length = kwargs.get("max_length")
+    mk = gc.update(**kwargs)
+    unknown = sorted(k for k in mk if k not in model._MODEL_KWARGS)
+    if unknown:
+        raise ValueError(f"The following `model_kwargs` are not used by the model: {unknown}")
+    unsupported = {k: getattr(gc, k) for k, neutral in model._NEUTRAL_GENERATION_KNOBS.items() if getattr(gc, k, neutral) != neutral}
+    if unsupported or gc.num_beams != 1:
+        raise ValueError(f"generation options {unsupported or {'num_beams': gc.num_beams}} are not supported by the device loop")
+    for k in ("output_attentions", "output_hidden_states"):   # model kwargs in generate(); here refused like the config fields
+        if mk.get(k):
+            setattr(gc, k, True)
+    check_continuous_generate(gc, mk, streamer, logits_processor, stopping_criteria)
+    if gc.max_new_tokens is not None:
+        max_length = int(gc.max_new_tokens) + 1
+    else:
+        max_length = int(user_max_length if user_max_length is not None else gc.max_length)
+    if max_length < 2:
+        raise ValueError(f"max_length must allow at least one new token, got {max_length}")
+    return gc, mk, max_length, suppress_special
+
+
+def slot_outputs(raw: torch.Tensor, eos_last: torch.Tensor, cur_len, shift: torch.Tensor, max_length, codebook_size: int,
                  live: bool = False):
     """Every slot's state at a refill boundary, on the device (nothing here waits for it).  raw [B, K, ld] the history, eos_last [B]
     = 1 + the column of the last codebook's first EOS (0: none; a row stopped by max_length records the PAD it writes after, when
@@ -266,18 +304,24 @@ def slot_outputs(raw: torch.Tensor, eos_last: torch.Tensor, cur_len, shift: torc
     of codebook k is column f + k + 1, F = n - K, once n reaches the delay pattern's 2K - 1 columns; below that every column, F = n.
     live: an unfinished slot with col = cur_len - shift columns also gets its complete frames, F = col - K (the last codebook of
     frame f is column f + K), and none while col < 2K - 1, where the row may still end under the cut without the pattern.  Its
-    compacted frames are then a prefix of those its finished cut will hold (the compaction keeps the frame order)."""
+    compacted frames are then a prefix of those its finished cut will hold (the compaction keeps the frame order).
+    max_length: an int, or an integer tensor [B] of per-slot limits (ContinuousEngine's per-request max_new_tokens): slot b is then
+    cut at its own max_length[b], as generate() with that max_length cuts it, and codes / packed are ld frames wide."""
     B, K, ld = raw.shape
-    L = int(max_length)
+    if isinstance(max_length, torch.Tensor):
+        L, width = max_length.to(device=eos_last.device, dtype=eos_last.dtype), ld
+        n = torch.where(eos_last > 0, torch.minimum(eos_last, L), L)
+    else:
+        L = width = int(max_length)
+        n = torch.where(eos_last > 0, eos_last.clamp(max=L), torch.full_like(eos_last, L))
     finished = (eos_last > 0) | (cur_len - shift >= L)
-    n = torch.where(eos_last > 0, eos_last.clamp(max=L), torch.full_like(eos_last, L))
     pattern = n >= 2 * K - 1
     frames = torch.where(pattern, n - K, n)
     if live:
         col = cur_len - shift
         pattern = pattern | ~finished
         frames = torch.where(finished, frames, torch.where(col >= 2 * K - 1, col - K, torch.zeros_like(col)).to(frames.dtype))
-    f = torch.arange(L, device=raw.device)
+    f = torch.arange(width, device=raw.device)
     off = pattern[:, None].long() * torch.arange(1, K + 1, device=raw.device)[None, :]
     codes = torch.gather(raw, 2, (f[None, None, :] + off[:, :, None]).clamp(max=ld - 1))
     valid = (codes < codebook_size).all(dim=1) & (f[None, :] < frames[:, None])
@@ -328,18 +372,274 @@ class ContinuousRun:
     """generate_continuous()'s iterator of (request index, waveform[, codes]) in completion order, or with stream=True of
     (request index, chunk, final[, codes]) events.  `refills` logs every request
     put into a slot at a boundary as (slot, request, batch column of that boundary); `boundaries` and `steps` count the
-    boundaries and the decode steps enqueued."""
+    boundaries and the decode steps enqueued (those of the ContinuousEngine it drains)."""
 
-    def __init__(self):
-        self.refills: list[tuple[int, int, int]] = []
-        self.boundaries = self.steps = 0
-        self._it = None
+    def __init__(self, engine: "ContinuousEngine"):
+        self.engine = engine
+        self._it = engine._drain()
+
+    refills = property(lambda self: self.engine.refills)
+    boundaries = property(lambda self: self.engine.boundaries)
+    steps = property(lambda self: self.engine.steps)
 
     def __iter__(self):
         return self
 
     def __next__(self):
         return next(self._it)
+
+
+def left_pad(states: Optional[torch.Tensor], mask: Optional[torch.Tensor], n: int, what: str):
+    """One request's states [1, s, H] and mask [1, s] (None: every position attended) left-padded to n positions with zero states
+    and a zero mask, the way a padded batch holds a shorter description or prompt.  No padding keeps the mask as given.  Raises
+    ValueError for s > n."""
+    if states is None:
+        return None, None
+    s = states.shape[1]
+    if s > n:
+        raise ValueError(f"the {what} has {s} positions, more than the engine's max_{what}_length = {n}")
+    if s == n:
+        return states, mask
+    m = torch.ones(1, s, dtype=torch.long, device=states.device) if mask is None else mask.to(states.device, torch.long)
+    pad = n - s
+    states = torch.cat([states.new_zeros(1, pad, states.shape[2]), states], dim=1)
+    return states, torch.cat([m.new_zeros(1, pad), m], dim=1)
+
+
+class ContinuousEngine:
+    """Online continuous batching (ParlerTTSForConditionalGeneration.continuous_engine): requests are submitted, cancelled and
+    stepped while the batch decodes.  One live session of `batch_size` slots; every step() reads the boundary of the interval the
+    previous step() launched, yields its events, admits queued requests into the free slots and launches the next `refill_every`
+    decode steps before it returns, so the device decodes while the caller handles the events and submits.
+
+    Request r draws with Philox key r (its submission index), what row r of one generate() over the submissions in order draws; its
+    codes and waveform equal that row's under the conditions generate_continuous() states.  Each request may have its own
+    max_new_tokens in [2K - 2, the engine's bound] (K codebooks): the slot sampler stops it and applies its delay pattern at its
+    own limit (ptts_generate_set_slots2), and its cut follows that limit (slot_outputs with per-slot limits).
+
+    Calls are serialised by the caller (one handle is not thread-safe): submit() and cancel() belong between step() calls."""
+
+    QUEUED, LIVE, DONE, CANCELLED = range(4)
+
+    def __init__(self, model, sampling: "Sampling", batch_size: int, refill_every: int, S: int, P: int, stream: bool,
+                 return_codes: bool):
+        self._m, self._s = model, sampling
+        self.batch_size, self.refill_every, self.S, self.P = batch_size, refill_every, S, P
+        self.stream, self.return_codes = stream, return_codes
+        self.max_length = sampling.max_length
+        self._K, self._cs = model.config.decoder.num_codebooks, model.config.audio_encoder.codebook_size
+        self._radius = dac_dependency_radius(model.audio_encoder.config.decoder_rates)
+        L, B = self.max_length, batch_size
+        self._live = self._fill = None   # the live and the refill session, made at the first admission and the first refill
+        self._reqs: list = []       # per request: (enc, enc mask, prompt, prompt mask, max_length) until admitted, then None
+        self._status: list[int] = []
+        self._queue: collections.deque = collections.deque()
+        self._slot_req: list = [None] * B
+        self._slot_len = [L] * B    # each slot's max_length (idle slots: the bound)
+        self._cols = [1] * B        # the column each slot draws next
+        self._shift = [0] * B
+        self._emitted = [0] * B     # stream: valid frames of each slot's request already played
+        self._cur_len = 2
+        self._running = False       # an interval is in flight whose boundary has not been read
+        self.refills: list[tuple[int, int, int]] = []
+        self.boundaries = self.steps = 0
+
+    # -- requests -------------------------------------------------------------------------------------------------------------
+    @torch.no_grad()
+    def submit(self, input_ids=None, attention_mask=None, prompt_input_ids=None, prompt_attention_mask=None, encoder_outputs=None,
+               max_new_tokens=None, prompt_hidden_states=None) -> int:
+        """Queue one request (batch of 1: a description, or `encoder_outputs`, and the prompt) and return its id, its submission
+        index.  Its conditioning runs now (text encoder, enc_to_dec_proj, the prompt_cross_attention assembly); the description
+        states are left-padded to max_description_length and the prompt to max_prompt_length.  No decode work is launched: the
+        request is admitted at a later step().  max_new_tokens: None (the engine's bound) or an int in [2K - 2, the bound]."""
+        limit = self._limit(max_new_tokens)
+        enc, em, ph, pm, _, _ = self._m._conditioning("submit", input_ids, attention_mask, encoder_outputs, prompt_input_ids,
+                                                      prompt_attention_mask, prompt_hidden_states,
+                                                      cross_prompt_after_encoder_outputs=True)
+        if enc.shape[0] != 1 or (ph is not None and ph.shape[0] != 1):
+            raise ValueError(f"submit() takes one request, got a batch of {enc.shape[0]}")
+        return self._submit(enc, em, ph, pm, limit)
+
+    def _limit(self, max_new_tokens) -> int:
+        if max_new_tokens is None:
+            return self.max_length
+        if isinstance(max_new_tokens, bool) or not isinstance(max_new_tokens, int):
+            raise ValueError(f"max_new_tokens must be an int, got {max_new_tokens!r}")
+        lo = max(2 * self._K - 1, 2)
+        if self.max_length < lo:
+            raise ValueError(f"an engine with max_length {self.max_length} < {lo} (below the delay pattern's 2K - 1 columns) "
+                             "takes no per-request max_new_tokens")
+        if not lo - 1 <= max_new_tokens <= self.max_length - 1:
+            raise ValueError(f"max_new_tokens {max_new_tokens} outside [{lo - 1}, {self.max_length - 1}] (2K - 2 .. the engine's bound)")
+        return max_new_tokens + 1
+
+    def _submit(self, enc, em, ph, pm, limit: int) -> int:
+        if ph is not None and self.P == 0:
+            raise ValueError("a prompt on an engine with max_prompt_length = 0")
+        if ph is None and self.P > 0:
+            raise ValueError(f"every request on an engine with max_prompt_length = {self.P} needs a prompt")
+        enc, em = left_pad(enc, em, self.S, "description")
+        ph, pm = left_pad(ph, pm, self.P, "prompt")
+        rid = len(self._reqs)
+        self._reqs.append((enc, em, ph, pm, limit))
+        self._status.append(self.QUEUED)
+        self._queue.append(rid)
+        return rid
+
+    def cancel(self, rid: int) -> bool:
+        """Drop request rid: a queued one at once, a live one at the next boundary (its slot is free then; it yields nothing more and
+        takes no codec call).  False if it already finished or was cancelled; ValueError for an id never returned by submit()."""
+        if isinstance(rid, bool) or not isinstance(rid, int) or not 0 <= rid < len(self._status):
+            raise ValueError(f"no request {rid!r}: ids are 0 .. {len(self._status) - 1}")
+        st = self._status[rid]
+        if st == self.QUEUED:
+            self._queue.remove(rid)
+            self._reqs[rid] = None
+        elif st != self.LIVE:
+            return False
+        self._status[rid] = self.CANCELLED
+        return True
+
+    @property
+    def idle(self) -> bool:
+        """No live and no queued request."""
+        return not self._queue and all(r is None or self._status[r] == self.CANCELLED for r in self._slot_req)
+
+    # -- the loop -------------------------------------------------------------------------------------------------------------
+    @torch.no_grad()
+    def step(self) -> list:
+        """One boundary and one interval: the events of the boundary of the interval the previous step() launched (the tuples
+        generate_continuous() yields), after admitting queued requests into the free slots and launching the next refill_every
+        decode steps.  An idle engine returns [] and launches nothing."""
+        if self.idle:
+            return []
+        events, done = [], None
+        if self._running:
+            events, done = self._boundary()
+        self._admit()
+        self._running = any(r is not None for r in self._slot_req)
+        if self._running:
+            self._cur_len, self._shift = rebase_slots(self._cur_len, [c if r is not None else None
+                                                                      for c, r in zip(self._cols, self._slot_req)])
+            lims = None if all(v == self.max_length for v in self._slot_len) else self._slot_len
+            self._live.set_slots(self._cur_len, self._shift, [0 if r is None else r for r in self._slot_req], lims)
+            self._live.decode_steps(self.refill_every)   # enqueued before the finished requests' codec call and the caller's turn
+            self.steps += self.refill_every
+        if done is not None and done[0] and not self.stream:
+            # the codes were cut before any import overwrote their slots; the codec call queues behind the next interval
+            slots, reqs, codes, packed, frames, n_valid = done
+            audio, lengths = packed_to_waveform(self._m.audio_encoder, torch.stack([packed[b] for b in slots]),
+                                                [n_valid[b] for b in slots], self._m.dtype)
+            for j, (b, r) in enumerate(zip(slots, reqs)):
+                wav = audio[j, :lengths[j]]
+                events.append((r, wav, codes[b, :, :frames[b]]) if self.return_codes else (r, wav))
+        return events
+
+    def _boundary(self):
+        """Read the boundary in one host sync (every slot's outcome is computed on the device first): free the cancelled and the
+        finished slots; with stream=True enqueue the boundary's codec windows.  Returns (stream events, the finished slots)."""
+        B, K, live = self.batch_size, self._K, self._live
+        self.boundaries += 1
+        rows = torch.tensor([self._shift, self._slot_len], dtype=torch.int32).pin_memory().to(self._m.device, non_blocking=True)
+        fin, frames, codes, packed, n_valid = slot_outputs(live.raw_ids.view(B, K, -1), live.eos_seen.view(B, K)[:, K - 1],
+                                                           live.state[0], rows[0], rows[1], self._cs, live=self.stream)
+        status = torch.cat([live.state[:1].long(), fin.long(), frames.long(), n_valid.long()]).cpu().tolist()
+        self._cur_len = status[0]
+        fin, frames, n_valid = status[1:1 + B], status[1 + B:1 + 2 * B], status[1 + 2 * B:]
+        self._cols = [self._cur_len - sh for sh in self._shift]
+        for b, r in enumerate(self._slot_req):
+            if r is not None and self._status[r] == self.CANCELLED:
+                self._slot_req[b] = None
+        events = self._stream_events(packed, codes, fin, frames, n_valid) if self.stream else []
+        slots = [b for b, r in enumerate(self._slot_req) if r is not None and fin[b]]
+        reqs = [self._slot_req[b] for b in slots]
+        for b, r in zip(slots, reqs):
+            self._status[r] = self.DONE
+            self._slot_req[b] = None
+        return events, (slots, reqs, codes, packed, frames, n_valid)
+
+    def _admit(self):
+        """Queued requests into free slots: the live session's own prefill the first time, then a prefill of the refill session
+        and ptts_session_import_rows.  Request r takes row r - r0 of the prefill (r0 the first admitted), so that row_base r0 * K
+        gives it Philox key r; rows of no admitted request repeat the last one (one prefill of batch_size rows, whose GEMMs take a
+        batch_size-row batch's kernels)."""
+        free = [b for b, r in enumerate(self._slot_req) if r is None]
+        if not free or not self._queue:
+            return
+        B, r0, picked = self.batch_size, self._queue[0], []
+        while self._queue and len(picked) < len(free) and self._queue[0] - r0 < B:
+            picked.append(self._queue.popleft())
+        by_row = {r - r0: self._reqs[r] for r in picked}
+        last = self._reqs[picked[-1]]
+        rows = [by_row.get(j, last) for j in range(B)]
+        conds = self._stack(rows)
+        s, eng, first = self._s, self._m.decoder.engine, self._live is None
+        if first:
+            # max_input_len 2 gives the per-row offsets; finished rows decode PAD until their boundary, hence + refill_every
+            self._live = GenSession(eng, B, self.P, self.S, self.P + self.max_length + self.refill_every, max_input_len=2)
+            sess, slots = self._live, [r - r0 for r in picked]
+        else:
+            if self._fill is None:
+                self._fill = GenSession(eng, B, self.P, self.S, self.P + self.max_length, max_input_len=2)
+            sess, slots = self._fill, free[:len(picked)]
+        sess.begin(s.max_length, do_sample=s.do_sample, temperature=s.temperature, top_k=s.top_k, top_p=s.top_p,
+                   min_new_tokens=s.min_new_tokens, seed=s.seed, suppress_special=s.suppress_special, codebook_size=s.codebook_size,
+                   row_base=r0 * self._K, ext=s.ext, lext=s.lext)
+        enc, em, ph, pm = conds
+        sess.prefill(ph, pm, enc, em)
+        sess.sample()   # the first column, drawn under the engine's max_length (set_slots2 states why that is the request's own)
+        if not first:
+            self._live.import_rows(self._fill, [r - r0 for r in picked], slots)
+        for r, b in zip(picked, slots):
+            self._slot_req[b], self._cols[b], self._emitted[b], self._slot_len[b] = r, 2, 0, self._reqs[r][4]
+            self._status[r], self._reqs[r] = self.LIVE, None
+            if not first:
+                self.refills.append((b, r, self._cur_len))
+
+    def _stack(self, rows) -> list:
+        """The rows' (description states, mask, prompt states, mask) as batch tensors.  A mask is None when no row has one; a row
+        without one (a request given no mask, at full length) then attends everywhere."""
+        out, dev = [], self._m.device
+        for i, n in ((0, None), (1, self.S), (2, None), (3, self.P)):
+            ts = [row[i] for row in rows]
+            if all(t is None for t in ts):
+                out.append(None)
+            elif n is None:
+                out.append(torch.cat(ts))
+            else:
+                out.append(torch.cat([torch.ones(1, n, dtype=torch.long, device=dev) if t is None else t.to(dev, torch.long) for t in ts]))
+        return out
+
+    def _stream_events(self, packed, codes, fin, frames, n_valid):
+        """One streamed boundary: every slot's window through one windowed codec call (enqueued here, waited for by nobody), and
+        the events, in slot order.  Advances `_emitted`."""
+        m, slot_req, emitted = self._m, self._slot_req, self._emitted
+        wins = stream_windows(n_valid, [e if r is not None else None for e, r in zip(emitted, slot_req)],
+                              [r is not None and bool(f) for r, f in zip(slot_req, fin)], self._radius)
+        # a fresh buffer per boundary: the chunks yielded are views into it
+        audio = m.audio_encoder._decode_windows(packed, wins) if any(w[1] > 0 for w in wins) else None
+        hop, events = m.audio_encoder.hop_length, []
+        for b, (r, (start, n, lo, hi)) in enumerate(zip(slot_req, wins)):
+            final = r is not None and bool(fin[b])
+            if r is None or not (final or hi > lo):
+                continue
+            if final and n_valid[b] == 0:      # no valid frame: the [1] zero waveform, as stream=False gives
+                chunk = torch.zeros(1, device=m.device, dtype=m.dtype)
+            elif hi > lo:
+                chunk = audio[b, lo * hop:hi * hop]
+                emitted[b] = start + hi
+            else:
+                chunk = torch.zeros(0, device=m.device, dtype=m.dtype)
+            if self.return_codes:
+                events.append((r, chunk, final, codes[b, :, :frames[b]] if final else None))
+            else:
+                events.append((r, chunk, final))
+        return events
+
+    def _drain(self):
+        """generate_continuous()'s loop: step until idle, yielding the events."""
+        while not self.idle:
+            yield from self.step()
 
 
 def shift_tokens_right(input_ids: torch.Tensor, pad_token_id: int, decoder_start_token_id: int):
@@ -1054,12 +1354,14 @@ class GenSession:
         arr = lambda v: (C.c_int32 * max(n, 1))(*[int(x) for x in v])
         _lib.check(_lib.lib().ptts_session_import_rows(self.h, src.h, arr(src_rows), arr(dst_rows), n, _lib.stream_ptr()))
 
-    def set_slots(self, cur_len: int, row_shift: list[int], row_key: list[int]):
-        """ptts_generate_set_slots: slot mode, row b at its own column cur_len - row_shift[b] with Philox key row_key[b]."""
-        if len(row_shift) != self.B or len(row_key) != self.B:
-            raise ValueError(f"row_shift and row_key must hold {self.B} entries")
+    def set_slots(self, cur_len: int, row_shift: list[int], row_key: list[int], row_max_length: Optional[list[int]] = None):
+        """ptts_generate_set_slots2: slot mode, row b at its own column cur_len - row_shift[b] with Philox key row_key[b] and, when
+        given, its own limit row_max_length[b] in [2K - 1, max_length] (None: every row max_length)."""
+        if len(row_shift) != self.B or len(row_key) != self.B or (row_max_length is not None and len(row_max_length) != self.B):
+            raise ValueError(f"row_shift, row_key and row_max_length must hold {self.B} entries")
         arr = lambda v: (C.c_int32 * self.B)(*[int(x) for x in v])
-        _lib.check(_lib.lib().ptts_generate_set_slots(self.h, int(cur_len), arr(row_shift), arr(row_key), _lib.stream_ptr()))
+        lims = None if row_max_length is None else arr(row_max_length)
+        _lib.check(_lib.lib().ptts_generate_set_slots2(self.h, int(cur_len), arr(row_shift), arr(row_key), lims, _lib.stream_ptr()))
 
     def set_outputs(self, logits: Optional[torch.Tensor], scores: Optional[torch.Tensor], first_step: int = 0, n_steps: int = 0,
                     step_stride: int = 0):
@@ -2299,7 +2601,8 @@ class ParlerTTSForConditionalGeneration:
         is enqueued, and the finished requests' valid frames go through one ragged codec call behind it (the codec's range check
         waits for that interval, which the next boundary waits for anyway).  Finished rows keep
         decoding PAD until their boundary, so the live session holds max_length + refill_every columns.  Raises ValueError for what
-        check_continuous_generate lists.
+        check_continuous_generate lists.  This is a ContinuousEngine (continuous_engine()) of min(batch_size, N) slots with every
+        request submitted up front, stepped until idle.
 
         stream=True yields each request's audio while it is generated: events (request index, chunk, final), or (request index,
         chunk, final, codes) with return_codes=True, where codes is the [K, T_i] tensor on the final event and None before it.
@@ -2310,135 +2613,38 @@ class ParlerTTSForConditionalGeneration:
         windows of all slots go through one windowed codec call (DACModel._decode_windows), enqueued before the refill and the
         next interval, and the events are yielded in slot order.  A request's first chunk comes at the first boundary that has
         more than dac_dependency_radius (10 for the 44.1 kHz codec) valid frames of it."""
-        import copy
-        if not isinstance(stream, bool):
-            raise ValueError(f"stream must be a bool, got {stream!r}")
-        if isinstance(batch_size, bool) or not isinstance(batch_size, int) or batch_size < 1:
-            raise ValueError(f"batch_size must be a positive int, got {batch_size!r}")
-        if isinstance(refill_every, bool) or not isinstance(refill_every, int) or refill_every < 1:
-            raise ValueError(f"refill_every must be a positive int, got {refill_every!r}")
-        gc = copy.deepcopy(self.generation_config)
-        suppress_special = kwargs.pop("_suppress_special", False)
-        user_max_length = kwargs.get("max_length")
-        mk = gc.update(**kwargs)
-        unknown = sorted(k for k in mk if k not in self._MODEL_KWARGS)
-        if unknown:
-            raise ValueError(f"The following `model_kwargs` are not used by the model: {unknown}")
-        unsupported = {k: getattr(gc, k) for k, neutral in self._NEUTRAL_GENERATION_KNOBS.items() if getattr(gc, k, neutral) != neutral}
-        if unsupported or gc.num_beams != 1:
-            raise ValueError(f"generation options {unsupported or {'num_beams': gc.num_beams}} are not supported by the device loop")
-        for k in ("output_attentions", "output_hidden_states"):   # model kwargs in generate(); here refused like the config fields
-            if mk.get(k):
-                setattr(gc, k, True)
-        check_continuous_generate(gc, mk, streamer, logits_processor, stopping_criteria)
-        if gc.max_new_tokens is not None:
-            max_length = int(gc.max_new_tokens) + 1
-        else:
-            max_length = int(user_max_length if user_max_length is not None else gc.max_length)
-        if max_length < 2:
-            raise ValueError(f"max_length must allow at least one new token, got {max_length}")
+        check_continuous_counts(stream, batch_size, refill_every)
+        gc, mk, max_length, suppress_special = continuous_settings(self, kwargs, streamer, logits_processor, stopping_criteria)
         enc_hidden, enc_mask, prompt_hidden, prompt_mask, _, _ = self._conditioning(
             "generate_continuous", input_ids, attention_mask, mk.get("encoder_outputs"), prompt_input_ids, prompt_attention_mask,
             mk.get("prompt_hidden_states"), cross_prompt_after_encoder_outputs=True)
         sampling = self._sampling(gc, 1, max_length, seed, suppress_special)
-        run = ContinuousRun()
-        run._it = self._continuous_loop(run, enc_hidden, enc_mask, prompt_hidden, prompt_mask, sampling, batch_size, refill_every,
-                                        bool(return_codes), stream)
-        return run
-
-    def _continuous_loop(self, run: ContinuousRun, enc_hidden, enc_mask, prompt_hidden, prompt_mask, s: Sampling, batch_size: int,
-                         refill_every: int, return_codes: bool, stream: bool):
-        d = self.config.decoder
-        K, eng, cs = d.num_codebooks, self.decoder.engine, self.config.audio_encoder.codebook_size
         N, S = enc_hidden.shape[0], enc_hidden.shape[1]
         P = 0 if prompt_hidden is None else prompt_hidden.shape[1]
-        Bl = min(batch_size, N)
+        engine = ContinuousEngine(self, sampling, max(1, min(batch_size, N)), refill_every, S, P, stream, bool(return_codes))
+        row = lambda t, i: None if t is None else t[i:i + 1]
+        for i in range(N):
+            engine._submit(enc_hidden[i:i + 1], row(enc_mask, i), row(prompt_hidden, i), row(prompt_mask, i), max_length)
+        return ContinuousRun(engine)
 
-        def start(sess, first, count, row_base):   # begin + prefill + the first column, as a generate() shard does
-            sess.begin(s.max_length, do_sample=s.do_sample, temperature=s.temperature, top_k=s.top_k, top_p=s.top_p,
-                       min_new_tokens=s.min_new_tokens, seed=s.seed, suppress_special=s.suppress_special,
-                       codebook_size=s.codebook_size, row_base=row_base, ext=s.ext, lext=s.lext)
-            rows = lambda t: refill_rows(t, first, count, Bl)
-            sess.prefill(rows(prompt_hidden), rows(prompt_mask), rows(enc_hidden), rows(enc_mask))
-            sess.sample()
-
-        # Sessions of our own (DecoderEngine.session keeps one live session); max_input_len 2 gives both the per-row offsets.  The
-        # refill session has the live session's rows, so one prefill serves a whole refill.
-        live = GenSession(eng, Bl, P, S, P + s.max_length + refill_every, max_input_len=2)
-        fill = GenSession(eng, Bl, P, S, P + s.max_length, max_input_len=2) if N > Bl else None
-        start(live, 0, Bl, 0)            # requests 0 .. Bl-1: the first shard generate() would run
-        slot_req: list = list(range(Bl))
-        nxt, cur_len = Bl, 2
-        shift = [0] * Bl
-        emitted = [0] * Bl   # stream: valid frames of each slot's request already played
-        radius = dac_dependency_radius(self.audio_encoder.config.decoder_rates)
-        live.set_slots(cur_len, shift, slot_req)
-        live.decode_steps(refill_every)
-        run.steps += refill_every
-        while True:
-            run.boundaries += 1
-            # every slot's outcome is computed on the device, then read in the boundary's one host sync
-            shift_dev = torch.tensor(shift, dtype=torch.int32).pin_memory().to(self.device, non_blocking=True)
-            fin, frames, codes, packed, n_valid = slot_outputs(live.raw_ids.view(Bl, K, -1), live.eos_seen.view(Bl, K)[:, K - 1],
-                                                               live.state[0], shift_dev, s.max_length, cs, live=stream)
-            status = torch.cat([live.state[:1].long(), fin.long(), frames.long(), n_valid.long()]).cpu().tolist()
-            cur_len = status[0]
-            fin, frames, n_valid = status[1:1 + Bl], status[1 + Bl:1 + 2 * Bl], status[1 + 2 * Bl:]
-            cols = [cur_len - sh for sh in shift]
-            if stream:   # the codec call goes ahead of the refill and the next interval: the chunks are ready one call after the sync
-                events = self._stream_events(packed, codes, slot_req, fin, frames, n_valid, emitted, radius, return_codes)
-            done = [b for b, r in enumerate(slot_req) if r is not None and fin[b]]
-            done_req = [slot_req[b] for b in done]
-            for b in done:
-                slot_req[b] = None
-            free = [b for b, r in enumerate(slot_req) if r is None]
-            g = min(len(free), N - nxt)
-            if g > 0:   # one prefill of Bl rows: the next g requests, padded with the last one
-                start(fill, nxt, g, nxt * K)
-                live.import_rows(fill, list(range(g)), free[:g])
-                for j, b in enumerate(free[:g]):
-                    slot_req[b], cols[b], emitted[b] = nxt + j, 2, 0
-                    run.refills.append((b, nxt + j, cur_len))
-                nxt += g
-            last = all(r is None for r in slot_req)
-            if not last:
-                cur_len, shift = rebase_slots(cur_len, [c if r is not None else None for c, r in zip(cols, slot_req)])
-                live.set_slots(cur_len, shift, [0 if r is None else r for r in slot_req])
-                live.decode_steps(refill_every)   # enqueued before the finished requests' codec call and the caller's turn
-                run.steps += refill_every
-            if stream:
-                yield from events
-            elif done:
-                # the codes were cut before any import overwrote their slots; the codec call queues behind the next interval
-                audio, lengths = packed_to_waveform(self.audio_encoder, torch.stack([packed[b] for b in done]),
-                                                    [n_valid[b] for b in done], self.dtype)
-                for j, (b, r) in enumerate(zip(done, done_req)):
-                    wav = audio[j, :lengths[j]]
-                    yield (r, wav, codes[b, :, :frames[b]]) if return_codes else (r, wav)
-            if last:
-                return
-
-    def _stream_events(self, packed, codes, slot_req, fin, frames, n_valid, emitted, radius, return_codes):
-        """One streamed boundary: every slot's window through one windowed codec call (enqueued here, waited for by nobody), and
-        the events to yield, in slot order.  Advances `emitted`."""
-        wins = stream_windows(n_valid, [e if r is not None else None for e, r in zip(emitted, slot_req)],
-                              [r is not None and bool(f) for r, f in zip(slot_req, fin)], radius)
-        # a fresh buffer per boundary: the chunks yielded are views into it
-        audio = self.audio_encoder._decode_windows(packed, wins) if any(w[1] > 0 for w in wins) else None
-        hop, events = self.audio_encoder.hop_length, []
-        for b, (r, (start, n, lo, hi)) in enumerate(zip(slot_req, wins)):
-            final = r is not None and bool(fin[b])
-            if r is None or not (final or hi > lo):
-                continue
-            if final and n_valid[b] == 0:      # no valid frame: the [1] zero waveform, as stream=False gives
-                chunk = torch.zeros(1, device=self.device, dtype=self.dtype)
-            elif hi > lo:
-                chunk = audio[b, lo * hop:hi * hop]
-                emitted[b] = start + hi
-            else:
-                chunk = torch.zeros(0, device=self.device, dtype=self.dtype)
-            if return_codes:
-                events.append((r, chunk, final, codes[b, :, :frames[b]] if final else None))
-            else:
-                events.append((r, chunk, final))
-        return events
+    @torch.no_grad()
+    def continuous_engine(self, batch_size: int = 32, refill_every: int = 16, max_description_length: Optional[int] = None,
+                          max_prompt_length: int = 0, stream: bool = False, return_codes: bool = False, seed=0, streamer=None,
+                          logits_processor=None, stopping_criteria=None, **kwargs) -> ContinuousEngine:
+        """An online ContinuousEngine: `batch_size` slots of one live session sized for the generation settings' max_length (the
+        engine's bound; each request may ask for less), descriptions of up to max_description_length positions (on a
+        prompt_cross_attention checkpoint, description and prompt together) and prompts of up to max_prompt_length.  It takes
+        generate_continuous()'s settings and refuses what it refuses; the requests' inputs go to submit().  Nothing is decoded
+        until step()."""
+        check_continuous_counts(stream, batch_size, refill_every)
+        for name, v in (("max_description_length", max_description_length), ("max_prompt_length", max_prompt_length)):
+            if isinstance(v, bool) or not isinstance(v, int) or v < (1 if name == "max_description_length" else 0):
+                raise ValueError(f"{name} must be a {'positive' if name == 'max_description_length' else 'non-negative'} int, got {v!r}")
+        gc, mk, max_length, suppress_special = continuous_settings(self, kwargs, streamer, logits_processor, stopping_criteria)
+        inputs = sorted(k for k in ("input_ids", "attention_mask", "prompt_input_ids", "prompt_attention_mask", "prompt_hidden_states",
+                                    "encoder_outputs", "padding_mask") if mk.get(k) is not None)
+        if inputs:
+            raise ValueError(f"continuous_engine() takes generation settings; the requests' inputs ({', '.join(inputs)}) go to submit()")
+        sampling = self._sampling(gc, 1, max_length, seed, suppress_special)
+        return ContinuousEngine(self, sampling, batch_size, refill_every, max_description_length, max_prompt_length, stream,
+                                bool(return_codes))
