@@ -415,6 +415,19 @@ int ptts_op_linear2(const ptts_decoder_config* cfg, const void* blob, int32_t te
 /* ptts_op_linear2 with path 0 (the decode GEMM): the original signature, kept for existing callers. */
 int ptts_op_linear(const ptts_decoder_config* cfg, const void* blob, int32_t tensor_id, int32_t index,
                    const void* x, int32_t M, int32_t use_ln, int32_t epilogue, const void* residual, void* y, void* stream);
+/* The scoring heads of ptts_score over a given residual stream, with no decoder forward in front: the same launch sequence
+ * (ptts_score calls the same function).  Test hook for the scoring kernels.
+ *   x         [B][P+T][H] in the model dtype: the decoder output; rows P .. P+T-1 of each utterance are the label positions
+ *   labels, dec_ids, token_nll, out_logits, codebook_sums   as for ptts_score ([B,T,K], [B*K,T], [B,T,K], [B*K,T,V], [K][2])
+ *   path 0    the unfused route: the lm heads GEMM (launch_linear, f32 logits) over the B rows of each frame into
+ *             logits_scratch [B*K][V] f32, then score_rows_kernel; every dtype; labels may be NULL (logits only)
+ *   path 1    the fused heads + cross-entropy kernel, under ptts_score's rule: bf16, labels given, no out_logits, hidden_size
+ *             % 64 == 0 and vocab_size <= 8192, heads_rm from ptts_lm_heads_rowmajor_pack.  xs_scratch [B*T][H] bf16 receives
+ *             the gathered label rows and row_stats [B*T][2] f32 their LayerNorm (mean, rstd).
+ * PTTS_EINVAL, with nothing launched, when an argument breaks these rules or a scratch buffer the path needs is NULL. */
+int ptts_op_score(const ptts_decoder_config* cfg, const void* blob, const void* heads_rm, const void* x, int32_t B, int32_t P,
+                  int32_t T, const int64_t* labels, const int64_t* dec_ids, int32_t path, float* token_nll, float* out_logits,
+                  float* codebook_sums, void* xs_scratch, float* row_stats, float* logits_scratch, void* stream);
 /* Self- or cross-attention of q_len new positions per batch row (ParlerTTSSdpaAttention after the projections, :858-914), with
  * the kernels the decoder launches.  Test hook for the attention sweeps.
  *   dtype PTTS_BF16 / PTTS_F32; nh query heads, nkv K/V heads (nh % nkv == 0); head_dim 64; scale 1/8.

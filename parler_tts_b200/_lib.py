@@ -107,6 +107,8 @@ _SIGS = {
     "ptts_op_sample_phase": (C.c_int, [_VP, _I32, _VP]),
     "ptts_op_linear": (C.c_int, [C.POINTER(DecoderConfigC), _VP, _I32, _I32, _VP, _I32, _I32, _I32, _VP, _VP, _VP]),
     "ptts_op_linear2": (C.c_int, [C.POINTER(DecoderConfigC), _VP, _I32, _I32, _VP, _I32, _I32, _I32, _VP, _VP, _I32, _VP, _VP]),
+    "ptts_op_score": (C.c_int, [C.POINTER(DecoderConfigC), _VP, _VP, _VP, _I32, _I32, _I32, _VP, _VP, _I32, _VP, _VP, _VP, _VP,
+                                _VP, _VP, _VP]),
     "ptts_op_attention": (C.c_int, [_I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _VP, _VP, _VP, _VP, _VP, _VP,
                                     _I32, _I32, _VP, _VP]),
     "ptts_op_attention_probs": (C.c_int, [_I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _VP, _VP, _VP, _I64, _VP,

@@ -737,6 +737,44 @@ int ptts_lm_heads_rowmajor_pack(const ptts_decoder_config* cfg, const void* blob
   return unpack_fragments((const char*)blob + L.heads, heads_rm, (int64_t)L.K * L.V, L.H, (cudaStream_t)stream);
 }
 
+// The scoring heads over the residual stream x [B][P+T][H] (ptts_score after its forward pass, and ptts_op_score): fused, the
+// label-row gather and the heads + cross-entropy kernel; unfused, the decoder's heads GEMM over the B rows of one frame at a time
+// into logits_scratch [B*K][V], then score_rows_kernel; then the per-codebook reduce when codebook_sums is given.
+static int score_heads(const ptts_decoder_config& c, const DecoderLayout& L, const char* blob, const void* heads_rm, const char* x,
+                       int B, int P, int T, const int64_t* labels, const int64_t* dec_ids, bool fused, float* token_nll,
+                       float* out_logits, float* codebook_sums, void* xs_scratch, float* row_stats, float* logits_scratch,
+                       int sm_count, int64_t* launches, cudaStream_t st) {
+  ScoreArgs a{};
+  a.labels = labels; a.dec_ids = dec_ids; a.token_nll = token_nll;
+  a.M = B * T; a.B = B; a.T = T; a.K = L.K; a.V = L.V; a.H = L.H;
+  a.bos = c.bos_token_id; a.eos = c.eos_token_id;
+  const int q_len = P + T;
+  const DecoderMatrix hm = decoder_matrix(L, MAT_HEADS, 0);
+  if (fused) {
+    a.c1 = (const float*)(blob + hm.c); a.c2 = a.c1 + hm.N;
+    *launches += 2;
+    if (int e = launch_score_fused(a, x, P, c.layer_norm_eps, xs_scratch, row_stats, heads_rm, st)) return e;
+  } else {
+    for (int t = 0; t < T; t++) {
+      LinearArgs h{};
+      h.X = x + (int64_t)(P + t) * L.H * L.es; h.ldx = (int64_t)q_len * L.H;
+      h.W = blob + hm.w; h.Y = logits_scratch; h.ldy = hm.N; h.ldr = h.ldy;
+      h.ln_w = (const float*)(blob + hm.ln_w); h.ln_b = (const float*)(blob + hm.ln_b); h.eps = c.layer_norm_eps;
+      if (c.dtype == PTTS_BF16) { h.c1 = (const float*)(blob + hm.c); h.c2 = h.c1 + hm.N; }
+      h.M = B; h.N = hm.N; h.K = hm.K; h.Kc = hm.K;
+      h.epi = EPI_F32; h.act = c.activation;
+      if (int e = launch_linear(h, c.dtype, st, false, sm_count)) return e;
+      if (int e = launch_score_rows(a, logits_scratch, t, out_logits, st)) return e;
+      *launches += 2;
+    }
+  }
+  if (codebook_sums != nullptr) {
+    (*launches)++;
+    if (int e = launch_score_reduce(a, codebook_sums, st)) return e;
+  }
+  return PTTS_OK;
+}
+
 int ptts_score(ptts_session* s, const void* prompt_hidden, const int64_t* prompt_mask, const void* enc_hidden, const int64_t* enc_mask,
                const int64_t* dec_ids, const int64_t* labels, int32_t T, const void* heads_rm, float* out_token_nll, float* out_logits,
                float* out_codebook_sums, void* stream) {
@@ -762,36 +800,9 @@ int ptts_score(ptts_session* s, const void* prompt_hidden, const int64_t* prompt
   s->ragged = s->slots = false;
   s->begun = s->prefilled = false;  // the caches now hold this call's positions: a generation has to begin again
   if (int e = run_forward(s, st, true, prompt_hidden, enc_hidden, false)) return e;
-
-  ScoreArgs a{};
-  a.labels = labels; a.dec_ids = dec_ids; a.token_nll = out_token_nll;
-  a.M = W.B * T; a.B = W.B; a.T = T; a.K = L.K; a.V = L.V; a.H = L.H;
-  a.bos = c.bos_token_id; a.eos = c.eos_token_id;
-  const int q_len = W.P + T;
-  const DecoderMatrix hm = decoder_matrix(L, MAT_HEADS, 0);
-  if (fused) {
-    a.c1 = (const float*)(s->blob + hm.c); a.c2 = a.c1 + hm.N;
-    s->launches += 2;
-    if (int e = launch_score_fused(a, s->ws + W.x, W.P, c.layer_norm_eps, s->ws + W.qc, (float*)(s->ws + W.row_stats), heads_rm, st)) return e;
-  } else {  // the decoder's heads GEMM over the B rows of one frame at a time, into the workspace logits [B*K][V]
-    for (int t = 0; t < T; t++) {
-      LinearArgs h{};
-      h.X = s->ws + W.x + (int64_t)(W.P + t) * L.H * L.es; h.ldx = (int64_t)q_len * L.H;
-      h.W = s->blob + hm.w; h.Y = s->ws + W.logits; h.ldy = hm.N; h.ldr = h.ldy;
-      h.ln_w = (const float*)(s->blob + hm.ln_w); h.ln_b = (const float*)(s->blob + hm.ln_b); h.eps = c.layer_norm_eps;
-      if (c.dtype == PTTS_BF16) { h.c1 = (const float*)(s->blob + hm.c); h.c2 = h.c1 + hm.N; }
-      h.M = W.B; h.N = hm.N; h.K = hm.K; h.Kc = hm.K;
-      h.epi = EPI_F32; h.act = c.activation;
-      if (int e = launch_linear(h, c.dtype, st, false, s->sm_count)) return e;
-      if (int e = launch_score_rows(a, (const float*)(s->ws + W.logits), t, out_logits, st)) return e;
-      s->launches += 2;
-    }
-  }
-  if (out_codebook_sums != nullptr) {
-    s->launches++;
-    if (int e = launch_score_reduce(a, out_codebook_sums, st)) return e;
-  }
-  return PTTS_OK;
+  return score_heads(c, L, s->blob, heads_rm, s->ws + W.x, W.B, W.P, T, labels, dec_ids, fused, out_token_nll, out_logits,
+                     out_codebook_sums, s->ws + W.qc, (float*)(s->ws + W.row_stats), (float*)(s->ws + W.logits), s->sm_count,
+                     &s->launches, st);
 }
 
 int ptts_decode_forward(ptts_session* s, void* stream) {
@@ -1070,6 +1081,32 @@ int ptts_op_linear2(const ptts_decoder_config* cfg, const void* blob, int32_t te
 int ptts_op_linear(const ptts_decoder_config* cfg, const void* blob, int32_t tensor_id, int32_t index, const void* x, int32_t M,
                    int32_t use_ln, int32_t epilogue, const void* residual, void* y, void* stream) {
   return ptts_op_linear2(cfg, blob, tensor_id, index, x, M, use_ln, epilogue, residual, y, 0, nullptr, stream);
+}
+
+int ptts_op_score(const ptts_decoder_config* cfg, const void* blob, const void* heads_rm, const void* x, int32_t B, int32_t P,
+                  int32_t T, const int64_t* labels, const int64_t* dec_ids, int32_t path, float* token_nll, float* out_logits,
+                  float* codebook_sums, void* xs_scratch, float* row_stats, float* logits_scratch, void* stream) {
+  PTTS_REQUIRE(cfg && blob && x && dec_ids, "null argument");
+  PTTS_REQUIRE(path == 0 || path == 1, "op_score: path is 0 (heads GEMM + score_rows) or 1 (fused heads + cross-entropy), got %d", path);
+  PTTS_REQUIRE(B >= 1 && P >= 0 && T >= 1, "op_score: needs B >= 1, P >= 0, T >= 1, got B %d P %d T %d", B, P, T);
+  if (int e = validate_config(*cfg)) return e;
+  const DecoderLayout L = make_layout(*cfg);
+  PTTS_REQUIRE(labels ? (token_nll != nullptr) : (out_logits != nullptr && codebook_sums == nullptr),
+               "op_score: labels need token_nll; without labels only out_logits can be filled");
+  if (path == 1) {  // the rule of ptts_score: bf16, no logits wanted, a shape the fused kernel takes, the row-major heads
+    PTTS_REQUIRE(cfg->dtype == PTTS_BF16, "op_score: the fused kernel is bf16 only");
+    PTTS_REQUIRE(labels && out_logits == nullptr, "op_score: the fused kernel needs labels and writes no logits");
+    PTTS_REQUIRE(score_fused_supported(L.H, L.V), "op_score: hidden_size %d / vocab_size %d are outside the fused kernel", L.H, L.V);
+    PTTS_REQUIRE(heads_rm && xs_scratch && row_stats, "op_score: the fused kernel needs heads_rm, xs_scratch [B*T][H] and row_stats [B*T][2]");
+  } else {
+    PTTS_REQUIRE(logits_scratch, "op_score: the heads GEMM needs logits_scratch [B*K][V]");
+  }
+  int sm = 132, dev = 0;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&sm, cudaDevAttrMultiProcessorCount, dev);
+  int64_t launches = 0;
+  return score_heads(*cfg, L, (const char*)blob, heads_rm, (const char*)x, B, P, T, labels, dec_ids, path == 1, token_nll, out_logits,
+                     codebook_sums, xs_scratch, row_stats, logits_scratch, sm, &launches, (cudaStream_t)stream);
 }
 
 int ptts_op_attention(int32_t dtype, int32_t B, int32_t nh, int32_t nkv, int32_t q_len, int32_t past_len, int32_t cross,

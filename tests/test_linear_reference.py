@@ -189,8 +189,9 @@ class Layer:
         return (self.gamma.float() * self.W.float()).bfloat16().double()
 
 
-def linear_f64(layer: Layer, x: torch.Tensor, bug: str | None = None):
-    """Exact pre-epilogue output y [M, N] and the bound E on the kernel's fp32 deviation from it."""
+def linear_f64(layer: Layer, x: torch.Tensor, bug: str | None = None, folded: bool = False):
+    """Exact pre-epilogue output y [M, N] and the bound E on the kernel's fp32 deviation from it.  folded (bf16 with
+    LayerNorm): y is the folded layer r sum_k (x_k - mu) W'_k + c2 itself, exact, and E has no E_fold term."""
     W, K = layer.W, layer.W.shape[1]
     if layer.gamma is None:
         xh = x
@@ -215,7 +216,10 @@ def linear_f64(layer: Layer, x: torch.Tensor, bug: str | None = None):
         if layer.bf16:
             Wf = layer.Wf
             mass = r * (x.abs() @ Wf.abs().T + mu.abs() * Wf.abs().sum(1)[None, :]) + layer.beta.abs() @ W.abs().T
-            e_fold = (r * ((x - mu) @ (Wf - layer.gamma[None, :] * W).T)).abs()
+            shift = r * ((x - mu) @ (Wf - layer.gamma[None, :] * W).T)
+            e_fold = shift.abs()
+            if folded:
+                y, e_fold = y + shift, 0.0
         else:
             mass = xh.abs() @ W.abs().T
             e_fold = 0.0
@@ -368,14 +372,16 @@ def ntile_variants(sm_count):
 _ENGINES: dict = {}
 
 
-def engine(shape, dtype):
+def engine(shape, dtype, cfg=None, weights=None):
+    """(cfg, weights, DecoderEngine) of SHAPES entry `shape`, or of `cfg` (a decoder config) under the name `shape`, with
+    weights(cfg) instead of make_weights(cfg, seed=11) when given."""
     from parler_tts_b200.modeling import DecoderEngine
     from tests.helpers import product_decoder_config
     key = (shape, dtype)
     if key not in _ENGINES:
         _ENGINES.clear()
-        cfg = shape_cfg(shape)
-        w = make_weights(cfg, seed=11)
+        cfg = shape_cfg(shape) if cfg is None else cfg
+        w = make_weights(cfg, seed=11) if weights is None else weights(cfg)
         _ENGINES[key] = (cfg, w, DecoderEngine(product_decoder_config(cfg), DEV, dtype).load_state_dict(w))
     return _ENGINES[key]
 
