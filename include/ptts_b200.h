@@ -549,6 +549,40 @@ int ptts_op_dac_conv(int32_t dtype, int32_t kernel, int32_t kind, int32_t B, int
                      const void* alpha_next, const void* x, const void* res, void* out_raw, void* out_act, int32_t tanh_out,
                      const int32_t* frame_lengths, int32_t frames, void* scratch, void* stream);
 
+/* One residual-quantizer launch as ptts_dac_encode2 makes it (test hook for quantize_kernel).  dtype bf16 or f32; every buffer
+ * belongs to the caller.  The weights are in src_dtype (bf16 or f32, as ptts_dac_pack and ptts_dac_encoder_pack take them),
+ * every other float buffer in dtype.
+ *   in_w [n_q][D][Z], in_b [n_q][D]:          in_proj.weight[:, :, 0] / in_proj.bias of the first n_q quantizers, stacked;
+ *   codebooks [n_q][codebook_size][D]:        codebook.weight;
+ *   out_w [n_q][Z][D], out_b [n_q][Z]:        out_proj.weight[:, :, 0] / out_proj.bias;
+ *   z [B][T][Z]:                              the latents (the encoder's output); a ragged launch sets frames past a row's end to 0;
+ *   sample_lengths (device int32 [B], or NULL) and hop: a ragged batch as in ptts_dac_encode2 (each length clamped to
+ *                                             [1, T * hop]; frames from ceil(n_b / hop) on code as codebook_size);
+ *   codes [B][n_q][T] int64.
+ * The codebooks go through the encoder blob's unit-row pack (rounded to bf16 first for bf16), the rest through the plain pack.
+ * scratch (at least 4 n_q cs D + (n_q (2 D Z + D + cs D + Z)) * dtype size + 6 * 256 bytes, 256-byte aligned) starts with
+ * the fp32 unit rows [n_q][codebook_size][D].  PTTS_EINVAL, with nothing launched, for D not in {4, 8, 16}, Z outside
+ * [1, 1536], sample_lengths without hop > 0, an empty shape or another dtype. */
+int ptts_op_dac_quantize(int32_t dtype, int32_t src_dtype, int32_t B, int32_t T, int32_t Z, int32_t D, int32_t n_q, int32_t codebook_size,
+                         const void* in_w, const void* in_b, const void* codebooks, const void* out_w, const void* out_b, void* z,
+                         const int32_t* sample_lengths, int32_t hop, int64_t* codes, void* scratch, void* stream);
+
+/* One quantizer.from_codes launch as the decode walks make it (test hook for from_codes_kernel): z [B][T][C] =
+ * sum over k < K, in the dtype, of out_proj_k(codebook_k[code]).  The weights are in src_dtype (bf16 or f32, converted by
+ * ptts_dac_pack's plain pack), z in dtype.
+ *   codes [B][K][codes_T] int64, each id in [0, codebook_size) wherever it is read;
+ *   codebooks [K][codebook_size][D], proj_w [K][C][D], proj_b [K][C]: codebook.weight, out_proj.weight[:, :, 0], out_proj.bias;
+ *   frame_lengths (device int32 [B], or NULL): as in ptts_dac_decode2, frames at or past row b's length are zero latents.
+ * Without a window (emit_lo == emit_hi == NULL) codes_T == T and frame_start is NULL.  With one, as in ptts_dac_decode3: latent
+ * frame t of row b reads code frame clamp(frame_start[b], 0, codes_T - n_b) + t, and only the frames
+ * [lo_b - m_lo, hi_b + m_hi) around the clamped emit range are written (none when it is empty); frame_lengths and frame_start
+ * are required and T <= codes_T.  scratch holds at least (K (codebook_size + C) D + K C) * dtype size + 3 * 256 bytes.
+ * PTTS_EINVAL, with nothing launched, for K > 32, D > 16, K D > 256, bad window arguments, an empty shape or another dtype. */
+int ptts_op_dac_from_codes(int32_t dtype, int32_t src_dtype, int32_t B, int32_t K, int32_t D, int32_t C, int32_t T, int32_t codebook_size,
+                           const int64_t* codes, int32_t codes_T, const void* codebooks, const void* proj_w, const void* proj_b,
+                           const int32_t* frame_lengths, const int32_t* frame_start, const int32_t* emit_lo, const int32_t* emit_hi,
+                           int32_t m_lo, int32_t m_hi, void* z, void* scratch, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -128,6 +128,10 @@ _SIGS = {
     "ptts_dac_encode2": (C.c_int, [C.POINTER(DacConfigC), _VP, _VP, _VP, _I64, _VP, _I32, _I32, _VP, _I32, _VP, _VP, _VP]),
     "ptts_op_dac_conv": (C.c_int, [_I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _VP, _VP, _VP, _VP, _VP, _VP, _VP,
                                    _VP, _I32, _VP, _I32, _VP, _VP]),
+    "ptts_op_dac_quantize": (C.c_int, [_I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _VP, _VP, _VP, _VP, _VP, _VP, _VP, _I32, _VP, _VP,
+                                       _VP]),
+    "ptts_op_dac_from_codes": (C.c_int, [_I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _VP, _I32, _VP, _VP, _VP, _VP, _VP, _VP, _VP,
+                                         _I32, _I32, _VP, _VP, _VP]),
 }
 EXPORTED_SYMBOLS = tuple(_SIGS)
 

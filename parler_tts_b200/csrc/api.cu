@@ -1374,4 +1374,71 @@ int ptts_op_dac_conv(int32_t dtype, int32_t kernel, int32_t kind, int32_t B, int
   }
 }
 
+// One residual-quantizer launch (test hook).  The weights go through the packs of the encoder and decode blobs: the unit rows
+// first in scratch, where the caller can read them, then the plain arrays.
+int ptts_op_dac_quantize(int32_t dtype, int32_t src_dtype, int32_t B, int32_t T, int32_t Z, int32_t D, int32_t n_q, int32_t codebook_size,
+                         const void* in_w, const void* in_b, const void* codebooks, const void* out_w, const void* out_b, void* z,
+                         const int32_t* sample_lengths, int32_t hop, int64_t* codes, void* scratch, void* stream) {
+  PTTS_REQUIRE(in_w && in_b && codebooks && out_w && out_b && z && codes && scratch, "null argument");
+  PTTS_REQUIRE((dtype == PTTS_BF16 || dtype == PTTS_F32) && (src_dtype == PTTS_BF16 || src_dtype == PTTS_F32),
+               "op_dac_quantize: dtype and src_dtype must be bf16 or f32");
+  PTTS_REQUIRE(B > 0 && T > 0 && n_q > 0 && codebook_size > 0, "op_dac_quantize: bad shape");
+  PTTS_REQUIRE(quantize_supported(Z, D), "op_dac_quantize: latent %d / codebook_dim %d unsupported", Z, D);
+  PTTS_REQUIRE(sample_lengths == nullptr || hop > 0, "op_dac_quantize: a ragged launch needs the hop");
+  cudaStream_t st = (cudaStream_t)stream;
+  const int es = dtype_size(dtype);
+  char* p = (char*)scratch;
+  float* cb_norm = (float*)p;
+  if (int e = pack_normalized_codebook(codebooks, src_dtype, cb_norm, n_q * codebook_size, D, dtype == PTTS_BF16, st)) return e;
+  p += align_up((int64_t)n_q * codebook_size * D * 4, 256);
+  auto plain = [&](const void* src, int64_t n, const void** dst) {
+    *dst = p;
+    const int e = pack_plain(src, src_dtype, n, p, dtype, st);
+    p += align_up(n * es, 256);
+    return e;
+  };
+  QuantizeArgs a{z, nullptr, nullptr, cb_norm, nullptr, nullptr, nullptr, codes, n_q, D, Z, T, codebook_size, sample_lengths, hop};
+  if (int e = plain(in_w, (int64_t)n_q * D * Z, &a.in_w)) return e;
+  if (int e = plain(in_b, (int64_t)n_q * D, &a.in_b)) return e;
+  if (int e = plain(codebooks, (int64_t)n_q * codebook_size * D, &a.codebooks)) return e;
+  if (int e = plain(out_w, (int64_t)n_q * Z * D, &a.out_w)) return e;
+  if (int e = plain(out_b, (int64_t)n_q * Z, &a.out_b)) return e;
+  return launch_quantize(a, dtype, B, st);
+}
+
+// One from_codes launch (test hook), the weights packed into scratch as the decode blob packs them.
+int ptts_op_dac_from_codes(int32_t dtype, int32_t src_dtype, int32_t B, int32_t K, int32_t D, int32_t C, int32_t T, int32_t codebook_size,
+                           const int64_t* codes, int32_t codes_T, const void* codebooks, const void* proj_w, const void* proj_b,
+                           const int32_t* frame_lengths, const int32_t* frame_start, const int32_t* emit_lo, const int32_t* emit_hi,
+                           int32_t m_lo, int32_t m_hi, void* z, void* scratch, void* stream) {
+  PTTS_REQUIRE(codes && codebooks && proj_w && proj_b && z && scratch, "null argument");
+  PTTS_REQUIRE((dtype == PTTS_BF16 || dtype == PTTS_F32) && (src_dtype == PTTS_BF16 || src_dtype == PTTS_F32),
+               "op_dac_from_codes: dtype and src_dtype must be bf16 or f32");
+  PTTS_REQUIRE(B > 0 && K > 0 && D > 0 && C > 0 && T > 0 && codebook_size > 0, "op_dac_from_codes: bad shape");
+  PTTS_REQUIRE(K <= 32 && D <= 16 && K * D <= 256, "op_dac_from_codes: K=%d D=%d unsupported", K, D);
+  PTTS_REQUIRE(!emit_lo == !emit_hi, "op_dac_from_codes: emit_lo and emit_hi go together");
+  if (emit_lo != nullptr)
+    PTTS_REQUIRE(frame_lengths && frame_start && T <= codes_T, "op_dac_from_codes: a window needs frame_lengths, frame_start and T <= codes_T");
+  else
+    PTTS_REQUIRE(codes_T == T && !frame_start, "op_dac_from_codes: without a window codes_T is T and there is no frame_start");
+  cudaStream_t st = (cudaStream_t)stream;
+  const int es = dtype_size(dtype);
+  char* p = (char*)scratch;
+  auto plain = [&](const void* src, int64_t n, const void** dst) {
+    *dst = p;
+    const int e = pack_plain(src, src_dtype, n, p, dtype, st);
+    p += align_up(n * es, 256);
+    return e;
+  };
+  FromCodesArgs a{codes, nullptr, nullptr, nullptr, z, K, D, C, T, codebook_size, frame_lengths};
+  if (int e = plain(codebooks, (int64_t)K * codebook_size * D, &a.codebooks)) return e;
+  if (int e = plain(proj_w, (int64_t)K * C * D, &a.proj_w)) return e;
+  if (int e = plain(proj_b, (int64_t)K * C, &a.proj_b)) return e;
+  if (emit_lo != nullptr) {
+    a.frame_start = frame_start; a.emit_lo = emit_lo; a.emit_hi = emit_hi;
+    a.codes_T = codes_T; a.m_lo = m_lo; a.m_hi = m_hi;
+  }
+  return launch_from_codes(a, dtype, B, st);
+}
+
 }  // extern "C"

@@ -248,6 +248,10 @@ static inline int validate_dac_encoder(const ptts_dac_config& c) {
   }
   PTTS_REQUIRE(hop == dac_hop(c), "dac encoder hop %d differs from the decoder hop %d", hop, dac_hop(c));
   PTTS_REQUIRE(((int64_t)c.encoder_dim << c.n_enc_blocks) <= 65536, "dac encoder_dim too large");
+  // refused here rather than at the quantizer's launch, after the whole encoder network has run
+  PTTS_REQUIRE(quantize_supported(c.latent_dim, c.codebook_dim),
+               "dac quantizer: latent_dim %d / codebook_dim %d unsupported (codebook_dim 4, 8 or 16, latent_dim 1..1536)", c.latent_dim,
+               c.codebook_dim);
   return PTTS_OK;
 }
 

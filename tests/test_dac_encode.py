@@ -156,6 +156,21 @@ def test_encode_input_validation():
         off.encode(wav)
 
 
+def test_encoder_refused_where_the_quantizer_cannot_run():
+    """A codebook_dim or latent_dim the quantizer kernel does not take leaves the codec decode-only: no encoder blob, and encode()
+    raises before any launch."""
+    from parler_tts_b200 import DACConfig
+    from parler_tts_b200.dac_wrapper import DACModel
+    wav = torch.zeros(1, 1, 1000)
+    for kw in (dict(codebook_dim=12), dict(latent_dim=2048)):
+        m = DACModel(DACConfig(**kw), device="cpu")
+        assert m.encoder_blob is None and m.blob.numel() > 0, kw
+        with pytest.raises(ValueError, match="quantizer"):
+            m.encode(wav)
+    for D in (4, 8, 16):
+        assert DACModel(DACConfig(codebook_dim=D, latent_dim=1536), device="cpu").encoder_blob is not None
+
+
 # ---- GPU -------------------------------------------------------------------------------------------
 @pytest.mark.gpu
 @pytest.mark.parametrize("dtype", [torch.float32, torch.bfloat16])
